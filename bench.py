@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — render-quanta/sec of the OfflineAudioContext hot path on N B200s (one process per GPU).
+"""bench.py — render-quanta/sec of the OfflineAudioContext hot path on N H100s (one process per GPU).
 
 Workload (BASELINE.json configs[1], "C2"): 1000 independent OfflineAudioContexts per GPU, each
 AudioBufferSource(stereo, seeded uniform noise) -> BiquadFilter(lowpass, seeded f0/Q) -> Gain -> destination,
@@ -15,6 +15,8 @@ north_star / C5 at N=1 (fixed per-GPU sizes), C4 as "512 graphs, 2/4 GPU shard" 
 gather" at N=8, both also WITH the gather of the rendered PCM inside the step (all-gather of group k overlapped with the render of
 group k+1).
 --impl reference times the reference's CPU algorithm (the oracle port, all host threads) on the same config and batch size.
+--steps sets the number of timed steps of every leg; --dump-outputs DIR writes the PCM of the kernel-only leg's last step (a seeded
+sample of the graphs, at most 64 MB) and of every other timed workload as DIR/*.npy, so that two builds can be compared output for output.
 """
 import argparse
 import ctypes
@@ -33,8 +35,10 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 
 SR = 48000.0
 METRIC = "offline render-quanta/sec (48kHz stereo, 128-frame)"
-FP64_PEAK_TFLOPS = 148 * 64 * 2 * 1.965e9 / 1e12  # B200 non-tensor FP64 (nominal)
-FP32_PEAK_TFLOPS = 148 * 128 * 2 * 1.965e9 / 1e12  # B200 non-tensor FP32: 148 SMs x 128 lanes x FMA at the 1965 MHz boost clock
+FP64_PEAK_TFLOPS = 132 * 64 * 2 * 1.98e9 / 1e12  # H100 SXM non-tensor FP64 (nominal)
+FP32_PEAK_TFLOPS = 132 * 128 * 2 * 1.98e9 / 1e12  # H100 SXM non-tensor FP32: 132 SMs x 128 lanes x FMA at the 1980 MHz boost clock
+DUMP_LIMIT_BYTES = 64 << 20  # all of --dump-outputs: C2 gets up to 40 MB, each of the (at most four) other workloads up to 6 MB
+DUMP_C2_BYTES, DUMP_EXTRA_BYTES = 40 << 20, 6 << 20
 PARKING_GARAGE_IR_FRAMES = 178899  # samples/parking-garage-response.wav (164 363 frames @ 44.1 kHz) resampled to 48 kHz (SURVEY §8a a9)
 
 
@@ -43,11 +47,11 @@ def load_peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "fallback (H100 SXM data sheet, 3.35 TB/s HBM3)"
 
 
 class ClockSampler:
-    """nvidia-smi clocks + throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks + throttle reasons DURING the timed region (read-only queries)."""
 
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -154,7 +158,8 @@ def add_models(a, b2):
     return out
 
 
-def measure_workload(pkg, eng, D, oracle, name, build, n_gpu, n_cpu, length, steps, cores, note, model=None, gather=False, groups=0):
+def measure_workload(pkg, eng, D, oracle, name, build, n_gpu, n_cpu, length, steps, cores, note, model=None, gather=False, groups=0,
+                     dump_dir=None):
     """One additional BASELINE workload: kernel-only (max over ranks), one-shot e2e, optional NCCL gather inside the step, CPU port."""
     import torch
     import torch.distributed as dist
@@ -172,6 +177,8 @@ def measure_workload(pkg, eng, D, oracle, name, build, n_gpu, n_cpu, length, ste
         batch.run()
         batch.sync()
         ms.append(D.max(batch.stats().last_run_ms))
+    if dump_dir and D.rank == 0:
+        dump_outputs(dump_dir, name.lower(), batch, n_gpu, length, 2, DUMP_EXTRA_BYTES)
     stages = {}
     for n, t, _k in batch.stage_times():
         stages[n] = stages.get(n, 0.0) + t
@@ -238,7 +245,7 @@ def measure_workload(pkg, eng, D, oracle, name, build, n_gpu, n_cpu, length, ste
     host = np.zeros((n_gpu, 2, length), np.float32)
     eng.set_option(pkg.OPT_PIPELINE_GROUPS, 0)
     e2e = []
-    for i in range(3):
+    for i in range(1 + steps):
         fresh = [build(eng.backend, g) for g in range(n_gpu)]
         D.barrier()
         t0 = time.perf_counter()
@@ -248,7 +255,7 @@ def measure_workload(pkg, eng, D, oracle, name, build, n_gpu, n_cpu, length, ste
     e2e_s = float(np.median(e2e[1:]))
     out["e2e_value"] = quanta / e2e_s
     out["e2e_ms_per_step"] = e2e_s * 1e3
-    out["e2e_how"] = "one wae_render_batch(HOST) call on fresh graphs, pageable out, median of 2 after 1 warm-up"
+    out["e2e_how"] = f"one wae_render_batch(HOST) call on fresh graphs, pageable out, median of {steps} after 1 warm-up"
     if model is not None:
         out["time_batched_model"] = model
     if oracle is not None and n_cpu > 0 and D.rank == 0:
@@ -287,8 +294,8 @@ def kernel_rooflines(w, peak_gbs):
     if vf:
         # oscillator -> biquad voices: SURVEY §8(d) counts 0 HBM bytes for them (state in registers), so the bound is arithmetic.  Model: the
         # biquad of one voice frame = 3 feed-forward + 2 x 2 recurrence DFMA (the time-parallel scan runs the recurrence twice) = 14 f64
-        # flops; oscillator, conversions and the warp scan come on top and are not counted.  Peak: 148 SMs x 64 f64 lanes x FMA at 1965 MHz
-        # (nominal, not in MEASURED_PEAKS.json).
+        # flops; oscillator, conversions and the warp scan come on top and are not counted.  Peak: 132 SMs x 64 f64 lanes x FMA at 1980 MHz
+        # (H100 SXM, nominal, not in MEASURED_PEAKS.json).
         names = [k for k in st if k in ("k_voice_sum", "k_chain", "k_mix")]
         ms = sum(st[k] for k in names)
         if ms > 0:
@@ -299,11 +306,14 @@ def kernel_rooflines(w, peak_gbs):
     return res
 
 
-def run_extra_workloads(pkg, eng, D, oracle, cores, steps, peak_gbs):
+def run_extra_workloads(pkg, eng, D, oracle, cores, steps, peak_gbs, dump_dir=None):
+    def measure(*a, **k):  # every workload's last timed step goes to --dump-outputs as well
+        return measure_workload(*a, dump_dir=dump_dir, **k)
+
     import graphs as G
     res = []
     ir = G.synthetic_ir(PARKING_GARAGE_IR_FRAMES, 2, decay=0.6)  # synthetic response of the parking-garage IR's length: 175 partitions of 1024
-    # the reference's IRC_1003_C sphere (44.1 kHz, 512 taps, 187 vertices) cannot travel: synthetic data of the same rate and size,
+    # the reference's IRC_1003_C sphere (44.1 kHz, 512 taps, 187 vertices) is not stored in the repository: synthetic data of the same rate and size,
     # resampled to the 48 kHz context rate by the library exactly as the embedded one would be (~417 taps)
     sphere = G.synthetic_hrir_sphere(44100, 512)
     eng.backend.set_hrir_sphere(sphere)
@@ -318,30 +328,30 @@ def run_extra_workloads(pkg, eng, D, oracle, cores, steps, peak_gbs):
         return G.c5_full_chain(pkg, be, g + D.rank * 100000, c5_len, ir, curve_points=1024)
 
     if D.world == 1:
-        res.append(measure_workload(pkg, eng, D, oracle, "C3", lambda be, g: G.c3_many_voices(pkg, be, 4096, 48000), 1, 1, 48000, steps, cores,
+        res.append(measure(pkg, eng, D, oracle, "C3", lambda be, g: G.c3_many_voices(pkg, be, 4096, 48000), 1, 1, 48000, steps, cores,
                                     "configs[2]: ONE graph, 4096 x (Oscillator -> Biquad) summed in reference order at the destination, 1 s"))
-        res.append(measure_workload(pkg, eng, D, oracle, "C4", c4, 128, min(cores, 128), 480000, steps, cores,
+        res.append(measure(pkg, eng, D, oracle, "C4", c4, 128, min(cores, 128), 480000, steps, cores,
                                     "configs[3] at 128 graphs/GPU (the 4-GPU share of 512): stereo source -> Convolver(3.73 s stereo IR = 175 "
                                     "partitions of 1024, normalize) -> destination, 10 s", model=conv_model(128, 480000, PARKING_GARAGE_IR_FRAMES)))
-        res.append(measure_workload(pkg, eng, D, oracle, "north_star", lambda be, g: G.north_star_voices_convolver(pkg, be, 1000, 480000, ir, seed=g),
+        res.append(measure(pkg, eng, D, oracle, "north_star", lambda be, g: G.north_star_voices_convolver(pkg, be, 1000, 480000, ir, seed=g),
                                     8, 8, 480000, steps, cores,
                                     "north_star: 8 graphs/GPU, each 1000 voices (Oscillator -> Biquad -> Gain) summed into one Convolver -> destination, 10 s",
                                     model=conv_model(8, 480000, PARKING_GARAGE_IR_FRAMES, in_ch=1, paths=2)))
-        res.append(measure_workload(pkg, eng, D, oracle, "C5", c5, 256, min(cores, 64), c5_len, steps, cores,
+        res.append(measure(pkg, eng, D, oracle, "C5", c5, 256, min(cores, 64), c5_len, steps, cores,
                                     "configs[4] per-GPU share (2048 graphs / 8 GPUs): Oscillator -> WaveShaper(1024-pt tanh) -> Biquad -> Convolver -> "
                                     "Panner(HRTF, 44.1 kHz / 512-tap sphere resampled to 48 kHz) -> Analyser -> destination, 5 s; HRTF parity is UNPINNED "
                                     "(hrtf crate absent from the reference tree, SURVEY §8c)", model=add_models(conv_model(256, c5_len, PARKING_GARAGE_IR_FRAMES, in_ch=1, paths=2), conv_model(256, c5_len, 558, in_ch=2, paths=4))))
     elif D.world > 1 and os.environ.get("WAE_BENCH_EXTRA") == "c5_small":  # validation of the N = 8 leg on fewer GPUs (not a BASELINE size)
-        res.append(measure_workload(pkg, eng, D, None, "C5", c5, 32, 0, c5_len, steps, cores,
+        res.append(measure(pkg, eng, D, None, "C5", c5, 32, 0, c5_len, steps, cores,
                                     "configs[4] path check: 32 graphs per GPU, with the NCCL gather inside the step", gather=True, groups=4))
     elif D.world in (2, 4):
         n = 512 // D.world
-        res.append(measure_workload(pkg, eng, D, None, "C4", c4, n, 0, 480000, steps, cores,
+        res.append(measure(pkg, eng, D, None, "C4", c4, n, 0, 480000, steps, cores,
                                     f"configs[3]: 512 graphs sharded over {D.world} GPUs ({n} per GPU): stereo source -> Convolver(175-partition stereo IR, "
                                     "normalize) -> destination, 10 s; also with the NCCL gather of the PCM inside the step",
                                     model=conv_model(n, 480000, PARKING_GARAGE_IR_FRAMES), gather=True, groups=8))
     elif D.world == 8:
-        res.append(measure_workload(pkg, eng, D, None, "C5", c5, 256, 0, c5_len, steps, cores,
+        res.append(measure(pkg, eng, D, None, "C5", c5, 256, 0, c5_len, steps, cores,
                                     "configs[4]: 2048 graphs over 8 GPUs (256 per GPU), full chain with HRTF panner (parity unpinned, SURVEY §8c), 5 s; also "
                                     "with the NCCL gather of the PCM inside the step", model=add_models(conv_model(256, c5_len, PARKING_GARAGE_IR_FRAMES, in_ch=1, paths=2), conv_model(256, c5_len, 558, in_ch=2, paths=4)),
                                     gather=True, groups=8))
@@ -370,6 +380,33 @@ def load_oracle_only():
         subprocess.check_call(["make", "-C", os.path.join(ROOT, "oracle"), "-j8"], stdout=subprocess.DEVNULL)
     pkg = ge.load_package()
     return pkg, pkg.context.Backend(pkg.Api(ctypes.CDLL(ge.ORACLE_SO), "wao_"))
+
+
+def dump_outputs(out_dir, name, batch, n_graphs, length, max_graphs, limit_bytes):
+    """The PCM a timed batch rendered in its last step, as a caller of Batch.run / fetch receives it ([graph][channel][frame] f32),
+    for a fixed seeded sample of at most `max_graphs` graphs: DIR/<name>_output.npy plus the graphs' indices
+    (DIR/<name>_graph_index.npy) and, when the sample would be over `limit_bytes` at full length, the first frame of the stored
+    window (DIR/<name>_frame_offset.npy)."""
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    p, n_floats = batch.device_ptr()
+    ch = batch.channels
+    assert n_floats >= n_graphs * ch * length
+
+    class _W:  # the engine's output buffer as a torch tensor (CUDA array interface, no copy)
+        __cuda_array_interface__ = {"shape": (n_graphs, ch, length), "typestr": "<f4", "data": (p, False), "version": 2}
+    pcm = torch.as_tensor(_W(), device="cuda")
+    per_graph = ch * length * 4
+    k = max(1, min(n_graphs, max_graphs, limit_bytes // per_graph))
+    rng = np.random.default_rng(20240601)
+    idx = np.sort(rng.choice(n_graphs, size=k, replace=False))
+    frames = min(length, limit_bytes // (ch * 4 * k))
+    f0 = int(rng.integers(0, length - frames + 1)) if frames < length else 0
+    sample = pcm[torch.as_tensor(idx, device="cuda")][:, :, f0:f0 + frames].cpu().numpy()
+    np.save(os.path.join(out_dir, f"{name}_output.npy"), np.ascontiguousarray(sample, np.float32))
+    np.save(os.path.join(out_dir, f"{name}_graph_index.npy"), idx.astype(np.float64))
+    if frames < length:
+        np.save(os.path.join(out_dir, f"{name}_frame_offset.npy"), np.array([f0], np.float64))
 
 
 def build_c2_batch(pkg, backend, n_graphs, length, seed_base=0, pcm=None):
@@ -429,7 +466,11 @@ def main():
     ap.add_argument("--bind-numa", type=int, default=1, help="bind every rank's host threads to its GPU's NUMA node (pinned memory local to the GPU)")
     ap.add_argument("--kernel-only", action="store_true", help="tuning runs: only the kernel-only leg of C2 (no e2e legs, no other workloads)")
     ap.add_argument("--extra", type=int, default=1, help="also measure the other BASELINE configs (C3 / C4 / north_star / C5 at N=1; C4 at N=2,4; C5 at N=8)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the PCM of the last timed step of every workload (seeded sample of the graphs, <= 64 MB in all) as DIR/*.npy")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
 
     D = Dist()
     if args.impl == "reference":
@@ -486,7 +527,7 @@ def main():
         wall = time.perf_counter() - t0
         return D.max(e0.elapsed_time(e1)), wall
 
-    # ---- kernel-only: inputs resident in HBM (3.84 GB of source PCM per 1000 graphs >> 126 MB L2: every step
+    # ---- kernel-only: inputs resident in HBM (3.84 GB of source PCM per 1000 graphs >> 50 MB L2: every step
     # streams its inputs from HBM again, no explicit L2 flush needed)
     batch.set_timing(True)
     for _ in range(args.warmup):
@@ -502,6 +543,8 @@ def main():
     value = total_quanta / (ms_per_step * 1e-3)
     batch.set_timing(False)
     batch.sync()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, "c2", batch, n_graphs, length, 8, DUMP_C2_BYTES)
     if args.kernel_only:
         agg = {}
         for name, ms, _n in stage_times:
@@ -533,10 +576,9 @@ def main():
             del fresh
         return walls
 
-    e2e_steps = max(1, min(args.steps, 5))
-    e2e_walls = oneshot(pageable_out, e2e_steps, max(1, min(args.warmup, 2)))
+    e2e_walls = oneshot(pageable_out, args.steps, max(1, min(args.warmup, 2)))
     e2e_s = float(np.mean(e2e_walls))
-    e2e_pinned_walls = oneshot(pinned_view, max(1, min(args.steps, 3)), 1)
+    e2e_pinned_walls = oneshot(pinned_view, args.steps, 1)
     e2e_pinned_s = float(np.mean(e2e_pinned_walls))
     h2d = stats.asset_bytes * world  # whole job, like `value`: every rank copies its own shard over its own PCIe link
     d2h = out_floats * 4 * world
@@ -548,9 +590,8 @@ def main():
     prepare_ms = (time.perf_counter() - t_prep) * 1e3
     pinned_ptr = ctypes.c_void_p(pinned_out.data_ptr())
     batch_e2e.run_pipelined(pinned_ptr)
-    warm_steps = max(1, min(args.steps, 3))
-    _, warm_wall = timed(lambda: batch_e2e.run_pipelined(pinned_ptr), warm_steps)
-    warm_s = D.max(warm_wall / warm_steps)
+    _, warm_wall = timed(lambda: batch_e2e.run_pipelined(pinned_ptr), args.steps)
+    warm_s = D.max(warm_wall / args.steps)
     batch_e2e.destroy()
 
     # ---- roofline of the dominant kernel (CUDA events around every stage launch, on the launching stream)
@@ -639,7 +680,7 @@ def main():
         if rank == 0 and world == 1 and not args.no_cpu_baseline:
             os.sched_setaffinity(0, all_cpus)
             oracle2 = pkg.context.Backend(pkg.Api(ctypes.CDLL(ge.ORACLE_SO), "wao_"))
-        extra = run_extra_workloads(pkg, eng, D, oracle2, len(all_cpus), max(2, min(args.steps, 5)), load_peaks()[0])
+        extra = run_extra_workloads(pkg, eng, D, oracle2, len(all_cpus), args.steps, load_peaks()[0], dump_dir=args.dump_outputs)
         if line is not None:
             line["other_workloads"] = extra
     if line is not None:

@@ -1,5 +1,5 @@
 /*
- * wae.h — C ABI of the B200 render-quantum engine ("wae" = web-audio engine).
+ * wae.h — C ABI of the H100 render-quantum engine ("wae" = web-audio engine).
  *
  * This is the drop-in boundary for web-audio-api-rs's OfflineAudioContext hot path.
  * The reference has NO FFI today: its plug-in point is the Rust trait
@@ -239,7 +239,7 @@ typedef struct wae_param_event {
 
 /* ---- engine ------------------------------------------------------------------------------------ */
 
-/* device_ordinal: CUDA device of this process rank. Fails with WAE_NO_DEVICE when no sm_100 GPU is
+/* device_ordinal: CUDA device of this process rank. Fails with WAE_NO_DEVICE when no sm_90 GPU (H100) is
  * usable — there is NO CPU fallback in this library. */
 WAE_API wae_status wae_engine_create(int32_t device_ordinal, wae_engine** out_engine);
 WAE_API wae_status wae_engine_destroy(wae_engine* engine);

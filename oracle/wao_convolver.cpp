@@ -3,7 +3,7 @@
 // ConvolverNode: src/node/convolver.rs (normalize_buffer :16-53, set_buffer :259-317, process :343-490).
 //
 // The arithmetic lives in the third-party crate `fft-convolver = "0.3"` (Cargo.toml:24), which is NOT in
-// /root/reference (no vendored sources, no Cargo.lock).  FFTConvolver below restates that crate's
+// the reference source tree (no vendored sources, no Cargo.lock).  FFTConvolver below restates that crate's
 // published algorithm (a Rust port of HiFi-LoFi's FFTConvolver): uniformly partitioned overlap-add
 // convolution, block = next_pow2(block_size), FFT = 2*block, the partially filled input block is
 // re-transformed on every process() call, the products of all but the newest segment are cached in

@@ -7,7 +7,7 @@
 // FTZ/DAZ set while rendering like src/render/thread.rs:373-380).
 //
 // Parity status: pinned against the reference's own known-answer tests (tests/test_oracle_kat.py lists
-// each vector with its reference file:line).  Third-party arithmetic that is not in /root/reference
+// each vector with its reference file:line).  Third-party arithmetic that is not in the reference source tree
 // (fft-convolver 0.3, hrtf 0.8.1, rubato 0.16, realfft 3.3) is restated from the published algorithms;
 // see the header of the respective file for what is and is not pinned.
 #pragma once

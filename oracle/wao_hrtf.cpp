@@ -1,7 +1,7 @@
 // ORACLE — TEST INFRASTRUCTURE ONLY (see wao_core.h).
 //
 // HRTF panning.  The reference delegates to the third-party crate `hrtf = "0.8.1"` (Cargo.toml:41; call sites
-// src/node/panner.rs:39-68 load_hrtf_processor, :239-271 HrtfState::process) whose source is NOT in /root/reference.
+// src/node/panner.rs:39-68 load_hrtf_processor, :239-271 HrtfState::process) whose source is NOT in the reference source tree.
 // This file restates that crate's PUBLISHED algorithm as used by those call sites (interpolation_steps = 1,
 // block_len = 128):
 //   * HrirSphere::new parses the "HRIR" container (magic, sample rate, HRIR length L, vertex count, index count,
@@ -19,7 +19,7 @@
 // `process` call over the whole response, parameters sinc_len 256 / f_cutoff 0.95 / oversampling 160 / cubic / BlackmanHarris2).
 // resample_hrir() below restates that algorithm from rubato's published description (windowed-sinc bank, 4 neighbouring sinc
 // phases, cubic polynomial between them, start index -sinc_len/2, stop at chunk - sinc_len - 1).  Neither crate is in
-// /root/reference, so the tap values of a resampled sphere are unpinned like the rest of this file.
+// the reference source tree, so the tap values of a resampled sphere are unpinned like the rest of this file.
 // Degenerate rays (through a mesh vertex / edge) pick the face with the largest minimum barycentric coordinate instead of
 // the crate's first-hit order.
 // PARITY UNPINNED: the only reference test (panner.rs:1225-1269) asserts "output != input" and "tail is non-zero"

@@ -1,7 +1,7 @@
 // ORACLE — TEST INFRASTRUCTURE ONLY (see wao_core.h).
 //
 // rubato::FftFixedInOut<f32> as used by the over-sampled WaveShaper (src/node/waveshaper.rs:236-348,409-480).  The crate
-// (rubato = "0.16", Cargo.toml:46) is NOT in /root/reference: this restates its PUBLISHED algorithm (synchronous FFT
+// (rubato = "0.16", Cargo.toml:46) is NOT in the reference source tree: this restates its PUBLISHED algorithm (synchronous FFT
 // resampler): per chunk of fft_size_in frames
 //     X = rFFT([chunk | zeros])                          (2 * fft_size_in points)
 //     Y[k] = X[k] * F[k]   for k < min(fft_size_in, fft_size_out),  0 above

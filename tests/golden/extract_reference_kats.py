@@ -1,8 +1,8 @@
 #!/usr/bin/env python
 """Extracts known-answer vectors from the reference's own #[test]s into tests/golden/reference_kats.json.
 
-Run HERE (where /root/reference exists); the JSON travels to the GPU box, /root/reference does not.
-Only numeric literals of test tables are read — no reference code is copied.
+Usage: python tests/golden/extract_reference_kats.py <checkout of the reference>.  The JSON is committed, so the tests do
+not need the reference's sources.  Only numeric literals of test tables are read — no reference code is copied.
   - biquad frequency responses, Chrome/Firefox values  (src/node/biquad_filter.rs:1000-1412)
   - un-normalised biquad coefficients for f0=2000, Q=1, gain=3 @44.1k (src/node/iir_filter.rs:611-755)
   - IIR magnitude response vs scipy                      (src/node/iir_filter.rs:757-800)
@@ -10,8 +10,9 @@ Only numeric literals of test tables are read — no reference code is copied.
 import json
 import os
 import re
+import sys
 
-REF = "/root/reference"
+REF = sys.argv[1] if len(sys.argv) > 1 else "reference"
 OUT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "reference_kats.json")
 NUM = r"-?\d[\d_]*\.?[\d_]*(?:[eE]-?\d+)?"
 

@@ -161,6 +161,21 @@ def synthetic_hrir_sphere(sample_rate=48000, taps=256, subdivisions=2, seed=5):
     return b"".join(out)
 
 
+def reference_hrir_subset():
+    """The reference's IRC_1003_C sphere as stored in tests/golden/irc_1003_c_subset.npz (tools/extract_hrir_subset.py): every
+    vertex position and face, the responses of the vertices a source at x = 1 blends, zeros elsewhere.  Container bytes."""
+    import os
+    import struct
+    z = np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "irc_1003_c_subset.npz"))
+    pos, faces, taps = z["positions"], z["faces"], int(z["taps"])
+    ir = np.zeros((len(pos), 2, taps), np.float32)
+    ir[z["vertices"], 0], ir[z["vertices"], 1] = z["left"], z["right"]
+    out = [b"HRIR", struct.pack("<IIII", int(z["sample_rate"]), taps, len(pos), faces.size), np.asarray(faces, "<u4").tobytes()]
+    for v in range(len(pos)):
+        out += [np.asarray(pos[v], "<f4").tobytes(), ir[v].astype("<f4").tobytes()]
+    return b"".join(out)
+
+
 def parse_hrir_sphere(data):
     """(sample_rate, positions [v][3], faces [f][3], left [v][taps], right [v][taps]) of an HRIR container."""
     import struct

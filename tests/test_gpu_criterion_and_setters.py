@@ -1,6 +1,5 @@
 """GPU parity of the reference's criterion / iai benchmark graphs (benches/my_benchmark.rs), of graphs configured through the
-post-construction setters, of the WPT buffer-stitching case, and of the two AudioParam kernels against each other.
-(First run on a B200 in round 2: all green, profiles/README.md r2_a.)"""
+post-construction setters, of the WPT buffer-stitching case, and of the two AudioParam kernels against each other."""
 
 import numpy as np
 import pytest

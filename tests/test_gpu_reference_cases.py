@@ -1,4 +1,4 @@
-"""The reference's OWN known-answer tests, run through the CUDA path (C ABI -> sm_100a kernels) instead of the oracle.
+"""The reference's OWN known-answer tests, run through the CUDA path (C ABI -> sm_90a kernels) instead of the oracle.
 
 tests/test_oracle_kat.py and tests/test_oracle_offline.py restate the reference's `#[test]`s (each names its file:line) and
 pin the oracle with them; the graph-rendering ones only need a backend, so the very same functions are executed here with

@@ -3,7 +3,7 @@ sum in registers and walks the voices in the port's edge order — Graph::render
 (examples/many_oscillators.rs, the north_star graph).  The planner only takes that path when the launch has enough (tile, port) work items
 (tests/test_planner_cpu.py); here WAE_OPT_VOICE_SUM = 2 forces it on small graphs, and every case is rendered three ways: fused, unfused
 (k_chain + k_mix) and on the oracle.  Tolerance 1e-5 absolute (north_star).  The option is OFF by default: on the north_star workload the
-kernel measured slower than the two it replaces (profiles/README.md r2_q / r2_r) — it stays in the tree as a tested alternative."""
+kernel measured slower than the two it replaces — it stays in the tree as a tested alternative."""
 import numpy as np
 import pytest
 

@@ -1,5 +1,5 @@
 """Pins the oracle's graph / mixer / scheduling semantics against the reference's integration tests
-(/root/reference/tests/offline.rs).  Each test restates one reference `#[test]` (name + line cited)."""
+(the reference's tests/offline.rs).  Each test restates one reference `#[test]` (name + line cited)."""
 import numpy as np
 import pytest
 

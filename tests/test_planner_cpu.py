@@ -73,7 +73,7 @@ def test_c4_north_star_c5_stage_lists(pkg, be):
     # enough (2048-frame tile, graph) work items to fill the machine about twice: the voices and their ordered sum become ONE kernel
     # (k_voice_sum), no voice is written to the arena (what is left is the convolver's mono input), the render is one chunk
     big = [G.north_star_voices_convolver(pkg, be, 12, 8192 * 48, ir, seed=g) for g in range(8)]
-    assert "k_voice_sum" not in plan(pkg, big)["kinds"]  # (off by default: measured slower than k_chain + k_mix, profiles/README.md r2_r)
+    assert "k_voice_sum" not in plan(pkg, big)["kinds"]  # (off by default: measured slower than k_chain + k_mix)
     os.environ["WAE_VOICE_SUM"] = "1"
     try:
         p = plan(pkg, big)

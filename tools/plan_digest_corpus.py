@@ -2,8 +2,7 @@
 """Regression harness for refactorings of the planner (CPU, no GPU): prints, for a corpus of graphs (BASELINE configs, the 24 reference
 scenarios, fuzz graphs and fuzz batches), the WAE_PLAN_DIGEST hash of every instance record the sizing pass builds.  Run it with the
 library before and after a change and diff the outputs:
-    python tools/plan_digest_corpus.py /path/to/old/libwae_b200.so 2> before.txt ; python tools/plan_digest_corpus.py 2> after.txt ; diff before.txt after.txt
-(round 2: 407 + 620 plans unchanged across the NodeMap / node-table / scan-constant / split-planning changes, profiles/README.md r2_ac, r2_ae)"""
+    python tools/plan_digest_corpus.py /path/to/old/libwae_b200.so 2> before.txt ; python tools/plan_digest_corpus.py 2> after.txt ; diff before.txt after.txt"""
 import sys, os, subprocess
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(ROOT, "tests")); sys.path.insert(0, ROOT)

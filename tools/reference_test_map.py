@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Which of the reference's own #[test]s are restated in tests/ ?  Run in the build container (needs /root/reference); writes
+"""Which of the reference's own #[test]s are restated in tests/ ?  Needs a checkout of the reference (first argument); writes
 tests/REFERENCE_TESTS.md.  A reference test counts as restated when one of our test files cites a line range of its source file that
 contains the test function (citations look like `param.rs:1814-1872`, or `:1874-1899` after the file was named), or names the function."""
 import glob
@@ -8,7 +8,7 @@ import re
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = sys.argv[1] if len(sys.argv) > 1 else "/root/reference"
+REF = sys.argv[1] if len(sys.argv) > 1 else "reference"
 # the files SURVEY.md section 8 puts on the path (+ the integration tests that render offline)
 FILES = ["src/param.rs", "src/node/audio_buffer_source.rs", "src/node/oscillator.rs", "src/node/scheduled_source.rs", "src/analysis.rs", "src/buffer.rs",
          "src/node/convolver.rs", "src/node/iir_filter.rs", "src/node/delay.rs", "src/context/offline.rs", "src/node/biquad_filter.rs", "src/render/quantum.rs",

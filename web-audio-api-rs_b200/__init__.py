@@ -1,10 +1,10 @@
-"""web-audio-api-rs_b200 — B200-native render-quantum engine for web-audio-api-rs's OfflineAudioContext path.
+"""web-audio-api-rs_b200 — H100-native render-quantum engine for web-audio-api-rs's OfflineAudioContext path.
 
 The directory name carries a hyphen (it mirrors the reference's name), so import it through
 `__graft_entry__.load_package()` / tests/conftest.py, which register it as `web_audio_api_rs_b200`.
 
 Layout:
-  csrc/            hand-written sm_100a CUDA kernels + the C-ABI implementation (include/wae.h)
+  csrc/            hand-written sm_90a CUDA kernels + the C-ABI implementation (include/wae.h)
   _binding.py      ctypes view of the C ABI
   context.py       host-side mirror of the reference's control API (OfflineAudioContext, AudioNode, AudioParam)
 

@@ -230,7 +230,7 @@ static std::shared_ptr<PcmBuffer> copy_buffer(wae_graph* g, const wae_audio_buff
 extern "C" {
 
 WAE_API const char* wae_last_error(void) { return g_err.c_str(); }
-WAE_API const char* wae_version(void) { return "wae-b200 0.1 (sm_100a)"; }
+WAE_API const char* wae_version(void) { return "wae-b200 0.1 (sm_90a)"; }
 
 // OfflineAudioContext::new, src/context/offline.rs:78-105
 WAE_API wae_status wae_graph_create(wae_engine* engine, uint32_t number_of_channels, uint64_t length, float sample_rate,

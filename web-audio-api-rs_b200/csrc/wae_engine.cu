@@ -715,7 +715,7 @@ struct Planner {
     std::map<std::pair<uint32_t, uint32_t>, DelayRing> delay_rings;       // (graph, writer id)
     bool dry = false;                     // sizing pass: count arena floats per frame, touch no device memory
     int group_graphs = 1;                 // graphs of the group being planned (k_voice_sum: are there enough work items?)
-    // 0 off (default: measured slower than k_chain + k_mix on north_star, profiles/README.md r2_q / r2_r), 1 when the launch is large enough,
+    // 0 off (default: measured slower than k_chain + k_mix on north_star), 1 when the launch is large enough,
     // 2 whenever the port has the shape (tests).  WAE_OPT_VOICE_SUM, else WAE_VOICE_SUM from the environment (read per plan).
     int vs_mode = -1;
     int voice_sum_mode() {
@@ -2772,7 +2772,8 @@ WAE_API wae_status wae_engine_create(int32_t device_ordinal, wae_engine** out) {
     CUDA_TRY(cudaSetDevice(device_ordinal));
     cudaDeviceProp prop;
     CUDA_TRY(cudaGetDeviceProperties(&prop, device_ordinal));
-    if (prop.major < 10) return fail(WAE_NO_DEVICE, "the kernels are built for sm_100a only");
+    if (prop.major != 9 || prop.minor != 0) return fail(WAE_NO_DEVICE, "the kernels are built for sm_90a (H100) only");
+    set_num_sms(prop.multiProcessorCount);
     auto* eng = new wae_engine;
     eng->device = device_ordinal;
     CUDA_TRY(cudaStreamCreateWithFlags(&eng->stream, cudaStreamNonBlocking));
@@ -2986,7 +2987,7 @@ static wae_status prep_begin(wae_engine* eng, wae_graph* const* graphs, uint32_t
     }
     // graph groups for the H2D / render / D2H pipeline
     int n_groups = eng->pipeline_groups;
-    if (n_groups == 0) n_groups = n_graphs >= 512 ? 32 : (n_graphs >= 64 ? 8 : 1);  // measured on C2: 8 groups 88 ms, 16: 83.7, 32: 80.6 (fill / drain of the 3-stage pipeline)
+    if (n_groups == 0) n_groups = n_graphs >= 512 ? 32 : (n_graphs >= 64 ? 8 : 1);  // more groups = shorter fill / drain of the 3-stage pipeline
     if (eng->pipeline_groups == 0 && n_graphs >= 512) {  // (tuning: WAE_AUTO_GROUPS overrides the automatic choice for large batches)
         static const int env_groups = [] { const char* e = getenv("WAE_AUTO_GROUPS"); return e ? atoi(e) : 0; }();
         if (env_groups > 0) n_groups = env_groups;
@@ -3989,7 +3990,7 @@ static wae_status render_oneshot_host(wae_engine* eng, wae_graph* const* graphs,
     size_t max_group_bytes = 0;
     for (auto& grp : b->groups) max_group_bytes = std::max(max_group_bytes, (size_t)(grp.g1 - grp.g0) * per_graph * sizeof(float));
     // Pageable `out`, default: whole-group page-locked staging slots, copied out in parts by the workers (below).  WAE_STAGE_RING=1 (an
-    // experiment that lost, kept for the record: profiles/README.md r2_x): the PCM comes down in PIECES of a couple of MB through a small
+    // experiment that lost, kept for the record): the PCM comes down in PIECES of a couple of MB through a small
     // ring of page-locked slots meant to stay in the last-level cache (inbound DMA writes allocate there), each piece copied out as soon
     // as it has landed.  Two ranks on one socket: 414 - 1117 ms per call against 184 ms with the group slots — a piece pays a blocking
     // event wait and two thread wake-ups, and 2 MB is not enough work to hide them.

@@ -1,4 +1,4 @@
-// Hand-written sm_100a kernels of the render-quantum engine, one per node renderer of SURVEY §8(a).
+// Hand-written sm_90a kernels of the render-quantum engine, one per node renderer of SURVEY §8(a).
 //
 // All kernels are HBM/latency-bound streaming or scan kernels (no dense contraction -> no tensor cores):
 // coalesced planar f32 loads/stores, f64 only where the reference computes in f64 (biquad / IIR state,
@@ -944,7 +944,7 @@ DEVI void chain_load_source(const ChainInst& q, int c, const ChunkInfo& ci, int 
         } else {
             // ragged / looping runs, frame by frame; a looping buffer costs ONE modulo per thread and then a wrapping index (was: a 64-bit
             // modulo per frame).  (Kept this small: the out-of-line gather's register needs are saved and restored around every call
-            // in k_chain — a float4 fast path for loops here made the streamed kernel spill, r2_p.)
+            // in k_chain — a float4 fast path for loops here made the streamed kernel spill.)
             int64_t pos = 0;
             if (o.loop) {
                 pos = idx % o.buf_len;
@@ -1003,8 +1003,8 @@ DEVI void chain_load_source(const ChainInst& q, int c, const ChunkInfo& ci, int 
                 // (around 0 and 0.5) are u mod 2^63 < 2 dph; the test looks at the high words only, so it flags a few frames too many —
                 // the out-of-line evaluation decides exactly, in f64, and returns the plain wave for those.  Pass 2 visits the flagged
                 // frames lane by lane: a warp whose lanes have their windows at different frames runs the f64 evaluation as often as its
-                // busiest lane has flagged frames (1 - 2 times per tile at 440 Hz) instead of once per frame that ANY lane flags (7 of 16;
-                // ncu r2_p: the polyBLEP lines were 32 % of the oscillator chain's instructions).
+                // busiest lane has flagged frames (1 - 2 times per tile at 440 Hz) instead of once per frame that ANY lane flags (7 of 16:
+                // the polyBLEP lines were a large share of the oscillator chain's instructions).
                 const unsigned long long ph0 = ph;
                 const unsigned thr = (unsigned)((dph + dph) >> 32);
                 unsigned mask = 0;
@@ -1263,7 +1263,7 @@ DEVI void chain_biquad(ChainSmem& sm, int bq, const double b0, const double b1, 
     }
 }
 
-// ---- Blackwell async-copy primitives used by the TMA variant of k_chain (1-D bulk copies, mbarrier completion) ----
+// ---- Hopper async-copy primitives used by the TMA variant of k_chain (1-D bulk copies, mbarrier completion) ----
 DEVI unsigned smem_u32(const void* p) { return (unsigned)__cvta_generic_to_shared(p); }
 DEVI void mbar_init(uint64_t* bar, unsigned count) { asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory"); }
 DEVI void mbar_expect_tx(uint64_t* bar, unsigned bytes) {
@@ -1313,8 +1313,8 @@ DEVI void cswap4(bool p, float4& a, float4& b) {
 // Work decomposition.  A work item is (time slab, instance, channel); items are numbered slab-major and handed out in
 // order of CTA start (one atomic ticket per CTA), so the slab before a given one of the same (instance, channel) always
 // belongs to a CTA that is already running or done: waiting for the filter state it leaves behind cannot deadlock.
-// With S slabs the launch has S x more, S x shorter CTAs: the tail of the last wave (2000 equal CTAs on 888 slots used to
-// leave the machine a quarter full for a third of the run) shrinks to one short item.  Chains without a filter carry no
+// With S slabs the launch has S x more, S x shorter CTAs: the tail of the last wave (equal whole-render CTAs
+// leave the machine partly empty for the last fraction of the run) shrinks to one short item.  Chains without a filter carry no
 // state: their slabs are independent.  TMA = true: the source tiles arrive through 1-D bulk copies (cp.async.bulk +
 // mbarrier), results leave through bulk stores; TMA = false: 16-byte cp.async pieces / coalesced stores (kept as the
 // reference data path: WAE_OPT_CHAIN_TMA = 0).
@@ -2165,8 +2165,8 @@ __global__ void __launch_bounds__(256) k_biquad_coefs(const BiquadArInst* __rest
 // M_n = [[-a1_n, -a2_n], [1, 0]],  t_n = (b0_n x[n] + b1_n x[n-1]) + b2_n x[n-2]  — so the quantum is a scan over affine maps: every lane
 // composes the maps of its four frames, a Kogge-Stone scan over the 32 lanes gives each lane the map from the quantum's start to its
 // first frame, and the lane then runs its four frames from that state in the reference's own operation order (biquad_filter.rs:869-883,
-// with its flush of non-normal values).  About 25 dependent f64 operations per quantum instead of 640 (measured: a dependent f64
-// operation of a lone warp costs ~100 cycles here; "Substractive Synth", 64 graphs x 120 s: 77 s -> 11 s -> 2.8 s -> see profiles r2_o).
+// with its flush of non-normal values).  About 25 dependent f64 operations per quantum instead of 640 (a dependent f64 operation
+// of a lone warp costs on the order of 100 cycles; "Substractive Synth", 64 graphs x 120 s, is the case that needs it).
 // Differs from the serial evaluation by the re-association of the state carried between lanes (~1e-16 relative); a NaN / Inf going
 // through the recurrence (the reference recovers from it sample by sample) sends the quantum to the serial code, which stays below.
 constexpr int BQA_WARPS = 2;
@@ -3851,7 +3851,7 @@ constexpr int CV_MAC_THREADS = 256;
 // PACKED: bin 0 holds (DC, Nyquist), two real bins that multiply component-wise.  FIRST: the head group (i_base = 0), only i = jj - r >= 0.
 // The IR spectra are stored with WAE_CONV_H_PAD_LO zero partitions before H_0 and zero partitions behind H_{S-1} up to the end of the
 // last group (plan_convolver): the loads of a group need no range tests at all — 23 loads and 256 FMAs per group, where the tests of
-// the exact walk cost more issue slots than the multiplications with zero they saved (ncu r2_l: ALU pipe 59 % against FMA 32 %).
+// the exact walk cost more issue slots than the multiplications with zero they saved (the ALU pipe, not the FMA pipe, was the busier one).
 template <bool PACKED, bool FIRST>
 DEVI void conv_mac_group(const float2* __restrict__ hp /* H_{i_base - (CV_J - 1)}[k] */, const float2 (&x)[CV_J], float2 acc[CV_J]) {
     float2 hw[2 * CV_J - 1];
@@ -4181,6 +4181,10 @@ __global__ void __launch_bounds__(256) k_resample_linear(const float* __restrict
 // ---------------------------------------------------------------------------------------------------------
 // launchers
 // ---------------------------------------------------------------------------------------------------------
+static int g_num_sms = 132;  // H100 SXM; wae_engine_create sets the device's own count
+void set_num_sms(int n) {
+    if (n > 0) g_num_sms = n;
+}
 static inline dim3 grid_tiles(int nf, int per_block, int n_inst) {
     return dim3((unsigned)((nf + per_block - 1) / per_block), (unsigned)(n_inst < 32768 ? n_inst : 32768));
 }
@@ -4196,11 +4200,11 @@ void launch_mix(const MixInst* d, const MixEdge* e, int n, ChunkInfo ci, cudaStr
     // few instances x few frames (one graph with a huge fan-in): one frame per thread keeps more loads in flight
     const long ctas4 = (long)((ci.nf + 1023) / 1024) * n;
     if (max_edges < 16) {  // no port of this stage is wide enough for the staged kernel
-        if (ctas4 < 2 * 148) k_mix_narrow<1><<<grid_tiles(ci.nf, 256, n), 256, 0, s>>>(d, e, n, ci);
+        if (ctas4 < 2 * g_num_sms) k_mix_narrow<1><<<grid_tiles(ci.nf, 256, n), 256, 0, s>>>(d, e, n, ci);
         else k_mix_narrow<4><<<grid_tiles(ci.nf, 1024, n), 256, 0, s>>>(d, e, n, ci);
         return;
     }
-    if (ctas4 < 2 * 148) k_mix<1><<<grid_tiles(ci.nf, 256, n), 256, 0, s>>>(d, e, n, ci);
+    if (ctas4 < 2 * g_num_sms) k_mix<1><<<grid_tiles(ci.nf, 256, n), 256, 0, s>>>(d, e, n, ci);
     else k_mix<4><<<grid_tiles(ci.nf, 1024, n), 256, 0, s>>>(d, e, n, ci);
 }
 void launch_mix_dyn(const MixDynInst* d, const MixEdge* e, int n, ChunkInfo ci, cudaStream_t s) { k_mix_dyn<<<grid_tiles(ci.nf, 512, n), 128, 0, s>>>(d, e, n, ci); }
@@ -4215,7 +4219,7 @@ void chain_set_prepass(int on) { g_chain_prepass = on != 0; }
 static void chain_env() {
     if (g_chain_tma < 0) {
         const char* e = getenv("WAE_CHAIN_TMA");
-        g_chain_tma = e ? (atoi(e) != 0) : 0;  // measured on C2 (profiles/README.md r2_d): cp.async 1.39 ms, bulk copies 1.58 ms
+        g_chain_tma = e ? (atoi(e) != 0) : 0;  // default: the cp.async path (WAE_CHAIN_TMA=1 selects the bulk copies)
         e = getenv("WAE_CHAIN_WAVES");
         g_chain_waves = e ? atoi(e) : 20;
         if (g_chain_waves < 0) g_chain_waves = 0;
@@ -4226,13 +4230,13 @@ void chain_set_tuning(int tma, int waves) {
     if (tma >= 0) g_chain_tma = tma != 0;
     if (waves >= 0) g_chain_waves = waves;
 }
-// Time slabs of one launch: enough work items for `waves` waves of resident CTAs (148 SMs x 6), at least 8 tiles each.  Filtered
+// Time slabs of one launch: enough work items for `waves` waves of resident CTAs (SMs x 6), at least 8 tiles each.  Filtered
 // chains are only cut when the launch has enough (instance, channel) pairs to fill half the machine without it: the slabs of one
 // pair run one after the other (the state is handed over), so with few pairs more slabs would only add waiting CTAs.
 void chain_plan_slabs(int n, int max_ch, int nf, int nb, int* n_slabs, int* tiles_per_slab, int* pre_log2) {
     chain_env();
     const long ctas = (long)n * max_ch, tiles = (nf + CH_THREADS * CH_K - 1) / (CH_THREADS * CH_K);
-    const long slots = 148L * (WAE_CH_MINB * 128 / CH_THREADS);
+    const long slots = (long)g_num_sms * (WAE_CH_MINB * 128 / CH_THREADS);
     if (pre_log2) *pre_log2 = -1;
     // Few (instance, channel) pairs and a long render (64 files of two minutes instead of 1000 of ten seconds): the pairs alone leave
     // the machine empty and the slabs of one pair would wait for each other — unless every slab first finds out what it hands on
@@ -4341,7 +4345,7 @@ void launch_chain(int variant, const ChainInst* d, const ScanCoef* c, int n, int
         default: launch_chain_s<CHAIN_SRC_CONST>(nb, shaper, d, c, n, max_ch, ci, s, aux); break;
     }
 }
-int voice_sum_slots() { return 148 * (WAE_VS_MINB * 128 / CH_THREADS); }
+int voice_sum_slots() { return g_num_sms * (WAE_VS_MINB * 128 / CH_THREADS); }
 void launch_voice_sum(int nb, const ChainInst* d, const ScanCoef* c, const VoiceGroup* g, int n_groups, ChunkInfo ci, cudaStream_t s, ChainAux aux) {
     ChainSched sc{};
     const int n_tiles = (ci.nf + CH_THREADS * CH_K - 1) / (CH_THREADS * CH_K);

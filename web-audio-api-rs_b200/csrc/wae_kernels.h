@@ -1,4 +1,4 @@
-// Launch wrappers of the sm_100a kernels (wae_kernels.cu).
+// Launch wrappers of the sm_90a kernels (wae_kernels.cu).
 #pragma once
 #include "wae_device.h"
 
@@ -38,6 +38,7 @@ void launch_chain(int variant, const ChainInst* d, const ScanCoef* c, int n, int
 // [n_groups][aux.slab_stride tiles], state hand-off [voices][2][4]
 void launch_voice_sum(int nb, const ChainInst* d, const ScanCoef* c, const VoiceGroup* g, int n_groups, ChunkInfo ci, cudaStream_t s, ChainAux aux);
 int voice_sum_slots();  // resident CTAs of k_voice_sum on the machine (host: is a launch big enough to be worth it?)
+void set_num_sms(int n);  // SM count of the engine's device (launch geometry; 132 on an H100 SXM until an engine sets it)
 void chain_plan_slabs(int n, int max_ch, int nf, int nb, int* n_slabs, int* tiles_per_slab, int* pre_log2 = nullptr);  // launch geometry of k_chain (host); *pre_log2 >= 0: slabs publish their end state before they render
 void chain_set_prepass(int on);            // WAE_OPT_CHAIN_PREPASS / WAE_CHAIN_PREPASS (default on)
 void chain_set_tuning(int tma, int waves);  // < 0: keep (defaults: WAE_CHAIN_TMA / WAE_CHAIN_WAVES or 0 / 20)
