@@ -161,8 +161,17 @@ struct ShaperOsInst {
     int32_t n;           // curve length
     int32_t ch;
     int32_t factor;      // 2 or 4
-    int32_t pad;
+    // != 0: the input changes its channel count.  Before a processed quantum whose count differs from the one the resamplers were built
+    // for (initially 1) both are rebuilt with zero state (waveshaper.rs:409-420,527-531): history older than the last rebuild reads as
+    // zero, and the down-sampler's overlap (the dn_{q-1} term) is zero at the rebuild quantum itself.  1: the curve does not map 0 to 0,
+    // every quantum is processed (a silent one as ONE zero channel); 2: it does, silent quanta are not processed (waveshaper.rs:395-398).
+    // prev then holds [0] the count the resamplers were built for (0: not yet, i.e. 1), [1] processed quanta since the last rebuild
+    // (capped at 2) — both carried across chunks — followed by the table above and, at 2 nq + 2 + q, OS_INFO words of quantum q.
+    int32_t rebuild;
 };
+// k_shaper_os_prev -> k_shaper_os: per quantum, its channel count, whether it is processed, and the processed quanta since the last rebuild
+constexpr int32_t OS_INFO_PROCESSED = 0x40;
+constexpr int OS_INFO_SINCE_SHIFT = 8;
 
 struct SPanInst {
     BufRef in, out;
@@ -475,6 +484,25 @@ struct ConvPath {    // one FFTConvolver of the reference: (input channel, IR ch
     int32_t out_channel;
     int32_t accumulate;  // 1: out += (true-stereo mix-down, convolver.rs:436-452)
     int64_t limit;       // >= 0: `out` is the rendered PCM itself (the convolver is the destination's only input): frames from `limit` on do not exist
+};
+// Second path of a ConvolverNode with a ONE-channel response whose input switches between one and two channels (convolver.rs:343-400):
+// the reference's convolvers[1] is fed the R channel of the two-channel quanta only and freezes (history, partly filled block and all)
+// whenever the input is mono or silent.  Its input is therefore the STREAM of those quanta with the gaps removed: per chunk the map kernel
+// lists the chunk quanta it processes and advances the stream cursor, the stream window [previous full stream block | partial block
+// carried from the last chunk | new frames] is transformed block by block (a partial block again once it holds more frames, like the
+// reference re-transforms its partly filled block), the MAC / inverse transform run over the stream's blocks, and the output frames of
+// the new stream frames are scattered back to channel 1 of the quanta they came from.
+struct ConvCmpInst {
+    BufRef in;         // canonical PCM of the input (2 static channels, layout track)
+    ConvInput x;       // x.xring: input spectra at the stream's absolute block index (x.in / prev / in_channel unused)
+    ConvPath path;     // h, S, y ([window blocks][block] scratch), out (channel 1 = out_channel); input / accumulate / limit unused
+    int64_t* cursor;   // [1] frames fed to convolvers[1] so far (persistent)
+    float* carry;      // [2 block] the stream's last full block before the cursor | its partial block (persistent)
+    float* win;        // [(window blocks + 1) block] stream window of the chunk, from block cursor / block - 1 on (scratch)
+    int32_t* qmap;     // [quanta per chunk] chunk quanta processed this chunk, in order (scratch)
+    int64_t* wdesc;    // [2] cursor before the chunk, new frames of the chunk (scratch, written by the map kernel)
+    int32_t in_ch;     // static channels of `in`
+    int32_t pad;
 };
 
 }  // namespace wae

@@ -246,11 +246,11 @@ namespace {
 // (the order of the kinds is the launch order inside one level: mixes first; k_delay_mono before the delay reader that needs it)
 enum StageKind : int {
     S_MIX = 0, S_MIX_DYN, S_OSC, S_CONST, S_ABSN, S_BIQUAD, S_IIR, S_GAIN, S_SHAPER, S_SPAN, S_PAN, S_ROUTE, S_DELAY_MONO, S_DELAY, S_DELAY_WRITE, S_COMP, S_ANALYSER,
-    S_CONV_FFT, S_CONV_MAC, S_CONV_MAC_ACC, S_CHAIN, S_PARAM, S_OSC_AR, S_BIQUAD_AR, S_ABSN_SLOW, S_HRTF, S_PAN_DYN, S_ABSN_SERIAL, S_SHAPER_OS, S_META, S_VSUM, S_KINDS
+    S_CONV_FFT, S_CONV_MAC, S_CONV_MAC_ACC, S_CHAIN, S_PARAM, S_OSC_AR, S_BIQUAD_AR, S_ABSN_SLOW, S_HRTF, S_PAN_DYN, S_ABSN_SERIAL, S_SHAPER_OS, S_META, S_VSUM, S_CONV_CMP, S_KINDS
 };
 const char* kStageNames[S_KINDS] = {"k_mix", "k_mix_dyn", "k_oscillator", "k_constant", "k_buffer_source", "k_biquad_serial", "k_iir_serial", "k_gain",
                                     "k_shaper", "k_stereo_panner", "k_panner_eq", "k_route", "k_delay_mono", "k_delay_read", "k_ring_write", "k_compressor",
-                                    "k_analyser", "k_conv_fft_in", "k_conv_mac_ifft", "k_conv_mac_ifft(acc)", "k_chain", "k_param", "k_osc_arate", "k_biquad_arate", "k_buffer_source_slow", "k_hrtf_fir", "k_panner_dyn", "k_buffer_source_serial", "k_shaper_os", "k_meta", "k_voice_sum"};
+                                    "k_analyser", "k_conv_fft_in", "k_conv_mac_ifft", "k_conv_mac_ifft(acc)", "k_chain", "k_param", "k_osc_arate", "k_biquad_arate", "k_buffer_source_slow", "k_hrtf_fir", "k_panner_dyn", "k_buffer_source_serial", "k_shaper_os", "k_meta", "k_voice_sum", "k_conv_compact"};
 
 // host-side accumulation of instances for one (level, kind) stage
 struct StageBuild {
@@ -296,6 +296,7 @@ struct StageBuild {
     std::vector<MetaInst> meta;
     std::vector<ConvInput> conv_in;
     std::vector<ConvPath> conv_path;
+    std::vector<ConvCmpInst> conv_cmp;  // S_CONV_CMP: compacted second path of a mono-response convolver
     std::vector<VoiceGroup> vgroups;  // S_VSUM: groups of consecutive `chain` records
     int max_ch = 1;
 };
@@ -713,6 +714,7 @@ struct Planner {
         int32_t mono_len;
     };
     std::map<std::pair<uint32_t, uint32_t>, DelayRing> delay_rings;       // (graph, writer id)
+    std::map<std::pair<uint32_t, uint32_t>, int> conv_paths_seen;        // (graph, convolver id) -> 1: compacted second path, 2: ordinary one (all segments)
     bool dry = false;                     // sizing pass: count arena floats per frame, touch no device memory
     int group_graphs = 1;                 // graphs of the group being planned (k_voice_sum: are there enough work items?)
     // 0 off (default: measured slower than k_chain + k_mix on north_star), 1 when the launch is large enough,
@@ -952,6 +954,7 @@ static uint64_t digest_builds(const std::map<std::pair<int, int>, StageBuild>& b
         h = digest_vec(s.absn_serial, h); h = digest_vec(s.shaper_os, h); h = digest_vec(s.route, h); h = digest_vec(s.delay, h); h = digest_vec(s.comp, h);
         h = digest_vec(s.analyser, h); h = digest_vec(s.mix, h); h = digest_vec(s.mix_edges, h); h = digest_vec(s.mix_dyn, h); h = digest_vec(s.meta, h);
         h = digest_vec(s.conv_in, h); h = digest_vec(s.conv_path, h); h = digest_vec(s.vgroups, h);
+        if (!s.conv_cmp.empty()) h = digest_vec(s.conv_cmp, h);  // (only where it exists: the digests of plans without it stay comparable)
     }
     return h;
 }
@@ -1005,7 +1008,7 @@ static void merge_builds(Builds& dst, Builds& src) {
         append_vec(d.pan_dyn, s.pan_dyn); append_vec(d.absn_serial, s.absn_serial); append_vec(d.shaper_os, s.shaper_os); append_vec(d.route, s.route);
         append_vec(d.delay, s.delay); append_vec(d.comp, s.comp); append_vec(d.analyser, s.analyser); append_vec(d.mix, s.mix);
         append_vec(d.mix_edges, s.mix_edges); append_vec(d.mix_dyn, s.mix_dyn); append_vec(d.meta, s.meta); append_vec(d.conv_in, s.conv_in);
-        append_vec(d.conv_path, s.conv_path); append_vec(d.vgroups, s.vgroups);
+        append_vec(d.conv_path, s.conv_path); append_vec(d.vgroups, s.vgroups); append_vec(d.conv_cmp, s.conv_cmp);
         d.n_scan_coef += s.n_scan_coef;
         d.max_ch = std::max(d.max_ch, s.max_ch);
     }
@@ -1118,9 +1121,24 @@ bool Planner::plan_convolver(wae_graph* g, PNode& pn, int level, const BufRef* d
     }
     int Smax = *std::max_element(S.begin(), S.end());
     pn.out_ch = {ir_ch == 1 && in_ch == 1 ? 1 : 2};
-    if (in_lay.dyn() && ir_ch == 1 && in_lay.hi >= 2)
-        return bail(WAE_UNSUPPORTED, "a ConvolverNode with a mono response whose input changes between one and two channels is not lowered to the GPU "
-                                     "(the reference stops feeding its second convolver whenever the input is mono or silent, convolver.rs:378-400)");
+    // a mono response behind an input that switches between one and two channels: the reference feeds its second convolver the
+    // two-channel quanta only (convolver.rs:378-400), so input R -> output 1 runs as a compacted path of its own (ConvCmpInst)
+    const bool compact = in_lay.dyn() && ir_ch == 1 && in_lay.hi >= 2;
+    if (compact && in_ch != 2) return bail(WAE_UNSUPPORTED, "unsupported convolver channel routing");
+    if (ir_ch == 1 && in_ch == 2 && !ir_override) {
+        // the second convolver's history lives in the compacted path's stream state or in the ordinary path's input ring, not in both:
+        // a node whose input turns from a changing layout to a constant two-channel one (or back) at a suspend point cannot hand it on
+        int& seen = conv_paths_seen[{key_graph, key_node}];
+        seen |= compact ? 1 : 2;
+        if (seen == 3)
+            return bail(WAE_UNSUPPORTED, "a ConvolverNode with a mono response whose input changes between a constant two-channel layout and a "
+                                         "changing one at a suspend point is not lowered to the GPU (its second convolver's history would not "
+                                         "carry over, convolver.rs:378-400)");
+    }
+    // node state is keyed by its role, not by the order of the allocations: which of them happen depends on the input's layout, and that
+    // can change at a suspend point (a tone alone, then a stereo source added from the callback) while the history has to carry over
+    const uint32_t key_base = key_seq;
+    auto role = [&](uint32_t r) { key_seq = key_base + r; };
     // silent once the input has been silent for the length of the response (convolver.rs:357-366); channels from the routing table (:378-487)
     const bool conv_dyn = in_lay.dyn();
     // the destination's only input, same channel count, constant layout: the inverse transforms write the rendered PCM themselves
@@ -1130,6 +1148,10 @@ bool Planner::plan_convolver(wae_graph* g, PNode& pn, int level, const BufRef* d
     if (conv_dyn && Smax > 0) {
         const int oc = pn.out_ch[0];
         pn.out_lay = {Lay{(uint8_t)(in_lay.may_silent ? 1 : oc), (uint8_t)oc, (uint8_t)oc, (uint8_t)oc, in_lay.may_silent}};
+        if (compact)  // (a mono response: one output channel wherever the input has one)
+            pn.out_lay = {Lay{(uint8_t)(in_lay.may_silent || in_lay.lo < 2 ? 1 : 2), 2,
+                              // (a silent input quantum while the tail runs: a SOUNDING one-channel output)
+                              (uint8_t)(in_lay.may_silent || in_lay.nlo < 2 ? 1 : 2), 2, in_lay.may_silent}};
         MetaInst m{};
         m.in = pn.in_buf[0];
         m.out = pn.out_buf[0];
@@ -1138,6 +1160,7 @@ bool Planner::plan_convolver(wae_graph* g, PNode& pn, int level, const BufRef* d
         m.out_ch = oc;
         m.aux = ir_ch;
         m.tail_len = (int64_t)ir_len;
+        role(0);
         m.state = alloc<int64_t>(1, true, true);
         if (!m.state) return bail(WAE_OUT_OF_MEMORY, "out of device memory (convolver tail counter)");
         stage(level, S_META).meta.push_back(m);
@@ -1163,7 +1186,9 @@ bool Planner::plan_convolver(wae_graph* g, PNode& pn, int level, const BufRef* d
         if (!dry) cudaStreamSynchronize(eng->stream);  // `flat` is about to go out of scope
         spec.S = Smax;
         spec.channels = ir_ch;
-        spec.h = alloc<float2>((size_t)ir_ch * (Smax + WAE_CONV_H_PAD) * WAE_CONV_SPEC, true);  // (zeroed: the padding partitions of every channel)
+        // (zeroed: the padding partitions of every channel).  An asset shared by content, not node state: not drawn through the node's
+        // state keys, whose sequence would otherwise depend on whether this segment's plan found the spectra in the cache
+        spec.h = dry ? alloc<float2>(1) : b->dalloc<float2>((size_t)ir_ch * (Smax + WAE_CONV_H_PAD) * WAE_CONV_SPEC, true);
         if (!d_ir || !spec.h) return bail(WAE_OUT_OF_MEMORY, "out of device memory (IR spectra)");
         if (!dry) launch_conv_ir_fft(d_ir, (int64_t)ir_len, (int64_t)ir_len, spec.h, Smax, ir_ch, eng->stream);
         b->asset_bytes += (size_t)ir_ch * (Smax + WAE_CONV_H_PAD) * WAE_CONV_SPEC * 8;
@@ -1175,10 +1200,11 @@ bool Planner::plan_convolver(wae_graph* g, PNode& pn, int level, const BufRef* d
     int blocks_per_chunk = (int)((b->chunk + WAE_CONV_BLOCK - 1) / WAE_CONV_BLOCK);
     int ring_blocks = Smax + blocks_per_chunk;
     int in_base = (int)fs.conv_in.size();
-    for (int c = 0; c < in_ch; c++) {
+    for (int c = 0; c < (compact ? 1 : in_ch); c++) {
         ConvInput ci;
         ci.in = pn.in_buf[0];
         ci.in_channel = mono_mix ? -1 : c;
+        role(1 + 2 * (uint32_t)c);
         ci.prev = alloc<float>(WAE_CONV_BLOCK, true, true);
         ci.xring = alloc<float2>((size_t)ring_blocks * WAE_CONV_SPEC);
         ci.xring_blocks = ring_blocks;
@@ -1191,7 +1217,8 @@ bool Planner::plan_convolver(wae_graph* g, PNode& pn, int level, const BufRef* d
         int in, ir, out, acc;
     };
     std::vector<R> routes;
-    if (in_ch == 1 && ir_ch == 1) routes = {{0, 0, 0, 0}};
+    if (compact) routes = {{0, 0, 0, 0}};  // (+ the compacted path below)
+    else if (in_ch == 1 && ir_ch == 1) routes = {{0, 0, 0, 0}};
     else if (in_ch == 1 && ir_ch == 2) routes = {{0, 0, 0, 0}, {0, 1, 1, 0}};
     else if (in_ch == 2 && ir_ch == 1) routes = {{0, 0, 0, 0}, {1, 0, 1, 0}};
     else if (in_ch == 2 && ir_ch == 2) routes = {{0, 0, 0, 0}, {1, 1, 1, 0}};
@@ -1200,6 +1227,7 @@ bool Planner::plan_convolver(wae_graph* g, PNode& pn, int level, const BufRef* d
     else return bail(WAE_UNSUPPORTED, "unsupported convolver channel routing");
     (void)n_conv;
     for (auto& r : routes) {
+        role(12 + (uint32_t)(&r - routes.data()));
         ConvPath p;
         p.out = pn.out_buf[0];
         p.h = spec.h + ((size_t)r.ir * (Smax + WAE_CONV_H_PAD) + WAE_CONV_H_PAD_LO) * WAE_CONV_SPEC;
@@ -1216,9 +1244,35 @@ bool Planner::plan_convolver(wae_graph* g, PNode& pn, int level, const BufRef* d
         }
         stage(level, r.acc ? S_CONV_MAC_ACC : S_CONV_MAC).conv_path.push_back(p);
     }
+    if (compact) {
+        // stream frames of a chunk: at most the chunk's; with the partial block in front they touch one block more
+        const int wblocks = blocks_per_chunk + 1;
+        ConvCmpInst cc{};
+        cc.in = pn.in_buf[0];
+        cc.in_ch = in_ch;
+        cc.x.xring_blocks = Smax + wblocks;
+        role(16);  // (16 .. 22, in this order)
+        cc.x.xring = alloc<float2>((size_t)cc.x.xring_blocks * WAE_CONV_SPEC, true);  // (finite: the MAC multiplies stale slots by zero partitions)
+        cc.path.out = pn.out_buf[0];
+        cc.path.h = spec.h + (size_t)WAE_CONV_H_PAD_LO * WAE_CONV_SPEC;
+        cc.path.S = Smax;
+        cc.path.out_channel = 1;
+        cc.path.limit = -1;
+        cc.path.y = alloc<float2>((size_t)wblocks * WAE_CONV_SPEC);
+        cc.cursor = alloc<int64_t>(1, true, true);
+        cc.carry = alloc<float>(2 * WAE_CONV_BLOCK, true, true);
+        cc.win = alloc<float>((size_t)(wblocks + 1) * WAE_CONV_BLOCK);
+        cc.qmap = alloc<int32_t>((size_t)(b->chunk / 128 + 1));
+        cc.wdesc = alloc<int64_t>(2);
+        if (!cc.x.xring || !cc.path.y || !cc.cursor || !cc.carry || !cc.win || !cc.qmap || !cc.wdesc)
+            return bail(WAE_OUT_OF_MEMORY, "out of device memory (convolver, compacted path)");
+        b->arena_bytes += ((size_t)cc.x.xring_blocks + wblocks) * WAE_CONV_SPEC * 8 + (size_t)(wblocks + 1) * WAE_CONV_BLOCK * 4;
+        stage(level, S_CONV_CMP).conv_cmp.push_back(cc);
+    }
     // SURVEY §8(d): S*1025*8 B of input-history spectra per convolver-block of 1024 frames
     // (the reference's 1024-frame partitioning defines the algorithmic figure, whatever block size the kernels use)
-    if (!ir_override) algorithmic_bytes += (uint64_t)routes.size() * (uint64_t)((trimmed_len + 1023) / 1024) * 1025ull * 8ull * (uint64_t)((b->lq + 1023) / 1024);
+    role(32);  // (whatever the caller allocates next)
+    if (!ir_override) algorithmic_bytes += (uint64_t)(routes.size() + (compact ? 1 : 0)) * (uint64_t)((trimmed_len + 1023) / 1024) * 1025ull * 8ull * (uint64_t)((b->lq + 1023) / 1024);
     return true;
 }
 
@@ -2269,11 +2323,15 @@ bool Planner::plan_graph(wae_graph* g, uint32_t gi) {
                     // one channel of a silent quantum, which rebuilds the resamplers of a wider node (waveshaper.rs:395-420)
                     const bool freeze = in0.dyn() && keeps_silence && in0.nlo == in0.nhi && in0.nhi == ch;
                     const bool as_static = !in0.dyn() || (!keeps_silence && ch == 1 && in0.hi == 1);
-                    if (!freeze && !as_static)
-                        return bail(WAE_UNSUPPORTED, "an over-sampled WaveShaperNode whose input changes its channel count is not lowered to the GPU "
-                                                     "(the reference rebuilds its resamplers then, waveshaper.rs:409-420)");
+                    // every other dynamic input: the count of the processed quanta changes, and the resamplers are rebuilt with it
+                    const bool rebuild = !freeze && !as_static;
                     if (!need_out(ch)) return bail(WAE_OUT_OF_MEMORY, "out of device memory (arena)");
-                    if (freeze) out_like_input();
+                    if (freeze || (rebuild && keeps_silence)) {
+                        out_like_input();
+                    } else if (rebuild) {  // silent quanta processed: a sounding output with the input's count (one channel when silent)
+                        out_dynamic(shaper_lay(in0));
+                        if (p.out_buf[0].meta) meta_stage(L, META_SHAPER, p.in_buf[0], ch, p.out_buf[0], ch);
+                    }
                     const int factor = n.oversample == WAE_OVERSAMPLE_X2 ? 2 : 4;
                     auto& filt = os_filters[factor];
                     if (!filt.first) {
@@ -2296,6 +2354,11 @@ bool Planner::plan_graph(wae_graph* g, uint32_t gi) {
                     if (!so.hist || !so.f_up || !so.f_dn) return bail(WAE_OUT_OF_MEMORY, "out of device memory (over-sampled shaper)");
                     if (freeze) {
                         so.prev = alloc<int32_t>((size_t)(2 * (b->chunk / 128) + 2));
+                        if (!so.prev) return bail(WAE_OUT_OF_MEMORY, "out of device memory (over-sampled shaper)");
+                    }
+                    if (rebuild) {  // (the two words in front carry the resamplers' state across chunks and segments)
+                        so.rebuild = keeps_silence ? 2 : 1;
+                        so.prev = alloc<int32_t>((size_t)(2 + 3 * (b->chunk / 128) + 2), true, true);
                         if (!so.prev) return bail(WAE_OUT_OF_MEMORY, "out of device memory (over-sampled shaper)");
                     }
                     StageBuild& os = stage(L, S_SHAPER_OS);
@@ -3476,6 +3539,7 @@ static void prep_plan_group(wae_batch* b, wae_graph* const* graphs, int k, PrepS
                 case S_COMP: st.n = (int)s.comp.size(); st.d_a = up(b, s.comp); break;
                 case S_ANALYSER: st.n = (int)s.analyser.size(); st.d_a = up(b, s.analyser); break;
                 case S_CONV_FFT: st.n = (int)s.conv_in.size(); st.d_a = up(b, s.conv_in); last_conv_inputs = st.d_a; break;
+                case S_CONV_CMP: st.n = (int)s.conv_cmp.size(); st.d_a = up(b, s.conv_cmp); break;
                 case S_CONV_MAC:
                 case S_CONV_MAC_ACC:
                     st.n = (int)s.conv_path.size();
@@ -3522,7 +3586,7 @@ static wae_status prep_finish(wae_batch* b, PrepState& ps) {
     uint64_t launches = 0;
     for (auto& st : b->stages) {
         const uint64_t k = (st.kind == S_CONV_FFT || st.kind == S_CONV_MAC || st.kind == S_CONV_MAC_ACC || st.kind == S_SHAPER_OS) ? 2
-                           : st.kind == S_HRTF ? (st.n_b > 0 ? 3 : 2) : 1;
+                           : st.kind == S_HRTF ? (st.n_b > 0 ? 3 : 2) : st.kind == S_CONV_CMP ? 6 : 1;
         // per-quantum stages (class 1) launch once per render quantum of their segment, the others once per chunk of it
         const std::vector<int64_t>& sb = b->groups[st.group].seg_bounds;
         const int64_t seg_len = sb[st.seg + 1] - sb[st.seg];
@@ -3644,6 +3708,7 @@ static void launch_stage(wae_batch* b, Stage& st, ChunkInfo ci) {
         case S_CONV_FFT: launch_conv_fft_in((ConvInput*)st.d_a, st.n, ci, s); break;
         case S_CONV_MAC:
         case S_CONV_MAC_ACC: launch_conv_mac_ifft((ConvPath*)st.d_a, (ConvInput*)st.d_b, st.n, ci, s); break;
+        case S_CONV_CMP: launch_conv_compact((ConvCmpInst*)st.d_a, st.n, ci, s); break;
     }
 }
 

@@ -2595,18 +2595,34 @@ __global__ void __launch_bounds__(128) k_shaper_os(const ShaperOsInst* __restric
     const float* in = chan(p.in, c, ci);
     const float* hist = p.hist + 256 * c;
     int q_of[3] = {q - 2, q - 1, q};
+    int since = 2;  // processed quanta since the resamplers were (re)built, before q (capped at 2; always 2 without rebuilds)
     if (p.prev) {  // silent quanta are not processed at all (block-uniform): the neighbours are the last processed quanta
-        if (buf_silent(p.in, p.ch, meta_qi(ci, q * 128))) {
+        const int32_t* pv = p.prev;
+        bool skip;
+        if (p.rebuild) {
+            pv = p.prev + 2;
+            const int32_t info = pv[2 * (ci.nf / 128) + 2 + q];
+            skip = !(info & OS_INFO_PROCESSED);
+            if (!skip && c >= (info & 0x3f)) return;  // (no such channel in this quantum: unspecified)
+            since = info >> OS_INFO_SINCE_SHIFT;
+        } else {
+            skip = buf_silent(p.in, p.ch, meta_qi(ci, q * 128));
+        }
+        if (skip) {
             chan(p.out, c, ci)[q * 128 + t] = 0.f;
             return;
         }
-        q_of[0] = p.prev[2 * q + 1];
-        q_of[1] = p.prev[2 * q];
+        q_of[0] = pv[2 * q + 1];
+        q_of[1] = pv[2 * q];
     }
     // three up-transforms: quanta q-2, q-1, q
     for (int r = 0; r < 3; r++) {
         const int qq = q_of[r];
-        float x = qq >= 0 ? in[qq * 128 + t] : hist[(qq + 2) * 128 + t];
+        float x;
+        if (r < 2 - since) x = 0.f;  // older than the last rebuild
+        else if (qq < 0) x = hist[(qq + 2) * 128 + t];
+        else if (p.rebuild && buf_silent(p.in, p.ch, meta_qi(ci, qq * 128))) x = 0.f;  // a processed silent quantum: one zero channel
+        else x = in[qq * 128 + t];
         z[t] = make_float2(x, 0.f);
         z[128 + t] = make_float2(0.f, 0.f);
         __syncthreads();
@@ -2635,7 +2651,8 @@ __global__ void __launch_bounds__(128) k_shaper_os(const ShaperOsInst* __restric
         else result = z[t].x;
         __syncthreads();
     }
-    chan(p.out, c, ci)[q * 128 + t] = result + dn_prev[t];
+    // (at a rebuild the fresh down-sampler's overlap is zero in the SHAPED domain: not the transform of curve(0))
+    chan(p.out, c, ci)[q * 128 + t] = since > 0 ? result + dn_prev[t] : result;
 }
 // dynamic input layout: the processed quanta before every quantum of the chunk (ShaperOsInst::prev), one thread per instance
 __global__ void __launch_bounds__(64) k_shaper_os_prev(const ShaperOsInst* __restrict__ insts, int n_inst, ChunkInfo ci) {
@@ -2645,6 +2662,34 @@ __global__ void __launch_bounds__(64) k_shaper_os_prev(const ShaperOsInst* __res
     if (!p.prev) return;
     int last1 = -1, last2 = -2;
     const int nq = ci.nf / 128;
+    if (p.rebuild) {  // + which quanta are processed, their counts, the rebuilds (waveshaper.rs:395-420)
+        int32_t* pv = p.prev + 2;
+        int built = p.prev[0] ? p.prev[0] : 1, since = p.prev[1];
+        for (int q = 0; q < nq; q++) {
+            pv[2 * q] = last1;
+            pv[2 * q + 1] = last2;
+            const int qi = meta_qi(ci, q * 128);
+            const bool silent = buf_silent(p.in, p.ch, qi);
+            int32_t info = 0;
+            if (!silent || p.rebuild == 1) {
+                const int count = silent ? 1 : buf_count(p.in, p.ch, qi);
+                if (count != built) {
+                    built = count;
+                    since = 0;
+                }
+                info = OS_INFO_PROCESSED | count | since << OS_INFO_SINCE_SHIFT;
+                since = since < 2 ? since + 1 : 2;
+                last2 = last1;
+                last1 = q;
+            }
+            pv[2 * nq + 2 + q] = info;
+        }
+        pv[2 * nq] = last1;
+        pv[2 * nq + 1] = last2;
+        p.prev[0] = built;
+        p.prev[1] = since;
+        return;
+    }
     for (int q = 0; q < nq; q++) {
         p.prev[2 * q] = last1;
         p.prev[2 * q + 1] = last2;
@@ -2663,9 +2708,16 @@ __global__ void __launch_bounds__(256) k_shaper_os_hist(const ShaperOsInst* __re
     for (int c = 0; c < p.ch; c++) {
         if (p.prev) {  // the two PROCESSED quanta before the next chunk: slot 1 (t >= 128) the latest, slot 0 the one before
             const int nq = ci.nf / 128;
-            const int qq = t >= 128 ? p.prev[2 * nq] : p.prev[2 * nq + 1];
+            const int32_t* pv = p.rebuild ? p.prev + 2 : p.prev;
+            const int qq = t >= 128 ? pv[2 * nq] : pv[2 * nq + 1];
             const int i = t & 127;
-            const float v = qq >= 0 ? chan(p.in, c, ci)[qq * 128 + i] : p.hist[256 * c + (qq + 2) * 128 + i];
+            float v;
+            if (p.rebuild && (t >= 128 ? 1 : 2) > p.prev[1]) v = 0.f;  // older than the last rebuild
+            else if (qq < 0) v = p.hist[256 * c + (qq + 2) * 128 + i];
+            else if (p.rebuild && (!(pv[2 * nq + 2 + qq] & OS_INFO_PROCESSED) || c >= (pv[2 * nq + 2 + qq] & 0x3f) ||
+                                   buf_silent(p.in, p.ch, meta_qi(ci, qq * 128))))
+                v = 0.f;  // a processed silent quantum (one zero channel) / a channel the quantum does not have
+            else v = chan(p.in, c, ci)[qq * 128 + i];
             __syncthreads();
             p.hist[256 * c + t] = v;
             __syncthreads();
@@ -4016,6 +4068,139 @@ __global__ void __launch_bounds__(CV_THREADS, 3) k_conv_ifft(const ConvPath* __r
     }
 }
 
+// ---- compacted second path of a mono-response convolver (ConvCmpInst, convolver.rs:378-400) -------------------------------------
+// The stream is what the reference's convolvers[1] is fed: channel 1 of the chunk quanta that are not silent and have two channels.
+// Stream frame s of the chunk's new frames (s - c0 = k) is chunk frame qmap[k / 128] * 128 + k % 128; the cursor c0 is a multiple of 128.
+// Window frame w is stream frame (c0 / B - 1) * B + w: [last full block before c0 | partial block | new frames | zeros].  The grids are
+// sized for the largest window (a chunk of nothing but two-channel quanta); CTAs past the chunk's own window exit.
+
+// which chunk quanta convolvers[1] processes, and the stream cursor.  One warp per instance: 32 quanta per step, their positions in
+// the list by a ballot and a population count.
+__global__ void __launch_bounds__(128) k_conv_cmp_map(const ConvCmpInst* __restrict__ insts, int n_inst, ChunkInfo ci) {
+    const int ii = blockIdx.x * 4 + (threadIdx.x >> 5);
+    if (ii >= n_inst) return;
+    const int lane = threadIdx.x & 31;
+    const ConvCmpInst& p = insts[ii];
+    const int nq = ci.nf / 128;
+    int n_proc = 0;
+    for (int q0 = 0; q0 < nq; q0 += 32) {
+        const int q = q0 + lane;
+        bool fed = false;
+        if (q < nq) {
+            const int qi = meta_qi(ci, q * 128);
+            fed = !buf_silent(p.in, p.in_ch, qi) && buf_count(p.in, p.in_ch, qi) >= 2;
+        }
+        const unsigned m = __ballot_sync(0xffffffffu, fed);
+        if (fed) p.qmap[n_proc + __popc(m & ((1u << lane) - 1u))] = q;
+        n_proc += __popc(m);
+    }
+    if (lane == 0) {
+        const int64_t c0 = *p.cursor;
+        p.wdesc[0] = c0;
+        p.wdesc[1] = (int64_t)n_proc * 128;
+        *p.cursor = c0 + (int64_t)n_proc * 128;
+    }
+}
+// the stream window of the chunk.  grid: (window frames / 256, instances)
+__global__ void __launch_bounds__(256) k_conv_cmp_gather(const ConvCmpInst* __restrict__ insts, ChunkInfo ci) {
+    const ConvCmpInst& p = insts[blockIdx.y];
+    const int64_t c0 = p.wdesc[0], n_new = p.wdesc[1];
+    const int64_t w = (int64_t)blockIdx.x * 256 + threadIdx.x;
+    const int64_t carried = CV_B + c0 % CV_B;  // last full block + partial block
+    float v = 0.f;
+    if (w < carried) {
+        v = p.carry[w];
+    } else if (w - carried < n_new) {
+        const int k = (int)(w - carried);
+        v = chan(p.in, 1, ci)[p.qmap[k >> 7] * 128 + (k & 127)];
+    }
+    p.win[w] = v;
+}
+// X_j of every stream block j the chunk's new frames reach (the partial one zero-padded), stored at the stream's absolute block index.
+// grid: (window blocks, instances)
+__global__ void __launch_bounds__(CV_THREADS, 3) k_conv_cmp_fft(const ConvCmpInst* __restrict__ insts, ChunkInfo ci) {
+    extern __shared__ float2 z[];
+    const ConvCmpInst& p = insts[blockIdx.y];
+    const int64_t c0 = p.wdesc[0], c1 = c0 + p.wdesc[1];
+    const int jb = blockIdx.x;
+    const int64_t j = c0 / CV_B + jb;
+    if (c1 == c0 || j * CV_B >= c1) return;
+    const FftTw w = fft_tw_load(-1);
+    const float2 lane_tw = cv_lane_tw();
+    const float* win = p.win + (size_t)jb * CV_B;  // window block jb = stream block j - 1
+    const int64_t left = c1 - j * CV_B;
+    conv_load_half(z, 0, win, CV_B);
+    conv_load_half(z, CV_B / 2, win + CV_B, (int)(left < CV_B ? left : CV_B));
+    __syncthreads();
+    fft_dif_smem(z, w);
+    rfft_store(z, p.x.xring + (size_t)(j % p.x.xring_blocks) * CV_BINS, lane_tw);
+}
+// the last full stream block and the partial block for the next chunk's window.  grid: (2 B / 256, instances)
+__global__ void __launch_bounds__(256) k_conv_cmp_carry(const ConvCmpInst* __restrict__ insts) {
+    const ConvCmpInst& p = insts[blockIdx.y];
+    const int64_t c0 = p.wdesc[0], c1 = c0 + p.wdesc[1];
+    const int64_t first = (c1 / CV_B - c0 / CV_B) * CV_B;  // window frame of stream block c1 / B - 1
+    const int i = blockIdx.x * 256 + threadIdx.x;
+    p.carry[i] = p.win[first + i];
+}
+// Y_j = sum_i H_i X_{j-i} for the stream blocks of the window (conv_mac_bin of k_conv_mac).  grid: (B / 256 * groups of CV_J blocks, instances)
+__global__ void __launch_bounds__(CV_MAC_THREADS, WAE_CV_MAC_MINB) k_conv_cmp_mac(const ConvCmpInst* __restrict__ insts, ChunkInfo ci) {
+    const int64_t c0 = insts[blockIdx.y].wdesc[0], c1 = c0 + insts[blockIdx.y].wdesc[1];
+    if (c1 == c0) return;
+    const int64_t jfirst = c0 / CV_B, jlast = (c1 - 1) / CV_B;
+    constexpr int TILES = CV_B / CV_MAC_THREADS;
+    const int k = (blockIdx.x % TILES) * CV_MAC_THREADS + threadIdx.x;
+    const int j0 = (blockIdx.x / TILES) * CV_J;  // first output block of this CTA, window-relative
+    if (jfirst + j0 > jlast) return;
+    const ConvPath path = insts[blockIdx.y].path;
+    const ConvInput x = insts[blockIdx.y].x;
+    float2 acc[CV_J];
+#pragma unroll
+    for (int jj = 0; jj < CV_J; jj++) acc[jj] = make_float2(0.f, 0.f);
+    if (k == 0) conv_mac_bin<true>(path, x, k, jfirst + j0, jlast, acc);
+    else conv_mac_bin<false>(path, x, k, jfirst + j0, jlast, acc);
+#pragma unroll
+    for (int jj = 0; jj < CV_J; jj++)
+        if (jfirst + j0 + jj <= jlast) path.y[(size_t)(j0 + jj) * CV_BINS + k] = acc[jj];
+}
+// out_j = IFFT(Y_j)[B..2B) / 2B; the frames of the NEW stream frames go to channel 1 of the quanta they came from.  grid: (window blocks, instances)
+__global__ void __launch_bounds__(CV_THREADS, 3) k_conv_cmp_ifft(const ConvCmpInst* __restrict__ insts, ChunkInfo ci) {
+    extern __shared__ float2 z[];
+    const ConvCmpInst& p = insts[blockIdx.y];
+    const int64_t c0 = p.wdesc[0], c1 = c0 + p.wdesc[1];
+    const int jb = blockIdx.x;
+    const int64_t j = c0 / CV_B + jb;
+    if (c1 == c0 || j * CV_B >= c1) return;
+    const FftTw w = fft_tw_load(+1);
+    const float2 lane_tw = cv_lane_tw();
+    const float2* __restrict__ Y = p.path.y + (size_t)jb * CV_BINS;
+    const int t = threadIdx.x;
+#pragma unroll 4
+    for (int q = t; q < CV_B; q += CV_THREADS) {
+        float2 yk, ym;
+        if (q == 0) {
+            const float2 y0 = Y[0];
+            yk = make_float2(y0.x, 0.f);
+            ym = make_float2(y0.y, 0.f);
+        } else {
+            yk = Y[q];
+            ym = Y[cv_mirror(q)];
+        }
+        z[cv_pad(q)] = irfft_merge(yk, ym, cv_bin_tw(lane_tw, q));
+    }
+    __syncthreads();
+    fft_dit_smem(z, w);
+    const float scale = 1.f / (float)(2 * CV_B);
+    float* out = chan(p.path.out, p.path.out_channel, ci);
+    const int64_t b0 = j * CV_B;
+    const int lo = (int)((c0 > b0 ? c0 : b0) - b0), hi = (int)((c1 < b0 + CV_B ? c1 : b0 + CV_B) - b0);
+    for (int i = lo + t; i < hi; i += CV_THREADS) {
+        const float2 c = z[cv_pad(CV_B / 2 + (i >> 1))];
+        const int k = (int)(b0 + i - c0);
+        out[p.qmap[k >> 7] * 128 + (k & 127)] = ((i & 1) ? c.y : c.x) * scale;
+    }
+}
+
 // IR segment spectra H_i (host uploads the scaled IR; one CTA per segment), position order like X.  grid: (S, ir channels)
 __global__ void __launch_bounds__(CV_THREADS) k_conv_ir_fft(const float* __restrict__ ir, int64_t ir_len, int64_t ir_stride, float2* __restrict__ h,
                                                             int S) {
@@ -4438,6 +4623,8 @@ static void conv_configure() {
     cudaFuncSetAttribute(k_conv_fft_in, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     cudaFuncSetAttribute(k_conv_ifft, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     cudaFuncSetAttribute(k_conv_ir_fft, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    cudaFuncSetAttribute(k_conv_cmp_fft, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    cudaFuncSetAttribute(k_conv_cmp_ifft, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     configured = true;
 }
 void launch_conv_fft_in(const ConvInput* d, int n, ChunkInfo ci, cudaStream_t s) {
@@ -4451,6 +4638,17 @@ void launch_conv_mac_ifft(const ConvPath* p, const ConvInput* in, int n, ChunkIn
     const int nb = (ci.nf + CV_B - 1) / CV_B;
     k_conv_mac<<<dim3((unsigned)((CV_B / CV_MAC_THREADS) * ((nb + CV_J - 1) / CV_J)), (unsigned)n), CV_MAC_THREADS, 0, s>>>(p, in, n, ci);
     k_conv_ifft<<<dim3((unsigned)nb, (unsigned)n), CV_THREADS, CV_SMEM_ELEMS * sizeof(float2), s>>>(p, in, n, ci);
+}
+void launch_conv_compact(const ConvCmpInst* d, int n, ChunkInfo ci, cudaStream_t s) {
+    conv_configure();
+    const int wb = (ci.nf + CV_B - 1) / CV_B + 1;  // stream blocks the chunk's new frames can reach (the partial block in front: one more)
+    const size_t smem = CV_SMEM_ELEMS * sizeof(float2);
+    k_conv_cmp_map<<<(n + 3) / 4, 128, 0, s>>>(d, n, ci);
+    k_conv_cmp_gather<<<dim3((unsigned)((wb + 1) * (CV_B / 256)), (unsigned)n), 256, 0, s>>>(d, ci);
+    k_conv_cmp_fft<<<dim3((unsigned)wb, (unsigned)n), CV_THREADS, smem, s>>>(d, ci);
+    k_conv_cmp_carry<<<dim3(2 * CV_B / 256, (unsigned)n), 256, 0, s>>>(d);
+    k_conv_cmp_mac<<<dim3((unsigned)((CV_B / CV_MAC_THREADS) * ((wb + CV_J - 1) / CV_J)), (unsigned)n), CV_MAC_THREADS, 0, s>>>(d, ci);
+    k_conv_cmp_ifft<<<dim3((unsigned)wb, (unsigned)n), CV_THREADS, smem, s>>>(d, ci);
 }
 void launch_conv_ir_fft(const float* ir, int64_t ir_len, int64_t ir_stride, float2* h, int S, int channels, cudaStream_t s) {
     conv_configure();

@@ -64,6 +64,7 @@ void launch_compressor(const CompInst* d, int n, ChunkInfo ci, cudaStream_t s);
 void launch_analyser(const AnalyserInst* d, int n, ChunkInfo ci, cudaStream_t s);
 void launch_conv_fft_in(const ConvInput* d, int n, ChunkInfo ci, cudaStream_t s);
 void launch_conv_mac_ifft(const ConvPath* p, const ConvInput* in, int n, ChunkInfo ci, cudaStream_t s);
+void launch_conv_compact(const ConvCmpInst* d, int n, ChunkInfo ci, cudaStream_t s);
 void launch_conv_ir_fft(const float* ir, int64_t ir_len, int64_t ir_stride, float2* h, int S, int channels, cudaStream_t s);
 
 }  // namespace wae
