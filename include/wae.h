@@ -469,6 +469,31 @@ typedef struct wae_plan_info {
 } wae_plan_info;
 WAE_API wae_status wae_batch_plan(wae_graph* const* graphs, uint32_t n_graphs, wae_plan_info* info);
 
+/* ---- batches of contexts that differ in number_of_channels, length or sample_rate --------------------------------------------
+ * The calls above take graphs of one shape and refuse anything else.  The calls below take any mix.  Graphs are grouped by
+ * sample rate, suspend frames and length; a group renders all its graphs to its longest graph's length (whole quanta), and the
+ * shortest graph of a group is at least 3/4 of the longest.  Each graph's output, analyser and compressor read-outs are exactly
+ * what it renders alone.  A batch whose graphs all share one shape is planned exactly as by wae_batch_prepare / wae_batch_plan. */
+
+/* OfflineAudioContext::start_rendering_sync for each graph, in one call: outs[i] = [channels_i][length_i] f32 host memory (pageable
+ * or page-locked) of graph i.  Synchronous. */
+WAE_API wae_status wae_render_many(wae_engine* engine, wae_graph* const* graphs, uint32_t n_graphs, float* const* outs);
+/* wae_batch_prepare for any mix of shapes.  run / run_group / sync / stats / destroy, the analyser read-outs and
+ * wae_compressor_reduction work on the batch (graph_index = the graph's index in `graphs`).  The device output is packed: see
+ * wae_batch_graph_output.  On a batch whose graphs differ in shape wae_batch_fetch and wae_batch_run_pipelined answer
+ * WAE_INVALID_STATE, and the ranges of wae_batch_group_range index the batch's own order (graphs sorted into groups). */
+WAE_API wae_status wae_batch_prepare_many(wae_engine* engine, wae_graph* const* graphs, uint32_t n_graphs, wae_batch** out_batch);
+/* where graph `graph_index` lies in wae_batch_output_device_ptr's buffer: [channels][length] f32 from offset_floats on */
+WAE_API wae_status wae_batch_graph_output(wae_batch* batch, uint32_t graph_index, uint64_t* offset_floats, uint32_t* channels, uint64_t* length);
+/* D2H of one graph's rendered PCM into `out` ([channels][length] f32) */
+WAE_API wae_status wae_batch_fetch_graph(wae_batch* batch, uint32_t graph_index, float* out);
+/* wae_batch_plan for any mix of shapes (host only) */
+WAE_API wae_status wae_batch_plan_many(wae_graph* const* graphs, uint32_t n_graphs, wae_plan_info* info);
+/* The grouping wae_batch_plan_many / wae_batch_prepare_many / wae_render_many make under the default engine options (host only):
+ * group_of[i] (may be NULL; n_graphs entries) = the group of graph i; *rendered = render quanta over all graphs (each graph rendered
+ * to its group's length); *needed = the sum over graphs of ceil(length_i / 128). */
+WAE_API wae_status wae_batch_plan_quanta(wae_graph* const* graphs, uint32_t n_graphs, uint32_t* group_of, uint64_t* rendered, uint64_t* needed);
+
 /* PeriodicWave::new(context, PeriodicWaveOptions { real, imag, disable_normalization }) (src/periodic_wave.rs:104-209): fills `table`
  * (PERIODIC_WAVE_TABLE_LENGTH = 2048 in the reference) with the wavetable an OscillatorNode of type Custom plays.  `real` / `imag` may be
  * NULL (= zeros); both NULL = the sine default.  Host math, no engine needed. */

@@ -155,6 +155,7 @@ WAE_SYMBOLS = [
     "wae_param_sim_set_automation_rate", "wae_param_sim_compute", "wae_biquad_coefs", "wae_biquad_frequency_response", "wae_iir_frequency_response",
     "wae_node_set_channel_count", "wae_node_set_channel_count_mode", "wae_node_set_channel_interpretation", "wae_graph_render_order", "wae_hrir_resample", "wae_batch_plan", "wae_buffer_source_set_buffer", "wae_convolver_set_buffer", "wae_wave_shaper_set_curve",
     "wae_oscillator_set_periodic_wave", "wae_node_set_attribute", "wae_disconnect_from", "wae_disconnect_param", "wae_periodic_wave_table", "wae_param_sim_set_walker", "wae_sched_first_frame_at_or_after", "wae_spatial_params", "wae_hrtf_locate",
+    "wae_render_many", "wae_batch_prepare_many", "wae_batch_graph_output", "wae_batch_fetch_graph", "wae_batch_plan_many", "wae_batch_plan_quanta",
 ]
 
 
@@ -248,6 +249,13 @@ class Api:
             f("analyser_get_byte_frequency_data", C.c_int32, [C.c_void_p, C.c_uint32, C.c_uint32, C.POINTER(C.c_uint8), C.c_uint32])
             f("engine_set_hrir_sphere", C.c_int32, [C.c_void_p, C.c_void_p, C.c_uint64])
             f("resample_linear", C.c_int32, [C.c_void_p, c_float_p, C.c_uint64, C.c_float, C.c_float, c_float_p, C.c_uint64, C.POINTER(C.c_uint64)])
+            # contexts of different shapes in one batch
+            f("render_many", C.c_int32, [C.c_void_p, C.POINTER(C.c_void_p), C.c_uint32, C.POINTER(c_float_p)])
+            f("batch_prepare_many", C.c_int32, [C.c_void_p, C.POINTER(C.c_void_p), C.c_uint32, C.POINTER(C.c_void_p)])
+            f("batch_graph_output", C.c_int32, [C.c_void_p, C.c_uint32, C.POINTER(C.c_uint64), C.POINTER(C.c_uint32), C.POINTER(C.c_uint64)])
+            f("batch_fetch_graph", C.c_int32, [C.c_void_p, C.c_uint32, c_float_p])
+            f("batch_plan_many", C.c_int32, [C.POINTER(C.c_void_p), C.c_uint32, C.POINTER(PlanInfo)])
+            f("batch_plan_quanta", C.c_int32, [C.POINTER(C.c_void_p), C.c_uint32, C.POINTER(C.c_uint32), C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)])
         else:
             f("graph_create", C.c_int32, [C.c_uint32, C.c_uint64, C.c_float, C.POINTER(C.c_void_p)])
             f("render", C.c_int32, [gp, c_float_p])

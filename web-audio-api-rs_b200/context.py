@@ -629,9 +629,10 @@ class OfflineAudioContext:
 
 
 class Batch:
-    """wae_batch_prepare / run / fetch: a compiled batch of contexts (product only)."""
+    """wae_batch_prepare / run / fetch: a compiled batch of contexts (product only).  many=True: wae_batch_prepare_many, contexts of
+    any mix of channel counts, lengths and sample rates (read each one's PCM with fetch_graph)."""
 
-    def __init__(self, contexts):
+    def __init__(self, contexts, many=False):
         ctx0 = contexts[0]
         self.api = ctx0._api
         self.contexts = contexts
@@ -641,7 +642,8 @@ class Batch:
             c._run_suspend_callbacks()
         arr = (C.c_void_p * self.n)(*[c._g for c in contexts])
         h = C.c_void_p()
-        self.api.check(self.api.batch_prepare(ctx0._backend.engine, arr, self.n, C.byref(h)))
+        prepare = self.api.batch_prepare_many if many else self.api.batch_prepare
+        self.api.check(prepare(ctx0._backend.engine, arr, self.n, C.byref(h)))
         self.handle = h
         self._backend = ctx0._backend
         self._backend.batches.add(self)
@@ -683,6 +685,21 @@ class Batch:
         if out is None:
             out = np.empty((self.n, self.channels, self.length), np.float32)
         self.api.check(self.api.batch_fetch(self.handle, out.ctypes.data_as(C.c_void_p)))
+        return out
+
+    def graph_output(self, i):
+        """(offset in floats, channels, length) of context i in the packed device output (device_ptr)."""
+        off, ch, length = C.c_uint64(), C.c_uint32(), C.c_uint64()
+        self.api.check(self.api.batch_graph_output(self.handle, i, C.byref(off), C.byref(ch), C.byref(length)))
+        return off.value, ch.value, length.value
+
+    def fetch_graph(self, i, out=None):
+        """context i's rendered PCM, [channels][length] float32."""
+        _, ch, length = self.graph_output(i)
+        if out is None:
+            out = np.empty((ch, length), np.float32)
+        assert out.dtype == np.float32 and out.flags.c_contiguous and out.size >= ch * length
+        self.api.check(self.api.batch_fetch_graph(self.handle, i, B.fptr(out)))
         return out
 
     def device_ptr(self):
@@ -729,6 +746,10 @@ def plan_batch(contexts):
     arr = (C.c_void_p * len(contexts))(*[c._g for c in contexts])
     info = B.PlanInfo()
     api.check(api.batch_plan(arr, len(contexts), C.byref(info)))
+    return _plan_dict(info)
+
+
+def _plan_dict(info):
     kinds = {}
     for part in info.stage_kinds.decode().split(", "):
         if part:
@@ -737,6 +758,52 @@ def plan_batch(contexts):
     return {"groups": info.groups, "segments": info.segments, "stages": info.stages, "has_feedback": bool(info.has_feedback),
             "chunk_frames": info.chunk_frames, "chunks": info.chunks, "arena_floats_per_frame": info.arena_floats_per_frame,
             "source_floats": info.source_floats, "kinds": kinds}
+
+
+def plan_many(contexts):
+    """wae_batch_plan_many: plan_batch for contexts of any mix of shapes -> the same dict, plus the grouping: "group_of" (the group of
+    each context), "rendered_quanta" (each context rendered to its group's length) and "needed_quanta" (sum of ceil(length / 128))."""
+    api = contexts[0]._api
+    assert api.is_product
+    for c in contexts:
+        c._run_suspend_callbacks()
+    n = len(contexts)
+    arr = (C.c_void_p * n)(*[c._g for c in contexts])
+    info = B.PlanInfo()
+    api.check(api.batch_plan_many(arr, n, C.byref(info)))
+    group_of = (C.c_uint32 * n)()
+    rendered, needed = C.c_uint64(), C.c_uint64()
+    api.check(api.batch_plan_quanta(arr, n, group_of, C.byref(rendered), C.byref(needed)))
+    return dict(_plan_dict(info), group_of=list(group_of), rendered_quanta=rendered.value, needed_quanta=needed.value)
+
+
+def render_many(contexts, outs=None):
+    """ONE wae_render_many call for contexts of any mix of channel counts, lengths and sample rates -> a list of AudioBuffer, each of its
+    context's own shape.  `outs`: optional list of float32 arrays, outs[i] with at least channels_i * length_i contiguous floats
+    (pageable, or the numpy view of page-locked memory); the buffers then view them.  Product: one call; oracle (tests only): each
+    context rendered on its own."""
+    api = contexts[0]._api
+    for c in contexts:
+        c._run_suspend_callbacks()
+    n = len(contexts)
+    if outs is None:
+        outs = [np.empty((c._channels, c._length), np.float32) for c in contexts]
+    for c, o in zip(contexts, outs):
+        assert o.dtype == np.float32 and o.flags.c_contiguous and o.size >= c._channels * c._length
+    if api.is_product:
+        arr = (C.c_void_p * n)(*[c._g for c in contexts])
+        ptrs = (B.c_float_p * n)(*[B.fptr(o) for o in outs])
+        api.check(api.render_many(contexts[0]._backend.engine, arr, n, ptrs))
+    else:
+        for c, o in zip(contexts, outs):
+            secs = C.c_double()
+            one = (C.c_void_p * 1)(c._g)
+            api.check(api.render_many(one, 1, B.fptr(o), 1, C.byref(secs)))
+    result = []
+    for c, o in zip(contexts, outs):
+        pcm = o.reshape(-1)[:c._channels * c._length].reshape(c._channels, c._length)
+        result.append(AudioBuffer([pcm[k] for k in range(c._channels)], c._sample_rate))
+    return result
 
 
 def render_batch_oneshot(contexts, out=None):

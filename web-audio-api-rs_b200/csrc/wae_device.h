@@ -281,6 +281,7 @@ struct CompInst {
     int32_t delay_frames;  // (ring_size - 1) * 128
     float threshold, knee, ratio, attack, release, sample_rate;
     int32_t pad;
+    int64_t end;      // the graph's last rendered frame + 1: the detector state and `reduction` stop there (a shorter graph of a longer group)
     BufRef track[5];  // attack, knee, ratio, release, threshold: p != nullptr -> automated (k-rate: first value of a quantum)
 };
 
@@ -289,6 +290,7 @@ struct AnalyserInst {
     float* ring;  // 32768 + 128 floats (analysis.rs:74)
     int32_t ch;
     int32_t pad;
+    int64_t end;  // the graph's last rendered frame + 1: the ring is not written from there on (a shorter graph of a longer group)
 };
 
 
@@ -431,6 +433,7 @@ struct ChainInst {
     ConstInst cst;       // CHAIN_SRC_CONST (out unused)
     BufRef out;
     int64_t limit;       // frames >= limit are not written (destination); < 0: none
+    int64_t end;         // the graph's render end (its length in whole quanta): a work item starting there has nothing to render
     ChainBiquad bq[CHAIN_MAX_BIQUADS];
 };
 
@@ -474,6 +477,7 @@ struct ConvInput {   // one input channel of one convolver instance
     float2* xring;   // [xring_blocks][block] input spectra ring
     int32_t in_channel;
     int32_t xring_blocks;
+    int64_t end;     // the graph's render end (its length in whole quanta): input from there on is zero, blocks starting there are not built
 };
 struct ConvPath {    // one FFTConvolver of the reference: (input channel, IR channel) -> output channel
     BufRef out;
@@ -484,6 +488,7 @@ struct ConvPath {    // one FFTConvolver of the reference: (input channel, IR ch
     int32_t out_channel;
     int32_t accumulate;  // 1: out += (true-stereo mix-down, convolver.rs:436-452)
     int64_t limit;       // >= 0: `out` is the rendered PCM itself (the convolver is the destination's only input): frames from `limit` on do not exist
+    int64_t end;         // the graph's render end (its length in whole quanta): output blocks starting there are not computed
 };
 // Second path of a ConvolverNode with a ONE-channel response whose input switches between one and two channels (convolver.rs:343-400):
 // the reference's convolvers[1] is fed the R channel of the two-channel quanta only and freezes (history, partly filled block and all)

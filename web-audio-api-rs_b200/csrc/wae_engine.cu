@@ -327,6 +327,7 @@ struct AnalyserRec {
     float* d_db;        // read-out scratch
     bool computed;      // frequency data already computed for the end-of-render time (analysis.rs:353-361)
     double min_db, max_db;
+    int64_t lq;         // frames the graph renders (its own length padded to whole quanta): the ring's write index after the render
 };
 
 }  // namespace
@@ -334,12 +335,20 @@ struct AnalyserRec {
 struct wae_batch {
     wae_engine* engine = nullptr;
     uint32_t n_graphs = 0, channels = 0;
-    uint64_t length = 0;   // frames requested
-    int64_t lq = 0;        // frames rendered: whole quanta (src/render/thread.rs:273)
+    uint64_t length = 0;   // frames requested (the longest graph's when the graphs differ in shape)
+    int64_t lq = 0;        // frames rendered: whole quanta (src/render/thread.rs:273); the longest group's
     int64_t chunk = 0;     // frames per chunk
     std::vector<void*> allocs;
     std::vector<Stage> stages;
-    float* d_out = nullptr;  // [n_graphs][channels][length]
+    float* d_out = nullptr;  // packed: graph i (batch order) is [channels_i][length_i] at out_off[i]
+    std::vector<size_t> out_off;  // [n_graphs + 1] floats
+    // Graphs of different shapes (wae_batch_prepare_many / wae_render_many): the batch holds them sorted into groups, `order` maps
+    // the batch position to the caller's index and `pos` back.  Both are empty for a batch of one shape, which keeps the caller's order.
+    bool mixed = false;
+    std::vector<uint32_t> order, pos;
+    uint64_t needed_quanta = 0;  // sum over graphs of ceil(length / 128)
+    std::vector<std::pair<uint32_t, uint64_t>> shape;  // per graph (batch order): number_of_channels, length
+    uint32_t batch_pos(uint32_t caller_index) const { return pos.empty() ? caller_index : pos[caller_index]; }
     // state that must be reset before every run
     std::vector<std::pair<void*, size_t>> zero_on_run;
     std::vector<AnalyserRec> analysers;
@@ -351,6 +360,7 @@ struct wae_batch {
     // streams (wae_batch_run_pipelined).  All groups share the arena-sizing chunk.
     struct Group {
         uint32_t g0 = 0, g1 = 0;        // graphs [g0, g1)
+        int64_t lq = 0;                 // frames the group renders: its longest graph's length in whole quanta
         size_t stage0 = 0, stage1 = 0;  // stages [stage0, stage1) of `stages` (all segments)
         std::vector<std::pair<size_t, size_t>> seg_stages;  // per render segment: its stages
         std::vector<int64_t> seg_bounds;                    // 0 = b0 < b1 < ... < lq: the suspend frames of this group's graphs
@@ -749,7 +759,7 @@ struct Planner {
     template <typename T>
     T* alloc(size_t count, bool zero = false, bool rezero_on_run = false) {
         if (dry) return reinterpret_cast<T*>(uintptr_t(256));
-        if (seg_start == 0 && seg_end >= b->lq) return b->dalloc<T>(count, zero, rezero_on_run);  // no suspend point: no later plan looks it up
+        if (seg_start == 0 && seg_end >= lq) return b->dalloc<T>(count, zero, rezero_on_run);  // no suspend point: no later plan looks it up
         const wae_batch::StateKey key{key_graph, key_node, key_seq++, key_salt};
         const size_t bytes = count * sizeof(T);
         std::lock_guard<std::recursive_mutex> lk(b->mu);
@@ -812,6 +822,11 @@ struct Planner {
         return &r.tl;
     }
     int64_t seg_start = 0, seg_end = 0;
+    // frames the group renders (every kernel runs to here; buffers and tables are sized for it) and frames the graph being planned
+    // renders (its own length in whole quanta): a graph shorter than its group decides what depends on the end of ITS render
+    int64_t lq = 0, glq = 0;
+    // the graph's rendered PCM in the packed output: [channels][length], frames from `length` on are not written (limit)
+    BufRef dest_ref(const wae_graph* g, uint32_t gi) const { return BufRef{b->d_out + b->out_off[gi], (uint32_t)g->length, 1}; }
     void begin_segment(int64_t f0, int64_t f1) {
         seg_start = f0;
         seg_end = f1;
@@ -942,19 +957,44 @@ static uint64_t digest_vec(const std::vector<T>& v, uint64_t h) {
     }
     return fnv1a(v.data(), v.size() * sizeof(T), h);
 }
+// The records that carry a graph's end frame (`end`: k_chain, the convolver kernels, k_analyser, k_compressor) are digested without it,
+// so that the plan of a batch of one shape (where it is the render length) digests as it did before the field existed.  `skip`: the
+// offsets of the 8-byte fields left out of each record.
+template <typename T>
+static uint64_t digest_vec_skipping(const std::vector<T>& v, std::initializer_list<size_t> skip, uint64_t h) {
+    const uint64_t n = v.size();
+    h = fnv1a(&n, sizeof n, h);
+    if (v.empty()) return h;
+    std::vector<uint8_t> bytes;
+    bytes.reserve(v.size() * sizeof(T));
+    for (const T& x : v) {
+        const uint8_t* p = reinterpret_cast<const uint8_t*>(&x);
+        size_t at = 0;
+        for (size_t off : skip) {
+            bytes.insert(bytes.end(), p + at, p + off);
+            at = off + sizeof(int64_t);
+        }
+        bytes.insert(bytes.end(), p + at, p + sizeof(T));
+    }
+    return fnv1a(bytes.data(), bytes.size(), h);
+}
+template <typename T>
+static uint64_t digest_vec_without_end(const std::vector<T>& v, uint64_t h) { return digest_vec_skipping(v, {offsetof(T, end)}, h); }
+
 static uint64_t digest_builds(const std::map<std::pair<int, int>, StageBuild>& builds, uint64_t h) {
     for (auto& kv : builds) {
         const StageBuild& s = kv.second;
         const int key[6] = {kv.first.first, kv.first.second, s.cls, s.level, s.kind * 64 + s.variant, s.max_ch};
         h = fnv1a(key, sizeof key, h);
-        h = digest_vec(s.osc, h); h = digest_vec(s.cst, h); h = digest_vec(s.absn, h); h = digest_vec(s.biquad, h); h = digest_vec(s.chain, h);
+        h = digest_vec(s.osc, h); h = digest_vec(s.cst, h); h = digest_vec(s.absn, h); h = digest_vec(s.biquad, h); h = digest_vec_without_end(s.chain, h);
         h = digest_vec(s.param, h); h = digest_vec(s.osc_ar, h); h = digest_vec(s.biquad_ar, h); h = digest_vec(s.absn_slow, h);
         h = digest_vec(s.scan_coef, h); h = digest_vec(s.iir, h); h = digest_vec(s.gain, h); h = digest_vec(s.shaper, h); h = digest_vec(s.span, h);
         h = digest_vec(s.span_gains, h); h = digest_vec(s.pan, h); h = digest_vec(s.hrtf, h); h = digest_vec(s.hrtf_sel, h); h = digest_vec(s.pan_dyn, h);
-        h = digest_vec(s.absn_serial, h); h = digest_vec(s.shaper_os, h); h = digest_vec(s.route, h); h = digest_vec(s.delay, h); h = digest_vec(s.comp, h);
-        h = digest_vec(s.analyser, h); h = digest_vec(s.mix, h); h = digest_vec(s.mix_edges, h); h = digest_vec(s.mix_dyn, h); h = digest_vec(s.meta, h);
-        h = digest_vec(s.conv_in, h); h = digest_vec(s.conv_path, h); h = digest_vec(s.vgroups, h);
-        if (!s.conv_cmp.empty()) h = digest_vec(s.conv_cmp, h);  // (only where it exists: the digests of plans without it stay comparable)
+        h = digest_vec(s.absn_serial, h); h = digest_vec(s.shaper_os, h); h = digest_vec(s.route, h); h = digest_vec(s.delay, h); h = digest_vec_without_end(s.comp, h);
+        h = digest_vec_without_end(s.analyser, h); h = digest_vec(s.mix, h); h = digest_vec(s.mix_edges, h); h = digest_vec(s.mix_dyn, h); h = digest_vec(s.meta, h);
+        h = digest_vec_without_end(s.conv_in, h); h = digest_vec_without_end(s.conv_path, h); h = digest_vec(s.vgroups, h);
+        if (!s.conv_cmp.empty())
+            h = digest_vec_skipping(s.conv_cmp, {offsetof(ConvCmpInst, x) + offsetof(ConvInput, end), offsetof(ConvCmpInst, path) + offsetof(ConvPath, end)}, h);  // (only where it exists: the digests of plans without it stay comparable)
     }
     return h;
 }
@@ -1142,7 +1182,7 @@ bool Planner::plan_convolver(wae_graph* g, PNode& pn, int level, const BufRef* d
     // silent once the input has been silent for the length of the response (convolver.rs:357-366); channels from the routing table (:378-487)
     const bool conv_dyn = in_lay.dyn();
     // the destination's only input, same channel count, constant layout: the inverse transforms write the rendered PCM themselves
-    const bool direct = dest && !conv_dyn && Smax > 0 && pn.out_ch[0] == (int)b->channels;
+    const bool direct = dest && !conv_dyn && Smax > 0 && pn.out_ch[0] == (int)g->channels;
     pn.out_buf = {direct ? *dest : arena_buf(pn.out_ch[0], conv_dyn && Smax > 0)};
     pn.wrote_dest = direct;
     if (conv_dyn && Smax > 0) {
@@ -1208,6 +1248,7 @@ bool Planner::plan_convolver(wae_graph* g, PNode& pn, int level, const BufRef* d
         ci.prev = alloc<float>(WAE_CONV_BLOCK, true, true);
         ci.xring = alloc<float2>((size_t)ring_blocks * WAE_CONV_SPEC);
         ci.xring_blocks = ring_blocks;
+        ci.end = glq;
         if (!ci.prev || !ci.xring) return bail(WAE_OUT_OF_MEMORY, "out of device memory (convolver input spectra)");
         b->arena_bytes += (size_t)ring_blocks * WAE_CONV_SPEC * 8;
         fs.conv_in.push_back(ci);
@@ -1236,6 +1277,7 @@ bool Planner::plan_convolver(wae_graph* g, PNode& pn, int level, const BufRef* d
         p.out_channel = r.out;
         p.accumulate = r.acc;
         p.limit = direct ? dest_limit : -1;
+        p.end = glq;
         p.y = nullptr;
         if (Smax > 1) {  // (one partition: k_conv_ifft forms the product itself, there are no output spectra)
             p.y = alloc<float2>((size_t)blocks_per_chunk * WAE_CONV_SPEC);
@@ -1272,7 +1314,7 @@ bool Planner::plan_convolver(wae_graph* g, PNode& pn, int level, const BufRef* d
     // SURVEY §8(d): S*1025*8 B of input-history spectra per convolver-block of 1024 frames
     // (the reference's 1024-frame partitioning defines the algorithmic figure, whatever block size the kernels use)
     role(32);  // (whatever the caller allocates next)
-    if (!ir_override) algorithmic_bytes += (uint64_t)(routes.size() + (compact ? 1 : 0)) * (uint64_t)((trimmed_len + 1023) / 1024) * 1025ull * 8ull * (uint64_t)((b->lq + 1023) / 1024);
+    if (!ir_override) algorithmic_bytes += (uint64_t)(routes.size() + (compact ? 1 : 0)) * (uint64_t)((trimmed_len + 1023) / 1024) * 1025ull * 8ull * (uint64_t)((lq + 1023) / 1024);
     return true;
 }
 
@@ -1288,6 +1330,7 @@ Planner::PRef Planner::param_ref(wae_graph* g, uint32_t pid) {
 }
 
 bool Planner::plan_graph(wae_graph* g, uint32_t gi) {
+    glq = (int64_t)((g->length + 127) / 128 * 128);
     Orderer ord{g};
     ord.run();
     if (!ord.broken.empty()) has_feedback = true;  // feedback through a DelayNode: its levels are replayed quantum by quantum
@@ -1380,8 +1423,8 @@ bool Planner::plan_graph(wae_graph* g, uint32_t gi) {
             bool unit = true;
             for (int i = 0; i < 4; i++) unit = unit && ci.g[i] == 1.f;
             if (may_alias && ci.src_kind == CHAIN_SRC_ABSN && ci.n_biquad == 0 && !ci.has_shaper && unit && it->second.phase == 0 &&
-                !it->second.lay.dyn() && a.n_start == 0 && !a.loop && a.buf_offset == 0 && a.buf_len >= b->lq && a.buf_stride <= 0xffffffffll &&
-                seg_start == 0 && seg_end >= b->lq) {
+                !it->second.lay.dyn() && a.n_start == 0 && !a.loop && a.buf_offset == 0 && a.buf_len >= lq && a.buf_stride <= 0xffffffffll &&
+                seg_start == 0 && seg_end >= lq) {
                 sp.out_buf = {BufRef{const_cast<float*>(a.buf), (uint32_t)a.buf_stride, 1}};
                 pending.erase(it);
                 return true;
@@ -1418,7 +1461,7 @@ bool Planner::plan_graph(wae_graph* g, uint32_t gi) {
             // GPU work; a constant param is a scalar in its owner's instance
             auto& edges = p.in_edges[0];
             // (a render without suspend points never replays a timeline: a constant param needs no record at all — most params are)
-            if (seg_start == 0 && seg_end >= b->lq && edges.empty() && n.param.constant()) continue;
+            if (seg_start == 0 && seg_end >= lq && edges.empty() && n.param.constant()) continue;
             const ParamTimeline* tlp = param_timeline(gi, id, n.param, g->sample_rate);
             if (n.param.constant() && edges.empty()) continue;
             int level = 0;
@@ -1509,8 +1552,8 @@ bool Planner::plan_graph(wae_graph* g, uint32_t gi) {
                 if (chain_kind && computed_channels(n.cfg, sch) == sch && chain_accepts(it->second, n.kind)) {
                     extend = true;
                     fuse_src = it->first;
-                } else if (n.kind == K_DEST && b->length <= 0xffffffffull &&
-                           (sch == (int)b->channels || (sch == 1 && b->channels == 2 && n.cfg.interp == WAE_INTERPRETATION_SPEAKERS))) {
+                } else if (n.kind == K_DEST && g->length <= 0xffffffffull &&
+                           (sch == (int)g->channels || (sch == 1 && g->channels == 2 && n.cfg.interp == WAE_INTERPRETATION_SPEAKERS))) {
                     dest_direct = true;
                     fuse_src = it->first;
                 }
@@ -1529,7 +1572,7 @@ bool Planner::plan_graph(wae_graph* g, uint32_t gi) {
                 if ((int)edges.size() < 8) continue;
                 const int ch = computed_channels(n.cfg, 1);
                 if (!(ch == 1 || (ch == 2 && n.cfg.interp == WAE_INTERPRETATION_SPEAKERS))) continue;
-                if (n.kind == K_DEST && b->length > 0xffffffffull) continue;
+                if (n.kind == K_DEST && g->length > 0xffffffffull) continue;
                 const int64_t tiles = (seg_end - seg_start + 2047) / 2048;
                 if (voice_sum_mode() < 2 && tiles * (int64_t)group_graphs < 2 * (int64_t)voice_sum_slots()) continue;
                 int nb = -1;
@@ -1581,8 +1624,8 @@ bool Planner::plan_graph(wae_graph* g, uint32_t gi) {
                 vg.out_dup = ch;
                 vg.limit = -1;
                 if (is_dest) {
-                    vg.out = BufRef{b->d_out + (size_t)gi * b->channels * b->length, (uint32_t)b->length, 1};
-                    vg.limit = (int64_t)b->length;
+                    vg.out = dest_ref(g, gi);
+                    vg.limit = (int64_t)g->length;
                 } else {
                     vg.out = arena_buf(ch);
                     if (!vg.out.p) return bail(WAE_OUT_OF_MEMORY, "out of device memory (arena)");
@@ -1658,9 +1701,9 @@ bool Planner::plan_graph(wae_graph* g, uint32_t gi) {
                 m.edge_offset = (uint32_t)ms.mix_edges.size();
                 m.limit = -1;
                 if (is_dest) {
-                    m.out = BufRef{b->d_out + (size_t)gi * b->channels * b->length, (uint32_t)b->length, 1};
-                    m.limit = (int64_t)b->length;
-                    if (b->length > 0xffffffffull) return bail(WAE_UNSUPPORTED, "render length above 2^32 frames");
+                    m.out = dest_ref(g, gi);
+                    m.limit = (int64_t)g->length;
+                    if (g->length > 0xffffffffull) return bail(WAE_UNSUPPORTED, "render length above 2^32 frames");
                 } else {
                     m.out = arena_buf(ch, pl.dyn());
                     if (!m.out.p) return bail(WAE_OUT_OF_MEMORY, "out of device memory (arena)");
@@ -1682,9 +1725,9 @@ bool Planner::plan_graph(wae_graph* g, uint32_t gi) {
             m.edge_offset = (uint32_t)ms.mix_edges.size();
             m.limit = -1;
             if (is_dest) {
-                m.out = BufRef{b->d_out + (size_t)gi * b->channels * b->length, (uint32_t)b->length, 1};
-                m.limit = (int64_t)b->length;
-                if (b->length > 0xffffffffull) return bail(WAE_UNSUPPORTED, "render length above 2^32 frames");
+                m.out = dest_ref(g, gi);
+                m.limit = (int64_t)g->length;
+                if (g->length > 0xffffffffull) return bail(WAE_UNSUPPORTED, "render length above 2^32 frames");
             } else {
                 m.out = arena_buf(ch);
                 if (!m.out.p) return bail(WAE_OUT_OF_MEMORY, "out of device memory (arena)");
@@ -1711,7 +1754,7 @@ bool Planner::plan_graph(wae_graph* g, uint32_t gi) {
             }
         };
         // a scheduled source: `ch` channels inside [n_first, n_stop), one silent channel outside (never silent when it covers the render)
-        auto source_lay = [&](int64_t n_first, int64_t n_stop, int ch) { return (n_first <= 0 && n_stop >= b->lq) ? Lay::fixed(ch) : Lay::gated(ch); };
+        auto source_lay = [&](int64_t n_first, int64_t n_stop, int ch) { return (n_first <= 0 && n_stop >= glq) ? Lay::fixed(ch) : Lay::gated(ch); };
         auto source_meta = [&](int64_t n_first, int64_t n_stop, int ch) {
             MetaInst m{};
             m.out = p.out_buf[0];
@@ -1749,6 +1792,7 @@ bool Planner::plan_graph(wae_graph* g, uint32_t gi) {
             pc.inst.src_kind = kind;
             pc.inst.ch = ch;
             pc.inst.limit = -1;
+            pc.inst.end = glq;
             for (int i = 0; i < 4; i++) pc.inst.g[i] = 1.f;
             pc.ch = ch;
             pc.cls = cur_cls;
@@ -1769,20 +1813,20 @@ bool Planner::plan_graph(wae_graph* g, uint32_t gi) {
         };
         switch (n.kind) {
             case K_DEST: {
-                p.out_ch = {(int)b->channels};
+                p.out_ch = {(int)g->channels};
                 if (dest_direct) {  // the chain writes the rendered PCM itself (speaker up-mix 1->2 = copy, quantum.rs:301-305)
                     PendingChain pc = std::move(pending.at(fuse_src));
                     pending.erase(fuse_src);
-                    BufRef fin{b->d_out + (size_t)gi * b->channels * b->length, (uint32_t)b->length, 1};
+                    const BufRef fin = dest_ref(g, gi);
                     pc.inst.out = fin;
-                    pc.inst.limit = (int64_t)b->length;
-                    pc.inst.out_dup = (pc.ch == 1 && b->channels == 2) ? 2 : 0;
+                    pc.inst.limit = (int64_t)g->length;
+                    pc.inst.out_dup = (pc.ch == 1 && g->channels == 2) ? 2 : 0;
                     emit_chain(pc, L);
                     pn.at(fuse_src).out_buf = {fin};
                     p.in_buf[0] = fin;
                 }
                 p.out_buf = {p.in_buf[0]};
-                algorithmic_bytes += (uint64_t)b->channels * b->length * 4;  // destination write, SURVEY §8(d)
+                algorithmic_bytes += (uint64_t)g->channels * g->length * 4;  // destination write, SURVEY §8(d)
                 break;
             }
             case K_OSC: {
@@ -1979,7 +2023,7 @@ bool Planner::plan_graph(wae_graph* g, uint32_t gi) {
                     out_dynamic(Lay::gated(ch));  // when it plays depends on the automated rate: the kernel writes the layout track
                     a.out = p.out_buf[0];
                     stage(L, S_ABSN_SERIAL).absn_serial.push_back(a);
-                    algorithmic_bytes += (uint64_t)ch * 4ull * (uint64_t)std::min<int64_t>(b->lq, (int64_t)len);
+                    algorithmic_bytes += (uint64_t)ch * 4ull * (uint64_t)std::min<int64_t>(lq, (int64_t)len);
                     break;
                 }
                 if (!fast) {
@@ -2054,7 +2098,7 @@ bool Planner::plan_graph(wae_graph* g, uint32_t gi) {
                     std::vector<double> seg_bt{off};
                     if (n.loop && off < a.loop_end) {
                         const double ls2 = a.loop_start, le2 = a.loop_end, len2 = le2 - ls2, step = a.step;
-                        const int64_t n_end = std::min<int64_t>(b->lq, a.n_stop);
+                        const int64_t n_end = std::min<int64_t>(lq, a.n_stop);
                         int64_t m = 0;   // frames since n_first
                         double v = off;  // buffer_time of frame m
                         bool entered = false;
@@ -2105,7 +2149,7 @@ bool Planner::plan_graph(wae_graph* g, uint32_t gi) {
                         if (p.out_lay[0].dyn()) source_meta(n_first, n_end, ch);
                     }
                     stage(L, S_ABSN_SLOW).absn_slow.push_back(a);
-                    algorithmic_bytes += (uint64_t)ch * 4ull * (uint64_t)std::min<int64_t>(b->lq, (int64_t)len);
+                    algorithmic_bytes += (uint64_t)ch * 4ull * (uint64_t)std::min<int64_t>(lq, (int64_t)len);
                     break;
                 }
                 AbsnInst a{};
@@ -2122,7 +2166,7 @@ bool Planner::plan_graph(wae_graph* g, uint32_t gi) {
                     // the quantum after which the source has `ended`: the reference accumulates buffer_time += block_duration and stops
                     // once it reaches the buffer's duration (audio_buffer_source.rs:609,826-838) — replayed, not divided
                     const double block_duration = clock.dt * 128.;
-                    const int64_t max_q = (b->lq - a.n_start) / 128 + 2;
+                    const int64_t max_q = (lq - a.n_start) / 128 + 2;
                     int64_t played = 0;
                     double bt = 0.;
                     while (played < max_q) {
@@ -2144,7 +2188,7 @@ bool Planner::plan_graph(wae_graph* g, uint32_t gi) {
                     stage(L, S_ABSN).absn.push_back(a);
                 }
                 // compulsory read of the source PCM that is actually played
-                algorithmic_bytes += (uint64_t)ch * 4ull * (uint64_t)std::max<int64_t>(0, std::min<int64_t>(b->lq - a.n_start, n.loop ? b->lq : (int64_t)len));
+                algorithmic_bytes += (uint64_t)ch * 4ull * (uint64_t)std::max<int64_t>(0, std::min<int64_t>(lq - a.n_start, n.loop ? lq : (int64_t)len));
                 break;
             }
             case K_BIQUAD: {
@@ -2225,7 +2269,7 @@ bool Planner::plan_graph(wae_graph* g, uint32_t gi) {
                 std::vector<double> ff = n.feedforward, fb = n.feedback;  // iir_filter.rs:282-309
                 if (ff.size() < fb.size()) ff.resize(fb.size(), 0.);
                 if (ff.size() > fb.size()) fb.resize(ff.size(), 0.);
-                if (ff.size() <= 3 && !eng->serial_filters && !in0.dyn() && seg_start == 0 && seg_end >= b->lq) {
+                if (ff.size() <= 3 && !eng->serial_filters && !in0.dyn() && seg_start == 0 && seg_end >= lq) {
                     // Order <= 2 with a constant input layout: the same transfer function as a biquad — rendered by the time-parallel scan
                     // of k_chain (direct form I there, transposed direct form II in iir_filter.rs:386-407: the outputs differ in the last
                     // bits of the f64 arithmetic only) instead of one serial thread per channel.  With an input that can fall silent the
@@ -2421,7 +2465,7 @@ bool Planner::plan_graph(wae_graph* g, uint32_t gi) {
                 // (a static HRTF panner with a constant-layout input is lowered to the convolver kernels, which take their own output buffer)
                 static const bool hrtf_fft_on = [] { const char* e = getenv("WAE_HRTF_FFT"); return !e || atoi(e) != 0; }();
                 const bool hrtf_as_conv = n.panning_model == WAE_PANNING_HRTF && hrtf_fft_on && eng->sphere && !moving && !in0.dyn() && cur_cls != 1 &&
-                                          seg_start == 0 && seg_end >= b->lq && (ch == 1 || ch == 2);
+                                          seg_start == 0 && seg_end >= lq && (ch == 1 || ch == 2);
                 if (!hrtf_as_conv && !need_out(2)) return bail(WAE_OUT_OF_MEMORY, "out of device memory (arena)");
                 if (hrtf_as_conv) p.out_lay = {Lay::fixed(2)};
                 else out_dynamic(in0.may_silent ? Lay{1, 2, 2, 2, true} : Lay::fixed(2));  // panner.rs:698-708
@@ -2653,6 +2697,7 @@ bool Planner::plan_graph(wae_graph* g, uint32_t gi) {
                 c.threshold = th; c.knee = kn; c.ratio = ra; c.attack = at; c.release = re;
                 for (int i = 0; i < 5; i++) c.track[i] = cp[i].dyn ? cp[i].track : BufRef{nullptr, 0, 0};
                 c.sample_rate = g->sample_rate;
+                c.end = glq;
                 stage(L, S_COMP).comp.push_back(c);
                 if (!dry) {
                     std::lock_guard<std::recursive_mutex> lk(b->mu);  // (groups are planned on worker threads)
@@ -2673,6 +2718,7 @@ bool Planner::plan_graph(wae_graph* g, uint32_t gi) {
                 a.in = p.in_buf[0];
                 a.out = BufRef{nullptr, 0, 0};
                 a.ch = ch;
+                a.end = glq;
                 a.ring = alloc<float>(32768 + 128, true, true);
                 if (!a.ring) return bail(WAE_OUT_OF_MEMORY, "out of device memory (analyser ring)");
                 stage(L, S_ANALYSER).analyser.push_back(a);
@@ -2684,10 +2730,10 @@ bool Planner::plan_graph(wae_graph* g, uint32_t gi) {
                         std::lock_guard<std::recursive_mutex> lk(b->mu);
                         bool known = false;
                         for (auto& r : b->analysers) known = known || (r.graph_index == gi && r.node == id);
-                        if (!known) b->analysers.push_back(AnalyserRec{gi, id, a.ring, n.fft_size, n.smoothing, last, db, false, n.min_db, n.max_db});
+                        if (!known) b->analysers.push_back(AnalyserRec{gi, id, a.ring, n.fft_size, n.smoothing, last, db, false, n.min_db, n.max_db, glq});
                     }
                 }
-                algorithmic_bytes += (uint64_t)b->lq * 4;  // ring write, SURVEY §8(d)
+                algorithmic_bytes += (uint64_t)lq * 4;  // ring write, SURVEY §8(d)
                 break;
             }
             case K_MERGER: {
@@ -2744,18 +2790,18 @@ bool Planner::plan_graph(wae_graph* g, uint32_t gi) {
             case K_CONV: {
                 // the destination's only input (and this node's only consumer): the inverse transforms write the rendered PCM
                 const BufRef* dest = nullptr;
-                BufRef fin{b->d_out + (size_t)gi * b->channels * b->length, (uint32_t)b->length, 1};
-                if (fuse && cur_cls == 0 && b->length <= 0xffffffffull) {
+                const BufRef fin = dest_ref(g, gi);
+                if (fuse && cur_cls == 0 && g->length <= 0xffffffffull) {
                     int n_out = 0;
                     uint32_t to = 0;
                     int to_port = -1;
                     for (auto& e : ord.edges.at(id))
                         if (e.other_index >= 0) n_out++, to = e.other_id, to_port = e.other_index;
                     if (n_out == 1 && to_port == 0 && g->nodes.at(to).kind == K_DEST && pn.at(to).in_edges[0].size() == 1 &&
-                        computed_channels(g->nodes.at(to).cfg, (n.buffer && n.buffer->channels.size() == 1 && p.in_ch[0] == 1) ? 1 : 2) == (int)b->channels)
+                        computed_channels(g->nodes.at(to).cfg, (n.buffer && n.buffer->channels.size() == 1 && p.in_ch[0] == 1) ? 1 : 2) == (int)g->channels)
                         dest = &fin;
                 }
-                if (!plan_convolver(g, p, L, dest, (int64_t)b->length)) return false;
+                if (!plan_convolver(g, p, L, dest, (int64_t)g->length)) return false;
                 break;
             }
             default: return bail(WAE_UNSUPPORTED, "node kind not lowered to the GPU");
@@ -3006,14 +3052,87 @@ struct GroupPlan {  // result of phase B for one group
     std::string error;
 };
 
+static int64_t padded_length(const wae_graph* g) { return (int64_t)((g->length + 127) / 128 * 128); }
+
+// the suspend frames of a graph inside its own render
+static std::vector<int64_t> graph_cuts(const wae_graph* g) {
+    const int64_t lq = padded_length(g);
+    std::vector<int64_t> cuts;
+    for (auto& ep : g->epochs)
+        if ((int64_t)ep.frame > 0 && (int64_t)ep.frame < lq) cuts.push_back((int64_t)ep.frame);
+    return cuts;
+}
+
+// A group renders every graph to the group's longest padded length; a shorter graph's extra frames are dropped (the destination's
+// `limit`) or land in the arena, and the kernels whose state is read after the render stop at the graph's own end.  A group is at most
+// 4/3 of its shortest graph long: the shortest graph of a group is at least 3/4 of the longest.
+constexpr int64_t kGroupPadNum = 3, kGroupPadDen = 4;
+static bool fits_group(int64_t longest, int64_t lq) { return lq * kGroupPadDen >= longest * kGroupPadNum; }
+
+// Graph groups for the H2D / render / D2H pipeline: contiguous runs of graphs with the same suspend frames, the same sample rate and
+// lengths within the padding bound (in a batch of one shape only the suspend frames differ), cut further into about n_groups pieces.
+static std::vector<wae_batch::Group> form_groups(const wae_engine* eng, wae_graph* const* graphs, uint32_t n_graphs,
+                                                  const std::vector<std::vector<int64_t>>& cuts) {
+    int n_groups = eng->pipeline_groups;
+    if (n_groups == 0) n_groups = n_graphs >= 512 ? 32 : (n_graphs >= 64 ? 8 : 1);  // more groups = shorter fill / drain of the 3-stage pipeline
+    if (eng->pipeline_groups == 0 && n_graphs >= 512) {  // (tuning: WAE_AUTO_GROUPS overrides the automatic choice for large batches)
+        static const int env_groups = [] { const char* e = getenv("WAE_AUTO_GROUPS"); return e ? atoi(e) : 0; }();
+        if (env_groups > 0) n_groups = env_groups;
+    }
+    n_groups = std::max(1, std::min<int>(n_groups, (int)n_graphs));
+    const uint32_t target = (n_graphs + (uint32_t)n_groups - 1) / (uint32_t)n_groups;
+    std::vector<wae_batch::Group> groups;
+    uint32_t g0 = 0;
+    for (uint32_t i = 1; i <= n_graphs; i++)
+        if (i == n_graphs || cuts[i] != cuts[g0] || i - g0 >= target || graphs[i]->sample_rate != graphs[g0]->sample_rate ||
+            !fits_group(padded_length(graphs[g0]), padded_length(graphs[i]))) {
+            wae_batch::Group grp;
+            grp.g0 = g0;
+            grp.g1 = i;
+            for (uint32_t j = g0; j < i; j++) grp.lq = std::max(grp.lq, padded_length(graphs[j]));
+            grp.seg_bounds.push_back(0);
+            for (int64_t f : cuts[g0]) grp.seg_bounds.push_back(f);
+            grp.seg_bounds.push_back(grp.lq);
+            groups.push_back(std::move(grp));
+            g0 = i;
+        }
+    return groups;
+}
+
+// The batch order of graphs of different shapes: by sample rate, suspend frames, then longest first (the caller's order among equals),
+// so that the groups form_groups cuts are contiguous runs.  Empty when all graphs share one shape: that batch keeps the caller's order
+// and plans exactly as wae_batch_prepare plans it.
+static wae_status many_order(wae_graph* const* graphs, uint32_t n_graphs, std::vector<uint32_t>& order) {
+    order.clear();
+    if (!graphs || n_graphs == 0) return fail(WAE_INVALID_ARGUMENT, "null / empty batch");
+    bool uniform = true;
+    for (uint32_t i = 0; i < n_graphs; i++) {
+        if (!graphs[i]) return fail(WAE_INVALID_ARGUMENT, "null graph in the batch");
+        uniform = uniform && graphs[i]->channels == graphs[0]->channels && graphs[i]->length == graphs[0]->length &&
+                  graphs[i]->sample_rate == graphs[0]->sample_rate;
+    }
+    if (uniform) return WAE_OK;
+    std::vector<std::vector<int64_t>> cuts(n_graphs);
+    for (uint32_t i = 0; i < n_graphs; i++) cuts[i] = graph_cuts(graphs[i]);
+    order.resize(n_graphs);
+    for (uint32_t i = 0; i < n_graphs; i++) order[i] = i;
+    std::stable_sort(order.begin(), order.end(), [&](uint32_t x, uint32_t y) {
+        if (graphs[x]->sample_rate != graphs[y]->sample_rate) return graphs[x]->sample_rate < graphs[y]->sample_rate;
+        if (cuts[x] != cuts[y]) return cuts[x] < cuts[y];
+        return padded_length(graphs[x]) > padded_length(graphs[y]);
+    });
+    return WAE_OK;
+}
+
+// `order` != nullptr: the graphs differ in shape and are given in the batch order many_order made (`order` maps it to the caller's)
 static wae_status prep_begin(wae_engine* eng, wae_graph* const* graphs, uint32_t n_graphs, wae_plan_info* plan, wae_batch** out_b, PrepState& ps,
-                             bool want_d_out) {
+                             bool want_d_out, const std::vector<uint32_t>* order = nullptr) {
     if (!eng || !graphs || n_graphs == 0) return fail(WAE_INVALID_ARGUMENT, "null / empty batch");
     if (!plan) CUDA_TRY(cudaSetDevice(eng->device));
     for (uint32_t i = 0; i < n_graphs; i++) {
         if (!graphs[i]) return fail(WAE_INVALID_ARGUMENT, "null graph in the batch");
-        if (graphs[i]->channels != graphs[0]->channels || graphs[i]->length != graphs[0]->length ||
-            graphs[i]->sample_rate != graphs[0]->sample_rate)
+        if (!order && (graphs[i]->channels != graphs[0]->channels || graphs[i]->length != graphs[0]->length ||
+                       graphs[i]->sample_rate != graphs[0]->sample_rate))
             return fail(WAE_INVALID_ARGUMENT, "all graphs of a batch must share number_of_channels, length and sample_rate");
     }
     ps.t0 = std::chrono::steady_clock::now();
@@ -3023,8 +3142,20 @@ static wae_status prep_begin(wae_engine* eng, wae_graph* const* graphs, uint32_t
     b->s_d2h = eng->s_d2h;
     b->n_graphs = n_graphs;
     b->channels = graphs[0]->channels;
-    b->length = graphs[0]->length;
+    b->out_off.assign(n_graphs + 1, 0);
+    for (uint32_t i = 0; i < n_graphs; i++) {
+        b->length = std::max(b->length, graphs[i]->length);
+        b->out_off[i + 1] = b->out_off[i] + (size_t)graphs[i]->channels * graphs[i]->length;
+        b->shape.push_back({graphs[i]->channels, graphs[i]->length});
+    }
     b->lq = (int64_t)((b->length + 127) / 128 * 128);
+    for (uint32_t i = 0; i < n_graphs; i++) b->needed_quanta += (uint64_t)(padded_length(graphs[i]) / 128);
+    if (order) {
+        b->mixed = true;
+        b->order = *order;
+        b->pos.assign(n_graphs, 0);
+        for (uint32_t i = 0; i < n_graphs; i++) b->pos[b->order[i]] = i;
+    }
     bool has_conv = false, has_hrtf = false;
     std::vector<char> graph_has_conv(n_graphs, 0);
     std::vector<std::vector<int64_t>> cuts(n_graphs);  // per graph: its suspend frames inside the render
@@ -3033,14 +3164,13 @@ static wae_status prep_begin(wae_engine* eng, wae_graph* const* graphs, uint32_t
             if (kv.second.kind == K_CONV && kv.second.buffer) graph_has_conv[i] = 1;
             if (kv.second.kind == K_PANNER && kv.second.panning_model == WAE_PANNING_HRTF) has_hrtf = true;  // (static ones ride the convolver kernels)
         }
-        for (auto& ep : graphs[i]->epochs) {
-            if ((int64_t)ep.frame > 0 && (int64_t)ep.frame < b->lq) cuts[i].push_back((int64_t)ep.frame);
+        cuts[i] = graph_cuts(graphs[i]);
+        for (auto& ep : graphs[i]->epochs)
             for (auto& kv : ep.nodes)
                 if (kv.second.kind == K_CONV && kv.second.buffer) graph_has_conv[i] = 1;
-        }
         has_conv = has_conv || graph_has_conv[i];
     }
-    size_t out_floats = (size_t)n_graphs * b->channels * b->length;
+    size_t out_floats = b->out_off[n_graphs];
     if (!plan && want_d_out) {
         b->d_out = b->dalloc<float>(out_floats, true);
         if (!b->d_out) {
@@ -3048,38 +3178,15 @@ static wae_status prep_begin(wae_engine* eng, wae_graph* const* graphs, uint32_t
             return fail(WAE_OUT_OF_MEMORY, "out of device memory (output PCM)");
         }
     }
-    // graph groups for the H2D / render / D2H pipeline
-    int n_groups = eng->pipeline_groups;
-    if (n_groups == 0) n_groups = n_graphs >= 512 ? 32 : (n_graphs >= 64 ? 8 : 1);  // more groups = shorter fill / drain of the 3-stage pipeline
-    if (eng->pipeline_groups == 0 && n_graphs >= 512) {  // (tuning: WAE_AUTO_GROUPS overrides the automatic choice for large batches)
-        static const int env_groups = [] { const char* e = getenv("WAE_AUTO_GROUPS"); return e ? atoi(e) : 0; }();
-        if (env_groups > 0) n_groups = env_groups;
-    }
-    n_groups = std::max(1, std::min<int>(n_groups, (int)n_graphs));
-    {
-        // contiguous runs of graphs with the same suspend frames, cut further into about n_groups pieces
-        const uint32_t target = (n_graphs + (uint32_t)n_groups - 1) / (uint32_t)n_groups;
-        uint32_t g0 = 0;
-        for (uint32_t i = 1; i <= n_graphs; i++)
-            if (i == n_graphs || cuts[i] != cuts[g0] || i - g0 >= target) {
-                wae_batch::Group grp;
-                grp.g0 = g0;
-                grp.g1 = i;
-                grp.seg_bounds.push_back(0);
-                for (int64_t f : cuts[g0]) grp.seg_bounds.push_back(f);
-                grp.seg_bounds.push_back(b->lq);
-                b->groups.push_back(grp);
-                g0 = i;
-            }
-        n_groups = (int)b->groups.size();
-    }
+    b->groups = form_groups(eng, graphs, n_graphs, cuts);
+    int n_groups = (int)b->groups.size();
     // the convolver kernels work on whole partitions: a chunk (and so a render segment) has to start on one
     for (auto& grp : b->groups) {
         bool conv = false;
         for (uint32_t i = grp.g0; i < grp.g1; i++) conv = conv || graph_has_conv[i];
         if (!conv) continue;
         for (int64_t f : grp.seg_bounds)
-            if (f != b->lq && f % WAE_CONV_BLOCK != 0) {
+            if (f != grp.lq && f % WAE_CONV_BLOCK != 0) {
                 wae_batch_destroy(b);
                 return fail(WAE_UNSUPPORTED, "a suspend point that is not a multiple of the convolver partition (8192 frames) in a graph with a ConvolverNode is not lowered to the GPU");
             }
@@ -3131,11 +3238,12 @@ static wae_status prep_begin(wae_engine* eng, wae_graph* const* graphs, uint32_t
             Planner sizing{b, eng};
             sizing.dry = true;
             sizing.group_graphs = (int)(b->groups[k].g1 - b->groups[k].g0);
+            sizing.lq = b->groups[k].lq;
             sizing.delay_ch_hint = &ps.delay_ch_hint;
             sizing.d_src = reinterpret_cast<float*>(uintptr_t(256));
             sizing.src_copies = &ro.copies;
             sizing.src_cursor = cursor0;
-            sizing.begin_segment(0, b->lq);
+            sizing.begin_segment(0, b->groups[k].lq);
             for (uint32_t i = i0; i < i1; i++) {
                 EpochView view(graphs[i], 0);
                 ro.graph_base.push_back(sizing.src_cursor);
@@ -3208,6 +3316,7 @@ static wae_status prep_begin(wae_engine* eng, wae_graph* const* graphs, uint32_t
             Planner sizing{b, eng};
             sizing.dry = true;
             sizing.group_graphs = (int)n_in_group;
+            sizing.lq = b->groups[k].lq;
             sizing.delay_ch_hint = &ps.delay_ch_hint;
             sizing.d_src = reinterpret_cast<float*>(uintptr_t(256));
             b->groups[k].src_copies.clear();
@@ -3366,6 +3475,7 @@ static void prep_plan_group(wae_batch* b, wae_graph* const* graphs, int k, PrepS
     Planner pl{b, eng};
     pl.d_src = grp.d_src;
     pl.group_graphs = (int)(grp.g1 - grp.g0);
+    pl.lq = grp.lq;
     pl.src_copies = nullptr;  // recorded by the sizing pass
     pl.delay_ch_hint = &ps.delay_ch_hint;
     pl.ir_cache = &ps.ir_cache;
@@ -3406,6 +3516,7 @@ static void prep_plan_group(wae_batch* b, wae_graph* const* graphs, int k, PrepS
                 Planner rp{b, eng};
                 rp.d_src = grp.d_src;
                 rp.group_graphs = (int)n;
+                rp.lq = grp.lq;
                 rp.src_copies = nullptr;
                 rp.delay_ch_hint = &ps.delay_ch_hint;
                 rp.ir_cache = &ps.ir_cache;
@@ -3441,7 +3552,7 @@ static void prep_plan_group(wae_batch* b, wae_graph* const* graphs, int k, PrepS
             }
         }
         // the per-node byte counts assume the whole render: scale to this segment's share of it
-        gp.algorithmic_bytes += (uint64_t)((double)(pl.algorithmic_bytes - alg_before) * (double)(pl.seg_end - pl.seg_start) / (double)b->lq);
+        gp.algorithmic_bytes += (uint64_t)((double)(pl.algorithmic_bytes - alg_before) * (double)(pl.seg_end - pl.seg_start) / (double)grp.lq);
         // materialise the segment's stages in (class, level, kind) order
         const size_t seg_stage0 = gp.stages.size();
         void* last_conv_inputs = nullptr;
@@ -3599,17 +3710,18 @@ static wae_status prep_finish(wae_batch* b, PrepState& ps) {
     b->stats.arena_bytes = b->arena_bytes;
     b->stats.asset_bytes = b->asset_bytes;
     b->stats.algorithmic_bytes = ps.algorithmic_bytes;
-    b->stats.graph_quanta = (uint64_t)b->n_graphs * (uint64_t)(b->lq / 128);
+    b->stats.graph_quanta = b->needed_quanta;
     return WAE_OK;
 }
 
 // `plan` != nullptr: planning only — grouping, the sizing pass of the planner (which touches no device memory) and the chunk choice,
 // reported through *plan; nothing is allocated and no CUDA call is made (wae_batch_plan: runs without a GPU).
-static wae_status prepare_impl(wae_engine* eng, wae_graph* const* graphs, uint32_t n_graphs, wae_batch** out, wae_plan_info* plan) {
+static wae_status prepare_impl(wae_engine* eng, wae_graph* const* graphs, uint32_t n_graphs, wae_batch** out, wae_plan_info* plan,
+                               const std::vector<uint32_t>* order = nullptr) {
     if (!out && !plan) return fail(WAE_INVALID_ARGUMENT, "null out pointer");
     PrepState ps;
     wae_batch* b = nullptr;
-    wae_status st = prep_begin(eng, graphs, n_graphs, plan, &b, ps, true);
+    wae_status st = prep_begin(eng, graphs, n_graphs, plan, &b, ps, true, order);
     if (st != WAE_OK || plan) return st;
     const int n_groups = (int)b->groups.size();
     std::vector<GroupPlan> gps(n_groups);
@@ -3664,6 +3776,60 @@ WAE_API wae_status wae_batch_plan(wae_graph* const* graphs, uint32_t n_graphs, w
     if (!info) return fail(WAE_INVALID_ARGUMENT, "null info pointer");
     wae_engine host_only;  // default options; no stream, no sphere: HRTF panners answer WAE_UNSUPPORTED ("needs an HRIR sphere")
     return prepare_impl(&host_only, graphs, n_graphs, nullptr, info);
+}
+
+// Graphs of different shapes: the batch order (many_order) and the graphs in it.  A batch of one shape keeps the caller's array.
+struct ManyOrder {
+    std::vector<uint32_t> order;
+    std::vector<wae_graph*> sorted;
+    wae_graph* const* graphs = nullptr;  // what the planner walks
+    const std::vector<uint32_t>* order_ptr() const { return order.empty() ? nullptr : &order; }
+};
+static wae_status many_batch(wae_graph* const* graphs, uint32_t n_graphs, ManyOrder& mo) {
+    wae_status st = many_order(graphs, n_graphs, mo.order);
+    if (st != WAE_OK) return st;
+    mo.graphs = graphs;
+    if (!mo.order.empty()) {
+        for (uint32_t i : mo.order) mo.sorted.push_back(graphs[i]);
+        mo.graphs = mo.sorted.data();
+    }
+    return WAE_OK;
+}
+
+WAE_API wae_status wae_batch_prepare_many(wae_engine* eng, wae_graph* const* graphs, uint32_t n_graphs, wae_batch** out) {
+    if (!out) return fail(WAE_INVALID_ARGUMENT, "null out pointer");
+    ManyOrder mo;
+    wae_status st = many_batch(graphs, n_graphs, mo);
+    if (st != WAE_OK) return st;
+    return prepare_impl(eng, mo.graphs, n_graphs, out, nullptr, mo.order_ptr());
+}
+
+WAE_API wae_status wae_batch_plan_many(wae_graph* const* graphs, uint32_t n_graphs, wae_plan_info* info) {
+    if (!info) return fail(WAE_INVALID_ARGUMENT, "null info pointer");
+    ManyOrder mo;
+    wae_status st = many_batch(graphs, n_graphs, mo);
+    if (st != WAE_OK) return st;
+    wae_engine host_only;
+    return prepare_impl(&host_only, mo.graphs, n_graphs, nullptr, info, mo.order_ptr());
+}
+
+WAE_API wae_status wae_batch_plan_quanta(wae_graph* const* graphs, uint32_t n_graphs, uint32_t* group_of, uint64_t* rendered, uint64_t* needed) {
+    if (!rendered || !needed) return fail(WAE_INVALID_ARGUMENT, "null argument");
+    ManyOrder mo;
+    wae_status st = many_batch(graphs, n_graphs, mo);
+    if (st != WAE_OK) return st;
+    wae_engine host_only;
+    std::vector<std::vector<int64_t>> cuts(n_graphs);
+    for (uint32_t i = 0; i < n_graphs; i++) cuts[i] = graph_cuts(mo.graphs[i]);
+    const std::vector<wae_batch::Group> groups = form_groups(&host_only, mo.graphs, n_graphs, cuts);
+    *rendered = *needed = 0;
+    for (size_t k = 0; k < groups.size(); k++)
+        for (uint32_t j = groups[k].g0; j < groups[k].g1; j++) {
+            *rendered += (uint64_t)(groups[k].lq / 128);
+            *needed += (uint64_t)(padded_length(mo.graphs[j]) / 128);
+            if (group_of) group_of[mo.order.empty() ? j : mo.order[j]] = (uint32_t)k;
+        }
+    return WAE_OK;
 }
 
 static void launch_stage(wae_batch* b, Stage& st, ChunkInfo ci) {
@@ -3895,7 +4061,12 @@ static wae_status run_pipelined(wae_batch* b, float* host_out, bool resend_sourc
     return WAE_OK;
 }
 
-WAE_API wae_status wae_batch_run_pipelined(wae_batch* b, float* host_out) { return run_pipelined(b, host_out, true); }
+static const char* kMixedPacked = "the graphs of this batch differ in shape: there is no [n][channels][length] host layout, copy each graph with "
+                                  "wae_batch_fetch_graph (or render with wae_render_many)";
+WAE_API wae_status wae_batch_run_pipelined(wae_batch* b, float* host_out) {
+    if (b && b->mixed) return fail(WAE_INVALID_STATE, kMixedPacked);
+    return run_pipelined(b, host_out, true);
+}
 
 WAE_API wae_status wae_batch_sync(wae_batch* b) {
     CUDA_TRY(cudaSetDevice(b->engine->device));
@@ -3924,11 +4095,33 @@ WAE_API wae_status wae_batch_sync(wae_batch* b) {
 
 WAE_API wae_status wae_batch_output_device_ptr(wae_batch* b, float** out_dev, uint64_t* out_floats) {
     *out_dev = b->d_out;
-    *out_floats = (uint64_t)b->n_graphs * b->channels * b->length;
+    *out_floats = (uint64_t)b->out_off[b->n_graphs];
+    return WAE_OK;
+}
+
+WAE_API wae_status wae_batch_graph_output(wae_batch* b, uint32_t graph_index, uint64_t* offset_floats, uint32_t* channels, uint64_t* length) {
+    if (!b || !offset_floats || !channels || !length) return fail(WAE_INVALID_ARGUMENT, "null argument");
+    if (graph_index >= b->n_graphs) return fail(WAE_INVALID_ARGUMENT, "graph index out of range");
+    const uint32_t j = b->batch_pos(graph_index);
+    *offset_floats = b->out_off[j];
+    *channels = b->shape[j].first;
+    *length = b->shape[j].second;
+    return WAE_OK;
+}
+
+WAE_API wae_status wae_batch_fetch_graph(wae_batch* b, uint32_t graph_index, float* out) {
+    if (!b || !out) return fail(WAE_INVALID_ARGUMENT, "null argument");
+    if (graph_index >= b->n_graphs) return fail(WAE_INVALID_ARGUMENT, "graph index out of range");
+    const uint32_t j = b->batch_pos(graph_index);
+    CUDA_TRY(cudaSetDevice(b->engine->device));
+    const size_t bytes = (b->out_off[j + 1] - b->out_off[j]) * sizeof(float);
+    if (bytes) CUDA_TRY(cudaMemcpyAsync(out, b->d_out + b->out_off[j], bytes, cudaMemcpyDeviceToHost, b->engine->stream));
+    CUDA_TRY(cudaStreamSynchronize(b->engine->stream));
     return WAE_OK;
 }
 
 WAE_API wae_status wae_batch_fetch(wae_batch* b, float* host_out) {
+    if (b && b->mixed) return fail(WAE_INVALID_STATE, kMixedPacked);
     CUDA_TRY(cudaSetDevice(b->engine->device));
     size_t bytes = (size_t)b->n_graphs * b->channels * b->length * sizeof(float);
     CUDA_TRY(cudaMemcpyAsync(host_out, b->d_out, bytes, cudaMemcpyDeviceToHost, b->engine->stream));
@@ -3990,14 +4183,25 @@ static void copy_streaming(void* dst, const void* src, size_t n) {
     if (n) std::memcpy(d, sp, n);
 }
 
-static wae_status render_oneshot_host(wae_engine* eng, wae_graph* const* graphs, uint32_t n_graphs, float* out) {
-    if (!out) return fail(WAE_INVALID_ARGUMENT, "null output buffer");
+// `outs` != nullptr (wae_render_many): one host buffer per graph, outs[i] = [channels_i][length_i] of the caller's graph i; `out` unused.
+// `graphs` is then in the batch order of `order` (many_order) when that is given.
+static wae_status render_oneshot_host(wae_engine* eng, wae_graph* const* graphs, uint32_t n_graphs, float* out, float* const* outs = nullptr,
+                                      const std::vector<uint32_t>* order = nullptr) {
+    if (!out && !outs) return fail(WAE_INVALID_ARGUMENT, "null output buffer");
+    if (outs)
+        for (uint32_t i = 0; i < n_graphs; i++)
+            if (!outs[i]) return fail(WAE_INVALID_ARGUMENT, "null output buffer");
     PrepState ps;
     wae_batch* b = nullptr;
-    wae_status st = prep_begin(eng, graphs, n_graphs, nullptr, &b, ps, true);
+    wae_status st = prep_begin(eng, graphs, n_graphs, nullptr, &b, ps, true, order);
     if (st != WAE_OK) return st;
     const int n_groups = (int)b->groups.size();
-    const size_t per_graph = (size_t)b->channels * b->length;
+    // the packed rendered PCM of group k: floats [out_off[g0], out_off[g1])
+    auto group_off = [&](const wae_batch::Group& grp) { return b->out_off[grp.g0]; };
+    auto group_bytes = [&](const wae_batch::Group& grp) { return (b->out_off[grp.g1] - b->out_off[grp.g0]) * sizeof(float); };
+    // outs: the caller's buffer of the graph at batch position j, and whether it is page-locked (its own D2H) or not (staging slot)
+    auto graph_out = [&](uint32_t j) { return outs[order ? (*order)[j] : j]; };
+    std::vector<char> graph_pinned(outs ? n_graphs : 0, 0);
     cudaStream_t s = eng->stream;
     WorkerPool* pool = eng->workers();
     // ---- everything below must run to its end before the batch can be destroyed: `pending` counts worker tasks in flight
@@ -4046,14 +4250,24 @@ static wae_status render_oneshot_host(wae_engine* eng, wae_graph* const* graphs,
                 task_done();
             });
     // 3. where the rendered PCM lands
-    bool out_pinned = false;
-    {
+    auto is_pinned = [](const void* p) {
         cudaPointerAttributes attr;
-        if (cudaPointerGetAttributes(&attr, out) == cudaSuccess) out_pinned = attr.type == cudaMemoryTypeHost;
-        else cudaGetLastError();
-    }
+        if (cudaPointerGetAttributes(&attr, p) == cudaSuccess) return attr.type == cudaMemoryTypeHost;
+        cudaGetLastError();
+        return false;
+    };
+    const bool out_pinned = !outs && is_pinned(out);
+    for (uint32_t j = 0; outs && j < n_graphs; j++) graph_pinned[j] = is_pinned(graph_out(j)) ? 1 : 0;
+    // (outs: a group whose buffers are all page-locked needs no staging slot)
+    auto group_staged = [&](const wae_batch::Group& grp) {
+        if (!outs) return !out_pinned;
+        for (uint32_t j = grp.g0; j < grp.g1; j++)
+            if (!graph_pinned[j] && b->out_off[j + 1] > b->out_off[j]) return true;
+        return false;
+    };
     size_t max_group_bytes = 0;
-    for (auto& grp : b->groups) max_group_bytes = std::max(max_group_bytes, (size_t)(grp.g1 - grp.g0) * per_graph * sizeof(float));
+    for (auto& grp : b->groups)
+        if (group_staged(grp)) max_group_bytes = std::max(max_group_bytes, group_bytes(grp));
     // Pageable `out`, default: whole-group page-locked staging slots, copied out in parts by the workers (below).  WAE_STAGE_RING=1 (an
     // experiment that lost, kept for the record): the PCM comes down in PIECES of a couple of MB through a small
     // ring of page-locked slots meant to stay in the last-level cache (inbound DMA writes allocate there), each piece copied out as soon
@@ -4062,9 +4276,9 @@ static wae_status render_oneshot_host(wae_engine* eng, wae_graph* const* graphs,
     static const bool use_ring = [] { const char* e = getenv("WAE_STAGE_RING"); return e && atoi(e) != 0; }();
     static const size_t piece_bytes = [] { const char* e = getenv("WAE_STAGE_PIECE_KB"); long kb = e ? atol(e) : 2048; return (size_t)std::max(64l, std::min(65536l, kb)) * 1024; }();
     static const int ring_slots = [] { const char* e = getenv("WAE_STAGE_SLOTS"); int n = e ? atoi(e) : 8; return std::max(2, std::min(64, n)); }();
-    const bool ring = !out_pinned && use_ring;
+    const bool ring = !outs && !out_pinned && use_ring;
     if (result == WAE_OK && ring && !eng->ensure_ring(piece_bytes * (size_t)ring_slots)) set_fail(WAE_OUT_OF_MEMORY, "out of memory (page-locked staging ring of the rendered PCM)");
-    if (result == WAE_OK && !out_pinned && !ring && !eng->ensure_stage(max_group_bytes)) set_fail(WAE_OUT_OF_MEMORY, "out of memory (page-locked staging of the rendered PCM)");
+    if (result == WAE_OK && max_group_bytes && !ring && !eng->ensure_stage(max_group_bytes)) set_fail(WAE_OUT_OF_MEMORY, "out of memory (page-locked staging of the rendered PCM)");
     // ring state (guarded by `mu`): slot i is free again once its copy-out is done; groups are handed to the pump thread in order
     std::vector<char> ring_busy(ring ? ring_slots : 0, 0);
     std::vector<cudaEvent_t> ring_ev(ring ? ring_slots : 0, nullptr);
@@ -4090,7 +4304,7 @@ static wae_status render_oneshot_host(wae_engine* eng, wae_graph* const* graphs,
                     pump_error = "cudaStreamWaitEvent failed";
                     return;
                 }
-                const size_t off = (size_t)grp.g0 * per_graph * sizeof(float), bytes = (size_t)(grp.g1 - grp.g0) * per_graph * sizeof(float);
+                const size_t off = group_off(grp) * sizeof(float), bytes = group_bytes(grp);
                 for (size_t a0 = 0; a0 < bytes; a0 += piece_bytes, piece_no++) {
                     const size_t nb = std::min(piece_bytes, bytes - a0);
                     const int slot = (int)(piece_no % (size_t)ring_slots);
@@ -4156,7 +4370,7 @@ static wae_status render_oneshot_host(wae_engine* eng, wae_graph* const* graphs,
             set_fail(WAE_CUDA_ERROR, wae_last_error());
             break;
         }
-        const size_t off = (size_t)grp.g0 * per_graph, bytes = (size_t)(grp.g1 - grp.g0) * per_graph * sizeof(float);
+        const size_t off = group_off(grp), bytes = group_bytes(grp);
         // (ring: the pump thread makes the copy stream wait, in group order — a wait queued from here could land between the pieces of
         // the group before)
         if (cudaEventRecord(grp.ev_done, s) != cudaSuccess || (!ring && cudaStreamWaitEvent(eng->s_d2h, grp.ev_done, 0) != cudaSuccess)) {
@@ -4167,6 +4381,13 @@ static wae_status render_oneshot_host(wae_engine* eng, wae_graph* const* graphs,
             if (cudaMemcpyAsync(out + off, b->d_out + off, bytes, cudaMemcpyDeviceToHost, eng->s_d2h) != cudaSuccess) set_fail(WAE_CUDA_ERROR, "D2H failed");
             continue;
         }
+        for (uint32_t j = grp.g0; outs && j < grp.g1; j++)  // page-locked outs[i]: a copy of its own
+            if (graph_pinned[j] && b->out_off[j + 1] > b->out_off[j] &&
+                cudaMemcpyAsync(graph_out(j), b->d_out + b->out_off[j], (b->out_off[j + 1] - b->out_off[j]) * sizeof(float), cudaMemcpyDeviceToHost,
+                                eng->s_d2h) != cudaSuccess)
+                set_fail(WAE_CUDA_ERROR, "D2H failed");
+        if (result != WAE_OK) break;
+        if (!group_staged(grp)) continue;
         if (ring) {  // the pump thread brings this group down piece by piece
             std::lock_guard<std::mutex> lk(mu);
             issued_groups = k + 1;
@@ -4180,8 +4401,25 @@ static wae_status render_oneshot_host(wae_engine* eng, wae_graph* const* graphs,
             slot_busy[slot] = true;
             pending += copy_parts;
         }
-        if (cudaMemcpyAsync(eng->h_stage[slot], b->d_out + off, bytes, cudaMemcpyDeviceToHost, eng->s_d2h) != cudaSuccess ||
-            cudaEventRecord(ev_copy[k], eng->s_d2h) != cudaSuccess) {
+        // (outs: only the runs of graphs with pageable buffers come down into the slot, at their place in the group's packed PCM; the
+        // page-locked ones already have their own copy)
+        auto stage_group = [&]() -> cudaError_t {
+            if (!outs) return cudaMemcpyAsync(eng->h_stage[slot], b->d_out + off, bytes, cudaMemcpyDeviceToHost, eng->s_d2h);
+            for (uint32_t j = grp.g0; j < grp.g1;) {
+                if (graph_pinned[j]) { j++; continue; }
+                uint32_t j1 = j + 1;
+                while (j1 < grp.g1 && !graph_pinned[j1]) j1++;
+                const size_t n = (b->out_off[j1] - b->out_off[j]) * sizeof(float);
+                if (n) {
+                    const cudaError_t e = cudaMemcpyAsync((char*)eng->h_stage[slot] + (b->out_off[j] - off) * sizeof(float), b->d_out + b->out_off[j], n,
+                                                          cudaMemcpyDeviceToHost, eng->s_d2h);
+                    if (e != cudaSuccess) return e;
+                }
+                j = j1;
+            }
+            return cudaSuccess;
+        };
+        if (stage_group() != cudaSuccess || cudaEventRecord(ev_copy[k], eng->s_d2h) != cudaSuccess) {
             set_fail(WAE_CUDA_ERROR, "D2H failed");
             std::lock_guard<std::mutex> lk(mu);
             pending -= copy_parts;
@@ -4198,9 +4436,16 @@ static wae_status render_oneshot_host(wae_engine* eng, wae_graph* const* graphs,
                 // (non-temporal stores: a 15 MB part is far below glibc's non-temporal threshold — 3/4 of a 260 MB L3 — and a plain memcpy
                 // would fetch every destination line before overwriting it; WAE_STAGE_NT=0: memcpy)
                 static const bool nt = [] { const char* e = getenv("WAE_STAGE_NT"); return !e || atoi(e) != 0; }();
-                if (a1 > a0) {
-                    if (nt) copy_streaming((char*)(out + off) + a0, (const char*)eng->h_stage[slot] + a0, a1 - a0);
-                    else std::memcpy((char*)(out + off) + a0, (const char*)eng->h_stage[slot] + a0, a1 - a0);
+                auto put = [&](char* dst, size_t x0, size_t x1) {  // bytes [x0, x1) of the group's staged PCM
+                    if (nt) copy_streaming(dst, (const char*)eng->h_stage[slot] + x0, x1 - x0);
+                    else std::memcpy(dst, (const char*)eng->h_stage[slot] + x0, x1 - x0);
+                };
+                if (a1 > a0 && !outs) put((char*)(out + off) + a0, a0, a1);
+                const wae_batch::Group& grp_k = b->groups[k];
+                for (uint32_t j = grp_k.g0; a1 > a0 && outs && j < grp_k.g1; j++) {  // the pageable outs[i] this part overlaps
+                    const size_t j0 = (b->out_off[j] - off) * sizeof(float), j1 = (b->out_off[j + 1] - off) * sizeof(float);
+                    const size_t x0 = std::max(a0, j0), x1 = std::min(a1, j1);
+                    if (!graph_pinned[j] && x1 > x0) put((char*)graph_out(j) + (x0 - j0), x0, x1);
                 }
                 if (left->fetch_sub(1) == 1) {
                     std::lock_guard<std::mutex> lk(mu);
@@ -4271,6 +4516,14 @@ WAE_API wae_status wae_selftest_conv_fft(float* data, uint32_t mode) {
     return WAE_OK;
 }
 
+WAE_API wae_status wae_render_many(wae_engine* eng, wae_graph* const* graphs, uint32_t n_graphs, float* const* outs) {
+    if (!outs) return fail(WAE_INVALID_ARGUMENT, "null output buffers");
+    ManyOrder mo;
+    wae_status st = many_batch(graphs, n_graphs, mo);
+    if (st != WAE_OK) return st;
+    return render_oneshot_host(eng, mo.graphs, n_graphs, nullptr, outs, mo.order_ptr());
+}
+
 WAE_API wae_status wae_render_batch(wae_engine* eng, wae_graph* const* graphs, uint32_t n_graphs, float* out, uint32_t flags) {
     if (!(flags & WAE_RENDER_OUT_DEVICE)) return render_oneshot_host(eng, graphs, n_graphs, out);
     wae_batch* b = nullptr;
@@ -4291,7 +4544,9 @@ WAE_API wae_status wae_render_batch(wae_engine* eng, wae_graph* const* graphs, u
 }
 
 // AnalyserNode read-out: get_float_time_domain_data (src/analysis.rs:261-264, ring read :114-127)
-static const AnalyserRec* find_analyser(wae_batch* b, uint32_t gi, wae_node_id node) {
+static const AnalyserRec* find_analyser(wae_batch* b, uint32_t graph_index, wae_node_id node) {
+    if (!b || graph_index >= b->n_graphs) return nullptr;
+    const uint32_t gi = b->batch_pos(graph_index);
     for (auto& a : b->analysers)
         if (a.graph_index == gi && a.node == node) return &a;
     return nullptr;
@@ -4305,7 +4560,7 @@ WAE_API wae_status wae_analyser_get_float_time_domain_data(wae_batch* b, uint32_
     CUDA_TRY(cudaSetDevice(b->engine->device));
     CUDA_TRY(cudaMemcpy(ring.data(), a->d_ring, RING * sizeof(float), cudaMemcpyDeviceToHost));
     uint32_t n = std::min(len, a->fft_size);
-    uint64_t write_index = (uint64_t)b->lq % RING;
+    uint64_t write_index = (uint64_t)a->lq % RING;
     for (uint32_t i = 0; i < n; i++) out[i] = ring[(RING + write_index - n + i) % RING];
     return WAE_OK;
 }
@@ -4317,7 +4572,7 @@ WAE_API wae_status wae_analyser_get_float_frequency_data(wae_batch* b, uint32_t 
     const uint32_t RING = 32768 + 128;
     const uint32_t bins = a->fft_size / 2;
     if (!a->computed) {  // one FFT per distinct current_time (analysis.rs:353-361): the read-out happens after the render
-        launch_analyser_fft(a->d_ring, (uint32_t)((uint64_t)b->lq % RING), (int)a->fft_size, (float)a->smoothing, a->d_last_fft, a->d_db,
+        launch_analyser_fft(a->d_ring, (uint32_t)((uint64_t)a->lq % RING), (int)a->fft_size, (float)a->smoothing, a->d_last_fft, a->d_db,
                             b->engine->stream);
         a->computed = true;
     }
@@ -4362,8 +4617,9 @@ WAE_API wae_status wae_analyser_get_byte_frequency_data(wae_batch* b, uint32_t g
 // DynamicsCompressorNode::reduction (src/node/dynamics_compressor.rs:204-206,448): the reduction (dB) of the last frame
 WAE_API wae_status wae_compressor_reduction(wae_batch* b, uint32_t graph_index, wae_node_id node, float* out) {
     if (!b || !out) return fail(WAE_INVALID_ARGUMENT, "null argument");
+    if (graph_index >= b->n_graphs) return fail(WAE_INVALID_ARGUMENT, "not a dynamics compressor of this batch");
     for (auto& c : b->compressors)
-        if (c.graph == graph_index && c.node == node) {
+        if (c.graph == b->batch_pos(graph_index) && c.node == node) {
             CUDA_TRY(cudaSetDevice(b->engine->device));
             CUDA_TRY(cudaMemcpyAsync(out, c.d_state + 1, sizeof(float), cudaMemcpyDeviceToHost, b->engine->stream));
             CUDA_TRY(cudaStreamSynchronize(b->engine->stream));

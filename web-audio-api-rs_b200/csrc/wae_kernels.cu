@@ -1358,6 +1358,10 @@ __global__ void __launch_bounds__(CH_THREADS, chain_min_blocks(SRC, NB)) k_chain
         for (int i = t; i < (int)(sizeof(ChainInst) / 4); i += CH_THREADS) dst[i] = src[i];
     }
     __syncthreads();
+    // A work item that starts at or after its graph's end (a graph shorter than its group) has nothing to render: it leaves before any
+    // copy.  No slab waits for it: the later slabs of its (instance, channel) start later still and leave here too, before they wait for
+    // a hand-off (PRE slabs included).  (An output with a layout track is rendered to the end: its consumers read the track.)
+    if (ci.f0 + (int64_t)slab * sc.tiles_per_slab * (CH_THREADS * CH_K) >= sm.q.end && sm.q.out.meta == nullptr) return;
     // oscillator wavetable -> shared memory, as (entry, next entry) pairs: the 128 threads of a CTA are 16 frames apart, so their table
     // indices fall in different 128-byte lines (a 32-wavefront global gather per load); shared memory only pays bank conflicts, and the
     // pair makes the two taps of the interpolation one 8-byte load
@@ -3219,9 +3223,12 @@ __global__ void __launch_bounds__(32) k_compressor(const CompInst* __restrict__ 
             det = __fadd_rn(__fmul_rn(attack_tau, prev), __fmul_rn(1.f - attack_tau, attenuation));
         else
             det = __fadd_rn(__fmul_rn(release_tau, prev), __fmul_rn(1.f - release_tau, attenuation));
-        reduction_gain = -det + makeup_gain;
-        float g = db_to_lin(reduction_gain);
-        prev = det;
+        const float red = -det + makeup_gain;
+        float g = db_to_lin(red);
+        if (ci.f0 + n < q.end) {  // past the graph's own end (a shorter graph of a longer group) the state stays as the render left it
+            reduction_gain = red;
+            prev = det;
+        }
         int64_t m = ci.f0 + n - q.delay_frames;
         for (int c = 0; c < q.ch; c++) {
             float x = 0.f;
@@ -3246,9 +3253,12 @@ __global__ void __launch_bounds__(256) k_analyser(const AnalyserInst* __restrict
     const int RING = 32768 + 128;
     for (int ii = blockIdx.y; ii < n_inst; ii += gridDim.y) {
         const AnalyserInst a = insts[ii];
+        // frames from the graph's own end on (a shorter graph of a longer group) are not part of its render: they are not recorded
+        const int nf_end = (int)max((int64_t)0, min((int64_t)ci.nf, a.end - ci.f0));
         int n = blockIdx.x * blockDim.x + threadIdx.x;
         if (n >= ci.nf) continue;
-        if (!a.out.p && ci.nf - n > RING) continue;  // older than the ring: overwritten by this very chunk
+        const bool record = n < nf_end && nf_end - n <= RING;  // (older than the ring: overwritten by this very chunk)
+        if (!a.out.p && !record) continue;
         MixEdge e;
         e.src = a.in;
         e.src_ch = a.ch;
@@ -3262,7 +3272,7 @@ __global__ void __launch_bounds__(256) k_analyser(const AnalyserInst* __restrict
         }
         if (a.out.p)
             for (int c = 0; c < a.ch; c++) chan(a.out, c, ci)[n] = chan(a.in, c, ci)[n];
-        if (ci.nf - n <= RING) a.ring[(ci.f0 + n) % RING] = mono;
+        if (record) a.ring[(ci.f0 + n) % RING] = mono;
     }
 }
 
@@ -3864,11 +3874,15 @@ __global__ void __launch_bounds__(CV_THREADS, 3) k_conv_fft_in(const ConvInput* 
     const ConvInput ip = inputs[blockIdx.y];
     const int jb = blockIdx.x;                         // block within the chunk
     const int64_t jabs = ci.f0 / CV_B + jb;            // absolute block index
+    // the graph's end (a graph shorter than its group): a block starting there is never read for a frame before it, and the input from
+    // there on is zero, as in the graph's own render, whose last chunk ends there
+    const int64_t to_end = ip.end - (ci.f0 + (int64_t)jb * CV_B);
+    if (to_end <= 0) return;
     const bool mix = ip.in_channel < 0;
     const float* in = chan(ip.in, mix ? 0 : ip.in_channel, ci);
     const float* in2 = mix ? chan(ip.in, 1, ci) : nullptr;
     // frame = [previous block | current block]
-    const int64_t left = (int64_t)ci.nf - (int64_t)jb * CV_B;
+    const int64_t left = min((int64_t)ci.nf - (int64_t)jb * CV_B, to_end);
     if (jb == 0) conv_load_half(z, 0, ip.prev, CV_B);  // (already mixed)
     else conv_load_half(z, 0, in + (size_t)(jb - 1) * CV_B, CV_B, mix ? in2 + (size_t)(jb - 1) * CV_B : nullptr);
     conv_load_half(z, CV_B / 2, in + (size_t)jb * CV_B, (int)(left < CV_B ? left : CV_B), mix ? in2 + (size_t)jb * CV_B : nullptr);
@@ -3969,6 +3983,7 @@ __global__ void __launch_bounds__(CV_MAC_THREADS, WAE_CV_MAC_MINB) k_conv_mac(co
     constexpr int TILES = CV_B / CV_MAC_THREADS;
     const int k = (blockIdx.x % TILES) * CV_MAC_THREADS + threadIdx.x;  // bin (position order: index 0 is still the packed DC / Nyquist pair)
     const int j0 = (blockIdx.x / TILES) * CV_J;                         // first output block of this CTA (chunk-relative)
+    if (ci.f0 + (int64_t)j0 * CV_B >= p.end) return;                  // past the graph's end (a graph shorter than its group)
     const int64_t jabs0 = ci.f0 / CV_B + j0;
     const int64_t jabs_last = ci.f0 / CV_B + nb - 1;                    // newest input block transformed so far
     float2 acc[CV_J];
@@ -3990,6 +4005,7 @@ __global__ void __launch_bounds__(CV_THREADS, 3) k_conv_ifft(const ConvPath* __r
     const float2 lane_tw = cv_lane_tw();
     const ConvPath p = paths[blockIdx.y];
     const int jb = blockIdx.x;
+    if (ci.f0 + (int64_t)jb * CV_B >= p.end) return;  // past the graph's end (a graph shorter than its group)
     const float2* __restrict__ Y = p.y + (size_t)jb * CV_BINS;
     const int t = threadIdx.x;
     if (p.S == 1) {
