@@ -523,6 +523,8 @@ struct wae_batch {
     }
 };
 
+struct PrepState;  // wae_batch_prepare's state (below): what the planners of a batch share
+
 namespace {
 
 // ---- topological order: Graph::order_nodes / visit (src/render/graph.rs:331-487) ---------------------------
@@ -699,6 +701,9 @@ struct NodeTable {
 struct Planner {
     wae_batch* b;
     wae_engine* eng;
+    // a planner of group `grp`: its sizing pass when `sizing_copies` is given (the copies of the AudioBuffers into the group's source slab
+    // are recorded there), else its planning pass proper, which draws from the slab and shares the batch's IR spectra
+    Planner(wae_batch* b, const wae_batch::Group& grp, PrepState& ps, std::vector<wae_batch::Group::SrcCopy>* sizing_copies);
     std::map<std::pair<int, int>, StageBuild> builds;  // (level, kind * 64 + variant)
     std::string error;
     int error_code = 0;
@@ -755,10 +760,15 @@ struct Planner {
     // Node state is allocated through a key (graph, node, n-th allocation of that node, salt): the plans of consecutive
     // render segments (suspend_sync) find the state of a node that lives on, new nodes get fresh (zeroed) state.
     uint32_t key_graph = 0, key_node = 0, key_seq = 0;
+    // Sizing pass: every node-state and arena buffer gets its own placeholder address, numbered by (graph, n-th call in plan_graph), so
+    // that the plan digest sees which buffer feeds which instance.  16 MB apart: offsets into one (a splitter's channel aliases, a layout
+    // track) never reach the next.  Per graph, not per planner: the split sizing pass must number a graph as the serial one does.
+    uint64_t dry_gi = 0, dry_seq = 0;
+    uintptr_t dry_addr() { return (uintptr_t)256 + ((dry_gi + 1) << 44) + (dry_seq++ << 24); }
     uint64_t key_salt = 0;
     template <typename T>
     T* alloc(size_t count, bool zero = false, bool rezero_on_run = false) {
-        if (dry) return reinterpret_cast<T*>(uintptr_t(256));
+        if (dry) return reinterpret_cast<T*>(dry_addr());
         if (seg_start == 0 && seg_end >= lq) return b->dalloc<T>(count, zero, rezero_on_run);  // no suspend point: no later plan looks it up
         const wae_batch::StateKey key{key_graph, key_node, key_seq++, key_salt};
         const size_t bytes = count * sizeof(T);
@@ -826,7 +836,7 @@ struct Planner {
     // renders (its own length in whole quanta): a graph shorter than its group decides what depends on the end of ITS render
     int64_t lq = 0, glq = 0;
     // the graph's rendered PCM in the packed output: [channels][length], frames from `length` on are not written (limit)
-    BufRef dest_ref(const wae_graph* g, uint32_t gi) const { return BufRef{b->d_out + b->out_off[gi], (uint32_t)g->length, 1}; }
+    BufRef dest_ref() const { return BufRef{b->d_out + b->out_off[gi], (uint32_t)g->length, 1}; }
     void begin_segment(int64_t f0, int64_t f1) {
         seg_start = f0;
         seg_end = f1;
@@ -847,6 +857,7 @@ struct Planner {
         }
         return false;
     }
+    bool no_arena() { return bail(WAE_OUT_OF_MEMORY, "out of device memory (arena)"); }
 
     // Scheduling class of a stage.  Graphs without DelayNode feedback: 0 (whole chunks).  Graphs with feedback: 0 = strictly
     // upstream of every cycle (whole chunks, rendered first: sources, a reverb feeding an echo loop), 1 = on a path from a
@@ -869,7 +880,7 @@ struct Planner {
     BufRef arena_buf(int ch, bool with_meta = false) {
         arena_floats_per_frame += (uint64_t)ch;
         const uint32_t mstride = (uint32_t)((b->chunk / 128 + 16) / 16 * 16);
-        BufRef r{reinterpret_cast<float*>(uintptr_t(256)), (uint32_t)b->chunk, 0, nullptr, 0, 0};
+        BufRef r{dry ? reinterpret_cast<float*>(dry_addr()) : nullptr, (uint32_t)b->chunk, 0, nullptr, 0, 0};
         if (!dry) {
             std::vector<float*>& pool = arena_pool[ch];
             size_t& used = arena_used[ch];
@@ -905,18 +916,202 @@ struct Planner {
         stage(L, S_META).meta.push_back(m);
     }
 
-    NodeTable node_table;  // of the graph being planned (reused from graph to graph)
-    NodeTable* cur_pn = nullptr;
+    // ---- the graph being planned (plan_graph), reset from graph to graph
+    wae_graph* g = nullptr;
+    uint32_t gi = 0;
+    Orderer ord{};
+    NodeTable node_table;  // (the per-node vectors keep their capacity)
+    hm::SchedClock clock{48000.f};
+    bool want_scan_coefs = false;  // (the sizing pass needs their number only)
+    // ---- chain fusion (WAE_OPT_FUSE): sources and biquad/gain/shaper nodes are not emitted one stage each; a node
+    // with exactly one consumer stays PENDING, the consumer either extends the chain (same channel count, single
+    // edge) or forces it to be materialised into an arena buffer.  A chain that ends at a destination whose only
+    // input it is writes the final PCM directly.
+    std::map<uint32_t, PendingChain> pending;
+    // what the lowering of one node knows about it once its inputs are planned
+    struct NodeCtx {
+        uint32_t id;
+        Node& n;
+        PNode& p;
+        int level = 0, L = 1;  // L: the stage level of its kernels, after the mixes of its level
+        Lay in0;               // layout of input 0
+        bool dyn_params = false, fuse_n = false;
+        bool extend = false, dest_direct = false;  // it extends / the destination takes the pending chain of `fuse_src`
+        uint32_t fuse_src = 0;
+    };
     struct PRef {
         bool dyn = false;  // automated / audio-rate driven: one value per frame in `track`
         float v = 0.f;
         BufRef track{nullptr, 0, 0};
     };
-    PRef param_ref(wae_graph* g, uint32_t pid);
-    bool plan_graph(wae_graph* g, uint32_t gi);
+    PRef param_ref(uint32_t pid);
+    bool plan_graph(wae_graph* graph, uint32_t graph_index);
     // ir_override: the response of a STATIC HRTF panner (blended, gain folded in): no normalisation, no trimming of small trailing taps;
     // a two-channel input is mixed down to mono by the forward transform's loads (ConvInput::in_channel = -1)
-    bool plan_convolver(wae_graph* g, PNode& pn, int level, const BufRef* dest = nullptr, int64_t dest_limit = -1, const PcmBuffer* ir_override = nullptr);
+    bool plan_convolver(PNode& pn, int level, const BufRef* dest = nullptr, int64_t dest_limit = -1, const PcmBuffer* ir_override = nullptr);
+    bool ir_spectra(const PcmBuffer& ir, float scale, const std::vector<std::vector<float>>& scaled, int Smax, IrSpectra& spec);
+    bool conv_compact_path(PNode& pn, int level, int in_ch, const IrSpectra& spec, int Smax, int blocks_per_chunk);
+    // chain fusion
+    int consumers(uint32_t id) {
+        int k = 0;
+        for (auto& e : ord.edges.at(id))
+            if (e.other_index >= 0) k++;
+        return k;
+    }
+    void emit_chain(PendingChain& pc, int L);
+    bool materialize(uint32_t nid, bool may_alias = false);
+    // can a node of this kind still be appended to the canonical chain gain, A, gain, B, gain, shaper, gain?
+    static bool chain_accepts(const PendingChain& pc, Kind kind) {
+        if (kind == K_GAIN) return true;
+        if (kind == K_BIQUAD) return pc.phase <= 1;
+        if (kind == K_SHAPER) return pc.phase < 5;
+        return false;
+    }
+    // registers this node as the tail of a chain: pending while exactly one consumer may still fuse with it
+    bool finish_chain(NodeCtx& nc, PendingChain&& pc) {
+        nc.p.out_ch = {pc.ch};
+        nc.p.out_buf = {BufRef{nullptr, 0, 0}};
+        nc.p.out_lay = {pc.lay};
+        pending[nc.id] = std::move(pc);
+        if (!(eng->fuse && consumers(nc.n.id) == 1)) return materialize(nc.id);
+        return true;
+    }
+    PendingChain source_chain(int kind, int ch) {
+        PendingChain pc;
+        std::memset(&pc.inst, 0, sizeof(pc.inst));
+        pc.inst.src_kind = kind;
+        pc.inst.ch = ch;
+        pc.inst.limit = -1;
+        pc.inst.end = glq;
+        for (int i = 0; i < 4; i++) pc.inst.g[i] = 1.f;
+        pc.ch = ch;
+        pc.cls = cur_cls;
+        pc.lay = Lay::fixed(ch);
+        return pc;
+    }
+    // chain that this biquad / gain / shaper node joins: its producer's pending chain, or a new one reading in_buf
+    PendingChain open_chain(NodeCtx& nc) {
+        if (nc.extend) {
+            PendingChain pc = std::move(pending.at(nc.fuse_src));
+            pending.erase(nc.fuse_src);
+            return pc;
+        }
+        PendingChain pc = source_chain(CHAIN_SRC_BUFFER, nc.p.in_ch[0]);
+        pc.inst.in = nc.p.in_buf[0];
+        pc.lay = nc.in0;
+        return pc;
+    }
+    // a biquad (or an IIR filter of order <= 2, which opens a chain of its own with a constant layout) appended to the chain it joins
+    bool append_biquad(NodeCtx& nc, double* state, const hm::BiquadCoefs& c) {
+        PendingChain pc = open_chain(nc);
+        ChainBiquad& st = pc.inst.bq[pc.inst.n_biquad++];
+        st.state = state;
+        st.b0 = c.b0; st.b1 = c.b1; st.b2 = c.b2; st.a1 = c.a1; st.a2 = c.a2;
+        pc.coefs[pc.inst.n_biquad - 1] = c;
+        pc.phase = pc.phase == 0 ? 1 : 3;
+        pc.lay = filter_lay(pc.lay);
+        return finish_chain(nc, std::move(pc));
+    }
+    // a node's output buffer and layout
+    bool need_out(NodeCtx& nc, int ch) {
+        nc.p.out_ch = {ch};
+        nc.p.out_buf = {arena_buf(ch)};
+        return nc.p.out_buf[0].p != nullptr || no_arena();
+    }
+    // the node's (single) output has a layout that is not constant: give its buffer a layout track
+    void out_dynamic(NodeCtx& nc, const Lay& l) {
+        PNode& p = nc.p;
+        p.out_lay = {l};
+        if (l.dyn() && !p.out_buf.empty() && p.out_buf[0].p && !p.out_buf[0].absolute) {
+            p.out_buf[0].meta = dry ? reinterpret_cast<uint8_t*>(uintptr_t(256)) : reinterpret_cast<uint8_t*>(p.out_buf[0].p + (size_t)p.out_ch[0] * (size_t)b->chunk);
+            p.out_buf[0].meta_stride = (uint32_t)((b->chunk / 128 + 16) / 16 * 16);
+        }
+    }
+    // a scheduled source: `ch` channels inside [n_first, n_stop), one silent channel outside (never silent when it covers the render)
+    Lay source_lay(int64_t n_first, int64_t n_stop, int ch) const { return (n_first <= 0 && n_stop >= glq) ? Lay::fixed(ch) : Lay::gated(ch); }
+    void source_meta(NodeCtx& nc, int64_t n_first, int64_t n_stop, int ch) {
+        MetaInst m{};
+        m.out = nc.p.out_buf[0];
+        m.mode = META_SOURCE;
+        m.out_ch = ch;
+        m.count = ch;
+        m.n_first = n_first;
+        m.n_stop = n_stop;
+        stage(nc.L, S_META).meta.push_back(m);
+    }
+    // a scheduled source's output buffer: its layout, and the layout track (k_meta) where that is not constant
+    BufRef source_out(NodeCtx& nc, int64_t n_first, int64_t n_stop, int ch) {
+        out_dynamic(nc, source_lay(n_first, n_stop, ch));
+        if (nc.p.out_lay[0].dyn()) source_meta(nc, n_first, n_stop, ch);
+        return nc.p.out_buf[0];
+    }
+    // biquad / IIR (biquad_filter.rs:778-815): silent once the input is and the tail has rung out; keeps the channels of the last
+    // input that was not silent
+    static Lay filter_lay(const Lay& l) { return Lay{(uint8_t)(l.may_silent ? 1 : l.lo), l.hi, l.nlo, l.nhi, l.may_silent}; }
+    // a serial filter behind an input whose layout changes follows the channel count of its last sounding input quantum
+    bool filter_dyn_len(NodeCtx& nc, int ch, int32_t*& dyn_len) {
+        if (!nc.in0.dyn()) return true;
+        dyn_len = alloc<int32_t>((size_t)ch, true, true);
+        if (!dyn_len) return bail(WAE_OUT_OF_MEMORY, "out of device memory (state)");
+        out_dynamic(nc, filter_lay(nc.in0));
+        return true;
+    }
+    // output with the input's layout and channel count: share the input's layout track
+    void out_like_input(NodeCtx& nc) {
+        PNode& p = nc.p;
+        p.out_lay = {nc.in0};
+        if (nc.in0.dyn() && !p.out_buf.empty() && p.out_buf[0].p) {
+            p.out_buf[0].meta = p.in_buf[0].meta;
+            p.out_buf[0].meta_stride = p.in_buf[0].meta_stride;
+        }
+    }
+    // inputs
+    bool mix(int level, const std::vector<PortRef>& edges, int ch, const ChannelCfg& cfg, bool to_dest, bool dyn, bool with_meta, BufRef& out);
+    bool lower_param(uint32_t id, Node& n, PNode& p);
+    bool plan_inputs(NodeCtx& nc);
+    std::vector<int> voice_sum_ports(const NodeCtx& nc);
+    bool plan_port(NodeCtx& nc, int port, int vsum_nb);
+    bool sum_voices(NodeCtx& nc, int port, int ch, int nb);
+    // one method per node kind
+    bool lower_dest(NodeCtx& nc);
+    bool lower_osc(NodeCtx& nc);
+    bool lower_const(NodeCtx& nc);
+    struct AbsnPlay {  // what every playback path of an AudioBufferSourceNode reads
+        const PcmBuffer* pb;
+        float* buf;  // its PCM in the group's slab
+        size_t len, stride;
+        int ch;
+        double duration, ls, le, computed_rate;  // ls / le: the clamped loop boundaries
+    };
+    bool lower_absn(NodeCtx& nc);
+    bool absn_silent(NodeCtx& nc);
+    bool absn_serial(NodeCtx& nc, const AbsnPlay& s, const PRef& pdet, const PRef& prate);
+    bool absn_slow(NodeCtx& nc, const AbsnPlay& s);
+    void absn_schedule(const AbsnSlowInst& a, int64_t n_first, double off, std::vector<int64_t>& seg_n, std::vector<double>& seg_bt) const;
+    bool absn_fast(NodeCtx& nc, const AbsnPlay& s, int64_t q, bool fused);
+    bool lower_biquad(NodeCtx& nc);
+    bool lower_iir(NodeCtx& nc);
+    bool lower_gain(NodeCtx& nc);
+    bool lower_shaper(NodeCtx& nc);
+    bool lower_stereo_panner(NodeCtx& nc);
+    struct HrirAtRate {  // the HRIR sphere at the context's rate
+        uint32_t sr, taps;
+        const float* d_ir;
+        const float* h_ir;  // [vertex][2][taps] on the host
+    };
+    bool lower_panner(NodeCtx& nc);
+    bool hrir_at_rate(HrirAtRate& hr);
+    HrtfSel static_hrtf_sel(const spatial::SpatialParams& sp0) const;
+    bool panner_hrtf_conv(NodeCtx& nc, const spatial::SpatialParams& sp0, const HrirAtRate& hr);
+    bool panner_hrtf_fir(NodeCtx& nc, const spatial::SpatialParams& sp0, const HrirAtRate& hr, bool moving, const SpatialTracks& tr,
+                         const spatial::PanModel& model);
+    bool lower_delay_writer(NodeCtx& nc);
+    bool lower_delay_reader(NodeCtx& nc);
+    bool lower_compressor(NodeCtx& nc);
+    bool lower_analyser(NodeCtx& nc);
+    bool lower_merger(NodeCtx& nc);
+    bool lower_splitter(NodeCtx& nc);
+    bool lower_convolver(NodeCtx& nc);
 };
 
 static uint64_t fnv1a(const void* data, size_t bytes, uint64_t h = 1469598103934665603ull) {
@@ -1106,7 +1301,7 @@ static ScanCoef make_scan_coef(const hm::BiquadCoefs& c) {
     return sc;
 }
 
-bool Planner::plan_convolver(wae_graph* g, PNode& pn, int level, const BufRef* dest, int64_t dest_limit, const PcmBuffer* ir_override) {
+bool Planner::plan_convolver(PNode& pn, int level, const BufRef* dest, int64_t dest_limit, const PcmBuffer* ir_override) {
     Node& n = *pn.n;
     int in_ch = pn.in_ch[0];
     const bool mono_mix = ir_override && in_ch == 2;
@@ -1210,31 +1405,8 @@ bool Planner::plan_convolver(wae_graph* g, PNode& pn, int level, const BufRef* d
         ms.mix.push_back(MixInst{pn.out_buf[0], pn.out_ch[0], 0, 0, (uint32_t)ms.mix_edges.size(), -1});
         return true;
     }
-    // IR spectra (deduplicated across the batch by content)
-    uint64_t key = fnv1a(&scale, sizeof(scale));
-    for (int c = 0; c < ir_ch; c++) key = fnv1a(ir.channels[c].data(), ir_len * sizeof(float), key);
-    key = fnv1a(&ir_len, sizeof(ir_len), key);
     IrSpectra spec;
-    std::unique_lock<std::recursive_mutex> ir_lock(b->mu);
-    auto it = ir_cache->find(key);
-    if (it != ir_cache->end()) {
-        spec = it->second;
-    } else {
-        std::vector<float> flat((size_t)ir_ch * ir_len);
-        for (int c = 0; c < ir_ch; c++) std::memcpy(flat.data() + (size_t)c * ir_len, scaled[c].data(), ir_len * sizeof(float));
-        float* d_ir = dry ? upload(flat) : b->dupload_now(flat);  // (read by launch_conv_ir_fft below: not through the deferred upload slabs)
-        if (!dry) cudaStreamSynchronize(eng->stream);  // `flat` is about to go out of scope
-        spec.S = Smax;
-        spec.channels = ir_ch;
-        // (zeroed: the padding partitions of every channel).  An asset shared by content, not node state: not drawn through the node's
-        // state keys, whose sequence would otherwise depend on whether this segment's plan found the spectra in the cache
-        spec.h = dry ? alloc<float2>(1) : b->dalloc<float2>((size_t)ir_ch * (Smax + WAE_CONV_H_PAD) * WAE_CONV_SPEC, true);
-        if (!d_ir || !spec.h) return bail(WAE_OUT_OF_MEMORY, "out of device memory (IR spectra)");
-        if (!dry) launch_conv_ir_fft(d_ir, (int64_t)ir_len, (int64_t)ir_len, spec.h, Smax, ir_ch, eng->stream);
-        b->asset_bytes += (size_t)ir_ch * (Smax + WAE_CONV_H_PAD) * WAE_CONV_SPEC * 8;
-        (*ir_cache)[key] = spec;
-    }
-    ir_lock.unlock();
+    if (!ir_spectra(ir, scale, scaled, Smax, spec)) return false;
     // inputs: one spectra ring per input channel
     StageBuild& fs = stage(level, S_CONV_FFT);
     int blocks_per_chunk = (int)((b->chunk + WAE_CONV_BLOCK - 1) / WAE_CONV_BLOCK);
@@ -1287,29 +1459,8 @@ bool Planner::plan_convolver(wae_graph* g, PNode& pn, int level, const BufRef* d
         stage(level, r.acc ? S_CONV_MAC_ACC : S_CONV_MAC).conv_path.push_back(p);
     }
     if (compact) {
-        // stream frames of a chunk: at most the chunk's; with the partial block in front they touch one block more
-        const int wblocks = blocks_per_chunk + 1;
-        ConvCmpInst cc{};
-        cc.in = pn.in_buf[0];
-        cc.in_ch = in_ch;
-        cc.x.xring_blocks = Smax + wblocks;
         role(16);  // (16 .. 22, in this order)
-        cc.x.xring = alloc<float2>((size_t)cc.x.xring_blocks * WAE_CONV_SPEC, true);  // (finite: the MAC multiplies stale slots by zero partitions)
-        cc.path.out = pn.out_buf[0];
-        cc.path.h = spec.h + (size_t)WAE_CONV_H_PAD_LO * WAE_CONV_SPEC;
-        cc.path.S = Smax;
-        cc.path.out_channel = 1;
-        cc.path.limit = -1;
-        cc.path.y = alloc<float2>((size_t)wblocks * WAE_CONV_SPEC);
-        cc.cursor = alloc<int64_t>(1, true, true);
-        cc.carry = alloc<float>(2 * WAE_CONV_BLOCK, true, true);
-        cc.win = alloc<float>((size_t)(wblocks + 1) * WAE_CONV_BLOCK);
-        cc.qmap = alloc<int32_t>((size_t)(b->chunk / 128 + 1));
-        cc.wdesc = alloc<int64_t>(2);
-        if (!cc.x.xring || !cc.path.y || !cc.cursor || !cc.carry || !cc.win || !cc.qmap || !cc.wdesc)
-            return bail(WAE_OUT_OF_MEMORY, "out of device memory (convolver, compacted path)");
-        b->arena_bytes += ((size_t)cc.x.xring_blocks + wblocks) * WAE_CONV_SPEC * 8 + (size_t)(wblocks + 1) * WAE_CONV_BLOCK * 4;
-        stage(level, S_CONV_CMP).conv_cmp.push_back(cc);
+        if (!conv_compact_path(pn, level, in_ch, spec, Smax, blocks_per_chunk)) return false;
     }
     // SURVEY §8(d): S*1025*8 B of input-history spectra per convolver-block of 1024 frames
     // (the reference's 1024-frame partitioning defines the algorithmic figure, whatever block size the kernels use)
@@ -1318,9 +1469,66 @@ bool Planner::plan_convolver(wae_graph* g, PNode& pn, int level, const BufRef* d
     return true;
 }
 
-Planner::PRef Planner::param_ref(wae_graph* g, uint32_t pid) {
+// IR spectra (deduplicated across the batch by content)
+bool Planner::ir_spectra(const PcmBuffer& ir, float scale, const std::vector<std::vector<float>>& scaled, int Smax, IrSpectra& spec) {
+    const int ir_ch = (int)ir.channels.size();
+    const size_t ir_len = ir.length();
+    uint64_t key = fnv1a(&scale, sizeof(scale));
+    for (int c = 0; c < ir_ch; c++) key = fnv1a(ir.channels[c].data(), ir_len * sizeof(float), key);
+    key = fnv1a(&ir_len, sizeof(ir_len), key);
+    std::unique_lock<std::recursive_mutex> ir_lock(b->mu);
+    auto it = ir_cache->find(key);
+    if (it != ir_cache->end()) {
+        spec = it->second;
+    } else {
+        std::vector<float> flat((size_t)ir_ch * ir_len);
+        for (int c = 0; c < ir_ch; c++) std::memcpy(flat.data() + (size_t)c * ir_len, scaled[c].data(), ir_len * sizeof(float));
+        float* d_ir = dry ? upload(flat) : b->dupload_now(flat);  // (read by launch_conv_ir_fft below: not through the deferred upload slabs)
+        if (!dry) cudaStreamSynchronize(eng->stream);  // `flat` is about to go out of scope
+        spec.S = Smax;
+        spec.channels = ir_ch;
+        // (zeroed: the padding partitions of every channel).  An asset shared by content, not node state: not drawn through the node's
+        // state keys, whose sequence would otherwise depend on whether this segment's plan found the spectra in the cache
+        spec.h = dry ? reinterpret_cast<float2*>(uintptr_t(256)) : b->dalloc<float2>((size_t)ir_ch * (Smax + WAE_CONV_H_PAD) * WAE_CONV_SPEC, true);
+        if (!d_ir || !spec.h) return bail(WAE_OUT_OF_MEMORY, "out of device memory (IR spectra)");
+        if (!dry) launch_conv_ir_fft(d_ir, (int64_t)ir_len, (int64_t)ir_len, spec.h, Smax, ir_ch, eng->stream);
+        b->asset_bytes += (size_t)ir_ch * (Smax + WAE_CONV_H_PAD) * WAE_CONV_SPEC * 8;
+        (*ir_cache)[key] = spec;
+    }
+    return true;
+}
+
+// the second convolver of a mono response behind an input that switches between one and two channels: input R -> output 1, fed the
+// two-channel quanta only (ConvCmpInst)
+bool Planner::conv_compact_path(PNode& pn, int level, int in_ch, const IrSpectra& spec, int Smax, int blocks_per_chunk) {
+    // stream frames of a chunk: at most the chunk's; with the partial block in front they touch one block more
+    const int wblocks = blocks_per_chunk + 1;
+    ConvCmpInst cc{};
+    cc.in = pn.in_buf[0];
+    cc.in_ch = in_ch;
+    cc.x.xring_blocks = Smax + wblocks;
+    cc.x.xring = alloc<float2>((size_t)cc.x.xring_blocks * WAE_CONV_SPEC, true);  // (finite: the MAC multiplies stale slots by zero partitions)
+    cc.path.out = pn.out_buf[0];
+    cc.path.h = spec.h + (size_t)WAE_CONV_H_PAD_LO * WAE_CONV_SPEC;
+    cc.path.S = Smax;
+    cc.path.out_channel = 1;
+    cc.path.limit = -1;
+    cc.path.y = alloc<float2>((size_t)wblocks * WAE_CONV_SPEC);
+    cc.cursor = alloc<int64_t>(1, true, true);
+    cc.carry = alloc<float>(2 * WAE_CONV_BLOCK, true, true);
+    cc.win = alloc<float>((size_t)(wblocks + 1) * WAE_CONV_BLOCK);
+    cc.qmap = alloc<int32_t>((size_t)(b->chunk / 128 + 1));
+    cc.wdesc = alloc<int64_t>(2);
+    if (!cc.x.xring || !cc.path.y || !cc.cursor || !cc.carry || !cc.win || !cc.qmap || !cc.wdesc)
+        return bail(WAE_OUT_OF_MEMORY, "out of device memory (convolver, compacted path)");
+    b->arena_bytes += ((size_t)cc.x.xring_blocks + wblocks) * WAE_CONV_SPEC * 8 + (size_t)(wblocks + 1) * WAE_CONV_BLOCK * 4;
+    stage(level, S_CONV_CMP).conv_cmp.push_back(cc);
+    return true;
+}
+
+Planner::PRef Planner::param_ref(uint32_t pid) {
     PRef r;
-    PNode* it = cur_pn->find(pid);
+    PNode* it = node_table.find(pid);
     r.v = (it ? *it->n : g->nodes.at(pid)).param.constant_value();
     if (it && !it->out_buf.empty()) {
         r.dyn = true;
@@ -1329,9 +1537,1365 @@ Planner::PRef Planner::param_ref(wae_graph* g, uint32_t pid) {
     return r;
 }
 
-bool Planner::plan_graph(wae_graph* g, uint32_t gi) {
+// ---- chain fusion ---------------------------------------------------------------------------------------------------------
+void Planner::emit_chain(PendingChain& pc, int L) {
+    const int variant = pc.inst.src_kind * 6 + pc.inst.n_biquad * 2 + (pc.inst.has_shaper ? 1 : 0);
+    const int consumer_cls = cur_cls;  // a chain is emitted while its consumer is planned, but runs with its own nodes' class
+    cur_cls = pc.cls;
+    StageBuild& cs = stage(L, S_CHAIN, variant);
+    cur_cls = consumer_cls;
+    for (int k = 0; k < pc.inst.n_biquad; k++) {
+        pc.inst.bq[k].coef = cs.add_scan_coef(want_scan_coefs, [&] { return make_scan_coef(pc.coefs[k]); });
+    }
+    cs.max_ch = std::max(cs.max_ch, pc.ch);
+    cs.chain.push_back(pc.inst);
+}
+
+// may_alias: the consumer reads its input through chan() with any alignment (the convolver's forward transform): a pending chain that
+// is nothing but an AudioBufferSourceNode playing its buffer 1:1 from frame 0, the buffer covering the whole (quantum-padded) render,
+// IS that buffer — no copy into the arena
+bool Planner::materialize(uint32_t nid, bool may_alias) {
+    auto it = pending.find(nid);
+    if (it == pending.end()) return true;
+    PNode& sp = node_table.at(nid);
+    {
+        const ChainInst& ci = it->second.inst;
+        const AbsnInst& a = ci.absn;
+        bool unit = true;
+        for (int i = 0; i < 4; i++) unit = unit && ci.g[i] == 1.f;
+        if (may_alias && ci.src_kind == CHAIN_SRC_ABSN && ci.n_biquad == 0 && !ci.has_shaper && unit && it->second.phase == 0 &&
+            !it->second.lay.dyn() && a.n_start == 0 && !a.loop && a.buf_offset == 0 && a.buf_len >= lq && a.buf_stride <= 0xffffffffll &&
+            seg_start == 0 && seg_end >= lq) {
+            sp.out_buf = {BufRef{const_cast<float*>(a.buf), (uint32_t)a.buf_stride, 1}};
+            pending.erase(it);
+            return true;
+        }
+    }
+    BufRef buf = arena_buf(it->second.ch, it->second.lay.dyn());  // (k_chain writes the layout track itself)
+    if (!buf.p) return no_arena();
+    it->second.inst.out = buf;
+    it->second.inst.limit = -1;
+    it->second.inst.out_dup = 0;
+    emit_chain(it->second, 2 * sp.level + 1);
+    sp.out_buf = {buf};
+    pending.erase(it);
+    return true;
+}
+
+// ---- inputs ---------------------------------------------------------------------------------------------------------------
+// AudioRenderQuantum::add of `edges` into `ch` channels under `cfg` (k_mix, or k_mix_dyn when `dyn`), written to the graph's rendered PCM
+// (`to_dest`) or to a new arena buffer (`with_meta`: with a layout track): `out`
+bool Planner::mix(int level, const std::vector<PortRef>& edges, int ch, const ChannelCfg& cfg, bool to_dest, bool dyn, bool with_meta, BufRef& out) {
+    StageBuild& ms = stage(level, dyn ? S_MIX_DYN : S_MIX);
+    if (to_dest) {
+        if (g->length > 0xffffffffull) return bail(WAE_UNSUPPORTED, "render length above 2^32 frames");
+        out = dest_ref();
+    } else {
+        out = arena_buf(ch, with_meta);
+        if (!out.p) return no_arena();
+    }
+    const uint32_t edge_offset = (uint32_t)ms.mix_edges.size();
+    for (auto& r : edges) {
+        PNode& s = node_table.at(r.node);
+        ms.mix_edges.push_back(MixEdge{s.out_buf[r.port], s.out_ch[r.port], 0});
+    }
+    const int64_t limit = to_dest ? (int64_t)g->length : -1;
+    if (dyn) {
+        MixDynInst m{};
+        m.out = out;
+        m.out_ch = ch;
+        m.interp = cfg.interp;
+        m.mode = cfg.mode;
+        m.cfg_count = cfg.count;
+        m.n_edges = (int)edges.size();
+        m.edge_offset = edge_offset;
+        m.limit = limit;
+        ms.mix_dyn.push_back(m);
+    } else {
+        MixInst m{};
+        m.out = out;
+        m.out_ch = ch;
+        m.interp = cfg.interp;
+        m.n_edges = (int)edges.size();
+        m.edge_offset = edge_offset;
+        m.limit = limit;
+        ms.mix.push_back(m);
+    }
+    return true;
+}
+
+// AudioParamProcessor (param.rs:685-797): only params with automation events or audio-rate inputs become
+// GPU work; a constant param is a scalar in its owner's instance
+bool Planner::lower_param(uint32_t id, Node& n, PNode& p) {
+    auto& edges = p.in_edges[0];
+    // (a render without suspend points never replays a timeline: a constant param needs no record at all — most params are)
+    if (seg_start == 0 && seg_end >= lq && edges.empty() && n.param.constant()) return true;
+    const ParamTimeline* tlp = param_timeline(gi, id, n.param, g->sample_rate);
+    if (n.param.constant() && edges.empty()) return true;
+    int level = 0;
+    for (auto& r : edges) level = std::max(level, node_table.at(r.node).level + 1);
+    p.level = level;
+    for (auto& r : edges)
+        if (!materialize(r.node)) return false;
+    const ParamTimeline& tl = *tlp;
+    if (!tl.error.empty()) return bail(WAE_NOT_SUPPORTED, tl.error);
+    ParamInst pi{};
+    if (!edges.empty()) {  // sum of the connected signals, first channel each (1 / explicit / discrete, param.rs:296-310)
+        bool any_dyn = false;
+        for (auto& r : edges) any_dyn = any_dyn || node_table.at(r.node).lay_out(r.port).dyn();
+        // edges whose layout changes: folded per quantum; a silent sum reads as zeros, which is what the param adds then
+        const ChannelCfg first_channel{1, WAE_COUNT_MODE_EXPLICIT, WAE_INTERPRETATION_DISCRETE};
+        if (!mix(2 * level, edges, 1, first_channel, false, any_dyn, false, pi.in)) return false;
+    }
+    pi.events = tl.events.empty() ? nullptr : upload(tl.events);
+    pi.curves = tl.curves.empty() ? nullptr : upload(tl.curves);
+    pi.state = alloc<ParamState>(1, true, true);
+    pi.out = arena_buf(2);  // channel 0: value per frame, channel 1: single-valued flag per quantum
+    if (!pi.state || !pi.out.p) return bail(WAE_OUT_OF_MEMORY, "out of device memory (param)");
+    pi.def = n.param.default_value;
+    pi.mn = n.param.min_value;
+    pi.mx = n.param.max_value;
+    pi.intrinsic0 = tl.intrinsic;
+    pi.has_last0 = tl.has_last ? 1 : 0;
+    pi.last0 = tl.last;
+    pi.sample_rate = g->sample_rate;
+    pi.n_events = (int32_t)tl.events.size();
+    pi.a_rate = n.param.a_rate ? 1 : 0;
+    stage(2 * level + 1, S_PARAM).param.push_back(pi);
+    p.out_ch = {1};
+    p.out_buf = {pi.out};
+    return true;
+}
+
+// ---- inputs: static channel count + mix stage where needed
+bool Planner::plan_inputs(NodeCtx& nc) {
+    Node& n = nc.n; PNode& p = nc.p;
+    NodeTable& pn = node_table;
+    int level = 0;
+    for (auto& port : p.in_edges)
+        for (auto& r : port) level = std::max(level, pn.at(r.node).level + 1);
+    bool dyn_params = false;
+    for (uint32_t pid : n.params) {
+        PNode& pp = pn.at(pid);
+        if (!pp.out_buf.empty()) {
+            dyn_params = true;
+            level = std::max(level, pp.level + 1);
+        }
+    }
+    if (n.kind == K_PANNER)
+        for (uint32_t pid = 2; pid <= 10; pid++)
+            if (pn.count(pid) && !pn.at(pid).out_buf.empty()) level = std::max(level, pn.at(pid).level + 1);
+    p.level = level;
+    nc.level = level;
+    nc.L = 2 * level + 1;  // node kernels run after the mixes of their level
+    nc.dyn_params = dyn_params;
+    const bool fuse = eng->fuse;
+    nc.fuse_n = fuse && !dyn_params;  // nodes with automated params run their own a-rate kernels
+    // does this node extend the pending chain of its only producer / take it as the destination's only input?
+    const bool chain_kind = !dyn_params && ((n.kind == K_BIQUAD && !eng->serial_filters) || (fuse && (n.kind == K_GAIN || (n.kind == K_SHAPER && !(n.oversample && n.has_curve)))));
+    if (fuse && n.n_inputs == 1 && p.in_edges[0].size() == 1 && p.in_edges[0][0].port == 0) {
+        auto it = pending.find(p.in_edges[0][0].node);
+        if (it != pending.end()) {
+            int sch = pn.at(it->first).out_ch[0];
+            if (chain_kind && computed_channels(n.cfg, sch) == sch && chain_accepts(it->second, n.kind)) {
+                nc.extend = true;
+                nc.fuse_src = it->first;
+            } else if (n.kind == K_DEST && g->length <= 0xffffffffull &&
+                       (sch == (int)g->channels || (sch == 1 && g->channels == 2 && n.cfg.interp == WAE_INTERPRETATION_SPEAKERS))) {
+                nc.dest_direct = true;
+                nc.fuse_src = it->first;
+            }
+        }
+    }
+    const std::vector<int> vsum_nb = voice_sum_ports(nc);
+    for (size_t pi = 0; pi < p.in_edges.size(); pi++) {
+        if (vsum_nb[pi] >= 0) continue;
+        auto& port = p.in_edges[pi];
+        for (auto& r : port)
+            if (!((nc.extend || nc.dest_direct) && r.node == nc.fuse_src))
+                if (!materialize(r.node, n.kind == K_CONV && n.buffer && port.size() == 1)) return false;
+    }
+    p.in_ch.assign(n.n_inputs, 1);
+    p.in_buf.assign(n.n_inputs, BufRef{nullptr, 0, 0});
+    p.in_lay.assign(n.n_inputs, Lay::fixed(1));
+    for (int port = 0; port < n.n_inputs; port++)
+        if (!plan_port(nc, port, vsum_nb[port])) return false;
+    nc.in0 = p.in_lay.empty() ? Lay::fixed(1) : p.in_lay[0];
+    return true;
+}
+
+// ---- k_voice_sum (WAE_OPT_VOICE_SUM): a port fed by many oscillator -> [biquad] -> gain voices, all of them still pending chains
+// (mono, constant layout, one consumer): the voices are not materialised, one kernel renders them and keeps the running sum in
+// registers, in the port's edge order.  Only when the launch has enough (2048-frame tile, port) work items to fill the machine
+// about twice: one graph with thousands of voices and a short render (configs[2]) is better served by k_chain + k_mix, which
+// take their parallelism from the voices.
+// Per input port: the biquads of each of its voices when it is rendered that way, else -1.
+std::vector<int> Planner::voice_sum_ports(const NodeCtx& nc) {
+    const Node& n = nc.n;
+    std::vector<int> port_vsum_nb(nc.p.in_edges.size(), -1);
+    if (!(eng->fuse && voice_sum_mode() != 0 && !nc.extend && !nc.dest_direct && cur_cls == 0 && n.kind != K_DELAY_R)) return port_vsum_nb;
+    for (size_t pi = 0; pi < nc.p.in_edges.size() && (int)pi < n.n_inputs; pi++) {
+        const auto& edges = nc.p.in_edges[pi];
+        if ((int)edges.size() < 8) continue;
+        const int ch = computed_channels(n.cfg, 1);
+        if (!(ch == 1 || (ch == 2 && n.cfg.interp == WAE_INTERPRETATION_SPEAKERS))) continue;
+        if (n.kind == K_DEST && g->length > 0xffffffffull) continue;
+        const int64_t tiles = (seg_end - seg_start + 2047) / 2048;
+        if (voice_sum_mode() < 2 && tiles * (int64_t)group_graphs < 2 * (int64_t)voice_sum_slots()) continue;
+        int nb = -1;
+        bool ok = true;
+        std::set<uint32_t> seen_nodes;
+        for (auto& r : edges) {
+            auto it = pending.find(r.node);
+            if (r.port != 0 || it == pending.end()) { ok = false; break; }
+            const PendingChain& pc = it->second;
+            if (pc.inst.src_kind != CHAIN_SRC_OSC || pc.ch != 1 || pc.inst.has_shaper || pc.inst.n_biquad > 1 || pc.lay.dyn() || pc.cls != cur_cls ||
+                (nb >= 0 && nb != pc.inst.n_biquad) || !seen_nodes.insert(r.node).second) { ok = false; break; }
+            nb = pc.inst.n_biquad;
+        }
+        if (!ok) continue;
+        port_vsum_nb[pi] = nb;
+    }
+    return port_vsum_nb;
+}
+
+// one input port: its channel count, layout and buffer (`vsum_nb` >= 0: its voices and their sum in one kernel, see voice_sum_ports)
+bool Planner::plan_port(NodeCtx& nc, int port, int vsum_nb) {
+    Node& n = nc.n; PNode& p = nc.p;
+    NodeTable& pn = node_table;
+    auto& edges = p.in_edges[port];
+    int max_in = 1;
+    for (auto& r : edges) max_in = std::max(max_in, pn.at(r.node).out_ch[r.port]);
+    int ch = computed_channels(n.cfg, max_in);
+    if (n.kind == K_DELAY_R) {  // the reader's only input is the hidden writer edge: take the writer's layout
+        ch = max_in;
+    }
+    p.in_ch[port] = ch;
+    p.in_lay[port] = Lay::fixed(ch);
+    bool is_dest = n.kind == K_DEST;
+    if (nc.extend || nc.dest_direct) {  // the producer's chain is consumed in registers / written directly
+        if (nc.extend) p.in_lay[port] = pending.at(nc.fuse_src).lay;
+        return true;
+    }
+    if (vsum_nb >= 0) return sum_voices(nc, port, ch, vsum_nb);
+    if (is_dest && edges.size() == 1 && pn.at(edges[0].node).wrote_dest) {  // the producer already wrote the rendered PCM
+        p.in_buf[port] = pn.at(edges[0].node).out_buf[edges[0].port];
+        return true;
+    }
+    // ---- the port's layout over time: AudioRenderQuantum::add folded over the edges (quantum.rs:532-569)
+    bool any_dyn = false;
+    Lay pl = Lay::fixed(ch);
+    if (!edges.empty()) {
+        int lo = 1, hi = 1, on_nlo = 0, min_nlo = 255;
+        bool all_may_silent = true;
+        for (auto& r : edges) {
+            const Lay el = pn.at(r.node).lay_out(r.port);
+            any_dyn = any_dyn || el.dyn();
+            lo = std::max<int>(lo, el.lo);
+            hi = std::max<int>(hi, el.hi);
+            if (!el.may_silent) on_nlo = std::max<int>(on_nlo, el.nlo);
+            min_nlo = std::min<int>(min_nlo, el.nlo);
+            all_may_silent = all_may_silent && el.may_silent;
+        }
+        const int nlo = std::max(on_nlo, min_nlo);
+        pl.lo = (uint8_t)computed_channels(n.cfg, lo);
+        pl.hi = (uint8_t)computed_channels(n.cfg, hi);
+        pl.nlo = (uint8_t)computed_channels(n.cfg, nlo);
+        pl.nhi = pl.hi;
+        pl.may_silent = all_may_silent;
+        if (n.kind == K_DELAY_R) pl = pn.at(edges[0].node).lay_out(edges[0].port);
+    }
+    // more than two layouts meeting in a port wider than stereo: the order of the up-mixes matters (mono, stereo, 5.1: the
+    // reference goes 1 -> 2 -> 6): fold edge by edge like it does
+    bool needs_fold = false;
+    if (ch > 2 && n.cfg.mode != WAE_COUNT_MODE_EXPLICIT)
+        for (auto& r : edges) needs_fold = needs_fold || pn.at(r.node).out_ch[r.port] != ch;
+    if (!is_dest && edges.size() == 1 && pn.at(edges[0].node).out_ch[edges[0].port] == ch) {
+        const Lay el = pn.at(edges[0].node).lay_out(edges[0].port);
+        // a single edge IS the port when computedNumberOfChannels leaves every count it can have alone
+        const bool identity = !el.dyn() || n.kind == K_DELAY_R || n.cfg.mode == WAE_COUNT_MODE_MAX ||
+                              (n.cfg.mode == WAE_COUNT_MODE_CLAMPED_MAX && el.hi <= n.cfg.count);
+        // the time-batched convolver reads all static channels of every quantum: it needs the canonical PCM k_mix_dyn writes
+        const bool canonical_needed = el.dyn() && n.kind == K_CONV;
+        if (identity && !canonical_needed) {
+            p.in_buf[port] = pn.at(edges[0].node).out_buf[edges[0].port];  // alias, no copy
+            p.in_lay[port] = el;
+            return true;
+        }
+    }
+    const bool dyn = any_dyn || needs_fold;
+    if (!mix(2 * nc.level, edges, ch, n.cfg, is_dest, dyn, dyn && pl.dyn(), p.in_buf[port])) return false;
+    if (dyn) p.in_lay[port] = pl;
+    return true;
+}
+
+// the voices of this port and their sum in one kernel
+bool Planner::sum_voices(NodeCtx& nc, int port, int ch, int nb) {
+    auto& edges = nc.p.in_edges[port];
+    StageBuild& vs = stage(2 * nc.level, S_VSUM, nb);
+    VoiceGroup vg{};
+    vg.first = (int32_t)vs.chain.size();
+    vg.n_voices = (int32_t)edges.size();
+    vg.out_dup = ch;
+    vg.limit = -1;
+    if (nc.n.kind == K_DEST) {
+        vg.out = dest_ref();
+        vg.limit = (int64_t)g->length;
+    } else {
+        vg.out = arena_buf(ch);
+        if (!vg.out.p) return no_arena();
+    }
+    for (auto& r : edges) {
+        PendingChain pc = std::move(pending.at(r.node));
+        pending.erase(r.node);
+        // (k_voice_sum prefetches the constants of voice k as coefficient set k: one set per voice, in voice order)
+        if (pc.inst.n_biquad == 1 && vs.n_scan_coef != vs.chain.size()) return bail(WAE_UNSUPPORTED, "internal: voice-sum coefficient table out of step");
+        for (int k = 0; k < pc.inst.n_biquad; k++)
+            pc.inst.bq[k].coef = vs.add_scan_coef(want_scan_coefs, [&] { return make_scan_coef(pc.coefs[k]); });
+        pc.inst.limit = -1;
+        pc.inst.out_dup = 0;
+        vs.chain.push_back(pc.inst);
+    }
+    vs.vgroups.push_back(vg);
+    nc.p.in_buf[port] = vg.out;
+    return true;
+}
+
+// ---- one lowering per node kind -------------------------------------------------------------------------------------------
+bool Planner::lower_dest(NodeCtx& nc) {
+    PNode& p = nc.p;
+    p.out_ch = {(int)g->channels};
+    if (nc.dest_direct) {  // the chain writes the rendered PCM itself (speaker up-mix 1->2 = copy, quantum.rs:301-305)
+        PendingChain pc = std::move(pending.at(nc.fuse_src));
+        pending.erase(nc.fuse_src);
+        const BufRef fin = dest_ref();
+        pc.inst.out = fin;
+        pc.inst.limit = (int64_t)g->length;
+        pc.inst.out_dup = (pc.ch == 1 && g->channels == 2) ? 2 : 0;
+        emit_chain(pc, nc.L);
+        node_table.at(nc.fuse_src).out_buf = {fin};
+        p.in_buf[0] = fin;
+    }
+    p.out_buf = {p.in_buf[0]};
+    algorithmic_bytes += (uint64_t)g->channels * g->length * 4;  // destination write, SURVEY §8(d)
+    return true;
+}
+
+bool Planner::lower_osc(NodeCtx& nc) {
+    Node& n = nc.n; PNode& p = nc.p;
+    const double sr = (double)g->sample_rate;
+    PRef pf = param_ref(n.params[0]), pd = param_ref(n.params[1]);
+    float freq = pf.v, detune = pd.v;
+    if (!nc.fuse_n && !need_out(nc, 1)) return false;
+    OscInst o{};
+    double start_ratio = 0.;
+    if (!nc.fuse_n) o.out = p.out_buf[0];
+    o.type = n.type;
+    double computed_freq = (double)freq * std::exp2((double)detune / 1200.);  // oscillator.rs:30-32
+    o.incr = computed_freq / sr;
+    o.inv_incr = o.incr != 0. ? 1. / o.incr : 0.;
+    o.outside_nyquist = std::fabs(computed_freq) >= sr / 2.;
+    o.n_first = std::numeric_limits<int64_t>::max();
+    o.n_stop = std::numeric_limits<int64_t>::max();
+    o.phase0 = 0.;
+    if (n.start_time < 1e300) {
+        // oscillator.rs:391-428,511-540: first rendered frame and its phase
+        int64_t q = clock.quantum_containing(n.start_time);
+        double start = n.start_time;
+        if (start < clock.block_time(q)) start = clock.block_time(q);  // "prevent scheduling in the past"
+        double t = 0.;
+        // walk the accumulated per-frame clock of that quantum
+        double cur = clock.block_time(q);
+        int i = 0;
+        for (; i < 128; i++) {
+            if (!(cur < start)) break;
+            cur += clock.dt;
+        }
+        t = cur;
+        o.n_first = q * 128 + i;
+        if (i < 128 && t > start) {
+            double ratio = (t - start) / clock.dt;
+            start_ratio = ratio;
+            double ph = o.incr * ratio;
+            if (o.outside_nyquist) {
+                ph = std::fmod(ph, 1.);
+                if (ph < 0.) ph += 1.;
+            } else {
+                ph = hm::unroll_phase(ph);
+            }
+            o.phase0 = ph;
+        }
+        if (n.stop_time < 1e300) {
+            int64_t qs = clock.quantum_containing(n.stop_time);
+            if (n.stop_time <= clock.block_time(qs)) o.n_stop = qs * 128;
+            else o.n_stop = clock.first_frame_at_or_after(n.stop_time);
+        }
+    }
+    if (n.type == WAE_OSC_CUSTOM) {
+        float* d = upload(n.table);
+        o.table = d;
+        o.table_len = (int)n.table.size();
+    } else {
+        o.table = eng->d_sine;
+        o.table_len = 2048;
+    }
+    o.fast = (!o.outside_nyquist && o.incr > 0. && o.incr < 0.5 && (o.table_len == 2048 || (o.type != WAE_OSC_SINE && o.type != WAE_OSC_CUSTOM))) ? 1 : 0;
+    if (nc.dyn_params) {  // automated / audio-rate frequency or detune: running-sum phase
+        OscArInst oa{};
+        oa.base = o;
+        oa.freq = pf.dyn ? pf.track : BufRef{nullptr, 0, 0};
+        oa.detune = pd.dyn ? pd.track : BufRef{nullptr, 0, 0};
+        oa.f_val = freq;
+        oa.d_val = detune;
+        oa.start_ratio = start_ratio;
+        oa.phase = alloc<double>(1, true, true);
+        oa.sample_rate = g->sample_rate;
+        if (!oa.phase) return bail(WAE_OUT_OF_MEMORY, "out of device memory (state)");
+        oa.base.out = source_out(nc, o.n_first, o.n_stop, 1);
+        stage(nc.L, S_OSC_AR).osc_ar.push_back(oa);
+    } else if (nc.fuse_n) {
+        PendingChain pc = source_chain(CHAIN_SRC_OSC, 1);
+        pc.inst.osc = o;
+        pc.lay = source_lay(o.n_first, o.n_stop, 1);
+        return finish_chain(nc, std::move(pc));
+    } else {
+        o.out = source_out(nc, o.n_first, o.n_stop, 1);
+        stage(nc.L, S_OSC).osc.push_back(o);
+    }
+    return true;
+}
+
+bool Planner::lower_const(NodeCtx& nc) {
+    Node& n = nc.n; PNode& p = nc.p;
+    PRef po = param_ref(n.params[0]);
+    float v = po.v;
+    if (!nc.fuse_n && !need_out(nc, 1)) return false;
+    ConstInst c{};
+    if (!nc.fuse_n) c.out = p.out_buf[0];
+    if (po.dyn) c.track = po.track;
+    c.value = v;
+    c.n_first = std::numeric_limits<int64_t>::max();
+    c.n_stop = std::numeric_limits<int64_t>::max();
+    if (n.start_time < 1e300) {
+        // constant_source.rs:203-246
+        c.n_first = clock.first_frame_at_or_after(n.start_time);
+        if (n.stop_time < 1e300) c.n_stop = clock.first_frame_at_or_after(n.stop_time);
+    }
+    if (nc.fuse_n) {
+        PendingChain pc = source_chain(CHAIN_SRC_CONST, 1);
+        pc.inst.cst = c;
+        pc.lay = source_lay(c.n_first, c.n_stop, 1);
+        return finish_chain(nc, std::move(pc));
+    }
+    c.out = source_out(nc, c.n_first, c.n_stop, 1);
+    stage(nc.L, S_CONST).cst.push_back(c);
+    return true;
+}
+
+static bool almost_equal(double x, double y) {
+    if (x == y) return true;
+    const double tol = 1.4901161193847656e-8;
+    double d = std::fabs(y - x);
+    return d <= tol || d <= std::max(std::fabs(x), std::fabs(y)) * tol;
+}
+
+bool Planner::lower_absn(NodeCtx& nc) {
+    Node& n = nc.n;
+    const double sr = (double)g->sample_rate;
+    PRef pdet = param_ref(n.params[0]), prate = param_ref(n.params[1]);
+    const float detune = pdet.v, rate = prate.v;
+    const bool rate_automated = pdet.dyn || prate.dyn;
+    int ch = n.buffer ? (int)n.buffer->channels.size() : 1;
+    if (!n.buffer || n.start_time >= 1e300 || ch == 0) return absn_silent(nc);  // never plays: silence
+    PcmBuffer& pb = *n.buffer;
+    double computed_rate = (double)rate * std::exp2((double)detune / 1200.);
+    double duration = pb.duration();
+    double ls = n.loop_start, le = n.loop_end;  // clamp_loop_boundaries, audio_buffer_source.rs:400-417
+    if (ls < 0.) ls = 0.; else if (ls > duration) ls = duration;
+    if (le <= 0. || le > duration) le = duration;
+    int64_t q = clock.quantum_containing(n.start_time);
+    // a start time that IS the next block boundary but compares below next_block_time by one rounding:
+    // the reference goes through one all-silent slow-track quantum, then aligns (audio_buffer_source.rs:521-523)
+    if (n.start_time > clock.block_time(q) && n.start_time == clock.block_time(q + 1)) q = q + 1;
+    bool aligned = (n.start_time <= clock.block_time(q)) && n.offset == 0.;  // start in the past snaps to the block
+    bool fast = !rate_automated && aligned && (double)pb.sample_rate / sr == 1. && computed_rate == 1. && ls == 0. && le == duration &&
+                n.duration > 1e300 && n.stop_time > 1e300;
+    // everything the closed-form tracks do not cover runs the renderer's own frame loop (one warp per source)
+    bool serial = rate_automated || (!fast && !(computed_rate > 0.));
+    if (!fast && !serial && n.loop) {
+        const bool custom = ls >= 0. && le > 0. && ls < le;
+        const double loop_len = custom ? le - ls : duration;
+        if (!(loop_len > 4. * clock.dt * computed_rate)) serial = true;  // loop shorter than four output frames
+    }
+    const bool fused = nc.fuse_n && fast;
+    if (!fused && !need_out(nc, ch)) return false;
+    size_t len = pb.length();
+    size_t stride = (len + 3) / 4 * 4;  // every channel starts 16 B aligned (LDG.128)
+    // one copy of the PCM per AudioBuffer in the group's slab (the grains of a granular patch all play the same one: the graph
+    // holds it once, wae_abi_graph.cpp copy_buffer), shared by the plans of all render segments
+    auto so = src_offsets.find({gi, nc.id});
+    bool first_use = so == src_offsets.end();
+    if (first_use) {
+        auto bo = buf_offsets.find(n.buffer.get());
+        if (bo != buf_offsets.end()) first_use = false;  // (already in the slab for another node)
+        else bo = buf_offsets.emplace(n.buffer.get(), src_cursor).first;
+        so = src_offsets.emplace(std::make_pair(gi, nc.id), bo->second).first;
+    }
+    float* d_buf = d_src + so->second;
+    if (first_use) {
+        if (src_copies)  // recorded by the sizing pass: uploaded straight from the graph's buffer, planar [ch][stride] like the slab
+            src_copies->push_back(wae_batch::Group::SrcCopy{n.buffer, src_cursor, (size_t)ch * stride});
+        src_cursor += (size_t)ch * stride;
+        b->asset_bytes += (size_t)ch * len * 4;
+    }
+    const AbsnPlay s{&pb, d_buf, len, stride, ch, duration, ls, le, computed_rate};
+    if (serial) return absn_serial(nc, s, pdet, prate);
+    if (!fast) return absn_slow(nc, s);
+    return absn_fast(nc, s, q, fused);
+}
+
+bool Planner::absn_silent(NodeCtx& nc) {
+    if (!need_out(nc, 1)) return false;
+    StageBuild& ms = stage(nc.L, S_MIX);
+    ms.mix.push_back(MixInst{nc.p.out_buf[0], 1, 0, 0, (uint32_t)ms.mix_edges.size(), -1});
+    out_dynamic(nc, Lay{1, 1, 1, 1, true});  // silent for good
+    if (nc.p.out_buf[0].meta) source_meta(nc, 0, 0, 1);
+    return true;
+}
+
+bool Planner::absn_serial(NodeCtx& nc, const AbsnPlay& s, const PRef& pdet, const PRef& prate) {
+    Node& n = nc.n;
+    AbsnSerialInst a{};
+    a.out = nc.p.out_buf[0];
+    a.buf = s.buf;
+    a.buf_len = (int64_t)s.len;
+    a.buf_stride = (int64_t)s.stride;
+    a.start_time = n.start_time;
+    a.stop_time = n.stop_time;
+    a.offset = n.offset;
+    a.duration = n.duration;
+    a.loop_start = s.ls;
+    a.loop_end = s.le;
+    a.buffer_duration = s.duration;
+    a.buffer_sample_rate = (double)s.pb->sample_rate;
+    a.sample_rate = (double)g->sample_rate;
+    const BufRef none{nullptr, 0, 0};
+    a.rate_track = prate.dyn ? prate.track : none;
+    a.detune_track = pdet.dyn ? pdet.track : none;
+    a.rate = prate.v;
+    a.detune = pdet.v;
+    a.ch = s.ch;
+    a.loop = n.loop ? 1 : 0;
+    a.state = alloc<AbsnSerialState>(1, true, true);
+    if (!a.state) return bail(WAE_OUT_OF_MEMORY, "out of device memory (buffer source state)");
+    out_dynamic(nc, Lay::gated(s.ch));  // when it plays depends on the automated rate: the kernel writes the layout track
+    a.out = nc.p.out_buf[0];
+    stage(nc.L, S_ABSN_SERIAL).absn_serial.push_back(a);
+    algorithmic_bytes += (uint64_t)s.ch * 4ull * (uint64_t)std::min<int64_t>(lq, (int64_t)s.len);
+    return true;
+}
+
+// ---- slow track (audio_buffer_source.rs:625-823): fractional playhead
+bool Planner::absn_slow(NodeCtx& nc, const AbsnPlay& s) {
+    Node& n = nc.n;
+    const double sr = (double)g->sample_rate;
+    const double duration = s.duration, computed_rate = s.computed_rate;
+    AbsnSlowInst a{};
+    a.out = nc.p.out_buf[0];
+    a.buf = s.buf;
+    a.buf_len = (int64_t)s.len;
+    a.buf_stride = (int64_t)s.stride;
+    a.ch = s.ch;
+    a.loop = n.loop ? 1 : 0;
+    a.sample_rate = sr;
+    a.buffer_duration = duration;
+    a.pos_scale = ((double)s.pb->sample_rate / sr) * sr;  // position = buffer_time * sampling_ratio; playhead = position * sr
+    a.step = clock.dt * computed_rate;
+    a.duration = n.duration;
+    // actual loop points (:627-636)
+    if (n.loop && s.ls >= 0. && s.le > 0. && s.ls < s.le) {
+        a.loop_start = s.ls;
+        a.loop_end = s.le;
+    } else {
+        a.loop_start = 0.;
+        a.loop_end = duration;
+    }
+    // first frame at / after the start time: current_time = block_time + i * dt (:648), sticky within
+    // almost::equal (:652-654)
+    double start = n.start_time;
+    int64_t qq = clock.quantum_containing(start);
+    int64_t n_first = -1;
+    double t_first = 0.;
+    for (int guard = 0; guard < 3 && n_first < 0; guard++, qq++) {
+        double bt0 = clock.block_time(qq);
+        for (int i = 0; i < 128; i++) {
+            double t = bt0 + (double)i * clock.dt;
+            if (almost_equal(t, start)) start = t;
+            if (!(t < start)) {
+                n_first = qq * 128 + i;
+                t_first = t;
+                break;
+            }
+        }
+    }
+    if (n_first < 0) n_first = qq * 128;
+    double delta = t_first - start;
+    double off = n.offset + delta * computed_rate;  // :672-674
+    off = std::min(std::max(off, 0.), duration);
+    if (n.loop && off > a.loop_end) off = a.loop_end;  // :676-678 (rate >= 0)
+    a.offset0 = off;
+    a.elapsed0 = std::fabs(delta * computed_rate);
+    a.n_first = n_first;
+    a.n_stop = std::numeric_limits<int64_t>::max();
+    if (n.stop_time < 1e300) {  // first frame with current_time >= stop_time (:663)
+        int64_t qs = clock.quantum_containing(n.stop_time);
+        int64_t ns = (qs + 1) * 128;
+        double bt0 = clock.block_time(qs);
+        for (int i = 0; i < 128; i++)
+            if (bt0 + (double)i * clock.dt >= n.stop_time) {
+                ns = qs * 128 + i;
+                break;
+            }
+        a.n_stop = ns;
+    }
+    std::vector<int64_t> seg_n{n_first};
+    std::vector<double> seg_bt{off};
+    if (n.loop && off < a.loop_end) absn_schedule(a, n_first, off, seg_n, seg_bt);
+    a.n_seg = (int32_t)seg_n.size();
+    a.seg_n = upload(seg_n);
+    a.seg_bt = upload(seg_bt);
+    {
+        // layout: silent before the quantum of the first playing frame and after the quantum in which the source ends
+        // (stop time, explicit duration, or — not looping — the end of the buffer; audio_buffer_source.rs:826-838)
+        int64_t n_end = a.n_stop;
+        if (a.step > 0.) {
+            if (!n.loop) n_end = std::min<int64_t>(n_end, n_first + (int64_t)std::ceil(std::max(0., duration - off) / a.step));
+            if (n.duration < 1e300) n_end = std::min<int64_t>(n_end, n_first + (int64_t)std::ceil(std::max(0., n.duration - a.elapsed0) / a.step));
+        }
+        a.out = source_out(nc, n_first, n_end, s.ch);
+    }
+    stage(nc.L, S_ABSN_SLOW).absn_slow.push_back(a);
+    algorithmic_bytes += (uint64_t)s.ch * 4ull * (uint64_t)std::min<int64_t>(lq, (int64_t)s.len);
+    return true;
+}
+
+// playhead schedule of a looping slow-track source: walk the reference's per-frame bookkeeping (:730-770) from event to event — a
+// frame where buffer_time is snapped to a loop point (almost::equal) or wrapped starts a new segment
+void Planner::absn_schedule(const AbsnSlowInst& a, int64_t n_first, double off, std::vector<int64_t>& seg_n, std::vector<double>& seg_bt) const {
+    const double ls2 = a.loop_start, le2 = a.loop_end, len2 = le2 - ls2, step = a.step;
+    const int64_t n_end = std::min<int64_t>(lq, a.n_stop);
+    int64_t m = 0;   // frames since n_first
+    double v = off;  // buffer_time of frame m
+    bool entered = false;
+    auto tz = [&](double x) { return 3.0e-8 * (1.0 + std::fabs(x)); };  // a little wider than almost::equal
+    while (n_first + m < n_end) {
+        // frames until the playhead can touch the tolerance zone of a loop point
+        double to_ls = v < ls2 - tz(ls2) ? (ls2 - tz(ls2) - v) / step : 0.;
+        double to_le = v < le2 - tz(le2) ? (le2 - tz(le2) - v) / step : 0.;
+        double skip = (!entered && to_ls > 0.) ? std::min(to_ls, to_le) : to_le;
+        int64_t adv = (int64_t)std::floor(skip);
+        if (adv > 0) {
+            v += (double)adv * step;
+            m += adv;
+            continue;
+        }
+        // exact per-frame logic of the reference
+        double w = v;
+        if (almost_equal(w, le2)) w = le2;
+        if (almost_equal(w, ls2)) w = ls2;
+        if (!entered && w >= ls2) entered = true;
+        if (entered) {
+            while (w >= le2) w -= len2;
+            while (w < ls2) w += len2;
+        }
+        if (w != v && n_first + m > seg_n.back()) {
+            seg_n.push_back(n_first + m);
+            seg_bt.push_back(w);
+        } else if (w != v) {
+            seg_bt.back() = w;
+        }
+        v = w + step;
+        m += 1;
+    }
+}
+
+// fast track: the buffer played 1:1 from a block boundary (a chain source when it fuses)
+bool Planner::absn_fast(NodeCtx& nc, const AbsnPlay& s, int64_t q, bool fused) {
+    Node& n = nc.n; PNode& p = nc.p;
+    AbsnInst a{};
+    if (!fused) a.out = p.out_buf[0];
+    a.buf = s.buf;
+    a.buf_len = (int64_t)s.len;
+    a.buf_stride = (int64_t)s.stride;
+    a.n_start = q * 128;
+    a.n_stop = std::numeric_limits<int64_t>::max();
+    a.buf_offset = 0;
+    a.ch = s.ch;
+    a.loop = n.loop ? 1 : 0;
+    if (!n.loop) {
+        // the quantum after which the source has `ended`: the reference accumulates buffer_time += block_duration and stops
+        // once it reaches the buffer's duration (audio_buffer_source.rs:609,826-838) — replayed, not divided
+        const double block_duration = clock.dt * 128.;
+        const int64_t max_q = (lq - a.n_start) / 128 + 2;
+        int64_t played = 0;
+        double bt = 0.;
+        while (played < max_q) {
+            bt += block_duration;
+            played++;
+            if (bt >= s.duration) break;
+        }
+        a.n_stop = a.n_start + played * 128;
+    }
+    if (fused) {
+        PendingChain pc = source_chain(CHAIN_SRC_ABSN, s.ch);
+        pc.inst.absn = a;
+        pc.lay = source_lay(a.n_start, a.n_stop, s.ch);
+        if (!finish_chain(nc, std::move(pc))) return false;
+    } else {
+        a.out = source_out(nc, a.n_start, a.n_stop, s.ch);
+        stage(nc.L, S_ABSN).absn.push_back(a);
+    }
+    // compulsory read of the source PCM that is actually played
+    algorithmic_bytes += (uint64_t)s.ch * 4ull * (uint64_t)std::max<int64_t>(0, std::min<int64_t>(lq - a.n_start, n.loop ? lq : (int64_t)s.len));
+    return true;
+}
+
+bool Planner::lower_biquad(NodeCtx& nc) {
+    Node& n = nc.n; PNode& p = nc.p; const Lay& in0 = nc.in0;
+    PRef pq = param_ref(n.params[0]), pdt = param_ref(n.params[1]), pfr = param_ref(n.params[2]), pg = param_ref(n.params[3]);
+    float q = pq.v, detune = pdt.v, freq = pfr.v, gain = pg.v;
+    int ch = p.in_ch[0];
+    if (nc.dyn_params) {  // per-frame coefficients (biquad_filter.rs:837-855): serial a-rate kernel
+        if (!need_out(nc, ch)) return false;
+        BiquadArInst ba{};
+        ba.in = p.in_buf[0];
+        ba.out = p.out_buf[0];
+        const BufRef none{nullptr, 0, 0};
+        ba.q = pq.dyn ? pq.track : none;
+        ba.detune = pdt.dyn ? pdt.track : none;
+        ba.freq = pfr.dyn ? pfr.track : none;
+        ba.gain = pg.dyn ? pg.track : none;
+        ba.q_val = q; ba.detune_val = detune; ba.freq_val = freq; ba.gain_val = gain;
+        ba.state = alloc<double>((size_t)ch * 4, true, true);
+        if (!ba.state) return bail(WAE_OUT_OF_MEMORY, "out of device memory (state)");
+        if (!filter_dyn_len(nc, ch, ba.dyn_len)) return false;
+        ba.out = p.out_buf[0];
+        {
+            // five planes of f64 coefficients per frame of the chunk (an arena buffer of 10 float channels read as doubles)
+            BufRef cb = arena_buf(10);
+            if (!cb.p) return no_arena();
+            cb.stride = (uint32_t)b->chunk;  // in DOUBLES: plane k starts at double index k * chunk
+            ba.coefs = cb;
+        }
+        ba.sample_rate = g->sample_rate;
+        ba.type = n.type;
+        ba.ch = ch;
+        StageBuild& sb = stage(nc.L, S_BIQUAD_AR);
+        sb.max_ch = std::max(sb.max_ch, ch);
+        sb.biquad_ar.push_back(ba);
+        return true;
+    }
+    float cf = hm::biquad_computed_freq(freq, detune);
+    hm::BiquadCoefs c = hm::biquad_coefs(n.type, (double)g->sample_rate, (double)cf, (double)gain, (double)q);
+    double* state = alloc<double>((size_t)ch * 4, true, true);
+    if (!state) return bail(WAE_OUT_OF_MEMORY, "out of device memory (state)");
+    // An input whose channel COUNT changes while it sounds resets / drops channels of the filter mid-render
+    // (biquad_filter.rs:798-815): the serial kernel follows it quantum by quantum; the scan keeps one state per channel
+    const bool count_varies = !nc.extend && in0.dyn() && !(in0.nlo == in0.nhi && in0.nhi == ch);
+    if (!eng->serial_filters && !count_varies) return append_biquad(nc, state, c);
+    // bit-faithful serial recurrence, one stage per biquad
+    if (!need_out(nc, ch)) return false;
+    BiquadInst bi{};
+    if (!filter_dyn_len(nc, ch, bi.dyn_len)) return false;
+    bi.in = p.in_buf[0];
+    bi.out = p.out_buf[0];
+    bi.b0 = c.b0; bi.b1 = c.b1; bi.b2 = c.b2; bi.a1 = c.a1; bi.a2 = c.a2;
+    bi.ch = ch;
+    bi.state = state;
+    StageBuild& s = stage(nc.L, S_BIQUAD);
+    s.max_ch = std::max(s.max_ch, ch);
+    s.biquad.push_back(bi);
+    return true;
+}
+
+bool Planner::lower_iir(NodeCtx& nc) {
+    Node& n = nc.n; PNode& p = nc.p; const Lay& in0 = nc.in0;
+    int ch = p.in_ch[0];
+    std::vector<double> ff = n.feedforward, fb = n.feedback;  // iir_filter.rs:282-309
+    if (ff.size() < fb.size()) ff.resize(fb.size(), 0.);
+    if (ff.size() > fb.size()) fb.resize(ff.size(), 0.);
+    if (ff.size() <= 3 && !eng->serial_filters && !in0.dyn() && seg_start == 0 && seg_end >= lq) {
+        // Order <= 2 with a constant input layout: the same transfer function as a biquad — rendered by the time-parallel scan
+        // of k_chain (direct form I there, transposed direct form II in iir_filter.rs:386-407: the outputs differ in the last
+        // bits of the f64 arithmetic only) instead of one serial thread per channel.  With an input that can fall silent the
+        // serial kernel stays: its tail test looks at the reference's own state variables.  Same for a render cut by suspend
+        // points: the two forms keep different state (x / y history here, the reference's 20 accumulators there) and a later
+        // segment may see a layout that needs the serial kernel — the filter memory must survive the cut (fuzz seeds 31, 33).
+        ff.resize(3, 0.);
+        fb.resize(3, 0.);
+        const double a0 = fb[0];
+        hm::BiquadCoefs c{ff[0] / a0, ff[1] / a0, ff[2] / a0, fb[1] / a0, fb[2] / a0};
+        double* state = alloc<double>((size_t)ch * 4, true, true);
+        if (!state) return bail(WAE_OUT_OF_MEMORY, "out of device memory (state)");
+        return append_biquad(nc, state, c);
+    }
+    if (!need_out(nc, ch)) return false;
+    IirInst ii{};
+    ii.in = p.in_buf[0];
+    ii.out = p.out_buf[0];
+    ii.n = (int)ff.size();
+    ii.ch = ch;
+    double a0 = fb[0];
+    for (size_t i = 0; i < ff.size(); i++) {
+        ii.b[i] = ff[i] / a0;
+        ii.a[i] = fb[i] / a0;
+    }
+    ii.state = alloc<double>((size_t)ch * 20, true, true);
+    if (!ii.state) return bail(WAE_OUT_OF_MEMORY, "out of device memory (state)");
+    if (!filter_dyn_len(nc, ch, ii.dyn_len)) return false;
+    ii.out = p.out_buf[0];
+    StageBuild& s = stage(nc.L, S_IIR);
+    s.max_ch = std::max(s.max_ch, ch);
+    s.iir.push_back(ii);
+    return true;
+}
+
+bool Planner::lower_gain(NodeCtx& nc) {
+    PNode& p = nc.p;
+    PRef pgn = param_ref(nc.n.params[0]);
+    float gv = pgn.v;
+    int ch = p.in_ch[0];
+    if (pgn.dyn) {  // a-rate gain (gain.rs:189-197)
+        if (!need_out(nc, ch)) return false;
+        out_like_input(nc);  // silent in -> silent out (gain.rs:155-158); the ~0 / ~1 shortcuts only exist for single values
+        stage(nc.L, S_GAIN).gain.push_back(GainInst{p.in_buf[0], p.out_buf[0], gv, ch, pgn.track});
+        return true;
+    }
+    // gain.rs:153-169: |g| <= 1e-6 -> silence, |1-g| <= 1e-6 -> pass-through (quanta >= 1; quantum 0 takes
+    // the multiply path, a difference of at most 1e-6 * |x| that is below the parity tolerance)
+    if (std::fabs(gv) <= 1e-6f) gv = 0.f;
+    else if (std::fabs(1.f - gv) <= 1e-6f) gv = 1.f;
+    if (nc.fuse_n) {
+        PendingChain pc = open_chain(nc);
+        // consecutive gains of one slot are folded (differs from two f32 multiplies by <= 1 ulp)
+        pc.inst.g[pc.phase == 0 ? 0 : (pc.phase == 1 ? 1 : (pc.phase == 3 ? 2 : 3))] *= gv;
+        if (gv == 0.f) pc.lay = Lay{1, 1, 1, 1, true};  // a gain of (about) zero answers with silence (gain.rs:160-163)
+        return finish_chain(nc, std::move(pc));
+    }
+    if (!need_out(nc, ch)) return false;
+    if (gv == 0.f) {
+        out_dynamic(nc, Lay{1, 1, 1, 1, true});
+        if (p.out_buf[0].meta) source_meta(nc, 0, 0, 1);
+    } else {
+        out_like_input(nc);
+    }
+    stage(nc.L, S_GAIN).gain.push_back(GainInst{p.in_buf[0], p.out_buf[0], gv, ch, BufRef{nullptr, 0, 0}});
+    return true;
+}
+
+bool Planner::lower_shaper(NodeCtx& nc) {
+    Node& n = nc.n; PNode& p = nc.p; const Lay& in0 = nc.in0;
+    int ch = p.in_ch[0];
+    const float* curve = n.has_curve ? upload(n.table) : nullptr;
+    // can_propagate_silence (waveshaper.rs:480-503): the curve maps 0 to 0
+    bool keeps_silence = true;
+    if (n.has_curve && !n.table.empty()) {
+        const size_t cn = n.table.size();
+        keeps_silence = cn % 2 == 1 ? std::fabs(n.table[cn / 2]) < 1e-9f : std::fabs((n.table[cn / 2 - 1] + n.table[cn / 2]) / 2.f) < 1e-9f;
+    }
+    // a silent input that still produces sound does so on the ONE channel a silent quantum has (waveshaper.rs:395-400)
+    auto shaper_lay = [keeps_silence](const Lay& l) {
+        if (keeps_silence || !l.may_silent) return l;
+        return Lay{1, l.hi, 1, l.nhi, false};
+    };
+    if (n.oversample && n.has_curve) {  // waveshaper.rs:409-480: up-sample, shape, down-sample
+        // input that can fall silent: a curve that maps 0 to 0 makes the node return early WITHOUT feeding its resamplers
+        // (frozen state: the kernel then works on the last processed quanta); a curve that does not keeps processing — on the
+        // one channel of a silent quantum, which rebuilds the resamplers of a wider node (waveshaper.rs:395-420)
+        const bool freeze = in0.dyn() && keeps_silence && in0.nlo == in0.nhi && in0.nhi == ch;
+        const bool as_static = !in0.dyn() || (!keeps_silence && ch == 1 && in0.hi == 1);
+        // every other dynamic input: the count of the processed quanta changes, and the resamplers are rebuilt with it
+        const bool rebuild = !freeze && !as_static;
+        if (!need_out(nc, ch)) return false;
+        if (freeze || (rebuild && keeps_silence)) {
+            out_like_input(nc);
+        } else if (rebuild) {  // silent quanta processed: a sounding output with the input's count (one channel when silent)
+            out_dynamic(nc, shaper_lay(in0));
+            if (p.out_buf[0].meta) meta_stage(nc.L, META_SHAPER, p.in_buf[0], ch, p.out_buf[0], ch);
+        }
+        const int factor = n.oversample == WAE_OVERSAMPLE_X2 ? 2 : 4;
+        auto& filt = os_filters[factor];
+        if (!filt.first) {
+            const std::vector<float2> fu = resampler_filter_bins(128, 128 * factor, 128);
+            const std::vector<float2> fd = resampler_filter_bins(128 * factor, 128, 128);
+            filt.first = upload(fu);
+            filt.second = upload(fd);
+            if (!dry) cudaStreamSynchronize(eng->stream);  // the host vectors go out of scope
+        }
+        ShaperOsInst so{};
+        so.in = p.in_buf[0];
+        so.out = p.out_buf[0];
+        so.curve = curve;
+        so.n = (int)n.table.size();
+        so.ch = ch;
+        so.factor = factor;
+        so.f_up = filt.first;
+        so.f_dn = filt.second;
+        so.hist = alloc<float>((size_t)256 * ch, true, true);
+        if (!so.hist || !so.f_up || !so.f_dn) return bail(WAE_OUT_OF_MEMORY, "out of device memory (over-sampled shaper)");
+        if (freeze) {
+            so.prev = alloc<int32_t>((size_t)(2 * (b->chunk / 128) + 2));
+            if (!so.prev) return bail(WAE_OUT_OF_MEMORY, "out of device memory (over-sampled shaper)");
+        }
+        if (rebuild) {  // (the two words in front carry the resamplers' state across chunks and segments)
+            so.rebuild = keeps_silence ? 2 : 1;
+            so.prev = alloc<int32_t>((size_t)(2 + 3 * (b->chunk / 128) + 2), true, true);
+            if (!so.prev) return bail(WAE_OUT_OF_MEMORY, "out of device memory (over-sampled shaper)");
+        }
+        StageBuild& os = stage(nc.L, S_SHAPER_OS);
+        os.max_ch = std::max(os.max_ch, ch);
+        os.shaper_os.push_back(so);
+        return true;
+    }
+    if (nc.fuse_n) {
+        PendingChain pc = open_chain(nc);
+        pc.inst.has_shaper = 1;
+        pc.inst.curve = curve;
+        pc.inst.shaper_n = (int)n.table.size();
+        pc.inst.shaper_keeps_silence = keeps_silence ? 1 : 0;
+        pc.lay = shaper_lay(pc.lay);
+        pc.phase = 5;
+        return finish_chain(nc, std::move(pc));
+    }
+    if (!need_out(nc, ch)) return false;
+    ShaperInst sh{};
+    if (in0.dyn() && !keeps_silence && n.has_curve) {
+        out_dynamic(nc, shaper_lay(in0));
+        if (p.out_buf[0].meta) meta_stage(nc.L, META_SHAPER, p.in_buf[0], ch, p.out_buf[0], ch);
+    } else {
+        out_like_input(nc);
+    }
+    sh.in = p.in_buf[0];
+    sh.out = p.out_buf[0];
+    sh.ch = ch;
+    sh.n = (int)n.table.size();
+    sh.curve = curve;
+    stage(nc.L, S_SHAPER).shaper.push_back(sh);
+    return true;
+}
+
+bool Planner::lower_stereo_panner(NodeCtx& nc) {
+    PNode& p = nc.p;
+    PRef ppan = param_ref(nc.n.params[0]);
+    float pan = ppan.v;
+    int ch = p.in_ch[0];
+    if (!need_out(nc, 2)) return false;
+    // silent in -> silent out, else two channels (stereo_panner.rs:230-235); the kernel picks the mono / stereo law per quantum
+    out_dynamic(nc, nc.in0.may_silent ? Lay{1, 2, 2, 2, true} : Lay::fixed(2));
+    if (p.out_buf[0].meta) meta_stage(nc.L, META_PAN, p.in_buf[0], ch, p.out_buf[0], 2);
+    float x = ch == 1 ? (pan + 1.f) * 0.5f : (pan <= 0.f ? pan + 1.f : pan);  // stereo_panner.rs:247-249,274-276
+    float gl, gr;
+    hm::stereo_gains(x, gl, gr);
+    StageBuild& s = stage(nc.L, S_SPAN);
+    s.span.push_back(SPanInst{p.in_buf[0], p.out_buf[0], pan, ch, ppan.dyn ? ppan.track : BufRef{nullptr, 0, 0}});
+    s.span_gains.push_back(make_float2(gl, gr));
+    return true;
+}
+
+bool Planner::lower_panner(NodeCtx& nc) {
+    Node& n = nc.n; PNode& p = nc.p; const Lay& in0 = nc.in0;
+    // the 15 spatial params (panner.rs:714-780): 6 of the node, 9 of the AudioListener (graph ids 2..10)
+    PRef pr[15];
+    bool moving = false;
+    for (int i = 0; i < 15; i++) {
+        pr[i] = param_ref(i < 6 ? n.params[i] : (uint32_t)(2 + i - 6));
+        moving = moving || pr[i].dyn;
+    }
+    int ch = p.in_ch[0];
+    // (a static HRTF panner with a constant-layout input is lowered to the convolver kernels, which take their own output buffer)
+    static const bool hrtf_fft_on = [] { const char* e = getenv("WAE_HRTF_FFT"); return !e || atoi(e) != 0; }();
+    const bool hrtf_as_conv = n.panning_model == WAE_PANNING_HRTF && hrtf_fft_on && eng->sphere && !moving && !in0.dyn() && cur_cls != 1 &&
+                              seg_start == 0 && seg_end >= lq && (ch == 1 || ch == 2);
+    if (!hrtf_as_conv && !need_out(nc, 2)) return false;
+    if (hrtf_as_conv) p.out_lay = {Lay::fixed(2)};
+    else out_dynamic(nc, in0.may_silent ? Lay{1, 2, 2, 2, true} : Lay::fixed(2));  // panner.rs:698-708
+    // (the HRTF panner keeps its own tail budget: its layout track is written by k_hrtf_map)
+    if (!hrtf_as_conv && p.out_buf[0].meta && n.panning_model != WAE_PANNING_HRTF) meta_stage(nc.L, META_PAN, p.in_buf[0], ch, p.out_buf[0], 2);
+    spatial::PanModel model{};
+    model.distance_model = n.distance_model;
+    model.ref_distance = n.ref_distance;
+    model.max_distance = n.max_distance;
+    model.rolloff_factor = n.rolloff_factor;
+    model.cone_inner_angle = n.cone_inner_angle;
+    model.cone_outer_angle = n.cone_outer_angle;
+    model.cone_outer_gain = n.cone_outer_gain;
+    SpatialTracks tr{};
+    float v[15];
+    for (int i = 0; i < 15; i++) {
+        v[i] = tr.value[i] = pr[i].v;
+        tr.track[i] = pr[i].dyn ? pr[i].track : BufRef{nullptr, 0, 0};
+    }
+    const spatial::SpatialParams sp0 = spatial::spatial_params(model, v);  // static source and listener
+    if (n.panning_model == WAE_PANNING_HRTF) {  // panner.rs:781-830
+        HrirAtRate hr;
+        if (!hrir_at_rate(hr)) return false;
+        if (hrtf_as_conv) return panner_hrtf_conv(nc, sp0, hr);
+        return panner_hrtf_fir(nc, sp0, hr, moving, tr, model);
+    }
+    if (moving) {
+        PanDynInst d{};
+        d.in = p.in_buf[0];
+        d.out = p.out_buf[0];
+        d.sp = tr;
+        d.model = model;
+        d.in_ch = ch;
+        stage(nc.L, S_PAN_DYN).pan_dyn.push_back(d);
+        return true;
+    }
+    PanInst pi{};
+    pi.in = p.in_buf[0];
+    pi.out = p.out_buf[0];
+    pi.in_ch = ch;
+    pi.azimuth = sp0.azimuth;
+    pi.dist_gain = sp0.dist_gain;
+    pi.cone_gain = sp0.cone_gain;
+    stage(nc.L, S_PAN).pan.push_back(pi);
+    return true;
+}
+
+// the HRIR sphere at the context's rate (panner.rs:46: at least 27 kHz)
+bool Planner::hrir_at_rate(HrirAtRate& hr) {
+    const HrirSphere* sph = eng->sphere;
+    if (!sph) return bail(WAE_UNSUPPORTED, "HRTF panning needs an HRIR sphere: call wae_engine_set_hrir_sphere first");
+    uint32_t sr = (uint32_t)g->sample_rate;
+    if (sr < 27000) sr = 27000;  // panner.rs:46
+    uint32_t taps = sph->taps;
+    const float* d_ir = eng->d_sphere_ir;
+    const float* h_ir = sph->ir.data();  // [vertex][2][taps] on the host
+    if (sr != sph->sample_rate) {  // the crate resamples the responses to the context rate once (wae_hrtf_host.h)
+        std::lock_guard<std::mutex> slk(eng->sphere_mu);
+        auto it = eng->sphere_rates.find(sr);
+        if (it == eng->sphere_rates.end()) {
+            const HrirSphere rs = sph->at_rate(sr);
+            wae_engine::RateSphere r;
+            r.taps = rs.taps;
+            if (r.taps < 2) return bail(WAE_UNSUPPORTED, "HRTF panning: the HRIR sphere is too short to be resampled to the context rate");
+            if (cudaMalloc(&r.d_ir, rs.ir.size() * sizeof(float)) != cudaSuccess) return bail(WAE_OUT_OF_MEMORY, "out of device memory (resampled HRIR sphere)");
+            cudaMemcpy(r.d_ir, rs.ir.data(), rs.ir.size() * sizeof(float), cudaMemcpyHostToDevice);
+            r.ir_host = rs.ir;
+            it = eng->sphere_rates.emplace(sr, r).first;
+        }
+        taps = it->second.taps;
+        d_ir = it->second.d_ir;
+        h_ir = it->second.ir_host.data();  // (map nodes are stable; entries are only dropped with the sphere)
+    }
+    hr = HrirAtRate{sr, taps, d_ir, h_ir};
+    return true;
+}
+
+// the three sphere vertices and their weights of a static source and listener, with the distance and cone gains
+HrtfSel Planner::static_hrtf_sel(const spatial::SpatialParams& sp0) const {
+    float proj[3];
+    spatial::projected_source(sp0, proj);
+    const float dir[3] = {proj[0], proj[2], proj[1]};  // HrtfState::process swaps y / z (panner.rs:248-252)
+    HrtfSel sel{{0, 0, 0}, {0.f, 0.f, 0.f}, sp0.cone_gain * sp0.dist_gain, 0.f};
+    eng->sphere->locate(dir, sel.v, sel.w);  // no face: all-zero weights (silence)
+    return sel;
+}
+
+// A static source heard by a static listener through a constant-layout input is ONE fixed pair of impulse responses:
+// out_ear = gain * (h_ear * mono(in)).  The crate evaluates that by FFT overlap-save per 128-frame block (hrtf 0.8.1
+// process_samples); here it is handed to the time-batched convolver kernels as a ConvolverNode-shaped problem —
+// response = the blended pair with the gain (and the reference's correction of 2 for a two-channel input,
+// panner.rs:805-812) folded in; a two-channel input is mixed down to mono by the forward transform's loads; one
+// partition, so the product is formed inside the inverse transform — instead of 2 x taps multiply-adds per output
+// frame in k_hrtf_fir.  WAE_HRTF_FFT=0: keep the FIR kernel.
+bool Planner::panner_hrtf_conv(NodeCtx& nc, const spatial::SpatialParams& sp0, const HrirAtRate& hr) {
+    const uint32_t taps = hr.taps;
+    const int ch = nc.p.in_ch[0];
+    const HrtfSel sel = static_hrtf_sel(sp0);
+    PcmBuffer resp;
+    if (!resp.allocate(2, taps, false)) return bail(WAE_OUT_OF_MEMORY, "out of host memory (hrtf response)");
+    const float corr = ch == 2 ? 2.f : 1.f;  // overall_gain_correction of a two-channel input (panner.rs:805-812)
+    const float* A = hr.h_ir + (size_t)sel.v[0] * 2 * taps;
+    const float* B = hr.h_ir + (size_t)sel.v[1] * 2 * taps;
+    const float* C = hr.h_ir + (size_t)sel.v[2] * 2 * taps;
+    for (uint32_t k = 0; k < taps; k++) {  // (the blend k_hrtf_fir does, same f32 operations)
+        const float l = (A[k] * sel.w[0] + B[k] * sel.w[1]) + C[k] * sel.w[2];
+        const float r = (A[taps + k] * sel.w[0] + B[taps + k] * sel.w[1]) + C[taps + k] * sel.w[2];
+        resp.channels[0].p[k] = corr * (l * sel.gain);
+        resp.channels[1].p[k] = corr * (r * sel.gain);
+    }
+    resp.sample_rate = (float)hr.sr;
+    return plan_convolver(nc.p, nc.L, nullptr, -1, &resp);
+}
+
+bool Planner::panner_hrtf_fir(NodeCtx& nc, const spatial::SpatialParams& sp0, const HrirAtRate& hr, bool moving, const SpatialTracks& tr,
+                              const spatial::PanModel& model) {
+    PNode& p = nc.p;
+    const HrirSphere* sph = eng->sphere;
+    const int ch = p.in_ch[0];
+    HrtfInst h{};
+    h.in = p.in_buf[0];
+    h.out = p.out_buf[0];
+    h.in_ch = ch;
+    h.L = (int)hr.taps;
+    h.sphere_ir = hr.d_ir;
+    h.sel = nullptr;
+    h.correction = ch == 2 ? 2.f : 1.f;
+    h.hist = alloc<float>(hr.taps, true, true);
+    if (!h.hist) return bail(WAE_OUT_OF_MEMORY, "out of device memory (hrtf history)");
+    if (nc.in0.dyn()) {  // the node stops processing (and freezes) once its tail budget is used up: panner.rs:697-711
+        h.dyn = 1;
+        h.cmap = alloc<int32_t>((size_t)(b->chunk / 128 + 2));
+        h.tail = alloc<int64_t>(1, true, true);
+        if (!h.cmap || !h.tail) return bail(WAE_OUT_OF_MEMORY, "out of device memory (hrtf layout)");
+    }
+    StageBuild& hs = stage(nc.L, S_HRTF);
+    if (moving) {
+        HrtfSelInst si{};
+        si.sp = tr;
+        si.model = model;
+        si.pos = eng->d_sphere_pos;
+        si.tri = eng->d_sphere_tri;
+        si.n_faces = (int)(sph->tri.size() / 3);
+        si.sel = alloc<HrtfSel>((size_t)(b->chunk / 128 + 1));
+        if (!si.sel) return bail(WAE_OUT_OF_MEMORY, "out of device memory (hrtf selection)");
+        h.sel = si.sel;
+        hs.hrtf_sel.push_back(si);
+    } else {
+        h.static_sel = static_hrtf_sel(sp0);
+    }
+    hs.hrtf.push_back(h);
+    return true;
+}
+
+bool Planner::lower_delay_writer(NodeCtx& nc) {
+    PNode& p = nc.p;
+    p.out_ch = {p.in_ch[0]};
+    p.out_buf = {p.in_buf[0]};
+    p.out_lay = {nc.in0};
+    if (!Orderer::contains(ord.broken, nc.id)) return true;
+    // cycle breaker applied (graph.rs:458-466): the hidden writer->reader edge is gone, the reader ran
+    // earlier in this quantum from the ring; record this quantum's input now
+    delay_ch_seen[{gi, nc.n.delay_peer}] = p.in_ch[0];
+    auto it = delay_rings.find({gi, nc.id});
+    if (it == delay_rings.end()) return bail(WAE_UNSUPPORTED, "DelayNode writer processed before its reader inside a cycle");
+    if (it->second.ch != p.in_ch[0]) {
+        if (!dry) return bail(WAE_UNSUPPORTED, "channel layout of a DelayNode in a feedback cycle did not converge");
+        return true;  // sizing pass: the hint is corrected and the pass repeated
+    }
+    DelayInst d{};
+    d.in = p.in_buf[0];
+    d.ch = it->second.ch;
+    d.ring = it->second.ring;
+    d.ring_len = it->second.ring_len;
+    d.mono_at = it->second.mono_at;
+    d.mono_len = it->second.mono_len;
+    d.dyn = it->second.mono_at ? 3 : 0;  // inside a cycle the writer runs after the reader: it extends the one-channel track
+    stage(nc.L, S_DELAY_WRITE).delay.push_back(d);
+    return true;
+}
+
+bool Planner::lower_delay_reader(NodeCtx& nc) {
+    Node& n = nc.n; PNode& p = nc.p;
+    const double sr = (double)g->sample_rate;
+    PRef pdl = param_ref(n.params[0]);
+    float dt = pdl.v;
+    const bool in_cycle = Orderer::contains(ord.broken, n.delay_peer);
+    int ch = p.in_ch[0];
+    if (in_cycle) {
+        ch = 1;
+        if (delay_ch_hint) {
+            auto it = delay_ch_hint->find({gi, nc.id});
+            if (it != delay_ch_hint->end()) ch = it->second;
+        }
+    }
+    if (!need_out(nc, ch)) return false;
+    DelayInst d{};
+    d.in = p.in_buf[0];
+    d.out = p.out_buf[0];
+    d.ch = ch;
+    d.in_cycle = in_cycle ? 1 : 0;
+    if (pdl.dyn) d.delay_track = pdl.track;
+    d.sample_rate = g->sample_rate;
+    double delay = (double)dt;
+    if (in_cycle) delay = std::max(delay, 128. / sr);  // delay.rs:699-703: at least one quantum inside a cycle
+    double num_samples = delay * sr;               // delay.rs:706
+    double position = 0. - num_samples;            // sample_index 0
+    double pf = std::floor(position);
+    d.fl = (int64_t)pf;
+    d.k = (float)(position - pf);
+    uint64_t max_frames = (uint64_t)std::ceil(std::max(n.max_delay_time, 128. / sr) * sr) + 2;
+    d.ring_len = next_pow2(max_frames + 128);
+    d.ring = alloc<float>((size_t)ch * d.ring_len, true, true);
+    if (!d.ring) return bail(WAE_OUT_OF_MEMORY, "out of device memory (delay ring)");
+    b->arena_bytes += (size_t)ch * d.ring_len * 4;
+    if (ch <= 2) {
+        // The reader reports a quantum without any normal sample as silent (delay.rs:654-664) and the ring follows the
+        // channel count of the writer's input (:470-488): its output layout is never constant.  (Wider than stereo: the
+        // static layout is kept, the re-mix of the ring is not followed.)
+        d.dyn = 1;
+        d.mono_len = (int32_t)next_pow2((uint64_t)(b->chunk / 128 + 2));
+        d.mono_at = alloc<int64_t>((size_t)d.mono_len, true, true);
+        if (!d.mono_at) return bail(WAE_OUT_OF_MEMORY, "out of device memory (delay layout track)");
+        const Lay wl = in_cycle ? Lay{1, (uint8_t)ch, 1, (uint8_t)ch, true} : nc.in0;
+        out_dynamic(nc, Lay{1, (uint8_t)ch, (uint8_t)(wl.dyn() ? 1 : ch), (uint8_t)ch, true});
+        d.out = p.out_buf[0];
+        if (!in_cycle) stage(nc.L, S_DELAY_MONO).delay.push_back(d);
+    }
+    stage(nc.L, S_DELAY).delay.push_back(d);
+    if (in_cycle) delay_rings[{gi, n.delay_peer}] = DelayRing{d.ring, d.ring_len, ch, d.mono_at, d.mono_len};
+    else stage(nc.L, S_DELAY_WRITE).delay.push_back(d);  // acyclic: history is recorded right after the read
+    return true;
+}
+
+bool Planner::lower_compressor(NodeCtx& nc) {
+    PNode& p = nc.p; const Lay& in0 = nc.in0;
+    PRef cp[5];
+    for (int i = 0; i < 5; i++) cp[i] = param_ref(nc.n.params[i]);
+    const float at = cp[0].v, kn = cp[1].v, ra = cp[2].v, re = cp[3].v, th = cp[4].v;
+    int ch = p.in_ch[0];
+    if (!need_out(nc, ch)) return false;
+    CompInst c{};
+    c.in = p.in_buf[0];
+    c.out = p.out_buf[0];
+    c.ch = ch;
+    int ring_size = (int)std::ceil(g->sample_rate * 0.006f / 128.f) + 1;  // dynamics_compressor.rs:250-255
+    c.delay_frames = (ring_size - 1) * 128;
+    c.ring_len = next_pow2((uint64_t)c.delay_frames + 128);
+    c.ring = alloc<float>((size_t)ch * c.ring_len, true, true);
+    c.state = alloc<float>(2, true, true);
+    c.meta_ring = alloc<uint8_t>(8, true, true);
+    if (!c.ring || !c.state || !c.meta_ring) return bail(WAE_OUT_OF_MEMORY, "out of device memory (compressor)");
+    // the look-ahead ring starts out silent and hands on the layout of the quantum it delays (dynamics_compressor.rs:340-349,452-468)
+    out_dynamic(nc, Lay{1, in0.hi, in0.nlo, in0.nhi, true});
+    c.out = p.out_buf[0];
+    c.threshold = th; c.knee = kn; c.ratio = ra; c.attack = at; c.release = re;
+    for (int i = 0; i < 5; i++) c.track[i] = cp[i].dyn ? cp[i].track : BufRef{nullptr, 0, 0};
+    c.sample_rate = g->sample_rate;
+    c.end = glq;
+    stage(nc.L, S_COMP).comp.push_back(c);
+    if (!dry) {
+        std::lock_guard<std::recursive_mutex> lk(b->mu);  // (groups are planned on worker threads)
+        bool known = false;
+        for (auto& r : b->compressors) known = known || (r.graph == gi && r.node == nc.id);
+        if (!known) b->compressors.push_back(wae_batch::CompRec{gi, nc.id, c.state});
+    }
+    return true;
+}
+
+bool Planner::lower_analyser(NodeCtx& nc) {
+    Node& n = nc.n; PNode& p = nc.p;
+    int ch = p.in_ch[0];
+    // pass-through (analyser.rs:267-294): the output IS the input buffer (nobody writes an edge buffer after its
+    // producer), only the ring is written
+    p.out_ch = {ch};
+    p.out_buf = {p.in_buf[0]};
+    p.out_lay = {nc.in0};
+    AnalyserInst a{};
+    a.in = p.in_buf[0];
+    a.out = BufRef{nullptr, 0, 0};
+    a.ch = ch;
+    a.end = glq;
+    a.ring = alloc<float>(32768 + 128, true, true);
+    if (!a.ring) return bail(WAE_OUT_OF_MEMORY, "out of device memory (analyser ring)");
+    stage(nc.L, S_ANALYSER).analyser.push_back(a);
+    {
+        float* last = alloc<float>(16384, true, true);
+        float* db = alloc<float>(16384);
+        if (!last || !db) return bail(WAE_OUT_OF_MEMORY, "out of device memory (analyser)");
+        if (!dry) {
+            std::lock_guard<std::recursive_mutex> lk(b->mu);
+            bool known = false;
+            for (auto& r : b->analysers) known = known || (r.graph_index == gi && r.node == nc.id);
+            if (!known) b->analysers.push_back(AnalyserRec{gi, nc.id, a.ring, n.fft_size, n.smoothing, last, db, false, n.min_db, n.max_db, glq});
+        }
+    }
+    algorithmic_bytes += (uint64_t)lq * 4;  // ring write, SURVEY §8(d)
+    return true;
+}
+
+bool Planner::lower_merger(NodeCtx& nc) {
+    PNode& p = nc.p;
+    int k = nc.n.n_inputs;
+    if (!need_out(nc, k)) return false;
+    {
+        // `k` channels as soon as one input is not silent, else silent (channel_merger.rs:160-168)
+        bool some_always_on = false, any_dyn = false;
+        for (int i = 0; i < k; i++) {
+            some_always_on = some_always_on || !p.in_lay[i].may_silent;
+            any_dyn = any_dyn || p.in_lay[i].dyn();
+        }
+        if (any_dyn && !some_always_on) {
+            out_dynamic(nc, Lay{1, (uint8_t)k, (uint8_t)k, (uint8_t)k, true});
+            if (p.out_buf[0].meta) {
+                MetaInst m{};
+                m.out = p.out_buf[0];
+                m.mode = META_MERGE;
+                m.out_ch = k;
+                m.count = k;
+                m.n_more = k;
+                m.more = upload(p.in_buf);
+                if (!m.more) return bail(WAE_OUT_OF_MEMORY, "out of device memory (merger inputs)");
+                stage(nc.L, S_META).meta.push_back(m);
+            }
+        }
+    }
+    for (int i = 0; i < k; i++) stage(nc.L, S_ROUTE).route.push_back(RouteInst{p.in_buf[i], p.out_buf[0], 0, i, 0, 1});
+    return true;
+}
+
+bool Planner::lower_splitter(NodeCtx& nc) {
+    PNode& p = nc.p;
+    int k = nc.n.n_outputs;
+    p.out_ch.assign(k, 1);
+    p.out_buf.resize(k);
+    p.out_lay.assign(k, Lay::fixed(1));
+    for (int i = 0; i < k; i++) {
+        if (i < p.in_ch[0] && nc.in0.dyn()) {  // channel i exists only in some quanta: copy it, zeros elsewhere, own layout track
+            p.out_buf[i] = arena_buf(1, true);
+            if (!p.out_buf[i].p) return no_arena();
+            p.out_lay[i] = Lay{1, 1, 1, 1, true};
+            stage(nc.L, S_ROUTE).route.push_back(RouteInst{p.in_buf[0], p.out_buf[i], i, 0, 0, p.in_ch[0]});
+            meta_stage(nc.L, META_SPLIT, p.in_buf[0], p.in_ch[0], p.out_buf[i], 1, 0, i);
+        } else if (i < p.in_ch[0]) {  // alias channel i of the input
+            BufRef r = p.in_buf[0];
+            r.p += (size_t)i * r.stride;
+            p.out_buf[i] = r;
+        } else {
+            p.out_buf[i] = arena_buf(1);
+            stage(nc.L, S_ROUTE).route.push_back(RouteInst{p.in_buf[0], p.out_buf[i], 0, 0, 1, 0});
+        }
+    }
+    return true;
+}
+
+bool Planner::lower_convolver(NodeCtx& nc) {
+    Node& n = nc.n;
+    // the destination's only input (and this node's only consumer): the inverse transforms write the rendered PCM
+    const BufRef* dest = nullptr;
+    const BufRef fin = dest_ref();
+    if (eng->fuse && cur_cls == 0 && g->length <= 0xffffffffull) {
+        int n_out = 0;
+        uint32_t to = 0;
+        int to_port = -1;
+        for (auto& e : ord.edges.at(nc.id))
+            if (e.other_index >= 0) n_out++, to = e.other_id, to_port = e.other_index;
+        if (n_out == 1 && to_port == 0 && g->nodes.at(to).kind == K_DEST && node_table.at(to).in_edges[0].size() == 1 &&
+            computed_channels(g->nodes.at(to).cfg, (n.buffer && n.buffer->channels.size() == 1 && nc.p.in_ch[0] == 1) ? 1 : 2) == (int)g->channels)
+            dest = &fin;
+    }
+    return plan_convolver(nc.p, nc.L, dest, (int64_t)g->length);
+}
+
+bool Planner::plan_graph(wae_graph* graph, uint32_t graph_index) {
+    g = graph;
+    gi = graph_index;
     glq = (int64_t)((g->length + 127) / 128 * 128);
-    Orderer ord{g};
+    dry_gi = gi;
+    dry_seq = 0;
+    ord = Orderer{g};
     ord.run();
     if (!ord.broken.empty()) has_feedback = true;  // feedback through a DelayNode: its levels are replayed quantum by quantum
     // nodes from which a broken DelayWriter is reachable (reverse reachability over the ordered graph's edges, AudioParam ->
@@ -1370,12 +2934,10 @@ bool Planner::plan_graph(wae_graph* g, uint32_t gi) {
         return fed_by_cycle.count(id) ? 1 : 0;
     };
     NodeTable& pn = node_table;
-    cur_pn = &pn;
     pn.reset(g->nodes.empty() ? 0 : g->nodes.max_id());
     for (auto& kv : g->nodes) pn.put(kv.first, &kv.second);
     // Graph::render (graph.rs:500-535): walk the order, append each audio edge to its destination port
     for (uint32_t id : ord.ordered) {
-        Node& n = g->nodes.at(id);
         for (auto& e : ord.edges.at(id)) {
             if (e.other_index < 0) continue;
             PNode* it = pn.find(e.other_id);
@@ -1383,70 +2945,9 @@ bool Planner::plan_graph(wae_graph* g, uint32_t gi) {
             it->in_edges[e.other_index].push_back(PortRef{id, e.self_index});
         }
     }
-    hm::SchedClock clock(g->sample_rate);
-    const double sr = (double)g->sample_rate;
-    // ---- chain fusion (WAE_OPT_FUSE): sources and biquad/gain/shaper nodes are not emitted one stage each; a node
-    // with exactly one consumer stays PENDING, the consumer either extends the chain (same channel count, single
-    // edge) or forces it to be materialised into an arena buffer.  A chain that ends at a destination whose only
-    // input it is writes the final PCM directly.
-    const bool fuse = eng->fuse;
-    const bool want_scan_coefs = !dry || plan_digest_wanted();  // (the sizing pass needs their number only)
-    std::map<uint32_t, PendingChain> pending;
-    auto consumers = [&](const Node& nd) {
-        int k = 0;
-        for (auto& e : ord.edges.at(nd.id))
-            if (e.other_index >= 0) k++;
-        return k;
-    };
-    auto emit_chain = [&](PendingChain& pc, int L) {
-        const int variant = pc.inst.src_kind * 6 + pc.inst.n_biquad * 2 + (pc.inst.has_shaper ? 1 : 0);
-        const int consumer_cls = cur_cls;  // a chain is emitted while its consumer is planned, but runs with its own nodes' class
-        cur_cls = pc.cls;
-        StageBuild& cs = stage(L, S_CHAIN, variant);
-        cur_cls = consumer_cls;
-        for (int k = 0; k < pc.inst.n_biquad; k++) {
-            pc.inst.bq[k].coef = cs.add_scan_coef(want_scan_coefs, [&] { return make_scan_coef(pc.coefs[k]); });
-        }
-        cs.max_ch = std::max(cs.max_ch, pc.ch);
-        cs.chain.push_back(pc.inst);
-    };
-    // may_alias: the consumer reads its input through chan() with any alignment (the convolver's forward transform): a pending chain that
-    // is nothing but an AudioBufferSourceNode playing its buffer 1:1 from frame 0, the buffer covering the whole (quantum-padded) render,
-    // IS that buffer — no copy into the arena
-    auto materialize = [&](uint32_t nid, bool may_alias = false) -> bool {
-        auto it = pending.find(nid);
-        if (it == pending.end()) return true;
-        PNode& sp = pn.at(nid);
-        {
-            const ChainInst& ci = it->second.inst;
-            const AbsnInst& a = ci.absn;
-            bool unit = true;
-            for (int i = 0; i < 4; i++) unit = unit && ci.g[i] == 1.f;
-            if (may_alias && ci.src_kind == CHAIN_SRC_ABSN && ci.n_biquad == 0 && !ci.has_shaper && unit && it->second.phase == 0 &&
-                !it->second.lay.dyn() && a.n_start == 0 && !a.loop && a.buf_offset == 0 && a.buf_len >= lq && a.buf_stride <= 0xffffffffll &&
-                seg_start == 0 && seg_end >= lq) {
-                sp.out_buf = {BufRef{const_cast<float*>(a.buf), (uint32_t)a.buf_stride, 1}};
-                pending.erase(it);
-                return true;
-            }
-        }
-        BufRef buf = arena_buf(it->second.ch, it->second.lay.dyn());  // (k_chain writes the layout track itself)
-        if (!buf.p) return bail(WAE_OUT_OF_MEMORY, "out of device memory (arena)");
-        it->second.inst.out = buf;
-        it->second.inst.limit = -1;
-        it->second.inst.out_dup = 0;
-        emit_chain(it->second, 2 * sp.level + 1);
-        sp.out_buf = {buf};
-        pending.erase(it);
-        return true;
-    };
-    // can a node of this kind still be appended to the canonical chain gain, A, gain, B, gain, shaper, gain?
-    auto chain_accepts = [&](const PendingChain& pc, Kind kind) {
-        if (kind == K_GAIN) return true;
-        if (kind == K_BIQUAD) return pc.phase <= 1;
-        if (kind == K_SHAPER) return pc.phase < 5;
-        return false;
-    };
+    clock = hm::SchedClock(g->sample_rate);
+    want_scan_coefs = !dry || plan_digest_wanted();
+    pending.clear();
     for (uint32_t id : ord.ordered) {
         Node& n = g->nodes.at(id);
         if (n.kind == K_LISTENER) continue;
@@ -1457,1355 +2958,33 @@ bool Planner::plan_graph(wae_graph* g, uint32_t gi) {
         key_seq = 0;
         key_salt = n.kind == K_PARAM ? (uint64_t)n.param.events.size() : 0;  // a param whose event list grew restarts its timeline
         if (n.kind == K_PARAM) {
-            // AudioParamProcessor (param.rs:685-797): only params with automation events or audio-rate inputs become
-            // GPU work; a constant param is a scalar in its owner's instance
-            auto& edges = p.in_edges[0];
-            // (a render without suspend points never replays a timeline: a constant param needs no record at all — most params are)
-            if (seg_start == 0 && seg_end >= lq && edges.empty() && n.param.constant()) continue;
-            const ParamTimeline* tlp = param_timeline(gi, id, n.param, g->sample_rate);
-            if (n.param.constant() && edges.empty()) continue;
-            int level = 0;
-            for (auto& r : edges) level = std::max(level, pn.at(r.node).level + 1);
-            p.level = level;
-            for (auto& r : edges)
-                if (!materialize(r.node)) return false;
-            const ParamTimeline& tl = *tlp;
-            if (!tl.error.empty()) return bail(WAE_NOT_SUPPORTED, tl.error);
-            ParamInst pi{};
-            if (!edges.empty()) {  // sum of the connected signals, first channel each (1 / explicit / discrete, param.rs:296-310)
-                bool any_dyn = false;
-                for (auto& r : edges) any_dyn = any_dyn || pn.at(r.node).lay_out(r.port).dyn();
-                if (any_dyn) {  // edges whose layout changes: folded per quantum; a silent sum reads as zeros, which is what the param adds then
-                    StageBuild& ms = stage(2 * level, S_MIX_DYN);
-                    MixDynInst m{};
-                    m.out = arena_buf(1);
-                    if (!m.out.p) return bail(WAE_OUT_OF_MEMORY, "out of device memory (arena)");
-                    m.out_ch = 1;
-                    m.interp = WAE_INTERPRETATION_DISCRETE;
-                    m.mode = WAE_COUNT_MODE_EXPLICIT;
-                    m.cfg_count = 1;
-                    m.n_edges = (int)edges.size();
-                    m.edge_offset = (uint32_t)ms.mix_edges.size();
-                    m.limit = -1;
-                    for (auto& r : edges) ms.mix_edges.push_back(MixEdge{pn.at(r.node).out_buf[r.port], pn.at(r.node).out_ch[r.port], 0});
-                    ms.mix_dyn.push_back(m);
-                    pi.in = m.out;
-                } else {
-                    StageBuild& ms = stage(2 * level, S_MIX);
-                    MixInst m{};
-                    m.out = arena_buf(1);
-                    if (!m.out.p) return bail(WAE_OUT_OF_MEMORY, "out of device memory (arena)");
-                    m.out_ch = 1;
-                    m.interp = WAE_INTERPRETATION_DISCRETE;
-                    m.n_edges = (int)edges.size();
-                    m.edge_offset = (uint32_t)ms.mix_edges.size();
-                    m.limit = -1;
-                    for (auto& r : edges) ms.mix_edges.push_back(MixEdge{pn.at(r.node).out_buf[r.port], pn.at(r.node).out_ch[r.port], 0});
-                    ms.mix.push_back(m);
-                    pi.in = m.out;
-                }
-            }
-            pi.events = tl.events.empty() ? nullptr : upload(tl.events);
-            pi.curves = tl.curves.empty() ? nullptr : upload(tl.curves);
-            pi.state = alloc<ParamState>(1, true, true);
-            pi.out = arena_buf(2);  // channel 0: value per frame, channel 1: single-valued flag per quantum
-            if (!pi.state || !pi.out.p) return bail(WAE_OUT_OF_MEMORY, "out of device memory (param)");
-            pi.def = n.param.default_value;
-            pi.mn = n.param.min_value;
-            pi.mx = n.param.max_value;
-            pi.intrinsic0 = tl.intrinsic;
-            pi.has_last0 = tl.has_last ? 1 : 0;
-            pi.last0 = tl.last;
-            pi.sample_rate = g->sample_rate;
-            pi.n_events = (int32_t)tl.events.size();
-            pi.a_rate = n.param.a_rate ? 1 : 0;
-            stage(2 * level + 1, S_PARAM).param.push_back(pi);
-            p.out_ch = {1};
-            p.out_buf = {pi.out};
+            if (!lower_param(id, n, p)) return false;
             continue;
         }
-        // ---- inputs: static channel count + mix stage where needed
-        int level = 0;
-        for (auto& port : p.in_edges)
-            for (auto& r : port) level = std::max(level, pn.at(r.node).level + 1);
-        bool dyn_params = false;
-        for (uint32_t pid : n.params) {
-            PNode& pp = pn.at(pid);
-            if (!pp.out_buf.empty()) {
-                dyn_params = true;
-                level = std::max(level, pp.level + 1);
-            }
-        }
-        if (n.kind == K_PANNER)
-            for (uint32_t pid = 2; pid <= 10; pid++)
-                if (pn.count(pid) && !pn.at(pid).out_buf.empty()) level = std::max(level, pn.at(pid).level + 1);
-        p.level = level;
-        const bool fuse_n = fuse && !dyn_params;  // nodes with automated params run their own a-rate kernels
-        // does this node extend the pending chain of its only producer / take it as the destination's only input?
-        uint32_t fuse_src = 0;
-        bool extend = false, dest_direct = false;
-        const bool chain_kind = !dyn_params && ((n.kind == K_BIQUAD && !eng->serial_filters) || (fuse && (n.kind == K_GAIN || (n.kind == K_SHAPER && !(n.oversample && n.has_curve)))));
-        if (fuse && n.n_inputs == 1 && p.in_edges[0].size() == 1 && p.in_edges[0][0].port == 0) {
-            auto it = pending.find(p.in_edges[0][0].node);
-            if (it != pending.end()) {
-                int sch = pn.at(it->first).out_ch[0];
-                if (chain_kind && computed_channels(n.cfg, sch) == sch && chain_accepts(it->second, n.kind)) {
-                    extend = true;
-                    fuse_src = it->first;
-                } else if (n.kind == K_DEST && g->length <= 0xffffffffull &&
-                           (sch == (int)g->channels || (sch == 1 && g->channels == 2 && n.cfg.interp == WAE_INTERPRETATION_SPEAKERS))) {
-                    dest_direct = true;
-                    fuse_src = it->first;
-                }
-            }
-        }
-        // ---- k_voice_sum (WAE_OPT_VOICE_SUM): a port fed by many oscillator -> [biquad] -> gain voices, all of them still pending chains
-        // (mono, constant layout, one consumer): the voices are not materialised, one kernel renders them and keeps the running sum in
-        // registers, in the port's edge order.  Only when the launch has enough (2048-frame tile, port) work items to fill the machine
-        // about twice: one graph with thousands of voices and a short render (configs[2]) is better served by k_chain + k_mix, which
-        // take their parallelism from the voices.
-        std::vector<char> port_vsum(p.in_edges.size(), 0);
-        std::vector<int> port_vsum_nb(p.in_edges.size(), 0);
-        if (fuse && voice_sum_mode() != 0 && !extend && !dest_direct && cur_cls == 0 && n.kind != K_DELAY_R) {
-            for (size_t pi = 0; pi < p.in_edges.size() && (int)pi < n.n_inputs; pi++) {
-                const auto& edges = p.in_edges[pi];
-                if ((int)edges.size() < 8) continue;
-                const int ch = computed_channels(n.cfg, 1);
-                if (!(ch == 1 || (ch == 2 && n.cfg.interp == WAE_INTERPRETATION_SPEAKERS))) continue;
-                if (n.kind == K_DEST && g->length > 0xffffffffull) continue;
-                const int64_t tiles = (seg_end - seg_start + 2047) / 2048;
-                if (voice_sum_mode() < 2 && tiles * (int64_t)group_graphs < 2 * (int64_t)voice_sum_slots()) continue;
-                int nb = -1;
-                bool ok = true;
-                std::set<uint32_t> seen_nodes;
-                for (auto& r : edges) {
-                    auto it = pending.find(r.node);
-                    if (r.port != 0 || it == pending.end()) { ok = false; break; }
-                    const PendingChain& pc = it->second;
-                    if (pc.inst.src_kind != CHAIN_SRC_OSC || pc.ch != 1 || pc.inst.has_shaper || pc.inst.n_biquad > 1 || pc.lay.dyn() || pc.cls != cur_cls ||
-                        (nb >= 0 && nb != pc.inst.n_biquad) || !seen_nodes.insert(r.node).second) { ok = false; break; }
-                    nb = pc.inst.n_biquad;
-                }
-                if (!ok) continue;
-                port_vsum[pi] = 1;
-                port_vsum_nb[pi] = nb;
-            }
-        }
-        for (size_t pi = 0; pi < p.in_edges.size(); pi++) {
-            if (port_vsum[pi]) continue;
-            auto& port = p.in_edges[pi];
-            for (auto& r : port)
-                if (!((extend || dest_direct) && r.node == fuse_src))
-                    if (!materialize(r.node, n.kind == K_CONV && n.buffer && port.size() == 1)) return false;
-        }
-        p.in_ch.assign(n.n_inputs, 1);
-        p.in_buf.assign(n.n_inputs, BufRef{nullptr, 0, 0});
-        p.in_lay.assign(n.n_inputs, Lay::fixed(1));
-        for (int port = 0; port < n.n_inputs; port++) {
-            auto& edges = p.in_edges[port];
-            int max_in = 1;
-            for (auto& r : edges) max_in = std::max(max_in, pn.at(r.node).out_ch[r.port]);
-            int ch = computed_channels(n.cfg, max_in);
-            if (n.kind == K_DELAY_R) {  // the reader's only input is the hidden writer edge: take the writer's layout
-                ch = max_in;
-            }
-            p.in_ch[port] = ch;
-            p.in_lay[port] = Lay::fixed(ch);
-            bool is_dest = n.kind == K_DEST;
-            if (extend || dest_direct) {  // the producer's chain is consumed in registers / written directly
-                if (extend) p.in_lay[port] = pending.at(fuse_src).lay;
-                continue;
-            }
-            if (port_vsum[port]) {  // the voices of this port and their sum in one kernel
-                StageBuild& vs = stage(2 * level, S_VSUM, port_vsum_nb[port]);
-                VoiceGroup vg{};
-                vg.first = (int32_t)vs.chain.size();
-                vg.n_voices = (int32_t)edges.size();
-                vg.out_dup = ch;
-                vg.limit = -1;
-                if (is_dest) {
-                    vg.out = dest_ref(g, gi);
-                    vg.limit = (int64_t)g->length;
-                } else {
-                    vg.out = arena_buf(ch);
-                    if (!vg.out.p) return bail(WAE_OUT_OF_MEMORY, "out of device memory (arena)");
-                }
-                for (auto& r : edges) {
-                    PendingChain pc = std::move(pending.at(r.node));
-                    pending.erase(r.node);
-                    // (k_voice_sum prefetches the constants of voice k as coefficient set k: one set per voice, in voice order)
-                    if (pc.inst.n_biquad == 1 && vs.n_scan_coef != vs.chain.size()) return bail(WAE_UNSUPPORTED, "internal: voice-sum coefficient table out of step");
-                    for (int k = 0; k < pc.inst.n_biquad; k++)
-                        pc.inst.bq[k].coef = vs.add_scan_coef(want_scan_coefs, [&] { return make_scan_coef(pc.coefs[k]); });
-                    pc.inst.limit = -1;
-                    pc.inst.out_dup = 0;
-                    vs.chain.push_back(pc.inst);
-                }
-                vs.vgroups.push_back(vg);
-                p.in_buf[port] = vg.out;
-                continue;
-            }
-            if (is_dest && edges.size() == 1 && pn.at(edges[0].node).wrote_dest) {  // the producer already wrote the rendered PCM
-                p.in_buf[port] = pn.at(edges[0].node).out_buf[edges[0].port];
-                continue;
-            }
-            // ---- the port's layout over time: AudioRenderQuantum::add folded over the edges (quantum.rs:532-569)
-            bool any_dyn = false;
-            Lay pl = Lay::fixed(ch);
-            if (!edges.empty()) {
-                int lo = 1, hi = 1, on_nlo = 0, min_nlo = 255;
-                bool all_may_silent = true;
-                for (auto& r : edges) {
-                    const Lay el = pn.at(r.node).lay_out(r.port);
-                    any_dyn = any_dyn || el.dyn();
-                    lo = std::max<int>(lo, el.lo);
-                    hi = std::max<int>(hi, el.hi);
-                    if (!el.may_silent) on_nlo = std::max<int>(on_nlo, el.nlo);
-                    min_nlo = std::min<int>(min_nlo, el.nlo);
-                    all_may_silent = all_may_silent && el.may_silent;
-                }
-                const int nlo = std::max(on_nlo, min_nlo);
-                pl.lo = (uint8_t)computed_channels(n.cfg, lo);
-                pl.hi = (uint8_t)computed_channels(n.cfg, hi);
-                pl.nlo = (uint8_t)computed_channels(n.cfg, nlo);
-                pl.nhi = pl.hi;
-                pl.may_silent = all_may_silent;
-                if (n.kind == K_DELAY_R) pl = pn.at(edges[0].node).lay_out(edges[0].port);
-            }
-            // more than two layouts meeting in a port wider than stereo: the order of the up-mixes matters (mono, stereo, 5.1: the
-            // reference goes 1 -> 2 -> 6): fold edge by edge like it does
-            bool needs_fold = false;
-            if (ch > 2 && n.cfg.mode != WAE_COUNT_MODE_EXPLICIT)
-                for (auto& r : edges) needs_fold = needs_fold || pn.at(r.node).out_ch[r.port] != ch;
-            if (!is_dest && edges.size() == 1 && pn.at(edges[0].node).out_ch[edges[0].port] == ch) {
-                const Lay el = pn.at(edges[0].node).lay_out(edges[0].port);
-                // a single edge IS the port when computedNumberOfChannels leaves every count it can have alone
-                const bool identity = !el.dyn() || n.kind == K_DELAY_R || n.cfg.mode == WAE_COUNT_MODE_MAX ||
-                                      (n.cfg.mode == WAE_COUNT_MODE_CLAMPED_MAX && el.hi <= n.cfg.count);
-                // the time-batched convolver reads all static channels of every quantum: it needs the canonical PCM k_mix_dyn writes
-                const bool canonical_needed = el.dyn() && n.kind == K_CONV;
-                if (identity && !canonical_needed) {
-                    p.in_buf[port] = pn.at(edges[0].node).out_buf[edges[0].port];  // alias, no copy
-                    p.in_lay[port] = el;
-                    continue;
-                }
-            }
-            if (any_dyn || needs_fold) {
-                StageBuild& ms = stage(2 * level, S_MIX_DYN);
-                MixDynInst m{};
-                m.out_ch = ch;
-                m.interp = n.cfg.interp;
-                m.mode = n.cfg.mode;
-                m.cfg_count = n.cfg.count;
-                m.n_edges = (int)edges.size();
-                m.edge_offset = (uint32_t)ms.mix_edges.size();
-                m.limit = -1;
-                if (is_dest) {
-                    m.out = dest_ref(g, gi);
-                    m.limit = (int64_t)g->length;
-                    if (g->length > 0xffffffffull) return bail(WAE_UNSUPPORTED, "render length above 2^32 frames");
-                } else {
-                    m.out = arena_buf(ch, pl.dyn());
-                    if (!m.out.p) return bail(WAE_OUT_OF_MEMORY, "out of device memory (arena)");
-                }
-                for (auto& r : edges) {
-                    PNode& sn = pn.at(r.node);
-                    ms.mix_edges.push_back(MixEdge{sn.out_buf[r.port], sn.out_ch[r.port], 0});
-                }
-                ms.mix_dyn.push_back(m);
-                p.in_buf[port] = m.out;
-                p.in_lay[port] = pl;
-                continue;
-            }
-            StageBuild& ms = stage(2 * level, S_MIX);
-            MixInst m{};
-            m.out_ch = ch;
-            m.interp = n.cfg.interp;
-            m.n_edges = (int)edges.size();
-            m.edge_offset = (uint32_t)ms.mix_edges.size();
-            m.limit = -1;
-            if (is_dest) {
-                m.out = dest_ref(g, gi);
-                m.limit = (int64_t)g->length;
-                if (g->length > 0xffffffffull) return bail(WAE_UNSUPPORTED, "render length above 2^32 frames");
-            } else {
-                m.out = arena_buf(ch);
-                if (!m.out.p) return bail(WAE_OUT_OF_MEMORY, "out of device memory (arena)");
-            }
-            for (auto& r : edges) {
-                PNode& s = pn.at(r.node);
-                ms.mix_edges.push_back(MixEdge{s.out_buf[r.port], s.out_ch[r.port], 0});
-            }
-            ms.mix.push_back(m);
-            p.in_buf[port] = m.out;
-        }
-        const int L = 2 * level + 1;  // node kernels run after the mixes of their level
-        auto need_out = [&](int ch) {
-            p.out_ch = {ch};
-            p.out_buf = {arena_buf(ch)};
-            return p.out_buf[0].p != nullptr;
-        };
-        // the node's (single) output has a layout that is not constant: give its buffer a layout track
-        auto out_dynamic = [&](const Lay& l) {
-            p.out_lay = {l};
-            if (l.dyn() && !p.out_buf.empty() && p.out_buf[0].p && !p.out_buf[0].absolute) {
-                p.out_buf[0].meta = dry ? reinterpret_cast<uint8_t*>(uintptr_t(256)) : reinterpret_cast<uint8_t*>(p.out_buf[0].p + (size_t)p.out_ch[0] * (size_t)b->chunk);
-                p.out_buf[0].meta_stride = (uint32_t)((b->chunk / 128 + 16) / 16 * 16);
-            }
-        };
-        // a scheduled source: `ch` channels inside [n_first, n_stop), one silent channel outside (never silent when it covers the render)
-        auto source_lay = [&](int64_t n_first, int64_t n_stop, int ch) { return (n_first <= 0 && n_stop >= glq) ? Lay::fixed(ch) : Lay::gated(ch); };
-        auto source_meta = [&](int64_t n_first, int64_t n_stop, int ch) {
-            MetaInst m{};
-            m.out = p.out_buf[0];
-            m.mode = META_SOURCE;
-            m.out_ch = ch;
-            m.count = ch;
-            m.n_first = n_first;
-            m.n_stop = n_stop;
-            stage(L, S_META).meta.push_back(m);
-        };
-        const Lay in0 = p.in_lay.empty() ? Lay::fixed(1) : p.in_lay[0];
-        // biquad / IIR (biquad_filter.rs:778-815): silent once the input is and the tail has rung out; keeps the channels of the last
-        // input that was not silent
-        auto filter_lay = [](const Lay& l) { return Lay{(uint8_t)(l.may_silent ? 1 : l.lo), l.hi, l.nlo, l.nhi, l.may_silent}; };
-        // output with the input's layout and channel count: share the input's layout track
-        auto out_like_input = [&]() {
-            p.out_lay = {in0};
-            if (in0.dyn() && !p.out_buf.empty() && p.out_buf[0].p) {
-                p.out_buf[0].meta = p.in_buf[0].meta;
-                p.out_buf[0].meta_stride = p.in_buf[0].meta_stride;
-            }
-        };
-        // registers this node as the tail of a chain: pending while exactly one consumer may still fuse with it
-        auto finish_chain = [&](PendingChain&& pc) -> bool {
-            p.out_ch = {pc.ch};
-            p.out_buf = {BufRef{nullptr, 0, 0}};
-            p.out_lay = {pc.lay};
-            pending[id] = std::move(pc);
-            if (!(fuse && consumers(n) == 1)) return materialize(id);
-            return true;
-        };
-        auto source_chain = [&](int kind, int ch) {
-            PendingChain pc;
-            std::memset(&pc.inst, 0, sizeof(pc.inst));
-            pc.inst.src_kind = kind;
-            pc.inst.ch = ch;
-            pc.inst.limit = -1;
-            pc.inst.end = glq;
-            for (int i = 0; i < 4; i++) pc.inst.g[i] = 1.f;
-            pc.ch = ch;
-            pc.cls = cur_cls;
-            pc.lay = Lay::fixed(ch);
-            return pc;
-        };
-        // chain that this biquad / gain / shaper node joins: its producer's pending chain, or a new one reading in_buf
-        auto open_chain = [&]() {
-            if (extend) {
-                PendingChain pc = std::move(pending.at(fuse_src));
-                pending.erase(fuse_src);
-                return pc;
-            }
-            PendingChain pc = source_chain(CHAIN_SRC_BUFFER, p.in_ch[0]);
-            pc.inst.in = p.in_buf[0];
-            pc.lay = in0;
-            return pc;
-        };
+        NodeCtx nc{id, n, p};
+        if (!plan_inputs(nc)) return false;
+        bool ok = false;
         switch (n.kind) {
-            case K_DEST: {
-                p.out_ch = {(int)g->channels};
-                if (dest_direct) {  // the chain writes the rendered PCM itself (speaker up-mix 1->2 = copy, quantum.rs:301-305)
-                    PendingChain pc = std::move(pending.at(fuse_src));
-                    pending.erase(fuse_src);
-                    const BufRef fin = dest_ref(g, gi);
-                    pc.inst.out = fin;
-                    pc.inst.limit = (int64_t)g->length;
-                    pc.inst.out_dup = (pc.ch == 1 && g->channels == 2) ? 2 : 0;
-                    emit_chain(pc, L);
-                    pn.at(fuse_src).out_buf = {fin};
-                    p.in_buf[0] = fin;
-                }
-                p.out_buf = {p.in_buf[0]};
-                algorithmic_bytes += (uint64_t)g->channels * g->length * 4;  // destination write, SURVEY §8(d)
-                break;
-            }
-            case K_OSC: {
-                PRef pf = param_ref(g, n.params[0]), pd = param_ref(g, n.params[1]);
-                float freq = pf.v, detune = pd.v;
-                if (!fuse_n && !need_out(1)) return bail(WAE_OUT_OF_MEMORY, "out of device memory (arena)");
-                OscInst o{};
-                double start_ratio = 0.;
-                if (!fuse_n) o.out = p.out_buf[0];
-                o.type = n.type;
-                double computed_freq = (double)freq * std::exp2((double)detune / 1200.);  // oscillator.rs:30-32
-                o.incr = computed_freq / sr;
-                o.inv_incr = o.incr != 0. ? 1. / o.incr : 0.;
-                o.outside_nyquist = std::fabs(computed_freq) >= sr / 2.;
-                o.n_first = std::numeric_limits<int64_t>::max();
-                o.n_stop = std::numeric_limits<int64_t>::max();
-                o.phase0 = 0.;
-                if (n.start_time < 1e300) {
-                    // oscillator.rs:391-428,511-540: first rendered frame and its phase
-                    int64_t q = clock.quantum_containing(n.start_time);
-                    double start = n.start_time;
-                    if (start < clock.block_time(q)) start = clock.block_time(q);  // "prevent scheduling in the past"
-                    double t = 0.;
-                    // walk the accumulated per-frame clock of that quantum
-                    double cur = clock.block_time(q);
-                    int i = 0;
-                    for (; i < 128; i++) {
-                        if (!(cur < start)) break;
-                        cur += clock.dt;
-                    }
-                    t = cur;
-                    o.n_first = q * 128 + i;
-                    if (i < 128 && t > start) {
-                        double ratio = (t - start) / clock.dt;
-                        start_ratio = ratio;
-                        double ph = o.incr * ratio;
-                        if (o.outside_nyquist) {
-                            ph = std::fmod(ph, 1.);
-                            if (ph < 0.) ph += 1.;
-                        } else {
-                            ph = hm::unroll_phase(ph);
-                        }
-                        o.phase0 = ph;
-                    }
-                    if (n.stop_time < 1e300) {
-                        int64_t qs = clock.quantum_containing(n.stop_time);
-                        if (n.stop_time <= clock.block_time(qs)) o.n_stop = qs * 128;
-                        else o.n_stop = clock.first_frame_at_or_after(n.stop_time);
-                    }
-                }
-                if (n.type == WAE_OSC_CUSTOM) {
-                    float* d = upload(n.table);
-                    o.table = d;
-                    o.table_len = (int)n.table.size();
-                } else {
-                    o.table = eng->d_sine;
-                    o.table_len = 2048;
-                }
-                o.fast = (!o.outside_nyquist && o.incr > 0. && o.incr < 0.5 && (o.table_len == 2048 || (o.type != WAE_OSC_SINE && o.type != WAE_OSC_CUSTOM))) ? 1 : 0;
-                if (dyn_params) {  // automated / audio-rate frequency or detune: running-sum phase
-                    OscArInst oa{};
-                    oa.base = o;
-                    oa.freq = pf.dyn ? pf.track : BufRef{nullptr, 0, 0};
-                    oa.detune = pd.dyn ? pd.track : BufRef{nullptr, 0, 0};
-                    oa.f_val = freq;
-                    oa.d_val = detune;
-                    oa.start_ratio = start_ratio;
-                    oa.phase = alloc<double>(1, true, true);
-                    oa.sample_rate = g->sample_rate;
-                    if (!oa.phase) return bail(WAE_OUT_OF_MEMORY, "out of device memory (state)");
-                    out_dynamic(source_lay(o.n_first, o.n_stop, 1));
-                    oa.base.out = p.out_buf[0];
-                    if (p.out_lay[0].dyn()) source_meta(o.n_first, o.n_stop, 1);
-                    stage(L, S_OSC_AR).osc_ar.push_back(oa);
-                } else if (fuse_n) {
-                    PendingChain pc = source_chain(CHAIN_SRC_OSC, 1);
-                    pc.inst.osc = o;
-                    pc.lay = source_lay(o.n_first, o.n_stop, 1);
-                    if (!finish_chain(std::move(pc))) return false;
-                } else {
-                    out_dynamic(source_lay(o.n_first, o.n_stop, 1));
-                    o.out = p.out_buf[0];
-                    if (p.out_lay[0].dyn()) source_meta(o.n_first, o.n_stop, 1);
-                    stage(L, S_OSC).osc.push_back(o);
-                }
-                break;
-            }
-            case K_CONST: {
-                PRef po = param_ref(g, n.params[0]);
-                float v = po.v;
-                if (!fuse_n && !need_out(1)) return bail(WAE_OUT_OF_MEMORY, "out of device memory (arena)");
-                ConstInst c{};
-                if (!fuse_n) c.out = p.out_buf[0];
-                if (po.dyn) c.track = po.track;
-                c.value = v;
-                c.n_first = std::numeric_limits<int64_t>::max();
-                c.n_stop = std::numeric_limits<int64_t>::max();
-                if (n.start_time < 1e300) {
-                    // constant_source.rs:203-246
-                    c.n_first = clock.first_frame_at_or_after(n.start_time);
-                    if (n.stop_time < 1e300) c.n_stop = clock.first_frame_at_or_after(n.stop_time);
-                }
-                if (fuse_n) {
-                    PendingChain pc = source_chain(CHAIN_SRC_CONST, 1);
-                    pc.inst.cst = c;
-                    pc.lay = source_lay(c.n_first, c.n_stop, 1);
-                    if (!finish_chain(std::move(pc))) return false;
-                } else {
-                    out_dynamic(source_lay(c.n_first, c.n_stop, 1));
-                    c.out = p.out_buf[0];
-                    if (p.out_lay[0].dyn()) source_meta(c.n_first, c.n_stop, 1);
-                    stage(L, S_CONST).cst.push_back(c);
-                }
-                break;
-            }
-            case K_ABSN: {
-                PRef pdet = param_ref(g, n.params[0]), prate = param_ref(g, n.params[1]);
-                const float detune = pdet.v, rate = prate.v;
-                const bool rate_automated = pdet.dyn || prate.dyn;
-                int ch = n.buffer ? (int)n.buffer->channels.size() : 1;
-                if (!n.buffer || n.start_time >= 1e300 || ch == 0) {  // never plays: silence
-                    if (!need_out(1)) return bail(WAE_OUT_OF_MEMORY, "out of device memory (arena)");
-                    StageBuild& ms = stage(L, S_MIX);
-                    ms.mix.push_back(MixInst{p.out_buf[0], 1, 0, 0, (uint32_t)ms.mix_edges.size(), -1});
-                    out_dynamic(Lay{1, 1, 1, 1, true});  // silent for good
-                    if (p.out_buf[0].meta) source_meta(0, 0, 1);
-                    break;
-                }
-                PcmBuffer& pb = *n.buffer;
-                double computed_rate = (double)rate * std::exp2((double)detune / 1200.);
-                double duration = pb.duration();
-                double ls = n.loop_start, le = n.loop_end;  // clamp_loop_boundaries, audio_buffer_source.rs:400-417
-                if (ls < 0.) ls = 0.; else if (ls > duration) ls = duration;
-                if (le <= 0. || le > duration) le = duration;
-                int64_t q = clock.quantum_containing(n.start_time);
-                // a start time that IS the next block boundary but compares below next_block_time by one rounding:
-                // the reference goes through one all-silent slow-track quantum, then aligns (audio_buffer_source.rs:521-523)
-                if (n.start_time > clock.block_time(q) && n.start_time == clock.block_time(q + 1)) q = q + 1;
-                bool aligned = (n.start_time <= clock.block_time(q)) && n.offset == 0.;  // start in the past snaps to the block
-                bool fast = !rate_automated && aligned && (double)pb.sample_rate / sr == 1. && computed_rate == 1. && ls == 0. && le == duration &&
-                            n.duration > 1e300 && n.stop_time > 1e300;
-                // everything the closed-form tracks do not cover runs the renderer's own frame loop (one warp per source)
-                bool serial = rate_automated || (!fast && !(computed_rate > 0.));
-                if (!fast && !serial && n.loop) {
-                    const bool custom = ls >= 0. && le > 0. && ls < le;
-                    const double loop_len = custom ? le - ls : duration;
-                    if (!(loop_len > 4. * clock.dt * computed_rate)) serial = true;  // loop shorter than four output frames
-                }
-                const bool fuse_src = fuse_n && fast;
-                if (!fuse_src && !need_out(ch)) return bail(WAE_OUT_OF_MEMORY, "out of device memory (arena)");
-                size_t len = pb.length();
-                size_t stride = (len + 3) / 4 * 4;  // every channel starts 16 B aligned (LDG.128)
-                // one copy of the PCM per AudioBuffer in the group's slab (the grains of a granular patch all play the same one: the graph
-                // holds it once, wae_abi_graph.cpp copy_buffer), shared by the plans of all render segments
-                auto so = src_offsets.find({gi, id});
-                bool first_use = so == src_offsets.end();
-                if (first_use) {
-                    auto bo = buf_offsets.find(n.buffer.get());
-                    if (bo != buf_offsets.end()) first_use = false;  // (already in the slab for another node)
-                    else bo = buf_offsets.emplace(n.buffer.get(), src_cursor).first;
-                    so = src_offsets.emplace(std::make_pair(gi, id), bo->second).first;
-                }
-                float* d_buf = d_src + so->second;
-                if (first_use) {
-                    if (src_copies)  // recorded by the sizing pass: uploaded straight from the graph's buffer, planar [ch][stride] like the slab
-                        src_copies->push_back(wae_batch::Group::SrcCopy{n.buffer, src_cursor, (size_t)ch * stride});
-                    src_cursor += (size_t)ch * stride;
-                    b->asset_bytes += (size_t)ch * len * 4;
-                }
-                if (serial) {
-                    AbsnSerialInst a{};
-                    a.out = p.out_buf[0];
-                    a.buf = d_buf;
-                    a.buf_len = (int64_t)len;
-                    a.buf_stride = (int64_t)stride;
-                    a.start_time = n.start_time;
-                    a.stop_time = n.stop_time;
-                    a.offset = n.offset;
-                    a.duration = n.duration;
-                    a.loop_start = ls;
-                    a.loop_end = le;
-                    a.buffer_duration = duration;
-                    a.buffer_sample_rate = (double)pb.sample_rate;
-                    a.sample_rate = sr;
-                    const BufRef none{nullptr, 0, 0};
-                    a.rate_track = prate.dyn ? prate.track : none;
-                    a.detune_track = pdet.dyn ? pdet.track : none;
-                    a.rate = rate;
-                    a.detune = detune;
-                    a.ch = ch;
-                    a.loop = n.loop ? 1 : 0;
-                    a.state = alloc<AbsnSerialState>(1, true, true);
-                    if (!a.state) return bail(WAE_OUT_OF_MEMORY, "out of device memory (buffer source state)");
-                    out_dynamic(Lay::gated(ch));  // when it plays depends on the automated rate: the kernel writes the layout track
-                    a.out = p.out_buf[0];
-                    stage(L, S_ABSN_SERIAL).absn_serial.push_back(a);
-                    algorithmic_bytes += (uint64_t)ch * 4ull * (uint64_t)std::min<int64_t>(lq, (int64_t)len);
-                    break;
-                }
-                if (!fast) {
-                    // ---- slow track (audio_buffer_source.rs:625-823): fractional playhead
-                    auto almost_equal = [](double x, double y) {
-                        if (x == y) return true;
-                        const double tol = 1.4901161193847656e-8;
-                        double d = std::fabs(y - x);
-                        return d <= tol || d <= std::max(std::fabs(x), std::fabs(y)) * tol;
-                    };
-                    AbsnSlowInst a{};
-                    a.out = p.out_buf[0];
-                    a.buf = d_buf;
-                    a.buf_len = (int64_t)len;
-                    a.buf_stride = (int64_t)stride;
-                    a.ch = ch;
-                    a.loop = n.loop ? 1 : 0;
-                    a.sample_rate = sr;
-                    a.buffer_duration = duration;
-                    a.pos_scale = ((double)pb.sample_rate / sr) * sr;  // position = buffer_time * sampling_ratio; playhead = position * sr
-                    a.step = clock.dt * computed_rate;
-                    a.duration = n.duration;
-                    // actual loop points (:627-636)
-                    if (n.loop && ls >= 0. && le > 0. && ls < le) {
-                        a.loop_start = ls;
-                        a.loop_end = le;
-                    } else {
-                        a.loop_start = 0.;
-                        a.loop_end = duration;
-                    }
-                    // first frame at / after the start time: current_time = block_time + i * dt (:648), sticky within
-                    // almost::equal (:652-654)
-                    double start = n.start_time;
-                    int64_t qq = clock.quantum_containing(start);
-                    int64_t n_first = -1;
-                    double t_first = 0.;
-                    for (int guard = 0; guard < 3 && n_first < 0; guard++, qq++) {
-                        double bt0 = clock.block_time(qq);
-                        for (int i = 0; i < 128; i++) {
-                            double t = bt0 + (double)i * clock.dt;
-                            if (almost_equal(t, start)) start = t;
-                            if (!(t < start)) {
-                                n_first = qq * 128 + i;
-                                t_first = t;
-                                break;
-                            }
-                        }
-                    }
-                    if (n_first < 0) n_first = qq * 128;
-                    double delta = t_first - start;
-                    double off = n.offset + delta * computed_rate;  // :672-674
-                    off = std::min(std::max(off, 0.), duration);
-                    if (n.loop && off > a.loop_end) off = a.loop_end;  // :676-678 (rate >= 0)
-                    a.offset0 = off;
-                    a.elapsed0 = std::fabs(delta * computed_rate);
-                    a.n_first = n_first;
-                    a.n_stop = std::numeric_limits<int64_t>::max();
-                    if (n.stop_time < 1e300) {  // first frame with current_time >= stop_time (:663)
-                        int64_t qs = clock.quantum_containing(n.stop_time);
-                        int64_t ns = (qs + 1) * 128;
-                        double bt0 = clock.block_time(qs);
-                        for (int i = 0; i < 128; i++)
-                            if (bt0 + (double)i * clock.dt >= n.stop_time) {
-                                ns = qs * 128 + i;
-                                break;
-                            }
-                        a.n_stop = ns;
-                    }
-                    // playhead schedule: walk the reference's per-frame bookkeeping (:730-770) from event to event — a
-                    // frame where buffer_time is snapped to a loop point (almost::equal) or wrapped starts a new segment
-                    std::vector<int64_t> seg_n{n_first};
-                    std::vector<double> seg_bt{off};
-                    if (n.loop && off < a.loop_end) {
-                        const double ls2 = a.loop_start, le2 = a.loop_end, len2 = le2 - ls2, step = a.step;
-                        const int64_t n_end = std::min<int64_t>(lq, a.n_stop);
-                        int64_t m = 0;   // frames since n_first
-                        double v = off;  // buffer_time of frame m
-                        bool entered = false;
-                        auto tz = [&](double x) { return 3.0e-8 * (1.0 + std::fabs(x)); };  // a little wider than almost::equal
-                        while (n_first + m < n_end) {
-                            // frames until the playhead can touch the tolerance zone of a loop point
-                            double to_ls = v < ls2 - tz(ls2) ? (ls2 - tz(ls2) - v) / step : 0.;
-                            double to_le = v < le2 - tz(le2) ? (le2 - tz(le2) - v) / step : 0.;
-                            double skip = (!entered && to_ls > 0.) ? std::min(to_ls, to_le) : to_le;
-                            int64_t adv = (int64_t)std::floor(skip);
-                            if (adv > 0) {
-                                v += (double)adv * step;
-                                m += adv;
-                                continue;
-                            }
-                            // exact per-frame logic of the reference
-                            double w = v;
-                            if (almost_equal(w, le2)) w = le2;
-                            if (almost_equal(w, ls2)) w = ls2;
-                            if (!entered && w >= ls2) entered = true;
-                            if (entered) {
-                                while (w >= le2) w -= len2;
-                                while (w < ls2) w += len2;
-                            }
-                            if (w != v && n_first + m > seg_n.back()) {
-                                seg_n.push_back(n_first + m);
-                                seg_bt.push_back(w);
-                            } else if (w != v) {
-                                seg_bt.back() = w;
-                            }
-                            v = w + step;
-                            m += 1;
-                        }
-                    }
-                    a.n_seg = (int32_t)seg_n.size();
-                    a.seg_n = upload(seg_n);
-                    a.seg_bt = upload(seg_bt);
-                    {
-                        // layout: silent before the quantum of the first playing frame and after the quantum in which the source ends
-                        // (stop time, explicit duration, or — not looping — the end of the buffer; audio_buffer_source.rs:826-838)
-                        int64_t n_end = a.n_stop;
-                        if (a.step > 0.) {
-                            if (!n.loop) n_end = std::min<int64_t>(n_end, n_first + (int64_t)std::ceil(std::max(0., duration - off) / a.step));
-                            if (n.duration < 1e300) n_end = std::min<int64_t>(n_end, n_first + (int64_t)std::ceil(std::max(0., n.duration - a.elapsed0) / a.step));
-                        }
-                        out_dynamic(source_lay(n_first, n_end, ch));
-                        a.out = p.out_buf[0];
-                        if (p.out_lay[0].dyn()) source_meta(n_first, n_end, ch);
-                    }
-                    stage(L, S_ABSN_SLOW).absn_slow.push_back(a);
-                    algorithmic_bytes += (uint64_t)ch * 4ull * (uint64_t)std::min<int64_t>(lq, (int64_t)len);
-                    break;
-                }
-                AbsnInst a{};
-                if (!fuse_src) a.out = p.out_buf[0];
-                a.buf = d_buf;
-                a.buf_len = (int64_t)len;
-                a.buf_stride = (int64_t)stride;
-                a.n_start = q * 128;
-                a.n_stop = std::numeric_limits<int64_t>::max();
-                a.buf_offset = 0;
-                a.ch = ch;
-                a.loop = n.loop ? 1 : 0;
-                if (!n.loop) {
-                    // the quantum after which the source has `ended`: the reference accumulates buffer_time += block_duration and stops
-                    // once it reaches the buffer's duration (audio_buffer_source.rs:609,826-838) — replayed, not divided
-                    const double block_duration = clock.dt * 128.;
-                    const int64_t max_q = (lq - a.n_start) / 128 + 2;
-                    int64_t played = 0;
-                    double bt = 0.;
-                    while (played < max_q) {
-                        bt += block_duration;
-                        played++;
-                        if (bt >= duration) break;
-                    }
-                    a.n_stop = a.n_start + played * 128;
-                }
-                if (fuse_src) {
-                    PendingChain pc = source_chain(CHAIN_SRC_ABSN, ch);
-                    pc.inst.absn = a;
-                    pc.lay = source_lay(a.n_start, a.n_stop, ch);
-                    if (!finish_chain(std::move(pc))) return false;
-                } else {
-                    out_dynamic(source_lay(a.n_start, a.n_stop, ch));
-                    a.out = p.out_buf[0];
-                    if (p.out_lay[0].dyn()) source_meta(a.n_start, a.n_stop, ch);
-                    stage(L, S_ABSN).absn.push_back(a);
-                }
-                // compulsory read of the source PCM that is actually played
-                algorithmic_bytes += (uint64_t)ch * 4ull * (uint64_t)std::max<int64_t>(0, std::min<int64_t>(lq - a.n_start, n.loop ? lq : (int64_t)len));
-                break;
-            }
-            case K_BIQUAD: {
-                PRef pq = param_ref(g, n.params[0]), pdt = param_ref(g, n.params[1]), pfr = param_ref(g, n.params[2]), pg = param_ref(g, n.params[3]);
-                float q = pq.v, detune = pdt.v, freq = pfr.v, gain = pg.v;
-                int ch = p.in_ch[0];
-                if (dyn_params) {  // per-frame coefficients (biquad_filter.rs:837-855): serial a-rate kernel
-                    if (!need_out(ch)) return bail(WAE_OUT_OF_MEMORY, "out of device memory (arena)");
-                    BiquadArInst ba{};
-                    ba.in = p.in_buf[0];
-                    ba.out = p.out_buf[0];
-                    const BufRef none{nullptr, 0, 0};
-                    ba.q = pq.dyn ? pq.track : none;
-                    ba.detune = pdt.dyn ? pdt.track : none;
-                    ba.freq = pfr.dyn ? pfr.track : none;
-                    ba.gain = pg.dyn ? pg.track : none;
-                    ba.q_val = q; ba.detune_val = detune; ba.freq_val = freq; ba.gain_val = gain;
-                    ba.state = alloc<double>((size_t)ch * 4, true, true);
-                    if (!ba.state) return bail(WAE_OUT_OF_MEMORY, "out of device memory (state)");
-                    if (in0.dyn()) {
-                        ba.dyn_len = alloc<int32_t>((size_t)ch, true, true);
-                        if (!ba.dyn_len) return bail(WAE_OUT_OF_MEMORY, "out of device memory (state)");
-                        out_dynamic(filter_lay(in0));
-                        ba.out = p.out_buf[0];
-                    }
-                    {
-                        // five planes of f64 coefficients per frame of the chunk (an arena buffer of 10 float channels read as doubles)
-                        BufRef cb = arena_buf(10);
-                        if (!cb.p) return bail(WAE_OUT_OF_MEMORY, "out of device memory (arena)");
-                        cb.stride = (uint32_t)b->chunk;  // in DOUBLES: plane k starts at double index k * chunk
-                        ba.coefs = cb;
-                    }
-                    ba.sample_rate = g->sample_rate;
-                    ba.type = n.type;
-                    ba.ch = ch;
-                    StageBuild& sb = stage(L, S_BIQUAD_AR);
-                    sb.max_ch = std::max(sb.max_ch, ch);
-                    sb.biquad_ar.push_back(ba);
-                    break;
-                }
-                float cf = hm::biquad_computed_freq(freq, detune);
-                hm::BiquadCoefs c = hm::biquad_coefs(n.type, sr, (double)cf, (double)gain, (double)q);
-                double* state = alloc<double>((size_t)ch * 4, true, true);
-                if (!state) return bail(WAE_OUT_OF_MEMORY, "out of device memory (state)");
-                // An input whose channel COUNT changes while it sounds resets / drops channels of the filter mid-render
-                // (biquad_filter.rs:798-815): the serial kernel follows it quantum by quantum; the scan keeps one state per channel
-                const bool count_varies = !extend && in0.dyn() && !(in0.nlo == in0.nhi && in0.nhi == ch);
-                if (eng->serial_filters || count_varies) {  // bit-faithful serial recurrence, one stage per biquad
-                    if (!need_out(ch)) return bail(WAE_OUT_OF_MEMORY, "out of device memory (arena)");
-                    BiquadInst bi{};
-                    if (in0.dyn()) {
-                        bi.dyn_len = alloc<int32_t>((size_t)ch, true, true);
-                        if (!bi.dyn_len) return bail(WAE_OUT_OF_MEMORY, "out of device memory (state)");
-                        out_dynamic(filter_lay(in0));
-                    }
-                    bi.in = p.in_buf[0];
-                    bi.out = p.out_buf[0];
-                    bi.b0 = c.b0; bi.b1 = c.b1; bi.b2 = c.b2; bi.a1 = c.a1; bi.a2 = c.a2;
-                    bi.ch = ch;
-                    bi.state = state;
-                    StageBuild& s = stage(L, S_BIQUAD);
-                    s.max_ch = std::max(s.max_ch, ch);
-                    s.biquad.push_back(bi);
-                    break;
-                }
-                PendingChain pc = open_chain();
-                ChainBiquad& st = pc.inst.bq[pc.inst.n_biquad++];
-                st.state = state;
-                st.b0 = c.b0; st.b1 = c.b1; st.b2 = c.b2; st.a1 = c.a1; st.a2 = c.a2;
-                pc.coefs[pc.inst.n_biquad - 1] = c;
-                pc.phase = pc.phase == 0 ? 1 : 3;
-                pc.lay = filter_lay(pc.lay);
-                if (!finish_chain(std::move(pc))) return false;
-                break;
-            }
-            case K_IIR: {
-                int ch = p.in_ch[0];
-                std::vector<double> ff = n.feedforward, fb = n.feedback;  // iir_filter.rs:282-309
-                if (ff.size() < fb.size()) ff.resize(fb.size(), 0.);
-                if (ff.size() > fb.size()) fb.resize(ff.size(), 0.);
-                if (ff.size() <= 3 && !eng->serial_filters && !in0.dyn() && seg_start == 0 && seg_end >= lq) {
-                    // Order <= 2 with a constant input layout: the same transfer function as a biquad — rendered by the time-parallel scan
-                    // of k_chain (direct form I there, transposed direct form II in iir_filter.rs:386-407: the outputs differ in the last
-                    // bits of the f64 arithmetic only) instead of one serial thread per channel.  With an input that can fall silent the
-                    // serial kernel stays: its tail test looks at the reference's own state variables.  Same for a render cut by suspend
-                    // points: the two forms keep different state (x / y history here, the reference's 20 accumulators there) and a later
-                    // segment may see a layout that needs the serial kernel — the filter memory must survive the cut (fuzz seeds 31, 33).
-                    ff.resize(3, 0.);
-                    fb.resize(3, 0.);
-                    const double a0 = fb[0];
-                    hm::BiquadCoefs c{ff[0] / a0, ff[1] / a0, ff[2] / a0, fb[1] / a0, fb[2] / a0};
-                    double* state = alloc<double>((size_t)ch * 4, true, true);
-                    if (!state) return bail(WAE_OUT_OF_MEMORY, "out of device memory (state)");
-                    PendingChain pc = open_chain();
-                    ChainBiquad& st = pc.inst.bq[pc.inst.n_biquad++];
-                    st.state = state;
-                    st.b0 = c.b0; st.b1 = c.b1; st.b2 = c.b2; st.a1 = c.a1; st.a2 = c.a2;
-                    pc.coefs[pc.inst.n_biquad - 1] = c;
-                    pc.phase = 1;
-                    if (!finish_chain(std::move(pc))) return false;
-                    break;
-                }
-                if (!need_out(ch)) return bail(WAE_OUT_OF_MEMORY, "out of device memory (arena)");
-                IirInst ii{};
-                ii.in = p.in_buf[0];
-                ii.out = p.out_buf[0];
-                ii.n = (int)ff.size();
-                ii.ch = ch;
-                double a0 = fb[0];
-                for (size_t i = 0; i < ff.size(); i++) {
-                    ii.b[i] = ff[i] / a0;
-                    ii.a[i] = fb[i] / a0;
-                }
-                ii.state = alloc<double>((size_t)ch * 20, true, true);
-                if (!ii.state) return bail(WAE_OUT_OF_MEMORY, "out of device memory (state)");
-                if (in0.dyn()) {
-                    ii.dyn_len = alloc<int32_t>((size_t)ch, true, true);
-                    if (!ii.dyn_len) return bail(WAE_OUT_OF_MEMORY, "out of device memory (state)");
-                    out_dynamic(filter_lay(in0));
-                    ii.out = p.out_buf[0];
-                }
-                StageBuild& s = stage(L, S_IIR);
-                s.max_ch = std::max(s.max_ch, ch);
-                s.iir.push_back(ii);
-                break;
-            }
-            case K_GAIN: {
-                PRef pgn = param_ref(g, n.params[0]);
-                float gv = pgn.v;
-                int ch = p.in_ch[0];
-                if (pgn.dyn) {  // a-rate gain (gain.rs:189-197)
-                    if (!need_out(ch)) return bail(WAE_OUT_OF_MEMORY, "out of device memory (arena)");
-                    out_like_input();  // silent in -> silent out (gain.rs:155-158); the ~0 / ~1 shortcuts only exist for single values
-                    stage(L, S_GAIN).gain.push_back(GainInst{p.in_buf[0], p.out_buf[0], gv, ch, pgn.track});
-                    break;
-                }
-                // gain.rs:153-169: |g| <= 1e-6 -> silence, |1-g| <= 1e-6 -> pass-through (quanta >= 1; quantum 0 takes
-                // the multiply path, a difference of at most 1e-6 * |x| that is below the parity tolerance)
-                if (std::fabs(gv) <= 1e-6f) gv = 0.f;
-                else if (std::fabs(1.f - gv) <= 1e-6f) gv = 1.f;
-                if (fuse_n) {
-                    PendingChain pc = open_chain();
-                    // consecutive gains of one slot are folded (differs from two f32 multiplies by <= 1 ulp)
-                    pc.inst.g[pc.phase == 0 ? 0 : (pc.phase == 1 ? 1 : (pc.phase == 3 ? 2 : 3))] *= gv;
-                    if (gv == 0.f) pc.lay = Lay{1, 1, 1, 1, true};  // a gain of (about) zero answers with silence (gain.rs:160-163)
-                    if (!finish_chain(std::move(pc))) return false;
-                    break;
-                }
-                if (!need_out(ch)) return bail(WAE_OUT_OF_MEMORY, "out of device memory (arena)");
-                if (gv == 0.f) {
-                    out_dynamic(Lay{1, 1, 1, 1, true});
-                    if (p.out_buf[0].meta) source_meta(0, 0, 1);
-                } else {
-                    out_like_input();
-                }
-                stage(L, S_GAIN).gain.push_back(GainInst{p.in_buf[0], p.out_buf[0], gv, ch, BufRef{nullptr, 0, 0}});
-                break;
-            }
-            case K_SHAPER: {
-                int ch = p.in_ch[0];
-                const float* curve = n.has_curve ? upload(n.table) : nullptr;
-                // can_propagate_silence (waveshaper.rs:480-503): the curve maps 0 to 0
-                bool keeps_silence = true;
-                if (n.has_curve && !n.table.empty()) {
-                    const size_t cn = n.table.size();
-                    keeps_silence = cn % 2 == 1 ? std::fabs(n.table[cn / 2]) < 1e-9f : std::fabs((n.table[cn / 2 - 1] + n.table[cn / 2]) / 2.f) < 1e-9f;
-                }
-                // a silent input that still produces sound does so on the ONE channel a silent quantum has (waveshaper.rs:395-400)
-                auto shaper_lay = [&](const Lay& l) {
-                    if (keeps_silence || !l.may_silent) return l;
-                    return Lay{1, l.hi, 1, l.nhi, false};
-                };
-                if (n.oversample && n.has_curve) {  // waveshaper.rs:409-480: up-sample, shape, down-sample
-                    // input that can fall silent: a curve that maps 0 to 0 makes the node return early WITHOUT feeding its resamplers
-                    // (frozen state: the kernel then works on the last processed quanta); a curve that does not keeps processing — on the
-                    // one channel of a silent quantum, which rebuilds the resamplers of a wider node (waveshaper.rs:395-420)
-                    const bool freeze = in0.dyn() && keeps_silence && in0.nlo == in0.nhi && in0.nhi == ch;
-                    const bool as_static = !in0.dyn() || (!keeps_silence && ch == 1 && in0.hi == 1);
-                    // every other dynamic input: the count of the processed quanta changes, and the resamplers are rebuilt with it
-                    const bool rebuild = !freeze && !as_static;
-                    if (!need_out(ch)) return bail(WAE_OUT_OF_MEMORY, "out of device memory (arena)");
-                    if (freeze || (rebuild && keeps_silence)) {
-                        out_like_input();
-                    } else if (rebuild) {  // silent quanta processed: a sounding output with the input's count (one channel when silent)
-                        out_dynamic(shaper_lay(in0));
-                        if (p.out_buf[0].meta) meta_stage(L, META_SHAPER, p.in_buf[0], ch, p.out_buf[0], ch);
-                    }
-                    const int factor = n.oversample == WAE_OVERSAMPLE_X2 ? 2 : 4;
-                    auto& filt = os_filters[factor];
-                    if (!filt.first) {
-                        const std::vector<float2> fu = resampler_filter_bins(128, 128 * factor, 128);
-                        const std::vector<float2> fd = resampler_filter_bins(128 * factor, 128, 128);
-                        filt.first = upload(fu);
-                        filt.second = upload(fd);
-                        if (!dry) cudaStreamSynchronize(eng->stream);  // the host vectors go out of scope
-                    }
-                    ShaperOsInst so{};
-                    so.in = p.in_buf[0];
-                    so.out = p.out_buf[0];
-                    so.curve = curve;
-                    so.n = (int)n.table.size();
-                    so.ch = ch;
-                    so.factor = factor;
-                    so.f_up = filt.first;
-                    so.f_dn = filt.second;
-                    so.hist = alloc<float>((size_t)256 * ch, true, true);
-                    if (!so.hist || !so.f_up || !so.f_dn) return bail(WAE_OUT_OF_MEMORY, "out of device memory (over-sampled shaper)");
-                    if (freeze) {
-                        so.prev = alloc<int32_t>((size_t)(2 * (b->chunk / 128) + 2));
-                        if (!so.prev) return bail(WAE_OUT_OF_MEMORY, "out of device memory (over-sampled shaper)");
-                    }
-                    if (rebuild) {  // (the two words in front carry the resamplers' state across chunks and segments)
-                        so.rebuild = keeps_silence ? 2 : 1;
-                        so.prev = alloc<int32_t>((size_t)(2 + 3 * (b->chunk / 128) + 2), true, true);
-                        if (!so.prev) return bail(WAE_OUT_OF_MEMORY, "out of device memory (over-sampled shaper)");
-                    }
-                    StageBuild& os = stage(L, S_SHAPER_OS);
-                    os.max_ch = std::max(os.max_ch, ch);
-                    os.shaper_os.push_back(so);
-                    break;
-                }
-                if (fuse_n) {
-                    PendingChain pc = open_chain();
-                    pc.inst.has_shaper = 1;
-                    pc.inst.curve = curve;
-                    pc.inst.shaper_n = (int)n.table.size();
-                    pc.inst.shaper_keeps_silence = keeps_silence ? 1 : 0;
-                    pc.lay = shaper_lay(pc.lay);
-                    pc.phase = 5;
-                    if (!finish_chain(std::move(pc))) return false;
-                    break;
-                }
-                if (!need_out(ch)) return bail(WAE_OUT_OF_MEMORY, "out of device memory (arena)");
-                ShaperInst sh{};
-                if (in0.dyn() && !keeps_silence && n.has_curve) {
-                    out_dynamic(shaper_lay(in0));
-                    if (p.out_buf[0].meta) meta_stage(L, META_SHAPER, p.in_buf[0], ch, p.out_buf[0], ch);
-                } else {
-                    out_like_input();
-                }
-                sh.in = p.in_buf[0];
-                sh.out = p.out_buf[0];
-                sh.ch = ch;
-                sh.n = (int)n.table.size();
-                sh.curve = curve;
-                stage(L, S_SHAPER).shaper.push_back(sh);
-                break;
-            }
-            case K_SPANNER: {
-                PRef ppan = param_ref(g, n.params[0]);
-                float pan = ppan.v;
-                int ch = p.in_ch[0];
-                if (!need_out(2)) return bail(WAE_OUT_OF_MEMORY, "out of device memory (arena)");
-                // silent in -> silent out, else two channels (stereo_panner.rs:230-235); the kernel picks the mono / stereo law per quantum
-                out_dynamic(in0.may_silent ? Lay{1, 2, 2, 2, true} : Lay::fixed(2));
-                if (p.out_buf[0].meta) meta_stage(L, META_PAN, p.in_buf[0], ch, p.out_buf[0], 2);
-                float x = ch == 1 ? (pan + 1.f) * 0.5f : (pan <= 0.f ? pan + 1.f : pan);  // stereo_panner.rs:247-249,274-276
-                float gl, gr;
-                hm::stereo_gains(x, gl, gr);
-                StageBuild& s = stage(L, S_SPAN);
-                s.span.push_back(SPanInst{p.in_buf[0], p.out_buf[0], pan, ch, ppan.dyn ? ppan.track : BufRef{nullptr, 0, 0}});
-                s.span_gains.push_back(make_float2(gl, gr));
-                break;
-            }
-            case K_PANNER: {
-                // the 15 spatial params (panner.rs:714-780): 6 of the node, 9 of the AudioListener (graph ids 2..10)
-                PRef pr[15];
-                bool moving = false;
-                for (int i = 0; i < 15; i++) {
-                    pr[i] = param_ref(g, i < 6 ? n.params[i] : (uint32_t)(2 + i - 6));
-                    moving = moving || pr[i].dyn;
-                }
-                int ch = p.in_ch[0];
-                // (a static HRTF panner with a constant-layout input is lowered to the convolver kernels, which take their own output buffer)
-                static const bool hrtf_fft_on = [] { const char* e = getenv("WAE_HRTF_FFT"); return !e || atoi(e) != 0; }();
-                const bool hrtf_as_conv = n.panning_model == WAE_PANNING_HRTF && hrtf_fft_on && eng->sphere && !moving && !in0.dyn() && cur_cls != 1 &&
-                                          seg_start == 0 && seg_end >= lq && (ch == 1 || ch == 2);
-                if (!hrtf_as_conv && !need_out(2)) return bail(WAE_OUT_OF_MEMORY, "out of device memory (arena)");
-                if (hrtf_as_conv) p.out_lay = {Lay::fixed(2)};
-                else out_dynamic(in0.may_silent ? Lay{1, 2, 2, 2, true} : Lay::fixed(2));  // panner.rs:698-708
-                // (the HRTF panner keeps its own tail budget: its layout track is written by k_hrtf_map)
-                if (!hrtf_as_conv && p.out_buf[0].meta && n.panning_model != WAE_PANNING_HRTF) meta_stage(L, META_PAN, p.in_buf[0], ch, p.out_buf[0], 2);
-                spatial::PanModel model{};
-                model.distance_model = n.distance_model;
-                model.ref_distance = n.ref_distance;
-                model.max_distance = n.max_distance;
-                model.rolloff_factor = n.rolloff_factor;
-                model.cone_inner_angle = n.cone_inner_angle;
-                model.cone_outer_angle = n.cone_outer_angle;
-                model.cone_outer_gain = n.cone_outer_gain;
-                SpatialTracks tr{};
-                float v[15];
-                for (int i = 0; i < 15; i++) {
-                    v[i] = tr.value[i] = pr[i].v;
-                    tr.track[i] = pr[i].dyn ? pr[i].track : BufRef{nullptr, 0, 0};
-                }
-                const spatial::SpatialParams sp0 = spatial::spatial_params(model, v);  // static source and listener
-                if (n.panning_model == WAE_PANNING_HRTF) {  // panner.rs:781-830
-                    const HrirSphere* sph = eng->sphere;
-                    if (!sph) return bail(WAE_UNSUPPORTED, "HRTF panning needs an HRIR sphere: call wae_engine_set_hrir_sphere first");
-                    uint32_t sr = (uint32_t)g->sample_rate;
-                    if (sr < 27000) sr = 27000;  // panner.rs:46
-                    uint32_t taps = sph->taps;
-                    const float* d_ir = eng->d_sphere_ir;
-                    const float* h_ir = sph->ir.data();  // [vertex][2][taps] on the host
-                    if (sr != sph->sample_rate) {  // the crate resamples the responses to the context rate once (wae_hrtf_host.h)
-                        std::lock_guard<std::mutex> slk(eng->sphere_mu);
-                        auto it = eng->sphere_rates.find(sr);
-                        if (it == eng->sphere_rates.end()) {
-                            const HrirSphere rs = sph->at_rate(sr);
-                            wae_engine::RateSphere r;
-                            r.taps = rs.taps;
-                            if (r.taps < 2) return bail(WAE_UNSUPPORTED, "HRTF panning: the HRIR sphere is too short to be resampled to the context rate");
-                            if (cudaMalloc(&r.d_ir, rs.ir.size() * sizeof(float)) != cudaSuccess) return bail(WAE_OUT_OF_MEMORY, "out of device memory (resampled HRIR sphere)");
-                            cudaMemcpy(r.d_ir, rs.ir.data(), rs.ir.size() * sizeof(float), cudaMemcpyHostToDevice);
-                            r.ir_host = rs.ir;
-                            it = eng->sphere_rates.emplace(sr, r).first;
-                        }
-                        taps = it->second.taps;
-                        d_ir = it->second.d_ir;
-                        h_ir = it->second.ir_host.data();  // (map nodes are stable; entries are only dropped with the sphere)
-                    }
-                    // A static source heard by a static listener through a constant-layout input is ONE fixed pair of impulse responses:
-                    // out_ear = gain * (h_ear * mono(in)).  The crate evaluates that by FFT overlap-save per 128-frame block (hrtf 0.8.1
-                    // process_samples); here it is handed to the time-batched convolver kernels as a ConvolverNode-shaped problem —
-                    // response = the blended pair with the gain (and the reference's correction of 2 for a two-channel input,
-                    // panner.rs:805-812) folded in; a two-channel input is mixed down to mono by the forward transform's loads; one
-                    // partition, so the product is formed inside the inverse transform — instead of 2 x taps multiply-adds per output
-                    // frame in k_hrtf_fir.  WAE_HRTF_FFT=0: keep the FIR kernel.
-                    if (hrtf_as_conv) {
-                        float proj[3];
-                        spatial::projected_source(sp0, proj);
-                        const float dir[3] = {proj[0], proj[2], proj[1]};  // HrtfState::process swaps y / z (panner.rs:248-252)
-                        HrtfSel sel{{0, 0, 0}, {0.f, 0.f, 0.f}, sp0.cone_gain * sp0.dist_gain, 0.f};
-                        sph->locate(dir, sel.v, sel.w);  // no face: all-zero weights (silence)
-                        PcmBuffer resp;
-                        if (!resp.allocate(2, taps, false)) return bail(WAE_OUT_OF_MEMORY, "out of host memory (hrtf response)");
-                        const float corr = ch == 2 ? 2.f : 1.f;  // overall_gain_correction of a two-channel input (panner.rs:805-812)
-                        const float* A = h_ir + (size_t)sel.v[0] * 2 * taps;
-                        const float* B = h_ir + (size_t)sel.v[1] * 2 * taps;
-                        const float* C = h_ir + (size_t)sel.v[2] * 2 * taps;
-                        for (uint32_t k = 0; k < taps; k++) {  // (the blend k_hrtf_fir does, same f32 operations)
-                            const float l = (A[k] * sel.w[0] + B[k] * sel.w[1]) + C[k] * sel.w[2];
-                            const float r = (A[taps + k] * sel.w[0] + B[taps + k] * sel.w[1]) + C[taps + k] * sel.w[2];
-                            resp.channels[0].p[k] = corr * (l * sel.gain);
-                            resp.channels[1].p[k] = corr * (r * sel.gain);
-                        }
-                        resp.sample_rate = (float)sr;
-                        if (!plan_convolver(g, p, L, nullptr, -1, &resp)) return false;
-                        break;
-                    }
-                    HrtfInst h{};
-                    h.in = p.in_buf[0];
-                    h.out = p.out_buf[0];
-                    h.in_ch = ch;
-                    h.L = (int)taps;
-                    h.sphere_ir = d_ir;
-                    h.sel = nullptr;
-                    h.correction = ch == 2 ? 2.f : 1.f;
-                    h.hist = alloc<float>(taps, true, true);
-                    if (!h.hist) return bail(WAE_OUT_OF_MEMORY, "out of device memory (hrtf history)");
-                    if (in0.dyn()) {  // the node stops processing (and freezes) once its tail budget is used up: panner.rs:697-711
-                        h.dyn = 1;
-                        h.cmap = alloc<int32_t>((size_t)(b->chunk / 128 + 2));
-                        h.tail = alloc<int64_t>(1, true, true);
-                        if (!h.cmap || !h.tail) return bail(WAE_OUT_OF_MEMORY, "out of device memory (hrtf layout)");
-                    }
-                    StageBuild& hs = stage(L, S_HRTF);
-                    if (moving) {
-                        HrtfSelInst si{};
-                        si.sp = tr;
-                        si.model = model;
-                        si.pos = eng->d_sphere_pos;
-                        si.tri = eng->d_sphere_tri;
-                        si.n_faces = (int)(sph->tri.size() / 3);
-                        si.sel = alloc<HrtfSel>((size_t)(b->chunk / 128 + 1));
-                        if (!si.sel) return bail(WAE_OUT_OF_MEMORY, "out of device memory (hrtf selection)");
-                        h.sel = si.sel;
-                        hs.hrtf_sel.push_back(si);
-                    } else {
-                        float proj[3];
-                        spatial::projected_source(sp0, proj);
-                        const float dir[3] = {proj[0], proj[2], proj[1]};  // HrtfState::process swaps y / z (panner.rs:248-252)
-                        h.static_sel = HrtfSel{{0, 0, 0}, {0.f, 0.f, 0.f}, sp0.cone_gain * sp0.dist_gain, 0.f};
-                        sph->locate(dir, h.static_sel.v, h.static_sel.w);  // no face: all-zero weights (silence)
-                    }
-                    hs.hrtf.push_back(h);
-                    break;
-                }
-                if (moving) {
-                    PanDynInst d{};
-                    d.in = p.in_buf[0];
-                    d.out = p.out_buf[0];
-                    d.sp = tr;
-                    d.model = model;
-                    d.in_ch = ch;
-                    stage(L, S_PAN_DYN).pan_dyn.push_back(d);
-                    break;
-                }
-                PanInst pi{};
-                pi.in = p.in_buf[0];
-                pi.out = p.out_buf[0];
-                pi.in_ch = ch;
-                pi.azimuth = sp0.azimuth;
-                pi.dist_gain = sp0.dist_gain;
-                pi.cone_gain = sp0.cone_gain;
-                stage(L, S_PAN).pan.push_back(pi);
-                break;
-            }
-            case K_DELAY_W: {
-                p.out_ch = {p.in_ch[0]};
-                p.out_buf = {p.in_buf[0]};
-                p.out_lay = {in0};
-                if (Orderer::contains(ord.broken, id)) {
-                    // cycle breaker applied (graph.rs:458-466): the hidden writer->reader edge is gone, the reader ran
-                    // earlier in this quantum from the ring; record this quantum's input now
-                    delay_ch_seen[{gi, n.delay_peer}] = p.in_ch[0];
-                    auto it = delay_rings.find({gi, id});
-                    if (it == delay_rings.end()) return bail(WAE_UNSUPPORTED, "DelayNode writer processed before its reader inside a cycle");
-                    if (it->second.ch != p.in_ch[0]) {
-                        if (!dry) return bail(WAE_UNSUPPORTED, "channel layout of a DelayNode in a feedback cycle did not converge");
-                        break;  // sizing pass: the hint is corrected and the pass repeated
-                    }
-                    DelayInst d{};
-                    d.in = p.in_buf[0];
-                    d.ch = it->second.ch;
-                    d.ring = it->second.ring;
-                    d.ring_len = it->second.ring_len;
-                    d.mono_at = it->second.mono_at;
-                    d.mono_len = it->second.mono_len;
-                    d.dyn = it->second.mono_at ? 3 : 0;  // inside a cycle the writer runs after the reader: it extends the one-channel track
-                    stage(L, S_DELAY_WRITE).delay.push_back(d);
-                }
-                break;
-            }
-            case K_DELAY_R: {
-                PRef pdl = param_ref(g, n.params[0]);
-                float dt = pdl.v;
-                const bool in_cycle = Orderer::contains(ord.broken, n.delay_peer);
-                int ch = p.in_ch[0];
-                if (in_cycle) {
-                    ch = 1;
-                    if (delay_ch_hint) {
-                        auto it = delay_ch_hint->find({gi, id});
-                        if (it != delay_ch_hint->end()) ch = it->second;
-                    }
-                }
-                if (!need_out(ch)) return bail(WAE_OUT_OF_MEMORY, "out of device memory (arena)");
-                DelayInst d{};
-                d.in = p.in_buf[0];
-                d.out = p.out_buf[0];
-                d.ch = ch;
-                d.in_cycle = in_cycle ? 1 : 0;
-                if (pdl.dyn) d.delay_track = pdl.track;
-                d.sample_rate = g->sample_rate;
-                double delay = (double)dt;
-                if (in_cycle) delay = std::max(delay, 128. / sr);  // delay.rs:699-703: at least one quantum inside a cycle
-                double num_samples = delay * sr;               // delay.rs:706
-                double position = 0. - num_samples;            // sample_index 0
-                double pf = std::floor(position);
-                d.fl = (int64_t)pf;
-                d.k = (float)(position - pf);
-                uint64_t max_frames = (uint64_t)std::ceil(std::max(n.max_delay_time, 128. / sr) * sr) + 2;
-                d.ring_len = next_pow2(max_frames + 128);
-                d.ring = alloc<float>((size_t)ch * d.ring_len, true, true);
-                if (!d.ring) return bail(WAE_OUT_OF_MEMORY, "out of device memory (delay ring)");
-                b->arena_bytes += (size_t)ch * d.ring_len * 4;
-                if (ch <= 2) {
-                    // The reader reports a quantum without any normal sample as silent (delay.rs:654-664) and the ring follows the
-                    // channel count of the writer's input (:470-488): its output layout is never constant.  (Wider than stereo: the
-                    // static layout is kept, the re-mix of the ring is not followed.)
-                    d.dyn = 1;
-                    d.mono_len = (int32_t)next_pow2((uint64_t)(b->chunk / 128 + 2));
-                    d.mono_at = alloc<int64_t>((size_t)d.mono_len, true, true);
-                    if (!d.mono_at) return bail(WAE_OUT_OF_MEMORY, "out of device memory (delay layout track)");
-                    const Lay wl = in_cycle ? Lay{1, (uint8_t)ch, 1, (uint8_t)ch, true} : in0;
-                    out_dynamic(Lay{1, (uint8_t)ch, (uint8_t)(wl.dyn() ? 1 : ch), (uint8_t)ch, true});
-                    d.out = p.out_buf[0];
-                    if (!in_cycle) stage(L, S_DELAY_MONO).delay.push_back(d);
-                }
-                stage(L, S_DELAY).delay.push_back(d);
-                if (in_cycle) delay_rings[{gi, n.delay_peer}] = DelayRing{d.ring, d.ring_len, ch, d.mono_at, d.mono_len};
-                else stage(L, S_DELAY_WRITE).delay.push_back(d);  // acyclic: history is recorded right after the read
-                break;
-            }
-            case K_COMP: {
-                PRef cp[5];
-                for (int i = 0; i < 5; i++) cp[i] = param_ref(g, n.params[i]);
-                const float at = cp[0].v, kn = cp[1].v, ra = cp[2].v, re = cp[3].v, th = cp[4].v;
-                int ch = p.in_ch[0];
-                if (!need_out(ch)) return bail(WAE_OUT_OF_MEMORY, "out of device memory (arena)");
-                CompInst c{};
-                c.in = p.in_buf[0];
-                c.out = p.out_buf[0];
-                c.ch = ch;
-                int ring_size = (int)std::ceil(g->sample_rate * 0.006f / 128.f) + 1;  // dynamics_compressor.rs:250-255
-                c.delay_frames = (ring_size - 1) * 128;
-                c.ring_len = next_pow2((uint64_t)c.delay_frames + 128);
-                c.ring = alloc<float>((size_t)ch * c.ring_len, true, true);
-                c.state = alloc<float>(2, true, true);
-                c.meta_ring = alloc<uint8_t>(8, true, true);
-                if (!c.ring || !c.state || !c.meta_ring) return bail(WAE_OUT_OF_MEMORY, "out of device memory (compressor)");
-                // the look-ahead ring starts out silent and hands on the layout of the quantum it delays (dynamics_compressor.rs:340-349,452-468)
-                out_dynamic(Lay{1, in0.hi, in0.nlo, in0.nhi, true});
-                c.out = p.out_buf[0];
-                c.threshold = th; c.knee = kn; c.ratio = ra; c.attack = at; c.release = re;
-                for (int i = 0; i < 5; i++) c.track[i] = cp[i].dyn ? cp[i].track : BufRef{nullptr, 0, 0};
-                c.sample_rate = g->sample_rate;
-                c.end = glq;
-                stage(L, S_COMP).comp.push_back(c);
-                if (!dry) {
-                    std::lock_guard<std::recursive_mutex> lk(b->mu);  // (groups are planned on worker threads)
-                    bool known = false;
-                    for (auto& r : b->compressors) known = known || (r.graph == gi && r.node == id);
-                    if (!known) b->compressors.push_back(wae_batch::CompRec{gi, id, c.state});
-                }
-                break;
-            }
-            case K_ANALYSER: {
-                int ch = p.in_ch[0];
-                // pass-through (analyser.rs:267-294): the output IS the input buffer (nobody writes an edge buffer after its
-                // producer), only the ring is written
-                p.out_ch = {ch};
-                p.out_buf = {p.in_buf[0]};
-                p.out_lay = {in0};
-                AnalyserInst a{};
-                a.in = p.in_buf[0];
-                a.out = BufRef{nullptr, 0, 0};
-                a.ch = ch;
-                a.end = glq;
-                a.ring = alloc<float>(32768 + 128, true, true);
-                if (!a.ring) return bail(WAE_OUT_OF_MEMORY, "out of device memory (analyser ring)");
-                stage(L, S_ANALYSER).analyser.push_back(a);
-                {
-                    float* last = alloc<float>(16384, true, true);
-                    float* db = alloc<float>(16384);
-                    if (!last || !db) return bail(WAE_OUT_OF_MEMORY, "out of device memory (analyser)");
-                    if (!dry) {
-                        std::lock_guard<std::recursive_mutex> lk(b->mu);
-                        bool known = false;
-                        for (auto& r : b->analysers) known = known || (r.graph_index == gi && r.node == id);
-                        if (!known) b->analysers.push_back(AnalyserRec{gi, id, a.ring, n.fft_size, n.smoothing, last, db, false, n.min_db, n.max_db, glq});
-                    }
-                }
-                algorithmic_bytes += (uint64_t)lq * 4;  // ring write, SURVEY §8(d)
-                break;
-            }
-            case K_MERGER: {
-                int k = n.n_inputs;
-                if (!need_out(k)) return bail(WAE_OUT_OF_MEMORY, "out of device memory (arena)");
-                {
-                    // `k` channels as soon as one input is not silent, else silent (channel_merger.rs:160-168)
-                    bool some_always_on = false, any_dyn = false;
-                    for (int i = 0; i < k; i++) {
-                        some_always_on = some_always_on || !p.in_lay[i].may_silent;
-                        any_dyn = any_dyn || p.in_lay[i].dyn();
-                    }
-                    if (any_dyn && !some_always_on) {
-                        out_dynamic(Lay{1, (uint8_t)k, (uint8_t)k, (uint8_t)k, true});
-                        if (p.out_buf[0].meta) {
-                            MetaInst m{};
-                            m.out = p.out_buf[0];
-                            m.mode = META_MERGE;
-                            m.out_ch = k;
-                            m.count = k;
-                            m.n_more = k;
-                            m.more = upload(p.in_buf);
-                            if (!m.more) return bail(WAE_OUT_OF_MEMORY, "out of device memory (merger inputs)");
-                            stage(L, S_META).meta.push_back(m);
-                        }
-                    }
-                }
-                for (int i = 0; i < k; i++) stage(L, S_ROUTE).route.push_back(RouteInst{p.in_buf[i], p.out_buf[0], 0, i, 0, 1});
-                break;
-            }
-            case K_SPLITTER: {
-                int k = n.n_outputs;
-                p.out_ch.assign(k, 1);
-                p.out_buf.resize(k);
-                p.out_lay.assign(k, Lay::fixed(1));
-                for (int i = 0; i < k; i++) {
-                    if (i < p.in_ch[0] && in0.dyn()) {  // channel i exists only in some quanta: copy it, zeros elsewhere, own layout track
-                        p.out_buf[i] = arena_buf(1, true);
-                        if (!p.out_buf[i].p) return bail(WAE_OUT_OF_MEMORY, "out of device memory (arena)");
-                        p.out_lay[i] = Lay{1, 1, 1, 1, true};
-                        stage(L, S_ROUTE).route.push_back(RouteInst{p.in_buf[0], p.out_buf[i], i, 0, 0, p.in_ch[0]});
-                        meta_stage(L, META_SPLIT, p.in_buf[0], p.in_ch[0], p.out_buf[i], 1, 0, i);
-                    } else if (i < p.in_ch[0]) {  // alias channel i of the input
-                        BufRef r = p.in_buf[0];
-                        r.p += (size_t)i * r.stride;
-                        p.out_buf[i] = r;
-                    } else {
-                        p.out_buf[i] = arena_buf(1);
-                        stage(L, S_ROUTE).route.push_back(RouteInst{p.in_buf[0], p.out_buf[i], 0, 0, 1, 0});
-                    }
-                }
-                break;
-            }
-            case K_CONV: {
-                // the destination's only input (and this node's only consumer): the inverse transforms write the rendered PCM
-                const BufRef* dest = nullptr;
-                const BufRef fin = dest_ref(g, gi);
-                if (fuse && cur_cls == 0 && g->length <= 0xffffffffull) {
-                    int n_out = 0;
-                    uint32_t to = 0;
-                    int to_port = -1;
-                    for (auto& e : ord.edges.at(id))
-                        if (e.other_index >= 0) n_out++, to = e.other_id, to_port = e.other_index;
-                    if (n_out == 1 && to_port == 0 && g->nodes.at(to).kind == K_DEST && pn.at(to).in_edges[0].size() == 1 &&
-                        computed_channels(g->nodes.at(to).cfg, (n.buffer && n.buffer->channels.size() == 1 && p.in_ch[0] == 1) ? 1 : 2) == (int)g->channels)
-                        dest = &fin;
-                }
-                if (!plan_convolver(g, p, L, dest, (int64_t)g->length)) return false;
-                break;
-            }
+            case K_DEST: ok = lower_dest(nc); break;
+            case K_OSC: ok = lower_osc(nc); break;
+            case K_CONST: ok = lower_const(nc); break;
+            case K_ABSN: ok = lower_absn(nc); break;
+            case K_BIQUAD: ok = lower_biquad(nc); break;
+            case K_IIR: ok = lower_iir(nc); break;
+            case K_GAIN: ok = lower_gain(nc); break;
+            case K_SHAPER: ok = lower_shaper(nc); break;
+            case K_SPANNER: ok = lower_stereo_panner(nc); break;
+            case K_PANNER: ok = lower_panner(nc); break;
+            case K_DELAY_W: ok = lower_delay_writer(nc); break;
+            case K_DELAY_R: ok = lower_delay_reader(nc); break;
+            case K_COMP: ok = lower_compressor(nc); break;
+            case K_ANALYSER: ok = lower_analyser(nc); break;
+            case K_MERGER: ok = lower_merger(nc); break;
+            case K_SPLITTER: ok = lower_splitter(nc); break;
+            case K_CONV: ok = lower_convolver(nc); break;
             default: return bail(WAE_UNSUPPORTED, "node kind not lowered to the GPU");
         }
+        if (!ok) return false;
     }
     // chains whose single consumer never showed up as an audio input (e.g. it feeds an AudioParam): materialise
     while (!pending.empty())
@@ -3044,6 +3223,11 @@ struct PrepState {
     uint64_t algorithmic_bytes = 0;
     std::chrono::steady_clock::time_point t0, t1;
 };
+Planner::Planner(wae_batch* b_, const wae_batch::Group& grp, PrepState& ps, std::vector<wae_batch::Group::SrcCopy>* sizing_copies)
+    : b(b_), eng(b_->engine), delay_ch_hint(&ps.delay_ch_hint), dry(sizing_copies != nullptr), group_graphs((int)(grp.g1 - grp.g0)),
+      d_src(dry ? reinterpret_cast<float*>(uintptr_t(256)) : grp.d_src), src_copies(sizing_copies), lq(grp.lq) {
+    if (!dry) ir_cache = &ps.ir_cache;
+}
 struct GroupPlan {  // result of phase B for one group
     std::vector<Stage> stages;
     std::vector<std::pair<size_t, size_t>> seg_ranges;  // per segment: [first, last) into `stages`
@@ -3235,13 +3419,7 @@ static wae_status prep_begin(wae_engine* eng, wae_graph* const* graphs, uint32_t
         // `cursor0`: where the run starts in the slab — 0 while that is not known yet (the sizing pass proper: rebased by the merge), the
         // recorded base of graph i0 once it is (the planning pass and the self-check of the merged stage builds)
         auto size_range = [&](int k, uint32_t i0, uint32_t i1, RangeOut& ro, size_t cursor0) {  // single-segment groups only
-            Planner sizing{b, eng};
-            sizing.dry = true;
-            sizing.group_graphs = (int)(b->groups[k].g1 - b->groups[k].g0);
-            sizing.lq = b->groups[k].lq;
-            sizing.delay_ch_hint = &ps.delay_ch_hint;
-            sizing.d_src = reinterpret_cast<float*>(uintptr_t(256));
-            sizing.src_copies = &ro.copies;
+            Planner sizing(b, b->groups[k], ps, &ro.copies);
             sizing.src_cursor = cursor0;
             sizing.begin_segment(0, b->groups[k].lq);
             for (uint32_t i = i0; i < i1; i++) {
@@ -3313,15 +3491,9 @@ static wae_status prep_begin(wae_engine* eng, wae_graph* const* graphs, uint32_t
                 so[k].delay_ch_seen = std::move(out.delay_ch_seen);
                 return;
             }
-            Planner sizing{b, eng};
-            sizing.dry = true;
-            sizing.group_graphs = (int)n_in_group;
-            sizing.lq = b->groups[k].lq;
-            sizing.delay_ch_hint = &ps.delay_ch_hint;
-            sizing.d_src = reinterpret_cast<float*>(uintptr_t(256));
             b->groups[k].src_copies.clear();
             b->groups[k].graph_src_base.clear();
-            sizing.src_copies = &b->groups[k].src_copies;
+            Planner sizing(b, b->groups[k], ps, &b->groups[k].src_copies);
             const std::vector<int64_t>& bounds = b->groups[k].seg_bounds;
             uint64_t serial_digest = 0;
             for (size_t sg = 0; sg + 1 < bounds.size(); sg++) {
@@ -3472,13 +3644,7 @@ static wae_status prep_begin(wae_engine* eng, wae_graph* const* graphs, uint32_t
 static void prep_plan_group(wae_batch* b, wae_graph* const* graphs, int k, PrepState& ps, GroupPlan& gp) {
     wae_engine* eng = b->engine;
     wae_batch::Group& grp = b->groups[k];
-    Planner pl{b, eng};
-    pl.d_src = grp.d_src;
-    pl.group_graphs = (int)(grp.g1 - grp.g0);
-    pl.lq = grp.lq;
-    pl.src_copies = nullptr;  // recorded by the sizing pass
-    pl.delay_ch_hint = &ps.delay_ch_hint;
-    pl.ir_cache = &ps.ir_cache;
+    Planner pl(b, grp, ps, nullptr);  // (the source copies are recorded by the sizing pass)
     auto oom = [&](const char* what) {
         gp.code = WAE_OUT_OF_MEMORY;
         gp.error = std::string("out of device memory (") + what + ")";
@@ -3513,13 +3679,7 @@ static void prep_plan_group(wae_batch* b, wae_graph* const* graphs, int k, PrepS
             const uint32_t n = grp.g1 - grp.g0;
             eng->workers()->parallel_for(split_parts, [&](int t) {
                 const uint32_t i0 = (uint32_t)((uint64_t)n * t / split_parts), i1 = (uint32_t)((uint64_t)n * (t + 1) / split_parts);
-                Planner rp{b, eng};
-                rp.d_src = grp.d_src;
-                rp.group_graphs = (int)n;
-                rp.lq = grp.lq;
-                rp.src_copies = nullptr;
-                rp.delay_ch_hint = &ps.delay_ch_hint;
-                rp.ir_cache = &ps.ir_cache;
+                Planner rp(b, grp, ps, nullptr);
                 rp.src_cursor = grp.graph_src_base[i0];
                 rp.begin_segment(grp.seg_bounds[sg], grp.seg_bounds[sg + 1]);
                 for (uint32_t i = grp.g0 + i0; i < grp.g0 + i1; i++) {
