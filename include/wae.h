@@ -494,6 +494,38 @@ WAE_API wae_status wae_batch_plan_many(wae_graph* const* graphs, uint32_t n_grap
  * to its group's length); *needed = the sum over graphs of ceil(length_i / 128). */
 WAE_API wae_status wae_batch_plan_quanta(wae_graph* const* graphs, uint32_t n_graphs, uint32_t* group_of, uint64_t* rendered, uint64_t* needed);
 
+/* ---- source audio bound from device memory ---------------------------------------------------------------------------------
+ * A prepared batch renders the PCM its graphs were built with; the calls below let it render new audio that already lives on the GPU
+ * (decoded, augmented or generated there) without building, planning or uploading anything again: declare the source at build time,
+ * prepare once, then any number of times bind new device audio, run, and read the output on the device (wae_batch_output_device_ptr).
+ * wae_render_batch and wae_render_many answer WAE_INVALID_STATE on graphs with device inputs (a one-shot call leaves no point to bind
+ * at); wae_batch_plan / wae_batch_plan_many plan them as usual. */
+
+/* An AudioBufferSourceNode whose PCM is supplied per run from device memory (wae_batch_bind_sources) instead of an AudioBuffer.
+ * Counts as the node's buffer: the node then behaves exactly like one given an AudioBuffer of this shape.  Same validation and texts
+ * as AudioBuffer::new (channels 1..32, length > 0), same "cannot assign buffer twice" rule as set_buffer, in both directions. */
+WAE_API wae_status wae_buffer_source_set_device_input(wae_graph* graph, wae_node_id node, uint32_t number_of_channels,
+                                                      uint64_t length, float sample_rate);
+
+typedef struct wae_source_binding {
+    uint32_t graph_index;    /* caller's index, as wae_batch_fetch_graph (also for wae_batch_prepare_many batches) */
+    wae_node_id node;        /* a node declared with wae_buffer_source_set_device_input */
+    const float* pcm;        /* device memory on the engine's GPU: channel c is `length` floats at pcm + c * channel_stride */
+    uint64_t channel_stride; /* floats, >= the declared length; any alignment */
+} wae_source_binding;
+
+/* Copies the audio into the batch's source slab, asynchronously on the engine stream, after the work already queued on `stream`
+ * (a cudaStream_t of the engine's device, or cudaStreamLegacy for the legacy default stream, or cudaStreamPerThread; NULL = no extra
+ * ordering: the engine stream is non-blocking and does NOT wait for the legacy default stream by itself).  All-or-nothing: every item
+ * is validated before anything is enqueued.  Bound audio stays until it is bound again; runs never alter it.  A device input that is
+ * never started renders silence and reads nothing: binding it is validated and copies nothing.  WAE_INVALID_ARGUMENT: `pcm` is not
+ * device (or managed) memory of the engine's GPU, or the extent [pcm, pcm + (channels - 1) * channel_stride + length) does not lie
+ * inside one allocation, or channel_stride is below the declared length, or one (graph, node) is named twice in the call.
+ * WAE_INVALID_STATE: graph_index out of range, or the node is not a device input.
+ * wae_batch_run, wae_batch_run_group and wae_batch_run_pipelined answer WAE_INVALID_STATE while a device input of the batch has never
+ * been bound. */
+WAE_API wae_status wae_batch_bind_sources(wae_batch* batch, const wae_source_binding* items, uint32_t n, void* stream);
+
 /* PeriodicWave::new(context, PeriodicWaveOptions { real, imag, disable_normalization }) (src/periodic_wave.rs:104-209): fills `table`
  * (PERIODIC_WAVE_TABLE_LENGTH = 2048 in the reference) with the wavetable an OscillatorNode of type Custom plays.  `real` / `imag` may be
  * NULL (= zeros); both NULL = the sine default.  Host math, no engine needed. */

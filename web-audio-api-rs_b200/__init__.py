@@ -44,7 +44,7 @@ class Engine:
         h = ctypes.c_void_p()
         a.check(a.engine_create(int(device), ctypes.byref(h)))
         self.handle = h
-        self.backend = context.Backend(a, h)
+        self.backend = context.Backend(a, h, int(device))
         self.device = device
 
     def set_option(self, option, value):

@@ -118,6 +118,11 @@ class BatchStats(C.Structure):
                 ("dominant_kernel", C.c_char * 64)]
 
 
+class SourceBinding(C.Structure):
+    """wae_source_binding: device audio for one device input of a prepared batch (wae_batch_bind_sources)."""
+    _fields_ = [("graph_index", C.c_uint32), ("node", C.c_uint32), ("pcm", c_float_p), ("channel_stride", C.c_uint64)]
+
+
 STATUS_NAMES = {0: "OK", 1: "INVALID_ARGUMENT", 2: "INVALID_STATE", 3: "NOT_SUPPORTED", 4: "UNSUPPORTED",
                 5: "CUDA_ERROR", 6: "OUT_OF_MEMORY", 7: "NO_DEVICE"}
 
@@ -156,6 +161,7 @@ WAE_SYMBOLS = [
     "wae_node_set_channel_count", "wae_node_set_channel_count_mode", "wae_node_set_channel_interpretation", "wae_graph_render_order", "wae_hrir_resample", "wae_batch_plan", "wae_buffer_source_set_buffer", "wae_convolver_set_buffer", "wae_wave_shaper_set_curve",
     "wae_oscillator_set_periodic_wave", "wae_node_set_attribute", "wae_disconnect_from", "wae_disconnect_param", "wae_periodic_wave_table", "wae_param_sim_set_walker", "wae_sched_first_frame_at_or_after", "wae_spatial_params", "wae_hrtf_locate",
     "wae_render_many", "wae_batch_prepare_many", "wae_batch_graph_output", "wae_batch_fetch_graph", "wae_batch_plan_many", "wae_batch_plan_quanta",
+    "wae_buffer_source_set_device_input", "wae_batch_bind_sources",
 ]
 
 
@@ -256,6 +262,9 @@ class Api:
             f("batch_fetch_graph", C.c_int32, [C.c_void_p, C.c_uint32, c_float_p])
             f("batch_plan_many", C.c_int32, [C.POINTER(C.c_void_p), C.c_uint32, C.POINTER(PlanInfo)])
             f("batch_plan_quanta", C.c_int32, [C.POINTER(C.c_void_p), C.c_uint32, C.POINTER(C.c_uint32), C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)])
+            # source audio bound from device memory
+            f("buffer_source_set_device_input", C.c_int32, [gp, C.c_uint32, C.c_uint32, C.c_uint64, C.c_float])
+            f("batch_bind_sources", C.c_int32, [C.c_void_p, C.POINTER(SourceBinding), C.c_uint32, C.c_void_p])
         else:
             f("graph_create", C.c_int32, [C.c_uint32, C.c_uint64, C.c_float, C.POINTER(C.c_void_p)])
             f("render", C.c_int32, [gp, c_float_p])

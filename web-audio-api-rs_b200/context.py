@@ -33,10 +33,11 @@ OVERSAMPLE_NONE, OVERSAMPLE_X2, OVERSAMPLE_X4 = range(3)
 class Backend:
     """An Api plus (for the product) an engine handle."""
 
-    def __init__(self, api, engine=None):
+    def __init__(self, api, engine=None, device=0):
         import weakref
         self.api = api
         self.engine = engine
+        self.device = device  # CUDA device ordinal of the engine
         self.batches = weakref.WeakSet()  # live wae_batch handles: destroyed before their engine (Engine.close)
         self.closed = False
 
@@ -255,6 +256,15 @@ class AudioBufferSourceNode(AudioScheduledSourceNode):
     def set_buffer(self, buffer):
         self._set_buffer("buffer_source_set_buffer", buffer)
 
+    def set_device_input(self, number_of_channels, length, sample_rate):
+        """wae_buffer_source_set_device_input (product only): the node plays audio of this shape that Batch.bind_sources supplies from
+        device memory before each run, instead of an AudioBuffer.  Counts as the node's buffer."""
+        api = self._ctx._api
+        if not api.is_product:
+            raise B.WaeError(3, "device inputs are a feature of the GPU engine")
+        api.check(api.buffer_source_set_device_input(self._ctx._g, self.id, int(number_of_channels), int(length), float(sample_rate)))
+        self._ctx._device_inputs[self.id] = (int(number_of_channels), int(length))
+
     def set_loop(self, value):
         self._set_attribute(B.ATTR_LOOP, 1.0 if value else 0.0)
 
@@ -429,6 +439,7 @@ class OfflineAudioContext:
         self._listener = None
         self._suspends = []
         self._current_time = 0.0
+        self._device_inputs = {}  # node id -> (channels, length) declared with set_device_input
 
     def __del__(self):
         try:
@@ -645,12 +656,15 @@ class Batch:
         prepare = self.api.batch_prepare_many if many else self.api.batch_prepare
         self.api.check(prepare(ctx0._backend.engine, arr, self.n, C.byref(h)))
         self.handle = h
+        self._guard = None  # bind_sources: torch stream the bound tensors are recorded on
+        self._views_out = False  # output_tensor was called: runs are ordered after torch's current stream
         self._backend = ctx0._backend
         self._backend.batches.add(self)
         for i, c in enumerate(contexts):
             c._batch, c._batch_index = self, i
 
     def run(self):
+        self._after_torch_readers()
         self.api.check(self.api.batch_run(self.handle))
 
     def upload(self):
@@ -675,10 +689,12 @@ class Batch:
 
     def run_group(self, k):
         """render of ONE graph group, asynchronous on the engine stream (call the groups in order)"""
+        self._after_torch_readers()
         self.api.check(self.api.batch_run_group(self.handle, k))
 
     def run_pipelined(self, host_out_ptr):
         """H2D + render + D2H, overlapped per graph group; `host_out_ptr` = address of [n][ch][length] f32 (pinned)."""
+        self._after_torch_readers()
         self.api.check(self.api.batch_run_pipelined(self.handle, host_out_ptr))
 
     def fetch(self, out=None):
@@ -706,6 +722,89 @@ class Batch:
         p, n = C.c_void_p(), C.c_uint64()
         self.api.check(self.api.batch_output_device_ptr(self.handle, C.byref(p), C.byref(n)))
         return p.value, n.value
+
+    def _engine_stream(self):
+        import torch
+        p = C.c_void_p()
+        self.api.check(self.api.engine_stream(self._backend.engine, C.byref(p)))
+        return torch.cuda.ExternalStream(p.value or 0, device=self._device())
+
+    def _device(self):
+        import torch
+        return torch.device("cuda", self._backend.device)
+
+    def _torch_stream_handle(self):
+        """cudaStream_t of torch's current stream.  torch reports its default stream, the legacy NULL stream, as 0, which the library
+        reads as 'no ordering' (and the non-blocking engine stream does not wait for the legacy stream by itself): cudaStreamLegacy."""
+        import torch
+        return torch.cuda.current_stream(self._device()).cuda_stream or 1  # 1 = cudaStreamLegacy
+
+    def _after_torch_readers(self):
+        """A run overwrites the device output: once output_tensor views were handed out, order it after the work torch has queued so far
+        on its current stream (the readers of the last output)."""
+        if self._views_out:
+            import torch
+            self._engine_stream().wait_stream(torch.cuda.current_stream(self._device()))
+
+    def bind_sources(self, nodes, pcm, graphs=None):
+        """wae_batch_bind_sources: pcm[k] ([channels][length] of a float32 CUDA tensor [n][channels][length], unit stride on the last
+        dimension) becomes the audio of device input nodes[k] of context graphs[k] (default: 0..n-1).  `nodes`: one node (or id) for all
+        graphs (graphs built the same way share ids) or one per graph.  One call, ordered after torch's current stream (its default
+        stream included); the copy runs on the engine stream, and the tensor's memory is kept from reuse until it has (record_stream)."""
+        import torch
+        if not (isinstance(pcm, torch.Tensor) and pcm.is_cuda and pcm.dtype == torch.float32 and pcm.dim() == 3):
+            raise B.WaeError(1, "bind_sources: pcm must be a float32 CUDA tensor [n][channels][length]")
+        n = pcm.shape[0]
+        graphs = list(range(n)) if graphs is None else [int(g) for g in graphs]
+        if isinstance(nodes, (list, tuple)):
+            ids = [getattr(x, "id", x) for x in nodes]
+        else:
+            ids = [getattr(nodes, "id", nodes)] * n
+        if len(graphs) != n or len(ids) != n:
+            raise B.WaeError(1, f"bind_sources: {n} tensors for {len(graphs)} graphs and {len(ids)} nodes")
+        if n and pcm.stride(2) != 1:
+            raise B.WaeError(1, "bind_sources: the frames of a channel must be contiguous (unit stride on the last dimension)")
+        items = (B.SourceBinding * max(n, 1))()
+        base = pcm.data_ptr()
+        # (torch may give the channel dimension of a one-channel tensor any stride: only channel 0 is read then)
+        channel_stride = pcm.stride(1) if pcm.shape[1] > 1 else pcm.shape[2]
+        for k, (g, nid) in enumerate(zip(graphs, ids)):
+            if not 0 <= g < self.n:
+                raise B.WaeError(2, f"bind_sources: graph index {g} is out of range")
+            declared = self.contexts[g]._device_inputs.get(int(nid))
+            # the library checks the CUDA allocation; torch's caching allocator may hold several tensors in one, so the tensor's own
+            # shape is checked here
+            if declared is not None and (pcm.shape[1], pcm.shape[2]) != declared:
+                raise B.WaeError(1, f"bind_sources: pcm[{k}] is [{pcm.shape[1]}][{pcm.shape[2]}], node {nid} of graph {g} was declared "
+                                    f"[{declared[0]}][{declared[1]}]")
+            items[k] = B.SourceBinding(g, int(nid), C.cast(C.c_void_p(base + 4 * k * pcm.stride(0)), B.c_float_p), channel_stride)
+        self.api.check(self.api.batch_bind_sources(self.handle, items, n, C.c_void_p(self._torch_stream_handle())))
+        # keep torch's caching allocator from reusing the memory before the copy has run.  The tensor is recorded on a torch-owned stream
+        # that waits for the engine stream, not on the engine stream itself: the allocator records an event on that stream whenever the
+        # tensor is freed, which may be after the engine (and its stream) are gone
+        if self._guard is None:
+            self._guard = torch.cuda.Stream(device=self._device())
+        self._guard.wait_stream(self._engine_stream())
+        pcm.record_stream(self._guard)
+
+    def output_tensor(self, i=None):
+        """Zero-copy torch view of the rendered output on the device: [n][channels][length] for a batch of one shape, [channels_i][length_i]
+        of context i.  The view keeps the batch alive; torch's current stream is made to wait for the engine stream first, and later
+        runs of the batch (which overwrite the view) wait for the work then queued on torch's current stream."""
+        import torch
+        base, _ = self.device_ptr()
+        if i is None:
+            shapes = {(c._channels, c._length) for c in self.contexts}
+            if len(shapes) != 1:
+                raise B.WaeError(2, "output_tensor: the contexts of this batch differ in shape; view one with output_tensor(i)")
+            off, shape = 0, (self.n, self.channels, self.length)
+        else:
+            off, ch, length = self.graph_output(i)
+            shape = (ch, length)
+        view = torch.as_tensor(_DeviceView(self, base + 4 * off, shape), device=self._device())
+        self._views_out = True
+        torch.cuda.current_stream(self._device()).wait_stream(self._engine_stream())
+        return view
 
     def stats(self):
         s = B.BatchStats()
@@ -735,6 +834,16 @@ class Batch:
             self.destroy()
         except Exception:
             pass
+
+
+class _DeviceView:
+    """__cuda_array_interface__ of a float32 range of a batch's device output; torch.as_tensor keeps this object, and so the batch,
+    alive as long as the tensor."""
+
+    def __init__(self, batch, ptr, shape):
+        self.batch = batch
+        self.__cuda_array_interface__ = {"shape": tuple(int(s) for s in shape), "typestr": "<f4", "data": (int(ptr), False),
+                                         "version": 2}
 
 
 def plan_batch(contexts):

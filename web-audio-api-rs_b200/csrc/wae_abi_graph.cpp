@@ -971,20 +971,46 @@ Node* node_of_kind(wae_graph* g, wae_node_id id, Kind kind) {
 }
 }  // namespace
 
+// "if start called and buffer is null, should fire ended event and ignore any subsequent buffer assignment"
+// (audio_buffer_source.rs:443-451): a source that was started before the last suspend point and has been rendered without a
+// buffer since has ended for good
+static void end_if_started_without_buffer(wae_graph* g, wae_node_id node, Node* n) {
+    if (g->epochs.empty()) return;
+    const auto& before = g->epochs.back().nodes;
+    auto pi = before.find(node);
+    if (pi != before.end() && pi->second.has_start && !pi->second.buffer) n->start_time = 1.7976931348623157e308;
+}
+
 // AudioBufferSourceNode::set_buffer (src/node/audio_buffer_source.rs:278-288): once
 WAE_API wae_status wae_buffer_source_set_buffer(wae_graph* g, wae_node_id node, const wae_audio_buffer* buffer) {
     Node* n = node_of_kind(g, node, K_ABSN);
     if (!n || !buffer) return fail(WAE_INVALID_ARGUMENT, "not an AudioBufferSourceNode / null buffer");
     if (n->buffer) return fail(WAE_INVALID_STATE, "InvalidStateError - cannot assign buffer twice");
     if (!(n->buffer = copy_buffer(g, buffer, true))) return WAE_NOT_SUPPORTED;
-    // "if start called and buffer is null, should fire ended event and ignore any subsequent buffer assignment"
-    // (audio_buffer_source.rs:443-451): a source that was started before the last suspend point and has been rendered without a
-    // buffer since has ended for good
-    if (!g->epochs.empty()) {
-        const auto& before = g->epochs.back().nodes;
-        auto pi = before.find(node);
-        if (pi != before.end() && pi->second.has_start && !pi->second.buffer) n->start_time = 1.7976931348623157e308;
-    }
+    end_if_started_without_buffer(g, node, n);
+    return WAE_OK;
+}
+
+// A device input counts as the node's buffer: the placeholder has the declared shape and rate and no host block.  It is not entered in
+// g->assets, so content sharing never merges two device inputs; each gets its own slot in the group's source slab.
+WAE_API wae_status wae_buffer_source_set_device_input(wae_graph* g, wae_node_id node, uint32_t number_of_channels, uint64_t length,
+                                                      float sample_rate) {
+    Node* n = node_of_kind(g, node, K_ABSN);
+    if (!n) return fail(WAE_INVALID_ARGUMENT, "not an AudioBufferSourceNode");
+    // AudioBuffer::new (src/buffer.rs:96-115), as copy_buffer checks it
+    if (number_of_channels < 1 || number_of_channels > WAE_MAX_CHANNELS)
+        return fail(WAE_NOT_SUPPORTED, "NotSupportedError - Invalid number of channels: " + std::to_string(number_of_channels) + " is outside range [1, 32]");
+    if (length == 0) return fail(WAE_NOT_SUPPORTED, "NotSupportedError - Invalid length: 0 is less than or equal to minimum bound (0)");
+    if (n->buffer) return fail(WAE_INVALID_STATE, "InvalidStateError - cannot assign buffer twice");
+    auto p = std::make_shared<PcmBuffer>();
+    p->sample_rate = sample_rate;
+    p->device_input = true;
+    p->stride = (size_t)(length + 3) / 4 * 4;
+    p->channels.resize(number_of_channels);
+    for (auto& c : p->channels) c.n = (size_t)length;
+    n->buffer = std::move(p);
+    g->device_inputs++;
+    end_if_started_without_buffer(g, node, n);
     return WAE_OK;
 }
 

@@ -510,4 +510,15 @@ struct ConvCmpInst {
     int32_t pad;
 };
 
+// ---- wae_batch_bind_sources: device audio -> a device-input slot of a group's source slab --------------------------------------
+struct BindItem {
+    float* dst;          // the slot: [channels][stride], 16 B aligned (slab offsets are multiples of 4 floats)
+    const float* src;    // caller's device audio: channel c is `len` floats at src + c * src_stride (any alignment)
+    int64_t stride;      // slot channel stride, floats (len rounded up to 4; [len, stride) is written as zeros)
+    int64_t src_stride;  // floats
+    int64_t len;
+    int32_t channels;
+    int32_t pad;
+};
+
 }  // namespace wae

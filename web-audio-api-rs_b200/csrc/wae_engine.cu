@@ -13,6 +13,7 @@
 #include "wae_param_core.h"
 #include "wae_param_host.h"
 
+#include <cuda.h>  // (types of cuMemGetAddressRange only: it is reached through cudaGetDriverEntryPoint)
 #include <cuda_runtime.h>
 #include <emmintrin.h>
 
@@ -369,13 +370,42 @@ struct wae_batch {
         struct SrcCopy {                // the PCM of one AudioBufferSourceNode inside the slab: planar [ch][stride], as PcmBuffer holds it
             std::shared_ptr<PcmBuffer> buf;
             size_t offset, floats;      // floats
+            uint32_t graph;             // (batch position) and node of its first user: names a device input (buf->device_input)
+            wae_node_id node;
         };
-        std::vector<SrcCopy> src_copies;
+        std::vector<SrcCopy> src_copies;  // device inputs included: every path that copies host PCM skips them
+        bool has_device_inputs = false;
         std::vector<size_t> graph_src_base;  // groups without suspend points: the slab cursor each graph starts at (split planning)
         size_t src_floats = 0;
         cudaEvent_t ev_h2d = nullptr, ev_done = nullptr;
     };
     std::vector<Group> groups;
+    // wae_buffer_source_set_device_input: the slot of each device input in its group's slab, filled by wae_batch_bind_sources
+    struct DevInput {
+        uint32_t graph;  // batch position
+        wae_node_id node;
+        float* slot;     // [channels][stride]
+        uint32_t channels;
+        uint64_t length, stride;
+        bool bound;
+    };
+    std::vector<DevInput> dev_inputs;
+    std::map<std::pair<uint32_t, wae_node_id>, size_t> dev_index;  // (batch position, node) -> dev_inputs
+    size_t dev_unbound = 0;
+    // The item table of a bind is staged in page-locked memory (a copy from pageable memory would wait for the engine stream first) and
+    // copied to d_bind, which the next bind may overwrite at once (its copy is queued behind this bind's kernel on the same stream).  A
+    // staging buffer is reused once its copy has run (its event has completed); while all are in flight a new one is made, so a bind
+    // does not wait on the host for runs queued before it (up to kMaxBindStages staging buffers; then the bind waits for the first one that fits).
+    struct BindStage {
+        BindItem* h;
+        size_t cap;
+        cudaEvent_t ev;  // the copy out of `h`
+    };
+    static constexpr size_t kMaxBindStages = 8;
+    std::vector<BindStage> bind_stages;
+    BindItem* d_bind = nullptr;
+    size_t bind_cap = 0;
+    cudaEvent_t ev_bind = nullptr;  // orders a bind after the caller's stream
     // OfflineAudioContext::suspend_sync: a group's render is cut at the suspend frames of its graphs (graphs with different
     // suspend points are put in different groups); every segment has its own plan, node state is shared between the plans
     // through `state_map` (graph, node, allocation sequence, salt)
@@ -2044,7 +2074,7 @@ bool Planner::lower_absn(NodeCtx& nc) {
     float* d_buf = d_src + so->second;
     if (first_use) {
         if (src_copies)  // recorded by the sizing pass: uploaded straight from the graph's buffer, planar [ch][stride] like the slab
-            src_copies->push_back(wae_batch::Group::SrcCopy{n.buffer, src_cursor, (size_t)ch * stride});
+            src_copies->push_back(wae_batch::Group::SrcCopy{n.buffer, src_cursor, (size_t)ch * stride, gi, nc.id});
         src_cursor += (size_t)ch * stride;
         b->asset_bytes += (size_t)ch * len * 4;
     }
@@ -3194,6 +3224,8 @@ WAE_API wae_status wae_batch_destroy(wae_batch* b) {
     for (void* p : b->allocs) b->engine->dev_release(p);  // kept by the engine for the next batch (wae_engine::dev_alloc)
     if (b->ev0) cudaEventDestroy(b->ev0);
     if (b->ev1) cudaEventDestroy(b->ev1);
+    if (b->ev_bind) cudaEventDestroy(b->ev_bind);
+    for (auto& bs : b->bind_stages) cudaEventDestroy(bs.ev);  // (the staging memory is in `pinned`)
     for (auto e : b->stage_events) cudaEventDestroy(e);
     delete b;
     return WAE_OK;
@@ -3455,7 +3487,7 @@ static wae_status prep_begin(wae_engine* eng, wae_graph* const* graphs, uint32_t
                     return false;
                 }
                 const size_t rebase = known_base ? 0 : out.src_floats;
-                for (auto& c : r.copies) out.copies.push_back(wae_batch::Group::SrcCopy{c.buf, c.offset + rebase, c.floats});
+                for (auto& c : r.copies) out.copies.push_back(wae_batch::Group::SrcCopy{c.buf, c.offset + rebase, c.floats, c.graph, c.node});
                 for (size_t gb : r.graph_base) out.graph_base.push_back(gb + rebase);
                 if (plan) merge_builds(out.builds, r.builds);
                 out.fpf += r.fpf;
@@ -3838,9 +3870,53 @@ static void prep_append_group(wae_batch* b, int k, PrepState& ps, GroupPlan& gp)
 }
 
 // H2D of a group's source PCM, one copy per AudioBufferSourceNode, straight from the buffers the graphs own
+// (device inputs have no host PCM: their slots are written by wae_batch_bind_sources only)
 static wae_status enqueue_source_copies(wae_batch* b, wae_batch::Group& grp, cudaStream_t s) {
     for (auto& sc : grp.src_copies)
-        CUDA_TRY(cudaMemcpyAsync(grp.d_src + sc.offset, sc.buf->base, sc.floats * sizeof(float), cudaMemcpyHostToDevice, s));
+        if (!sc.buf->device_input)
+            CUDA_TRY(cudaMemcpyAsync(grp.d_src + sc.offset, sc.buf->base, sc.floats * sizeof(float), cudaMemcpyHostToDevice, s));
+    return WAE_OK;
+}
+
+// The device inputs of the batch (`graphs` in batch order): the slots of the planned groups, all unbound, then the declared device
+// inputs the planner gave no slot (a source that is never started renders silence without reading its buffer): binding one is
+// validated like any other and copies nothing, and runs do not wait for it — it behaves like a node given an AudioBuffer of that shape.
+static void record_device_inputs(wae_batch* b, wae_graph* const* graphs, uint32_t n_graphs) {
+    for (auto& grp : b->groups)
+        for (auto& sc : grp.src_copies)
+            if (sc.buf->device_input) {
+                grp.has_device_inputs = true;
+                b->dev_index[{sc.graph, sc.node}] = b->dev_inputs.size();
+                b->dev_inputs.push_back(wae_batch::DevInput{sc.graph, sc.node, grp.d_src + sc.offset, (uint32_t)sc.buf->channels.size(),
+                                                            (uint64_t)sc.buf->length(), (uint64_t)sc.buf->stride, false});
+            }
+    b->dev_unbound = b->dev_inputs.size();
+    for (uint32_t j = 0; j < n_graphs; j++) {
+        if (!graphs[j]->device_inputs) continue;
+        auto scan = [&](const NodeMap& nodes) {
+            for (const auto& kv : nodes) {
+                const Node& nd = kv.second;
+                if (nd.kind != K_ABSN || !nd.buffer || !nd.buffer->device_input || b->dev_index.count({j, nd.id})) continue;
+                b->dev_index[{j, nd.id}] = b->dev_inputs.size();
+                b->dev_inputs.push_back(wae_batch::DevInput{j, nd.id, nullptr, (uint32_t)nd.buffer->channels.size(), (uint64_t)nd.buffer->length(),
+                                                            (uint64_t)nd.buffer->stride, true});
+            }
+        };
+        scan(graphs[j]->nodes);
+        for (const auto& ep : graphs[j]->epochs) scan(ep.nodes);
+    }
+}
+
+// runs of a batch need every device input bound once
+static wae_status check_bound(wae_batch* b) {
+    if (!b) return fail(WAE_INVALID_ARGUMENT, "null batch");
+    if (b->dev_unbound == 0) return WAE_OK;
+    for (auto& d : b->dev_inputs)
+        if (!d.bound) {
+            const uint32_t caller = b->order.empty() ? d.graph : b->order[d.graph];
+            return fail(WAE_INVALID_STATE, "device input never bound: graph " + std::to_string(caller) + ", node " + std::to_string(d.node) +
+                                               " (wae_batch_bind_sources)");
+        }
     return WAE_OK;
 }
 
@@ -3883,6 +3959,7 @@ static wae_status prepare_impl(wae_engine* eng, wae_graph* const* graphs, uint32
     wae_batch* b = nullptr;
     wae_status st = prep_begin(eng, graphs, n_graphs, plan, &b, ps, true, order);
     if (st != WAE_OK || plan) return st;
+    record_device_inputs(b, graphs, n_graphs);
     const int n_groups = (int)b->groups.size();
     std::vector<GroupPlan> gps(n_groups);
     WorkerPool* pool = (n_groups > 1 && n_graphs >= 64) ? eng->workers() : nullptr;
@@ -4040,9 +4117,10 @@ static void launch_stage(wae_batch* b, Stage& st, ChunkInfo ci) {
 
 // Groups whose source PCM is not all page-locked (graphs built without an engine, buffers below the pinning threshold) get a pinned
 // mirror of their slab, built once, when the PCM is uploaded a second time; page-locked buffers are copied from where they are.
+// Device inputs take no part: they have no host PCM, and their slots keep the bound audio.
 static bool group_sources_pinned(const wae_batch::Group& g) {
     for (auto& sc : g.src_copies)
-        if (!sc.buf->pinned) return false;
+        if (!sc.buf->device_input && !sc.buf->pinned) return false;
     return true;
 }
 static wae_status ensure_host_mirror(wae_batch* b) {
@@ -4055,14 +4133,30 @@ static wae_status ensure_host_mirror(wae_batch* b) {
         }
         b->pinned.push_back(hp);
         g.h_src = (float*)hp;
-        for (auto& sc : g.src_copies) std::memcpy(g.h_src + sc.offset, sc.buf->base, sc.floats * sizeof(float));
+        for (auto& sc : g.src_copies)
+            if (!sc.buf->device_input) std::memcpy(g.h_src + sc.offset, sc.buf->base, sc.floats * sizeof(float));
     }
     return WAE_OK;
 }
 static wae_status resend_group_sources(wae_batch* b, wae_batch::Group& g, cudaStream_t s) {
     if (!g.src_floats) return WAE_OK;
-    if (g.h_src) {
+    if (g.h_src && !g.has_device_inputs) {
         CUDA_TRY(cudaMemcpyAsync(g.d_src, g.h_src, g.src_floats * sizeof(float), cudaMemcpyHostToDevice, s));
+        return WAE_OK;
+    }
+    if (g.h_src) {  // only the host ranges of the mirror: one copy per run of consecutive host-PCM copies, device-input slots left out
+        size_t i = 0;
+        const auto& cs = g.src_copies;
+        while (i < cs.size()) {
+            if (cs[i].buf->device_input) {
+                i++;
+                continue;
+            }
+            size_t j = i + 1, end = cs[i].offset + cs[i].floats;
+            while (j < cs.size() && !cs[j].buf->device_input && cs[j].offset == end) end += cs[j++].floats;
+            CUDA_TRY(cudaMemcpyAsync(g.d_src + cs[i].offset, g.h_src + cs[i].offset, (end - cs[i].offset) * sizeof(float), cudaMemcpyHostToDevice, s));
+            i = j;
+        }
         return WAE_OK;
     }
     return enqueue_source_copies(b, g, s);
@@ -4152,7 +4246,9 @@ static wae_status begin_run(wae_batch* b) {
 }
 
 WAE_API wae_status wae_batch_run(wae_batch* b) {
-    wae_status st = begin_run(b);
+    wae_status st = check_bound(b);
+    if (st != WAE_OK) return st;
+    st = begin_run(b);
     if (st != WAE_OK) return st;
     for (auto& g : b->groups) {
         st = run_group(b, g);
@@ -4177,7 +4273,8 @@ WAE_API wae_status wae_batch_group_range(wae_batch* b, uint32_t group, uint32_t*
 }
 WAE_API wae_status wae_batch_run_group(wae_batch* b, uint32_t group) {
     if (!b || group >= b->groups.size()) return fail(WAE_INVALID_ARGUMENT, "null batch / group out of range");
-    wae_status st = WAE_OK;
+    wae_status st = check_bound(b);
+    if (st != WAE_OK) return st;
     if (group == 0) st = begin_run(b);
     else CUDA_TRY(cudaSetDevice(b->engine->device));
     if (st != WAE_OK) return st;
@@ -4225,7 +4322,140 @@ static const char* kMixedPacked = "the graphs of this batch differ in shape: the
                                   "wae_batch_fetch_graph (or render with wae_render_many)";
 WAE_API wae_status wae_batch_run_pipelined(wae_batch* b, float* host_out) {
     if (b && b->mixed) return fail(WAE_INVALID_STATE, kMixedPacked);
+    wae_status st = check_bound(b);
+    if (st != WAE_OK) return st;
     return run_pipelined(b, host_out, true);
+}
+
+// The caller's pointer must be device (or managed) memory of the engine's GPU and the whole extent must lie in ONE allocation: checked
+// on the host before anything is enqueued, so that a bad pointer never reaches the kernel.  cuMemGetAddressRange is reached through the
+// runtime's driver entry point (no link dependency on libcuda).
+static wae_status check_bind_extent(int device, const float* pcm, uint64_t extent_floats) {
+    using MemRange = CUresult(CUDAAPI*)(CUdeviceptr*, size_t*, CUdeviceptr);
+    static MemRange mem_range = [] {
+        void* fn = nullptr;
+        cudaDriverEntryPointQueryResult q = cudaDriverEntryPointSymbolNotFound;
+        if (cudaGetDriverEntryPoint("cuMemGetAddressRange", &fn, cudaEnableDefault, &q) != cudaSuccess || q != cudaDriverEntryPointSuccess) {
+            cudaGetLastError();
+            fn = nullptr;
+        }
+        return reinterpret_cast<MemRange>(fn);
+    }();
+    cudaPointerAttributes a{};
+    if (cudaPointerGetAttributes(&a, pcm) != cudaSuccess) {
+        cudaGetLastError();
+        return fail(WAE_INVALID_ARGUMENT, "bind: pcm is not device memory");
+    }
+    if (!(a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged) || a.device != device)
+        return fail(WAE_INVALID_ARGUMENT, "bind: pcm is not device (or managed) memory of the engine's GPU");
+    if (!mem_range) return fail(WAE_CUDA_ERROR, "bind: cuMemGetAddressRange is not available");
+    CUdeviceptr base = 0;
+    size_t size = 0;
+    if (mem_range(&base, &size, (CUdeviceptr)(uintptr_t)pcm) != CUDA_SUCCESS)
+        return fail(WAE_INVALID_ARGUMENT, "bind: pcm lies in no device allocation");
+    const uint64_t at = (uint64_t)((uintptr_t)pcm - (uintptr_t)base);
+    if (extent_floats > (uint64_t)size / sizeof(float) || at > (uint64_t)size - extent_floats * sizeof(float))
+        return fail(WAE_INVALID_ARGUMENT, "bind: [pcm, pcm + (channels - 1) * channel_stride + length) runs past the end of its allocation");
+    return WAE_OK;
+}
+
+WAE_API wae_status wae_batch_bind_sources(wae_batch* b, const wae_source_binding* items, uint32_t n, void* stream) {
+    if (!b || (n && !items)) return fail(WAE_INVALID_ARGUMENT, "null batch / items");
+    if (n == 0) return WAE_OK;
+    CUDA_TRY(cudaSetDevice(b->engine->device));
+    // every item is validated before anything is enqueued
+    std::vector<BindItem> table;
+    std::vector<size_t> slot_of;
+    std::vector<char> named(b->dev_inputs.size(), 0);
+    int64_t max_vec = 0;
+    int max_ch = 0;
+    for (uint32_t i = 0; i < n; i++) {
+        const wae_source_binding& it = items[i];
+        if (it.graph_index >= b->n_graphs)
+            return fail(WAE_INVALID_STATE, "bind: graph index " + std::to_string(it.graph_index) + " is out of range");
+        auto di = b->dev_index.find({b->batch_pos(it.graph_index), it.node});
+        if (di == b->dev_index.end())
+            return fail(WAE_INVALID_STATE, "bind: node " + std::to_string(it.node) + " of graph " + std::to_string(it.graph_index) +
+                                               " is not a device input (wae_buffer_source_set_device_input)");
+        const size_t k = di->second;
+        if (named[k]++)  // (two items of one launch writing one slot: which one lands would be undefined)
+            return fail(WAE_INVALID_ARGUMENT, "bind: node " + std::to_string(it.node) + " of graph " + std::to_string(it.graph_index) +
+                                                  " is named twice in one call");
+        const wae_batch::DevInput& d = b->dev_inputs[k];
+        if (!it.pcm) return fail(WAE_INVALID_ARGUMENT, "bind: null pcm");
+        if (it.channel_stride < d.length)
+            return fail(WAE_INVALID_ARGUMENT, "bind: channel_stride " + std::to_string(it.channel_stride) + " is below the declared length " +
+                                                  std::to_string(d.length));
+        if (it.channel_stride > (UINT64_MAX / 4 - d.length) / WAE_MAX_CHANNELS)
+            return fail(WAE_INVALID_ARGUMENT, "bind: channel_stride runs past the end of its allocation");
+        wae_status st = check_bind_extent(b->engine->device, it.pcm, (uint64_t)(d.channels - 1) * it.channel_stride + d.length);
+        if (st != WAE_OK) return st;
+        if (!d.slot) continue;  // declared, never rendered: nothing to copy
+        table.push_back(BindItem{d.slot, it.pcm, (int64_t)d.stride, (int64_t)it.channel_stride, (int64_t)d.length, (int32_t)d.channels, 0});
+        slot_of.push_back(k);
+        max_vec = std::max<int64_t>(max_vec, (int64_t)d.stride / 4);
+        max_ch = std::max<int>(max_ch, (int)d.channels);
+    }
+    const size_t m = table.size();
+    if (m == 0) return WAE_OK;
+    cudaStream_t s = b->engine->stream;
+    // `stream` may be any stream of the engine's device, cudaStreamLegacy (the legacy default stream, which a non-blocking engine stream
+    // does not wait for by itself) or cudaStreamPerThread
+    if (stream && (cudaStream_t)stream != s) {
+        if (!b->ev_bind) CUDA_TRY(cudaEventCreateWithFlags(&b->ev_bind, cudaEventDisableTiming));
+        CUDA_TRY(cudaEventRecord(b->ev_bind, (cudaStream_t)stream));
+        CUDA_TRY(cudaStreamWaitEvent(s, b->ev_bind, 0));
+    }
+    wae_batch::BindStage* stage = nullptr;
+    for (auto& bs : b->bind_stages) {  // a staging buffer whose copy has run
+        if (bs.cap < m) continue;
+        const cudaError_t q = cudaEventQuery(bs.ev);
+        if (q == cudaSuccess) {
+            stage = &bs;
+            break;
+        }
+        if (q != cudaErrorNotReady) return fail(WAE_CUDA_ERROR, std::string("bind: ") + cudaGetErrorString(q));
+        cudaGetLastError();  // (not ready is no error)
+    }
+    if (!stage && b->bind_stages.size() >= wae_batch::kMaxBindStages) {  // all in flight: wait for the first one that fits
+        for (auto& bs : b->bind_stages)
+            if (bs.cap >= m) {
+                CUDA_TRY(cudaEventSynchronize(bs.ev));
+                stage = &bs;
+                break;
+            }
+    }
+    if (!stage) {
+        const size_t cap = std::max<size_t>(m, 64);
+        void* hp = nullptr;
+        cudaEvent_t ev = nullptr;
+        if (cudaHostAlloc(&hp, cap * sizeof(BindItem), cudaHostAllocDefault) != cudaSuccess) {
+            cudaGetLastError();
+            return fail(WAE_OUT_OF_MEMORY, "out of memory (bind table staging)");
+        }
+        b->pinned.push_back(hp);
+        CUDA_TRY(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
+        b->bind_stages.push_back(wae_batch::BindStage{(BindItem*)hp, cap, ev});
+        stage = &b->bind_stages.back();
+    }
+    if (m > b->bind_cap) {
+        BindItem* t = b->dalloc<BindItem>(m);
+        if (!t) return fail(WAE_OUT_OF_MEMORY, "out of device memory (bind table)");
+        b->d_bind = t;
+        b->bind_cap = m;
+    }
+    std::memcpy(stage->h, table.data(), m * sizeof(BindItem));
+    CUDA_TRY(cudaMemcpyAsync(b->d_bind, stage->h, m * sizeof(BindItem), cudaMemcpyHostToDevice, s));
+    CUDA_TRY(cudaEventRecord(stage->ev, s));
+    launch_bind_sources(b->d_bind, (int)m, max_vec, max_ch, s);
+    cudaError_t le = cudaGetLastError();
+    if (le != cudaSuccess) return fail(WAE_CUDA_ERROR, std::string("bind: ") + cudaGetErrorString(le));
+    for (size_t k : slot_of)
+        if (!b->dev_inputs[k].bound) {
+            b->dev_inputs[k].bound = true;
+            b->dev_unbound--;
+        }
+    return WAE_OK;
 }
 
 WAE_API wae_status wae_batch_sync(wae_batch* b) {
@@ -4676,8 +4906,18 @@ WAE_API wae_status wae_selftest_conv_fft(float* data, uint32_t mode) {
     return WAE_OK;
 }
 
+// a one-shot call renders the graphs before a caller could bind anything to their device inputs
+static wae_status refuse_device_inputs(wae_graph* const* graphs, uint32_t n_graphs) {
+    for (uint32_t i = 0; graphs && i < n_graphs; i++)
+        if (graphs[i] && graphs[i]->device_inputs)
+            return fail(WAE_INVALID_STATE, "graph " + std::to_string(i) + " has device inputs: render it with wae_batch_prepare (or _prepare_many), "
+                                           "wae_batch_bind_sources and wae_batch_run");
+    return WAE_OK;
+}
+
 WAE_API wae_status wae_render_many(wae_engine* eng, wae_graph* const* graphs, uint32_t n_graphs, float* const* outs) {
     if (!outs) return fail(WAE_INVALID_ARGUMENT, "null output buffers");
+    if (wae_status ds = refuse_device_inputs(graphs, n_graphs)) return ds;
     ManyOrder mo;
     wae_status st = many_batch(graphs, n_graphs, mo);
     if (st != WAE_OK) return st;
@@ -4685,6 +4925,7 @@ WAE_API wae_status wae_render_many(wae_engine* eng, wae_graph* const* graphs, ui
 }
 
 WAE_API wae_status wae_render_batch(wae_engine* eng, wae_graph* const* graphs, uint32_t n_graphs, float* out, uint32_t flags) {
+    if (wae_status ds = refuse_device_inputs(graphs, n_graphs)) return ds;
     if (!(flags & WAE_RENDER_OUT_DEVICE)) return render_oneshot_host(eng, graphs, n_graphs, out);
     wae_batch* b = nullptr;
     wae_status st = wae_batch_prepare(eng, graphs, n_graphs, &b);

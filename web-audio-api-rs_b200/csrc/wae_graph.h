@@ -57,6 +57,9 @@ struct PcmBuffer {  // an AudioBuffer asset (src/buffer.rs:69-72), host copy: ON
     float* base = nullptr;
     size_t stride = 0, bytes = 0;
     bool pinned = false;
+    // wae_buffer_source_set_device_input: a placeholder of the declared shape (channels[c].n = length) with no host block; its PCM is
+    // written into the device slab by wae_batch_bind_sources, and nothing copies host memory over it
+    bool device_input = false;
     PcmBuffer() = default;
     PcmBuffer(const PcmBuffer&) = delete;
     PcmBuffer& operator=(const PcmBuffer&) = delete;
@@ -244,6 +247,7 @@ struct wae_graph {
     // AudioBuffer assets of this graph, by pin mode: a buffer handed in again (the reference clones an Arc: one `AudioBuffer` played by
     // hundreds of grains, src/buffer.rs:69-72) shares ONE host copy — and so one copy in the device slab (Planner::buf_offsets)
     std::vector<std::weak_ptr<wae::PcmBuffer>> assets[2];
+    uint32_t device_inputs = 0;  // AudioBufferSourceNodes declared with wae_buffer_source_set_device_input (never in `assets`)
 
     uint32_t create_param(uint32_t owner, float def, float mn, float mx, bool a_rate, float initial, bool send_set_value = true,
                           bool fixed_id = false, uint32_t id = 0, bool constrained = false);

@@ -4379,6 +4379,35 @@ __global__ void __launch_bounds__(256) k_resample_linear(const float* __restrict
     out[i] = __fadd_rn(__fmul_rn(1.f - k, in[prev]), __fmul_rn(k, in[next]));
 }
 
+// wae_batch_bind_sources: copies caller device audio into device-input slots of the source slabs (HBM-bound).  blockIdx.y walks the
+// items, blockIdx.z is the channel, x the slot's 16-byte vectors.  The whole slot is written, its zero padding [len, stride) included
+// (the chain kernel's LDG.128 / cp.async.bulk reads run into it), with 128-bit stores; the loads are 128-bit where the source channel
+// is 16 B aligned and scalar otherwise (torch views with odd lengths or storage offsets).
+__global__ void __launch_bounds__(256) k_bind_sources(const BindItem* __restrict__ items, int n) {
+    const int c = blockIdx.z;
+    for (int i = blockIdx.y; i < n; i += gridDim.y) {
+        const BindItem it = items[i];
+        if (c >= it.channels) continue;
+        const float* __restrict__ src = it.src + (int64_t)c * it.src_stride;
+        float4* __restrict__ dst = reinterpret_cast<float4*>(it.dst + (int64_t)c * it.stride);
+        const int64_t nvec = it.stride >> 2, full = it.len >> 2;
+        const bool vec = (reinterpret_cast<uintptr_t>(src) & 15) == 0;
+        for (int64_t v = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; v < nvec; v += (int64_t)gridDim.x * blockDim.x) {
+            float4 x;
+            if (vec && v < full) {
+                x = __ldcs(reinterpret_cast<const float4*>(src) + v);
+            } else {
+                const int64_t f = v * 4;
+                x.x = f < it.len ? __ldcs(src + f) : 0.f;
+                x.y = f + 1 < it.len ? __ldcs(src + f + 1) : 0.f;
+                x.z = f + 2 < it.len ? __ldcs(src + f + 2) : 0.f;
+                x.w = f + 3 < it.len ? __ldcs(src + f + 3) : 0.f;
+            }
+            dst[v] = x;
+        }
+    }
+}
+
 // ---------------------------------------------------------------------------------------------------------
 // launchers
 // ---------------------------------------------------------------------------------------------------------
@@ -4665,6 +4694,11 @@ void launch_conv_compact(const ConvCmpInst* d, int n, ChunkInfo ci, cudaStream_t
     k_conv_cmp_carry<<<dim3(2 * CV_B / 256, (unsigned)n), 256, 0, s>>>(d);
     k_conv_cmp_mac<<<dim3((unsigned)((CV_B / CV_MAC_THREADS) * ((wb + CV_J - 1) / CV_J)), (unsigned)n), CV_MAC_THREADS, 0, s>>>(d, ci);
     k_conv_cmp_ifft<<<dim3((unsigned)wb, (unsigned)n), CV_THREADS, smem, s>>>(d, ci);
+}
+void launch_bind_sources(const BindItem* d, int n, int64_t max_vec, int max_ch, cudaStream_t s) {
+    // about four vectors per thread along a channel; items beyond 65535 are walked by the grid-stride loop over blockIdx.y
+    const int64_t bx = std::max<int64_t>(1, std::min<int64_t>((max_vec + 1023) / 1024, 65535));
+    k_bind_sources<<<dim3((unsigned)bx, (unsigned)std::min(n, 65535), (unsigned)max_ch), 256, 0, s>>>(d, n);
 }
 void launch_conv_ir_fft(const float* ir, int64_t ir_len, int64_t ir_stride, float2* h, int S, int channels, cudaStream_t s) {
     conv_configure();

@@ -65,6 +65,8 @@ void launch_analyser(const AnalyserInst* d, int n, ChunkInfo ci, cudaStream_t s)
 void launch_conv_fft_in(const ConvInput* d, int n, ChunkInfo ci, cudaStream_t s);
 void launch_conv_mac_ifft(const ConvPath* p, const ConvInput* in, int n, ChunkInfo ci, cudaStream_t s);
 void launch_conv_compact(const ConvCmpInst* d, int n, ChunkInfo ci, cudaStream_t s);
+// one launch for all items of a bind call; max_vec = the largest slot stride / 4, max_ch = the most channels of an item
+void launch_bind_sources(const BindItem* d, int n, int64_t max_vec, int max_ch, cudaStream_t s);
 void launch_conv_ir_fft(const float* ir, int64_t ir_len, int64_t ir_stride, float2* h, int S, int channels, cudaStream_t s);
 
 }  // namespace wae
