@@ -526,6 +526,39 @@ typedef struct wae_source_binding {
  * been bound. */
 WAE_API wae_status wae_batch_bind_sources(wae_batch* batch, const wae_source_binding* items, uint32_t n, void* stream);
 
+/* ---- param values bound from device memory ----------------------------------------------------------------------------------
+ * Declares a param whose value is supplied per run from device memory (wae_batch_bind_params) instead of at build time, so that one
+ * prepared batch renders any number of parameter sets (EQ, gain, pan, compressor settings drawn on the GPU) without being built and
+ * planned again.  The param renders as a constant for the whole render, as a param with only a value does.  param_index numbers the
+ * params as wae_param_event_push does.  Bindable: GainNode gain; BiquadFilterNode q, detune, frequency, gain (0..3); StereoPannerNode
+ * pan; DynamicsCompressorNode attack, knee, ratio, release, threshold (0..4).  A bound value is clamped to [max(lo, minValue),
+ * min(hi, maxValue)], as AudioParam::set_value clamps to [minValue, maxValue].  The range matters for one decision only: a GainNode
+ * whose range excludes |gain| <= 1e-6 can never answer with silence, so its output keeps the layout of its input.
+ * Deviation: a non-finite bound value renders as the param's default value (the reference panics on a non-finite set_value, which a
+ * device bind cannot do; this is its rule for a NaN computed value).
+ * WAE_INVALID_ARGUMENT: lo > hi, a non-finite bound, or a range outside [minValue, maxValue].  WAE_UNSUPPORTED: another node kind or
+ * param.  WAE_INVALID_STATE: the param has automation events or an audio-rate input, is declared twice, or the graph already has a
+ * suspend point; after the declaration, events (set_value included, also from a suspend callback) and wae_connect_param to it answer
+ * WAE_INVALID_STATE.  wae_render_batch and wae_render_many answer WAE_INVALID_STATE on graphs with such params; wae_batch_plan plans
+ * them with the param's current value clamped to the range. */
+WAE_API wae_status wae_param_set_device_value(wae_graph* graph, wae_node_id node, uint32_t param_index, float lo, float hi);
+
+typedef struct wae_param_binding {
+    uint32_t graph_index;  /* caller's index, as wae_batch_fetch_graph */
+    wae_node_id node;      /* the param's node */
+    uint32_t param_index;  /* declared with wae_param_set_device_value */
+    const float* value;    /* one float of device (or managed) memory on the engine's GPU */
+} wae_param_binding;
+
+/* Reads the values on the device, asynchronously on the engine stream after the work already queued on `stream` (as
+ * wae_batch_bind_sources), and re-derives every planned record they reach (filter coefficients and scan constants, gain products,
+ * panner gains, compressor settings) in every render segment.  All-or-nothing: every item is validated before anything is enqueued.
+ * Bound values stay until they are bound again.  WAE_INVALID_ARGUMENT: `value` is not device (or managed) memory of the engine's GPU or
+ * its 4 bytes are not in one allocation, or one param is named twice in the call.  WAE_INVALID_STATE: graph_index out of range, or the
+ * param was not declared.  wae_batch_run, wae_batch_run_group and wae_batch_run_pipelined answer WAE_INVALID_STATE while a declared
+ * param of the batch has never been bound. */
+WAE_API wae_status wae_batch_bind_params(wae_batch* batch, const wae_param_binding* items, uint32_t n, void* stream);
+
 /* PeriodicWave::new(context, PeriodicWaveOptions { real, imag, disable_normalization }) (src/periodic_wave.rs:104-209): fills `table`
  * (PERIODIC_WAVE_TABLE_LENGTH = 2048 in the reference) with the wavetable an OscillatorNode of type Custom plays.  `real` / `imag` may be
  * NULL (= zeros); both NULL = the sine default.  Host math, no engine needed. */

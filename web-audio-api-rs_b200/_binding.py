@@ -123,6 +123,11 @@ class SourceBinding(C.Structure):
     _fields_ = [("graph_index", C.c_uint32), ("node", C.c_uint32), ("pcm", c_float_p), ("channel_stride", C.c_uint64)]
 
 
+class ParamBinding(C.Structure):
+    """wae_param_binding: the device address of one param value of a prepared batch (wae_batch_bind_params)."""
+    _fields_ = [("graph_index", C.c_uint32), ("node", C.c_uint32), ("param_index", C.c_uint32), ("value", c_float_p)]
+
+
 STATUS_NAMES = {0: "OK", 1: "INVALID_ARGUMENT", 2: "INVALID_STATE", 3: "NOT_SUPPORTED", 4: "UNSUPPORTED",
                 5: "CUDA_ERROR", 6: "OUT_OF_MEMORY", 7: "NO_DEVICE"}
 
@@ -162,6 +167,7 @@ WAE_SYMBOLS = [
     "wae_oscillator_set_periodic_wave", "wae_node_set_attribute", "wae_disconnect_from", "wae_disconnect_param", "wae_periodic_wave_table", "wae_param_sim_set_walker", "wae_sched_first_frame_at_or_after", "wae_spatial_params", "wae_hrtf_locate",
     "wae_render_many", "wae_batch_prepare_many", "wae_batch_graph_output", "wae_batch_fetch_graph", "wae_batch_plan_many", "wae_batch_plan_quanta",
     "wae_buffer_source_set_device_input", "wae_batch_bind_sources",
+    "wae_param_set_device_value", "wae_batch_bind_params",
 ]
 
 
@@ -265,6 +271,9 @@ class Api:
             # source audio bound from device memory
             f("buffer_source_set_device_input", C.c_int32, [gp, C.c_uint32, C.c_uint32, C.c_uint64, C.c_float])
             f("batch_bind_sources", C.c_int32, [C.c_void_p, C.POINTER(SourceBinding), C.c_uint32, C.c_void_p])
+            # param values bound from device memory
+            f("param_set_device_value", C.c_int32, [gp, C.c_uint32, C.c_uint32, C.c_float, C.c_float])
+            f("batch_bind_params", C.c_int32, [C.c_void_p, C.POINTER(ParamBinding), C.c_uint32, C.c_void_p])
         else:
             f("graph_create", C.c_int32, [C.c_uint32, C.c_uint64, C.c_float, C.POINTER(C.c_void_p)])
             f("render", C.c_int32, [gp, c_float_p])

@@ -143,6 +143,20 @@ class AudioParam:
     def set_value_curve_at_time(self, values, start_time, duration):
         return self._push(7, 0.0, start_time, duration, values)
 
+    def set_device_value(self, lo=None, hi=None):
+        """wae_param_set_device_value (product only): the param's value is supplied per run from device memory by Batch.bind_params,
+        clamped to [lo, hi] within [minValue, maxValue] (default: the whole range).  It renders as a constant over the render; until
+        bound, the batch is planned with the current value clamped to the range."""
+        api = self._ctx._api
+        if not api.is_product:
+            raise B.WaeError(3, "params bound from device memory are a feature of the GPU engine")
+        if self._node == "listener":
+            raise B.WaeError(4, "AudioListener params cannot be bound from device memory")
+        lo = -3.4028234663852886e38 if lo is None else float(lo)
+        hi = 3.4028234663852886e38 if hi is None else float(hi)
+        api.check(api.param_set_device_value(self._ctx._g, self._node, self._index, lo, hi))
+        return self
+
     def set_automation_rate(self, rate):
         api = self._ctx._api
         api.check(api.param_set_automation_rate(self._ctx._g, self._node, self._index, 0 if rate in ("a", "A", 0) else 1))
@@ -779,13 +793,47 @@ class Batch:
                                     f"[{declared[0]}][{declared[1]}]")
             items[k] = B.SourceBinding(g, int(nid), C.cast(C.c_void_p(base + 4 * k * pcm.stride(0)), B.c_float_p), channel_stride)
         self.api.check(self.api.batch_bind_sources(self.handle, items, n, C.c_void_p(self._torch_stream_handle())))
-        # keep torch's caching allocator from reusing the memory before the copy has run.  The tensor is recorded on a torch-owned stream
-        # that waits for the engine stream, not on the engine stream itself: the allocator records an event on that stream whenever the
-        # tensor is freed, which may be after the engine (and its stream) are gone
+        self._keep_until_read(pcm)
+
+    def _keep_until_read(self, t):
+        """Keeps torch's caching allocator from reusing a bound tensor's memory before the engine stream has read it.  The tensor is
+        recorded on a torch-owned stream that waits for the engine stream, not on the engine stream itself: the allocator records an event
+        on that stream whenever the tensor is freed, which may be after the engine (and its stream) are gone."""
+        import torch
         if self._guard is None:
             self._guard = torch.cuda.Stream(device=self._device())
         self._guard.wait_stream(self._engine_stream())
-        pcm.record_stream(self._guard)
+        t.record_stream(self._guard)
+
+    def bind_params(self, params, values, graphs=None):
+        """wae_batch_bind_params: values[i][j] (a float32 CUDA tensor [n][k], or [n] for one param) becomes the value of params[j] in
+        context graphs[i] (default: 0..n-1).  `params`: AudioParams declared with set_device_value, one per column; a param of a context
+        built like the others shares its node id and index, so the params of context 0 name those of every context.  One call, ordered
+        after torch's current stream; the values are read on the engine stream, and the tensor is kept from reuse until they have been."""
+        import torch
+        if not (isinstance(values, torch.Tensor) and values.is_cuda and values.dtype == torch.float32 and values.dim() in (1, 2)):
+            raise B.WaeError(1, "bind_params: values must be a float32 CUDA tensor [n] or [n][k]")
+        params = list(params) if isinstance(params, (list, tuple)) else [params]
+        v2 = values if values.dim() == 2 else values.unsqueeze(1)
+        n, k = v2.shape
+        if k != len(params):
+            raise B.WaeError(1, f"bind_params: {k} value columns for {len(params)} params")
+        graphs = list(range(n)) if graphs is None else [int(g) for g in graphs]
+        if len(graphs) != n:
+            raise B.WaeError(1, f"bind_params: {n} value rows for {len(graphs)} graphs")
+        items = (B.ParamBinding * max(n * k, 1))()
+        base = v2.data_ptr()
+        s0, s1 = v2.stride()
+        for i, g in enumerate(graphs):
+            if not 0 <= g < self.n:
+                raise B.WaeError(2, f"bind_params: graph index {g} is out of range")
+            for j, prm in enumerate(params):
+                if prm._node == "listener":
+                    raise B.WaeError(2, "bind_params: AudioListener params are not bound from device memory")
+                ptr = C.cast(C.c_void_p(base + 4 * (i * s0 + j * s1)), B.c_float_p)
+                items[i * k + j] = B.ParamBinding(g, int(prm._node), int(prm._index), ptr)
+        self.api.check(self.api.batch_bind_params(self.handle, items, n * k, C.c_void_p(self._torch_stream_handle())))
+        self._keep_until_read(values)
 
     def output_tensor(self, i=None):
         """Zero-copy torch view of the rendered output on the device: [n][channels][length] for a batch of one shape, [channels_i][length_i]

@@ -113,6 +113,10 @@ float Param::constant_value() const {
     if (std::isnan(v)) return default_value;
     v = v > min_value ? v : min_value;
     v = v < max_value ? v : max_value;
+    if (device_bound) {  // the placeholder a bound param is planned with
+        v = v > device_lo ? v : device_lo;
+        v = v < device_hi ? v : device_hi;
+    }
     return v;
 }
 }  // namespace wae
@@ -587,7 +591,50 @@ WAE_API wae_status wae_connect_param(wae_graph* g, wae_node_id from, uint32_t ou
     if (fi == g->nodes.end() || ti == g->nodes.end()) return fail(WAE_INVALID_ARGUMENT, "InvalidAccessError - unknown node");
     if ((int)output >= fi->second.n_outputs) return fail(WAE_INVALID_ARGUMENT, "IndexSizeError - output port out of bounds");
     if (param_index >= ti->second.params.size()) return fail(WAE_INVALID_ARGUMENT, "IndexSizeError - param index out of bounds");
+    if (g->nodes.at(ti->second.params[param_index]).param.device_bound)
+        return fail(WAE_INVALID_STATE, "InvalidStateError - the param's value is bound from device memory (wae_param_set_device_value): "
+                                       "it takes no audio-rate input");
     g->add_edge(fi->second.out_id, (int)output, ti->second.params[param_index], 0);
+    return WAE_OK;
+}
+
+// Params whose value stays constant over the render, so that a per-run value can be re-derived into the planned records (a GainNode's
+// gain, a BiquadFilterNode's four, a StereoPannerNode's pan, a DynamicsCompressorNode's five)
+static bool device_value_supported(Kind kind, uint32_t param_index) {
+    switch (kind) {
+        case K_GAIN: return param_index == 0;
+        case K_BIQUAD: return param_index < 4;
+        case K_SPANNER: return param_index == 0;
+        case K_COMP: return param_index < 5;
+        default: return false;
+    }
+}
+
+WAE_API wae_status wae_param_set_device_value(wae_graph* g, wae_node_id node, uint32_t param_index, float lo, float hi) {
+    if (!g) return fail(WAE_INVALID_ARGUMENT, "null graph");
+    Node* n = g->nodes.get(node);
+    if (!n || n->kind == K_PARAM || param_index >= n->params.size()) return fail(WAE_INVALID_ARGUMENT, "unknown param");
+    if (!std::isfinite(lo) || !std::isfinite(hi) || lo > hi)
+        return fail(WAE_INVALID_ARGUMENT, "device value range [" + std::to_string(lo) + ", " + std::to_string(hi) + "] is not a finite range");
+    if (!device_value_supported(n->kind, param_index))
+        return fail(WAE_UNSUPPORTED, "param " + std::to_string(param_index) + " of node " + std::to_string(node) +
+                                         " cannot be bound from device memory (GainNode gain, BiquadFilterNode q / detune / frequency / gain, "
+                                         "StereoPannerNode pan and DynamicsCompressorNode params can)");
+    const uint32_t pid = n->params[param_index];
+    Param& p = g->nodes.at(pid).param;
+    if (p.device_bound) return fail(WAE_INVALID_STATE, "InvalidStateError - the param is already bound from device memory");
+    if (!g->epochs.empty())  // (the segments before the suspend point were planned with the value of their own graph copy)
+        return fail(WAE_INVALID_STATE, "InvalidStateError - a param is bound from device memory before the first suspend point");
+    if (!p.constant()) return fail(WAE_INVALID_STATE, "InvalidStateError - the param has automation events");
+    for (const auto& kv : g->nodes)
+        for (const Edge& e : kv.second.outgoing)
+            if (e.other_id == pid) return fail(WAE_INVALID_STATE, "InvalidStateError - the param has an audio-rate input (connect_param)");
+    const float l = std::max(lo, p.min_value), h = std::min(hi, p.max_value);
+    if (l > h) return fail(WAE_INVALID_ARGUMENT, "device value range lies outside the param's [minValue, maxValue]");
+    p.device_bound = true;
+    p.device_lo = l;
+    p.device_hi = h;
+    g->device_params++;
     return WAE_OK;
 }
 
@@ -655,6 +702,9 @@ WAE_API wae_status wae_disconnect_param(wae_graph* g, wae_node_id from, int32_t 
 }
 
 static wae_status push_event(Param& p, const wae_param_event* e) {
+    if (p.device_bound)
+        return fail(WAE_INVALID_STATE, "InvalidStateError - the param's value is bound from device memory (wae_param_set_device_value): "
+                                       "it takes no events");
     auto finite = [](float v) { return std::isfinite(v); };
     auto valid_time = [](double t) { return std::isfinite(t) && t >= 0.; };
     ParamEv ev{(int)e->type, e->value, e->time, e->aux, {}};

@@ -521,4 +521,35 @@ struct BindItem {
     int32_t pad;
 };
 
+// ---- wae_batch_bind_params: per-run values of params planned as constants ------------------------------------------------------
+struct ParamBindItem {  // one float of the caller's device memory -> value slot `slot`
+    const float* src;
+    int32_t slot;
+    int32_t pad;
+};
+struct ParamSlotInfo {  // how a slot takes a bound value: clamped to [lo, hi]; non-finite -> def (the param's default value)
+    float lo, hi, def;
+    int32_t pad;
+};
+// A patch entry: one planned record field that a bound value reaches, re-derived from the value slots and the planned constants.
+// Operand i is slot[i] (>= 0) or the constant val[i].
+enum PatchKind : int32_t {
+    PATCH_GAIN = 0,    // float *dst = the product of the n operands in node order, each bound one after gain.rs's 1e-6 shortcuts
+    PATCH_META = 1,    // int32 *dst (MetaInst::mode of a gain that may answer with silence): META_CONST when that product is 0, else META_COPY
+    PATCH_BIQUAD = 2,  // operands q, detune, frequency, gain: double *dst = b0, b1, b2, a1, a2; ScanCoef *dst2 (k_chain) or nullptr
+    PATCH_SPAN = 3,    // operand pan: float *dst = pan, float2 *dst2 = the stereo gains for n input channels
+    PATCH_RAW = 4,     // float *dst = operand 0
+};
+constexpr int PATCH_OPS = 8;
+struct ParamPatch {
+    int32_t kind;
+    int32_t n;          // PATCH_GAIN / PATCH_META: operands; PATCH_BIQUAD: filter type; PATCH_SPAN: input channels
+    float sample_rate;  // PATCH_BIQUAD
+    int32_t pad;
+    void* dst;
+    void* dst2;
+    int32_t slot[PATCH_OPS];
+    float val[PATCH_OPS];
+};
+
 }  // namespace wae

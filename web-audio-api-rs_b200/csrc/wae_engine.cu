@@ -300,7 +300,30 @@ struct StageBuild {
     std::vector<ConvCmpInst> conv_cmp;  // S_CONV_CMP: compacted second path of a mono-response convolver
     std::vector<VoiceGroup> vgroups;  // S_VSUM: groups of consecutive `chain` records
     int max_ch = 1;
+    // Patch entries of params bound from device memory (wae_param_set_device_value) into this stage's records: record `rec` of the
+    // stage's own table, `off` bytes into it; `rec2`: the scan constants (S_CHAIN / S_VSUM) or the stereo gains (S_SPAN) it also
+    // re-derives, -1: none.  Operands name their param by node id (patch.slot) until the batch numbers its value slots.
+    struct PatchRec {
+        ParamPatch p;
+        uint32_t graph;  // batch position
+        int32_t rec, rec2;
+        uint32_t off;
+    };
+    std::vector<PatchRec> patches;
+    size_t records() const {  // size of the table patch entries point into
+        switch (kind) {
+            case S_CHAIN: case S_VSUM: return chain.size();
+            case S_BIQUAD: return biquad.size();
+            case S_BIQUAD_AR: return biquad_ar.size();
+            case S_GAIN: return gain.size();
+            case S_SPAN: return span.size();
+            case S_COMP: return comp.size();
+            case S_META: return meta.size();
+            default: return 0;
+        }
+    }
 };
+using PatchRec = StageBuild::PatchRec;
 
 struct Stage {
     int cls = 0;  // see Planner::stage()
@@ -396,15 +419,31 @@ struct wae_batch {
     // copied to d_bind, which the next bind may overwrite at once (its copy is queued behind this bind's kernel on the same stream).  A
     // staging buffer is reused once its copy has run (its event has completed); while all are in flight a new one is made, so a bind
     // does not wait on the host for runs queued before it (up to kMaxBindStages staging buffers; then the bind waits for the first one that fits).
+    // wae_batch_bind_params uses the same staging buffers and device table for its items.
     struct BindStage {
-        BindItem* h;
-        size_t cap;
+        void* h;
+        size_t cap;      // bytes
         cudaEvent_t ev;  // the copy out of `h`
     };
     static constexpr size_t kMaxBindStages = 8;
     std::vector<BindStage> bind_stages;
-    BindItem* d_bind = nullptr;
-    size_t bind_cap = 0;
+    void* d_bind = nullptr;
+    size_t bind_cap = 0;  // bytes
+    // wae_param_set_device_value: one value slot per declared param of the batch (batch position, node, param index), and the patch
+    // entries of every record a bound value reaches (re-derived by k_derive_params after each wae_batch_bind_params)
+    struct BoundParam {
+        uint32_t graph;  // batch position
+        wae_node_id node;
+        uint32_t param_index;
+        bool bound;
+    };
+    std::vector<BoundParam> bound_params;  // [slot]
+    std::map<std::tuple<uint32_t, wae_node_id, uint32_t>, int32_t> param_slot;
+    size_t params_unbound = 0;
+    ParamSlotInfo* d_slot_info = nullptr;
+    float* d_values = nullptr;
+    ParamPatch* d_patches = nullptr;
+    int n_patches = 0;
     cudaEvent_t ev_bind = nullptr;  // orders a bind after the caller's stream
     // OfflineAudioContext::suspend_sync: a group's render is cut at the suspend frames of its graphs (graphs with different
     // suspend points are put in different groups); every segment has its own plan, node state is shared between the plans
@@ -785,6 +824,10 @@ struct Planner {
         int phase = 0;  // 0: before biquad A, 1: after A, 3: after B, 5: after the shaper (canonical chain order)
         int cls = 0;    // scheduling class of the node that opened the chain (see stage())
         Lay lay;        // layout of the chain's output over time (the kernel writes the track when it is not constant)
+        // params bound from device memory: biquad k's patch entries (rec2 = k until the chain is emitted), and per gain slot the factors
+        // folded into it since the first bound one (gain_fold[s].p.n == 0: the slot has none)
+        std::vector<PatchRec> patches;
+        PatchRec gain_fold[4] = {};
     };
 
     // Node state is allocated through a key (graph, node, n-th allocation of that node, salt): the plans of consecutive
@@ -973,8 +1016,53 @@ struct Planner {
         bool dyn = false;  // automated / audio-rate driven: one value per frame in `track`
         float v = 0.f;
         BufRef track{nullptr, 0, 0};
+        int32_t bound = -1;      // bound from device memory: the param's id (`v` is the placeholder), -1: not bound
+        float lo = 0.f, hi = 0.f;  // bound: the range its values are clamped to
     };
     PRef param_ref(uint32_t pid);
+    // a patch entry of this graph; operand i of `r` is `pr` (its id when bound, else its planned value)
+    PatchRec patch(int kind, int n) const {
+        PatchRec r{};
+        r.p.kind = kind;
+        r.p.n = n;
+        for (int i = 0; i < PATCH_OPS; i++) r.p.slot[i] = -1;
+        r.graph = gi;
+        r.rec = r.rec2 = -1;
+        return r;
+    }
+    static void operand(PatchRec& r, int i, const PRef& pr, float planned) {
+        r.p.slot[i] = pr.bound;
+        r.p.val[i] = planned;
+    }
+    // records patch entry `r` for the last record of stage `s`
+    static void add_patch(StageBuild& s, PatchRec r, uint32_t off, bool with_rec2 = false) {
+        r.rec = (int32_t)s.records() - 1;
+        r.rec2 = with_rec2 ? r.rec : -1;
+        r.off = off;
+        s.patches.push_back(r);
+    }
+    // a chain's patch entries for its record at index `rec` of stage `s` (emit_chain, sum_voices)
+    static void chain_patches(StageBuild& s, const PendingChain& pc, int32_t rec) {
+        for (PatchRec r : pc.patches) {
+            const int k = r.rec2;
+            r.rec = rec;
+            r.rec2 = pc.inst.bq[k].coef;
+            r.off = (uint32_t)(offsetof(ChainInst, bq) + (size_t)k * sizeof(ChainBiquad) + offsetof(ChainBiquad, b0));
+            s.patches.push_back(r);
+        }
+        for (int slot = 0; slot < 4; slot++) {
+            if (pc.gain_fold[slot].p.n == 0) continue;
+            PatchRec r = pc.gain_fold[slot];
+            r.rec = rec;
+            r.off = (uint32_t)(offsetof(ChainInst, g) + (size_t)slot * sizeof(float));
+            s.patches.push_back(r);
+        }
+    }
+    static bool chain_has_patches(const PendingChain& pc) {
+        bool any = !pc.patches.empty();
+        for (const auto& f : pc.gain_fold) any = any || f.p.n > 0;
+        return any;
+    }
     bool plan_graph(wae_graph* graph, uint32_t graph_index);
     // ir_override: the response of a STATIC HRTF panner (blended, gain folded in): no normalisation, no trimming of small trailing taps;
     // a two-channel input is mixed down to mono by the forward transform's loads (ConvInput::in_channel = -1)
@@ -1032,12 +1120,17 @@ struct Planner {
         return pc;
     }
     // a biquad (or an IIR filter of order <= 2, which opens a chain of its own with a constant layout) appended to the chain it joins
-    bool append_biquad(NodeCtx& nc, double* state, const hm::BiquadCoefs& c) {
+    // `bound`: the patch entry of a biquad with params bound from device memory
+    bool append_biquad(NodeCtx& nc, double* state, const hm::BiquadCoefs& c, const PatchRec* bound = nullptr) {
         PendingChain pc = open_chain(nc);
         ChainBiquad& st = pc.inst.bq[pc.inst.n_biquad++];
         st.state = state;
         st.b0 = c.b0; st.b1 = c.b1; st.b2 = c.b2; st.a1 = c.a1; st.a2 = c.a2;
         pc.coefs[pc.inst.n_biquad - 1] = c;
+        if (bound) {
+            pc.patches.push_back(*bound);
+            pc.patches.back().rec2 = pc.inst.n_biquad - 1;
+        }
         pc.phase = pc.phase == 0 ? 1 : 3;
         pc.lay = filter_lay(pc.lay);
         return finish_chain(nc, std::move(pc));
@@ -1236,17 +1329,23 @@ static void append_vec(std::vector<T>& d, std::vector<T>& s) {
 }
 static void merge_builds(Builds& dst, Builds& src) {
     struct Base {
-        size_t mix_edges = 0, scan = 0, chain = 0, conv_in = 0;
+        size_t mix_edges = 0, scan = 0, chain = 0, conv_in = 0, records = 0;
     };
     std::map<std::pair<int, int>, Base> base;  // table sizes of `dst` before anything of `src` is appended
     for (auto& kv : src) {
         auto it = dst.find(kv.first);
-        if (it != dst.end()) base[kv.first] = Base{it->second.mix_edges.size(), it->second.n_scan_coef, it->second.chain.size(), it->second.conv_in.size()};
+        if (it != dst.end())
+            base[kv.first] = Base{it->second.mix_edges.size(), it->second.n_scan_coef, it->second.chain.size(), it->second.conv_in.size(),
+                                  it->second.records()};
         else base[kv.first] = Base{};
     }
     for (auto& kv : src) {
         StageBuild& s = kv.second;
         const Base bs = base[kv.first];
+        for (auto& pr : s.patches) {
+            pr.rec += (int32_t)bs.records;
+            if (pr.rec2 >= 0) pr.rec2 += (int32_t)(s.kind == S_SPAN ? bs.records : bs.scan);
+        }
         for (auto& m : s.mix) m.edge_offset += (uint32_t)bs.mix_edges;
         for (auto& m : s.mix_dyn) m.edge_offset += (uint32_t)bs.mix_edges;
         for (auto& c : s.chain)
@@ -1274,6 +1373,7 @@ static void merge_builds(Builds& dst, Builds& src) {
         append_vec(d.delay, s.delay); append_vec(d.comp, s.comp); append_vec(d.analyser, s.analyser); append_vec(d.mix, s.mix);
         append_vec(d.mix_edges, s.mix_edges); append_vec(d.mix_dyn, s.mix_dyn); append_vec(d.meta, s.meta); append_vec(d.conv_in, s.conv_in);
         append_vec(d.conv_path, s.conv_path); append_vec(d.vgroups, s.vgroups); append_vec(d.conv_cmp, s.conv_cmp);
+        append_vec(d.patches, s.patches);
         d.n_scan_coef += s.n_scan_coef;
         d.max_ch = std::max(d.max_ch, s.max_ch);
     }
@@ -1296,38 +1396,7 @@ static uint32_t next_pow2(uint64_t v) {
 // constants of the time-parallel biquad recurrence (see ScanCoef in wae_kernels.h), f64 on the host
 static ScanCoef make_scan_coef(const hm::BiquadCoefs& c) {
     ScanCoef sc{};
-    struct M2 {
-        double a, b, c, d;
-    };
-    auto mul = [](const M2& x, const M2& y) { return M2{x.a * y.a + x.b * y.c, x.a * y.b + x.b * y.d, x.c * y.a + x.d * y.c, x.c * y.b + x.d * y.d}; };
-    const M2 M{-c.a1, -c.a2, 1., 0.};
-    M2 r{1., 0., 0., 1.};
-    for (int j = 0; j < WAE_CHAIN_K; j++) r = mul(M, r);
-    const M2 A = r;  // M^K: one thread of k_chain
-    M2 pw = A;
-    for (int d = 0; d < 5; d++) {
-        sc.Pshfl[d][0] = pw.a; sc.Pshfl[d][1] = pw.b; sc.Pshfl[d][2] = pw.c; sc.Pshfl[d][3] = pw.d;
-        pw = mul(pw, pw);
-    }
-    sc.Pwarp[0] = pw.a; sc.Pwarp[1] = pw.b; sc.Pwarp[2] = pw.c; sc.Pwarp[3] = pw.d;  // A^32
-    M2 pl = A;
-    for (int l = 0; l < 32; l++) {
-        sc.Plane[l][0] = pl.a; sc.Plane[l][1] = pl.b; sc.Plane[l][2] = pl.c; sc.Plane[l][3] = pl.d;
-        pl = mul(A, pl);
-    }
-    // one frame with zero input: (x1, x2, y1, y2) -> (0, x1, b1 x1 + b2 x2 - a1 y1 - a2 y2, y1); G^L by squaring (L = 2^15 frames)
-    static_assert(WAE_CHAIN_PRE_TILES * WAE_CHAIN_K * 128 == 1 << 15, "GL below is G^(2^15)");
-    double g[16] = {0., 0., 0., 0., 1., 0., 0., 0., c.b1, c.b2, -c.a1, -c.a2, 0., 0., 1., 0.}, h[16];
-    for (int sq = 0; sq < 15; sq++) {
-        for (int r = 0; r < 4; r++)
-            for (int cc = 0; cc < 4; cc++) {
-                double a = 0.;
-                for (int k = 0; k < 4; k++) a += g[4 * r + k] * g[4 * k + cc];
-                h[4 * r + cc] = a;
-            }
-        std::memcpy(g, h, sizeof g);
-    }
-    std::memcpy(sc.GL, g, sizeof g);
+    make_scan_coef(c.b1, c.b2, c.a1, c.a2, sc);
     return sc;
 }
 
@@ -1559,7 +1628,13 @@ bool Planner::conv_compact_path(PNode& pn, int level, int in_ch, const IrSpectra
 Planner::PRef Planner::param_ref(uint32_t pid) {
     PRef r;
     PNode* it = node_table.find(pid);
-    r.v = (it ? *it->n : g->nodes.at(pid)).param.constant_value();
+    const Param& prm = (it ? *it->n : g->nodes.at(pid)).param;
+    r.v = prm.constant_value();
+    if (prm.device_bound) {
+        r.bound = (int32_t)pid;
+        r.lo = prm.device_lo;
+        r.hi = prm.device_hi;
+    }
     if (it && !it->out_buf.empty()) {
         r.dyn = true;
         r.track = it->out_buf[0];
@@ -1578,6 +1653,7 @@ void Planner::emit_chain(PendingChain& pc, int L) {
         pc.inst.bq[k].coef = cs.add_scan_coef(want_scan_coefs, [&] { return make_scan_coef(pc.coefs[k]); });
     }
     cs.max_ch = std::max(cs.max_ch, pc.ch);
+    chain_patches(cs, pc, (int32_t)cs.chain.size());
     cs.chain.push_back(pc.inst);
 }
 
@@ -1593,7 +1669,7 @@ bool Planner::materialize(uint32_t nid, bool may_alias) {
         const AbsnInst& a = ci.absn;
         bool unit = true;
         for (int i = 0; i < 4; i++) unit = unit && ci.g[i] == 1.f;
-        if (may_alias && ci.src_kind == CHAIN_SRC_ABSN && ci.n_biquad == 0 && !ci.has_shaper && unit && it->second.phase == 0 &&
+        if (may_alias && ci.src_kind == CHAIN_SRC_ABSN && ci.n_biquad == 0 && !ci.has_shaper && unit && !chain_has_patches(it->second) && it->second.phase == 0 &&
             !it->second.lay.dyn() && a.n_start == 0 && !a.loop && a.buf_offset == 0 && a.buf_len >= lq && a.buf_stride <= 0xffffffffll &&
             seg_start == 0 && seg_end >= lq) {
             sp.out_buf = {BufRef{const_cast<float*>(a.buf), (uint32_t)a.buf_stride, 1}};
@@ -1884,6 +1960,7 @@ bool Planner::sum_voices(NodeCtx& nc, int port, int ch, int nb) {
             pc.inst.bq[k].coef = vs.add_scan_coef(want_scan_coefs, [&] { return make_scan_coef(pc.coefs[k]); });
         pc.inst.limit = -1;
         pc.inst.out_dup = 0;
+        chain_patches(vs, pc, (int32_t)vs.chain.size());
         vs.chain.push_back(pc.inst);
     }
     vs.vgroups.push_back(vg);
@@ -2323,16 +2400,34 @@ bool Planner::lower_biquad(NodeCtx& nc) {
         StageBuild& sb = stage(nc.L, S_BIQUAD_AR);
         sb.max_ch = std::max(sb.max_ch, ch);
         sb.biquad_ar.push_back(ba);
+        // params bound from device memory next to automated ones: the constant operands of k_biquad_coefs
+        const PRef* refs[4] = {&pq, &pdt, &pfr, &pg};
+        const size_t offs[4] = {offsetof(BiquadArInst, q_val), offsetof(BiquadArInst, detune_val), offsetof(BiquadArInst, freq_val),
+                                offsetof(BiquadArInst, gain_val)};
+        for (int i = 0; i < 4; i++)
+            if (refs[i]->bound >= 0) {
+                PatchRec r = patch(PATCH_RAW, 1);
+                operand(r, 0, *refs[i], refs[i]->v);
+                add_patch(sb, r, (uint32_t)offs[i]);
+            }
         return true;
     }
     float cf = hm::biquad_computed_freq(freq, detune);
     hm::BiquadCoefs c = hm::biquad_coefs(n.type, (double)g->sample_rate, (double)cf, (double)gain, (double)q);
+    // coefficients that depend on params bound from device memory: re-derived per bind
+    const bool bound = pq.bound >= 0 || pdt.bound >= 0 || pfr.bound >= 0 || pg.bound >= 0;
+    PatchRec bp = patch(PATCH_BIQUAD, n.type);
+    bp.p.sample_rate = g->sample_rate;
+    operand(bp, 0, pq, q);
+    operand(bp, 1, pdt, detune);
+    operand(bp, 2, pfr, freq);
+    operand(bp, 3, pg, gain);
     double* state = alloc<double>((size_t)ch * 4, true, true);
     if (!state) return bail(WAE_OUT_OF_MEMORY, "out of device memory (state)");
     // An input whose channel COUNT changes while it sounds resets / drops channels of the filter mid-render
     // (biquad_filter.rs:798-815): the serial kernel follows it quantum by quantum; the scan keeps one state per channel
     const bool count_varies = !nc.extend && in0.dyn() && !(in0.nlo == in0.nhi && in0.nhi == ch);
-    if (!eng->serial_filters && !count_varies) return append_biquad(nc, state, c);
+    if (!eng->serial_filters && !count_varies) return append_biquad(nc, state, c, bound ? &bp : nullptr);
     // bit-faithful serial recurrence, one stage per biquad
     if (!need_out(nc, ch)) return false;
     BiquadInst bi{};
@@ -2345,6 +2440,7 @@ bool Planner::lower_biquad(NodeCtx& nc) {
     StageBuild& s = stage(nc.L, S_BIQUAD);
     s.max_ch = std::max(s.max_ch, ch);
     s.biquad.push_back(bi);
+    if (bound) add_patch(s, bp, (uint32_t)offsetof(BiquadInst, b0));
     return true;
 }
 
@@ -2405,21 +2501,49 @@ bool Planner::lower_gain(NodeCtx& nc) {
     // the multiply path, a difference of at most 1e-6 * |x| that is below the parity tolerance)
     if (std::fabs(gv) <= 1e-6f) gv = 0.f;
     else if (std::fabs(1.f - gv) <= 1e-6f) gv = 1.f;
+    // A gain bound from device memory is planned as this constant.  Whether it answers with silence depends on the value: when its
+    // range does not exclude |g| <= 1e-6 its output is planned as the input's layout OR silence, and the bind decides
+    const bool bound = pgn.bound >= 0;
+    const bool may_zero = bound && !(pgn.lo > 1e-6f || pgn.hi < -1e-6f);
+    const Lay or_silent{1, nc.in0.hi, nc.in0.nlo, nc.in0.nhi, true};
     if (nc.fuse_n) {
         PendingChain pc = open_chain(nc);
         // consecutive gains of one slot are folded (differs from two f32 multiplies by <= 1 ulp)
-        pc.inst.g[pc.phase == 0 ? 0 : (pc.phase == 1 ? 1 : (pc.phase == 3 ? 2 : 3))] *= gv;
-        if (gv == 0.f) pc.lay = Lay{1, 1, 1, 1, true};  // a gain of (about) zero answers with silence (gain.rs:160-163)
+        const int slot = pc.phase == 0 ? 0 : (pc.phase == 1 ? 1 : (pc.phase == 3 ? 2 : 3));
+        PatchRec& fold = pc.gain_fold[slot];
+        if (bound || fold.p.n > 0) {  // the slot's factors in node order, from the first bound one on (the constant product before it first)
+            if (fold.p.n == 0) {
+                fold = patch(PATCH_GAIN, 1);
+                fold.p.val[0] = pc.inst.g[slot];
+            }
+            if (fold.p.n >= PATCH_OPS) return bail(WAE_UNSUPPORTED, "too many gains folded into one chain slot behind a gain bound from device memory");
+            operand(fold, fold.p.n++, pgn, gv);
+        }
+        pc.inst.g[slot] *= gv;
+        if (may_zero) pc.lay = Lay{1, pc.lay.hi, pc.lay.nlo, pc.lay.nhi, true};  // (k_chain reports a zero slot on its track rows)
+        else if (gv == 0.f && !bound) pc.lay = Lay{1, 1, 1, 1, true};  // a gain of (about) zero answers with silence (gain.rs:160-163)
         return finish_chain(nc, std::move(pc));
     }
     if (!need_out(nc, ch)) return false;
-    if (gv == 0.f) {
+    PatchRec gp = patch(PATCH_GAIN, 1);
+    operand(gp, 0, pgn, gv);
+    if (may_zero) {
+        out_dynamic(nc, or_silent);
+        if (p.out_buf[0].meta) {  // META_COPY, or silent (META_CONST with count 1 and the silent flag) while the bound gain is about zero
+            meta_stage(nc.L, META_COPY, p.in_buf[0], ch, p.out_buf[0], ch, 1, 1);
+            PatchRec mp = gp;
+            mp.p.kind = PATCH_META;
+            add_patch(stage(nc.L, S_META), mp, (uint32_t)offsetof(MetaInst, mode));
+        }
+    } else if (gv == 0.f && !bound) {
         out_dynamic(nc, Lay{1, 1, 1, 1, true});
         if (p.out_buf[0].meta) source_meta(nc, 0, 0, 1);
     } else {
         out_like_input(nc);
     }
-    stage(nc.L, S_GAIN).gain.push_back(GainInst{p.in_buf[0], p.out_buf[0], gv, ch, BufRef{nullptr, 0, 0}});
+    StageBuild& s = stage(nc.L, S_GAIN);
+    s.gain.push_back(GainInst{p.in_buf[0], p.out_buf[0], gv, ch, BufRef{nullptr, 0, 0}});
+    if (bound) add_patch(s, gp, (uint32_t)offsetof(GainInst, gain));
     return true;
 }
 
@@ -2529,6 +2653,11 @@ bool Planner::lower_stereo_panner(NodeCtx& nc) {
     StageBuild& s = stage(nc.L, S_SPAN);
     s.span.push_back(SPanInst{p.in_buf[0], p.out_buf[0], pan, ch, ppan.dyn ? ppan.track : BufRef{nullptr, 0, 0}});
     s.span_gains.push_back(make_float2(gl, gr));
+    if (ppan.bound >= 0) {
+        PatchRec r = patch(PATCH_SPAN, ch);
+        operand(r, 0, ppan, pan);
+        add_patch(s, r, (uint32_t)offsetof(SPanInst, pan), true);
+    }
     return true;
 }
 
@@ -2805,7 +2934,16 @@ bool Planner::lower_compressor(NodeCtx& nc) {
     for (int i = 0; i < 5; i++) c.track[i] = cp[i].dyn ? cp[i].track : BufRef{nullptr, 0, 0};
     c.sample_rate = g->sample_rate;
     c.end = glq;
-    stage(nc.L, S_COMP).comp.push_back(c);
+    StageBuild& s = stage(nc.L, S_COMP);
+    s.comp.push_back(c);
+    const size_t offs[5] = {offsetof(CompInst, attack), offsetof(CompInst, knee), offsetof(CompInst, ratio), offsetof(CompInst, release),
+                            offsetof(CompInst, threshold)};
+    for (int i = 0; i < 5; i++)
+        if (cp[i].bound >= 0) {  // (the kernel takes the raw values)
+            PatchRec r = patch(PATCH_RAW, 1);
+            operand(r, 0, cp[i], cp[i].v);
+            add_patch(s, r, (uint32_t)offs[i]);
+        }
     if (!dry) {
         std::lock_guard<std::recursive_mutex> lk(b->mu);  // (groups are planned on worker threads)
         bool known = false;
@@ -3266,6 +3404,7 @@ struct GroupPlan {  // result of phase B for one group
     uint64_t algorithmic_bytes = 0;
     int code = WAE_OK;
     std::string error;
+    std::vector<std::pair<uint32_t, ParamPatch>> patches;  // (batch position, entry): device addresses set, operands still param ids
 };
 
 static int64_t padded_length(const wae_graph* g) { return (int64_t)((g->length + 127) / 128 * 128); }
@@ -3854,6 +3993,24 @@ static void prep_plan_group(wae_batch* b, wae_graph* const* graphs, int k, PrepS
                 if (!st.d_a) return oom("stage tables");
                 gp.stages.push_back(st);
             }
+            if (st.n > 0 && !s.patches.empty()) {  // patch entries: the device addresses of the fields they re-derive
+                size_t rec_size = 0, rec2_size = 0;
+                switch (s.kind) {
+                    case S_CHAIN: case S_VSUM: rec_size = sizeof(ChainInst); rec2_size = sizeof(ScanCoef); break;
+                    case S_BIQUAD: rec_size = sizeof(BiquadInst); break;
+                    case S_BIQUAD_AR: rec_size = sizeof(BiquadArInst); break;
+                    case S_GAIN: rec_size = sizeof(GainInst); break;
+                    case S_SPAN: rec_size = sizeof(SPanInst); rec2_size = sizeof(float2); break;
+                    case S_COMP: rec_size = sizeof(CompInst); break;
+                    case S_META: rec_size = sizeof(MetaInst); break;
+                }
+                for (const PatchRec& pr : s.patches) {
+                    ParamPatch p = pr.p;
+                    p.dst = static_cast<char*>(st.d_a) + (size_t)pr.rec * rec_size + pr.off;
+                    p.dst2 = pr.rec2 >= 0 ? static_cast<char*>(st.d_b) + (size_t)pr.rec2 * rec2_size : nullptr;
+                    gp.patches.push_back({pr.graph, p});
+                }
+            }
         }
         gp.seg_ranges.push_back({seg_stage0, gp.stages.size()});
     }  // segments
@@ -3910,13 +4067,58 @@ static void record_device_inputs(wae_batch* b, wae_graph* const* graphs, uint32_
 // runs of a batch need every device input bound once
 static wae_status check_bound(wae_batch* b) {
     if (!b) return fail(WAE_INVALID_ARGUMENT, "null batch");
-    if (b->dev_unbound == 0) return WAE_OK;
-    for (auto& d : b->dev_inputs)
-        if (!d.bound) {
+    for (size_t k = 0; b->dev_unbound && k < b->dev_inputs.size(); k++)
+        if (const auto& d = b->dev_inputs[k]; !d.bound) {
             const uint32_t caller = b->order.empty() ? d.graph : b->order[d.graph];
             return fail(WAE_INVALID_STATE, "device input never bound: graph " + std::to_string(caller) + ", node " + std::to_string(d.node) +
                                                " (wae_batch_bind_sources)");
         }
+    if (b->params_unbound == 0) return WAE_OK;
+    for (auto& d : b->bound_params)
+        if (!d.bound) {
+            const uint32_t caller = b->order.empty() ? d.graph : b->order[d.graph];
+            return fail(WAE_INVALID_STATE, "param bound from device memory never bound: graph " + std::to_string(caller) + ", node " +
+                                               std::to_string(d.node) + ", param " + std::to_string(d.param_index) + " (wae_batch_bind_params)");
+        }
+    return WAE_OK;
+}
+
+// The value slots of the params declared with wae_param_set_device_value (`graphs` in batch order: one slot per param, in graph and node
+// order) and the patch entries of the planned groups, their operands renumbered from param ids to slots; both uploaded (from `info` and
+// `patches`, which the caller keeps alive until the stream has been synchronised).
+static wae_status record_params(wae_batch* b, wae_graph* const* graphs, uint32_t n_graphs, std::vector<GroupPlan>& gps,
+                                std::vector<ParamSlotInfo>& info, std::vector<ParamPatch>& patches) {
+    std::unordered_map<uint64_t, int32_t> slot_of;  // (batch position << 32 | param id) -> slot
+    for (uint32_t j = 0; j < n_graphs; j++) {
+        if (!graphs[j]->device_params) continue;
+        for (const auto& kv : graphs[j]->nodes) {
+            const Node& nd = kv.second;
+            if (nd.kind == K_PARAM) continue;
+            for (uint32_t i = 0; i < nd.params.size(); i++) {
+                const Param& prm = graphs[j]->nodes.at(nd.params[i]).param;
+                if (!prm.device_bound) continue;
+                const int32_t slot = (int32_t)b->bound_params.size();
+                slot_of[(uint64_t)j << 32 | nd.params[i]] = slot;
+                b->param_slot[{j, nd.id, i}] = slot;
+                b->bound_params.push_back(wae_batch::BoundParam{j, nd.id, i, false});
+                info.push_back(ParamSlotInfo{prm.device_lo, prm.device_hi, prm.default_value, 0});
+            }
+        }
+    }
+    if (info.empty()) return WAE_OK;
+    b->params_unbound = info.size();
+    for (auto& gp : gps)
+        for (auto& gpp : gp.patches) {
+            ParamPatch p = gpp.second;
+            for (int i = 0; i < PATCH_OPS; i++)
+                if (p.slot[i] >= 0) p.slot[i] = slot_of.at((uint64_t)gpp.first << 32 | (uint32_t)p.slot[i]);
+            patches.push_back(p);
+        }
+    b->d_slot_info = b->dupload_now(info);
+    b->d_values = b->dalloc<float>(info.size(), true);
+    b->n_patches = (int)patches.size();
+    b->d_patches = patches.empty() ? nullptr : b->dupload_now(patches);
+    if (!b->d_slot_info || !b->d_values || (!patches.empty() && !b->d_patches)) return fail(WAE_OUT_OF_MEMORY, "out of device memory (bound params)");
     return WAE_OK;
 }
 
@@ -3980,6 +4182,13 @@ static wae_status prepare_impl(wae_engine* eng, wae_graph* const* graphs, uint32
             wae_batch_destroy(b);
             return cs;
         }
+    }
+    std::vector<ParamSlotInfo> slot_info;
+    std::vector<ParamPatch> patches;
+    st = record_params(b, graphs, n_graphs, gps, slot_info, patches);
+    if (st != WAE_OK) {
+        wae_batch_destroy(b);
+        return st;
     }
     const auto t_prep2 = std::chrono::steady_clock::now();  // planned, allocated, uploads enqueued
     st = prep_finish(b, ps);
@@ -4327,35 +4536,108 @@ WAE_API wae_status wae_batch_run_pipelined(wae_batch* b, float* host_out) {
     return run_pipelined(b, host_out, true);
 }
 
-// The caller's pointer must be device (or managed) memory of the engine's GPU and the whole extent must lie in ONE allocation: checked
-// on the host before anything is enqueued, so that a bad pointer never reaches the kernel.  cuMemGetAddressRange is reached through the
-// runtime's driver entry point (no link dependency on libcuda).
-static wae_status check_bind_extent(int device, const float* pcm, uint64_t extent_floats) {
-    using MemRange = CUresult(CUDAAPI*)(CUdeviceptr*, size_t*, CUdeviceptr);
-    static MemRange mem_range = [] {
-        void* fn = nullptr;
-        cudaDriverEntryPointQueryResult q = cudaDriverEntryPointSymbolNotFound;
-        if (cudaGetDriverEntryPoint("cuMemGetAddressRange", &fn, cudaEnableDefault, &q) != cudaSuccess || q != cudaDriverEntryPointSuccess) {
-            cudaGetLastError();
-            fn = nullptr;
+// The caller's pointers must be device (or managed) memory of the engine's GPU and each extent must lie in ONE allocation: checked on the
+// host before anything is enqueued, so that a bad pointer never reaches a kernel.  cuMemGetAddressRange is reached through the runtime's
+// driver entry point (no link dependency on libcuda).  One checker serves one bind call: the allocations it has looked up are remembered,
+// so items that point into one allocation (the rows of one tensor) cost one pair of driver calls, not one per item.
+struct BindExtents {
+    int device;
+    std::map<uintptr_t, size_t> known;  // base -> bytes of allocations of the engine's GPU looked up so far
+    // `what`: the pointer's name in the messages; `overrun`: the message when the extent runs past the end of its allocation
+    wae_status check(const void* ptr, uint64_t bytes, const char* what, const char* overrun) {
+        const uintptr_t p = (uintptr_t)ptr;
+        auto it = known.upper_bound(p);
+        if (it != known.begin() && p - std::prev(it)->first < std::prev(it)->second) {
+            --it;
+            return fits(p - it->first, it->second, bytes, overrun);
         }
-        return reinterpret_cast<MemRange>(fn);
-    }();
-    cudaPointerAttributes a{};
-    if (cudaPointerGetAttributes(&a, pcm) != cudaSuccess) {
-        cudaGetLastError();
-        return fail(WAE_INVALID_ARGUMENT, "bind: pcm is not device memory");
+        using MemRange = CUresult(CUDAAPI*)(CUdeviceptr*, size_t*, CUdeviceptr);
+        static MemRange mem_range = [] {
+            void* fn = nullptr;
+            cudaDriverEntryPointQueryResult q = cudaDriverEntryPointSymbolNotFound;
+            if (cudaGetDriverEntryPoint("cuMemGetAddressRange", &fn, cudaEnableDefault, &q) != cudaSuccess || q != cudaDriverEntryPointSuccess) {
+                cudaGetLastError();
+                fn = nullptr;
+            }
+            return reinterpret_cast<MemRange>(fn);
+        }();
+        cudaPointerAttributes a{};
+        if (cudaPointerGetAttributes(&a, ptr) != cudaSuccess) {
+            cudaGetLastError();
+            return fail(WAE_INVALID_ARGUMENT, std::string("bind: ") + what + " is not device memory");
+        }
+        if (!(a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged) || a.device != device)
+            return fail(WAE_INVALID_ARGUMENT, std::string("bind: ") + what + " is not device (or managed) memory of the engine's GPU");
+        if (!mem_range) return fail(WAE_CUDA_ERROR, "bind: cuMemGetAddressRange is not available");
+        CUdeviceptr base = 0;
+        size_t size = 0;
+        if (mem_range(&base, &size, (CUdeviceptr)p) != CUDA_SUCCESS)
+            return fail(WAE_INVALID_ARGUMENT, std::string("bind: ") + what + " lies in no device allocation");
+        known[(uintptr_t)base] = size;
+        return fits(p - (uintptr_t)base, size, bytes, overrun);
     }
-    if (!(a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged) || a.device != device)
-        return fail(WAE_INVALID_ARGUMENT, "bind: pcm is not device (or managed) memory of the engine's GPU");
-    if (!mem_range) return fail(WAE_CUDA_ERROR, "bind: cuMemGetAddressRange is not available");
-    CUdeviceptr base = 0;
-    size_t size = 0;
-    if (mem_range(&base, &size, (CUdeviceptr)(uintptr_t)pcm) != CUDA_SUCCESS)
-        return fail(WAE_INVALID_ARGUMENT, "bind: pcm lies in no device allocation");
-    const uint64_t at = (uint64_t)((uintptr_t)pcm - (uintptr_t)base);
-    if (extent_floats > (uint64_t)size / sizeof(float) || at > (uint64_t)size - extent_floats * sizeof(float))
-        return fail(WAE_INVALID_ARGUMENT, "bind: [pcm, pcm + (channels - 1) * channel_stride + length) runs past the end of its allocation");
+    static wae_status fits(uint64_t at, uint64_t size, uint64_t bytes, const char* overrun) {
+        if (bytes > size || at > size - bytes) return fail(WAE_INVALID_ARGUMENT, std::string("bind: ") + overrun);
+        return WAE_OK;
+    }
+};
+
+// A bind runs on the engine stream after the work already queued on the caller's `stream`: any stream of the engine's device,
+// cudaStreamLegacy (the legacy default stream, which a non-blocking engine stream does not wait for by itself) or cudaStreamPerThread
+static wae_status bind_after(wae_batch* b, void* stream) {
+    cudaStream_t s = b->engine->stream;
+    if (stream && (cudaStream_t)stream != s) {
+        if (!b->ev_bind) CUDA_TRY(cudaEventCreateWithFlags(&b->ev_bind, cudaEventDisableTiming));
+        CUDA_TRY(cudaEventRecord(b->ev_bind, (cudaStream_t)stream));
+        CUDA_TRY(cudaStreamWaitEvent(s, b->ev_bind, 0));
+    }
+    return WAE_OK;
+}
+
+// The item table of a bind -> b->d_bind on the engine stream, through a page-locked staging buffer whose last copy has run
+static wae_status stage_bind_table(wae_batch* b, const void* table, size_t bytes) {
+    cudaStream_t s = b->engine->stream;
+    wae_batch::BindStage* stage = nullptr;
+    for (auto& bs : b->bind_stages) {  // a staging buffer whose copy has run
+        if (bs.cap < bytes) continue;
+        const cudaError_t q = cudaEventQuery(bs.ev);
+        if (q == cudaSuccess) {
+            stage = &bs;
+            break;
+        }
+        if (q != cudaErrorNotReady) return fail(WAE_CUDA_ERROR, std::string("bind: ") + cudaGetErrorString(q));
+        cudaGetLastError();  // (not ready is no error)
+    }
+    if (!stage && b->bind_stages.size() >= wae_batch::kMaxBindStages) {  // all in flight: wait for the first one that fits
+        for (auto& bs : b->bind_stages)
+            if (bs.cap >= bytes) {
+                CUDA_TRY(cudaEventSynchronize(bs.ev));
+                stage = &bs;
+                break;
+            }
+    }
+    if (!stage) {
+        const size_t cap = std::max<size_t>(bytes, 64 * sizeof(BindItem));
+        void* hp = nullptr;
+        cudaEvent_t ev = nullptr;
+        if (cudaHostAlloc(&hp, cap, cudaHostAllocDefault) != cudaSuccess) {
+            cudaGetLastError();
+            return fail(WAE_OUT_OF_MEMORY, "out of memory (bind table staging)");
+        }
+        b->pinned.push_back(hp);
+        CUDA_TRY(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
+        b->bind_stages.push_back(wae_batch::BindStage{hp, cap, ev});
+        stage = &b->bind_stages.back();
+    }
+    if (bytes > b->bind_cap) {
+        void* t = b->dalloc<char>(bytes);
+        if (!t) return fail(WAE_OUT_OF_MEMORY, "out of device memory (bind table)");
+        b->d_bind = t;
+        b->bind_cap = bytes;
+    }
+    std::memcpy(stage->h, table, bytes);
+    CUDA_TRY(cudaMemcpyAsync(b->d_bind, stage->h, bytes, cudaMemcpyHostToDevice, s));
+    CUDA_TRY(cudaEventRecord(stage->ev, s));
     return WAE_OK;
 }
 
@@ -4367,6 +4649,7 @@ WAE_API wae_status wae_batch_bind_sources(wae_batch* b, const wae_source_binding
     std::vector<BindItem> table;
     std::vector<size_t> slot_of;
     std::vector<char> named(b->dev_inputs.size(), 0);
+    BindExtents extents{b->engine->device, {}};
     int64_t max_vec = 0;
     int max_ch = 0;
     for (uint32_t i = 0; i < n; i++) {
@@ -4388,7 +4671,8 @@ WAE_API wae_status wae_batch_bind_sources(wae_batch* b, const wae_source_binding
                                                   std::to_string(d.length));
         if (it.channel_stride > (UINT64_MAX / 4 - d.length) / WAE_MAX_CHANNELS)
             return fail(WAE_INVALID_ARGUMENT, "bind: channel_stride runs past the end of its allocation");
-        wae_status st = check_bind_extent(b->engine->device, it.pcm, (uint64_t)(d.channels - 1) * it.channel_stride + d.length);
+        wae_status st = extents.check(it.pcm, ((uint64_t)(d.channels - 1) * it.channel_stride + d.length) * sizeof(float), "pcm",
+                                      "[pcm, pcm + (channels - 1) * channel_stride + length) runs past the end of its allocation");
         if (st != WAE_OK) return st;
         if (!d.slot) continue;  // declared, never rendered: nothing to copy
         table.push_back(BindItem{d.slot, it.pcm, (int64_t)d.stride, (int64_t)it.channel_stride, (int64_t)d.length, (int32_t)d.channels, 0});
@@ -4398,62 +4682,54 @@ WAE_API wae_status wae_batch_bind_sources(wae_batch* b, const wae_source_binding
     }
     const size_t m = table.size();
     if (m == 0) return WAE_OK;
-    cudaStream_t s = b->engine->stream;
-    // `stream` may be any stream of the engine's device, cudaStreamLegacy (the legacy default stream, which a non-blocking engine stream
-    // does not wait for by itself) or cudaStreamPerThread
-    if (stream && (cudaStream_t)stream != s) {
-        if (!b->ev_bind) CUDA_TRY(cudaEventCreateWithFlags(&b->ev_bind, cudaEventDisableTiming));
-        CUDA_TRY(cudaEventRecord(b->ev_bind, (cudaStream_t)stream));
-        CUDA_TRY(cudaStreamWaitEvent(s, b->ev_bind, 0));
-    }
-    wae_batch::BindStage* stage = nullptr;
-    for (auto& bs : b->bind_stages) {  // a staging buffer whose copy has run
-        if (bs.cap < m) continue;
-        const cudaError_t q = cudaEventQuery(bs.ev);
-        if (q == cudaSuccess) {
-            stage = &bs;
-            break;
-        }
-        if (q != cudaErrorNotReady) return fail(WAE_CUDA_ERROR, std::string("bind: ") + cudaGetErrorString(q));
-        cudaGetLastError();  // (not ready is no error)
-    }
-    if (!stage && b->bind_stages.size() >= wae_batch::kMaxBindStages) {  // all in flight: wait for the first one that fits
-        for (auto& bs : b->bind_stages)
-            if (bs.cap >= m) {
-                CUDA_TRY(cudaEventSynchronize(bs.ev));
-                stage = &bs;
-                break;
-            }
-    }
-    if (!stage) {
-        const size_t cap = std::max<size_t>(m, 64);
-        void* hp = nullptr;
-        cudaEvent_t ev = nullptr;
-        if (cudaHostAlloc(&hp, cap * sizeof(BindItem), cudaHostAllocDefault) != cudaSuccess) {
-            cudaGetLastError();
-            return fail(WAE_OUT_OF_MEMORY, "out of memory (bind table staging)");
-        }
-        b->pinned.push_back(hp);
-        CUDA_TRY(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
-        b->bind_stages.push_back(wae_batch::BindStage{(BindItem*)hp, cap, ev});
-        stage = &b->bind_stages.back();
-    }
-    if (m > b->bind_cap) {
-        BindItem* t = b->dalloc<BindItem>(m);
-        if (!t) return fail(WAE_OUT_OF_MEMORY, "out of device memory (bind table)");
-        b->d_bind = t;
-        b->bind_cap = m;
-    }
-    std::memcpy(stage->h, table.data(), m * sizeof(BindItem));
-    CUDA_TRY(cudaMemcpyAsync(b->d_bind, stage->h, m * sizeof(BindItem), cudaMemcpyHostToDevice, s));
-    CUDA_TRY(cudaEventRecord(stage->ev, s));
-    launch_bind_sources(b->d_bind, (int)m, max_vec, max_ch, s);
+    wae_status st = bind_after(b, stream);
+    if (st == WAE_OK) st = stage_bind_table(b, table.data(), m * sizeof(BindItem));
+    if (st != WAE_OK) return st;
+    launch_bind_sources(static_cast<const BindItem*>(b->d_bind), (int)m, max_vec, max_ch, b->engine->stream);
     cudaError_t le = cudaGetLastError();
     if (le != cudaSuccess) return fail(WAE_CUDA_ERROR, std::string("bind: ") + cudaGetErrorString(le));
     for (size_t k : slot_of)
         if (!b->dev_inputs[k].bound) {
             b->dev_inputs[k].bound = true;
             b->dev_unbound--;
+        }
+    return WAE_OK;
+}
+
+WAE_API wae_status wae_batch_bind_params(wae_batch* b, const wae_param_binding* items, uint32_t n, void* stream) {
+    if (!b || (n && !items)) return fail(WAE_INVALID_ARGUMENT, "null batch / items");
+    if (n == 0) return WAE_OK;
+    CUDA_TRY(cudaSetDevice(b->engine->device));
+    // every item is validated before anything is enqueued
+    std::vector<ParamBindItem> table;
+    std::vector<char> named(b->bound_params.size(), 0);
+    BindExtents extents{b->engine->device, {}};
+    for (uint32_t i = 0; i < n; i++) {
+        const wae_param_binding& it = items[i];
+        if (it.graph_index >= b->n_graphs)
+            return fail(WAE_INVALID_STATE, "bind: graph index " + std::to_string(it.graph_index) + " is out of range");
+        auto si = b->param_slot.find(std::make_tuple(b->batch_pos(it.graph_index), it.node, it.param_index));
+        const std::string name = "param " + std::to_string(it.param_index) + " of node " + std::to_string(it.node) + " of graph " +
+                                 std::to_string(it.graph_index);
+        if (si == b->param_slot.end())
+            return fail(WAE_INVALID_STATE, "bind: " + name + " is not bound from device memory (wae_param_set_device_value)");
+        if (named[si->second]++) return fail(WAE_INVALID_ARGUMENT, "bind: " + name + " is named twice in one call");
+        if (!it.value) return fail(WAE_INVALID_ARGUMENT, "bind: null value");
+        wae_status st = extents.check(it.value, sizeof(float), "value", "the value's 4 bytes run past the end of its allocation");
+        if (st != WAE_OK) return st;
+        table.push_back(ParamBindItem{it.value, si->second, 0});
+    }
+    wae_status st = bind_after(b, stream);
+    if (st == WAE_OK) st = stage_bind_table(b, table.data(), table.size() * sizeof(ParamBindItem));
+    if (st != WAE_OK) return st;
+    launch_bind_params(static_cast<const ParamBindItem*>(b->d_bind), (int)table.size(), b->d_slot_info, b->d_values, b->d_patches, b->n_patches,
+                       b->engine->stream);
+    cudaError_t le = cudaGetLastError();
+    if (le != cudaSuccess) return fail(WAE_CUDA_ERROR, std::string("bind: ") + cudaGetErrorString(le));
+    for (const ParamBindItem& t : table)
+        if (!b->bound_params[t.slot].bound) {
+            b->bound_params[t.slot].bound = true;
+            b->params_unbound--;
         }
     return WAE_OK;
 }
@@ -4906,12 +5182,16 @@ WAE_API wae_status wae_selftest_conv_fft(float* data, uint32_t mode) {
     return WAE_OK;
 }
 
-// a one-shot call renders the graphs before a caller could bind anything to their device inputs
+// a one-shot call renders the graphs before a caller could bind anything to their device inputs or device-bound params
 static wae_status refuse_device_inputs(wae_graph* const* graphs, uint32_t n_graphs) {
-    for (uint32_t i = 0; graphs && i < n_graphs; i++)
+    for (uint32_t i = 0; graphs && i < n_graphs; i++) {
         if (graphs[i] && graphs[i]->device_inputs)
             return fail(WAE_INVALID_STATE, "graph " + std::to_string(i) + " has device inputs: render it with wae_batch_prepare (or _prepare_many), "
                                            "wae_batch_bind_sources and wae_batch_run");
+        if (graphs[i] && graphs[i]->device_params)
+            return fail(WAE_INVALID_STATE, "graph " + std::to_string(i) + " has params bound from device memory: render it with wae_batch_prepare "
+                                           "(or _prepare_many), wae_batch_bind_params and wae_batch_run");
+    }
     return WAE_OK;
 }
 

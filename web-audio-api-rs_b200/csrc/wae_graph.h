@@ -95,6 +95,10 @@ struct Param {  // AudioParam: its own graph node in the reference (src/context/
     bool a_rate = false;
     bool rate_constrained = false;
     std::vector<ParamEv> events;  // in arrival order
+    // wae_param_set_device_value: the value is supplied per run from device memory (wae_batch_bind_params), clamped to
+    // [device_lo, device_hi] (the declared range intersected with [min_value, max_value]); planned as constant_value()
+    bool device_bound = false;
+    float device_lo = 0.f, device_hi = 0.f;
     // lowering helpers
     bool constant() const;        // only SetValue events: value is constant over the render
     float constant_value() const; // clamped like AudioParamProcessor::mix_to_output (src/param.rs:755-760)
@@ -248,6 +252,7 @@ struct wae_graph {
     // hundreds of grains, src/buffer.rs:69-72) shares ONE host copy — and so one copy in the device slab (Planner::buf_offsets)
     std::vector<std::weak_ptr<wae::PcmBuffer>> assets[2];
     uint32_t device_inputs = 0;  // AudioBufferSourceNodes declared with wae_buffer_source_set_device_input (never in `assets`)
+    uint32_t device_params = 0;  // AudioParams declared with wae_param_set_device_value
 
     uint32_t create_param(uint32_t owner, float def, float mn, float mx, bool a_rate, float initial, bool send_set_value = true,
                           bool fixed_id = false, uint32_t id = 0, bool constrained = false);

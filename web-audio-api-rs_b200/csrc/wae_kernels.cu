@@ -4408,6 +4408,62 @@ __global__ void __launch_bounds__(256) k_bind_sources(const BindItem* __restrict
     }
 }
 
+// wae_batch_bind_params, step 1: each item's float from the caller's device memory into its value slot, clamped to the declared range
+// as AudioParam::set_value clamps (param.rs:407-413).  A non-finite value takes the param's default value, the reference's rule for a
+// NaN computed value (param.rs:755-795): a device bind cannot panic as the reference's set_value does.
+__global__ void __launch_bounds__(256) k_bind_params(const ParamBindItem* __restrict__ items, int n, const ParamSlotInfo* __restrict__ info,
+                                                     float* __restrict__ values) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const ParamBindItem it = items[i];
+    const ParamSlotInfo si = info[it.slot];
+    float v = *it.src;
+    if (!isfinite(v)) v = si.def;
+    else v = fminf(fmaxf(v, si.lo), si.hi);
+    values[it.slot] = v;
+}
+
+// step 2: every patch entry of the batch re-derived from the value slots and its planned constants, with the planner's own formulas
+DEVI float patch_op(const ParamPatch& p, int i, const float* values) { return p.slot[i] >= 0 ? values[p.slot[i]] : p.val[i]; }
+DEVI float patch_gain_product(const ParamPatch& p, const float* values) {
+    float g = 1.f;
+    for (int i = 0; i < p.n && i < PATCH_OPS; i++) {
+        float f = patch_op(p, i, values);
+        if (p.slot[i] >= 0) {  // gain.rs:153-169, as Planner::lower_gain applies it to a constant gain
+            if (fabsf(f) <= 1e-6f) f = 0.f;
+            else if (fabsf(1.f - f) <= 1e-6f) f = 1.f;
+        }
+        g *= f;
+    }
+    return g;
+}
+__global__ void __launch_bounds__(64) k_derive_params(const ParamPatch* __restrict__ patches, int n, const float* __restrict__ values) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const ParamPatch& p = patches[i];
+    switch (p.kind) {
+        case PATCH_GAIN: *static_cast<float*>(p.dst) = patch_gain_product(p, values); break;
+        case PATCH_META: *static_cast<int32_t*>(p.dst) = patch_gain_product(p, values) == 0.f ? META_CONST : META_COPY; break;
+        case PATCH_BIQUAD: {
+            const float q = patch_op(p, 0, values), detune = patch_op(p, 1, values), freq = patch_op(p, 2, values), gain = patch_op(p, 3, values);
+            const float computed = detune != 0.f ? freq * exp2f(detune / 1200.f) : freq;  // get_computed_freq, biquad_filter.rs:393-399
+            const BqC c = bq_coefs(p.n, (double)p.sample_rate, (double)computed, (double)gain, (double)q);
+            double* d = static_cast<double*>(p.dst);
+            d[0] = c.b0; d[1] = c.b1; d[2] = c.b2; d[3] = c.a1; d[4] = c.a2;
+            if (p.dst2) make_scan_coef(c.b1, c.b2, c.a1, c.a2, *static_cast<ScanCoef*>(p.dst2));
+            break;
+        }
+        case PATCH_SPAN: {  // stereo_panner.rs:247-249,274-276 and get_stereo_gains (:74-79), as k_stereo_panner computes them
+            const float pan = patch_op(p, 0, values), PI32 = 3.14159265358979323846f;
+            const float x = p.n == 1 ? (pan + 1.f) * 0.5f : (pan <= 0.f ? pan + 1.f : pan);
+            *static_cast<float*>(p.dst) = pan;
+            *static_cast<float2*>(p.dst2) = make_float2(sinf((1.f - x) * PI32 / 2.f), sinf(x * PI32 / 2.f));
+            break;
+        }
+        default: *static_cast<float*>(p.dst) = patch_op(p, 0, values); break;
+    }
+}
+
 // ---------------------------------------------------------------------------------------------------------
 // launchers
 // ---------------------------------------------------------------------------------------------------------
@@ -4699,6 +4755,11 @@ void launch_bind_sources(const BindItem* d, int n, int64_t max_vec, int max_ch, 
     // about four vectors per thread along a channel; items beyond 65535 are walked by the grid-stride loop over blockIdx.y
     const int64_t bx = std::max<int64_t>(1, std::min<int64_t>((max_vec + 1023) / 1024, 65535));
     k_bind_sources<<<dim3((unsigned)bx, (unsigned)std::min(n, 65535), (unsigned)max_ch), 256, 0, s>>>(d, n);
+}
+void launch_bind_params(const ParamBindItem* d, int n, const ParamSlotInfo* info, float* values, const ParamPatch* patches, int n_patches,
+                        cudaStream_t s) {
+    k_bind_params<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(d, n, info, values);
+    if (n_patches > 0) k_derive_params<<<(unsigned)((n_patches + 63) / 64), 64, 0, s>>>(patches, n_patches, values);
 }
 void launch_conv_ir_fft(const float* ir, int64_t ir_len, int64_t ir_stride, float2* h, int S, int channels, cudaStream_t s) {
     conv_configure();

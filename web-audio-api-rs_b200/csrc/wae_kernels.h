@@ -23,6 +23,45 @@ struct ScanCoef {
 };
 constexpr int WAE_CHAIN_PRE_TILES = 16;  // 32768 frames (k_chain PRE: slabs of WAE_CHAIN_PRE_TILES << pre_log2 tiles)
 
+// The scan constants of one biquad, in f64: one source for the planner (host) and for k_bind_params (device, bound coefficients).  The
+// build compiles without FMA contraction on both sides, so equal coefficients give bit-equal constants.
+struct ScanM2 {
+    double a, b, c, d;
+};
+WAE_HD ScanM2 scan_mul(const ScanM2& x, const ScanM2& y) {
+    return ScanM2{x.a * y.a + x.b * y.c, x.a * y.b + x.b * y.d, x.c * y.a + x.d * y.c, x.c * y.b + x.d * y.d};
+}
+WAE_HD void make_scan_coef(double b1, double b2, double a1, double a2, ScanCoef& sc) {
+    const ScanM2 M{-a1, -a2, 1., 0.};
+    ScanM2 r{1., 0., 0., 1.};
+    for (int j = 0; j < WAE_CHAIN_K; j++) r = scan_mul(M, r);
+    const ScanM2 A = r;  // M^K: one thread of k_chain
+    ScanM2 pw = A;
+    for (int d = 0; d < 5; d++) {
+        sc.Pshfl[d][0] = pw.a; sc.Pshfl[d][1] = pw.b; sc.Pshfl[d][2] = pw.c; sc.Pshfl[d][3] = pw.d;
+        pw = scan_mul(pw, pw);
+    }
+    sc.Pwarp[0] = pw.a; sc.Pwarp[1] = pw.b; sc.Pwarp[2] = pw.c; sc.Pwarp[3] = pw.d;  // A^32
+    ScanM2 pl = A;
+    for (int l = 0; l < 32; l++) {
+        sc.Plane[l][0] = pl.a; sc.Plane[l][1] = pl.b; sc.Plane[l][2] = pl.c; sc.Plane[l][3] = pl.d;
+        pl = scan_mul(A, pl);
+    }
+    // one frame with zero input: (x1, x2, y1, y2) -> (0, x1, b1 x1 + b2 x2 - a1 y1 - a2 y2, y1); G^L by squaring (L = 2^15 frames)
+    static_assert(WAE_CHAIN_PRE_TILES * WAE_CHAIN_K * 128 == 1 << 15, "GL below is G^(2^15)");
+    double g[16] = {0., 0., 0., 0., 1., 0., 0., 0., b1, b2, -a1, -a2, 0., 0., 1., 0.}, h[16];
+    for (int sq = 0; sq < 15; sq++) {
+        for (int rr = 0; rr < 4; rr++)
+            for (int cc = 0; cc < 4; cc++) {
+                double a = 0.;
+                for (int k = 0; k < 4; k++) a += g[4 * rr + k] * g[4 * k + cc];
+                h[4 * rr + cc] = a;
+            }
+        for (int i = 0; i < 16; i++) g[i] = h[i];
+    }
+    for (int i = 0; i < 16; i++) sc.GL[i] = g[i];
+}
+
 void upload_twiddles();                          // convolver FFT tables (computed in wae_kernels.cu, f64 -> f32)
 void conv_fft_selftest(float* data, int mode);   // host emulation of the convolver transforms (wae_selftest_conv_fft)
 void launch_oscillator(const OscInst* d, int n, ChunkInfo ci, cudaStream_t s);
@@ -67,6 +106,9 @@ void launch_conv_mac_ifft(const ConvPath* p, const ConvInput* in, int n, ChunkIn
 void launch_conv_compact(const ConvCmpInst* d, int n, ChunkInfo ci, cudaStream_t s);
 // one launch for all items of a bind call; max_vec = the largest slot stride / 4, max_ch = the most channels of an item
 void launch_bind_sources(const BindItem* d, int n, int64_t max_vec, int max_ch, cudaStream_t s);
+// a bind of n param values into their slots (k_bind_params), then every patch entry of the batch re-derived from the slots (k_derive_params)
+void launch_bind_params(const ParamBindItem* d, int n, const ParamSlotInfo* info, float* values, const ParamPatch* patches, int n_patches,
+                        cudaStream_t s);
 void launch_conv_ir_fft(const float* ir, int64_t ir_len, int64_t ir_stride, float2* h, int S, int channels, cudaStream_t s);
 
 }  // namespace wae
