@@ -559,6 +559,36 @@ typedef struct wae_param_binding {
  * param of the batch has never been bound. */
 WAE_API wae_status wae_batch_bind_params(wae_batch* batch, const wae_param_binding* items, uint32_t n, void* stream);
 
+/* ---- ConvolverNode responses bound from device memory -----------------------------------------------------------------------
+ * Declares a ConvolverNode whose impulse response is supplied per run from device memory (wae_batch_bind_responses) instead of an
+ * AudioBuffer, so that one prepared batch convolves with any number of response sets (room impulse responses drawn or generated on the
+ * GPU) without being built and planned again.  The declaration counts as the node's set_buffer: it fixes the normalisation (the
+ * `normalize` attribute as it is now), with set_buffer's checks and texts (WAE_NOT_SUPPORTED: a channel count other than 1, 2 or 4, a
+ * rate other than the context's; AudioBuffer::new's text for length 0).  The node is planned with ceil(length / 8192) partitions on
+ * every channel, as an untrimmed response of that length would be; normalisation and the trimming of the quiet tail run on the device
+ * in the bind, so a bound response renders exactly as an AudioBuffer of the same content given to set_buffer.
+ * WAE_INVALID_STATE: the node already has a response, is declared twice, or the graph already has a suspend point; set_buffer after the
+ * declaration answers WAE_INVALID_STATE.  Suspend points added later are allowed (every segment reads the one bound response).
+ * wae_render_batch and wae_render_many answer WAE_INVALID_STATE on graphs with such nodes; wae_batch_plan plans them. */
+WAE_API wae_status wae_convolver_set_device_response(wae_graph* graph, wae_node_id node, uint32_t number_of_channels,
+                                                     uint64_t length, float sample_rate);
+
+typedef struct wae_response_binding {
+    uint32_t graph_index;    /* caller's index, as wae_batch_fetch_graph */
+    wae_node_id node;        /* declared with wae_convolver_set_device_response */
+    const float* pcm;        /* device memory of the engine's GPU: channel c is `length` floats at pcm + c * channel_stride */
+    uint64_t channel_stride; /* floats, >= the declared length; any alignment */
+} wae_response_binding;
+
+/* Normalises, trims and transforms the responses on the device, asynchronously on the engine stream after the work already queued on
+ * `stream` (as wae_batch_bind_sources).  All-or-nothing: every item is validated before anything is enqueued.  A bound response stays
+ * until it is bound again.  WAE_INVALID_ARGUMENT: `pcm` is not device (or managed) memory of the engine's GPU, the extent does not lie
+ * in one allocation, channel_stride is below the declared length, one (graph, node) is named twice in the call, or the call has more
+ * than 65535 items that the batch renders.  WAE_INVALID_STATE:
+ * graph_index out of range, or the node was not declared.  wae_batch_run, wae_batch_run_group and wae_batch_run_pipelined answer
+ * WAE_INVALID_STATE while a declared response of the batch has never been bound. */
+WAE_API wae_status wae_batch_bind_responses(wae_batch* batch, const wae_response_binding* items, uint32_t n, void* stream);
+
 /* PeriodicWave::new(context, PeriodicWaveOptions { real, imag, disable_normalization }) (src/periodic_wave.rs:104-209): fills `table`
  * (PERIODIC_WAVE_TABLE_LENGTH = 2048 in the reference) with the wavetable an OscillatorNode of type Custom plays.  `real` / `imag` may be
  * NULL (= zeros); both NULL = the sine default.  Host math, no engine needed. */

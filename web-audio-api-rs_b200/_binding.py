@@ -128,6 +128,11 @@ class ParamBinding(C.Structure):
     _fields_ = [("graph_index", C.c_uint32), ("node", C.c_uint32), ("param_index", C.c_uint32), ("value", c_float_p)]
 
 
+class ResponseBinding(C.Structure):
+    """wae_response_binding: the device impulse response of one declared ConvolverNode of a prepared batch (wae_batch_bind_responses)."""
+    _fields_ = [("graph_index", C.c_uint32), ("node", C.c_uint32), ("pcm", c_float_p), ("channel_stride", C.c_uint64)]
+
+
 STATUS_NAMES = {0: "OK", 1: "INVALID_ARGUMENT", 2: "INVALID_STATE", 3: "NOT_SUPPORTED", 4: "UNSUPPORTED",
                 5: "CUDA_ERROR", 6: "OUT_OF_MEMORY", 7: "NO_DEVICE"}
 
@@ -168,6 +173,7 @@ WAE_SYMBOLS = [
     "wae_render_many", "wae_batch_prepare_many", "wae_batch_graph_output", "wae_batch_fetch_graph", "wae_batch_plan_many", "wae_batch_plan_quanta",
     "wae_buffer_source_set_device_input", "wae_batch_bind_sources",
     "wae_param_set_device_value", "wae_batch_bind_params",
+    "wae_convolver_set_device_response", "wae_batch_bind_responses",
 ]
 
 
@@ -274,6 +280,9 @@ class Api:
             # param values bound from device memory
             f("param_set_device_value", C.c_int32, [gp, C.c_uint32, C.c_uint32, C.c_float, C.c_float])
             f("batch_bind_params", C.c_int32, [C.c_void_p, C.POINTER(ParamBinding), C.c_uint32, C.c_void_p])
+            # convolver responses bound from device memory
+            f("convolver_set_device_response", C.c_int32, [gp, C.c_uint32, C.c_uint32, C.c_uint64, C.c_float])
+            f("batch_bind_responses", C.c_int32, [C.c_void_p, C.POINTER(ResponseBinding), C.c_uint32, C.c_void_p])
         else:
             f("graph_create", C.c_int32, [C.c_uint32, C.c_uint64, C.c_float, C.POINTER(C.c_void_p)])
             f("render", C.c_int32, [gp, c_float_p])

@@ -306,6 +306,16 @@ class ConvolverNode(AudioNode):
     def set_buffer(self, buffer):
         self._set_buffer("convolver_set_buffer", buffer)
 
+    def set_device_response(self, number_of_channels, length, sample_rate):
+        """wae_convolver_set_device_response (product only): the node convolves with a response of this shape that
+        Batch.bind_responses supplies from device memory before each run, instead of an AudioBuffer.  Counts as the node's set_buffer
+        (the normalisation is decided now)."""
+        api = self._ctx._api
+        if not api.is_product:
+            raise B.WaeError(3, "convolver responses bound from device memory are a feature of the GPU engine")
+        api.check(api.convolver_set_device_response(self._ctx._g, self.id, int(number_of_channels), int(length), float(sample_rate)))
+        self._ctx._device_responses[self.id] = (int(number_of_channels), int(length))
+
     def set_normalize(self, value):
         self._set_attribute(B.ATTR_NORMALIZE, 1.0 if value else 0.0)
 
@@ -454,6 +464,7 @@ class OfflineAudioContext:
         self._suspends = []
         self._current_time = 0.0
         self._device_inputs = {}  # node id -> (channels, length) declared with set_device_input
+        self._device_responses = {}  # node id -> (channels, length) declared with set_device_response
 
     def __del__(self):
         try:
@@ -765,9 +776,25 @@ class Batch:
         dimension) becomes the audio of device input nodes[k] of context graphs[k] (default: 0..n-1).  `nodes`: one node (or id) for all
         graphs (graphs built the same way share ids) or one per graph.  One call, ordered after torch's current stream (its default
         stream included); the copy runs on the engine stream, and the tensor's memory is kept from reuse until it has (record_stream)."""
+        items, n = self._pcm_items("bind_sources", "pcm", nodes, pcm, graphs, "_device_inputs", B.SourceBinding)
+        self.api.check(self.api.batch_bind_sources(self.handle, items, n, C.c_void_p(self._torch_stream_handle())))
+        self._keep_until_read(pcm)
+
+    def bind_responses(self, nodes, ir, graphs=None):
+        """wae_batch_bind_responses: ir[k] ([channels][length] of a float32 CUDA tensor [n][channels][length], unit stride on the last
+        dimension) becomes the impulse response of ConvolverNode nodes[k] (declared with set_device_response) of context graphs[k]
+        (default: 0..n-1).  `nodes` as for bind_sources.  One call, ordered after torch's current stream; the response is normalised,
+        trimmed and transformed on the engine stream, and the tensor's memory is kept from reuse until it has been read."""
+        items, n = self._pcm_items("bind_responses", "ir", nodes, ir, graphs, "_device_responses", B.ResponseBinding)
+        self.api.check(self.api.batch_bind_responses(self.handle, items, n, C.c_void_p(self._torch_stream_handle())))
+        self._keep_until_read(ir)
+
+    def _pcm_items(self, fn, arg, nodes, pcm, graphs, declarations, Struct):
+        """The binding items (graph index, node, device pointer, channel stride) of bind_sources / bind_responses: `declarations` names
+        the contexts' {node id: (channels, length)} the tensor's shape is checked against."""
         import torch
         if not (isinstance(pcm, torch.Tensor) and pcm.is_cuda and pcm.dtype == torch.float32 and pcm.dim() == 3):
-            raise B.WaeError(1, "bind_sources: pcm must be a float32 CUDA tensor [n][channels][length]")
+            raise B.WaeError(1, f"{fn}: {arg} must be a float32 CUDA tensor [n][channels][length]")
         n = pcm.shape[0]
         graphs = list(range(n)) if graphs is None else [int(g) for g in graphs]
         if isinstance(nodes, (list, tuple)):
@@ -775,25 +802,24 @@ class Batch:
         else:
             ids = [getattr(nodes, "id", nodes)] * n
         if len(graphs) != n or len(ids) != n:
-            raise B.WaeError(1, f"bind_sources: {n} tensors for {len(graphs)} graphs and {len(ids)} nodes")
+            raise B.WaeError(1, f"{fn}: {n} tensors for {len(graphs)} graphs and {len(ids)} nodes")
         if n and pcm.stride(2) != 1:
-            raise B.WaeError(1, "bind_sources: the frames of a channel must be contiguous (unit stride on the last dimension)")
-        items = (B.SourceBinding * max(n, 1))()
+            raise B.WaeError(1, f"{fn}: the frames of a channel must be contiguous (unit stride on the last dimension)")
+        items = (Struct * max(n, 1))()
         base = pcm.data_ptr()
         # (torch may give the channel dimension of a one-channel tensor any stride: only channel 0 is read then)
         channel_stride = pcm.stride(1) if pcm.shape[1] > 1 else pcm.shape[2]
         for k, (g, nid) in enumerate(zip(graphs, ids)):
             if not 0 <= g < self.n:
-                raise B.WaeError(2, f"bind_sources: graph index {g} is out of range")
-            declared = self.contexts[g]._device_inputs.get(int(nid))
+                raise B.WaeError(2, f"{fn}: graph index {g} is out of range")
+            declared = getattr(self.contexts[g], declarations).get(int(nid))
             # the library checks the CUDA allocation; torch's caching allocator may hold several tensors in one, so the tensor's own
             # shape is checked here
             if declared is not None and (pcm.shape[1], pcm.shape[2]) != declared:
-                raise B.WaeError(1, f"bind_sources: pcm[{k}] is [{pcm.shape[1]}][{pcm.shape[2]}], node {nid} of graph {g} was declared "
+                raise B.WaeError(1, f"{fn}: {arg}[{k}] is [{pcm.shape[1]}][{pcm.shape[2]}], node {nid} of graph {g} was declared "
                                     f"[{declared[0]}][{declared[1]}]")
-            items[k] = B.SourceBinding(g, int(nid), C.cast(C.c_void_p(base + 4 * k * pcm.stride(0)), B.c_float_p), channel_stride)
-        self.api.check(self.api.batch_bind_sources(self.handle, items, n, C.c_void_p(self._torch_stream_handle())))
-        self._keep_until_read(pcm)
+            items[k] = Struct(g, int(nid), C.cast(C.c_void_p(base + 4 * k * pcm.stride(0)), B.c_float_p), channel_stride)
+        return items, n
 
     def _keep_until_read(self, t):
         """Keeps torch's caching allocator from reusing a bound tensor's memory before the engine stream has read it.  The tensor is

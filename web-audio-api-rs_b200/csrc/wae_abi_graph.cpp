@@ -1068,6 +1068,8 @@ WAE_API wae_status wae_buffer_source_set_device_input(wae_graph* g, wae_node_id 
 WAE_API wae_status wae_convolver_set_buffer(wae_graph* g, wae_node_id node, const wae_audio_buffer* buffer) {
     Node* n = node_of_kind(g, node, K_CONV);
     if (!n || !buffer) return fail(WAE_INVALID_ARGUMENT, "not a ConvolverNode / null buffer");
+    if (n->buffer && n->buffer->device_input)
+        return fail(WAE_INVALID_STATE, "InvalidStateError - the response is bound from device memory (wae_convolver_set_device_response)");
     if (buffer->sample_rate != g->sample_rate)
         return fail(WAE_NOT_SUPPORTED, "NotSupportedError - sample rate of the convolution buffer must match the audio context");
     const uint32_t c = buffer->number_of_channels;
@@ -1078,6 +1080,35 @@ WAE_API wae_status wae_convolver_set_buffer(wae_graph* g, wae_node_id node, cons
     if (!fresh) return WAE_NOT_SUPPORTED;
     n->buffer = fresh;
     n->normalize = n->normalize_next;
+    return WAE_OK;
+}
+
+// A declared response counts as the node's set_buffer: a placeholder of the declared shape and rate with no host block, never shared by
+// content (not in g->assets).  The normalisation is decided now, as set_buffer decides it; the scale itself is computed in the bind.
+WAE_API wae_status wae_convolver_set_device_response(wae_graph* g, wae_node_id node, uint32_t number_of_channels, uint64_t length,
+                                                     float sample_rate) {
+    Node* n = node_of_kind(g, node, K_CONV);
+    if (!n) return fail(WAE_INVALID_ARGUMENT, "not a ConvolverNode");
+    // set_buffer's checks, in its order, then AudioBuffer::new's for the length (src/buffer.rs:96-115)
+    if (sample_rate != g->sample_rate)
+        return fail(WAE_NOT_SUPPORTED, "NotSupportedError - sample rate of the convolution buffer must match the audio context");
+    const uint32_t c = number_of_channels;
+    if (!(c == 1 || c == 2 || c == 4)) return fail(WAE_NOT_SUPPORTED, "NotSupportedError - the convolution buffer must consist of 1, 2 or 4 channels");
+    if (length == 0) return fail(WAE_NOT_SUPPORTED, "NotSupportedError - Invalid length: 0 is less than or equal to minimum bound (0)");
+    if (n->buffer && n->buffer->device_input)
+        return fail(WAE_INVALID_STATE, "InvalidStateError - the response is already bound from device memory (wae_convolver_set_device_response)");
+    if (n->buffer) return fail(WAE_INVALID_STATE, "InvalidStateError - the ConvolverNode already has a response (set_buffer)");
+    if (!g->epochs.empty())  // (the segments before the suspend point were planned with the graph copy of their own: no response)
+        return fail(WAE_INVALID_STATE, "InvalidStateError - a response is bound from device memory before the first suspend point");
+    auto p = std::make_shared<PcmBuffer>();
+    p->sample_rate = sample_rate;
+    p->device_input = true;
+    p->stride = (size_t)length;
+    p->channels.resize(number_of_channels);
+    for (auto& ch : p->channels) ch.n = (size_t)length;
+    n->buffer = std::move(p);
+    n->normalize = n->normalize_next;
+    g->device_responses++;
     return WAE_OK;
 }
 

@@ -521,6 +521,22 @@ struct BindItem {
     int32_t pad;
 };
 
+// ---- wae_batch_bind_responses: caller device audio -> the IR spectra of a declared ConvolverNode response --------------------------
+struct RespBindItem {
+    const float* src;    // caller's response: channel c is `len` floats at src + c * src_stride (any alignment)
+    float2* h;           // the node's spectra: [channels][S + WAE_CONV_H_PAD][WAE_CONV_SPEC], padding partitions zero
+    int64_t src_stride;  // floats
+    int64_t len;         // declared length
+    float sample_rate;   // the response's rate (normalisation)
+    int32_t channels;    // 1, 2 or 4
+    int32_t S;           // partitions: ceil(len / WAE_CONV_BLOCK)
+    int32_t normalize;
+    // written on the device by the bind's kernels: the scale (1 when not normalising) and per channel the trimmed length m (0 on entry)
+    float scale;
+    int32_t m[4];
+    int32_t pad;
+};
+
 // ---- wae_batch_bind_params: per-run values of params planned as constants ------------------------------------------------------
 struct ParamBindItem {  // one float of the caller's device memory -> value slot `slot`
     const float* src;

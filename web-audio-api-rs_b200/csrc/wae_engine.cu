@@ -444,6 +444,23 @@ struct wae_batch {
     float* d_values = nullptr;
     ParamPatch* d_patches = nullptr;
     int n_patches = 0;
+    // wae_convolver_set_device_response: the spectra of each declared response (made by the planner), rewritten by
+    // wae_batch_bind_responses.  A declared response the planner never reached (its convolver renders nothing) has no spectra: binding it
+    // is validated and writes nothing.
+    struct DevResponse {
+        uint32_t graph;  // batch position
+        wae_node_id node;
+        float2* h;       // [channels][S + WAE_CONV_H_PAD][WAE_CONV_SPEC]
+        uint32_t channels;
+        uint64_t length;
+        int S;
+        bool normalize;
+        float sample_rate;
+        bool bound;
+    };
+    std::vector<DevResponse> responses;
+    std::map<std::pair<uint32_t, wae_node_id>, size_t> response_index;  // (batch position, node) -> responses
+    size_t responses_unbound = 0;
     cudaEvent_t ev_bind = nullptr;  // orders a bind after the caller's stream
     // OfflineAudioContext::suspend_sync: a group's render is cut at the suspend frames of its graphs (graphs with different
     // suspend points are put in different groups); every segment has its own plan, node state is shared between the plans
@@ -1068,6 +1085,7 @@ struct Planner {
     // a two-channel input is mixed down to mono by the forward transform's loads (ConvInput::in_channel = -1)
     bool plan_convolver(PNode& pn, int level, const BufRef* dest = nullptr, int64_t dest_limit = -1, const PcmBuffer* ir_override = nullptr);
     bool ir_spectra(const PcmBuffer& ir, float scale, const std::vector<std::vector<float>>& scaled, int Smax, IrSpectra& spec);
+    bool device_response_spectra(const Node& n, int S, IrSpectra& spec);
     bool conv_compact_path(PNode& pn, int level, int in_ch, const IrSpectra& spec, int Smax, int blocks_per_chunk);
     // chain fusion
     int consumers(uint32_t id) {
@@ -1417,9 +1435,12 @@ bool Planner::plan_convolver(PNode& pn, int level, const BufRef* dest, int64_t d
     const PcmBuffer& ir = ir_override ? *ir_override : *n.buffer;
     int ir_ch = (int)ir.channels.size();
     size_t ir_len = ir.length();
+    // a response bound from device memory (wae_convolver_set_device_response): planned as an untrimmed response of the declared length;
+    // the bind normalises, trims and transforms it on the device
+    const bool declared = !ir_override && ir.device_input;
     // normalize_buffer, src/node/convolver.rs:16-53 (f32, channel by channel)
     float scale = 1.f;
-    if (n.normalize && !ir_override) {
+    if (n.normalize && !ir_override && !declared) {
         float power = 0.f;
         for (auto& c : ir.channels) {
             float s = 0.f;
@@ -1436,15 +1457,15 @@ bool Planner::plan_convolver(PNode& pn, int level, const BufRef* dest, int64_t d
     // convolvers: one per IR channel, a mono IR is duplicated (convolver.rs:289-293)
     int n_conv = std::max(ir_ch, 2);
     // trailing samples below 1e-6 are ignored by fft-convolver's init
-    std::vector<std::vector<float>> scaled(ir_ch);
-    size_t trimmed_len = 0;
-    for (int c = 0; c < ir_ch; c++) {
+    std::vector<std::vector<float>> scaled(declared ? 0 : ir_ch);
+    size_t trimmed_len = declared ? ir_len : 0;
+    for (int c = 0; c < (declared ? 0 : ir_ch); c++) {
         scaled[c].resize(ir_len);
         for (size_t i = 0; i < ir_len; i++) scaled[c][i] = ir.channels[c][i] * scale;
     }
     // per-channel trimmed length (each FFTConvolver trims its own IR); use per channel S
-    std::vector<int> S(ir_ch);
-    for (int c = 0; c < ir_ch; c++) {
+    std::vector<int> S(ir_ch, declared ? (int)((ir_len + WAE_CONV_BLOCK - 1) / WAE_CONV_BLOCK) : 0);
+    for (int c = 0; c < (declared ? 0 : ir_ch); c++) {
         size_t m = ir_len;
         while (!ir_override && m > 0 && std::fabs(scaled[c][m - 1]) < 0.000001f) m--;
         while (ir_override && m > 0 && scaled[c][m - 1] == 0.f) m--;  // (exact zeros only)
@@ -1505,7 +1526,7 @@ bool Planner::plan_convolver(PNode& pn, int level, const BufRef* dest, int64_t d
         return true;
     }
     IrSpectra spec;
-    if (!ir_spectra(ir, scale, scaled, Smax, spec)) return false;
+    if (!(declared ? device_response_spectra(n, Smax, spec) : ir_spectra(ir, scale, scaled, Smax, spec))) return false;
     // inputs: one spectra ring per input channel
     StageBuild& fs = stage(level, S_CONV_FFT);
     int blocks_per_chunk = (int)((b->chunk + WAE_CONV_BLOCK - 1) / WAE_CONV_BLOCK);
@@ -1594,6 +1615,33 @@ bool Planner::ir_spectra(const PcmBuffer& ir, float scale, const std::vector<std
         b->asset_bytes += (size_t)ir_ch * (Smax + WAE_CONV_H_PAD) * WAE_CONV_SPEC * 8;
         (*ir_cache)[key] = spec;
     }
+    return true;
+}
+
+// The spectra of a response bound from device memory: one zeroed [ch][S + WAE_CONV_H_PAD][WAE_CONV_SPEC] allocation per (batch graph,
+// node), never shared by content, that wae_batch_bind_responses rewrites in full on every bind (the padding partitions stay zero).  It is
+// keyed in the cache by (graph, node), so every suspend segment and both paths of a mono response read the same memory, and entered in
+// the batch's response table when it is made.
+bool Planner::device_response_spectra(const Node& n, int S, IrSpectra& spec) {
+    const PcmBuffer& ir = *n.buffer;
+    const int ir_ch = (int)ir.channels.size();
+    const uint64_t tag[3] = {0x646576696365ull /* "device" */, key_graph, n.id};
+    const uint64_t key = fnv1a(tag, sizeof(tag));
+    std::unique_lock<std::recursive_mutex> ir_lock(b->mu);
+    auto it = ir_cache->find(key);
+    if (it != ir_cache->end()) {
+        spec = it->second;
+        return true;
+    }
+    spec.S = S;
+    spec.channels = ir_ch;
+    spec.h = dry ? reinterpret_cast<float2*>(uintptr_t(256)) : b->dalloc<float2>((size_t)ir_ch * (S + WAE_CONV_H_PAD) * WAE_CONV_SPEC, true);
+    if (!spec.h) return bail(WAE_OUT_OF_MEMORY, "out of device memory (IR spectra)");
+    b->asset_bytes += (size_t)ir_ch * (S + WAE_CONV_H_PAD) * WAE_CONV_SPEC * 8;
+    (*ir_cache)[key] = spec;
+    if (!dry)
+        b->responses.push_back(wae_batch::DevResponse{key_graph, n.id, spec.h, (uint32_t)ir_ch, (uint64_t)ir.length(), S, n.normalize,
+                                                      ir.sample_rate, false});
     return true;
 }
 
@@ -4064,9 +4112,38 @@ static void record_device_inputs(wae_batch* b, wae_graph* const* graphs, uint32_
     }
 }
 
-// runs of a batch need every device input bound once
+// The declared responses of the batch (`graphs` in batch order), after planning: the ones the planner gave spectra, all unbound, then
+// the declared ones it never reached, which binding validates and writes nothing to, and which runs do not wait for.
+static void record_responses(wae_batch* b, wae_graph* const* graphs, uint32_t n_graphs) {
+    std::sort(b->responses.begin(), b->responses.end(),
+              [](const wae_batch::DevResponse& x, const wae_batch::DevResponse& y) { return std::tie(x.graph, x.node) < std::tie(y.graph, y.node); });
+    for (size_t k = 0; k < b->responses.size(); k++) b->response_index[{b->responses[k].graph, b->responses[k].node}] = k;
+    b->responses_unbound = b->responses.size();
+    for (uint32_t j = 0; j < n_graphs; j++) {
+        if (!graphs[j]->device_responses) continue;
+        auto scan = [&](const NodeMap& nodes) {
+            for (const auto& kv : nodes) {
+                const Node& nd = kv.second;
+                if (nd.kind != K_CONV || !nd.buffer || !nd.buffer->device_input || b->response_index.count({j, nd.id})) continue;
+                b->response_index[{j, nd.id}] = b->responses.size();
+                b->responses.push_back(wae_batch::DevResponse{j, nd.id, nullptr, (uint32_t)nd.buffer->channels.size(), (uint64_t)nd.buffer->length(),
+                                                              0, nd.normalize, nd.buffer->sample_rate, true});
+            }
+        };
+        scan(graphs[j]->nodes);
+        for (const auto& ep : graphs[j]->epochs) scan(ep.nodes);
+    }
+}
+
+// runs of a batch need every device input, param and response bound once
 static wae_status check_bound(wae_batch* b) {
     if (!b) return fail(WAE_INVALID_ARGUMENT, "null batch");
+    for (size_t k = 0; b->responses_unbound && k < b->responses.size(); k++)
+        if (const auto& d = b->responses[k]; !d.bound) {
+            const uint32_t caller = b->order.empty() ? d.graph : b->order[d.graph];
+            return fail(WAE_INVALID_STATE, "response bound from device memory never bound: graph " + std::to_string(caller) + ", node " +
+                                               std::to_string(d.node) + " (wae_batch_bind_responses)");
+        }
     for (size_t k = 0; b->dev_unbound && k < b->dev_inputs.size(); k++)
         if (const auto& d = b->dev_inputs[k]; !d.bound) {
             const uint32_t caller = b->order.empty() ? d.graph : b->order[d.graph];
@@ -4183,6 +4260,7 @@ static wae_status prepare_impl(wae_engine* eng, wae_graph* const* graphs, uint32
             return cs;
         }
     }
+    record_responses(b, graphs, n_graphs);
     std::vector<ParamSlotInfo> slot_info;
     std::vector<ParamPatch> patches;
     st = record_params(b, graphs, n_graphs, gps, slot_info, patches);
@@ -4734,6 +4812,76 @@ WAE_API wae_status wae_batch_bind_params(wae_batch* b, const wae_param_binding* 
     return WAE_OK;
 }
 
+// The spectra are rewritten in full on the engine stream: runs queued before the bind have read the previous ones by then.
+WAE_API wae_status wae_batch_bind_responses(wae_batch* b, const wae_response_binding* items, uint32_t n, void* stream) {
+    if (!b || (n && !items)) return fail(WAE_INVALID_ARGUMENT, "null batch / items");
+    if (n == 0) return WAE_OK;
+    CUDA_TRY(cudaSetDevice(b->engine->device));
+    // every item is validated before anything is enqueued
+    std::vector<RespBindItem> table;
+    std::vector<size_t> resp_of;
+    std::vector<char> named(b->responses.size(), 0);
+    BindExtents extents{b->engine->device, {}};
+    int64_t max_len = 0;
+    int max_S = 0, max_ch = 0;
+    bool any_normalize = false;
+    for (uint32_t i = 0; i < n; i++) {
+        const wae_response_binding& it = items[i];
+        if (it.graph_index >= b->n_graphs)
+            return fail(WAE_INVALID_STATE, "bind: graph index " + std::to_string(it.graph_index) + " is out of range");
+        auto ri = b->response_index.find({b->batch_pos(it.graph_index), it.node});
+        if (ri == b->response_index.end())
+            return fail(WAE_INVALID_STATE, "bind: node " + std::to_string(it.node) + " of graph " + std::to_string(it.graph_index) +
+                                               " is not a response bound from device memory (wae_convolver_set_device_response)");
+        const size_t k = ri->second;
+        if (named[k]++)  // (two items of one launch writing one set of spectra: which one lands would be undefined)
+            return fail(WAE_INVALID_ARGUMENT, "bind: node " + std::to_string(it.node) + " of graph " + std::to_string(it.graph_index) +
+                                                  " is named twice in one call");
+        const wae_batch::DevResponse& d = b->responses[k];
+        if (!it.pcm) return fail(WAE_INVALID_ARGUMENT, "bind: null pcm");
+        if (it.channel_stride < d.length)
+            return fail(WAE_INVALID_ARGUMENT, "bind: channel_stride " + std::to_string(it.channel_stride) + " is below the declared length " +
+                                                  std::to_string(d.length));
+        if (it.channel_stride > (UINT64_MAX / 4 - d.length) / 4)
+            return fail(WAE_INVALID_ARGUMENT, "bind: channel_stride runs past the end of its allocation");
+        wae_status st = extents.check(it.pcm, ((uint64_t)(d.channels - 1) * it.channel_stride + d.length) * sizeof(float), "pcm",
+                                      "[pcm, pcm + (channels - 1) * channel_stride + length) runs past the end of its allocation");
+        if (st != WAE_OK) return st;
+        if (!d.h) continue;  // declared, never rendered: nothing to write
+        RespBindItem r{};
+        r.src = it.pcm;
+        r.h = d.h;
+        r.src_stride = (int64_t)it.channel_stride;
+        r.len = (int64_t)d.length;
+        r.sample_rate = d.sample_rate;
+        r.channels = (int32_t)d.channels;
+        r.S = d.S;
+        r.normalize = d.normalize ? 1 : 0;
+        r.scale = 1.f;
+        table.push_back(r);
+        resp_of.push_back(k);
+        max_len = std::max<int64_t>(max_len, r.len);
+        max_S = std::max(max_S, d.S);
+        max_ch = std::max(max_ch, (int)d.channels);
+        any_normalize |= d.normalize;
+    }
+    const size_t m = table.size();
+    if (m == 0) return WAE_OK;
+    if (m > 65535) return fail(WAE_INVALID_ARGUMENT, "bind: more than 65535 responses in one call");
+    wae_status st = bind_after(b, stream);
+    if (st == WAE_OK) st = stage_bind_table(b, table.data(), m * sizeof(RespBindItem));
+    if (st != WAE_OK) return st;
+    launch_bind_responses(static_cast<RespBindItem*>(b->d_bind), (int)m, any_normalize, max_len, max_S, max_ch, b->engine->stream);
+    cudaError_t le = cudaGetLastError();
+    if (le != cudaSuccess) return fail(WAE_CUDA_ERROR, std::string("bind: ") + cudaGetErrorString(le));
+    for (size_t k : resp_of)
+        if (!b->responses[k].bound) {
+            b->responses[k].bound = true;
+            b->responses_unbound--;
+        }
+    return WAE_OK;
+}
+
 WAE_API wae_status wae_batch_sync(wae_batch* b) {
     CUDA_TRY(cudaSetDevice(b->engine->device));
     CUDA_TRY(cudaStreamSynchronize(b->engine->stream));
@@ -5191,6 +5339,9 @@ static wae_status refuse_device_inputs(wae_graph* const* graphs, uint32_t n_grap
         if (graphs[i] && graphs[i]->device_params)
             return fail(WAE_INVALID_STATE, "graph " + std::to_string(i) + " has params bound from device memory: render it with wae_batch_prepare "
                                            "(or _prepare_many), wae_batch_bind_params and wae_batch_run");
+        if (graphs[i] && graphs[i]->device_responses)
+            return fail(WAE_INVALID_STATE, "graph " + std::to_string(i) + " has convolver responses bound from device memory: render it with "
+                                           "wae_batch_prepare (or _prepare_many), wae_batch_bind_responses and wae_batch_run");
     }
     return WAE_OK;
 }

@@ -58,7 +58,8 @@ struct PcmBuffer {  // an AudioBuffer asset (src/buffer.rs:69-72), host copy: ON
     size_t stride = 0, bytes = 0;
     bool pinned = false;
     // wae_buffer_source_set_device_input: a placeholder of the declared shape (channels[c].n = length) with no host block; its PCM is
-    // written into the device slab by wae_batch_bind_sources, and nothing copies host memory over it
+    // written into the device slab by wae_batch_bind_sources, and nothing copies host memory over it.  The response of a ConvolverNode
+    // declared with wae_convolver_set_device_response is such a placeholder too: its spectra are written by wae_batch_bind_responses
     bool device_input = false;
     PcmBuffer() = default;
     PcmBuffer(const PcmBuffer&) = delete;
@@ -253,6 +254,7 @@ struct wae_graph {
     std::vector<std::weak_ptr<wae::PcmBuffer>> assets[2];
     uint32_t device_inputs = 0;  // AudioBufferSourceNodes declared with wae_buffer_source_set_device_input (never in `assets`)
     uint32_t device_params = 0;  // AudioParams declared with wae_param_set_device_value
+    uint32_t device_responses = 0;  // ConvolverNodes declared with wae_convolver_set_device_response (never in `assets`)
 
     uint32_t create_param(uint32_t owner, float def, float mn, float mx, bool a_rate, float initial, bool send_set_value = true,
                           bool fixed_id = false, uint32_t id = 0, bool constrained = false);

@@ -4233,6 +4233,98 @@ __global__ void __launch_bounds__(CV_THREADS) k_conv_ir_fft(const float* __restr
     rfft_store(z, h + ((size_t)c * (S + WAE_CONV_H_PAD) + WAE_CONV_H_PAD_LO + seg) * CV_BINS, lane_tw);  // (padding partitions stay zero)
 }
 
+// ---- wae_batch_bind_responses: the planner's normalisation, trimming and IR transform (plan_convolver), on the device --------------
+// Three launches for all items of a bind: the power of the normalising items, the trimmed length of every (item, channel), the spectra.
+
+// normalize_buffer (src/node/convolver.rs:16-53) with the planner's f32 operations in the planner's order, so that the scale is
+// bit-equal to the one the host computes for an AudioBuffer of the same content: per channel a sequential sum of s * s, then the
+// channels added in order.  One CTA per item; lane c of warp 0 runs channel c's dependent chain out of shared memory while the other
+// warps load the next tile of every channel (coalesced, any alignment).  Items that do not normalise keep the scale 1.
+constexpr int RB_TILE = 1024;
+__global__ void __launch_bounds__(256) k_resp_power(RespBindItem* __restrict__ items) {
+    __shared__ float buf[2][4][RB_TILE + 1];  // (+1: the four summing lanes read four different banks)
+    __shared__ float part[4];
+    RespBindItem& it = items[blockIdx.x];
+    if (!it.normalize) return;
+    const int ch = it.channels, t = threadIdx.x, warp = t >> 5;
+    const int64_t len = it.len;
+    const int64_t ntiles = (len + RB_TILE - 1) / RB_TILE;
+    auto load = [&](int64_t tile, int b, int t0, int nt) {
+        const int64_t f0 = tile * RB_TILE;
+        const int cnt = (int)(len - f0 < RB_TILE ? len - f0 : RB_TILE);
+        for (int k = t - t0; k < ch * RB_TILE; k += nt) {
+            const int c = k / RB_TILE, i = k % RB_TILE;
+            if (i < cnt) buf[b][c][i] = __ldcs(it.src + (int64_t)c * it.src_stride + f0 + i);
+        }
+    };
+    load(0, 0, 0, blockDim.x);
+    __syncthreads();
+    float s = 0.f;
+    for (int64_t tile = 0; tile < ntiles; tile++) {
+        if (warp != 0) {
+            if (tile + 1 < ntiles) load(tile + 1, (int)((tile + 1) & 1), 32, blockDim.x - 32);
+        } else if (t < ch) {
+            const float* __restrict__ x = buf[tile & 1][t];
+            const int cnt = (int)(len - tile * RB_TILE < RB_TILE ? len - tile * RB_TILE : RB_TILE);
+#pragma unroll 16
+            for (int i = 0; i < cnt; i++) s = __fadd_rn(s, __fmul_rn(x[i], x[i]));
+        }
+        __syncthreads();
+    }
+    if (t < ch) part[t] = s;
+    __syncthreads();
+    if (t == 0) {
+        float power = 0.f;
+        for (int c = 0; c < ch; c++) power = __fadd_rn(power, part[c]);
+        power = __fsqrt_rn(__fdiv_rn(power, (float)((uint64_t)ch * (uint64_t)len)));
+        if (!isfinite(power) || power < 0.000125f) power = 0.000125f;
+        float scale = __fdiv_rn(1.f, power);
+        scale = __fmul_rn(scale, 0.00125f);
+        scale = __fmul_rn(scale, __fdiv_rn(44100.f, it.sample_rate));
+        if (ch == 4) scale = __fmul_rn(scale, 0.5f);
+        it.scale = scale;
+    }
+}
+
+// fft-convolver's init ignores the trailing samples below 1e-6: m = 1 + the last index whose scaled sample is not below it (the host's
+// comparison, so NaN stops the trim), found as a max over the frames.  grid: (frame blocks, items, channels); it.m[c] is 0 on entry.
+__global__ void __launch_bounds__(256) k_resp_trim(RespBindItem* __restrict__ items) {
+    RespBindItem& it = items[blockIdx.y];
+    const int c = blockIdx.z;
+    if (c >= it.channels) return;
+    const float* __restrict__ src = it.src + (int64_t)c * it.src_stride;
+    const float scale = it.scale;
+    int best = 0;
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < it.len; i += (int64_t)gridDim.x * blockDim.x)
+        if (!(fabsf(__fmul_rn(__ldg(src + i), scale)) < 0.000001f)) best = (int)(i + 1);
+    best = __reduce_max_sync(0xffffffffu, best);
+    if ((threadIdx.x & 31) == 0 && best > 0) atomicMax(&it.m[c], best);
+}
+
+// The spectra of partition seg of channel c: the packed real FFT of x[i] * scale for i < m, zero after it — the values the planner
+// uploads for an AudioBuffer, through k_conv_ir_fft's transform.  Every partition < S is written; the padding ones stay zero.
+// grid: (partitions, channels, items)
+__global__ void __launch_bounds__(CV_THREADS) k_resp_fft(const RespBindItem* __restrict__ items) {
+    extern __shared__ float2 z[];
+    const RespBindItem& it = items[blockIdx.z];
+    const int seg = blockIdx.x, c = blockIdx.y;
+    if (seg >= it.S || c >= it.channels) return;
+    const FftTw w = fft_tw_load(-1);
+    const float2 lane_tw = cv_lane_tw();
+    const float* __restrict__ src = it.src + (int64_t)c * it.src_stride + (int64_t)seg * CV_B;
+    const int64_t left = (int64_t)it.m[c] - (int64_t)seg * CV_B;
+    const int valid = (int)(left < 0 ? 0 : left < CV_B ? left : CV_B);
+    const float scale = it.scale;
+    for (int i = threadIdx.x; i < CV_B / 2; i += CV_THREADS) {  // segment in the first half, zeros in the second
+        const int n = 2 * i;
+        z[cv_pad(i)] = make_float2(n < valid ? __fmul_rn(__ldg(src + n), scale) : 0.f, n + 1 < valid ? __fmul_rn(__ldg(src + n + 1), scale) : 0.f);
+    }
+    conv_load_half(z, CV_B / 2, nullptr, 0);
+    __syncthreads();
+    fft_dif_smem(z, w);
+    rfft_store(z, it.h + ((size_t)c * (it.S + WAE_CONV_H_PAD) + WAE_CONV_H_PAD_LO + seg) * CV_BINS, lane_tw);
+}
+
 // Host emulation of the transforms above with the SAME butterfly, index and twiddle code (tests/test_conv_fft_host.py pins them against
 // numpy on a machine without a GPU).  mode 0: complex forward, natural -> position order; 1: complex inverse, position -> natural order
 // (unnormalised); 2: 2B reals -> B packed bins in position order; 3: B packed bins -> 2B reals (scaled by 1 / 2B).  data: 2B floats in place.
@@ -4724,6 +4816,7 @@ static void conv_configure() {
     cudaFuncSetAttribute(k_conv_fft_in, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     cudaFuncSetAttribute(k_conv_ifft, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     cudaFuncSetAttribute(k_conv_ir_fft, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    cudaFuncSetAttribute(k_resp_fft, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     cudaFuncSetAttribute(k_conv_cmp_fft, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     cudaFuncSetAttribute(k_conv_cmp_ifft, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     configured = true;
@@ -4760,6 +4853,14 @@ void launch_bind_params(const ParamBindItem* d, int n, const ParamSlotInfo* info
                         cudaStream_t s) {
     k_bind_params<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(d, n, info, values);
     if (n_patches > 0) k_derive_params<<<(unsigned)((n_patches + 63) / 64), 64, 0, s>>>(patches, n_patches, values);
+}
+void launch_bind_responses(RespBindItem* d, int n, bool any_normalize, int64_t max_len, int max_S, int max_ch, cudaStream_t s) {
+    conv_configure();
+    if (any_normalize) k_resp_power<<<(unsigned)n, 256, 0, s>>>(d);
+    // about eight frames per thread; items and their channels in y / z (n <= 65535: checked by the caller)
+    const int64_t bx = std::max<int64_t>(1, std::min<int64_t>((max_len + 2047) / 2048, 65535));
+    k_resp_trim<<<dim3((unsigned)bx, (unsigned)n, (unsigned)max_ch), 256, 0, s>>>(d);
+    k_resp_fft<<<dim3((unsigned)max_S, (unsigned)max_ch, (unsigned)n), CV_THREADS, CV_SMEM_ELEMS * sizeof(float2), s>>>(d);
 }
 void launch_conv_ir_fft(const float* ir, int64_t ir_len, int64_t ir_stride, float2* h, int S, int channels, cudaStream_t s) {
     conv_configure();
