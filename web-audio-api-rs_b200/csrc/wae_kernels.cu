@@ -460,6 +460,27 @@ DEVI float mix_channel(LD ld, int s, int dst_ch, int c, int interp) {
         default: return c < s ? ld(c) : 0.f;
     }
 }
+// Where channel c of a quantum of s channels mixed to dst_ch channels comes from (quantum.rs:292-502): the channel it moves or copies
+// (>= 0), the silent channel the mix pushes (-1), or a sum it computes (-2).  AudioRenderQuantumChannel::add (quantum.rs:114-120) skips a
+// silent channel instead of adding its zeros and takes the other one as it is onto a silent one, so a -0.0 keeps the sign an added +0.0
+// would take from it.
+DEVI int mix_source(int s, int dst_ch, int c, int interp) {
+    if (s == dst_ch) return c;
+    if (interp == 1 || s > 6 || dst_ch > 6) return c < s ? c : -1;
+    switch (s * 16 + dst_ch) {
+        case 1 * 16 + 2: return 0;
+        case 1 * 16 + 4: return c < 2 ? 0 : -1;
+        case 1 * 16 + 6: return c == 2 ? 0 : -1;
+        case 2 * 16 + 4:
+        case 2 * 16 + 6: return c < 2 ? c : -1;
+        case 4 * 16 + 5: return c < 2 ? c : (c == 2 ? -1 : c - 1);
+        case 4 * 16 + 6: return c < 2 ? c : (c < 4 ? -1 : c - 2);
+        case 2 * 16 + 1: case 4 * 16 + 1: case 6 * 16 + 1: case 4 * 16 + 2: case 6 * 16 + 2: return -2;
+        case 6 * 16 + 4: return c < 2 ? -2 : c + 2;
+        default: return c < s ? c : -1;
+    }
+}
+DEVI bool mix_is_silence(int s, int dst_ch, int c, int interp) { return mix_source(s, dst_ch, c, interp) == -1; }
 DEVI float mixed_sample(const MixEdge& e, int dst_ch, int c, int interp, int n, const ChunkInfo& ci) {
     return mix_channel([&](int ch) { return chan(e.src, ch, ci)[n]; }, e.src_ch, dst_ch, c, interp);
 }
@@ -475,6 +496,7 @@ DEVI void mix_dyn_stereo4(const MixDynInst& m, const MixEdge* __restrict__ edges
     float4 a0 = make_float4(0.f, 0.f, 0.f, 0.f), a1 = a0;
     int cnt = 1;
     bool silent = true;
+    bool held1 = false;  // channel 1 of the running sum is not the silent channel (a discrete 1 -> 2 mix pushes silence: mix_source)
     const bool speakers = m.interp == 0;
     for (int e = 0; e < m.n_edges; e++) {
         const MixEdge& ed = edges[m.edge_offset + e];
@@ -483,8 +505,12 @@ DEVI void mix_dyn_stereo4(const MixDynInst& m, const MixEdge* __restrict__ edges
         const int mx = cnt > ce ? cnt : ce;
         const int nw = m.mode == WAE_COUNT_MODE_MAX ? mx : (m.mode == WAE_COUNT_MODE_EXPLICIT ? m.cfg_count : (mx < m.cfg_count ? mx : m.cfg_count));
         if (!silent && nw != cnt) {  // self.mix(new_channels): 1 -> 2 copy (speakers) / zero-fill (discrete); 2 -> 1 half sum / truncate
-            if (nw == 2) a1 = speakers ? a0 : make_float4(0.f, 0.f, 0.f, 0.f);
-            else if (speakers) a0 = make_float4(0.5f * (a0.x + a1.x), 0.5f * (a0.y + a1.y), 0.5f * (a0.z + a1.z), 0.5f * (a0.w + a1.w));
+            if (nw == 2) {
+                a1 = speakers ? a0 : make_float4(0.f, 0.f, 0.f, 0.f);
+                held1 = speakers;
+            } else if (speakers) {
+                a0 = make_float4(0.5f * (a0.x + a1.x), 0.5f * (a0.y + a1.y), 0.5f * (a0.z + a1.z), 0.5f * (a0.w + a1.w));
+            }
         }
         cnt = nw;
         if (!se) {
@@ -493,13 +519,18 @@ DEVI void mix_dyn_stereo4(const MixDynInst& m, const MixEdge* __restrict__ edges
             if (ce == 2) v1 = *reinterpret_cast<const float4*>(chan(ed.src, 1, ci) + n0);
             float4 x0 = v0, x1 = v1;  // the edge mixed to nw channels
             if (nw == 1 && ce == 2 && speakers) x0 = make_float4(0.5f * (v0.x + v1.x), 0.5f * (v0.y + v1.y), 0.5f * (v0.z + v1.z), 0.5f * (v0.w + v1.w));
-            if (nw == 2 && ce == 1 && !speakers) x1 = make_float4(0.f, 0.f, 0.f, 0.f);
+            const bool x1_silence = nw == 2 && ce == 1 && !speakers;
             if (silent) {
                 a0 = x0;
-                a1 = x1;
             } else {
                 a0.x += x0.x; a0.y += x0.y; a0.z += x0.z; a0.w += x0.w;
-                if (nw == 2) { a1.x += x1.x; a1.y += x1.y; a1.z += x1.z; a1.w += x1.w; }
+            }
+            if (nw == 2 && !x1_silence) {
+                if (silent || !held1) a1 = x1;
+                else { a1.x += x1.x; a1.y += x1.y; a1.z += x1.z; a1.w += x1.w; }
+                held1 = true;
+            } else if (silent) {
+                a1 = make_float4(0.f, 0.f, 0.f, 0.f);
             }
             silent = false;
         }
@@ -532,6 +563,7 @@ __global__ void __launch_bounds__(128) k_mix_dyn(const MixDynInst* __restrict__ 
         if (n >= ci.nf) continue;
         const int qi = meta_qi(ci, n);
         float acc[32], tmp[32];
+        uint32_t held = 0;  // bit c: channel c of the running sum is not the silent channel
         int cnt = 1;
         bool silent = true;
         for (int e = 0; e < m.n_edges; e++) {
@@ -541,18 +573,28 @@ __global__ void __launch_bounds__(128) k_mix_dyn(const MixDynInst* __restrict__ 
             const int mx = cnt > ce ? cnt : ce;
             const int nw = m.mode == WAE_COUNT_MODE_MAX ? mx : (m.mode == WAE_COUNT_MODE_EXPLICIT ? m.cfg_count : (mx < m.cfg_count ? mx : m.cfg_count));
             if (!silent && nw != cnt) {  // self.mix(new_channels, interpretation)
-                for (int c = 0; c < nw; c++) tmp[c] = mix_channel([&](int ch) { return acc[ch]; }, cnt, nw, c, m.interp);
+                uint32_t h = 0;
+                for (int c = 0; c < nw; c++) {
+                    tmp[c] = mix_channel([&](int ch) { return acc[ch]; }, cnt, nw, c, m.interp);
+                    const int from = mix_source(cnt, nw, c, m.interp);  // a moved channel stays what it was, a computed one is held
+                    if (from == -2 || (from >= 0 && ((held >> from) & 1u))) h |= 1u << c;
+                }
                 for (int c = 0; c < nw; c++) acc[c] = tmp[c];
+                held = h;
             }
             cnt = nw;
             if (!se) {
                 for (int c = 0; c < nw; c++) {
+                    if (mix_is_silence(ce, nw, c, m.interp)) continue;
                     const float v = mix_channel([&](int ch) { return chan(ed.src, ch, ci)[n]; }, ce, nw, c, m.interp);
-                    acc[c] = silent ? v : acc[c] + v;
+                    acc[c] = (held >> c) & 1u ? acc[c] + v : v;
+                    held |= 1u << c;
                 }
                 silent = false;
             }
         }
+        for (int c = 0; c < cnt; c++)
+            if (!((held >> c) & 1u)) acc[c] = 0.f;
         if ((n & 127) == 0 && m.out.meta) meta_put_all(m.out, m.out_ch, qi, cnt, silent);
         if (m.limit >= 0 && ci.f0 + n >= m.limit) continue;
         for (int c = 0; c < m.out_ch; c++) {
@@ -765,9 +807,13 @@ __global__ void __launch_bounds__(256) k_mix(const MixInst* __restrict__ insts, 
             if (m.limit >= 0 && ci.f0 + n >= m.limit) continue;
             for (int c = 0; c < m.out_ch; c++) {
                 float acc = 0.f;
+                bool any = false;
                 for (int e = 0; e < m.n_edges; e++) {
-                    float v = mixed_sample(edges[m.edge_offset + e], m.out_ch, c, m.interp, n, ci);
-                    acc = e == 0 ? v : acc + v;
+                    const MixEdge& ed = edges[m.edge_offset + e];
+                    if (mix_is_silence(ed.src_ch, m.out_ch, c, m.interp)) continue;
+                    const float v = mixed_sample(ed, m.out_ch, c, m.interp, n, ci);
+                    acc = any ? acc + v : v;
+                    any = true;
                 }
                 chan(m.out, c, ci)[n] = acc;
             }
@@ -807,9 +853,13 @@ __global__ void __launch_bounds__(256) k_mix_narrow(const MixInst* __restrict__ 
             if (m.limit >= 0 && ci.f0 + n >= m.limit) continue;
             for (int c = 0; c < m.out_ch; c++) {
                 float acc = 0.f;
+                bool any = false;
                 for (int e = 0; e < m.n_edges; e++) {
-                    float v = mixed_sample(edges[m.edge_offset + e], m.out_ch, c, m.interp, n, ci);
-                    acc = e == 0 ? v : acc + v;
+                    const MixEdge& ed = edges[m.edge_offset + e];
+                    if (mix_is_silence(ed.src_ch, m.out_ch, c, m.interp)) continue;
+                    const float v = mixed_sample(ed, m.out_ch, c, m.interp, n, ci);
+                    acc = any ? acc + v : v;
+                    any = true;
                 }
                 chan(m.out, c, ci)[n] = acc;
             }
