@@ -589,6 +589,31 @@ typedef struct wae_response_binding {
  * WAE_INVALID_STATE while a declared response of the batch has never been bound. */
 WAE_API wae_status wae_batch_bind_responses(wae_batch* batch, const wae_response_binding* items, uint32_t n, void* stream);
 
+/* ---- WaveShaperNode curves bound from device memory -------------------------------------------------------------------------
+ * Declares a WaveShaperNode whose curve of `length` points is supplied per run from device memory (wae_batch_bind_curves) instead of
+ * set_curve, so that one prepared batch shapes with any number of curve sets (saturation / distortion curves drawn on the GPU) without
+ * being built and planned again.  The declaration counts as the node's set_curve; the oversample attribute stays settable.  Any length
+ * >= 1 is accepted (WAE_INVALID_ARGUMENT: 0).  WAE_INVALID_STATE: the node already has a curve (options or set_curve), is declared
+ * twice, or the graph already has a suspend point; set_curve after the declaration answers WAE_INVALID_STATE.  Suspend points added
+ * later are allowed (every segment reads the one bound curve).  Whether the curve maps 0 to 0 (can_propagate_silence) is decided
+ * per bind on the device; the plan covers both answers.  wae_render_batch and wae_render_many answer WAE_INVALID_STATE on graphs with
+ * such nodes; wae_batch_plan plans them. */
+WAE_API wae_status wae_wave_shaper_set_device_curve(wae_graph* graph, wae_node_id node, uint32_t length);
+
+typedef struct wae_curve_binding {
+    uint32_t graph_index;   /* caller's index, as wae_batch_fetch_graph */
+    wae_node_id node;       /* declared with wae_wave_shaper_set_device_curve */
+    const float* curve;     /* device memory of the engine's GPU: `length` floats, any alignment */
+} wae_curve_binding;
+
+/* Copies the curves into the batch, asynchronously on the engine stream after the work already queued on `stream` (as
+ * wae_batch_bind_sources).  The values are used bit for bit, NaN and infinities included.  All-or-nothing: every item is validated before
+ * anything is enqueued.  A bound curve stays until it is bound again.  WAE_INVALID_ARGUMENT: `curve` is null or not device (or managed)
+ * memory of the engine's GPU, [curve, curve + length) does not lie in one allocation, or one (graph, node) is named twice in the call.
+ * WAE_INVALID_STATE: graph_index out of range, or the node was not declared.  wae_batch_run, wae_batch_run_group and
+ * wae_batch_run_pipelined answer WAE_INVALID_STATE while a declared curve of the batch has never been bound. */
+WAE_API wae_status wae_batch_bind_curves(wae_batch* batch, const wae_curve_binding* items, uint32_t n, void* stream);
+
 /* PeriodicWave::new(context, PeriodicWaveOptions { real, imag, disable_normalization }) (src/periodic_wave.rs:104-209): fills `table`
  * (PERIODIC_WAVE_TABLE_LENGTH = 2048 in the reference) with the wavetable an OscillatorNode of type Custom plays.  `real` / `imag` may be
  * NULL (= zeros); both NULL = the sine default.  Host math, no engine needed. */

@@ -133,6 +133,11 @@ class ResponseBinding(C.Structure):
     _fields_ = [("graph_index", C.c_uint32), ("node", C.c_uint32), ("pcm", c_float_p), ("channel_stride", C.c_uint64)]
 
 
+class CurveBinding(C.Structure):
+    """wae_curve_binding: the device curve of one declared WaveShaperNode of a prepared batch (wae_batch_bind_curves)."""
+    _fields_ = [("graph_index", C.c_uint32), ("node", C.c_uint32), ("curve", c_float_p)]
+
+
 STATUS_NAMES = {0: "OK", 1: "INVALID_ARGUMENT", 2: "INVALID_STATE", 3: "NOT_SUPPORTED", 4: "UNSUPPORTED",
                 5: "CUDA_ERROR", 6: "OUT_OF_MEMORY", 7: "NO_DEVICE"}
 
@@ -174,6 +179,7 @@ WAE_SYMBOLS = [
     "wae_buffer_source_set_device_input", "wae_batch_bind_sources",
     "wae_param_set_device_value", "wae_batch_bind_params",
     "wae_convolver_set_device_response", "wae_batch_bind_responses",
+    "wae_wave_shaper_set_device_curve", "wae_batch_bind_curves",
 ]
 
 
@@ -283,6 +289,9 @@ class Api:
             # convolver responses bound from device memory
             f("convolver_set_device_response", C.c_int32, [gp, C.c_uint32, C.c_uint32, C.c_uint64, C.c_float])
             f("batch_bind_responses", C.c_int32, [C.c_void_p, C.POINTER(ResponseBinding), C.c_uint32, C.c_void_p])
+            # WaveShaper curves bound from device memory
+            f("wave_shaper_set_device_curve", C.c_int32, [gp, C.c_uint32, C.c_uint32])
+            f("batch_bind_curves", C.c_int32, [C.c_void_p, C.POINTER(CurveBinding), C.c_uint32, C.c_void_p])
         else:
             f("graph_create", C.c_int32, [C.c_uint32, C.c_uint64, C.c_float, C.POINTER(C.c_void_p)])
             f("render", C.c_int32, [gp, c_float_p])

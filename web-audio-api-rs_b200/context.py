@@ -327,6 +327,15 @@ class WaveShaperNode(AudioNode):
         api = self._ctx._api
         api.check(api.wave_shaper_set_curve(self._ctx._g, self.id, B.fptr(c), len(c)))
 
+    def set_device_curve(self, length):
+        """wae_wave_shaper_set_device_curve (product only): the node shapes with a curve of `length` points that Batch.bind_curves
+        supplies from device memory before each run.  Counts as the node's set_curve."""
+        api = self._ctx._api
+        if not api.is_product:
+            raise B.WaeError(3, "WaveShaper curves bound from device memory are a feature of the GPU engine")
+        api.check(api.wave_shaper_set_device_curve(self._ctx._g, self.id, int(length)))
+        self._ctx._device_curves[self.id] = int(length)
+
     def set_oversample(self, oversample):
         self._set_attribute(B.ATTR_OVERSAMPLE, oversample)
 
@@ -465,6 +474,7 @@ class OfflineAudioContext:
         self._current_time = 0.0
         self._device_inputs = {}  # node id -> (channels, length) declared with set_device_input
         self._device_responses = {}  # node id -> (channels, length) declared with set_device_response
+        self._device_curves = {}  # node id -> length declared with set_device_curve
 
     def __del__(self):
         try:
@@ -788,6 +798,45 @@ class Batch:
         items, n = self._pcm_items("bind_responses", "ir", nodes, ir, graphs, "_device_responses", B.ResponseBinding)
         self.api.check(self.api.batch_bind_responses(self.handle, items, n, C.c_void_p(self._torch_stream_handle())))
         self._keep_until_read(ir)
+
+    def bind_curves(self, nodes, curves, graphs=None):
+        """wae_batch_bind_curves: curves[k] (a row of a float32 CUDA tensor [n][length], unit stride on the last dimension) becomes the
+        curve of WaveShaperNode nodes[k] (declared with set_device_curve) of context graphs[k] (default: 0..n-1).  `nodes` as for
+        bind_sources.  One call, ordered after torch's current stream; the curves are copied on the engine stream, and the tensor's memory
+        is kept from reuse until they have been."""
+        import torch
+        if not (isinstance(curves, torch.Tensor) and curves.is_cuda and curves.dtype == torch.float32 and curves.dim() == 2):
+            raise B.WaeError(1, "bind_curves: curves must be a float32 CUDA tensor [n][length]")
+        n = curves.shape[0]
+        graphs, ids = self._graphs_and_nodes("bind_curves", nodes, graphs, n)
+        if n and curves.stride(1) != 1:
+            raise B.WaeError(1, "bind_curves: the points of a curve must be contiguous (unit stride on the last dimension)")
+        items = (B.CurveBinding * max(n, 1))()
+        base = curves.data_ptr()
+        for k, (g, nid) in enumerate(zip(graphs, ids)):
+            declared = self.contexts[g]._device_curves.get(int(nid))
+            # (the tensor's own shape: the library checks only the CUDA allocation, which may hold several tensors)
+            if declared is not None and curves.shape[1] != declared:
+                raise B.WaeError(1, f"bind_curves: curves[{k}] has {curves.shape[1]} points, node {nid} of graph {g} was declared with "
+                                    f"{declared}")
+            items[k] = B.CurveBinding(g, int(nid), C.cast(C.c_void_p(base + 4 * k * curves.stride(0)), B.c_float_p))
+        self.api.check(self.api.batch_bind_curves(self.handle, items, n, C.c_void_p(self._torch_stream_handle())))
+        self._keep_until_read(curves)
+
+    def _graphs_and_nodes(self, fn, nodes, graphs, n):
+        """The graph index and node id of each of n binding items: `graphs` (default 0..n-1), `nodes` one node (or id) for all graphs or
+        one per graph."""
+        graphs = list(range(n)) if graphs is None else [int(g) for g in graphs]
+        if isinstance(nodes, (list, tuple)):
+            ids = [getattr(x, "id", x) for x in nodes]
+        else:
+            ids = [getattr(nodes, "id", nodes)] * n
+        if len(graphs) != n or len(ids) != n:
+            raise B.WaeError(1, f"{fn}: {n} tensors for {len(graphs)} graphs and {len(ids)} nodes")
+        for g in graphs:
+            if not 0 <= g < self.n:
+                raise B.WaeError(2, f"{fn}: graph index {g} is out of range")
+        return graphs, ids
 
     def _pcm_items(self, fn, arg, nodes, pcm, graphs, declarations, Struct):
         """The binding items (graph index, node, device pointer, channel stride) of bind_sources / bind_responses: `declarations` names

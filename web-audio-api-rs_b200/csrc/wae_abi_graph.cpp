@@ -1116,9 +1116,27 @@ WAE_API wae_status wae_convolver_set_device_response(wae_graph* g, wae_node_id n
 WAE_API wae_status wae_wave_shaper_set_curve(wae_graph* g, wae_node_id node, const float* curve, uint32_t len) {
     Node* n = node_of_kind(g, node, K_SHAPER);
     if (!n || (!curve && len)) return fail(WAE_INVALID_ARGUMENT, "not a WaveShaperNode / null curve");
+    if (n->device_curve)
+        return fail(WAE_INVALID_STATE, "InvalidStateError - the curve is bound from device memory (wae_wave_shaper_set_device_curve)");
     if (n->has_curve) return fail(WAE_INVALID_STATE, "InvalidStateError - cannot assign curve twice");
     n->has_curve = true;
     n->table.assign(curve, curve + len);
+    return WAE_OK;
+}
+
+// A declared curve counts as the node's set_curve: the node has a curve of `length` points whose values only the bind supplies
+WAE_API wae_status wae_wave_shaper_set_device_curve(wae_graph* g, wae_node_id node, uint32_t length) {
+    Node* n = node_of_kind(g, node, K_SHAPER);
+    if (!n) return fail(WAE_INVALID_ARGUMENT, "not a WaveShaperNode");
+    if (length == 0) return fail(WAE_INVALID_ARGUMENT, "a curve bound from device memory has at least one point");
+    if (n->device_curve)
+        return fail(WAE_INVALID_STATE, "InvalidStateError - the curve is already bound from device memory (wae_wave_shaper_set_device_curve)");
+    if (n->has_curve) return fail(WAE_INVALID_STATE, "InvalidStateError - the WaveShaperNode already has a curve (set_curve)");
+    if (!g->epochs.empty())  // (the segments before the suspend point were planned with the graph copy of their own: no curve)
+        return fail(WAE_INVALID_STATE, "InvalidStateError - a curve is bound from device memory before the first suspend point");
+    n->has_curve = true;
+    n->device_curve = length;
+    g->device_curves++;
     return WAE_OK;
 }
 

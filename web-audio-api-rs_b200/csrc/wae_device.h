@@ -537,6 +537,21 @@ struct RespBindItem {
     int32_t pad;
 };
 
+// ---- wae_batch_bind_curves: caller device curve -> the curve memory of a declared WaveShaperNode, and the records its value decides --
+// A record field that depends on whether the curve maps 0 to 0 (can_propagate_silence): ChainInst::shaper_keeps_silence, the
+// MetaInst::mode of the node's output track, ShaperOsInst::rebuild.  The bind writes `keeps` or `other` into it.
+struct CurvePatch {
+    int32_t* dst;
+    int32_t keeps, other;
+};
+struct CurveBindItem {
+    const float* src;            // caller's curve (any alignment)
+    float* dst;                  // the node's curve memory: 16 B aligned, `n` rounded up to 4 floats
+    const CurvePatch* patches;   // the node's entries
+    int32_t n;                   // curve length
+    int32_t n_patches;
+};
+
 // ---- wae_batch_bind_params: per-run values of params planned as constants ------------------------------------------------------
 struct ParamBindItem {  // one float of the caller's device memory -> value slot `slot`
     const float* src;

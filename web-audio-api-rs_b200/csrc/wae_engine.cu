@@ -310,8 +310,19 @@ struct StageBuild {
         uint32_t off;
     };
     std::vector<PatchRec> patches;
+    // Patch entries of WaveShaper curves bound from device memory (wae_wave_shaper_set_device_curve): the int32 field `off` bytes into
+    // record `rec` of this stage's table takes `keeps` or `other` as the bound curve maps 0 to 0 or not
+    struct CurvePatchRec {
+        uint32_t graph;  // batch position
+        wae_node_id node;
+        int32_t rec;
+        uint32_t off;
+        int32_t keeps, other;
+    };
+    std::vector<CurvePatchRec> curve_patches;
     size_t records() const {  // size of the table patch entries point into
         switch (kind) {
+            case S_SHAPER_OS: return shaper_os.size();
             case S_CHAIN: case S_VSUM: return chain.size();
             case S_BIQUAD: return biquad.size();
             case S_BIQUAD_AR: return biquad_ar.size();
@@ -461,6 +472,21 @@ struct wae_batch {
     std::vector<DevResponse> responses;
     std::map<std::pair<uint32_t, wae_node_id>, size_t> response_index;  // (batch position, node) -> responses
     size_t responses_unbound = 0;
+    // wae_wave_shaper_set_device_curve: the curve memory of each declared curve (made by the planner, zeroed, never in the upload slabs)
+    // and the range of its patch entries in d_curve_patches, both rewritten by wae_batch_bind_curves.  A declared curve the planner never
+    // reached has no memory: binding it is validated and writes nothing.
+    struct DevCurve {
+        uint32_t graph;  // batch position
+        wae_node_id node;
+        float* d;        // [length rounded up to 4]
+        uint32_t length;
+        int32_t p0, p1;  // its entries in d_curve_patches
+        bool bound;
+    };
+    std::vector<DevCurve> curves;
+    std::map<std::pair<uint32_t, wae_node_id>, size_t> curve_index;  // (batch position, node) -> curves
+    size_t curves_unbound = 0;
+    CurvePatch* d_curve_patches = nullptr;
     cudaEvent_t ev_bind = nullptr;  // orders a bind after the caller's stream
     // OfflineAudioContext::suspend_sync: a group's render is cut at the suspend frames of its graphs (graphs with different
     // suspend points are put in different groups); every segment has its own plan, node state is shared between the plans
@@ -845,6 +871,8 @@ struct Planner {
         // folded into it since the first bound one (gain_fold[s].p.n == 0: the slot has none)
         std::vector<PatchRec> patches;
         PatchRec gain_fold[4] = {};
+        // a shaper whose curve is bound from device memory: the entry of shaper_keeps_silence (rec / off set when the chain is emitted)
+        std::vector<StageBuild::CurvePatchRec> curve_patches;
     };
 
     // Node state is allocated through a key (graph, node, n-th allocation of that node, salt): the plans of consecutive
@@ -1074,6 +1102,11 @@ struct Planner {
             r.off = (uint32_t)(offsetof(ChainInst, g) + (size_t)slot * sizeof(float));
             s.patches.push_back(r);
         }
+        for (StageBuild::CurvePatchRec r : pc.curve_patches) {
+            r.rec = rec;
+            r.off = (uint32_t)offsetof(ChainInst, shaper_keeps_silence);
+            s.curve_patches.push_back(r);
+        }
     }
     static bool chain_has_patches(const PendingChain& pc) {
         bool any = !pc.patches.empty();
@@ -1086,6 +1119,11 @@ struct Planner {
     bool plan_convolver(PNode& pn, int level, const BufRef* dest = nullptr, int64_t dest_limit = -1, const PcmBuffer* ir_override = nullptr);
     bool ir_spectra(const PcmBuffer& ir, float scale, const std::vector<std::vector<float>>& scaled, int Smax, IrSpectra& spec);
     bool device_response_spectra(const Node& n, int S, IrSpectra& spec);
+    const float* device_curve(const Node& n);
+    // a patch entry of the declared curve of node `n` for the int32 field `off` bytes into the last record of stage `s`
+    void add_curve_patch(StageBuild& s, const Node& n, uint32_t off, int32_t keeps, int32_t other) {
+        s.curve_patches.push_back(StageBuild::CurvePatchRec{gi, n.id, (int32_t)s.records() - 1, off, keeps, other});
+    }
     bool conv_compact_path(PNode& pn, int level, int in_ch, const IrSpectra& spec, int Smax, int blocks_per_chunk);
     // chain fusion
     int consumers(uint32_t id) {
@@ -1364,6 +1402,7 @@ static void merge_builds(Builds& dst, Builds& src) {
             pr.rec += (int32_t)bs.records;
             if (pr.rec2 >= 0) pr.rec2 += (int32_t)(s.kind == S_SPAN ? bs.records : bs.scan);
         }
+        for (auto& cp : s.curve_patches) cp.rec += (int32_t)bs.records;
         for (auto& m : s.mix) m.edge_offset += (uint32_t)bs.mix_edges;
         for (auto& m : s.mix_dyn) m.edge_offset += (uint32_t)bs.mix_edges;
         for (auto& c : s.chain)
@@ -1392,6 +1431,7 @@ static void merge_builds(Builds& dst, Builds& src) {
         append_vec(d.mix_edges, s.mix_edges); append_vec(d.mix_dyn, s.mix_dyn); append_vec(d.meta, s.meta); append_vec(d.conv_in, s.conv_in);
         append_vec(d.conv_path, s.conv_path); append_vec(d.vgroups, s.vgroups); append_vec(d.conv_cmp, s.conv_cmp);
         append_vec(d.patches, s.patches);
+        append_vec(d.curve_patches, s.curve_patches);
         d.n_scan_coef += s.n_scan_coef;
         d.max_ch = std::max(d.max_ch, s.max_ch);
     }
@@ -1643,6 +1683,25 @@ bool Planner::device_response_spectra(const Node& n, int S, IrSpectra& spec) {
         b->responses.push_back(wae_batch::DevResponse{key_graph, n.id, spec.h, (uint32_t)ir_ch, (uint64_t)ir.length(), S, n.normalize,
                                                       ir.sample_rate, false});
     return true;
+}
+
+// The curve memory of a curve bound from device memory: one zeroed allocation per (batch graph, node), outside the upload slabs (nothing
+// but wae_batch_bind_curves writes it), shared by every suspend segment and lowering path of the node.  The sizing pass gets the
+// placeholder an uploaded curve gets, so that plan digests stay comparable.
+const float* Planner::device_curve(const Node& n) {
+    if (dry) return reinterpret_cast<const float*>(uintptr_t(256));
+    std::lock_guard<std::recursive_mutex> lk(b->mu);
+    auto it = b->curve_index.find({gi, n.id});
+    if (it != b->curve_index.end()) return b->curves[it->second].d;
+    float* d = b->dalloc<float>((size_t)(n.device_curve + 3) / 4 * 4, true);
+    if (!d) {
+        bail(WAE_OUT_OF_MEMORY, "out of device memory (WaveShaper curve)");
+        return nullptr;
+    }
+    b->asset_bytes += (size_t)(n.device_curve + 3) / 4 * 16;
+    b->curve_index[{gi, n.id}] = b->curves.size();
+    b->curves.push_back(wae_batch::DevCurve{gi, n.id, d, n.device_curve, 0, 0, false});
+    return d;
 }
 
 // the second convolver of a mono response behind an input that switches between one and two channels: input R -> output 1, fed the
@@ -2598,28 +2657,53 @@ bool Planner::lower_gain(NodeCtx& nc) {
 bool Planner::lower_shaper(NodeCtx& nc) {
     Node& n = nc.n; PNode& p = nc.p; const Lay& in0 = nc.in0;
     int ch = p.in_ch[0];
-    const float* curve = n.has_curve ? upload(n.table) : nullptr;
+    // A curve bound from device memory (wae_wave_shaper_set_device_curve): whether it maps 0 to 0 is known only once it is bound.  Behind
+    // an input that is never silent that answer changes no layout, and the node is planned as a curve that maps 0 to 0.  Otherwise the
+    // plan covers both answers (the output gets a layout track of its own), and the bind patches every field the answer decides:
+    // ChainInst::shaper_keeps_silence, the MetaInst::mode of the output track (META_COPY / META_SHAPER), ShaperOsInst::rebuild (2 / 1).
+    const bool declared = n.device_curve != 0;
+    const int curve_n = declared ? (int)n.device_curve : (int)n.table.size();
+    const float* curve = declared ? device_curve(n) : n.has_curve ? upload(n.table) : nullptr;
+    if (declared && !curve) return false;
     // can_propagate_silence (waveshaper.rs:480-503): the curve maps 0 to 0
     bool keeps_silence = true;
-    if (n.has_curve && !n.table.empty()) {
+    if (n.has_curve && !declared && !n.table.empty()) {
         const size_t cn = n.table.size();
         keeps_silence = cn % 2 == 1 ? std::fabs(n.table[cn / 2]) < 1e-9f : std::fabs((n.table[cn / 2 - 1] + n.table[cn / 2]) / 2.f) < 1e-9f;
     }
     // a silent input that still produces sound does so on the ONE channel a silent quantum has (waveshaper.rs:395-400)
-    auto shaper_lay = [keeps_silence](const Lay& l) {
+    auto shaper_lay = [keeps_silence, declared](const Lay& l) {
+        if (declared && l.may_silent) return Lay{1, l.hi, 1, l.nhi, true};  // (either answer)
         if (keeps_silence || !l.may_silent) return l;
         return Lay{1, l.hi, 1, l.nhi, false};
+    };
+    // the output track of a declared curve behind an input that may be silent: k_meta, its mode patched by the bind
+    auto declared_meta = [&]() {
+        out_dynamic(nc, shaper_lay(in0));
+        if (!p.out_buf[0].meta) return;
+        meta_stage(nc.L, META_COPY, p.in_buf[0], ch, p.out_buf[0], ch);
+        add_curve_patch(stage(nc.L, S_META), n, (uint32_t)offsetof(MetaInst, mode), META_COPY, META_SHAPER);
     };
     if (n.oversample && n.has_curve) {  // waveshaper.rs:409-480: up-sample, shape, down-sample
         // input that can fall silent: a curve that maps 0 to 0 makes the node return early WITHOUT feeding its resamplers
         // (frozen state: the kernel then works on the last processed quanta); a curve that does not keeps processing — on the
         // one channel of a silent quantum, which rebuilds the resamplers of a wider node (waveshaper.rs:395-420)
-        const bool freeze = in0.dyn() && keeps_silence && in0.nlo == in0.nhi && in0.nhi == ch;
-        const bool as_static = !in0.dyn() || (!keeps_silence && ch == 1 && in0.hi == 1);
+        bool freeze = in0.dyn() && keeps_silence && in0.nlo == in0.nhi && in0.nhi == ch;
+        bool as_static = !in0.dyn() || (!keeps_silence && ch == 1 && in0.hi == 1);
+        // a declared curve behind a dynamic input always rebuilds: which of freeze / as_static applies depends on the curve.  From zero
+        // state rebuild 2 renders what freeze renders (both count only the processed quanta).  Rebuild 1 behind a mono input never
+        // changes the count, and differs from as_static in the first quantum only: as_static adds the down-sampled curve(0) of its zero
+        // history there, rebuild starts from zero resamplers as the reference does (waveshaper.rs:409-420)
+        if (declared) {
+            freeze = false;
+            as_static = !in0.dyn();
+        }
         // every other dynamic input: the count of the processed quanta changes, and the resamplers are rebuilt with it
         const bool rebuild = !freeze && !as_static;
         if (!need_out(nc, ch)) return false;
-        if (freeze || (rebuild && keeps_silence)) {
+        if (rebuild && declared && in0.may_silent) {
+            declared_meta();
+        } else if (freeze || (rebuild && keeps_silence)) {
             out_like_input(nc);
         } else if (rebuild) {  // silent quanta processed: a sounding output with the input's count (one channel when silent)
             out_dynamic(nc, shaper_lay(in0));
@@ -2638,7 +2722,7 @@ bool Planner::lower_shaper(NodeCtx& nc) {
         so.in = p.in_buf[0];
         so.out = p.out_buf[0];
         so.curve = curve;
-        so.n = (int)n.table.size();
+        so.n = curve_n;
         so.ch = ch;
         so.factor = factor;
         so.f_up = filt.first;
@@ -2657,21 +2741,25 @@ bool Planner::lower_shaper(NodeCtx& nc) {
         StageBuild& os = stage(nc.L, S_SHAPER_OS);
         os.max_ch = std::max(os.max_ch, ch);
         os.shaper_os.push_back(so);
+        if (declared && rebuild) add_curve_patch(os, n, (uint32_t)offsetof(ShaperOsInst, rebuild), 2, 1);
         return true;
     }
     if (nc.fuse_n) {
         PendingChain pc = open_chain(nc);
         pc.inst.has_shaper = 1;
         pc.inst.curve = curve;
-        pc.inst.shaper_n = (int)n.table.size();
+        pc.inst.shaper_n = curve_n;
         pc.inst.shaper_keeps_silence = keeps_silence ? 1 : 0;
+        if (declared) pc.curve_patches.push_back(StageBuild::CurvePatchRec{gi, n.id, -1, 0, 1, 0});
         pc.lay = shaper_lay(pc.lay);
         pc.phase = 5;
         return finish_chain(nc, std::move(pc));
     }
     if (!need_out(nc, ch)) return false;
     ShaperInst sh{};
-    if (in0.dyn() && !keeps_silence && n.has_curve) {
+    if (declared && in0.may_silent) {
+        declared_meta();
+    } else if (in0.dyn() && !keeps_silence && n.has_curve) {
         out_dynamic(nc, shaper_lay(in0));
         if (p.out_buf[0].meta) meta_stage(nc.L, META_SHAPER, p.in_buf[0], ch, p.out_buf[0], ch);
     } else {
@@ -2680,7 +2768,7 @@ bool Planner::lower_shaper(NodeCtx& nc) {
     sh.in = p.in_buf[0];
     sh.out = p.out_buf[0];
     sh.ch = ch;
-    sh.n = (int)n.table.size();
+    sh.n = curve_n;
     sh.curve = curve;
     stage(nc.L, S_SHAPER).shaper.push_back(sh);
     return true;
@@ -3453,6 +3541,12 @@ struct GroupPlan {  // result of phase B for one group
     int code = WAE_OK;
     std::string error;
     std::vector<std::pair<uint32_t, ParamPatch>> patches;  // (batch position, entry): device addresses set, operands still param ids
+    struct CurveEntry {
+        uint32_t graph;  // batch position
+        wae_node_id node;
+        CurvePatch p;    // device address set
+    };
+    std::vector<CurveEntry> curve_patches;
 };
 
 static int64_t padded_length(const wae_graph* g) { return (int64_t)((g->length + 127) / 128 * 128); }
@@ -4059,6 +4153,13 @@ static void prep_plan_group(wae_batch* b, wae_graph* const* graphs, int k, PrepS
                     gp.patches.push_back({pr.graph, p});
                 }
             }
+            if (st.n > 0) {  // patch entries of curves bound from device memory: the device addresses of the int32 fields they set
+                const size_t rec_size = s.kind == S_META ? sizeof(MetaInst) : s.kind == S_SHAPER_OS ? sizeof(ShaperOsInst) : sizeof(ChainInst);
+                for (const auto& cp : s.curve_patches) {
+                    int32_t* dst = reinterpret_cast<int32_t*>(static_cast<char*>(st.d_a) + (size_t)cp.rec * rec_size + cp.off);
+                    gp.curve_patches.push_back({cp.graph, cp.node, CurvePatch{dst, cp.keeps, cp.other}});
+                }
+            }
         }
         gp.seg_ranges.push_back({seg_stage0, gp.stages.size()});
     }  // segments
@@ -4135,9 +4236,51 @@ static void record_responses(wae_batch* b, wae_graph* const* graphs, uint32_t n_
     }
 }
 
-// runs of a batch need every device input, param and response bound once
+// The declared curves of the batch (`graphs` in batch order), after planning: the ones the planner gave memory, all unbound, with their
+// patch entries gathered per curve and uploaded (from `patches`, which the caller keeps alive until the stream has been synchronised);
+// then the declared ones it never reached, which binding validates and writes nothing to, and which runs do not wait for.
+static wae_status record_curves(wae_batch* b, wae_graph* const* graphs, uint32_t n_graphs, const std::vector<GroupPlan>& gps,
+                                std::vector<CurvePatch>& patches) {
+    std::sort(b->curves.begin(), b->curves.end(),
+              [](const wae_batch::DevCurve& x, const wae_batch::DevCurve& y) { return std::tie(x.graph, x.node) < std::tie(y.graph, y.node); });
+    b->curve_index.clear();
+    for (size_t k = 0; k < b->curves.size(); k++) b->curve_index[{b->curves[k].graph, b->curves[k].node}] = k;
+    b->curves_unbound = b->curves.size();
+    std::vector<std::vector<CurvePatch>> per(b->curves.size());
+    for (const auto& gp : gps)
+        for (const auto& e : gp.curve_patches) per[b->curve_index.at({e.graph, e.node})].push_back(e.p);
+    for (size_t k = 0; k < per.size(); k++) {
+        b->curves[k].p0 = (int32_t)patches.size();
+        patches.insert(patches.end(), per[k].begin(), per[k].end());
+        b->curves[k].p1 = (int32_t)patches.size();
+    }
+    if (!patches.empty() && !(b->d_curve_patches = b->dupload_now(patches)))
+        return fail(WAE_OUT_OF_MEMORY, "out of device memory (curve patch entries)");
+    for (uint32_t j = 0; j < n_graphs; j++) {
+        if (!graphs[j]->device_curves) continue;
+        auto scan = [&](const NodeMap& nodes) {
+            for (const auto& kv : nodes) {
+                const Node& nd = kv.second;
+                if (nd.kind != K_SHAPER || !nd.device_curve || b->curve_index.count({j, nd.id})) continue;
+                b->curve_index[{j, nd.id}] = b->curves.size();
+                b->curves.push_back(wae_batch::DevCurve{j, nd.id, nullptr, nd.device_curve, 0, 0, true});
+            }
+        };
+        scan(graphs[j]->nodes);
+        for (const auto& ep : graphs[j]->epochs) scan(ep.nodes);
+    }
+    return WAE_OK;
+}
+
+// runs of a batch need every device input, param, response and curve bound once
 static wae_status check_bound(wae_batch* b) {
     if (!b) return fail(WAE_INVALID_ARGUMENT, "null batch");
+    for (size_t k = 0; b->curves_unbound && k < b->curves.size(); k++)
+        if (const auto& d = b->curves[k]; !d.bound) {
+            const uint32_t caller = b->order.empty() ? d.graph : b->order[d.graph];
+            return fail(WAE_INVALID_STATE, "curve bound from device memory never bound: graph " + std::to_string(caller) + ", node " +
+                                               std::to_string(d.node) + " (wae_batch_bind_curves)");
+        }
     for (size_t k = 0; b->responses_unbound && k < b->responses.size(); k++)
         if (const auto& d = b->responses[k]; !d.bound) {
             const uint32_t caller = b->order.empty() ? d.graph : b->order[d.graph];
@@ -4261,9 +4404,11 @@ static wae_status prepare_impl(wae_engine* eng, wae_graph* const* graphs, uint32
         }
     }
     record_responses(b, graphs, n_graphs);
+    std::vector<CurvePatch> curve_patches;
     std::vector<ParamSlotInfo> slot_info;
     std::vector<ParamPatch> patches;
-    st = record_params(b, graphs, n_graphs, gps, slot_info, patches);
+    st = record_curves(b, graphs, n_graphs, gps, curve_patches);
+    if (st == WAE_OK) st = record_params(b, graphs, n_graphs, gps, slot_info, patches);
     if (st != WAE_OK) {
         wae_batch_destroy(b);
         return st;
@@ -4882,6 +5027,52 @@ WAE_API wae_status wae_batch_bind_responses(wae_batch* b, const wae_response_bin
     return WAE_OK;
 }
 
+// The curve memory and the patched fields are rewritten on the engine stream: runs queued before the bind have read the previous ones.
+WAE_API wae_status wae_batch_bind_curves(wae_batch* b, const wae_curve_binding* items, uint32_t n, void* stream) {
+    if (!b || (n && !items)) return fail(WAE_INVALID_ARGUMENT, "null batch / items");
+    if (n == 0) return WAE_OK;
+    CUDA_TRY(cudaSetDevice(b->engine->device));
+    // every item is validated before anything is enqueued
+    std::vector<CurveBindItem> table;
+    std::vector<size_t> curve_of;
+    std::vector<char> named(b->curves.size(), 0);
+    BindExtents extents{b->engine->device, {}};
+    for (uint32_t i = 0; i < n; i++) {
+        const wae_curve_binding& it = items[i];
+        if (it.graph_index >= b->n_graphs)
+            return fail(WAE_INVALID_STATE, "bind: graph index " + std::to_string(it.graph_index) + " is out of range");
+        auto ci = b->curve_index.find({b->batch_pos(it.graph_index), it.node});
+        if (ci == b->curve_index.end())
+            return fail(WAE_INVALID_STATE, "bind: node " + std::to_string(it.node) + " of graph " + std::to_string(it.graph_index) +
+                                               " is not a curve bound from device memory (wae_wave_shaper_set_device_curve)");
+        const size_t k = ci->second;
+        if (named[k]++)  // (two items of one launch writing one curve: which one lands would be undefined)
+            return fail(WAE_INVALID_ARGUMENT, "bind: node " + std::to_string(it.node) + " of graph " + std::to_string(it.graph_index) +
+                                                  " is named twice in one call");
+        const wae_batch::DevCurve& d = b->curves[k];
+        if (!it.curve) return fail(WAE_INVALID_ARGUMENT, "bind: null curve");
+        wae_status st = extents.check(it.curve, (uint64_t)d.length * sizeof(float), "curve",
+                                      "[curve, curve + length) runs past the end of its allocation");
+        if (st != WAE_OK) return st;
+        if (!d.d) continue;  // declared, never rendered: nothing to write
+        table.push_back(CurveBindItem{it.curve, d.d, b->d_curve_patches + d.p0, (int32_t)d.length, d.p1 - d.p0});
+        curve_of.push_back(k);
+    }
+    if (table.empty()) return WAE_OK;
+    wae_status st = bind_after(b, stream);
+    if (st == WAE_OK) st = stage_bind_table(b, table.data(), table.size() * sizeof(CurveBindItem));
+    if (st != WAE_OK) return st;
+    launch_bind_curves(static_cast<const CurveBindItem*>(b->d_bind), (int)table.size(), b->engine->stream);
+    cudaError_t le = cudaGetLastError();
+    if (le != cudaSuccess) return fail(WAE_CUDA_ERROR, std::string("bind: ") + cudaGetErrorString(le));
+    for (size_t k : curve_of)
+        if (!b->curves[k].bound) {
+            b->curves[k].bound = true;
+            b->curves_unbound--;
+        }
+    return WAE_OK;
+}
+
 WAE_API wae_status wae_batch_sync(wae_batch* b) {
     CUDA_TRY(cudaSetDevice(b->engine->device));
     CUDA_TRY(cudaStreamSynchronize(b->engine->stream));
@@ -5342,6 +5533,9 @@ static wae_status refuse_device_inputs(wae_graph* const* graphs, uint32_t n_grap
         if (graphs[i] && graphs[i]->device_responses)
             return fail(WAE_INVALID_STATE, "graph " + std::to_string(i) + " has convolver responses bound from device memory: render it with "
                                            "wae_batch_prepare (or _prepare_many), wae_batch_bind_responses and wae_batch_run");
+        if (graphs[i] && graphs[i]->device_curves)
+            return fail(WAE_INVALID_STATE, "graph " + std::to_string(i) + " has WaveShaper curves bound from device memory: render it with "
+                                           "wae_batch_prepare (or _prepare_many), wae_batch_bind_curves and wae_batch_run");
     }
     return WAE_OK;
 }

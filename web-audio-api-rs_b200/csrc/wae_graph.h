@@ -126,6 +126,9 @@ struct Node {
     int type = 0;  // oscillator / biquad type
     std::vector<float> table;  // periodic wave / shaper curve
     bool has_curve = false;
+    // wae_wave_shaper_set_device_curve: the curve's length (has_curve is set, `table` stays empty); its points are written by
+    // wae_batch_bind_curves.  0: not declared
+    uint32_t device_curve = 0;
     int oversample = 0;  // WaveShaper: WAE_OVERSAMPLE_*
     std::vector<double> feedforward, feedback;  // IIR
     std::shared_ptr<PcmBuffer> buffer;          // ABSN buffer / convolver IR
@@ -255,6 +258,7 @@ struct wae_graph {
     uint32_t device_inputs = 0;  // AudioBufferSourceNodes declared with wae_buffer_source_set_device_input (never in `assets`)
     uint32_t device_params = 0;  // AudioParams declared with wae_param_set_device_value
     uint32_t device_responses = 0;  // ConvolverNodes declared with wae_convolver_set_device_response (never in `assets`)
+    uint32_t device_curves = 0;     // WaveShaperNodes declared with wae_wave_shaper_set_device_curve
 
     uint32_t create_param(uint32_t owner, float def, float mn, float mx, bool a_rate, float initial, bool send_set_value = true,
                           bool fixed_id = false, uint32_t id = 0, bool constrained = false);

@@ -4375,6 +4375,39 @@ __global__ void __launch_bounds__(CV_THREADS) k_resp_fft(const RespBindItem* __r
     rfft_store(z, it.h + ((size_t)c * (it.S + WAE_CONV_H_PAD) + WAE_CONV_H_PAD_LO + seg) * CV_BINS, lane_tw);
 }
 
+// ---- wae_batch_bind_curves: one CTA per declared WaveShaper curve ---------------------------------------------------------------
+// Copies the caller's curve into the node's curve memory (128-bit stores; 128-bit loads where the source is 16 B aligned; the padding to
+// a multiple of 4 floats is written as zeros), decides can_propagate_silence (waveshaper.rs:495-508) with the planner's f32 expression, and
+// writes every record field that answer reaches.  Values are copied bit for bit (NaN payloads included).
+__global__ void __launch_bounds__(256) k_bind_curves(const CurveBindItem* __restrict__ items) {
+    __shared__ int keeps;
+    const CurveBindItem it = items[blockIdx.x];
+    const int n = it.n, n4 = (n + 3) >> 2;
+    const bool aligned = (reinterpret_cast<uintptr_t>(it.src) & 15) == 0;
+    for (int i = threadIdx.x; i < n4; i += blockDim.x) {
+        float4 v;
+        if (aligned && 4 * i + 4 <= n) {
+            v = __ldcs(reinterpret_cast<const float4*>(it.src) + i);
+        } else {
+            const int k = 4 * i;
+            v.x = __ldcs(it.src + k);
+            v.y = k + 1 < n ? __ldcs(it.src + k + 1) : 0.f;
+            v.z = k + 2 < n ? __ldcs(it.src + k + 2) : 0.f;
+            v.w = k + 3 < n ? __ldcs(it.src + k + 3) : 0.f;
+        }
+        reinterpret_cast<float4*>(it.dst)[i] = v;
+    }
+    if (threadIdx.x == 0) {
+        const float* c = it.src;
+        keeps = n % 2 == 1 ? fabsf(c[n / 2]) < 1e-9f : fabsf(__fdiv_rn(__fadd_rn(c[n / 2 - 1], c[n / 2]), 2.f)) < 1e-9f;
+    }
+    __syncthreads();
+    for (int k = threadIdx.x; k < it.n_patches; k += blockDim.x) {
+        const CurvePatch p = it.patches[k];
+        *p.dst = keeps ? p.keeps : p.other;
+    }
+}
+
 // Host emulation of the transforms above with the SAME butterfly, index and twiddle code (tests/test_conv_fft_host.py pins them against
 // numpy on a machine without a GPU).  mode 0: complex forward, natural -> position order; 1: complex inverse, position -> natural order
 // (unnormalised); 2: 2B reals -> B packed bins in position order; 3: B packed bins -> 2B reals (scaled by 1 / 2B).  data: 2B floats in place.
@@ -4912,6 +4945,7 @@ void launch_bind_responses(RespBindItem* d, int n, bool any_normalize, int64_t m
     k_resp_trim<<<dim3((unsigned)bx, (unsigned)n, (unsigned)max_ch), 256, 0, s>>>(d);
     k_resp_fft<<<dim3((unsigned)max_S, (unsigned)max_ch, (unsigned)n), CV_THREADS, CV_SMEM_ELEMS * sizeof(float2), s>>>(d);
 }
+void launch_bind_curves(const CurveBindItem* d, int n, cudaStream_t s) { k_bind_curves<<<(unsigned)n, 256, 0, s>>>(d); }
 void launch_conv_ir_fft(const float* ir, int64_t ir_len, int64_t ir_stride, float2* h, int S, int channels, cudaStream_t s) {
     conv_configure();
     k_conv_ir_fft<<<dim3((unsigned)S, (unsigned)channels), CV_THREADS, CV_SMEM_ELEMS * sizeof(float2), s>>>(ir, ir_len, ir_stride, h, S);

@@ -112,6 +112,8 @@ void launch_bind_params(const ParamBindItem* d, int n, const ParamSlotInfo* info
 // a bind of n convolver responses: the power of the normalising items (k_resp_power, when any_normalize), the trimmed lengths
 // (k_resp_trim), the spectra (k_resp_fft); max_* over the items
 void launch_bind_responses(RespBindItem* d, int n, bool any_normalize, int64_t max_len, int max_S, int max_ch, cudaStream_t s);
+// a bind of n WaveShaper curves (k_bind_curves): copy, can_propagate_silence, the patch entries it decides
+void launch_bind_curves(const CurveBindItem* d, int n, cudaStream_t s);
 void launch_conv_ir_fft(const float* ir, int64_t ir_len, int64_t ir_stride, float2* h, int S, int channels, cudaStream_t s);
 
 }  // namespace wae
