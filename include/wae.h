@@ -614,8 +614,36 @@ typedef struct wae_curve_binding {
  * wae_batch_run_pipelined answer WAE_INVALID_STATE while a declared curve of the batch has never been bound. */
 WAE_API wae_status wae_batch_bind_curves(wae_batch* batch, const wae_curve_binding* items, uint32_t n, void* stream);
 
+/* ---- OscillatorNode periodic waves bound from device memory -----------------------------------------------------------------
+ * Declares an OscillatorNode whose PeriodicWave of `coefficients` (real, imag) pairs is supplied per run from device memory
+ * (wae_batch_bind_periodic_waves) instead of set_periodic_wave, so that one prepared batch plays any number of timbres (harmonic
+ * amplitudes predicted by a network, randomised wavetables) without being built and planned again.  The bind synthesises the wavetable
+ * of `table_len` points on the device as wae_periodic_wave_table does (normalised unless `disable_normalization`).  The declaration
+ * counts as the node's set_periodic_wave: the type becomes Custom for good, and an earlier host wave is replaced.
+ * WAE_INVALID_ARGUMENT: not an oscillator, `coefficients` < 2 or `table_len` 0.  WAE_INVALID_STATE: the node is declared twice, or the
+ * graph already has a suspend point; set_periodic_wave after the declaration answers WAE_INVALID_STATE.  Suspend points added later are
+ * allowed (every segment reads the one bound table).  wae_render_batch and wae_render_many answer WAE_INVALID_STATE on graphs with such
+ * nodes; wae_batch_plan plans them. */
+WAE_API wae_status wae_oscillator_set_device_periodic_wave(wae_graph* graph, wae_node_id node, uint32_t coefficients, uint32_t table_len,
+                                                           uint32_t disable_normalization);
+
+typedef struct wae_periodic_wave_binding {
+    uint32_t graph_index;   /* caller's index, as wae_batch_fetch_graph */
+    wae_node_id node;       /* declared with wae_oscillator_set_device_periodic_wave */
+    const float* real;      /* device memory of the engine's GPU: `coefficients` floats, or NULL (= zeros) */
+    const float* imag;      /* likewise; not both NULL */
+} wae_periodic_wave_binding;
+
+/* Synthesises the wavetables into the batch, asynchronously on the engine stream after the work already queued on `stream` (as
+ * wae_batch_bind_sources).  real[0] and imag[0] (DC) are ignored, as PeriodicWave ignores them.  All-or-nothing: every item is validated
+ * before anything is enqueued.  A bound wave stays until it is bound again.  WAE_INVALID_ARGUMENT: `real` and `imag` are both null, one
+ * of them is not device (or managed) memory of the engine's GPU or does not hold `coefficients` floats in one allocation, or one
+ * (graph, node) is named twice in the call.  WAE_INVALID_STATE: graph_index out of range, or the node was not declared.  wae_batch_run,
+ * wae_batch_run_group and wae_batch_run_pipelined answer WAE_INVALID_STATE while a declared wave of the batch has never been bound. */
+WAE_API wae_status wae_batch_bind_periodic_waves(wae_batch* batch, const wae_periodic_wave_binding* items, uint32_t n, void* stream);
+
 /* PeriodicWave::new(context, PeriodicWaveOptions { real, imag, disable_normalization }) (src/periodic_wave.rs:104-209): fills `table`
- * (PERIODIC_WAVE_TABLE_LENGTH = 2048 in the reference) with the wavetable an OscillatorNode of type Custom plays.  `real` / `imag` may be
+ * (PERIODIC_WAVE_TABLE_LENGTH = 8192 in the reference) with the wavetable an OscillatorNode of type Custom plays.  `real` / `imag` may be
  * NULL (= zeros); both NULL = the sine default.  Host math, no engine needed. */
 WAE_API wae_status wae_periodic_wave_table(const float* real, const float* imag, uint32_t len, uint32_t disable_normalization, float* table,
                                            uint32_t table_len);

@@ -138,6 +138,12 @@ class CurveBinding(C.Structure):
     _fields_ = [("graph_index", C.c_uint32), ("node", C.c_uint32), ("curve", c_float_p)]
 
 
+class PeriodicWaveBinding(C.Structure):
+    """wae_periodic_wave_binding: the device coefficients of one declared custom OscillatorNode of a prepared batch
+    (wae_batch_bind_periodic_waves); either pointer may be NULL (zeros)."""
+    _fields_ = [("graph_index", C.c_uint32), ("node", C.c_uint32), ("real", c_float_p), ("imag", c_float_p)]
+
+
 STATUS_NAMES = {0: "OK", 1: "INVALID_ARGUMENT", 2: "INVALID_STATE", 3: "NOT_SUPPORTED", 4: "UNSUPPORTED",
                 5: "CUDA_ERROR", 6: "OUT_OF_MEMORY", 7: "NO_DEVICE"}
 
@@ -180,6 +186,7 @@ WAE_SYMBOLS = [
     "wae_param_set_device_value", "wae_batch_bind_params",
     "wae_convolver_set_device_response", "wae_batch_bind_responses",
     "wae_wave_shaper_set_device_curve", "wae_batch_bind_curves",
+    "wae_oscillator_set_device_periodic_wave", "wae_batch_bind_periodic_waves",
 ]
 
 
@@ -292,6 +299,9 @@ class Api:
             # WaveShaper curves bound from device memory
             f("wave_shaper_set_device_curve", C.c_int32, [gp, C.c_uint32, C.c_uint32])
             f("batch_bind_curves", C.c_int32, [C.c_void_p, C.POINTER(CurveBinding), C.c_uint32, C.c_void_p])
+            # periodic waves bound from device memory
+            f("oscillator_set_device_periodic_wave", C.c_int32, [gp, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32])
+            f("batch_bind_periodic_waves", C.c_int32, [C.c_void_p, C.POINTER(PeriodicWaveBinding), C.c_uint32, C.c_void_p])
         else:
             f("graph_create", C.c_int32, [C.c_uint32, C.c_uint64, C.c_float, C.POINTER(C.c_void_p)])
             f("render", C.c_int32, [gp, c_float_p])

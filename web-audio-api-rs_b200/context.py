@@ -260,6 +260,17 @@ class OscillatorNode(AudioScheduledSourceNode):
         api = self._ctx._api
         api.check(api.oscillator_set_periodic_wave(self._ctx._g, self.id, B.fptr(t), len(t)))
 
+    def set_device_periodic_wave(self, coefficients, table_length=8192, disable_normalization=False):
+        """wae_oscillator_set_device_periodic_wave (product only): the node plays the wavetable of `table_length` points (8192, the
+        reference's PERIODIC_WAVE_TABLE_LENGTH, by default) that Batch.bind_periodic_waves synthesises from `coefficients` (real, imag)
+        pairs of device memory before each run.  Counts as the node's set_periodic_wave."""
+        api = self._ctx._api
+        if not api.is_product:
+            raise B.WaeError(3, "periodic waves bound from device memory are a feature of the GPU engine")
+        api.check(api.oscillator_set_device_periodic_wave(self._ctx._g, self.id, int(coefficients), int(table_length),
+                                                          1 if disable_normalization else 0))
+        self._ctx._device_waves[self.id] = int(coefficients)
+
     def set_type(self, type_):
         api = self._ctx._api
         api.check(api.oscillator_set_type(self._ctx._g, self.id, type_))
@@ -475,6 +486,7 @@ class OfflineAudioContext:
         self._device_inputs = {}  # node id -> (channels, length) declared with set_device_input
         self._device_responses = {}  # node id -> (channels, length) declared with set_device_response
         self._device_curves = {}  # node id -> length declared with set_device_curve
+        self._device_waves = {}  # node id -> coefficient count declared with set_device_periodic_wave
 
     def __del__(self):
         try:
@@ -822,6 +834,40 @@ class Batch:
             items[k] = B.CurveBinding(g, int(nid), C.cast(C.c_void_p(base + 4 * k * curves.stride(0)), B.c_float_p))
         self.api.check(self.api.batch_bind_curves(self.handle, items, n, C.c_void_p(self._torch_stream_handle())))
         self._keep_until_read(curves)
+
+    def bind_periodic_waves(self, nodes, real, imag=None, graphs=None):
+        """wae_batch_bind_periodic_waves: real[k] and imag[k] (rows of float32 CUDA tensors [n][coefficients], unit stride on the last
+        dimension; either may be None = zeros) become the PeriodicWave coefficients of OscillatorNode nodes[k] (declared with
+        set_device_periodic_wave) of context graphs[k] (default: 0..n-1).  `nodes` as for bind_sources.  One call, ordered after torch's
+        current stream; the wavetables are synthesised on the engine stream, and the tensors' memory is kept from reuse until they have
+        been."""
+        import torch
+        given = [t for t in (real, imag) if t is not None]
+        if not given:
+            raise B.WaeError(1, "bind_periodic_waves: real and imag are both None")
+        for t in given:
+            if not (isinstance(t, torch.Tensor) and t.is_cuda and t.dtype == torch.float32 and t.dim() == 2):
+                raise B.WaeError(1, "bind_periodic_waves: real and imag must be float32 CUDA tensors [n][coefficients]")
+        if len(given) == 2 and real.shape != imag.shape:
+            raise B.WaeError(1, f"bind_periodic_waves: real {tuple(real.shape)} and imag {tuple(imag.shape)} differ in shape")
+        n, count = given[0].shape
+        graphs, ids = self._graphs_and_nodes("bind_periodic_waves", nodes, graphs, n)
+        if n and any(t.stride(1) != 1 for t in given):
+            raise B.WaeError(1, "bind_periodic_waves: the coefficients of a wave must be contiguous (unit stride on the last dimension)")
+
+        def row(t, k):
+            return None if t is None else C.cast(C.c_void_p(t.data_ptr() + 4 * k * t.stride(0)), B.c_float_p)
+        items = (B.PeriodicWaveBinding * max(n, 1))()
+        for k, (g, nid) in enumerate(zip(graphs, ids)):
+            declared = self.contexts[g]._device_waves.get(int(nid))
+            # (the tensor's own shape: the library checks only the CUDA allocation, which may hold several tensors)
+            if declared is not None and count != declared:
+                raise B.WaeError(1, f"bind_periodic_waves: row {k} has {count} coefficients, node {nid} of graph {g} was declared "
+                                    f"with {declared}")
+            items[k] = B.PeriodicWaveBinding(g, int(nid), row(real, k), row(imag, k))
+        self.api.check(self.api.batch_bind_periodic_waves(self.handle, items, n, C.c_void_p(self._torch_stream_handle())))
+        for t in given:
+            self._keep_until_read(t)
 
     def _graphs_and_nodes(self, fn, nodes, graphs, n):
         """The graph index and node id of each of n binding items: `graphs` (default 0..n-1), `nodes` one node (or id) for all graphs or

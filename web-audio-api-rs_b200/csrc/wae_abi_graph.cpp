@@ -1145,8 +1145,34 @@ WAE_API wae_status wae_wave_shaper_set_device_curve(wae_graph* g, wae_node_id no
 WAE_API wae_status wae_oscillator_set_periodic_wave(wae_graph* g, wae_node_id node, const float* table, uint32_t len) {
     Node* n = node_of_kind(g, node, K_OSC);
     if (!n || !table || len == 0) return fail(WAE_INVALID_ARGUMENT, "not an OscillatorNode / empty wavetable");
+    if (n->device_wave)
+        return fail(WAE_INVALID_STATE,
+                    "InvalidStateError - the periodic wave is bound from device memory (wae_oscillator_set_device_periodic_wave)");
     n->type = WAE_OSC_CUSTOM;
     n->table.assign(table, table + len);
+    return WAE_OK;
+}
+
+// A declared wave counts as the node's set_periodic_wave: the type becomes Custom for good, and the oscillator plays a wavetable of
+// `table_len` points that wae_batch_bind_periodic_waves synthesises from `coefficients` bound coefficients (PeriodicWave::new)
+WAE_API wae_status wae_oscillator_set_device_periodic_wave(wae_graph* g, wae_node_id node, uint32_t coefficients, uint32_t table_len,
+                                                           uint32_t disable_normalization) {
+    Node* n = node_of_kind(g, node, K_OSC);
+    if (!n) return fail(WAE_INVALID_ARGUMENT, "not an OscillatorNode");
+    if (coefficients < 2) return fail(WAE_INVALID_ARGUMENT, "IndexSizeError - `real` and `imag` length should at least 2");
+    if (table_len == 0) return fail(WAE_INVALID_ARGUMENT, "a periodic wave bound from device memory has a wavetable of at least one point");
+    if (n->device_wave)
+        return fail(WAE_INVALID_STATE,
+                    "InvalidStateError - the periodic wave is already bound from device memory (wae_oscillator_set_device_periodic_wave)");
+    if (!g->epochs.empty())  // (the segments before the suspend point were planned with the graph copy of their own: no wave)
+        return fail(WAE_INVALID_STATE, "InvalidStateError - a periodic wave is bound from device memory before the first suspend point");
+    n->type = WAE_OSC_CUSTOM;
+    n->table.clear();  // (replaces an earlier host wave, as a second set_periodic_wave would)
+    n->table.shrink_to_fit();
+    n->device_wave = coefficients;
+    n->device_wave_len = table_len;
+    n->device_wave_normalize = disable_normalization == 0;
+    g->device_waves++;
     return WAE_OK;
 }
 

@@ -552,6 +552,17 @@ struct CurveBindItem {
     int32_t n_patches;
 };
 
+// ---- wae_batch_bind_periodic_waves: caller coefficients -> the wavetable of a declared custom OscillatorNode ------------------------
+struct WaveBindItem {
+    const float* re;   // caller's coefficients (null: zeros)
+    const float* im;
+    float* dst;        // the node's wavetable memory: `len` floats
+    int32_t n;         // coefficient count (>= 2)
+    int32_t len;       // wavetable length
+    int32_t normalize;
+    int32_t pad;
+};
+
 // ---- wae_batch_bind_params: per-run values of params planned as constants ------------------------------------------------------
 struct ParamBindItem {  // one float of the caller's device memory -> value slot `slot`
     const float* src;

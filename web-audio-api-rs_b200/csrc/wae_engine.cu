@@ -487,6 +487,20 @@ struct wae_batch {
     std::map<std::pair<uint32_t, wae_node_id>, size_t> curve_index;  // (batch position, node) -> curves
     size_t curves_unbound = 0;
     CurvePatch* d_curve_patches = nullptr;
+    // wae_oscillator_set_device_periodic_wave: the wavetable memory of each declared wave (made by the planner, zeroed, never in the
+    // upload slabs), rewritten by wae_batch_bind_periodic_waves.  A declared wave the planner never reached has no memory: binding it is
+    // validated and writes nothing.
+    struct DevWave {
+        uint32_t graph;  // batch position
+        wae_node_id node;
+        float* d;        // [table_len]
+        uint32_t coefficients, table_len;
+        bool normalize;
+        bool bound;
+    };
+    std::vector<DevWave> waves;
+    std::map<std::pair<uint32_t, wae_node_id>, size_t> wave_index;  // (batch position, node) -> waves
+    size_t waves_unbound = 0;
     cudaEvent_t ev_bind = nullptr;  // orders a bind after the caller's stream
     // OfflineAudioContext::suspend_sync: a group's render is cut at the suspend frames of its graphs (graphs with different
     // suspend points are put in different groups); every segment has its own plan, node state is shared between the plans
@@ -1120,6 +1134,7 @@ struct Planner {
     bool ir_spectra(const PcmBuffer& ir, float scale, const std::vector<std::vector<float>>& scaled, int Smax, IrSpectra& spec);
     bool device_response_spectra(const Node& n, int S, IrSpectra& spec);
     const float* device_curve(const Node& n);
+    float* device_wave(const Node& n);
     // a patch entry of the declared curve of node `n` for the int32 field `off` bytes into the last record of stage `s`
     void add_curve_patch(StageBuild& s, const Node& n, uint32_t off, int32_t keeps, int32_t other) {
         s.curve_patches.push_back(StageBuild::CurvePatchRec{gi, n.id, (int32_t)s.records() - 1, off, keeps, other});
@@ -1704,6 +1719,25 @@ const float* Planner::device_curve(const Node& n) {
     return d;
 }
 
+// The wavetable memory of a periodic wave bound from device memory: one zeroed allocation per (batch graph, node), outside the upload
+// slabs (nothing but wae_batch_bind_periodic_waves writes it), shared by every suspend segment and lowering path of the node.  The sizing
+// pass gets the placeholder an uploaded wavetable gets, so that plan digests stay comparable.
+float* Planner::device_wave(const Node& n) {
+    if (dry) return reinterpret_cast<float*>(uintptr_t(256));
+    std::lock_guard<std::recursive_mutex> lk(b->mu);
+    auto it = b->wave_index.find({gi, n.id});
+    if (it != b->wave_index.end()) return b->waves[it->second].d;
+    float* d = b->dalloc<float>((size_t)n.device_wave_len, true);
+    if (!d) {
+        bail(WAE_OUT_OF_MEMORY, "out of device memory (periodic wave)");
+        return nullptr;
+    }
+    b->asset_bytes += (size_t)n.device_wave_len * sizeof(float);
+    b->wave_index[{gi, n.id}] = b->waves.size();
+    b->waves.push_back(wae_batch::DevWave{gi, n.id, d, n.device_wave, n.device_wave_len, n.device_wave_normalize, false});
+    return d;
+}
+
 // the second convolver of a mono response behind an input that switches between one and two channels: input R -> output 1, fed the
 // two-channel quanta only (ConvCmpInst)
 bool Planner::conv_compact_path(PNode& pn, int level, int in_ch, const IrSpectra& spec, int Smax, int blocks_per_chunk) {
@@ -2145,7 +2179,11 @@ bool Planner::lower_osc(NodeCtx& nc) {
             else o.n_stop = clock.first_frame_at_or_after(n.stop_time);
         }
     }
-    if (n.type == WAE_OSC_CUSTOM) {
+    if (n.type == WAE_OSC_CUSTOM && n.device_wave) {  // a wave bound from device memory: planned as a host wave of its length
+        o.table = device_wave(n);
+        o.table_len = (int)n.device_wave_len;
+        if (!o.table) return false;
+    } else if (n.type == WAE_OSC_CUSTOM) {
         float* d = upload(n.table);
         o.table = d;
         o.table_len = (int)n.table.size();
@@ -4272,9 +4310,39 @@ static wae_status record_curves(wae_batch* b, wae_graph* const* graphs, uint32_t
     return WAE_OK;
 }
 
-// runs of a batch need every device input, param, response and curve bound once
+// The declared periodic waves of the batch (`graphs` in batch order), after planning: the ones the planner gave memory, all unbound; then
+// the declared ones it never reached (never started, pruned), which binding validates and writes nothing to, and which runs do not wait for.
+static void record_waves(wae_batch* b, wae_graph* const* graphs, uint32_t n_graphs) {
+    std::sort(b->waves.begin(), b->waves.end(),
+              [](const wae_batch::DevWave& x, const wae_batch::DevWave& y) { return std::tie(x.graph, x.node) < std::tie(y.graph, y.node); });
+    b->wave_index.clear();
+    for (size_t k = 0; k < b->waves.size(); k++) b->wave_index[{b->waves[k].graph, b->waves[k].node}] = k;
+    b->waves_unbound = b->waves.size();
+    for (uint32_t j = 0; j < n_graphs; j++) {
+        if (!graphs[j]->device_waves) continue;
+        auto scan = [&](const NodeMap& nodes) {
+            for (const auto& kv : nodes) {
+                const Node& nd = kv.second;
+                if (nd.kind != K_OSC || !nd.device_wave || b->wave_index.count({j, nd.id})) continue;
+                b->wave_index[{j, nd.id}] = b->waves.size();
+                b->waves.push_back(
+                    wae_batch::DevWave{j, nd.id, nullptr, nd.device_wave, nd.device_wave_len, nd.device_wave_normalize, true});
+            }
+        };
+        scan(graphs[j]->nodes);
+        for (const auto& ep : graphs[j]->epochs) scan(ep.nodes);
+    }
+}
+
+// runs of a batch need every device input, param, response, curve and periodic wave bound once
 static wae_status check_bound(wae_batch* b) {
     if (!b) return fail(WAE_INVALID_ARGUMENT, "null batch");
+    for (size_t k = 0; b->waves_unbound && k < b->waves.size(); k++)
+        if (const auto& d = b->waves[k]; !d.bound) {
+            const uint32_t caller = b->order.empty() ? d.graph : b->order[d.graph];
+            return fail(WAE_INVALID_STATE, "periodic wave bound from device memory never bound: graph " + std::to_string(caller) +
+                                               ", node " + std::to_string(d.node) + " (wae_batch_bind_periodic_waves)");
+        }
     for (size_t k = 0; b->curves_unbound && k < b->curves.size(); k++)
         if (const auto& d = b->curves[k]; !d.bound) {
             const uint32_t caller = b->order.empty() ? d.graph : b->order[d.graph];
@@ -4404,6 +4472,7 @@ static wae_status prepare_impl(wae_engine* eng, wae_graph* const* graphs, uint32
         }
     }
     record_responses(b, graphs, n_graphs);
+    record_waves(b, graphs, n_graphs);
     std::vector<CurvePatch> curve_patches;
     std::vector<ParamSlotInfo> slot_info;
     std::vector<ParamPatch> patches;
@@ -5073,6 +5142,60 @@ WAE_API wae_status wae_batch_bind_curves(wae_batch* b, const wae_curve_binding* 
     return WAE_OK;
 }
 
+// The wavetables are rewritten on the engine stream: runs queued before the bind have read the previous ones.
+WAE_API wae_status wae_batch_bind_periodic_waves(wae_batch* b, const wae_periodic_wave_binding* items, uint32_t n, void* stream) {
+    if (!b || (n && !items)) return fail(WAE_INVALID_ARGUMENT, "null batch / items");
+    if (n == 0) return WAE_OK;
+    CUDA_TRY(cudaSetDevice(b->engine->device));
+    // every item is validated before anything is enqueued
+    std::vector<WaveBindItem> table;
+    std::vector<size_t> wave_of;
+    std::vector<char> named(b->waves.size(), 0);
+    BindExtents extents{b->engine->device, {}};
+    int max_len = 0;
+    bool any_normalize = false;
+    for (uint32_t i = 0; i < n; i++) {
+        const wae_periodic_wave_binding& it = items[i];
+        if (it.graph_index >= b->n_graphs)
+            return fail(WAE_INVALID_STATE, "bind: graph index " + std::to_string(it.graph_index) + " is out of range");
+        auto wi = b->wave_index.find({b->batch_pos(it.graph_index), it.node});
+        if (wi == b->wave_index.end())
+            return fail(WAE_INVALID_STATE, "bind: node " + std::to_string(it.node) + " of graph " + std::to_string(it.graph_index) +
+                                               " is not a periodic wave bound from device memory (wae_oscillator_set_device_periodic_wave)");
+        const size_t k = wi->second;
+        if (named[k]++)  // (two items of one launch writing one wavetable: which one lands would be undefined)
+            return fail(WAE_INVALID_ARGUMENT, "bind: node " + std::to_string(it.node) + " of graph " + std::to_string(it.graph_index) +
+                                                  " is named twice in one call");
+        const wae_batch::DevWave& d = b->waves[k];
+        if (!it.real && !it.imag) return fail(WAE_INVALID_ARGUMENT, "bind: null real and imag");
+        const uint64_t bytes = (uint64_t)d.coefficients * sizeof(float);
+        for (const float* p : {it.real, it.imag}) {
+            if (!p) continue;
+            wae_status st = extents.check(p, bytes, p == it.real ? "real" : "imag",
+                                          "[coefficients, coefficients + count) runs past the end of its allocation");
+            if (st != WAE_OK) return st;
+        }
+        if (!d.d) continue;  // declared, never rendered: nothing to write
+        table.push_back(WaveBindItem{it.real, it.imag, d.d, (int32_t)d.coefficients, (int32_t)d.table_len, d.normalize ? 1 : 0, 0});
+        max_len = std::max(max_len, (int)d.table_len);
+        any_normalize = any_normalize || d.normalize;
+        wave_of.push_back(k);
+    }
+    if (table.empty()) return WAE_OK;
+    wae_status st = bind_after(b, stream);
+    if (st == WAE_OK) st = stage_bind_table(b, table.data(), table.size() * sizeof(WaveBindItem));
+    if (st != WAE_OK) return st;
+    launch_bind_waves(static_cast<const WaveBindItem*>(b->d_bind), (int)table.size(), max_len, any_normalize, b->engine->stream);
+    cudaError_t le = cudaGetLastError();
+    if (le != cudaSuccess) return fail(WAE_CUDA_ERROR, std::string("bind: ") + cudaGetErrorString(le));
+    for (size_t k : wave_of)
+        if (!b->waves[k].bound) {
+            b->waves[k].bound = true;
+            b->waves_unbound--;
+        }
+    return WAE_OK;
+}
+
 WAE_API wae_status wae_batch_sync(wae_batch* b) {
     CUDA_TRY(cudaSetDevice(b->engine->device));
     CUDA_TRY(cudaStreamSynchronize(b->engine->stream));
@@ -5536,6 +5659,9 @@ static wae_status refuse_device_inputs(wae_graph* const* graphs, uint32_t n_grap
         if (graphs[i] && graphs[i]->device_curves)
             return fail(WAE_INVALID_STATE, "graph " + std::to_string(i) + " has WaveShaper curves bound from device memory: render it with "
                                            "wae_batch_prepare (or _prepare_many), wae_batch_bind_curves and wae_batch_run");
+        if (graphs[i] && graphs[i]->device_waves)
+            return fail(WAE_INVALID_STATE, "graph " + std::to_string(i) + " has periodic waves bound from device memory: render it with "
+                                           "wae_batch_prepare (or _prepare_many), wae_batch_bind_periodic_waves and wae_batch_run");
     }
     return WAE_OK;
 }

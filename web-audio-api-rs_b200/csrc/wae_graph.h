@@ -129,6 +129,11 @@ struct Node {
     // wae_wave_shaper_set_device_curve: the curve's length (has_curve is set, `table` stays empty); its points are written by
     // wae_batch_bind_curves.  0: not declared
     uint32_t device_curve = 0;
+    // wae_oscillator_set_device_periodic_wave: the coefficient count of the wave (type is Custom, `table` stays empty), the length of
+    // the wavetable wae_batch_bind_periodic_waves synthesises from the bound coefficients, and whether it is normalised.  0: not declared
+    uint32_t device_wave = 0;
+    uint32_t device_wave_len = 0;
+    bool device_wave_normalize = true;
     int oversample = 0;  // WaveShaper: WAE_OVERSAMPLE_*
     std::vector<double> feedforward, feedback;  // IIR
     std::shared_ptr<PcmBuffer> buffer;          // ABSN buffer / convolver IR
@@ -259,6 +264,7 @@ struct wae_graph {
     uint32_t device_params = 0;  // AudioParams declared with wae_param_set_device_value
     uint32_t device_responses = 0;  // ConvolverNodes declared with wae_convolver_set_device_response (never in `assets`)
     uint32_t device_curves = 0;     // WaveShaperNodes declared with wae_wave_shaper_set_device_curve
+    uint32_t device_waves = 0;      // OscillatorNodes declared with wae_oscillator_set_device_periodic_wave
 
     uint32_t create_param(uint32_t owner, float def, float mn, float mx, bool a_rate, float initial, bool send_set_value = true,
                           bool fixed_id = false, uint32_t id = 0, bool constrained = false);

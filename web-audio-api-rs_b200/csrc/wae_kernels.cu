@@ -4408,6 +4408,62 @@ __global__ void __launch_bounds__(256) k_bind_curves(const CurveBindItem* __rest
     }
 }
 
+// ---- wae_batch_bind_periodic_waves: the wavetables of declared custom oscillators -----------------------------------------------
+// k_bind_waves: grid (tiles of WAVE_TILE table entries, items).  generate_wavetable (periodic_wave.rs:164-190) as
+// wae_periodic_wave_table evaluates it: every thread owns one table entry and sums the harmonics j = 1 .. n-1 in the host's order with
+// the host's f32 operations (the build has no FMA contraction); the CTA stages the coefficients through shared memory, so each one is
+// a broadcast read.  sin / cos of the f32 phase are the f64 values rounded to f32, which agree with the host's sinf / cosf on nearly
+// every argument (DESIGN.md §2).
+constexpr int WAVE_TILE = 256;
+__global__ void __launch_bounds__(WAVE_TILE) k_bind_waves(const WaveBindItem* __restrict__ items) {
+    __shared__ float s_re[WAVE_TILE], s_im[WAVE_TILE];
+    const WaveBindItem it = items[blockIdx.y];
+    if ((int)blockIdx.x * WAVE_TILE >= it.len) return;  // (the whole CTA: shorter tables than the launch's longest)
+    const int i = blockIdx.x * WAVE_TILE + threadIdx.x;
+    const float pi_2 = 2.f * 3.14159265358979323846f;
+    const float phase = __fdiv_rn(__fmul_rn(pi_2, (float)i), (float)it.len);
+    float sample = 0.f;
+    for (int c0 = 1; c0 < it.n; c0 += WAVE_TILE) {
+        const int cn = min(WAVE_TILE, it.n - c0);
+        __syncthreads();  // (the previous chunk is read)
+        if (threadIdx.x < cn) {
+            s_re[threadIdx.x] = it.re ? __ldg(it.re + c0 + threadIdx.x) : 0.f;
+            s_im[threadIdx.x] = it.im ? __ldg(it.im + c0 + threadIdx.x) : 0.f;
+        }
+        __syncthreads();
+        for (int k = 0; k < cn; k++) {
+            const float rad = __fmul_rn(phase, (float)(c0 + k));
+            double sd, cd;
+            sincos((double)rad, &sd, &cd);
+            sample = __fadd_rn(sample, __fadd_rn(__fmul_rn(s_re[k], (float)cd), __fmul_rn(s_im[k], (float)sd)));
+        }
+    }
+    if (i < it.len) it.dst[i] = sample;
+}
+
+// k_wave_normalize: one CTA per item that normalises (periodic_wave.rs:192-209): the largest |x| (fmaxf ignores NaN as the host's `>`
+// does; max is order-independent, so the result is the host's), then x *= 1 / max when max > 0
+__global__ void __launch_bounds__(1024) k_wave_normalize(const WaveBindItem* __restrict__ items) {
+    __shared__ float s_max[32];
+    const WaveBindItem it = items[blockIdx.x];
+    if (!it.normalize) return;
+    float mx = 0.f;
+    for (int i = threadIdx.x; i < it.len; i += blockDim.x) mx = fmaxf(mx, fabsf(it.dst[i]));
+    for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+    if ((threadIdx.x & 31) == 0) s_max[threadIdx.x >> 5] = mx;
+    __syncthreads();
+    if (threadIdx.x < 32) {
+        mx = threadIdx.x < (blockDim.x >> 5) ? s_max[threadIdx.x] : 0.f;
+        for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+        if (threadIdx.x == 0) s_max[0] = mx;
+    }
+    __syncthreads();
+    mx = s_max[0];
+    if (!(mx > 0.f)) return;
+    const float norm = __fdiv_rn(1.f, mx);
+    for (int i = threadIdx.x; i < it.len; i += blockDim.x) it.dst[i] = __fmul_rn(it.dst[i], norm);
+}
+
 // Host emulation of the transforms above with the SAME butterfly, index and twiddle code (tests/test_conv_fft_host.py pins them against
 // numpy on a machine without a GPU).  mode 0: complex forward, natural -> position order; 1: complex inverse, position -> natural order
 // (unnormalised); 2: 2B reals -> B packed bins in position order; 3: B packed bins -> 2B reals (scaled by 1 / 2B).  data: 2B floats in place.
@@ -4946,6 +5002,11 @@ void launch_bind_responses(RespBindItem* d, int n, bool any_normalize, int64_t m
     k_resp_fft<<<dim3((unsigned)max_S, (unsigned)max_ch, (unsigned)n), CV_THREADS, CV_SMEM_ELEMS * sizeof(float2), s>>>(d);
 }
 void launch_bind_curves(const CurveBindItem* d, int n, cudaStream_t s) { k_bind_curves<<<(unsigned)n, 256, 0, s>>>(d); }
+void launch_bind_waves(const WaveBindItem* d, int n, int max_len, bool any_normalize, cudaStream_t s) {
+    for (int k = 0; k < n; k += 65535)  // (grid.y is at most 65535)
+        k_bind_waves<<<dim3((unsigned)((max_len + WAVE_TILE - 1) / WAVE_TILE), (unsigned)std::min(n - k, 65535)), WAVE_TILE, 0, s>>>(d + k);
+    if (any_normalize) k_wave_normalize<<<(unsigned)n, 1024, 0, s>>>(d);
+}
 void launch_conv_ir_fft(const float* ir, int64_t ir_len, int64_t ir_stride, float2* h, int S, int channels, cudaStream_t s) {
     conv_configure();
     k_conv_ir_fft<<<dim3((unsigned)S, (unsigned)channels), CV_THREADS, CV_SMEM_ELEMS * sizeof(float2), s>>>(ir, ir_len, ir_stride, h, S);

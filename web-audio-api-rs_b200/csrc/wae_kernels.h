@@ -114,6 +114,9 @@ void launch_bind_params(const ParamBindItem* d, int n, const ParamSlotInfo* info
 void launch_bind_responses(RespBindItem* d, int n, bool any_normalize, int64_t max_len, int max_S, int max_ch, cudaStream_t s);
 // a bind of n WaveShaper curves (k_bind_curves): copy, can_propagate_silence, the patch entries it decides
 void launch_bind_curves(const CurveBindItem* d, int n, cudaStream_t s);
+// a bind of n periodic waves: the wavetables (k_bind_waves, max_len = the longest), then their normalisation (k_wave_normalize, when
+// any_normalize)
+void launch_bind_waves(const WaveBindItem* d, int n, int max_len, bool any_normalize, cudaStream_t s);
 void launch_conv_ir_fft(const float* ir, int64_t ir_len, int64_t ir_stride, float2* h, int S, int channels, cudaStream_t s);
 
 }  // namespace wae
