@@ -642,6 +642,34 @@ typedef struct wae_periodic_wave_binding {
  * wae_batch_run_group and wae_batch_run_pipelined answer WAE_INVALID_STATE while a declared wave of the batch has never been bound. */
 WAE_API wae_status wae_batch_bind_periodic_waves(wae_batch* batch, const wae_periodic_wave_binding* items, uint32_t n, void* stream);
 
+/* ---- IIRFilterNode coefficients bound from device memory --------------------------------------------------------------------
+ * The IIRFilterNode's coefficients are supplied per run from device memory (wae_batch_bind_iir_coefficients) instead of its options, so
+ * that one prepared batch filters with any number of coefficient sets (an EQ a network predicts, random filters for augmentation) without
+ * being built and planned again.  The counts are the node's own (as constructed); the constructed coefficients are what wae_batch_plan
+ * plans with (the lowering depends on the counts only, so the plan is that of the constructed node).  WAE_INVALID_ARGUMENT: not an
+ * IIRFilterNode.  WAE_INVALID_STATE: the node is declared twice, or the graph already has a suspend point.  Suspend points added later
+ * are allowed (every segment reads the one bound set).  wae_render_batch and wae_render_many answer WAE_INVALID_STATE on graphs with
+ * such nodes; wae_batch_plan plans them. */
+WAE_API wae_status wae_iir_filter_set_device_coefficients(wae_graph* graph, wae_node_id node);
+
+typedef struct wae_iir_binding {
+    uint32_t graph_index;      /* caller's index, as wae_batch_fetch_graph */
+    wae_node_id node;          /* declared with wae_iir_filter_set_device_coefficients */
+    const double* feedforward; /* device memory of the engine's GPU: the node's feedforward count of doubles, any 8 B alignment */
+    const double* feedback;    /* likewise, the node's feedback count */
+} wae_iir_binding;
+
+/* Writes the coefficients into the batch, asynchronously on the engine stream after the work already queued on `stream` (as
+ * wae_batch_bind_sources).  They are normalised by feedback[0] in f64 as the constructor's coefficients are, so bound coefficients render
+ * bit for bit what a node constructed with them renders; NaN and infinities are used as they are.  Deviation: the reference refuses
+ * feedback[0] == 0 at construction; such an item writes all-zero coefficients, and the filter outputs zeros.  All-or-nothing: every
+ * item is validated before anything is enqueued.  A bound set stays until it is bound again.  WAE_INVALID_ARGUMENT: a null pointer, one
+ * that is not 8-byte aligned or not device (or managed) memory of the engine's GPU, an extent that does not lie in one allocation, or
+ * one (graph, node) named twice in the call.  WAE_INVALID_STATE: graph_index out of range, or the node was not declared.  wae_batch_run,
+ * wae_batch_run_group and wae_batch_run_pipelined answer WAE_INVALID_STATE while a declared IIR filter of the batch has never been
+ * bound. */
+WAE_API wae_status wae_batch_bind_iir_coefficients(wae_batch* batch, const wae_iir_binding* items, uint32_t n, void* stream);
+
 /* PeriodicWave::new(context, PeriodicWaveOptions { real, imag, disable_normalization }) (src/periodic_wave.rs:104-209): fills `table`
  * (PERIODIC_WAVE_TABLE_LENGTH = 8192 in the reference) with the wavetable an OscillatorNode of type Custom plays.  `real` / `imag` may be
  * NULL (= zeros); both NULL = the sine default.  Host math, no engine needed. */

@@ -144,6 +144,11 @@ class PeriodicWaveBinding(C.Structure):
     _fields_ = [("graph_index", C.c_uint32), ("node", C.c_uint32), ("real", c_float_p), ("imag", c_float_p)]
 
 
+class IirBinding(C.Structure):
+    """wae_iir_binding: the device f64 coefficients of one declared IIRFilterNode of a prepared batch (wae_batch_bind_iir_coefficients)."""
+    _fields_ = [("graph_index", C.c_uint32), ("node", C.c_uint32), ("feedforward", c_double_p), ("feedback", c_double_p)]
+
+
 STATUS_NAMES = {0: "OK", 1: "INVALID_ARGUMENT", 2: "INVALID_STATE", 3: "NOT_SUPPORTED", 4: "UNSUPPORTED",
                 5: "CUDA_ERROR", 6: "OUT_OF_MEMORY", 7: "NO_DEVICE"}
 
@@ -187,6 +192,7 @@ WAE_SYMBOLS = [
     "wae_convolver_set_device_response", "wae_batch_bind_responses",
     "wae_wave_shaper_set_device_curve", "wae_batch_bind_curves",
     "wae_oscillator_set_device_periodic_wave", "wae_batch_bind_periodic_waves",
+    "wae_iir_filter_set_device_coefficients", "wae_batch_bind_iir_coefficients",
 ]
 
 
@@ -302,6 +308,9 @@ class Api:
             # periodic waves bound from device memory
             f("oscillator_set_device_periodic_wave", C.c_int32, [gp, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32])
             f("batch_bind_periodic_waves", C.c_int32, [C.c_void_p, C.POINTER(PeriodicWaveBinding), C.c_uint32, C.c_void_p])
+            # IIR coefficients bound from device memory
+            f("iir_filter_set_device_coefficients", C.c_int32, [gp, C.c_uint32])
+            f("batch_bind_iir_coefficients", C.c_int32, [C.c_void_p, C.POINTER(IirBinding), C.c_uint32, C.c_void_p])
         else:
             f("graph_create", C.c_int32, [C.c_uint32, C.c_uint64, C.c_float, C.POINTER(C.c_void_p)])
             f("render", C.c_int32, [gp, c_float_p])

@@ -394,8 +394,21 @@ class BiquadFilterNode(AudioNode):
 
 
 class IIRFilterNode(AudioNode):
+    def set_device_coefficients(self):
+        """wae_iir_filter_set_device_coefficients (product only): the node filters with the feedforward / feedback coefficients that
+        Batch.bind_iir_coefficients supplies from device memory before each run, as many of each as the node was constructed with.
+        Plans are made with the constructed coefficients."""
+        api = self._ctx._api
+        if not api.is_product:
+            raise B.WaeError(3, "IIR coefficients bound from device memory are a feature of the GPU engine")
+        api.check(api.iir_filter_set_device_coefficients(self._ctx._g, self.id))
+        self._ctx._device_iirs[self.id] = (len(self.feedforward), len(self.feedback))
+
     def get_frequency_response(self, frequency_hz):
         """IIRFilterNode::get_frequency_response (src/node/iir_filter.rs:215-265) -> (mag_response, phase_response)."""
+        if self.id in self._ctx._device_iirs:
+            raise B.WaeError(2, "get_frequency_response: the coefficients of this IIRFilterNode are bound from device memory "
+                                "(set_device_coefficients)")
         f, mag, phase = _response_arrays(frequency_hz)
         ff, fb = self.feedforward, self.feedback
         self._ctx._api.iir_frequency_response(ff.ctypes.data_as(B.c_double_p), len(ff), fb.ctypes.data_as(B.c_double_p), len(fb), self._ctx._sample_rate,
@@ -487,6 +500,7 @@ class OfflineAudioContext:
         self._device_responses = {}  # node id -> (channels, length) declared with set_device_response
         self._device_curves = {}  # node id -> length declared with set_device_curve
         self._device_waves = {}  # node id -> coefficient count declared with set_device_periodic_wave
+        self._device_iirs = {}  # node id -> (feedforward count, feedback count) declared with set_device_coefficients
 
     def __del__(self):
         try:
@@ -868,6 +882,36 @@ class Batch:
         self.api.check(self.api.batch_bind_periodic_waves(self.handle, items, n, C.c_void_p(self._torch_stream_handle())))
         for t in given:
             self._keep_until_read(t)
+
+    def bind_iir_coefficients(self, nodes, feedforward, feedback, graphs=None):
+        """wae_batch_bind_iir_coefficients: feedforward[k] and feedback[k] (rows of float64 CUDA tensors [n][nff] and [n][nfb], unit
+        stride on the last dimension) become the coefficients of IIRFilterNode nodes[k] (declared with set_device_coefficients) of context
+        graphs[k] (default: 0..n-1).  `nodes` as for bind_sources.  One call, ordered after torch's current stream; the coefficients are
+        read on the engine stream, and the tensors' memory is kept from reuse until they have been."""
+        import torch
+        for t in (feedforward, feedback):
+            if not (isinstance(t, torch.Tensor) and t.is_cuda and t.dtype == torch.float64 and t.dim() == 2):
+                raise B.WaeError(1, "bind_iir_coefficients: feedforward and feedback must be float64 CUDA tensors [n][count]")
+        n = feedforward.shape[0]
+        if feedback.shape[0] != n:
+            raise B.WaeError(1, f"bind_iir_coefficients: {n} feedforward rows and {feedback.shape[0]} feedback rows")
+        graphs, ids = self._graphs_and_nodes("bind_iir_coefficients", nodes, graphs, n)
+        if n and (feedforward.stride(1) != 1 or feedback.stride(1) != 1):
+            raise B.WaeError(1, "bind_iir_coefficients: the coefficients of a filter must be contiguous (unit stride on the last dimension)")
+
+        def row(t, k):
+            return C.cast(C.c_void_p(t.data_ptr() + 8 * k * t.stride(0)), B.c_double_p)
+        items = (B.IirBinding * max(n, 1))()
+        for k, (g, nid) in enumerate(zip(graphs, ids)):
+            declared = self.contexts[g]._device_iirs.get(int(nid))
+            # (the tensors' own shapes: the library checks only the CUDA allocations, which may hold several tensors)
+            if declared is not None and (feedforward.shape[1], feedback.shape[1]) != declared:
+                raise B.WaeError(1, f"bind_iir_coefficients: row {k} has {feedforward.shape[1]} feedforward and {feedback.shape[1]} "
+                                    f"feedback coefficients, node {nid} of graph {g} was declared with {declared[0]} and {declared[1]}")
+            items[k] = B.IirBinding(g, int(nid), row(feedforward, k), row(feedback, k))
+        self.api.check(self.api.batch_bind_iir_coefficients(self.handle, items, n, C.c_void_p(self._torch_stream_handle())))
+        self._keep_until_read(feedforward)
+        self._keep_until_read(feedback)
 
     def _graphs_and_nodes(self, fn, nodes, graphs, n):
         """The graph index and node id of each of n binding items: `graphs` (default 0..n-1), `nodes` one node (or id) for all graphs or

@@ -1176,6 +1176,21 @@ WAE_API wae_status wae_oscillator_set_device_periodic_wave(wae_graph* g, wae_nod
     return WAE_OK;
 }
 
+// A declared IIR filter keeps its coefficient counts; its coefficients are written per run by wae_batch_bind_iir_coefficients.  The
+// planner picks the filter's path from the counts alone, so the constructed coefficients plan the node as bound ones would.
+WAE_API wae_status wae_iir_filter_set_device_coefficients(wae_graph* g, wae_node_id node) {
+    Node* n = node_of_kind(g, node, K_IIR);
+    if (!n) return fail(WAE_INVALID_ARGUMENT, "not an IIRFilterNode");
+    if (n->device_iir)
+        return fail(WAE_INVALID_STATE,
+                    "InvalidStateError - the coefficients are already bound from device memory (wae_iir_filter_set_device_coefficients)");
+    if (!g->epochs.empty())  // (the segments before the suspend point were planned with the graph copy of their own: no declaration)
+        return fail(WAE_INVALID_STATE, "InvalidStateError - IIR coefficients are bound from device memory before the first suspend point");
+    n->device_iir = true;
+    g->device_iirs++;
+    return WAE_OK;
+}
+
 // the scalar setters of AudioBufferSourceNode (audio_buffer_source.rs:324-349), ConvolverNode (convolver.rs:325-328), WaveShaperNode
 // (waveshaper.rs:226-229), PannerNode (panner.rs:545-657) and AnalyserNode (analyser.rs:148-222)
 WAE_API wae_status wae_node_set_attribute(wae_graph* g, wae_node_id node, uint32_t attribute, double value) {

@@ -563,6 +563,23 @@ struct WaveBindItem {
     int32_t pad;
 };
 
+// ---- wae_batch_bind_iir_coefficients: caller f64 coefficients -> the records of a declared IIRFilterNode ---------------------------
+// One record the coefficients reach: an IirInst (k_iir_serial; `b` = IirInst::b, `a` = IirInst::a, n = max(nff, nfb) of each) or the
+// ChainBiquad of a k_chain record (`b` = ChainBiquad::b0: b0, b1, b2, a1, a2; `a` null) with its scan constants (`scan`, null: none).
+struct IirPatch {
+    double* b;
+    double* a;
+    void* scan;  // ScanCoef
+};
+struct IirBindItem {
+    const double* ff;         // caller's coefficients (8 B aligned)
+    const double* fb;
+    const IirPatch* patches;  // the node's entries
+    int32_t nff, nfb;         // 1..20 each
+    int32_t n_patches;
+    int32_t pad;
+};
+
 // ---- wae_batch_bind_params: per-run values of params planned as constants ------------------------------------------------------
 struct ParamBindItem {  // one float of the caller's device memory -> value slot `slot`
     const float* src;

@@ -320,8 +320,17 @@ struct StageBuild {
         int32_t keeps, other;
     };
     std::vector<CurvePatchRec> curve_patches;
+    // Patch entries of IIR coefficients bound from device memory (wae_iir_filter_set_device_coefficients): record `rec` of this stage's
+    // table, an IirInst (S_IIR, bq = -1) or biquad `bq` of a ChainInst (S_CHAIN / S_VSUM) with its scan constants `scan`
+    struct IirPatchRec {
+        uint32_t graph;  // batch position
+        wae_node_id node;
+        int32_t rec, bq, scan;
+    };
+    std::vector<IirPatchRec> iir_patches;
     size_t records() const {  // size of the table patch entries point into
         switch (kind) {
+            case S_IIR: return iir.size();
             case S_SHAPER_OS: return shaper_os.size();
             case S_CHAIN: case S_VSUM: return chain.size();
             case S_BIQUAD: return biquad.size();
@@ -501,6 +510,20 @@ struct wae_batch {
     std::vector<DevWave> waves;
     std::map<std::pair<uint32_t, wae_node_id>, size_t> wave_index;  // (batch position, node) -> waves
     size_t waves_unbound = 0;
+    // wae_iir_filter_set_device_coefficients: the range of each declared filter's patch entries in d_iir_patches (every record its
+    // coefficients reach), rewritten by wae_batch_bind_iir_coefficients.  A declared filter the planner never reached has none: binding it
+    // is validated and writes nothing, and runs do not wait for it.
+    struct DevIir {
+        uint32_t graph;  // batch position
+        wae_node_id node;
+        uint32_t nff, nfb;
+        int32_t p0, p1;  // its entries in d_iir_patches
+        bool bound;
+    };
+    std::vector<DevIir> iirs;
+    std::map<std::pair<uint32_t, wae_node_id>, size_t> iir_index;  // (batch position, node) -> iirs
+    size_t iirs_unbound = 0;
+    IirPatch* d_iir_patches = nullptr;
     cudaEvent_t ev_bind = nullptr;  // orders a bind after the caller's stream
     // OfflineAudioContext::suspend_sync: a group's render is cut at the suspend frames of its graphs (graphs with different
     // suspend points are put in different groups); every segment has its own plan, node state is shared between the plans
@@ -887,6 +910,9 @@ struct Planner {
         PatchRec gain_fold[4] = {};
         // a shaper whose curve is bound from device memory: the entry of shaper_keeps_silence (rec / off set when the chain is emitted)
         std::vector<StageBuild::CurvePatchRec> curve_patches;
+        // IIR filters whose coefficients are bound from device memory: the entry of their biquad (bq; rec / scan set when the chain is
+        // emitted)
+        std::vector<StageBuild::IirPatchRec> iir_patches;
     };
 
     // Node state is allocated through a key (graph, node, n-th allocation of that node, salt): the plans of consecutive
@@ -1121,6 +1147,11 @@ struct Planner {
             r.off = (uint32_t)offsetof(ChainInst, shaper_keeps_silence);
             s.curve_patches.push_back(r);
         }
+        for (StageBuild::IirPatchRec r : pc.iir_patches) {
+            r.rec = rec;
+            r.scan = pc.inst.bq[r.bq].coef;
+            s.iir_patches.push_back(r);
+        }
     }
     static bool chain_has_patches(const PendingChain& pc) {
         bool any = !pc.patches.empty();
@@ -1191,8 +1222,9 @@ struct Planner {
         return pc;
     }
     // a biquad (or an IIR filter of order <= 2, which opens a chain of its own with a constant layout) appended to the chain it joins
-    // `bound`: the patch entry of a biquad with params bound from device memory
-    bool append_biquad(NodeCtx& nc, double* state, const hm::BiquadCoefs& c, const PatchRec* bound = nullptr) {
+    // `bound`: the patch entry of a biquad with params bound from device memory; `iir_bound`: an IIR filter whose coefficients are bound
+    // from device memory
+    bool append_biquad(NodeCtx& nc, double* state, const hm::BiquadCoefs& c, const PatchRec* bound = nullptr, bool iir_bound = false) {
         PendingChain pc = open_chain(nc);
         ChainBiquad& st = pc.inst.bq[pc.inst.n_biquad++];
         st.state = state;
@@ -1202,6 +1234,7 @@ struct Planner {
             pc.patches.push_back(*bound);
             pc.patches.back().rec2 = pc.inst.n_biquad - 1;
         }
+        if (iir_bound) pc.iir_patches.push_back(StageBuild::IirPatchRec{gi, nc.n.id, -1, pc.inst.n_biquad - 1, -1});
         pc.phase = pc.phase == 0 ? 1 : 3;
         pc.lay = filter_lay(pc.lay);
         return finish_chain(nc, std::move(pc));
@@ -1418,6 +1451,10 @@ static void merge_builds(Builds& dst, Builds& src) {
             if (pr.rec2 >= 0) pr.rec2 += (int32_t)(s.kind == S_SPAN ? bs.records : bs.scan);
         }
         for (auto& cp : s.curve_patches) cp.rec += (int32_t)bs.records;
+        for (auto& ip : s.iir_patches) {
+            ip.rec += (int32_t)bs.records;
+            if (ip.scan >= 0) ip.scan += (int32_t)bs.scan;
+        }
         for (auto& m : s.mix) m.edge_offset += (uint32_t)bs.mix_edges;
         for (auto& m : s.mix_dyn) m.edge_offset += (uint32_t)bs.mix_edges;
         for (auto& c : s.chain)
@@ -1447,6 +1484,7 @@ static void merge_builds(Builds& dst, Builds& src) {
         append_vec(d.conv_path, s.conv_path); append_vec(d.vgroups, s.vgroups); append_vec(d.conv_cmp, s.conv_cmp);
         append_vec(d.patches, s.patches);
         append_vec(d.curve_patches, s.curve_patches);
+        append_vec(d.iir_patches, s.iir_patches);
         d.n_scan_coef += s.n_scan_coef;
         d.max_ch = std::max(d.max_ch, s.max_ch);
     }
@@ -2608,7 +2646,7 @@ bool Planner::lower_iir(NodeCtx& nc) {
         hm::BiquadCoefs c{ff[0] / a0, ff[1] / a0, ff[2] / a0, fb[1] / a0, fb[2] / a0};
         double* state = alloc<double>((size_t)ch * 4, true, true);
         if (!state) return bail(WAE_OUT_OF_MEMORY, "out of device memory (state)");
-        return append_biquad(nc, state, c);
+        return append_biquad(nc, state, c, nullptr, n.device_iir);
     }
     if (!need_out(nc, ch)) return false;
     IirInst ii{};
@@ -2628,6 +2666,9 @@ bool Planner::lower_iir(NodeCtx& nc) {
     StageBuild& s = stage(nc.L, S_IIR);
     s.max_ch = std::max(s.max_ch, ch);
     s.iir.push_back(ii);
+    // coefficients bound from device memory (wae_iir_filter_set_device_coefficients): the bind rewrites b[0..n) and a[0..n) of this
+    // segment's record
+    if (n.device_iir) s.iir_patches.push_back(StageBuild::IirPatchRec{gi, n.id, (int32_t)s.iir.size() - 1, -1, -1});
     return true;
 }
 
@@ -3585,6 +3626,12 @@ struct GroupPlan {  // result of phase B for one group
         CurvePatch p;    // device address set
     };
     std::vector<CurveEntry> curve_patches;
+    struct IirEntry {
+        uint32_t graph;  // batch position
+        wae_node_id node;
+        IirPatch p;      // device addresses set
+    };
+    std::vector<IirEntry> iir_patches;
 };
 
 static int64_t padded_length(const wae_graph* g) { return (int64_t)((g->length + 127) / 128 * 128); }
@@ -4197,6 +4244,22 @@ static void prep_plan_group(wae_batch* b, wae_graph* const* graphs, int k, PrepS
                     int32_t* dst = reinterpret_cast<int32_t*>(static_cast<char*>(st.d_a) + (size_t)cp.rec * rec_size + cp.off);
                     gp.curve_patches.push_back({cp.graph, cp.node, CurvePatch{dst, cp.keeps, cp.other}});
                 }
+                // patch entries of IIR coefficients bound from device memory: the coefficient fields of the IirInst or ChainBiquad, and
+                // the biquad's scan constants where they were built
+                for (const auto& ip : s.iir_patches) {
+                    IirPatch p{};
+                    if (ip.bq < 0) {
+                        IirInst* r = static_cast<IirInst*>(st.d_a) + ip.rec;
+                        p.b = reinterpret_cast<double*>(reinterpret_cast<char*>(r) + offsetof(IirInst, b));
+                        p.a = reinterpret_cast<double*>(reinterpret_cast<char*>(r) + offsetof(IirInst, a));
+                    } else {
+                        ChainInst* r = static_cast<ChainInst*>(st.d_a) + ip.rec;
+                        p.b = reinterpret_cast<double*>(reinterpret_cast<char*>(r) + offsetof(ChainInst, bq) + (size_t)ip.bq * sizeof(ChainBiquad) +
+                                                        offsetof(ChainBiquad, b0));
+                        if (ip.scan >= 0 && (size_t)ip.scan < s.scan_coef.size()) p.scan = static_cast<ScanCoef*>(st.d_b) + ip.scan;
+                    }
+                    gp.iir_patches.push_back({ip.graph, ip.node, p});
+                }
             }
         }
         gp.seg_ranges.push_back({seg_stage0, gp.stages.size()});
@@ -4334,9 +4397,51 @@ static void record_waves(wae_batch* b, wae_graph* const* graphs, uint32_t n_grap
     }
 }
 
-// runs of a batch need every device input, param, response, curve and periodic wave bound once
+// The declared IIR filters of the batch (`graphs` in batch order, each in graph and node order), after planning, with the patch
+// entries of the planned groups gathered per filter and uploaded (from `patches`, which the caller keeps alive until the stream has been
+// synchronised).  The ones the planner reached are unbound; the ones it never reached have no entries: binding them is validated and
+// writes nothing, and runs do not wait for them.
+static wae_status record_iirs(wae_batch* b, wae_graph* const* graphs, uint32_t n_graphs, const std::vector<GroupPlan>& gps,
+                              std::vector<IirPatch>& patches) {
+    for (uint32_t j = 0; j < n_graphs; j++) {
+        if (!graphs[j]->device_iirs) continue;
+        auto scan = [&](const NodeMap& nodes) {
+            for (const auto& kv : nodes) {
+                const Node& nd = kv.second;
+                if (nd.kind != K_IIR || !nd.device_iir || b->iir_index.count({j, nd.id})) continue;
+                b->iir_index[{j, nd.id}] = b->iirs.size();
+                b->iirs.push_back(wae_batch::DevIir{j, nd.id, (uint32_t)nd.feedforward.size(), (uint32_t)nd.feedback.size(), 0, 0, false});
+            }
+        };
+        scan(graphs[j]->nodes);
+        for (const auto& ep : graphs[j]->epochs) scan(ep.nodes);
+    }
+    std::vector<std::vector<IirPatch>> per(b->iirs.size());
+    for (const auto& gp : gps)
+        for (const auto& e : gp.iir_patches) per[b->iir_index.at({e.graph, e.node})].push_back(e.p);
+    b->iirs_unbound = 0;
+    for (size_t k = 0; k < per.size(); k++) {
+        wae_batch::DevIir& d = b->iirs[k];
+        d.p0 = (int32_t)patches.size();
+        patches.insert(patches.end(), per[k].begin(), per[k].end());
+        d.p1 = (int32_t)patches.size();
+        d.bound = d.p0 == d.p1;  // (never reached: nothing to wait for)
+        b->iirs_unbound += d.bound ? 0 : 1;
+    }
+    if (!patches.empty() && !(b->d_iir_patches = b->dupload_now(patches)))
+        return fail(WAE_OUT_OF_MEMORY, "out of device memory (IIR patch entries)");
+    return WAE_OK;
+}
+
+// runs of a batch need every device input, param, response, curve, periodic wave and IIR coefficient set bound once
 static wae_status check_bound(wae_batch* b) {
     if (!b) return fail(WAE_INVALID_ARGUMENT, "null batch");
+    for (size_t k = 0; b->iirs_unbound && k < b->iirs.size(); k++)
+        if (const auto& d = b->iirs[k]; !d.bound) {
+            const uint32_t caller = b->order.empty() ? d.graph : b->order[d.graph];
+            return fail(WAE_INVALID_STATE, "IIR coefficients bound from device memory never bound: graph " + std::to_string(caller) +
+                                               ", node " + std::to_string(d.node) + " (wae_batch_bind_iir_coefficients)");
+        }
     for (size_t k = 0; b->waves_unbound && k < b->waves.size(); k++)
         if (const auto& d = b->waves[k]; !d.bound) {
             const uint32_t caller = b->order.empty() ? d.graph : b->order[d.graph];
@@ -4474,9 +4579,11 @@ static wae_status prepare_impl(wae_engine* eng, wae_graph* const* graphs, uint32
     record_responses(b, graphs, n_graphs);
     record_waves(b, graphs, n_graphs);
     std::vector<CurvePatch> curve_patches;
+    std::vector<IirPatch> iir_patches;
     std::vector<ParamSlotInfo> slot_info;
     std::vector<ParamPatch> patches;
     st = record_curves(b, graphs, n_graphs, gps, curve_patches);
+    if (st == WAE_OK) st = record_iirs(b, graphs, n_graphs, gps, iir_patches);
     if (st == WAE_OK) st = record_params(b, graphs, n_graphs, gps, slot_info, patches);
     if (st != WAE_OK) {
         wae_batch_destroy(b);
@@ -5196,6 +5303,57 @@ WAE_API wae_status wae_batch_bind_periodic_waves(wae_batch* b, const wae_periodi
     return WAE_OK;
 }
 
+// The coefficient fields are rewritten on the engine stream: runs queued before the bind have read the previous ones.
+WAE_API wae_status wae_batch_bind_iir_coefficients(wae_batch* b, const wae_iir_binding* items, uint32_t n, void* stream) {
+    if (!b || (n && !items)) return fail(WAE_INVALID_ARGUMENT, "null batch / items");
+    if (n == 0) return WAE_OK;
+    CUDA_TRY(cudaSetDevice(b->engine->device));
+    // every item is validated before anything is enqueued
+    std::vector<IirBindItem> table;
+    std::vector<size_t> iir_of;
+    std::vector<char> named(b->iirs.size(), 0);
+    BindExtents extents{b->engine->device, {}};
+    for (uint32_t i = 0; i < n; i++) {
+        const wae_iir_binding& it = items[i];
+        if (it.graph_index >= b->n_graphs)
+            return fail(WAE_INVALID_STATE, "bind: graph index " + std::to_string(it.graph_index) + " is out of range");
+        auto ii = b->iir_index.find({b->batch_pos(it.graph_index), it.node});
+        if (ii == b->iir_index.end())
+            return fail(WAE_INVALID_STATE, "bind: node " + std::to_string(it.node) + " of graph " + std::to_string(it.graph_index) +
+                                               " is not an IIR filter bound from device memory (wae_iir_filter_set_device_coefficients)");
+        const size_t k = ii->second;
+        if (named[k]++)  // (two items of one launch writing one filter's records: which one lands would be undefined)
+            return fail(WAE_INVALID_ARGUMENT, "bind: node " + std::to_string(it.node) + " of graph " + std::to_string(it.graph_index) +
+                                                  " is named twice in one call");
+        const wae_batch::DevIir& d = b->iirs[k];
+        if (!it.feedforward || !it.feedback) return fail(WAE_INVALID_ARGUMENT, "bind: null feedforward / feedback");
+        if (((uintptr_t)it.feedforward | (uintptr_t)it.feedback) % alignof(double))
+            return fail(WAE_INVALID_ARGUMENT, "bind: feedforward / feedback is not 8-byte aligned");
+        wae_status st = extents.check(it.feedforward, (uint64_t)d.nff * sizeof(double), "feedforward",
+                                      "[feedforward, feedforward + count) runs past the end of its allocation");
+        if (st == WAE_OK)
+            st = extents.check(it.feedback, (uint64_t)d.nfb * sizeof(double), "feedback",
+                               "[feedback, feedback + count) runs past the end of its allocation");
+        if (st != WAE_OK) return st;
+        if (d.p0 == d.p1) continue;  // declared, never rendered: nothing to write
+        table.push_back(IirBindItem{it.feedforward, it.feedback, b->d_iir_patches + d.p0, (int32_t)d.nff, (int32_t)d.nfb, d.p1 - d.p0, 0});
+        iir_of.push_back(k);
+    }
+    if (table.empty()) return WAE_OK;
+    wae_status st = bind_after(b, stream);
+    if (st == WAE_OK) st = stage_bind_table(b, table.data(), table.size() * sizeof(IirBindItem));
+    if (st != WAE_OK) return st;
+    launch_bind_iir(static_cast<const IirBindItem*>(b->d_bind), (int)table.size(), b->engine->stream);
+    cudaError_t le = cudaGetLastError();
+    if (le != cudaSuccess) return fail(WAE_CUDA_ERROR, std::string("bind: ") + cudaGetErrorString(le));
+    for (size_t k : iir_of)
+        if (!b->iirs[k].bound) {
+            b->iirs[k].bound = true;
+            b->iirs_unbound--;
+        }
+    return WAE_OK;
+}
+
 WAE_API wae_status wae_batch_sync(wae_batch* b) {
     CUDA_TRY(cudaSetDevice(b->engine->device));
     CUDA_TRY(cudaStreamSynchronize(b->engine->stream));
@@ -5662,6 +5820,9 @@ static wae_status refuse_device_inputs(wae_graph* const* graphs, uint32_t n_grap
         if (graphs[i] && graphs[i]->device_waves)
             return fail(WAE_INVALID_STATE, "graph " + std::to_string(i) + " has periodic waves bound from device memory: render it with "
                                            "wae_batch_prepare (or _prepare_many), wae_batch_bind_periodic_waves and wae_batch_run");
+        if (graphs[i] && graphs[i]->device_iirs)
+            return fail(WAE_INVALID_STATE, "graph " + std::to_string(i) + " has IIR coefficients bound from device memory: render it with "
+                                           "wae_batch_prepare (or _prepare_many), wae_batch_bind_iir_coefficients and wae_batch_run");
     }
     return WAE_OK;
 }

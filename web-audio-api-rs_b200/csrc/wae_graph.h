@@ -136,6 +136,9 @@ struct Node {
     bool device_wave_normalize = true;
     int oversample = 0;  // WaveShaper: WAE_OVERSAMPLE_*
     std::vector<double> feedforward, feedback;  // IIR
+    // wae_iir_filter_set_device_coefficients: the coefficients are written per run by wae_batch_bind_iir_coefficients (as many as
+    // `feedforward` / `feedback` hold: the plan is made with these constructed ones)
+    bool device_iir = false;
     std::shared_ptr<PcmBuffer> buffer;          // ABSN buffer / convolver IR
     bool normalize = true;                      // convolver: the scale the CURRENT buffer was given (taken when the buffer is set)
     bool normalize_next = true;                 // ConvolverNode::set_normalize: applies to the next set_buffer (convolver.rs:325-328)
@@ -265,6 +268,7 @@ struct wae_graph {
     uint32_t device_responses = 0;  // ConvolverNodes declared with wae_convolver_set_device_response (never in `assets`)
     uint32_t device_curves = 0;     // WaveShaperNodes declared with wae_wave_shaper_set_device_curve
     uint32_t device_waves = 0;      // OscillatorNodes declared with wae_oscillator_set_device_periodic_wave
+    uint32_t device_iirs = 0;       // IIRFilterNodes declared with wae_iir_filter_set_device_coefficients
 
     uint32_t create_param(uint32_t owner, float def, float mn, float mx, bool a_rate, float initial, bool send_set_value = true,
                           bool fixed_id = false, uint32_t id = 0, bool constrained = false);

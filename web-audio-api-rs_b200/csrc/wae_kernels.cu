@@ -4464,6 +4464,36 @@ __global__ void __launch_bounds__(1024) k_wave_normalize(const WaveBindItem* __r
     for (int i = threadIdx.x; i < it.len; i += blockDim.x) it.dst[i] = __fmul_rn(it.dst[i], norm);
 }
 
+// ---- wae_batch_bind_iir_coefficients: one CTA per declared IIRFilterNode -----------------------------------------------------------
+// The shorter list padded with zeros to the longer one (and an order <= 2 filter to 3 on the chain path), every coefficient divided by
+// feedback[0] (iir_filter.rs:282-309): the IEEE f64 quotients Planner::lower_iir computes, so that bound coefficients are bit-equal to a
+// node constructed with them.  feedback[0] == 0, which the constructor refuses, writes zeros (the filter outputs silence).  Then every
+// patch entry of the item: the IirInst coefficients of each render segment, or the chain's biquad and its scan constants.
+__global__ void __launch_bounds__(32) k_bind_iir(const IirBindItem* __restrict__ items) {
+    __shared__ double s_b[20], s_a[20];
+    const IirBindItem it = items[blockIdx.x];
+    const double a0 = it.fb[0];
+    for (int i = threadIdx.x; i < 20; i += blockDim.x) {
+        const double x = i < it.nff ? it.ff[i] : 0., y = i < it.nfb ? it.fb[i] : 0.;
+        s_b[i] = a0 == 0. ? 0. : __ddiv_rn(x, a0);
+        s_a[i] = a0 == 0. ? 0. : __ddiv_rn(y, a0);
+    }
+    __syncthreads();
+    const int n = max(it.nff, it.nfb);
+    for (int k = threadIdx.x; k < it.n_patches; k += blockDim.x) {
+        const IirPatch p = it.patches[k];
+        if (p.a) {
+            for (int i = 0; i < n; i++) {
+                p.b[i] = s_b[i];
+                p.a[i] = s_a[i];
+            }
+        } else {
+            p.b[0] = s_b[0]; p.b[1] = s_b[1]; p.b[2] = s_b[2]; p.b[3] = s_a[1]; p.b[4] = s_a[2];
+            if (p.scan) make_scan_coef(s_b[1], s_b[2], s_a[1], s_a[2], *static_cast<ScanCoef*>(p.scan));
+        }
+    }
+}
+
 // Host emulation of the transforms above with the SAME butterfly, index and twiddle code (tests/test_conv_fft_host.py pins them against
 // numpy on a machine without a GPU).  mode 0: complex forward, natural -> position order; 1: complex inverse, position -> natural order
 // (unnormalised); 2: 2B reals -> B packed bins in position order; 3: B packed bins -> 2B reals (scaled by 1 / 2B).  data: 2B floats in place.
@@ -5007,6 +5037,7 @@ void launch_bind_waves(const WaveBindItem* d, int n, int max_len, bool any_norma
         k_bind_waves<<<dim3((unsigned)((max_len + WAVE_TILE - 1) / WAVE_TILE), (unsigned)std::min(n - k, 65535)), WAVE_TILE, 0, s>>>(d + k);
     if (any_normalize) k_wave_normalize<<<(unsigned)n, 1024, 0, s>>>(d);
 }
+void launch_bind_iir(const IirBindItem* d, int n, cudaStream_t s) { k_bind_iir<<<(unsigned)n, 32, 0, s>>>(d); }
 void launch_conv_ir_fft(const float* ir, int64_t ir_len, int64_t ir_stride, float2* h, int S, int channels, cudaStream_t s) {
     conv_configure();
     k_conv_ir_fft<<<dim3((unsigned)S, (unsigned)channels), CV_THREADS, CV_SMEM_ELEMS * sizeof(float2), s>>>(ir, ir_len, ir_stride, h, S);

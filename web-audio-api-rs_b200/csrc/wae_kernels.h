@@ -117,6 +117,8 @@ void launch_bind_curves(const CurveBindItem* d, int n, cudaStream_t s);
 // a bind of n periodic waves: the wavetables (k_bind_waves, max_len = the longest), then their normalisation (k_wave_normalize, when
 // any_normalize)
 void launch_bind_waves(const WaveBindItem* d, int n, int max_len, bool any_normalize, cudaStream_t s);
+// a bind of n IIR coefficient sets (k_bind_iir): normalised by feedback[0], written to every patch entry of each item
+void launch_bind_iir(const IirBindItem* d, int n, cudaStream_t s);
 void launch_conv_ir_fft(const float* ir, int64_t ir_len, int64_t ir_stride, float2* h, int S, int channels, cudaStream_t s);
 
 }  // namespace wae
