@@ -531,9 +531,13 @@ WAE_API wae_status wae_batch_bind_sources(wae_batch* batch, const wae_source_bin
  * prepared batch renders any number of parameter sets (EQ, gain, pan, compressor settings drawn on the GPU) without being built and
  * planned again.  The param renders as a constant for the whole render, as a param with only a value does.  param_index numbers the
  * params as wae_param_event_push does.  Bindable: GainNode gain; BiquadFilterNode q, detune, frequency, gain (0..3); StereoPannerNode
- * pan; DynamicsCompressorNode attack, knee, ratio, release, threshold (0..4).  A bound value is clamped to [max(lo, minValue),
- * min(hi, maxValue)], as AudioParam::set_value clamps to [minValue, maxValue].  The range matters for one decision only: a GainNode
- * whose range excludes |gain| <= 1e-6 can never answer with silence, so its output keeps the layout of its input.
+ * pan; DynamicsCompressorNode attack, knee, ratio, release, threshold (0..4); AudioBufferSourceNode detune, playbackRate (0, 1).  A
+ * bound value is clamped to [max(lo, minValue), min(hi, maxValue)], as AudioParam::set_value clamps to [minValue, maxValue].  The range
+ * decides what is planned, never the value: a GainNode whose range excludes |gain| <= 1e-6 can never answer with silence, so its output
+ * keeps the layout of its input.  An AudioBufferSourceNode's two ranges give the computed rates rate * 2^(detune / 1200) it may play
+ * at: a source that does not loop, whose other param is not automated and whose rates are all > 0 is rendered time-parallel (give
+ * detune a range: the default one allows a rate of 0), its output has a constant layout only when the clip lasts to the end of the
+ * render at the highest rate; any other source takes the serial renderer, which is right for every value but slow.
  * Deviation: a non-finite bound value renders as the param's default value (the reference panics on a non-finite set_value, which a
  * device bind cannot do; this is its rule for a NaN computed value).
  * WAE_INVALID_ARGUMENT: lo > hi, a non-finite bound, or a range outside [minValue, maxValue].  WAE_UNSUPPORTED: another node kind or

@@ -599,13 +599,15 @@ WAE_API wae_status wae_connect_param(wae_graph* g, wae_node_id from, uint32_t ou
 }
 
 // Params whose value stays constant over the render, so that a per-run value can be re-derived into the planned records (a GainNode's
-// gain, a BiquadFilterNode's four, a StereoPannerNode's pan, a DynamicsCompressorNode's five)
+// gain, a BiquadFilterNode's four, a StereoPannerNode's pan, a DynamicsCompressorNode's five, an AudioBufferSourceNode's detune and
+// playbackRate: the planner picks the source's playback path from the declared range)
 static bool device_value_supported(Kind kind, uint32_t param_index) {
     switch (kind) {
         case K_GAIN: return param_index == 0;
         case K_BIQUAD: return param_index < 4;
         case K_SPANNER: return param_index == 0;
         case K_COMP: return param_index < 5;
+        case K_ABSN: return param_index < 2;
         default: return false;
     }
 }
@@ -619,7 +621,8 @@ WAE_API wae_status wae_param_set_device_value(wae_graph* g, wae_node_id node, ui
     if (!device_value_supported(n->kind, param_index))
         return fail(WAE_UNSUPPORTED, "param " + std::to_string(param_index) + " of node " + std::to_string(node) +
                                          " cannot be bound from device memory (GainNode gain, BiquadFilterNode q / detune / frequency / gain, "
-                                         "StereoPannerNode pan and DynamicsCompressorNode params can)");
+                                         "StereoPannerNode pan, DynamicsCompressorNode params and AudioBufferSourceNode detune / "
+                                         "playbackRate can)");
     const uint32_t pid = n->params[param_index];
     Param& p = g->nodes.at(pid).param;
     if (p.device_bound) return fail(WAE_INVALID_STATE, "InvalidStateError - the param is already bound from device memory");

@@ -94,6 +94,21 @@ struct AbsnSlowInst {
     int32_t pad;
 };
 
+// A non-looping slow-track source whose playbackRate / detune are bound from device memory (wae_param_set_device_value) over a range of
+// positive computed rates (k_buffer_source_slow<true>).  The record holds what does not depend on the rate; each run derives the rest
+// from `rate` and `detune` (patched by wae_batch_bind_params) with absn_slow_derive, the planner's own expressions.
+struct AbsnBoundInst {
+    AbsnSlowInst s;        // step, offset0, elapsed0 and the segment table are derived per run (one segment: the source does not loop)
+    double dt;             // the planner clock's frame duration
+    double offset;         // start(when, offset): the requested offset
+    double start_delta;    // t_first - start: the first playing frame's time after the start time
+    int64_t n_start;       // fast track: output frames [n_start, fast_end) play buf[n - n_start]
+    int64_t fast_end;
+    int32_t fast_ok;       // aligned start, sampling ratio 1, default loop points, no stop / duration: a computed rate of 1 is the fast track
+    float rate, detune;    // the bound (or planned constant) param values
+    int32_t pad;
+};
+
 // AudioBufferSourceRenderer::process restated frame by frame (audio_buffer_source.rs:422-845) for everything the two
 // closed-form tracks do not cover: automated playbackRate / detune (k-rate), zero / negative rates, very short loops.
 // One warp per instance: lane 0 walks the renderer's state machine of a quantum, all lanes interpolate.

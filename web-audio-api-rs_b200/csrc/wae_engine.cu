@@ -247,11 +247,12 @@ namespace {
 // (the order of the kinds is the launch order inside one level: mixes first; k_delay_mono before the delay reader that needs it)
 enum StageKind : int {
     S_MIX = 0, S_MIX_DYN, S_OSC, S_CONST, S_ABSN, S_BIQUAD, S_IIR, S_GAIN, S_SHAPER, S_SPAN, S_PAN, S_ROUTE, S_DELAY_MONO, S_DELAY, S_DELAY_WRITE, S_COMP, S_ANALYSER,
-    S_CONV_FFT, S_CONV_MAC, S_CONV_MAC_ACC, S_CHAIN, S_PARAM, S_OSC_AR, S_BIQUAD_AR, S_ABSN_SLOW, S_HRTF, S_PAN_DYN, S_ABSN_SERIAL, S_SHAPER_OS, S_META, S_VSUM, S_CONV_CMP, S_KINDS
+    S_CONV_FFT, S_CONV_MAC, S_CONV_MAC_ACC, S_CHAIN, S_PARAM, S_OSC_AR, S_BIQUAD_AR, S_ABSN_SLOW, S_HRTF, S_PAN_DYN, S_ABSN_SERIAL, S_SHAPER_OS, S_META, S_VSUM, S_CONV_CMP, S_ABSN_BOUND, S_KINDS
 };
 const char* kStageNames[S_KINDS] = {"k_mix", "k_mix_dyn", "k_oscillator", "k_constant", "k_buffer_source", "k_biquad_serial", "k_iir_serial", "k_gain",
                                     "k_shaper", "k_stereo_panner", "k_panner_eq", "k_route", "k_delay_mono", "k_delay_read", "k_ring_write", "k_compressor",
-                                    "k_analyser", "k_conv_fft_in", "k_conv_mac_ifft", "k_conv_mac_ifft(acc)", "k_chain", "k_param", "k_osc_arate", "k_biquad_arate", "k_buffer_source_slow", "k_hrtf_fir", "k_panner_dyn", "k_buffer_source_serial", "k_shaper_os", "k_meta", "k_voice_sum", "k_conv_compact"};
+                                    "k_analyser", "k_conv_fft_in", "k_conv_mac_ifft", "k_conv_mac_ifft(acc)", "k_chain", "k_param", "k_osc_arate", "k_biquad_arate", "k_buffer_source_slow", "k_hrtf_fir", "k_panner_dyn", "k_buffer_source_serial", "k_shaper_os", "k_meta", "k_voice_sum", "k_conv_compact",
+                                    "k_buffer_source_slow(bound)"};
 
 // host-side accumulation of instances for one (level, kind) stage
 struct StageBuild {
@@ -286,6 +287,7 @@ struct StageBuild {
     std::vector<HrtfSelInst> hrtf_sel;
     std::vector<PanDynInst> pan_dyn;
     std::vector<AbsnSerialInst> absn_serial;
+    std::vector<AbsnBoundInst> absn_bound;  // S_ABSN_BOUND
     std::vector<ShaperOsInst> shaper_os;
     std::vector<RouteInst> route;
     std::vector<DelayInst> delay;
@@ -339,6 +341,8 @@ struct StageBuild {
             case S_SPAN: return span.size();
             case S_COMP: return comp.size();
             case S_META: return meta.size();
+            case S_ABSN_SERIAL: return absn_serial.size();
+            case S_ABSN_BOUND: return absn_bound.size();
             default: return 0;
         }
     }
@@ -1310,10 +1314,17 @@ struct Planner {
         int ch;
         double duration, ls, le, computed_rate;  // ls / le: the clamped loop boundaries
     };
+    struct AbsnStart {  // the slow track's first playing frame and stop frame
+        int64_t n_first, n_stop;
+        double t_first, start;  // the time of frame n_first, the start time (snapped to it when almost equal)
+    };
+    AbsnStart absn_start(const Node& n) const;
+    int64_t absn_fast_end(int64_t n_start, double duration) const;
     bool lower_absn(NodeCtx& nc);
     bool absn_silent(NodeCtx& nc);
     bool absn_serial(NodeCtx& nc, const AbsnPlay& s, const PRef& pdet, const PRef& prate);
     bool absn_slow(NodeCtx& nc, const AbsnPlay& s);
+    bool absn_bound(NodeCtx& nc, const AbsnPlay& s, const PRef& pdet, const PRef& prate, int64_t q, bool aligned, double rate_hi);
     void absn_schedule(const AbsnSlowInst& a, int64_t n_first, double off, std::vector<int64_t>& seg_n, std::vector<double>& seg_bt) const;
     bool absn_fast(NodeCtx& nc, const AbsnPlay& s, int64_t q, bool fused);
     bool lower_biquad(NodeCtx& nc);
@@ -1417,6 +1428,7 @@ static uint64_t digest_builds(const std::map<std::pair<int, int>, StageBuild>& b
         h = digest_vec_without_end(s.conv_in, h); h = digest_vec_without_end(s.conv_path, h); h = digest_vec(s.vgroups, h);
         if (!s.conv_cmp.empty())
             h = digest_vec_skipping(s.conv_cmp, {offsetof(ConvCmpInst, x) + offsetof(ConvInput, end), offsetof(ConvCmpInst, path) + offsetof(ConvPath, end)}, h);  // (only where it exists: the digests of plans without it stay comparable)
+        if (!s.absn_bound.empty()) h = digest_vec(s.absn_bound, h);  // (the same)
     }
     return h;
 }
@@ -1482,6 +1494,7 @@ static void merge_builds(Builds& dst, Builds& src) {
         append_vec(d.delay, s.delay); append_vec(d.comp, s.comp); append_vec(d.analyser, s.analyser); append_vec(d.mix, s.mix);
         append_vec(d.mix_edges, s.mix_edges); append_vec(d.mix_dyn, s.mix_dyn); append_vec(d.meta, s.meta); append_vec(d.conv_in, s.conv_in);
         append_vec(d.conv_path, s.conv_path); append_vec(d.vgroups, s.vgroups); append_vec(d.conv_cmp, s.conv_cmp);
+        append_vec(d.absn_bound, s.absn_bound);
         append_vec(d.patches, s.patches);
         append_vec(d.curve_patches, s.curve_patches);
         append_vec(d.iir_patches, s.iir_patches);
@@ -2295,6 +2308,7 @@ bool Planner::lower_absn(NodeCtx& nc) {
     PRef pdet = param_ref(n.params[0]), prate = param_ref(n.params[1]);
     const float detune = pdet.v, rate = prate.v;
     const bool rate_automated = pdet.dyn || prate.dyn;
+    const bool rate_bound = pdet.bound >= 0 || prate.bound >= 0;
     int ch = n.buffer ? (int)n.buffer->channels.size() : 1;
     if (!n.buffer || n.start_time >= 1e300 || ch == 0) return absn_silent(nc);  // never plays: silence
     PcmBuffer& pb = *n.buffer;
@@ -2308,10 +2322,20 @@ bool Planner::lower_absn(NodeCtx& nc) {
     // the reference goes through one all-silent slow-track quantum, then aligns (audio_buffer_source.rs:521-523)
     if (n.start_time > clock.block_time(q) && n.start_time == clock.block_time(q + 1)) q = q + 1;
     bool aligned = (n.start_time <= clock.block_time(q)) && n.offset == 0.;  // start in the past snaps to the block
-    bool fast = !rate_automated && aligned && (double)pb.sample_rate / sr == 1. && computed_rate == 1. && ls == 0. && le == duration &&
-                n.duration > 1e300 && n.stop_time > 1e300;
+    bool fast = !rate_automated && !rate_bound && aligned && (double)pb.sample_rate / sr == 1. && computed_rate == 1. && ls == 0. &&
+                le == duration && n.duration > 1e300 && n.stop_time > 1e300;
     // everything the closed-form tracks do not cover runs the renderer's own frame loop (one warp per source)
     bool serial = rate_automated || (!fast && !(computed_rate > 0.));
+    // playbackRate / detune bound from device memory: the path follows from the computed rates their declared ranges allow (the low
+    // corner's exp2 underflows to 0 far enough below 0 cents), never from the value.  A non-looping source whose rates are all positive
+    // takes the bound slow track; the serial kernel is right for every other value.
+    double rate_hi = computed_rate;
+    if (rate_bound) {
+        const bool br = prate.bound >= 0, bd = pdet.bound >= 0;
+        const double rate_lo = (double)(br ? prate.lo : rate) * std::exp2((double)(bd ? pdet.lo : detune) / 1200.);
+        rate_hi = (double)(br ? prate.hi : rate) * std::exp2((double)(bd ? pdet.hi : detune) / 1200.);
+        serial = rate_automated || n.loop || !(rate_lo > 0.);
+    }
     if (!fast && !serial && n.loop) {
         const bool custom = ls >= 0. && le > 0. && ls < le;
         const double loop_len = custom ? le - ls : duration;
@@ -2340,6 +2364,7 @@ bool Planner::lower_absn(NodeCtx& nc) {
     }
     const AbsnPlay s{&pb, d_buf, len, stride, ch, duration, ls, le, computed_rate};
     if (serial) return absn_serial(nc, s, pdet, prate);
+    if (rate_bound) return absn_bound(nc, s, pdet, prate, q, aligned, rate_hi);
     if (!fast) return absn_slow(nc, s);
     return absn_fast(nc, s, q, fused);
 }
@@ -2380,9 +2405,66 @@ bool Planner::absn_serial(NodeCtx& nc, const AbsnPlay& s, const PRef& pdet, cons
     if (!a.state) return bail(WAE_OUT_OF_MEMORY, "out of device memory (buffer source state)");
     out_dynamic(nc, Lay::gated(s.ch));  // when it plays depends on the automated rate: the kernel writes the layout track
     a.out = nc.p.out_buf[0];
-    stage(nc.L, S_ABSN_SERIAL).absn_serial.push_back(a);
+    StageBuild& sb = stage(nc.L, S_ABSN_SERIAL);
+    sb.absn_serial.push_back(a);
+    const PRef* refs[2] = {&pdet, &prate};
+    const size_t offs[2] = {offsetof(AbsnSerialInst, detune), offsetof(AbsnSerialInst, rate)};
+    for (int i = 0; i < 2; i++)
+        if (refs[i]->bound >= 0) {  // bound from device memory (the kernel takes the raw values)
+            PatchRec r = patch(PATCH_RAW, 1);
+            operand(r, 0, *refs[i], refs[i]->v);
+            add_patch(sb, r, (uint32_t)offs[i]);
+        }
     algorithmic_bytes += (uint64_t)s.ch * 4ull * (uint64_t)std::min<int64_t>(lq, (int64_t)s.len);
     return true;
+}
+
+// first frame at / after the start time: current_time = block_time + i * dt (:648), sticky within almost::equal (:652-654); first frame
+// with current_time >= stop_time (:663)
+Planner::AbsnStart Planner::absn_start(const Node& n) const {
+    AbsnStart r{-1, std::numeric_limits<int64_t>::max(), 0., n.start_time};
+    int64_t qq = clock.quantum_containing(r.start);
+    for (int guard = 0; guard < 3 && r.n_first < 0; guard++, qq++) {
+        double bt0 = clock.block_time(qq);
+        for (int i = 0; i < 128; i++) {
+            double t = bt0 + (double)i * clock.dt;
+            if (almost_equal(t, r.start)) r.start = t;
+            if (!(t < r.start)) {
+                r.n_first = qq * 128 + i;
+                r.t_first = t;
+                break;
+            }
+        }
+    }
+    if (r.n_first < 0) r.n_first = qq * 128;
+    if (n.stop_time < 1e300) {
+        int64_t qs = clock.quantum_containing(n.stop_time);
+        int64_t ns = (qs + 1) * 128;
+        double bt0 = clock.block_time(qs);
+        for (int i = 0; i < 128; i++)
+            if (bt0 + (double)i * clock.dt >= n.stop_time) {
+                ns = qs * 128 + i;
+                break;
+            }
+        r.n_stop = ns;
+    }
+    return r;
+}
+
+// the fast track of a non-looping source: the frame after the quantum in which it has `ended`.  The reference accumulates
+// buffer_time += block_duration and stops once it reaches the buffer's duration (audio_buffer_source.rs:609,826-838) — replayed, not
+// divided
+int64_t Planner::absn_fast_end(int64_t n_start, double duration) const {
+    const double block_duration = clock.dt * 128.;
+    const int64_t max_q = (lq - n_start) / 128 + 2;
+    int64_t played = 0;
+    double bt = 0.;
+    while (played < max_q) {
+        bt += block_duration;
+        played++;
+        if (bt >= duration) break;
+    }
+    return n_start + played * 128;
 }
 
 // ---- slow track (audio_buffer_source.rs:625-823): fractional playhead
@@ -2400,7 +2482,6 @@ bool Planner::absn_slow(NodeCtx& nc, const AbsnPlay& s) {
     a.sample_rate = sr;
     a.buffer_duration = duration;
     a.pos_scale = ((double)s.pb->sample_rate / sr) * sr;  // position = buffer_time * sampling_ratio; playhead = position * sr
-    a.step = clock.dt * computed_rate;
     a.duration = n.duration;
     // actual loop points (:627-636)
     if (n.loop && s.ls >= 0. && s.le > 0. && s.ls < s.le) {
@@ -2410,61 +2491,75 @@ bool Planner::absn_slow(NodeCtx& nc, const AbsnPlay& s) {
         a.loop_start = 0.;
         a.loop_end = duration;
     }
-    // first frame at / after the start time: current_time = block_time + i * dt (:648), sticky within
-    // almost::equal (:652-654)
-    double start = n.start_time;
-    int64_t qq = clock.quantum_containing(start);
-    int64_t n_first = -1;
-    double t_first = 0.;
-    for (int guard = 0; guard < 3 && n_first < 0; guard++, qq++) {
-        double bt0 = clock.block_time(qq);
-        for (int i = 0; i < 128; i++) {
-            double t = bt0 + (double)i * clock.dt;
-            if (almost_equal(t, start)) start = t;
-            if (!(t < start)) {
-                n_first = qq * 128 + i;
-                t_first = t;
-                break;
-            }
-        }
-    }
-    if (n_first < 0) n_first = qq * 128;
-    double delta = t_first - start;
-    double off = n.offset + delta * computed_rate;  // :672-674
-    off = std::min(std::max(off, 0.), duration);
-    if (n.loop && off > a.loop_end) off = a.loop_end;  // :676-678 (rate >= 0)
-    a.offset0 = off;
-    a.elapsed0 = std::fabs(delta * computed_rate);
+    const AbsnStart st = absn_start(n);
+    const int64_t n_first = st.n_first;
     a.n_first = n_first;
-    a.n_stop = std::numeric_limits<int64_t>::max();
-    if (n.stop_time < 1e300) {  // first frame with current_time >= stop_time (:663)
-        int64_t qs = clock.quantum_containing(n.stop_time);
-        int64_t ns = (qs + 1) * 128;
-        double bt0 = clock.block_time(qs);
-        for (int i = 0; i < 128; i++)
-            if (bt0 + (double)i * clock.dt >= n.stop_time) {
-                ns = qs * 128 + i;
-                break;
-            }
-        a.n_stop = ns;
-    }
+    a.n_stop = st.n_stop;
+    const AbsnSlowDerived d = absn_slow_derive(clock.dt, computed_rate, n.offset, st.t_first - st.start, duration, n.duration, n.loop, a.loop_end,
+                                               n_first, a.n_stop);
+    a.step = d.step;
+    a.offset0 = d.offset0;
+    a.elapsed0 = d.elapsed0;
+    const double off = d.offset0;
     std::vector<int64_t> seg_n{n_first};
     std::vector<double> seg_bt{off};
     if (n.loop && off < a.loop_end) absn_schedule(a, n_first, off, seg_n, seg_bt);
     a.n_seg = (int32_t)seg_n.size();
     a.seg_n = upload(seg_n);
     a.seg_bt = upload(seg_bt);
-    {
-        // layout: silent before the quantum of the first playing frame and after the quantum in which the source ends
-        // (stop time, explicit duration, or — not looping — the end of the buffer; audio_buffer_source.rs:826-838)
-        int64_t n_end = a.n_stop;
-        if (a.step > 0.) {
-            if (!n.loop) n_end = std::min<int64_t>(n_end, n_first + (int64_t)std::ceil(std::max(0., duration - off) / a.step));
-            if (n.duration < 1e300) n_end = std::min<int64_t>(n_end, n_first + (int64_t)std::ceil(std::max(0., n.duration - a.elapsed0) / a.step));
-        }
-        a.out = source_out(nc, n_first, n_end, s.ch);
-    }
+    // layout: silent before the quantum of the first playing frame and after the quantum in which the source ends
+    // (stop time, explicit duration, or — not looping — the end of the buffer; audio_buffer_source.rs:826-838)
+    a.out = source_out(nc, n_first, d.n_end, s.ch);
     stage(nc.L, S_ABSN_SLOW).absn_slow.push_back(a);
+    algorithmic_bytes += (uint64_t)s.ch * 4ull * (uint64_t)std::min<int64_t>(lq, (int64_t)s.len);
+    return true;
+}
+
+// ---- playbackRate / detune bound from device memory, a non-looping source whose declared rates are all positive: the slow track's
+// constants that do not depend on the rate, and the bound values (PATCH_RAW); k_buffer_source_slow<true> derives the rest per run
+bool Planner::absn_bound(NodeCtx& nc, const AbsnPlay& s, const PRef& pdet, const PRef& prate, int64_t q, bool aligned, double rate_hi) {
+    Node& n = nc.n;
+    const double sr = (double)g->sample_rate;
+    AbsnBoundInst r{};
+    AbsnSlowInst& a = r.s;
+    a.buf = s.buf;
+    a.buf_len = (int64_t)s.len;
+    a.buf_stride = (int64_t)s.stride;
+    a.ch = s.ch;
+    a.sample_rate = sr;
+    a.buffer_duration = s.duration;
+    a.pos_scale = ((double)s.pb->sample_rate / sr) * sr;
+    a.duration = n.duration;
+    a.loop_end = s.duration;
+    const AbsnStart st = absn_start(n);
+    a.n_first = st.n_first;
+    a.n_stop = st.n_stop;
+    r.dt = clock.dt;
+    r.offset = n.offset;
+    r.start_delta = st.t_first - st.start;
+    r.n_start = q * 128;
+    r.fast_end = absn_fast_end(r.n_start, s.duration);
+    r.fast_ok = aligned && (double)s.pb->sample_rate / sr == 1. && s.ls == 0. && s.le == s.duration && n.duration > 1e300 && n.stop_time > 1e300;
+    r.rate = prate.v;
+    r.detune = pdet.v;
+    // The one decision the range drives: a constant layout only when the source plays to the end of the render at every rate it allows.
+    // It ends first at the highest rate; a quantum of margin covers the device's exp2 rounding its last bit the other way.
+    const AbsnSlowDerived top = absn_slow_derive(clock.dt, rate_hi, n.offset, r.start_delta, s.duration, n.duration, false, s.duration, a.n_first,
+                                                 a.n_stop);
+    const int64_t margin = (pdet.bound >= 0 || pdet.v != 0.f) ? 128 : 0;
+    const bool fixed = a.n_first <= 0 && top.n_end >= glq + margin && !(r.fast_ok && r.fast_end < glq);
+    out_dynamic(nc, fixed ? Lay::fixed(s.ch) : Lay::gated(s.ch));  // (gated: the kernel writes the layout track)
+    a.out = nc.p.out_buf[0];
+    StageBuild& sb = stage(nc.L, S_ABSN_BOUND);
+    sb.absn_bound.push_back(r);
+    const PRef* refs[2] = {&pdet, &prate};
+    const size_t offs[2] = {offsetof(AbsnBoundInst, detune), offsetof(AbsnBoundInst, rate)};
+    for (int i = 0; i < 2; i++)
+        if (refs[i]->bound >= 0) {
+            PatchRec pr = patch(PATCH_RAW, 1);
+            operand(pr, 0, *refs[i], refs[i]->v);
+            add_patch(sb, pr, (uint32_t)offs[i]);
+        }
     algorithmic_bytes += (uint64_t)s.ch * 4ull * (uint64_t)std::min<int64_t>(lq, (int64_t)s.len);
     return true;
 }
@@ -2522,20 +2617,7 @@ bool Planner::absn_fast(NodeCtx& nc, const AbsnPlay& s, int64_t q, bool fused) {
     a.buf_offset = 0;
     a.ch = s.ch;
     a.loop = n.loop ? 1 : 0;
-    if (!n.loop) {
-        // the quantum after which the source has `ended`: the reference accumulates buffer_time += block_duration and stops
-        // once it reaches the buffer's duration (audio_buffer_source.rs:609,826-838) — replayed, not divided
-        const double block_duration = clock.dt * 128.;
-        const int64_t max_q = (lq - a.n_start) / 128 + 2;
-        int64_t played = 0;
-        double bt = 0.;
-        while (played < max_q) {
-            bt += block_duration;
-            played++;
-            if (bt >= s.duration) break;
-        }
-        a.n_stop = a.n_start + played * 128;
-    }
+    if (!n.loop) a.n_stop = absn_fast_end(a.n_start, s.duration);
     if (fused) {
         PendingChain pc = source_chain(CHAIN_SRC_ABSN, s.ch);
         pc.inst.absn = a;
@@ -4200,6 +4282,7 @@ static void prep_plan_group(wae_batch* b, wae_graph* const* graphs, int k, PrepS
                     st.n_b = (int)s.hrtf_sel.size(); st.d_b = up(b, s.hrtf_sel); break;
                 case S_PAN_DYN: st.n = (int)s.pan_dyn.size(); st.d_a = up(b, s.pan_dyn); break;
                 case S_ABSN_SERIAL: st.n = (int)s.absn_serial.size(); st.d_a = up(b, s.absn_serial); break;
+                case S_ABSN_BOUND: st.n = (int)s.absn_bound.size(); st.d_a = up(b, s.absn_bound); break;
                 case S_SHAPER_OS: st.n = (int)s.shaper_os.size(); st.d_a = up(b, s.shaper_os); break;
                 case S_ROUTE: st.n = (int)s.route.size(); st.d_a = up(b, s.route); break;
                 case S_DELAY_MONO:
@@ -4230,6 +4313,8 @@ static void prep_plan_group(wae_batch* b, wae_graph* const* graphs, int k, PrepS
                     case S_SPAN: rec_size = sizeof(SPanInst); rec2_size = sizeof(float2); break;
                     case S_COMP: rec_size = sizeof(CompInst); break;
                     case S_META: rec_size = sizeof(MetaInst); break;
+                    case S_ABSN_SERIAL: rec_size = sizeof(AbsnSerialInst); break;
+                    case S_ABSN_BOUND: rec_size = sizeof(AbsnBoundInst); break;
                 }
                 for (const PatchRec& pr : s.patches) {
                     ParamPatch p = pr.p;
@@ -4710,6 +4795,7 @@ static void launch_stage(wae_batch* b, Stage& st, ChunkInfo ci) {
         case S_HRTF: launch_hrtf((HrtfInst*)st.d_a, st.n, (HrtfSelInst*)st.d_b, st.n_b, st.max_ch, ci, s); break;
         case S_PAN_DYN: launch_panner_dyn((PanDynInst*)st.d_a, st.n, ci, s); break;
         case S_ABSN_SERIAL: launch_buffer_source_serial((AbsnSerialInst*)st.d_a, st.n, ci, s); break;
+        case S_ABSN_BOUND: launch_buffer_source_bound((AbsnBoundInst*)st.d_a, st.n, ci, s); break;
         case S_SHAPER_OS: launch_shaper_os((ShaperOsInst*)st.d_a, st.n, st.max_ch, ci, s); break;
         case S_ROUTE: launch_route((RouteInst*)st.d_a, st.n, ci, s); break;
         case S_DELAY: launch_delay_read((DelayInst*)st.d_a, st.n, ci, s); break;

@@ -196,58 +196,131 @@ DEVI bool almost_eq(double a, double b) {  // `almost` crate 0.2: absolute or re
     if (d <= tol) return true;
     return d <= fmax(fabs(a), fabs(b)) * tol;
 }
-__global__ void __launch_bounds__(256) k_buffer_source_slow(const AbsnSlowInst* __restrict__ insts, int n_inst, ChunkInfo ci) {
-    for (int ii = blockIdx.y; ii < n_inst; ii += gridDim.y) {
-        const AbsnSlowInst o = insts[ii];
-        const int n = blockIdx.x * blockDim.x + threadIdx.x;
-        if (n >= ci.nf) continue;
-        const int64_t na = ci.f0 + n;
-        bool play = na >= o.n_first && na < o.n_stop;
-        int64_t pfi = 0;
-        double k = 0.;
-        if (play) {
-            const double m = (double)(na - o.n_first);
-            double elapsed = fma(m, fabs(o.step), o.elapsed0);
-            if (almost_eq(elapsed, o.duration)) elapsed = o.duration;
-            if (elapsed >= o.duration) play = false;
-            // segment of the playhead schedule that contains this frame (binary search), then the linear playhead
-            int lo = 0, hi = o.n_seg - 1;
-            while (lo < hi) {
-                int mid = (lo + hi + 1) >> 1;
-                if (o.seg_n[mid] <= na) lo = mid;
-                else hi = mid - 1;
-            }
-            double bt = fma((double)(na - o.seg_n[lo]), o.step, o.seg_bt[lo]);
-            if (fabs(bt) < 1.4901161193847656e-8) bt = 0.;
-            if (play && bt >= 0. && bt < o.buffer_duration) {
-                double playhead = bt * o.pos_scale;
-                double fl = floor(playhead);
-                pfi = (int64_t)fl;
-                k = playhead - fl;
-                if (pfi >= o.buf_len) play = false;
-            } else {
-                play = false;
-            }
+// chunk frame n of a slow-track source
+DEVI void absn_slow_frame(const AbsnSlowInst& o, int n, const ChunkInfo& ci) {
+    const int64_t na = ci.f0 + n;
+    bool play = na >= o.n_first && na < o.n_stop;
+    int64_t pfi = 0;
+    double k = 0.;
+    if (play) {
+        const double m = (double)(na - o.n_first);
+        double elapsed = fma(m, fabs(o.step), o.elapsed0);
+        if (almost_eq(elapsed, o.duration)) elapsed = o.duration;
+        if (elapsed >= o.duration) play = false;
+        // segment of the playhead schedule that contains this frame (binary search), then the linear playhead
+        int lo = 0, hi = o.n_seg - 1;
+        while (lo < hi) {
+            int mid = (lo + hi + 1) >> 1;
+            if (o.seg_n[mid] <= na) lo = mid;
+            else hi = mid - 1;
         }
-        for (int c = 0; c < o.ch; c++) {
-            float v = 0.f;
-            if (play) {
-                const float* b = o.buf + (size_t)c * o.buf_stride;
-                double prev = (double)__ldg(b + pfi), next;
-                if (pfi + 1 < o.buf_len) {
-                    next = (double)__ldg(b + pfi + 1);
-                } else if (o.loop) {  // :788-800 (rate >= 0): first frame at / after the loop start
-                    double sp = o.loop_start * o.sample_rate;
-                    int64_t si = floor(sp) == sp ? (int64_t)sp : (int64_t)sp + 1;
-                    next = (double)__ldg(b + (si < o.buf_len ? si : o.buf_len - 1));
-                } else if (almost_eq(k, 1.) || pfi == 0) {
-                    next = 0.;
-                } else {
-                    next = 2. * prev - (double)__ldg(b + pfi - 1);  // extrapolate past the end (:815-819)
-                }
-                v = (float)fma(1. - k, prev, k * next);
+        double bt = fma((double)(na - o.seg_n[lo]), o.step, o.seg_bt[lo]);
+        if (fabs(bt) < 1.4901161193847656e-8) bt = 0.;
+        if (play && bt >= 0. && bt < o.buffer_duration) {
+            double playhead = bt * o.pos_scale;
+            double fl = floor(playhead);
+            pfi = (int64_t)fl;
+            k = playhead - fl;
+            if (pfi >= o.buf_len) play = false;
+        } else {
+            play = false;
+        }
+    }
+    for (int c = 0; c < o.ch; c++) {
+        float v = 0.f;
+        if (play) {
+            const float* b = o.buf + (size_t)c * o.buf_stride;
+            double prev = (double)__ldg(b + pfi), next;
+            if (pfi + 1 < o.buf_len) {
+                next = (double)__ldg(b + pfi + 1);
+            } else if (o.loop) {  // :788-800 (rate >= 0): first frame at / after the loop start
+                double sp = o.loop_start * o.sample_rate;
+                int64_t si = floor(sp) == sp ? (int64_t)sp : (int64_t)sp + 1;
+                next = (double)__ldg(b + (si < o.buf_len ? si : o.buf_len - 1));
+            } else if (almost_eq(k, 1.) || pfi == 0) {
+                next = 0.;
+            } else {
+                next = 2. * prev - (double)__ldg(b + pfi - 1);  // extrapolate past the end (:815-819)
             }
-            chan(o.out, c, ci)[n] = v;
+            v = (float)fma(1. - k, prev, k * next);
+        }
+        chan(o.out, c, ci)[n] = v;
+    }
+}
+
+// A source whose playback rate is bound from device memory, ABSN_BOUND_TILES tiles of 256 chunk frames from frame n0 (called by every
+// thread of the CTA).  Thread 0 derives the instance's constants from the bound rate with the planner's expressions: the fast track's 1:1
+// copy where the planner would have taken it (k_buffer_source), else the slow track over one playhead segment.  A gated output also gets
+// its layout track here, silent outside the frames that play, as k_meta's META_SOURCE writes it for a planned source.
+constexpr int ABSN_BOUND_TILES = 8;
+DEVI void absn_bound_tiles(const AbsnBoundInst& r, int n0, const ChunkInfo& ci) {
+    __shared__ AbsnSlowInst s_o;
+    __shared__ int64_t s_seg_n, s_first, s_end;
+    __shared__ double s_seg_bt;
+    __shared__ int s_fast;
+    __syncthreads();  // (the CTA's previous instance is done with them)
+    if (threadIdx.x == 0) {
+        AbsnSlowInst o = r.s;
+        const double computed_rate = (double)r.rate * exp2((double)r.detune / 1200.);
+        const AbsnSlowDerived d = absn_slow_derive(r.dt, computed_rate, r.offset, r.start_delta, o.buffer_duration, o.duration, false, o.loop_end,
+                                                   o.n_first, o.n_stop);
+        o.step = d.step;
+        o.offset0 = d.offset0;
+        o.elapsed0 = d.elapsed0;
+        o.n_seg = 1;
+        o.seg_n = &s_seg_n;
+        o.seg_bt = &s_seg_bt;
+        s_seg_n = o.n_first;
+        s_seg_bt = d.offset0;
+        const bool fast = r.fast_ok && computed_rate == 1.;
+        s_fast = fast;
+        s_first = fast ? r.n_start : o.n_first;
+        s_end = fast ? r.fast_end : d.n_end;
+        s_o = o;
+    }
+    __syncthreads();
+    const AbsnSlowInst o = s_o;
+    const bool fast = s_fast;
+    for (int t = 0; t < ABSN_BOUND_TILES; t++) {
+        const int n = n0 + t * 256 + (int)threadIdx.x;
+        if (n >= ci.nf) return;
+        const int64_t na = ci.f0 + n;
+        if (fast) {
+            for (int c = 0; c < o.ch; c++) {
+                float v = 0.f;
+                if (na >= r.n_start && na < r.fast_end && na - r.n_start < o.buf_len) v = __ldg(o.buf + (size_t)c * o.buf_stride + (na - r.n_start));
+                chan(o.out, c, ci)[n] = v;
+            }
+        } else {
+            absn_slow_frame(o, n, ci);
+        }
+        if (o.out.meta && (n & 127) == 0) {
+            const bool silent = s_end <= na || s_first >= na + 128;
+            meta_put_all(o.out, o.ch, meta_qi(ci, n), silent ? 1 : o.ch, silent);
+        }
+    }
+}
+
+// One thread per frame (BOUND: per frame of each of ABSN_BOUND_TILES tiles).  BOUND: the records are AbsnBoundInst (a playback rate
+// bound from device memory), else AbsnSlowInst.
+template <bool BOUND>
+struct AbsnSlowRecord {
+    using T = AbsnSlowInst;
+};
+template <>
+struct AbsnSlowRecord<true> {
+    using T = AbsnBoundInst;
+};
+template <bool BOUND>
+__global__ void __launch_bounds__(256) k_buffer_source_slow(const typename AbsnSlowRecord<BOUND>::T* __restrict__ insts, int n_inst, ChunkInfo ci) {
+    for (int ii = blockIdx.y; ii < n_inst; ii += gridDim.y) {
+        if constexpr (BOUND) {
+            absn_bound_tiles(insts[ii], blockIdx.x * ABSN_BOUND_TILES * 256, ci);
+        } else {
+            const int n = blockIdx.x * blockDim.x + threadIdx.x;
+            const AbsnSlowInst o = insts[ii];
+            if (n >= ci.nf) continue;
+            absn_slow_frame(o, n, ci);
         }
     }
 }
@@ -4741,7 +4814,10 @@ void launch_oscillator(const OscInst* d, int n, ChunkInfo ci, cudaStream_t s) { 
 void launch_constant(const ConstInst* d, int n, ChunkInfo ci, cudaStream_t s) { k_constant<<<grid_tiles(ci.nf, 1024, n), 256, 0, s>>>(d, n, ci); }
 void launch_buffer_source(const AbsnInst* d, int n, ChunkInfo ci, cudaStream_t s) { k_buffer_source<<<grid_tiles(ci.nf, 1024, n), 256, 0, s>>>(d, n, ci); }
 void launch_buffer_source_slow(const AbsnSlowInst* d, int n, ChunkInfo ci, cudaStream_t s) {
-    k_buffer_source_slow<<<grid_tiles(ci.nf, 256, n), 256, 0, s>>>(d, n, ci);
+    k_buffer_source_slow<false><<<grid_tiles(ci.nf, 256, n), 256, 0, s>>>(d, n, ci);
+}
+void launch_buffer_source_bound(const AbsnBoundInst* d, int n, ChunkInfo ci, cudaStream_t s) {
+    k_buffer_source_slow<true><<<grid_tiles(ci.nf, 256 * ABSN_BOUND_TILES, n), 256, 0, s>>>(d, n, ci);
 }
 void launch_mix(const MixInst* d, const MixEdge* e, int n, ChunkInfo ci, cudaStream_t s, int max_edges) {
     // few instances x few frames (one graph with a huge fan-in): one frame per thread keeps more loads in flight

@@ -62,12 +62,46 @@ WAE_HD void make_scan_coef(double b1, double b2, double a1, double a2, ScanCoef&
     for (int i = 0; i < 16; i++) sc.GL[i] = g[i];
 }
 
+// The rate-dependent constants of a slow-track source (audio_buffer_source.rs:660-678,826-838), in f64: one source for the planner
+// (host, absn_slow) and for k_buffer_source_slow<true> (device, rates bound from device memory).  `delta`: t_first - start; `n_stop`: the
+// stop frame; `duration`: the explicit duration (>= 1e300: none).  n_end is the frame after the last one the source can play.
+struct AbsnSlowDerived {
+    double step, offset0, elapsed0;
+    int64_t n_end;
+};
+WAE_HD AbsnSlowDerived absn_slow_derive(double dt, double computed_rate, double offset, double delta, double buffer_duration, double duration,
+                                        bool loop, double loop_end, int64_t n_first, int64_t n_stop) {
+    auto mx = [](double a, double b) { return a < b ? b : a; };  // std::max / std::min, -0. and all
+    auto mn = [](double a, double b) { return b < a ? b : a; };
+    AbsnSlowDerived d;
+    d.step = dt * computed_rate;
+    double off = offset + delta * computed_rate;  // :672-674
+    off = mn(mx(off, 0.), buffer_duration);
+    if (loop && off > loop_end) off = loop_end;  // :676-678 (rate >= 0)
+    d.offset0 = off;
+    d.elapsed0 = fabs(delta * computed_rate);
+    // the source has ended after the stop frame, the explicit duration, or (not looping) the end of the buffer
+    d.n_end = n_stop;
+    if (d.step > 0.) {
+        if (!loop) {
+            const int64_t e = n_first + (int64_t)ceil(mx(0., buffer_duration - off) / d.step);
+            d.n_end = e < d.n_end ? e : d.n_end;
+        }
+        if (duration < 1e300) {
+            const int64_t e = n_first + (int64_t)ceil(mx(0., duration - d.elapsed0) / d.step);
+            d.n_end = e < d.n_end ? e : d.n_end;
+        }
+    }
+    return d;
+}
+
 void upload_twiddles();                          // convolver FFT tables (computed in wae_kernels.cu, f64 -> f32)
 void conv_fft_selftest(float* data, int mode);   // host emulation of the convolver transforms (wae_selftest_conv_fft)
 void launch_oscillator(const OscInst* d, int n, ChunkInfo ci, cudaStream_t s);
 void launch_constant(const ConstInst* d, int n, ChunkInfo ci, cudaStream_t s);
 void launch_buffer_source(const AbsnInst* d, int n, ChunkInfo ci, cudaStream_t s);
 void launch_buffer_source_slow(const AbsnSlowInst* d, int n, ChunkInfo ci, cudaStream_t s);
+void launch_buffer_source_bound(const AbsnBoundInst* d, int n, ChunkInfo ci, cudaStream_t s);  // k_buffer_source_slow<true>
 void launch_mix(const MixInst* d, const MixEdge* e, int n, ChunkInfo ci, cudaStream_t s, int max_edges);  // max_edges: widest port of the stage (host)
 void launch_mix_dyn(const MixDynInst* d, const MixEdge* e, int n, ChunkInfo ci, cudaStream_t s);
 void launch_meta(const MetaInst* d, int n, ChunkInfo ci, cudaStream_t s);
