@@ -674,6 +674,39 @@ typedef struct wae_iir_binding {
  * bound. */
 WAE_API wae_status wae_batch_bind_iir_coefficients(wae_batch* batch, const wae_iir_binding* items, uint32_t n, void* stream);
 
+/* ---- AudioParam value curves bound from device memory -----------------------------------------------------------------------
+ * Declares one SetValueCurveAtTime event of `length` values at [start_time, start_time + duration) whose values are supplied per run
+ * from device memory (wae_batch_bind_value_curves), so that one prepared batch renders any number of envelopes, filter sweeps, pitch
+ * contours, pan trajectories or delay-time modulations without being built and planned again.  It works on every param
+ * wae_param_event_push accepts, including the ones wae_param_set_device_value refuses (OscillatorNode frequency / detune, DelayNode
+ * delayTime, PannerNode positions, ConstantSourceNode offset): no planning decision reads the values of an automated param.  The event is
+ * pushed in arrival order exactly as wae_param_event_push pushes a host curve, so folding, sorting, cancel handling and overlap errors
+ * (WAE_NOT_SUPPORTED at plan time) are the host's, and a bound curve renders bit for bit what the same values given to
+ * wae_param_event_push render.  The values are used as they are, NaN and infinities included (the reference checks only the length,
+ * start time and duration).  An audio-rate input (wae_connect_param) stays allowed.
+ * WAE_INVALID_ARGUMENT: an unknown node or param (AudioListener params included), an invalid start time, a duration that is not > 0.
+ * WAE_INVALID_STATE: length < 2, a param bound with wae_param_set_device_value, a second declaration on the param, or a graph that
+ * already has a suspend point.  After the declaration the param takes no further events (also from a suspend callback: WAE_INVALID_STATE);
+ * suspend points added later are allowed.  wae_render_batch and wae_render_many answer WAE_INVALID_STATE on graphs with declarations;
+ * wae_batch_plan plans them. */
+WAE_API wae_status wae_param_set_device_value_curve(wae_graph* graph, wae_node_id node, uint32_t param_index, uint32_t length,
+                                                    double start_time, double duration);
+
+typedef struct wae_value_curve_binding {
+    uint32_t graph_index;  /* caller's index, as wae_batch_fetch_graph */
+    wae_node_id node;      /* the param's node */
+    uint32_t param_index;  /* declared with wae_param_set_device_value_curve */
+    const float* values;   /* device memory of the engine's GPU: the declared `length` floats, 4-byte aligned */
+} wae_value_curve_binding;
+
+/* Copies the values into the batch, asynchronously on the engine stream after the work already queued on `stream` (as
+ * wae_batch_bind_sources).  All-or-nothing: every item is validated before anything is enqueued.  A bound curve stays until it is bound
+ * again.  WAE_INVALID_ARGUMENT: `values` is null, not 4-byte aligned or not device (or managed) memory of the engine's GPU,
+ * [values, values + length) does not lie in one allocation, or one param is named twice in the call.  WAE_INVALID_STATE: graph_index
+ * out of range, or the param has no declaration.  wae_batch_run, wae_batch_run_group and wae_batch_run_pipelined answer
+ * WAE_INVALID_STATE while a declared curve of the batch has never been bound (a declared param the batch never renders needs no bind). */
+WAE_API wae_status wae_batch_bind_value_curves(wae_batch* batch, const wae_value_curve_binding* items, uint32_t n, void* stream);
+
 /* PeriodicWave::new(context, PeriodicWaveOptions { real, imag, disable_normalization }) (src/periodic_wave.rs:104-209): fills `table`
  * (PERIODIC_WAVE_TABLE_LENGTH = 8192 in the reference) with the wavetable an OscillatorNode of type Custom plays.  `real` / `imag` may be
  * NULL (= zeros); both NULL = the sine default.  Host math, no engine needed. */

@@ -149,6 +149,11 @@ class IirBinding(C.Structure):
     _fields_ = [("graph_index", C.c_uint32), ("node", C.c_uint32), ("feedforward", c_double_p), ("feedback", c_double_p)]
 
 
+class ValueCurveBinding(C.Structure):
+    """wae_value_curve_binding: the device values of one declared SetValueCurveAtTime of a prepared batch (wae_batch_bind_value_curves)."""
+    _fields_ = [("graph_index", C.c_uint32), ("node", C.c_uint32), ("param_index", C.c_uint32), ("values", c_float_p)]
+
+
 STATUS_NAMES = {0: "OK", 1: "INVALID_ARGUMENT", 2: "INVALID_STATE", 3: "NOT_SUPPORTED", 4: "UNSUPPORTED",
                 5: "CUDA_ERROR", 6: "OUT_OF_MEMORY", 7: "NO_DEVICE"}
 
@@ -193,6 +198,7 @@ WAE_SYMBOLS = [
     "wae_wave_shaper_set_device_curve", "wae_batch_bind_curves",
     "wae_oscillator_set_device_periodic_wave", "wae_batch_bind_periodic_waves",
     "wae_iir_filter_set_device_coefficients", "wae_batch_bind_iir_coefficients",
+    "wae_param_set_device_value_curve", "wae_batch_bind_value_curves",
 ]
 
 
@@ -311,6 +317,9 @@ class Api:
             # IIR coefficients bound from device memory
             f("iir_filter_set_device_coefficients", C.c_int32, [gp, C.c_uint32])
             f("batch_bind_iir_coefficients", C.c_int32, [C.c_void_p, C.POINTER(IirBinding), C.c_uint32, C.c_void_p])
+            # AudioParam value curves bound from device memory
+            f("param_set_device_value_curve", C.c_int32, [gp, C.c_uint32, C.c_uint32, C.c_uint32, C.c_double, C.c_double])
+            f("batch_bind_value_curves", C.c_int32, [C.c_void_p, C.POINTER(ValueCurveBinding), C.c_uint32, C.c_void_p])
         else:
             f("graph_create", C.c_int32, [C.c_uint32, C.c_uint64, C.c_float, C.POINTER(C.c_void_p)])
             f("render", C.c_int32, [gp, c_float_p])

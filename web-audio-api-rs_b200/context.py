@@ -157,6 +157,18 @@ class AudioParam:
         api.check(api.param_set_device_value(self._ctx._g, self._node, self._index, lo, hi))
         return self
 
+    def set_device_value_curve(self, length, start_time, duration):
+        """wae_param_set_device_value_curve (product only): one setValueCurveAtTime of `length` values at [start_time, start_time +
+        duration) whose values Batch.bind_value_curves supplies from device memory before each run.  The param takes no further events."""
+        api = self._ctx._api
+        if not api.is_product:
+            raise B.WaeError(3, "value curves bound from device memory are a feature of the GPU engine")
+        if self._node == "listener":
+            raise B.WaeError(1, "AudioListener params cannot be bound from device memory")
+        api.check(api.param_set_device_value_curve(self._ctx._g, self._node, self._index, int(length), float(start_time), float(duration)))
+        self._ctx._device_value_curves[(int(self._node), int(self._index))] = int(length)
+        return self
+
     def set_automation_rate(self, rate):
         api = self._ctx._api
         api.check(api.param_set_automation_rate(self._ctx._g, self._node, self._index, 0 if rate in ("a", "A", 0) else 1))
@@ -501,6 +513,7 @@ class OfflineAudioContext:
         self._device_curves = {}  # node id -> length declared with set_device_curve
         self._device_waves = {}  # node id -> coefficient count declared with set_device_periodic_wave
         self._device_iirs = {}  # node id -> (feedforward count, feedback count) declared with set_device_coefficients
+        self._device_value_curves = {}  # (node id, param index) -> length declared with set_device_value_curve
 
     def __del__(self):
         try:
@@ -912,6 +925,47 @@ class Batch:
         self.api.check(self.api.batch_bind_iir_coefficients(self.handle, items, n, C.c_void_p(self._torch_stream_handle())))
         self._keep_until_read(feedforward)
         self._keep_until_read(feedback)
+
+    def bind_value_curves(self, params, values, graphs=None):
+        """wae_batch_bind_value_curves: values[j][i] (a float32 CUDA tensor [n][length] per param, unit stride on the last dimension)
+        becomes the curve of params[j] (declared with set_device_value_curve) in context graphs[i] (default: 0..n-1).  `params`: one
+        AudioParam or a list; a param of a context built like the others shares its node id and index, so the params of context 0 name
+        those of every context.  `values`: one tensor, or a list of tensors, one per param.  One call, ordered after torch's current
+        stream; the values are copied on the engine stream, and the tensors' memory is kept from reuse until they have been."""
+        import torch
+        params = list(params) if isinstance(params, (list, tuple)) else [params]
+        tensors = list(values) if isinstance(values, (list, tuple)) else [values]
+        if len(tensors) != len(params):
+            raise B.WaeError(1, f"bind_value_curves: {len(tensors)} tensors for {len(params)} params")
+        for t in tensors:
+            if not (isinstance(t, torch.Tensor) and t.is_cuda and t.dtype == torch.float32 and t.dim() == 2):
+                raise B.WaeError(1, "bind_value_curves: values must be float32 CUDA tensors [n][length]")
+        n = tensors[0].shape[0] if tensors else 0
+        if any(t.shape[0] != n for t in tensors):
+            raise B.WaeError(1, "bind_value_curves: the tensors differ in their number of rows")
+        graphs = list(range(n)) if graphs is None else [int(g) for g in graphs]
+        if len(graphs) != n:
+            raise B.WaeError(1, f"bind_value_curves: {n} rows for {len(graphs)} graphs")
+        if n and any(t.stride(1) != 1 for t in tensors):
+            raise B.WaeError(1, "bind_value_curves: the values of a curve must be contiguous (unit stride on the last dimension)")
+        items = (B.ValueCurveBinding * max(n * len(params), 1))()
+        for j, (prm, t) in enumerate(zip(params, tensors)):
+            if prm._node == "listener":
+                raise B.WaeError(2, "bind_value_curves: AudioListener params are not bound from device memory")
+            key = (int(prm._node), int(prm._index))
+            for i, g in enumerate(graphs):
+                if not 0 <= g < self.n:
+                    raise B.WaeError(2, f"bind_value_curves: graph index {g} is out of range")
+                declared = self.contexts[g]._device_value_curves.get(key)
+                # (the tensor's own shape: the library checks only the CUDA allocation, which may hold several tensors)
+                if declared is not None and t.shape[1] != declared:
+                    raise B.WaeError(1, f"bind_value_curves: values[{j}] has {t.shape[1]} points, param {key[1]} of node {key[0]} of "
+                                        f"graph {g} was declared with {declared}")
+                ptr = C.cast(C.c_void_p(t.data_ptr() + 4 * i * t.stride(0)), B.c_float_p)
+                items[j * n + i] = B.ValueCurveBinding(g, key[0], key[1], ptr)
+        self.api.check(self.api.batch_bind_value_curves(self.handle, items, n * len(params), C.c_void_p(self._torch_stream_handle())))
+        for t in tensors:
+            self._keep_until_read(t)
 
     def _graphs_and_nodes(self, fn, nodes, graphs, n):
         """The graph index and node id of each of n binding items: `graphs` (default 0..n-1), `nodes` one node (or id) for all graphs or

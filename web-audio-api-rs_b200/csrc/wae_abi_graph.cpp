@@ -708,6 +708,9 @@ static wae_status push_event(Param& p, const wae_param_event* e) {
     if (p.device_bound)
         return fail(WAE_INVALID_STATE, "InvalidStateError - the param's value is bound from device memory (wae_param_set_device_value): "
                                        "it takes no events");
+    if (p.device_curve)
+        return fail(WAE_INVALID_STATE, "InvalidStateError - the param's value curve is bound from device memory "
+                                       "(wae_param_set_device_value_curve): it takes no further events");
     auto finite = [](float v) { return std::isfinite(v); };
     auto valid_time = [](double t) { return std::isfinite(t) && t >= 0.; };
     ParamEv ev{(int)e->type, e->value, e->time, e->aux, {}};
@@ -883,6 +886,34 @@ WAE_API wae_status wae_param_event_push(wae_graph* g, wae_node_id node, uint32_t
     auto ni = g->nodes.find(node);
     if (ni == g->nodes.end() || param_index >= ni->second.params.size()) return fail(WAE_INVALID_ARGUMENT, "unknown param");
     return push_event(g->nodes.at(ni->second.params[param_index]).param, e);
+}
+
+// One SetValueCurveAtTime event of `length` values that wae_batch_bind_value_curves supplies per run, pushed in arrival order as
+// wae_param_event_push pushes a host curve (with zero placeholders for the values): folding, sorting and overlap errors are the host's.
+// The param takes no further events, so no planning decision ever reads the values.
+WAE_API wae_status wae_param_set_device_value_curve(wae_graph* g, wae_node_id node, uint32_t param_index, uint32_t length,
+                                                    double start_time, double duration) {
+    if (!g) return fail(WAE_INVALID_ARGUMENT, "null graph");
+    Node* n = g->nodes.get(node);
+    if (!n || n->kind == K_PARAM || param_index >= n->params.size()) return fail(WAE_INVALID_ARGUMENT, "unknown param");
+    if (n->kind == K_LISTENER) return fail(WAE_INVALID_ARGUMENT, "AudioListener params are not bound from device memory");
+    if (length < 2) return fail(WAE_INVALID_STATE, "InvalidStateError - sequence length should not be less than 2");
+    if (!(std::isfinite(start_time) && start_time >= 0.)) return fail(WAE_INVALID_ARGUMENT, "RangeError - time should be positive");
+    if (!(std::isfinite(duration) && duration > 0.)) return fail(WAE_INVALID_ARGUMENT, "RangeError - duration should be strictly positive");
+    Param& p = g->nodes.at(n->params[param_index]).param;
+    if (p.device_bound)
+        return fail(WAE_INVALID_STATE, "InvalidStateError - the param's value is bound from device memory (wae_param_set_device_value)");
+    if (p.device_curve)
+        return fail(WAE_INVALID_STATE, "InvalidStateError - the param's value curve is already bound from device memory "
+                                       "(wae_param_set_device_value_curve)");
+    if (!g->epochs.empty())  // (the segments before the suspend point were planned with the events of their own graph copy)
+        return fail(WAE_INVALID_STATE, "InvalidStateError - a value curve is bound from device memory before the first suspend point");
+    p.events.push_back(ParamEv{WAE_EVENT_SET_VALUE_CURVE_AT_TIME, 0.f, start_time, duration, std::vector<float>(length, 0.f)});
+    p.device_curve = length;
+    p.device_curve_node = node;
+    p.device_curve_index = param_index;
+    g->device_value_curves++;
+    return WAE_OK;
 }
 
 WAE_API wae_status wae_listener_param_event_push(wae_graph* g, uint32_t param_index, const wae_param_event* e) {

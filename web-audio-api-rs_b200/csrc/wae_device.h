@@ -595,6 +595,14 @@ struct IirBindItem {
     int32_t pad;
 };
 
+// ---- wae_batch_bind_value_curves: caller values -> the SetValueCurveAtTime values of a declared param (ParamInst::curves + values_off)
+struct ValueCurveBindItem {
+    const float* src;  // caller's values (4 B aligned)
+    float* dst;        // in the param's curve pool
+    int32_t n;         // the declared length
+    int32_t pad;
+};
+
 // ---- wae_batch_bind_params: per-run values of params planned as constants ------------------------------------------------------
 struct ParamBindItem {  // one float of the caller's device memory -> value slot `slot`
     const float* src;

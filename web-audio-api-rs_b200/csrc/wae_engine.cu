@@ -528,6 +528,24 @@ struct wae_batch {
     std::map<std::pair<uint32_t, wae_node_id>, size_t> iir_index;  // (batch position, node) -> iirs
     size_t iirs_unbound = 0;
     IirPatch* d_iir_patches = nullptr;
+    // wae_param_set_device_value_curve: the curve pool of each declared param (ParamInst::curves: made by the planner, zeroed, the param's
+    // host curves copied in once, never in the upload slabs) and where the declared values lie in it, rewritten by
+    // wae_batch_bind_value_curves.  A declared param the planner never lowered has no pool: binding it is validated and writes nothing,
+    // and runs do not wait for it.
+    struct DevValueCurve {
+        uint32_t graph;  // batch position
+        uint32_t pid;    // the param's node id
+        wae_node_id node;
+        uint32_t param_index;
+        float* pool;
+        int32_t values_off;
+        uint32_t length;
+        bool bound;
+    };
+    std::vector<DevValueCurve> value_curves;
+    std::map<std::pair<uint32_t, uint32_t>, size_t> value_curve_pool;  // (batch position, param id) -> value_curves, while planning
+    std::map<std::tuple<uint32_t, wae_node_id, uint32_t>, size_t> value_curve_index;  // (batch position, node, param index) -> value_curves
+    size_t value_curves_unbound = 0;
     cudaEvent_t ev_bind = nullptr;  // orders a bind after the caller's stream
     // OfflineAudioContext::suspend_sync: a group's render is cut at the suspend frames of its graphs (graphs with different
     // suspend points are put in different groups); every segment has its own plan, node state is shared between the plans
@@ -1170,6 +1188,7 @@ struct Planner {
     bool device_response_spectra(const Node& n, int S, IrSpectra& spec);
     const float* device_curve(const Node& n);
     float* device_wave(const Node& n);
+    float* device_value_curve(uint32_t pid, const Param& prm, const ParamTimeline& tl);
     // a patch entry of the declared curve of node `n` for the int32 field `off` bytes into the last record of stage `s`
     void add_curve_patch(StageBuild& s, const Node& n, uint32_t off, int32_t keeps, int32_t other) {
         s.curve_patches.push_back(StageBuild::CurvePatchRec{gi, n.id, (int32_t)s.records() - 1, off, keeps, other});
@@ -1789,6 +1808,28 @@ float* Planner::device_wave(const Node& n) {
     return d;
 }
 
+// The curve pool of a param with a value curve bound from device memory: one zeroed allocation per (batch graph, param), outside the
+// upload slabs (nothing but wae_batch_bind_value_curves writes the declared values), shared by every suspend segment.  The declared event
+// is the param's last, so its values are the last `device_curve` of the pool; the param's other curves are copied in once.  The sizing
+// pass gets the placeholder an uploaded pool gets, so that plan digests stay comparable.
+float* Planner::device_value_curve(uint32_t pid, const Param& prm, const ParamTimeline& tl) {
+    if (dry) return reinterpret_cast<float*>(uintptr_t(256));
+    std::lock_guard<std::recursive_mutex> lk(b->mu);
+    auto it = b->value_curve_pool.find({gi, pid});
+    if (it != b->value_curve_pool.end()) return b->value_curves[it->second].pool;
+    const size_t host_part = tl.curves.size() - prm.device_curve;
+    float* d = b->dalloc<float>((tl.curves.size() + 3) / 4 * 4, true);
+    if (!d || (host_part && cudaMemcpyAsync(d, tl.curves.data(), host_part * sizeof(float), cudaMemcpyHostToDevice, b->engine->stream) !=
+                                cudaSuccess)) {
+        bail(WAE_OUT_OF_MEMORY, "out of device memory (value curve)");
+        return nullptr;
+    }
+    b->asset_bytes += (tl.curves.size() + 3) / 4 * 16;
+    b->value_curve_pool[{gi, pid}] = b->value_curves.size();
+    b->value_curves.push_back(wae_batch::DevValueCurve{gi, pid, 0, 0, d, (int32_t)host_part, prm.device_curve, false});
+    return d;
+}
+
 // the second convolver of a mono response behind an input that switches between one and two channels: input R -> output 1, fed the
 // two-channel quanta only (ConvCmpInst)
 bool Planner::conv_compact_path(PNode& pn, int level, int in_ch, const IrSpectra& spec, int Smax, int blocks_per_chunk) {
@@ -1946,7 +1987,12 @@ bool Planner::lower_param(uint32_t id, Node& n, PNode& p) {
         if (!mix(2 * level, edges, 1, first_channel, false, any_dyn, false, pi.in)) return false;
     }
     pi.events = tl.events.empty() ? nullptr : upload(tl.events);
-    pi.curves = tl.curves.empty() ? nullptr : upload(tl.curves);
+    // (a value curve bound from device memory: the pool of its own the bind writes into)
+    if (n.param.device_curve) {
+        if (!(pi.curves = device_value_curve(id, n.param, tl))) return false;
+    } else {
+        pi.curves = tl.curves.empty() ? nullptr : upload(tl.curves);
+    }
     pi.state = alloc<ParamState>(1, true, true);
     pi.out = arena_buf(2);  // channel 0: value per frame, channel 1: single-valued flag per quantum
     if (!pi.state || !pi.out.p) return bail(WAE_OUT_OF_MEMORY, "out of device memory (param)");
@@ -4518,9 +4564,53 @@ static wae_status record_iirs(wae_batch* b, wae_graph* const* graphs, uint32_t n
     return WAE_OK;
 }
 
-// runs of a batch need every device input, param, response, curve, periodic wave and IIR coefficient set bound once
+// The declared value curves of the batch (`graphs` in batch order), after planning: each named by the (node, param index) it was declared
+// through, the ones the planner gave a pool unbound, in graph, node and param order; then the declared ones it never lowered, which
+// binding validates and writes nothing to, and which runs do not wait for.
+static void record_value_curves(wae_batch* b, wae_graph* const* graphs, uint32_t n_graphs) {
+    std::vector<wae_batch::DevValueCurve> never;
+    for (uint32_t j = 0; j < n_graphs; j++) {
+        if (!graphs[j]->device_value_curves) continue;
+        auto scan = [&](const NodeMap& nodes) {
+            for (const auto& kv : nodes) {
+                const Node& nd = kv.second;
+                if (nd.kind != K_PARAM || !nd.param.device_curve) continue;
+                auto pi = b->value_curve_pool.find({j, nd.id});
+                if (pi != b->value_curve_pool.end()) {
+                    b->value_curves[pi->second].node = nd.param.device_curve_node;
+                    b->value_curves[pi->second].param_index = nd.param.device_curve_index;
+                } else if (std::none_of(never.begin(), never.end(), [&](const wae_batch::DevValueCurve& d) { return d.graph == j && d.pid == nd.id; })) {
+                    never.push_back(wae_batch::DevValueCurve{j, nd.id, nd.param.device_curve_node, nd.param.device_curve_index, nullptr, 0,
+                                                             nd.param.device_curve, true});
+                }
+            }
+        };
+        scan(graphs[j]->nodes);
+        for (const auto& ep : graphs[j]->epochs) scan(ep.nodes);
+    }
+    auto by_name = [](const wae_batch::DevValueCurve& x, const wae_batch::DevValueCurve& y) {
+        return std::tie(x.graph, x.node, x.param_index) < std::tie(y.graph, y.node, y.param_index);
+    };
+    std::sort(b->value_curves.begin(), b->value_curves.end(), by_name);
+    b->value_curves_unbound = b->value_curves.size();
+    b->value_curves.insert(b->value_curves.end(), never.begin(), never.end());
+    b->value_curve_pool.clear();
+    for (size_t k = 0; k < b->value_curves.size(); k++) {
+        const auto& d = b->value_curves[k];
+        b->value_curve_index[{d.graph, d.node, d.param_index}] = k;
+    }
+}
+
+// runs of a batch need every device input, param, response, curve, periodic wave, IIR coefficient set and value curve bound once
 static wae_status check_bound(wae_batch* b) {
     if (!b) return fail(WAE_INVALID_ARGUMENT, "null batch");
+    for (size_t k = 0; b->value_curves_unbound && k < b->value_curves.size(); k++)
+        if (const auto& d = b->value_curves[k]; !d.bound) {
+            const uint32_t caller = b->order.empty() ? d.graph : b->order[d.graph];
+            return fail(WAE_INVALID_STATE, "value curve bound from device memory never bound: graph " + std::to_string(caller) + ", node " +
+                                               std::to_string(d.node) + ", param " + std::to_string(d.param_index) +
+                                               " (wae_batch_bind_value_curves)");
+        }
     for (size_t k = 0; b->iirs_unbound && k < b->iirs.size(); k++)
         if (const auto& d = b->iirs[k]; !d.bound) {
             const uint32_t caller = b->order.empty() ? d.graph : b->order[d.graph];
@@ -4663,6 +4753,7 @@ static wae_status prepare_impl(wae_engine* eng, wae_graph* const* graphs, uint32
     }
     record_responses(b, graphs, n_graphs);
     record_waves(b, graphs, n_graphs);
+    record_value_curves(b, graphs, n_graphs);
     std::vector<CurvePatch> curve_patches;
     std::vector<IirPatch> iir_patches;
     std::vector<ParamSlotInfo> slot_info;
@@ -5440,6 +5531,55 @@ WAE_API wae_status wae_batch_bind_iir_coefficients(wae_batch* b, const wae_iir_b
     return WAE_OK;
 }
 
+// The declared values are rewritten on the engine stream: runs queued before the bind have read the previous ones.
+WAE_API wae_status wae_batch_bind_value_curves(wae_batch* b, const wae_value_curve_binding* items, uint32_t n, void* stream) {
+    if (!b || (n && !items)) return fail(WAE_INVALID_ARGUMENT, "null batch / items");
+    if (n == 0) return WAE_OK;
+    CUDA_TRY(cudaSetDevice(b->engine->device));
+    // every item is validated before anything is enqueued
+    std::vector<ValueCurveBindItem> table;
+    std::vector<size_t> curve_of;
+    std::vector<char> named(b->value_curves.size(), 0);
+    BindExtents extents{b->engine->device, {}};
+    int64_t max_len = 0;
+    for (uint32_t i = 0; i < n; i++) {
+        const wae_value_curve_binding& it = items[i];
+        if (it.graph_index >= b->n_graphs)
+            return fail(WAE_INVALID_STATE, "bind: graph index " + std::to_string(it.graph_index) + " is out of range");
+        auto ci = b->value_curve_index.find(std::make_tuple(b->batch_pos(it.graph_index), it.node, it.param_index));
+        const std::string name = "param " + std::to_string(it.param_index) + " of node " + std::to_string(it.node) + " of graph " +
+                                 std::to_string(it.graph_index);
+        if (ci == b->value_curve_index.end())
+            return fail(WAE_INVALID_STATE, "bind: " + name + " has no value curve bound from device memory (wae_param_set_device_value_curve)");
+        const size_t k = ci->second;
+        if (named[k]++)  // (two items of one launch writing one curve: which one lands would be undefined)
+            return fail(WAE_INVALID_ARGUMENT, "bind: " + name + " is named twice in one call");
+        const wae_batch::DevValueCurve& d = b->value_curves[k];
+        if (!it.values) return fail(WAE_INVALID_ARGUMENT, "bind: null values");
+        if ((uintptr_t)it.values % alignof(float)) return fail(WAE_INVALID_ARGUMENT, "bind: values is not 4-byte aligned");
+        wae_status st = extents.check(it.values, (uint64_t)d.length * sizeof(float), "values",
+                                      "[values, values + length) runs past the end of its allocation");
+        if (st != WAE_OK) return st;
+        if (!d.pool) continue;  // declared, never rendered: nothing to write
+        table.push_back(ValueCurveBindItem{it.values, d.pool + d.values_off, (int32_t)d.length, 0});
+        max_len = std::max<int64_t>(max_len, d.length);
+        curve_of.push_back(k);
+    }
+    if (table.empty()) return WAE_OK;
+    wae_status st = bind_after(b, stream);
+    if (st == WAE_OK) st = stage_bind_table(b, table.data(), table.size() * sizeof(ValueCurveBindItem));
+    if (st != WAE_OK) return st;
+    launch_bind_value_curves(static_cast<const ValueCurveBindItem*>(b->d_bind), (int)table.size(), max_len, b->engine->stream);
+    cudaError_t le = cudaGetLastError();
+    if (le != cudaSuccess) return fail(WAE_CUDA_ERROR, std::string("bind: ") + cudaGetErrorString(le));
+    for (size_t k : curve_of)
+        if (!b->value_curves[k].bound) {
+            b->value_curves[k].bound = true;
+            b->value_curves_unbound--;
+        }
+    return WAE_OK;
+}
+
 WAE_API wae_status wae_batch_sync(wae_batch* b) {
     CUDA_TRY(cudaSetDevice(b->engine->device));
     CUDA_TRY(cudaStreamSynchronize(b->engine->stream));
@@ -5909,6 +6049,9 @@ static wae_status refuse_device_inputs(wae_graph* const* graphs, uint32_t n_grap
         if (graphs[i] && graphs[i]->device_iirs)
             return fail(WAE_INVALID_STATE, "graph " + std::to_string(i) + " has IIR coefficients bound from device memory: render it with "
                                            "wae_batch_prepare (or _prepare_many), wae_batch_bind_iir_coefficients and wae_batch_run");
+        if (graphs[i] && graphs[i]->device_value_curves)
+            return fail(WAE_INVALID_STATE, "graph " + std::to_string(i) + " has value curves bound from device memory: render it with "
+                                           "wae_batch_prepare (or _prepare_many), wae_batch_bind_value_curves and wae_batch_run");
     }
     return WAE_OK;
 }

@@ -100,6 +100,11 @@ struct Param {  // AudioParam: its own graph node in the reference (src/context/
     // [device_lo, device_hi] (the declared range intersected with [min_value, max_value]); planned as constant_value()
     bool device_bound = false;
     float device_lo = 0.f, device_hi = 0.f;
+    // wae_param_set_device_value_curve: the length of the SetValueCurveAtTime event whose values are written per run by
+    // wae_batch_bind_value_curves.  That event is the last of `events` (its `values` are zero placeholders): the param takes no further
+    // events, so the planner never replays its timeline on the host.  0: not declared
+    uint32_t device_curve = 0;
+    uint32_t device_curve_node = 0, device_curve_index = 0;  // the (node, param index) it was declared through: its name in binds
     // lowering helpers
     bool constant() const;        // only SetValue events: value is constant over the render
     float constant_value() const; // clamped like AudioParamProcessor::mix_to_output (src/param.rs:755-760)
@@ -269,6 +274,7 @@ struct wae_graph {
     uint32_t device_curves = 0;     // WaveShaperNodes declared with wae_wave_shaper_set_device_curve
     uint32_t device_waves = 0;      // OscillatorNodes declared with wae_oscillator_set_device_periodic_wave
     uint32_t device_iirs = 0;       // IIRFilterNodes declared with wae_iir_filter_set_device_coefficients
+    uint32_t device_value_curves = 0;  // AudioParams declared with wae_param_set_device_value_curve
 
     uint32_t create_param(uint32_t owner, float def, float mn, float mx, bool a_rate, float initial, bool send_set_value = true,
                           bool fixed_id = false, uint32_t id = 0, bool constrained = false);

@@ -4567,6 +4567,29 @@ __global__ void __launch_bounds__(32) k_bind_iir(const IirBindItem* __restrict__
     }
 }
 
+// ---- wae_batch_bind_value_curves: tiles of VC_TILE values (x) of each item (y), both grid-stride --------------------------------------
+// The values are moved as 32-bit words, so they land bit for bit (NaN payloads included); nothing but k_param* reads them, so there is
+// nothing to derive.  128-bit accesses where source and destination are both 16 B aligned (a tile starts a multiple of 16 B into both).
+constexpr int VC_TILE = 1024;
+__global__ void __launch_bounds__(256) k_bind_value_curves(const ValueCurveBindItem* __restrict__ items, int n_items) {
+    for (int i = blockIdx.y; i < n_items; i += gridDim.y) {
+        const ValueCurveBindItem it = items[i];
+        for (int64_t t0 = (int64_t)blockIdx.x * VC_TILE; t0 < it.n; t0 += (int64_t)gridDim.x * VC_TILE) {
+            const int m = (int)min((int64_t)VC_TILE, (int64_t)it.n - t0);
+            const unsigned* src = reinterpret_cast<const unsigned*>(it.src) + t0;
+            unsigned* dst = reinterpret_cast<unsigned*>(it.dst) + t0;
+            int done = 0;
+            if (((reinterpret_cast<uintptr_t>(src) | reinterpret_cast<uintptr_t>(dst)) & 15) == 0) {
+                const int m4 = m >> 2;
+                for (int k = threadIdx.x; k < m4; k += blockDim.x)
+                    reinterpret_cast<uint4*>(dst)[k] = __ldcs(reinterpret_cast<const uint4*>(src) + k);
+                done = 4 * m4;
+            }
+            for (int k = done + threadIdx.x; k < m; k += blockDim.x) dst[k] = __ldcs(src + k);
+        }
+    }
+}
+
 // Host emulation of the transforms above with the SAME butterfly, index and twiddle code (tests/test_conv_fft_host.py pins them against
 // numpy on a machine without a GPU).  mode 0: complex forward, natural -> position order; 1: complex inverse, position -> natural order
 // (unnormalised); 2: 2B reals -> B packed bins in position order; 3: B packed bins -> 2B reals (scaled by 1 / 2B).  data: 2B floats in place.
@@ -5114,6 +5137,10 @@ void launch_bind_waves(const WaveBindItem* d, int n, int max_len, bool any_norma
     if (any_normalize) k_wave_normalize<<<(unsigned)n, 1024, 0, s>>>(d);
 }
 void launch_bind_iir(const IirBindItem* d, int n, cudaStream_t s) { k_bind_iir<<<(unsigned)n, 32, 0, s>>>(d); }
+void launch_bind_value_curves(const ValueCurveBindItem* d, int n, int64_t max_len, cudaStream_t s) {
+    const int64_t bx = std::max<int64_t>(1, std::min<int64_t>((max_len + VC_TILE - 1) / VC_TILE, 65535));
+    k_bind_value_curves<<<dim3((unsigned)bx, (unsigned)std::min(n, 65535)), 256, 0, s>>>(d, n);
+}
 void launch_conv_ir_fft(const float* ir, int64_t ir_len, int64_t ir_stride, float2* h, int S, int channels, cudaStream_t s) {
     conv_configure();
     k_conv_ir_fft<<<dim3((unsigned)S, (unsigned)channels), CV_THREADS, CV_SMEM_ELEMS * sizeof(float2), s>>>(ir, ir_len, ir_stride, h, S);
