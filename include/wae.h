@@ -707,6 +707,37 @@ typedef struct wae_value_curve_binding {
  * WAE_INVALID_STATE while a declared curve of the batch has never been bound (a declared param the batch never renders needs no bind). */
 WAE_API wae_status wae_batch_bind_value_curves(wae_batch* batch, const wae_value_curve_binding* items, uint32_t n, void* stream);
 
+/* ---- Start and stop times of scheduled sources bound from device memory -------------------------------------------------------------
+ * Declares that the start time of a started AudioBufferSourceNode, OscillatorNode or ConstantSourceNode (and, with `bind_stop`, its stop
+ * time) is supplied per run from device memory (wae_batch_bind_schedules), so that one prepared batch renders any number of event
+ * onsets, note sequences or onset jitters without being built and planned again.  The `when` given to wae_source_start becomes a
+ * placeholder (as does the stop time with `bind_stop`); an AudioBufferSourceNode's offset and duration stay the ones given to
+ * wae_source_start.  A bound time is clamped to its window [lo, hi] (a NaN becomes lo); the reference panics on a negative or non-finite
+ * `when`, which a bind on the device cannot do.  The source is always planned with a gated output layout, and its path never depends on
+ * the bound times: a non-looping AudioBufferSourceNode whose computed playback rates are all > 0 and not automated takes the bound slow
+ * track (k_buffer_source_slow(bound), which plays a rate of 1 from an aligned start 1:1), every other one the serial kernel.  A declared
+ * source is never fused into k_chain.
+ * WAE_INVALID_ARGUMENT: not a scheduled source node, a window that is not finite with 0 <= lo <= hi.  WAE_INVALID_STATE: a source that
+ * has not been started, a second declaration, or a graph with a suspend point.  After the declaration, wae_source_start / wae_source_stop
+ * on the node and wae_graph_suspend on the graph answer WAE_INVALID_STATE.  wae_render_batch and wae_render_many answer
+ * WAE_INVALID_STATE on graphs with declarations; wae_batch_plan plans them. */
+WAE_API wae_status wae_source_set_device_schedule(wae_graph* graph, wae_node_id node, double start_lo, double start_hi, int32_t bind_stop,
+                                                  double stop_lo, double stop_hi);
+
+typedef struct wae_schedule_binding {
+    uint32_t graph_index;  /* caller's index, as wae_batch_fetch_graph */
+    wae_node_id node;      /* declared with wae_source_set_device_schedule */
+    const double* times;   /* device memory of the engine's GPU, 8-byte aligned: times[0] = start, times[1] = stop (declared bind_stop) */
+} wae_schedule_binding;
+
+/* Writes the times into the batch, asynchronously on the engine stream after the work already queued on `stream` (as
+ * wae_batch_bind_sources).  All-or-nothing: every item is validated before anything is enqueued.  A bound schedule stays until it is
+ * bound again.  WAE_INVALID_ARGUMENT: `times` is null, not 8-byte aligned or not device (or managed) memory of the engine's GPU, the
+ * declared times do not lie in one allocation, or one node is named twice in the call.  WAE_INVALID_STATE: graph_index out of range, or
+ * the node has no declaration.  wae_batch_run, wae_batch_run_group and wae_batch_run_pipelined answer WAE_INVALID_STATE while a declared
+ * schedule of the batch has never been bound (a declared source the batch never renders needs no bind). */
+WAE_API wae_status wae_batch_bind_schedules(wae_batch* batch, const wae_schedule_binding* items, uint32_t n, void* stream);
+
 /* PeriodicWave::new(context, PeriodicWaveOptions { real, imag, disable_normalization }) (src/periodic_wave.rs:104-209): fills `table`
  * (PERIODIC_WAVE_TABLE_LENGTH = 8192 in the reference) with the wavetable an OscillatorNode of type Custom plays.  `real` / `imag` may be
  * NULL (= zeros); both NULL = the sine default.  Host math, no engine needed. */

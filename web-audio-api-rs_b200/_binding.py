@@ -154,6 +154,12 @@ class ValueCurveBinding(C.Structure):
     _fields_ = [("graph_index", C.c_uint32), ("node", C.c_uint32), ("param_index", C.c_uint32), ("values", c_float_p)]
 
 
+class ScheduleBinding(C.Structure):
+    """wae_schedule_binding: the device start (and stop) time of one declared scheduled source of a prepared batch
+    (wae_batch_bind_schedules)."""
+    _fields_ = [("graph_index", C.c_uint32), ("node", C.c_uint32), ("times", c_double_p)]
+
+
 STATUS_NAMES = {0: "OK", 1: "INVALID_ARGUMENT", 2: "INVALID_STATE", 3: "NOT_SUPPORTED", 4: "UNSUPPORTED",
                 5: "CUDA_ERROR", 6: "OUT_OF_MEMORY", 7: "NO_DEVICE"}
 
@@ -199,6 +205,7 @@ WAE_SYMBOLS = [
     "wae_oscillator_set_device_periodic_wave", "wae_batch_bind_periodic_waves",
     "wae_iir_filter_set_device_coefficients", "wae_batch_bind_iir_coefficients",
     "wae_param_set_device_value_curve", "wae_batch_bind_value_curves",
+    "wae_source_set_device_schedule", "wae_batch_bind_schedules",
 ]
 
 
@@ -320,6 +327,9 @@ class Api:
             # AudioParam value curves bound from device memory
             f("param_set_device_value_curve", C.c_int32, [gp, C.c_uint32, C.c_uint32, C.c_uint32, C.c_double, C.c_double])
             f("batch_bind_value_curves", C.c_int32, [C.c_void_p, C.POINTER(ValueCurveBinding), C.c_uint32, C.c_void_p])
+            # start / stop times bound from device memory
+            f("source_set_device_schedule", C.c_int32, [gp, C.c_uint32, C.c_double, C.c_double, C.c_int32, C.c_double, C.c_double])
+            f("batch_bind_schedules", C.c_int32, [C.c_void_p, C.POINTER(ScheduleBinding), C.c_uint32, C.c_void_p])
         else:
             f("graph_create", C.c_int32, [C.c_uint32, C.c_uint64, C.c_float, C.POINTER(C.c_void_p)])
             f("render", C.c_int32, [gp, c_float_p])

@@ -264,6 +264,19 @@ class AudioScheduledSourceNode(AudioNode):
         api = self._ctx._api
         api.check(api.source_stop(self._ctx._g, self.id, when))
 
+    def set_device_schedule(self, start, stop=None):
+        """wae_source_set_device_schedule (product only): the start time of this started source (and, given `stop`, its stop time) is
+        supplied by Batch.bind_schedules from device memory before each run, clamped to the window `start` = (lo, hi) (`stop` = (lo, hi)).
+        The node takes no further start / stop."""
+        api = self._ctx._api
+        if not api.is_product:
+            raise B.WaeError(3, "schedules bound from device memory are a feature of the GPU engine")
+        s_lo, s_hi = (float(x) for x in start)
+        t_lo, t_hi = (0.0, 0.0) if stop is None else (float(x) for x in stop)
+        api.check(api.source_set_device_schedule(self._ctx._g, self.id, s_lo, s_hi, 0 if stop is None else 1, t_lo, t_hi))
+        self._ctx._device_schedules[self.id] = stop is not None
+        return self
+
 
 class OscillatorNode(AudioScheduledSourceNode):
     def set_periodic_wave(self, table):
@@ -514,6 +527,7 @@ class OfflineAudioContext:
         self._device_waves = {}  # node id -> coefficient count declared with set_device_periodic_wave
         self._device_iirs = {}  # node id -> (feedforward count, feedback count) declared with set_device_coefficients
         self._device_value_curves = {}  # (node id, param index) -> length declared with set_device_value_curve
+        self._device_schedules = {}  # node id -> whether set_device_schedule declared the stop time too
 
     def __del__(self):
         try:
@@ -966,6 +980,45 @@ class Batch:
         self.api.check(self.api.batch_bind_value_curves(self.handle, items, n * len(params), C.c_void_p(self._torch_stream_handle())))
         for t in tensors:
             self._keep_until_read(t)
+
+    def bind_schedules(self, nodes, starts, stops=None, graphs=None):
+        """wae_batch_bind_schedules: starts[i] (and stops[i]) become the start (and stop) times of the scheduled source `nodes` (declared
+        with set_device_schedule) in context graphs[i] (default: 0..n-1).  `starts` / `stops`: float64 CUDA tensors [n] for one node, or
+        [n][k] for a list of k nodes; `stops` is given exactly when the nodes were declared with a stop window.  One call, ordered after
+        torch's current stream; the times are read on the engine stream, and their memory is kept from reuse until they have been."""
+        import torch
+        for t in (starts,) if stops is None else (starts, stops):
+            if not (isinstance(t, torch.Tensor) and t.is_cuda and t.dtype == torch.float64 and t.dim() in (1, 2)):
+                raise B.WaeError(1, "bind_schedules: starts / stops must be float64 CUDA tensors [n] or [n][k]")
+        many = isinstance(nodes, (list, tuple))
+        ids = [int(getattr(x, "id", x)) for x in nodes] if many else [int(getattr(nodes, "id", nodes))]
+        n, k = starts.shape[0], len(ids)
+        if (starts.dim() == 2) != many or (many and starts.shape[1] != k):
+            raise B.WaeError(1, f"bind_schedules: starts is {list(starts.shape)} for {k} node(s): [n] for one node, [n][k] for a list")
+        if stops is not None and stops.shape != starts.shape:
+            raise B.WaeError(1, f"bind_schedules: stops is {list(stops.shape)}, starts {list(starts.shape)}")
+        graphs = list(range(n)) if graphs is None else [int(g) for g in graphs]
+        if len(graphs) != n:
+            raise B.WaeError(1, f"bind_schedules: {n} rows for {len(graphs)} graphs")
+        for g in graphs:
+            if not 0 <= g < self.n:
+                raise B.WaeError(2, f"bind_schedules: graph index {g} is out of range")
+            for nid in ids:
+                declared = self.contexts[g]._device_schedules.get(nid)
+                if declared is not None and declared != (stops is not None):
+                    raise B.WaeError(1, f"bind_schedules: node {nid} of graph {g} was declared {'with' if declared else 'without'} a stop "
+                                        f"window, stops is {'missing' if declared else 'given'}")
+        # one item reads [start, stop] from adjacent memory: the times are packed on torch's current stream
+        s = starts.reshape(n, k)
+        times = (s if stops is None else torch.stack([s, stops.reshape(n, k)], dim=2)).reshape(n, k, -1).contiguous()
+        width = times.shape[2]
+        items = (B.ScheduleBinding * max(n * k, 1))()
+        base = times.data_ptr()
+        for i, g in enumerate(graphs):
+            for j, nid in enumerate(ids):
+                items[i * k + j] = B.ScheduleBinding(g, nid, C.cast(C.c_void_p(base + 8 * width * (i * k + j)), B.c_double_p))
+        self.api.check(self.api.batch_bind_schedules(self.handle, items, n * k, C.c_void_p(self._torch_stream_handle())))
+        self._keep_until_read(times)
 
     def _graphs_and_nodes(self, fn, nodes, graphs, n):
         """The graph index and node id of each of n binding items: `graphs` (default 0..n-1), `nodes` one node (or id) for all graphs or

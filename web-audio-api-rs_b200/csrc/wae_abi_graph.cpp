@@ -4,6 +4,7 @@
 #include "wae_graph.h"
 #include "wae_hostmath.h"
 #include "wae_hrtf_host.h"
+#include "wae_kernels.h"
 #include "wae_param_core.h"
 #include "wae_param_host.h"
 #include "wae_param_walk.h"
@@ -654,6 +655,8 @@ WAE_API wae_status wae_graph_suspend(wae_graph* g, double suspend_time) {
     if (!g->epochs.empty() && quantum < last)
         return fail(WAE_INVALID_STATE, "InvalidStateError - cannot suspend at a time that is not after the current time");
     if (quantum >= total) return fail(WAE_INVALID_STATE, "InvalidStateError - cannot suspend after the end of the rendering");
+    if (g->device_schedules)  // (sources are planned per render segment from their start time)
+        return fail(WAE_INVALID_STATE, "InvalidStateError - the graph has schedules bound from device memory (wae_source_set_device_schedule)");
     g->epochs.push_back(wae_graph::Epoch{quantum * 128, g->nodes});
     return WAE_OK;
 }
@@ -940,6 +943,8 @@ WAE_API wae_status wae_source_start(wae_graph* g, wae_node_id node, double when,
     Node& n = ni->second;
     if (!(n.kind == K_OSC || n.kind == K_ABSN || n.kind == K_CONST)) return fail(WAE_INVALID_ARGUMENT, "not a scheduled source node");
     if (!(std::isfinite(when) && when >= 0.)) return fail(WAE_INVALID_ARGUMENT, "RangeError - when should be positive");
+    if (n.device_schedule)
+        return fail(WAE_INVALID_STATE, "InvalidStateError - the start time is bound from device memory (wae_source_set_device_schedule)");
     if (n.has_start) return fail(WAE_INVALID_STATE, "InvalidStateError - Cannot call `start` twice");
     if (n.kind == K_ABSN && (!(offset >= 0.) || !(duration >= 0.))) return fail(WAE_INVALID_ARGUMENT, "RangeError - offset/duration should be positive");
     n.has_start = true;
@@ -962,7 +967,40 @@ WAE_API wae_status wae_source_stop(wae_graph* g, wae_node_id node, double when) 
     if (!(n.kind == K_OSC || n.kind == K_ABSN || n.kind == K_CONST)) return fail(WAE_INVALID_ARGUMENT, "not a scheduled source node");
     if (!(std::isfinite(when) && when >= 0.)) return fail(WAE_INVALID_ARGUMENT, "RangeError - when should be positive");
     if (!n.has_start) return fail(WAE_INVALID_STATE, "InvalidStateError cannot stop before start");
+    if (n.device_schedule)
+        return fail(WAE_INVALID_STATE, "InvalidStateError - the schedule is bound from device memory (wae_source_set_device_schedule)");
     n.stop_time = when;
+    return WAE_OK;
+}
+
+// The start time (and with bind_stop the stop time) becomes a placeholder, written per run by wae_batch_bind_schedules clamped to its
+// window.  The plan is made with the windows' low ends and a gated output layout, so no planning decision depends on the bound times.
+// Sources are planned per render segment from their start time, so a graph with suspend points takes no declaration (and the other way
+// round: wae_graph_suspend refuses a graph with one).
+WAE_API wae_status wae_source_set_device_schedule(wae_graph* g, wae_node_id node, double start_lo, double start_hi, int32_t bind_stop,
+                                                  double stop_lo, double stop_hi) {
+    if (!g) return fail(WAE_INVALID_ARGUMENT, "null graph");
+    Node* n = g->nodes.get(node);
+    if (!n || !(n->kind == K_OSC || n->kind == K_ABSN || n->kind == K_CONST)) return fail(WAE_INVALID_ARGUMENT, "not a scheduled source node");
+    auto window = [](double lo, double hi) { return std::isfinite(lo) && std::isfinite(hi) && 0. <= lo && lo <= hi; };
+    if (!window(start_lo, start_hi) || (bind_stop && !window(stop_lo, stop_hi)))
+        return fail(WAE_INVALID_ARGUMENT, "RangeError - a schedule window must be finite with 0 <= lo <= hi");
+    if (n->device_schedule)
+        return fail(WAE_INVALID_STATE, "InvalidStateError - the schedule is already bound from device memory (wae_source_set_device_schedule)");
+    if (!n->has_start) return fail(WAE_INVALID_STATE, "InvalidStateError - the source has not been started");
+    if (!g->epochs.empty())
+        return fail(WAE_INVALID_STATE, "InvalidStateError - a schedule is bound from device memory in a graph with a suspend point");
+    n->device_schedule = true;
+    n->sched_stop = bind_stop != 0;
+    n->start_time = start_lo;
+    n->sched_lo[0] = start_lo;
+    n->sched_hi[0] = start_hi;
+    if (bind_stop) {
+        n->stop_time = stop_lo;
+        n->sched_lo[1] = stop_lo;
+        n->sched_hi[1] = stop_hi;
+    }
+    g->device_schedules++;
     return WAE_OK;
 }
 
@@ -1015,12 +1053,12 @@ WAE_API wae_status wae_periodic_wave_table(const float* real, const float* imag,
     return WAE_OK;
 }
 
-// Test hook for the scheduling clock every AudioScheduledSourceNode is lowered with (csrc/wae_hostmath.h SchedClock): the first frame
+// Test hook for the scheduling clock every AudioScheduledSourceNode is lowered with (csrc/wae_kernels.h SchedClock): the first frame
 // whose time, accumulated the way the reference's renderers do (block time = frame / sample_rate, then `+= dt` per frame inside the
 // quantum that contains `time`), is >= `time`; *frame_time = that accumulated time.
 WAE_API wae_status wae_sched_first_frame_at_or_after(float sample_rate, double time, int64_t* frame, double* frame_time) {
     if (!frame || !frame_time || !(sample_rate > 0.f)) return fail(WAE_INVALID_ARGUMENT, "null / bad argument");
-    hostmath::SchedClock clock(sample_rate);
+    SchedClock clock(sample_rate);
     *frame = clock.first_frame_at_or_after(time, frame_time);
     return WAE_OK;
 }

@@ -603,6 +603,38 @@ struct ValueCurveBindItem {
     int32_t pad;
 };
 
+// ---- wae_batch_bind_schedules: caller start / stop times -> the record fields of a declared scheduled source they reach ------------
+// One entry per record; the bind re-derives the fields from the times with the planner's own functions (wae_kernels.h).
+enum SchedKind : int32_t {
+    SCHED_OSC = 0,          // OscInst (S_OSC, ChainInst::osc): n_first, n_stop, phase0
+    SCHED_OSC_AR = 1,       // OscArInst: base.n_first, base.n_stop, base.phase0, start_ratio
+    SCHED_CONST = 2,        // ConstInst (S_CONST, ChainInst::cst): n_first, n_stop
+    SCHED_META_OSC = 3,     // MetaInst (META_SOURCE) of an oscillator's gated output: n_first, n_stop
+    SCHED_META_CONST = 4,   // MetaInst (META_SOURCE) of a constant source's gated output: n_first, n_stop
+    SCHED_ABSN_BOUND = 5,   // AbsnBoundInst: s.n_first, s.n_stop, start_delta, n_start, fast_end, fast_ok
+    SCHED_ABSN_SERIAL = 6,  // AbsnSerialInst: start_time, stop_time (the kernel takes them raw)
+};
+struct SchedPatch {
+    void* dst;            // the record
+    int32_t kind;
+    int32_t flag;         // SCHED_OSC*: outside Nyquist; SCHED_ABSN_BOUND: fast_ok but for the start and stop (sampling ratio 1, default
+                          // loop points, no duration)
+    float sample_rate;    // the graph's (the clock)
+    int32_t pad;
+    double incr;          // SCHED_OSC*: the phase increment per frame
+    double offset;        // SCHED_ABSN_BOUND: start(when, offset)
+    double duration;      // SCHED_ABSN_BOUND: the buffer's duration
+    double stop_time;     // the planned stop time, taken when the stop is not bound (>= 1e300: none)
+    int64_t lq;           // SCHED_ABSN_BOUND: the render length of the plan (absn_fast_end)
+};
+struct SchedBindItem {
+    const double* times;        // caller's [start] or [start, stop] (8 B aligned)
+    const SchedPatch* patches;  // the node's entries
+    double lo[2], hi[2];        // the declared windows the times are clamped to (a NaN becomes lo)
+    int32_t n_patches;
+    int32_t bind_stop;
+};
+
 // ---- wae_batch_bind_params: per-run values of params planned as constants ------------------------------------------------------
 struct ParamBindItem {  // one float of the caller's device memory -> value slot `slot`
     const float* src;

@@ -330,8 +330,21 @@ struct StageBuild {
         int32_t rec, bq, scan;
     };
     std::vector<IirPatchRec> iir_patches;
+    // Patch entries of schedules bound from device memory (wae_source_set_device_schedule): the source's fields `off` bytes into record
+    // `rec` of this stage's table (an OscInst / ConstInst inside a ChainInst, or the record itself)
+    struct SchedPatchRec {
+        uint32_t graph;  // batch position
+        wae_node_id node;
+        int32_t rec;
+        uint32_t off;
+        SchedPatch p;    // dst set when the tables are uploaded
+    };
+    std::vector<SchedPatchRec> sched_patches;
     size_t records() const {  // size of the table patch entries point into
         switch (kind) {
+            case S_OSC: return osc.size();
+            case S_OSC_AR: return osc_ar.size();
+            case S_CONST: return cst.size();
             case S_IIR: return iir.size();
             case S_SHAPER_OS: return shaper_os.size();
             case S_CHAIN: case S_VSUM: return chain.size();
@@ -528,6 +541,21 @@ struct wae_batch {
     std::map<std::pair<uint32_t, wae_node_id>, size_t> iir_index;  // (batch position, node) -> iirs
     size_t iirs_unbound = 0;
     IirPatch* d_iir_patches = nullptr;
+    // wae_source_set_device_schedule: the windows of each declared source and the range of its patch entries in d_sched_patches (every
+    // record its times reach), rewritten by wae_batch_bind_schedules.  A declared source the planner never reached has none: binding it is
+    // validated and writes nothing, and runs do not wait for it.
+    struct DevSchedule {
+        uint32_t graph;  // batch position
+        wae_node_id node;
+        bool bind_stop;
+        double lo[2], hi[2];
+        int32_t p0, p1;  // its entries in d_sched_patches
+        bool bound;
+    };
+    std::vector<DevSchedule> schedules;
+    std::map<std::pair<uint32_t, wae_node_id>, size_t> schedule_index;  // (batch position, node) -> schedules
+    size_t schedules_unbound = 0;
+    SchedPatch* d_sched_patches = nullptr;
     // wae_param_set_device_value_curve: the curve pool of each declared param (ParamInst::curves: made by the planner, zeroed, the param's
     // host curves copied in once, never in the upload slabs) and where the declared values lie in it, rewritten by
     // wae_batch_bind_value_curves.  A declared param the planner never lowered has no pool: binding it is validated and writes nothing,
@@ -935,6 +963,8 @@ struct Planner {
         // IIR filters whose coefficients are bound from device memory: the entry of their biquad (bq; rec / scan set when the chain is
         // emitted)
         std::vector<StageBuild::IirPatchRec> iir_patches;
+        // a source whose schedule is bound from device memory: the entry of ChainInst::osc / ::cst (rec set when the chain is emitted)
+        std::vector<StageBuild::SchedPatchRec> sched_patches;
     };
 
     // Node state is allocated through a key (graph, node, n-th allocation of that node, salt): the plans of consecutive
@@ -1101,7 +1131,7 @@ struct Planner {
     uint32_t gi = 0;
     Orderer ord{};
     NodeTable node_table;  // (the per-node vectors keep their capacity)
-    hm::SchedClock clock{48000.f};
+    SchedClock clock{48000.f};
     bool want_scan_coefs = false;  // (the sizing pass needs their number only)
     // ---- chain fusion (WAE_OPT_FUSE): sources and biquad/gain/shaper nodes are not emitted one stage each; a node
     // with exactly one consumer stays PENDING, the consumer either extends the chain (same channel count, single
@@ -1173,6 +1203,10 @@ struct Planner {
             r.rec = rec;
             r.scan = pc.inst.bq[r.bq].coef;
             s.iir_patches.push_back(r);
+        }
+        for (StageBuild::SchedPatchRec r : pc.sched_patches) {
+            r.rec = rec;
+            s.sched_patches.push_back(r);
         }
     }
     static bool chain_has_patches(const PendingChain& pc) {
@@ -1277,8 +1311,11 @@ struct Planner {
             p.out_buf[0].meta_stride = (uint32_t)((b->chunk / 128 + 16) / 16 * 16);
         }
     }
-    // a scheduled source: `ch` channels inside [n_first, n_stop), one silent channel outside (never silent when it covers the render)
-    Lay source_lay(int64_t n_first, int64_t n_stop, int ch) const { return (n_first <= 0 && n_stop >= glq) ? Lay::fixed(ch) : Lay::gated(ch); }
+    // a scheduled source: `ch` channels inside [n_first, n_stop), one silent channel outside (never silent when it covers the render; a
+    // schedule bound from device memory is always gated)
+    Lay source_lay(int64_t n_first, int64_t n_stop, int ch, bool declared = false) const {
+        return (!declared && n_first <= 0 && n_stop >= glq) ? Lay::fixed(ch) : Lay::gated(ch);
+    }
     void source_meta(NodeCtx& nc, int64_t n_first, int64_t n_stop, int ch) {
         MetaInst m{};
         m.out = nc.p.out_buf[0];
@@ -1289,10 +1326,14 @@ struct Planner {
         m.n_stop = n_stop;
         stage(nc.L, S_META).meta.push_back(m);
     }
-    // a scheduled source's output buffer: its layout, and the layout track (k_meta) where that is not constant
-    BufRef source_out(NodeCtx& nc, int64_t n_first, int64_t n_stop, int ch) {
-        out_dynamic(nc, source_lay(n_first, n_stop, ch));
-        if (nc.p.out_lay[0].dyn()) source_meta(nc, n_first, n_stop, ch);
+    // a scheduled source's output buffer: its layout, and the layout track (k_meta) where that is not constant.  `sched`: the patch entry
+    // of a schedule bound from device memory, for the track's record
+    BufRef source_out(NodeCtx& nc, int64_t n_first, int64_t n_stop, int ch, const SchedPatch* sched = nullptr) {
+        out_dynamic(nc, source_lay(n_first, n_stop, ch, sched != nullptr));
+        if (nc.p.out_lay[0].dyn()) {
+            source_meta(nc, n_first, n_stop, ch);
+            if (sched) add_sched_patch(stage(nc.L, S_META), nc.n, *sched);
+        }
         return nc.p.out_buf[0];
     }
     // biquad / IIR (biquad_filter.rs:778-815): silent once the input is and the tail has rung out; keeps the channels of the last
@@ -1333,12 +1374,19 @@ struct Planner {
         int ch;
         double duration, ls, le, computed_rate;  // ls / le: the clamped loop boundaries
     };
-    struct AbsnStart {  // the slow track's first playing frame and stop frame
-        int64_t n_first, n_stop;
-        double t_first, start;  // the time of frame n_first, the start time (snapped to it when almost equal)
-    };
-    AbsnStart absn_start(const Node& n) const;
-    int64_t absn_fast_end(int64_t n_start, double duration) const;
+    // a patch entry of the schedule of declared source `n` (wae_source_set_device_schedule) for the last record of stage `s`, its fields
+    // `off` bytes into it
+    SchedPatch sched_entry(const Node& n, int32_t kind) const {
+        SchedPatch p{};
+        p.kind = kind;
+        p.sample_rate = g->sample_rate;
+        p.stop_time = n.stop_time;
+        p.lq = lq;
+        return p;
+    }
+    void add_sched_patch(StageBuild& s, const Node& n, const SchedPatch& p, uint32_t off = 0) {
+        s.sched_patches.push_back(StageBuild::SchedPatchRec{gi, n.id, (int32_t)s.records() - 1, off, p});
+    }
     bool lower_absn(NodeCtx& nc);
     bool absn_silent(NodeCtx& nc);
     bool absn_serial(NodeCtx& nc, const AbsnPlay& s, const PRef& pdet, const PRef& prate);
@@ -1482,6 +1530,7 @@ static void merge_builds(Builds& dst, Builds& src) {
             if (pr.rec2 >= 0) pr.rec2 += (int32_t)(s.kind == S_SPAN ? bs.records : bs.scan);
         }
         for (auto& cp : s.curve_patches) cp.rec += (int32_t)bs.records;
+        for (auto& sp : s.sched_patches) sp.rec += (int32_t)bs.records;
         for (auto& ip : s.iir_patches) {
             ip.rec += (int32_t)bs.records;
             if (ip.scan >= 0) ip.scan += (int32_t)bs.scan;
@@ -1517,6 +1566,7 @@ static void merge_builds(Builds& dst, Builds& src) {
         append_vec(d.patches, s.patches);
         append_vec(d.curve_patches, s.curve_patches);
         append_vec(d.iir_patches, s.iir_patches);
+        append_vec(d.sched_patches, s.sched_patches);
         d.n_scan_coef += s.n_scan_coef;
         d.max_ch = std::max(d.max_ch, s.max_ch);
     }
@@ -2244,38 +2294,22 @@ bool Planner::lower_osc(NodeCtx& nc) {
     o.n_stop = std::numeric_limits<int64_t>::max();
     o.phase0 = 0.;
     if (n.start_time < 1e300) {
-        // oscillator.rs:391-428,511-540: first rendered frame and its phase
-        int64_t q = clock.quantum_containing(n.start_time);
-        double start = n.start_time;
-        if (start < clock.block_time(q)) start = clock.block_time(q);  // "prevent scheduling in the past"
-        double t = 0.;
-        // walk the accumulated per-frame clock of that quantum
-        double cur = clock.block_time(q);
-        int i = 0;
-        for (; i < 128; i++) {
-            if (!(cur < start)) break;
-            cur += clock.dt;
-        }
-        t = cur;
-        o.n_first = q * 128 + i;
-        if (i < 128 && t > start) {
-            double ratio = (t - start) / clock.dt;
-            start_ratio = ratio;
-            double ph = o.incr * ratio;
-            if (o.outside_nyquist) {
-                ph = std::fmod(ph, 1.);
-                if (ph < 0.) ph += 1.;
-            } else {
-                ph = hm::unroll_phase(ph);
-            }
-            o.phase0 = ph;
-        }
-        if (n.stop_time < 1e300) {
-            int64_t qs = clock.quantum_containing(n.stop_time);
-            if (n.stop_time <= clock.block_time(qs)) o.n_stop = qs * 128;
-            else o.n_stop = clock.first_frame_at_or_after(n.stop_time);
-        }
+        const OscStart st = osc_start(clock, n.start_time, o.incr, o.outside_nyquist);
+        o.n_first = st.n_first;
+        o.phase0 = st.phase0;
+        start_ratio = st.start_ratio;
+        o.n_stop = osc_stop_frame(clock, n.stop_time);
     }
+    // a schedule bound from device memory: the fields the times reach are re-derived by the bind (planned with the windows' low ends)
+    SchedPatch sched{};
+    if (n.device_schedule) {
+        sched = sched_entry(n, nc.dyn_params ? SCHED_OSC_AR : SCHED_OSC);
+        sched.incr = o.incr;
+        sched.flag = o.outside_nyquist;
+    }
+    SchedPatch meta_sched = sched;
+    meta_sched.kind = SCHED_META_OSC;
+    const SchedPatch* track_sched = n.device_schedule ? &meta_sched : nullptr;
     if (n.type == WAE_OSC_CUSTOM && n.device_wave) {  // a wave bound from device memory: planned as a host wave of its length
         o.table = device_wave(n);
         o.table_len = (int)n.device_wave_len;
@@ -2300,16 +2334,21 @@ bool Planner::lower_osc(NodeCtx& nc) {
         oa.phase = alloc<double>(1, true, true);
         oa.sample_rate = g->sample_rate;
         if (!oa.phase) return bail(WAE_OUT_OF_MEMORY, "out of device memory (state)");
-        oa.base.out = source_out(nc, o.n_first, o.n_stop, 1);
-        stage(nc.L, S_OSC_AR).osc_ar.push_back(oa);
+        oa.base.out = source_out(nc, o.n_first, o.n_stop, 1, track_sched);
+        StageBuild& sb = stage(nc.L, S_OSC_AR);
+        sb.osc_ar.push_back(oa);
+        if (n.device_schedule) add_sched_patch(sb, n, sched);
     } else if (nc.fuse_n) {
         PendingChain pc = source_chain(CHAIN_SRC_OSC, 1);
         pc.inst.osc = o;
-        pc.lay = source_lay(o.n_first, o.n_stop, 1);
+        pc.lay = source_lay(o.n_first, o.n_stop, 1, n.device_schedule);
+        if (n.device_schedule) pc.sched_patches.push_back(StageBuild::SchedPatchRec{gi, n.id, -1, (uint32_t)offsetof(ChainInst, osc), sched});
         return finish_chain(nc, std::move(pc));
     } else {
-        o.out = source_out(nc, o.n_first, o.n_stop, 1);
-        stage(nc.L, S_OSC).osc.push_back(o);
+        o.out = source_out(nc, o.n_first, o.n_stop, 1, track_sched);
+        StageBuild& sb = stage(nc.L, S_OSC);
+        sb.osc.push_back(o);
+        if (n.device_schedule) add_sched_patch(sb, n, sched);
     }
     return true;
 }
@@ -2330,22 +2369,22 @@ bool Planner::lower_const(NodeCtx& nc) {
         c.n_first = clock.first_frame_at_or_after(n.start_time);
         if (n.stop_time < 1e300) c.n_stop = clock.first_frame_at_or_after(n.stop_time);
     }
+    // a schedule bound from device memory: the fields the times reach are re-derived by the bind (planned with the windows' low ends)
+    const SchedPatch sched = sched_entry(n, SCHED_CONST);
+    SchedPatch meta_sched = sched;
+    meta_sched.kind = SCHED_META_CONST;
     if (nc.fuse_n) {
         PendingChain pc = source_chain(CHAIN_SRC_CONST, 1);
         pc.inst.cst = c;
-        pc.lay = source_lay(c.n_first, c.n_stop, 1);
+        pc.lay = source_lay(c.n_first, c.n_stop, 1, n.device_schedule);
+        if (n.device_schedule) pc.sched_patches.push_back(StageBuild::SchedPatchRec{gi, n.id, -1, (uint32_t)offsetof(ChainInst, cst), sched});
         return finish_chain(nc, std::move(pc));
     }
-    c.out = source_out(nc, c.n_first, c.n_stop, 1);
-    stage(nc.L, S_CONST).cst.push_back(c);
+    c.out = source_out(nc, c.n_first, c.n_stop, 1, n.device_schedule ? &meta_sched : nullptr);
+    StageBuild& sb = stage(nc.L, S_CONST);
+    sb.cst.push_back(c);
+    if (n.device_schedule) add_sched_patch(sb, n, sched);
     return true;
-}
-
-static bool almost_equal(double x, double y) {
-    if (x == y) return true;
-    const double tol = 1.4901161193847656e-8;
-    double d = std::fabs(y - x);
-    return d <= tol || d <= std::max(std::fabs(x), std::fabs(y)) * tol;
 }
 
 bool Planner::lower_absn(NodeCtx& nc) {
@@ -2363,15 +2402,13 @@ bool Planner::lower_absn(NodeCtx& nc) {
     double ls = n.loop_start, le = n.loop_end;  // clamp_loop_boundaries, audio_buffer_source.rs:400-417
     if (ls < 0.) ls = 0.; else if (ls > duration) ls = duration;
     if (le <= 0. || le > duration) le = duration;
-    int64_t q = clock.quantum_containing(n.start_time);
-    // a start time that IS the next block boundary but compares below next_block_time by one rounding:
-    // the reference goes through one all-silent slow-track quantum, then aligns (audio_buffer_source.rs:521-523)
-    if (n.start_time > clock.block_time(q) && n.start_time == clock.block_time(q + 1)) q = q + 1;
+    const int64_t q = absn_start_quantum(clock, n.start_time);
     bool aligned = (n.start_time <= clock.block_time(q)) && n.offset == 0.;  // start in the past snaps to the block
-    bool fast = !rate_automated && !rate_bound && aligned && (double)pb.sample_rate / sr == 1. && computed_rate == 1. && ls == 0. &&
-                le == duration && n.duration > 1e300 && n.stop_time > 1e300;
+    // (a schedule bound from device memory: the start may fall anywhere, the bound slow track or the serial kernel plays it)
+    bool fast = !rate_automated && !rate_bound && !n.device_schedule && aligned && (double)pb.sample_rate / sr == 1. && computed_rate == 1. &&
+                ls == 0. && le == duration && n.duration > 1e300 && n.stop_time > 1e300;
     // everything the closed-form tracks do not cover runs the renderer's own frame loop (one warp per source)
-    bool serial = rate_automated || (!fast && !(computed_rate > 0.));
+    bool serial = rate_automated || (!fast && !(computed_rate > 0.)) || (n.device_schedule && n.loop);
     // playbackRate / detune bound from device memory: the path follows from the computed rates their declared ranges allow (the low
     // corner's exp2 underflows to 0 far enough below 0 cents), never from the value.  A non-looping source whose rates are all positive
     // takes the bound slow track; the serial kernel is right for every other value.
@@ -2410,7 +2447,7 @@ bool Planner::lower_absn(NodeCtx& nc) {
     }
     const AbsnPlay s{&pb, d_buf, len, stride, ch, duration, ls, le, computed_rate};
     if (serial) return absn_serial(nc, s, pdet, prate);
-    if (rate_bound) return absn_bound(nc, s, pdet, prate, q, aligned, rate_hi);
+    if (rate_bound || n.device_schedule) return absn_bound(nc, s, pdet, prate, q, aligned, rate_hi);
     if (!fast) return absn_slow(nc, s);
     return absn_fast(nc, s, q, fused);
 }
@@ -2461,56 +2498,9 @@ bool Planner::absn_serial(NodeCtx& nc, const AbsnPlay& s, const PRef& pdet, cons
             operand(r, 0, *refs[i], refs[i]->v);
             add_patch(sb, r, (uint32_t)offs[i]);
         }
+    if (n.device_schedule) add_sched_patch(sb, n, sched_entry(n, SCHED_ABSN_SERIAL));  // (the raw start / stop times)
     algorithmic_bytes += (uint64_t)s.ch * 4ull * (uint64_t)std::min<int64_t>(lq, (int64_t)s.len);
     return true;
-}
-
-// first frame at / after the start time: current_time = block_time + i * dt (:648), sticky within almost::equal (:652-654); first frame
-// with current_time >= stop_time (:663)
-Planner::AbsnStart Planner::absn_start(const Node& n) const {
-    AbsnStart r{-1, std::numeric_limits<int64_t>::max(), 0., n.start_time};
-    int64_t qq = clock.quantum_containing(r.start);
-    for (int guard = 0; guard < 3 && r.n_first < 0; guard++, qq++) {
-        double bt0 = clock.block_time(qq);
-        for (int i = 0; i < 128; i++) {
-            double t = bt0 + (double)i * clock.dt;
-            if (almost_equal(t, r.start)) r.start = t;
-            if (!(t < r.start)) {
-                r.n_first = qq * 128 + i;
-                r.t_first = t;
-                break;
-            }
-        }
-    }
-    if (r.n_first < 0) r.n_first = qq * 128;
-    if (n.stop_time < 1e300) {
-        int64_t qs = clock.quantum_containing(n.stop_time);
-        int64_t ns = (qs + 1) * 128;
-        double bt0 = clock.block_time(qs);
-        for (int i = 0; i < 128; i++)
-            if (bt0 + (double)i * clock.dt >= n.stop_time) {
-                ns = qs * 128 + i;
-                break;
-            }
-        r.n_stop = ns;
-    }
-    return r;
-}
-
-// the fast track of a non-looping source: the frame after the quantum in which it has `ended`.  The reference accumulates
-// buffer_time += block_duration and stops once it reaches the buffer's duration (audio_buffer_source.rs:609,826-838) — replayed, not
-// divided
-int64_t Planner::absn_fast_end(int64_t n_start, double duration) const {
-    const double block_duration = clock.dt * 128.;
-    const int64_t max_q = (lq - n_start) / 128 + 2;
-    int64_t played = 0;
-    double bt = 0.;
-    while (played < max_q) {
-        bt += block_duration;
-        played++;
-        if (bt >= duration) break;
-    }
-    return n_start + played * 128;
 }
 
 // ---- slow track (audio_buffer_source.rs:625-823): fractional playhead
@@ -2537,7 +2527,7 @@ bool Planner::absn_slow(NodeCtx& nc, const AbsnPlay& s) {
         a.loop_start = 0.;
         a.loop_end = duration;
     }
-    const AbsnStart st = absn_start(n);
+    const AbsnStart st = absn_start(clock, n.start_time, n.stop_time);
     const int64_t n_first = st.n_first;
     a.n_first = n_first;
     a.n_stop = st.n_stop;
@@ -2577,15 +2567,16 @@ bool Planner::absn_bound(NodeCtx& nc, const AbsnPlay& s, const PRef& pdet, const
     a.pos_scale = ((double)s.pb->sample_rate / sr) * sr;
     a.duration = n.duration;
     a.loop_end = s.duration;
-    const AbsnStart st = absn_start(n);
+    const AbsnStart st = absn_start(clock, n.start_time, n.stop_time);
     a.n_first = st.n_first;
     a.n_stop = st.n_stop;
     r.dt = clock.dt;
     r.offset = n.offset;
     r.start_delta = st.t_first - st.start;
     r.n_start = q * 128;
-    r.fast_end = absn_fast_end(r.n_start, s.duration);
-    r.fast_ok = aligned && (double)s.pb->sample_rate / sr == 1. && s.ls == 0. && s.le == s.duration && n.duration > 1e300 && n.stop_time > 1e300;
+    r.fast_end = absn_fast_end(clock, lq, r.n_start, s.duration);
+    const bool fast_shape = (double)s.pb->sample_rate / sr == 1. && s.ls == 0. && s.le == s.duration && n.duration > 1e300;
+    r.fast_ok = aligned && fast_shape && n.stop_time > 1e300;
     r.rate = prate.v;
     r.detune = pdet.v;
     // The one decision the range drives: a constant layout only when the source plays to the end of the render at every rate it allows.
@@ -2593,11 +2584,19 @@ bool Planner::absn_bound(NodeCtx& nc, const AbsnPlay& s, const PRef& pdet, const
     const AbsnSlowDerived top = absn_slow_derive(clock.dt, rate_hi, n.offset, r.start_delta, s.duration, n.duration, false, s.duration, a.n_first,
                                                  a.n_stop);
     const int64_t margin = (pdet.bound >= 0 || pdet.v != 0.f) ? 128 : 0;
-    const bool fixed = a.n_first <= 0 && top.n_end >= glq + margin && !(r.fast_ok && r.fast_end < glq);
+    // (a schedule bound from device memory is always gated)
+    const bool fixed = !n.device_schedule && a.n_first <= 0 && top.n_end >= glq + margin && !(r.fast_ok && r.fast_end < glq);
     out_dynamic(nc, fixed ? Lay::fixed(s.ch) : Lay::gated(s.ch));  // (gated: the kernel writes the layout track)
     a.out = nc.p.out_buf[0];
     StageBuild& sb = stage(nc.L, S_ABSN_BOUND);
     sb.absn_bound.push_back(r);
+    if (n.device_schedule) {  // the start-dependent fields, re-derived by the bind; the kernel derives the rest per run as before
+        SchedPatch sp = sched_entry(n, SCHED_ABSN_BOUND);
+        sp.flag = fast_shape;
+        sp.offset = n.offset;
+        sp.duration = s.duration;
+        add_sched_patch(sb, n, sp);
+    }
     const PRef* refs[2] = {&pdet, &prate};
     const size_t offs[2] = {offsetof(AbsnBoundInst, detune), offsetof(AbsnBoundInst, rate)};
     for (int i = 0; i < 2; i++)
@@ -2663,7 +2662,7 @@ bool Planner::absn_fast(NodeCtx& nc, const AbsnPlay& s, int64_t q, bool fused) {
     a.buf_offset = 0;
     a.ch = s.ch;
     a.loop = n.loop ? 1 : 0;
-    if (!n.loop) a.n_stop = absn_fast_end(a.n_start, s.duration);
+    if (!n.loop) a.n_stop = absn_fast_end(clock, lq, a.n_start, s.duration);
     if (fused) {
         PendingChain pc = source_chain(CHAIN_SRC_ABSN, s.ch);
         pc.inst.absn = a;
@@ -3456,7 +3455,7 @@ bool Planner::plan_graph(wae_graph* graph, uint32_t graph_index) {
             it->in_edges[e.other_index].push_back(PortRef{id, e.self_index});
         }
     }
-    clock = hm::SchedClock(g->sample_rate);
+    clock = SchedClock(g->sample_rate);
     want_scan_coefs = !dry || plan_digest_wanted();
     pending.clear();
     for (uint32_t id : ord.ordered) {
@@ -3760,6 +3759,12 @@ struct GroupPlan {  // result of phase B for one group
         IirPatch p;      // device addresses set
     };
     std::vector<IirEntry> iir_patches;
+    struct SchedEntry {
+        uint32_t graph;  // batch position
+        wae_node_id node;
+        SchedPatch p;    // device address set
+    };
+    std::vector<SchedEntry> sched_patches;
 };
 
 static int64_t padded_length(const wae_graph* g) { return (int64_t)((g->length + 127) / 128 * 128); }
@@ -4391,6 +4396,22 @@ static void prep_plan_group(wae_batch* b, wae_graph* const* graphs, int k, PrepS
                     }
                     gp.iir_patches.push_back({ip.graph, ip.node, p});
                 }
+                // patch entries of schedules bound from device memory: the record whose fields the times reach
+                size_t sched_rec_size = 0;
+                switch (s.kind) {
+                    case S_CHAIN: case S_VSUM: sched_rec_size = sizeof(ChainInst); break;
+                    case S_OSC: sched_rec_size = sizeof(OscInst); break;
+                    case S_OSC_AR: sched_rec_size = sizeof(OscArInst); break;
+                    case S_CONST: sched_rec_size = sizeof(ConstInst); break;
+                    case S_META: sched_rec_size = sizeof(MetaInst); break;
+                    case S_ABSN_BOUND: sched_rec_size = sizeof(AbsnBoundInst); break;
+                    case S_ABSN_SERIAL: sched_rec_size = sizeof(AbsnSerialInst); break;
+                }
+                for (const auto& sp : s.sched_patches) {
+                    SchedPatch p = sp.p;
+                    p.dst = static_cast<char*>(st.d_a) + (size_t)sp.rec * sched_rec_size + sp.off;
+                    gp.sched_patches.push_back({sp.graph, sp.node, p});
+                }
             }
         }
         gp.seg_ranges.push_back({seg_stage0, gp.stages.size()});
@@ -4564,6 +4585,39 @@ static wae_status record_iirs(wae_batch* b, wae_graph* const* graphs, uint32_t n
     return WAE_OK;
 }
 
+// The declared schedules of the batch (`graphs` in batch order, each in graph and node order), after planning, with the patch entries of
+// the planned groups gathered per source and uploaded (from `patches`, which the caller keeps alive until the stream has been
+// synchronised).  The ones the planner reached are unbound; the ones it never reached have no entries: binding them is validated and
+// writes nothing, and runs do not wait for them.
+static wae_status record_schedules(wae_batch* b, wae_graph* const* graphs, uint32_t n_graphs, const std::vector<GroupPlan>& gps,
+                                   std::vector<SchedPatch>& patches) {
+    for (uint32_t j = 0; j < n_graphs; j++) {
+        if (!graphs[j]->device_schedules) continue;
+        for (const auto& kv : graphs[j]->nodes) {  // (a graph with a declaration has no suspend point)
+            const Node& nd = kv.second;
+            if (!nd.device_schedule || b->schedule_index.count({j, nd.id})) continue;
+            b->schedule_index[{j, nd.id}] = b->schedules.size();
+            b->schedules.push_back(wae_batch::DevSchedule{j, nd.id, nd.sched_stop, {nd.sched_lo[0], nd.sched_lo[1]},
+                                                          {nd.sched_hi[0], nd.sched_hi[1]}, 0, 0, false});
+        }
+    }
+    std::vector<std::vector<SchedPatch>> per(b->schedules.size());
+    for (const auto& gp : gps)
+        for (const auto& e : gp.sched_patches) per[b->schedule_index.at({e.graph, e.node})].push_back(e.p);
+    b->schedules_unbound = 0;
+    for (size_t k = 0; k < per.size(); k++) {
+        wae_batch::DevSchedule& d = b->schedules[k];
+        d.p0 = (int32_t)patches.size();
+        patches.insert(patches.end(), per[k].begin(), per[k].end());
+        d.p1 = (int32_t)patches.size();
+        d.bound = d.p0 == d.p1;  // (never reached: nothing to wait for)
+        b->schedules_unbound += d.bound ? 0 : 1;
+    }
+    if (!patches.empty() && !(b->d_sched_patches = b->dupload_now(patches)))
+        return fail(WAE_OUT_OF_MEMORY, "out of device memory (schedule patch entries)");
+    return WAE_OK;
+}
+
 // The declared value curves of the batch (`graphs` in batch order), after planning: each named by the (node, param index) it was declared
 // through, the ones the planner gave a pool unbound, in graph, node and param order; then the declared ones it never lowered, which
 // binding validates and writes nothing to, and which runs do not wait for.
@@ -4601,9 +4655,15 @@ static void record_value_curves(wae_batch* b, wae_graph* const* graphs, uint32_t
     }
 }
 
-// runs of a batch need every device input, param, response, curve, periodic wave, IIR coefficient set and value curve bound once
+// runs of a batch need every device input, param, response, curve, periodic wave, IIR coefficient set, value curve and schedule bound once
 static wae_status check_bound(wae_batch* b) {
     if (!b) return fail(WAE_INVALID_ARGUMENT, "null batch");
+    for (size_t k = 0; b->schedules_unbound && k < b->schedules.size(); k++)
+        if (const auto& d = b->schedules[k]; !d.bound) {
+            const uint32_t caller = b->order.empty() ? d.graph : b->order[d.graph];
+            return fail(WAE_INVALID_STATE, "schedule bound from device memory never bound: graph " + std::to_string(caller) + ", node " +
+                                               std::to_string(d.node) + " (wae_batch_bind_schedules)");
+        }
     for (size_t k = 0; b->value_curves_unbound && k < b->value_curves.size(); k++)
         if (const auto& d = b->value_curves[k]; !d.bound) {
             const uint32_t caller = b->order.empty() ? d.graph : b->order[d.graph];
@@ -4756,10 +4816,12 @@ static wae_status prepare_impl(wae_engine* eng, wae_graph* const* graphs, uint32
     record_value_curves(b, graphs, n_graphs);
     std::vector<CurvePatch> curve_patches;
     std::vector<IirPatch> iir_patches;
+    std::vector<SchedPatch> sched_patches;
     std::vector<ParamSlotInfo> slot_info;
     std::vector<ParamPatch> patches;
     st = record_curves(b, graphs, n_graphs, gps, curve_patches);
     if (st == WAE_OK) st = record_iirs(b, graphs, n_graphs, gps, iir_patches);
+    if (st == WAE_OK) st = record_schedules(b, graphs, n_graphs, gps, sched_patches);
     if (st == WAE_OK) st = record_params(b, graphs, n_graphs, gps, slot_info, patches);
     if (st != WAE_OK) {
         wae_batch_destroy(b);
@@ -5531,6 +5593,52 @@ WAE_API wae_status wae_batch_bind_iir_coefficients(wae_batch* b, const wae_iir_b
     return WAE_OK;
 }
 
+// The schedule fields are rewritten on the engine stream: runs queued before the bind have read the previous ones.
+WAE_API wae_status wae_batch_bind_schedules(wae_batch* b, const wae_schedule_binding* items, uint32_t n, void* stream) {
+    if (!b || (n && !items)) return fail(WAE_INVALID_ARGUMENT, "null batch / items");
+    if (n == 0) return WAE_OK;
+    CUDA_TRY(cudaSetDevice(b->engine->device));
+    // every item is validated before anything is enqueued
+    std::vector<SchedBindItem> table;
+    std::vector<size_t> schedule_of;
+    std::vector<char> named(b->schedules.size(), 0);
+    BindExtents extents{b->engine->device, {}};
+    for (uint32_t i = 0; i < n; i++) {
+        const wae_schedule_binding& it = items[i];
+        if (it.graph_index >= b->n_graphs)
+            return fail(WAE_INVALID_STATE, "bind: graph index " + std::to_string(it.graph_index) + " is out of range");
+        auto si = b->schedule_index.find({b->batch_pos(it.graph_index), it.node});
+        const std::string name = "node " + std::to_string(it.node) + " of graph " + std::to_string(it.graph_index);
+        if (si == b->schedule_index.end())
+            return fail(WAE_INVALID_STATE, "bind: " + name + " has no schedule bound from device memory (wae_source_set_device_schedule)");
+        const size_t k = si->second;
+        if (named[k]++)  // (two items of one launch writing one source's records: which one lands would be undefined)
+            return fail(WAE_INVALID_ARGUMENT, "bind: " + name + " is named twice in one call");
+        const wae_batch::DevSchedule& d = b->schedules[k];
+        if (!it.times) return fail(WAE_INVALID_ARGUMENT, "bind: null times");
+        if ((uintptr_t)it.times % alignof(double)) return fail(WAE_INVALID_ARGUMENT, "bind: times is not 8-byte aligned");
+        wae_status st = extents.check(it.times, (d.bind_stop ? 2 : 1) * sizeof(double), "times",
+                                      "[times, times + count) runs past the end of its allocation");
+        if (st != WAE_OK) return st;
+        if (d.p0 == d.p1) continue;  // declared, never rendered: nothing to write
+        table.push_back(SchedBindItem{it.times, b->d_sched_patches + d.p0, {d.lo[0], d.lo[1]}, {d.hi[0], d.hi[1]}, d.p1 - d.p0, d.bind_stop ? 1 : 0});
+        schedule_of.push_back(k);
+    }
+    if (table.empty()) return WAE_OK;
+    wae_status st = bind_after(b, stream);
+    if (st == WAE_OK) st = stage_bind_table(b, table.data(), table.size() * sizeof(SchedBindItem));
+    if (st != WAE_OK) return st;
+    launch_bind_schedules(static_cast<const SchedBindItem*>(b->d_bind), (int)table.size(), b->engine->stream);
+    cudaError_t le = cudaGetLastError();
+    if (le != cudaSuccess) return fail(WAE_CUDA_ERROR, std::string("bind: ") + cudaGetErrorString(le));
+    for (size_t k : schedule_of)
+        if (!b->schedules[k].bound) {
+            b->schedules[k].bound = true;
+            b->schedules_unbound--;
+        }
+    return WAE_OK;
+}
+
 // The declared values are rewritten on the engine stream: runs queued before the bind have read the previous ones.
 WAE_API wae_status wae_batch_bind_value_curves(wae_batch* b, const wae_value_curve_binding* items, uint32_t n, void* stream) {
     if (!b || (n && !items)) return fail(WAE_INVALID_ARGUMENT, "null batch / items");
@@ -6052,6 +6160,9 @@ static wae_status refuse_device_inputs(wae_graph* const* graphs, uint32_t n_grap
         if (graphs[i] && graphs[i]->device_value_curves)
             return fail(WAE_INVALID_STATE, "graph " + std::to_string(i) + " has value curves bound from device memory: render it with "
                                            "wae_batch_prepare (or _prepare_many), wae_batch_bind_value_curves and wae_batch_run");
+        if (graphs[i] && graphs[i]->device_schedules)
+            return fail(WAE_INVALID_STATE, "graph " + std::to_string(i) + " has schedules bound from device memory: render it with "
+                                           "wae_batch_prepare (or _prepare_many), wae_batch_bind_schedules and wae_batch_run");
     }
     return WAE_OK;
 }

@@ -149,6 +149,12 @@ struct Node {
     bool normalize_next = true;                 // ConvolverNode::set_normalize: applies to the next set_buffer (convolver.rs:325-328)
     double start_time = 1.7976931348623157e308, stop_time = 1.7976931348623157e308;
     double offset = 0., duration = 1.7976931348623157e308;
+    // wae_source_set_device_schedule: the start time (and, with sched_stop, the stop time) is written per run by wae_batch_bind_schedules,
+    // clamped to [sched_lo, sched_hi] (index 0: start, 1: stop).  start_time / stop_time hold the windows' low ends: the plan is made
+    // with them, always with a gated output layout, so no planning decision depends on the bound times.
+    bool device_schedule = false;
+    bool sched_stop = false;
+    double sched_lo[2] = {0., 0.}, sched_hi[2] = {0., 0.};
     bool loop = false;
     double loop_start = 0., loop_end = 0.;
     double max_delay_time = 1.;
@@ -275,6 +281,7 @@ struct wae_graph {
     uint32_t device_waves = 0;      // OscillatorNodes declared with wae_oscillator_set_device_periodic_wave
     uint32_t device_iirs = 0;       // IIRFilterNodes declared with wae_iir_filter_set_device_coefficients
     uint32_t device_value_curves = 0;  // AudioParams declared with wae_param_set_device_value_curve
+    uint32_t device_schedules = 0;     // scheduled sources declared with wae_source_set_device_schedule
 
     uint32_t create_param(uint32_t owner, float def, float mn, float mx, bool a_rate, float initial, bool send_set_value = true,
                           bool fixed_id = false, uint32_t id = 0, bool constrained = false);

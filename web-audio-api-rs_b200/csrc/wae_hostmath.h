@@ -98,42 +98,6 @@ inline std::vector<float> sine_table() {
     return t;
 }
 
-inline double unroll_phase(double p) { return p >= 1. ? p - 1. : (p < 0. ? p + 1. : p); }
-
-// Sample-accurate scheduling of AudioScheduledSourceNodes.  The reference walks quanta
-// (current_time = frame / sample_rate, src/render/thread.rs:357-360) and, inside the quantum that contains a
-// start/stop time, accumulates `current_time += dt` per frame (oscillator.rs:511-557, constant_source.rs:231-246).
-// first_frame_at_or_after(T) returns the first frame whose accumulated time is >= T, reproducing that walk.
-struct SchedClock {
-    double sample_rate, dt;
-    explicit SchedClock(float sr) : sample_rate((double)sr), dt(1. / (double)sr) {}
-    double block_time(int64_t q) const { return (double)(q * 128) / sample_rate; }
-    double next_block_time(int64_t q) const { return block_time(q) + dt * 128.; }
-    // first quantum whose next_block_time is > T (i.e. the node is not skipped by `T >= next_block_time`)
-    int64_t quantum_containing(double T) const {
-        if (!(T < 1e15)) return std::numeric_limits<int64_t>::max() / 256;
-        int64_t q = (int64_t)std::floor(T * sample_rate / 128.) - 2;
-        if (q < 0) q = 0;
-        while (!(T < next_block_time(q))) q++;
-        return q;
-    }
-    // returns frame index; *time_out = accumulated time of that frame
-    int64_t first_frame_at_or_after(double T, double* time_out = nullptr) const {
-        int64_t q = quantum_containing(T);
-        if (q >= std::numeric_limits<int64_t>::max() / 512) return std::numeric_limits<int64_t>::max();
-        double t = block_time(q);
-        for (int i = 0; i < 128; i++) {
-            if (t >= T) {
-                if (time_out) *time_out = t;
-                return q * 128 + i;
-            }
-            t += dt;
-        }
-        if (time_out) *time_out = block_time(q + 1);
-        return (q + 1) * 128;
-    }
-};
-
 // get_stereo_gains, src/node/stereo_panner.rs:74-79
 inline void stereo_gains(float x, float& gl, float& gr) {
     gl = sinf((1.f - x) * PI32 / 2.f);

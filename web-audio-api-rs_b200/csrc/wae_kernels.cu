@@ -4590,6 +4590,74 @@ __global__ void __launch_bounds__(256) k_bind_value_curves(const ValueCurveBindI
     }
 }
 
+// ---- wae_batch_bind_schedules: one thread per item -----------------------------------------------------------------------------------
+// The times are clamped to their windows, then every record field they reach is derived with the planner's functions (wae_kernels.h):
+// f64 without transcendentals or contraction, so each field gets the bits a host-built plan of those times holds.  The frame walks are
+// sequential (the slow track's start is sticky within almost_equal) and run once per bind.
+DEVI double sched_clamp(double v, double lo, double hi) { return v != v ? lo : (v < lo ? lo : (v > hi ? hi : v)); }
+__global__ void __launch_bounds__(128) k_bind_schedules(const SchedBindItem* __restrict__ items, int n_items) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n_items) return;
+    const SchedBindItem it = items[i];
+    const double start = sched_clamp(it.times[0], it.lo[0], it.hi[0]);
+    const double bound_stop = it.bind_stop ? sched_clamp(it.times[1], it.lo[1], it.hi[1]) : 0.;
+    for (int k = 0; k < it.n_patches; k++) {
+        const SchedPatch p = it.patches[k];
+        const double stop = it.bind_stop ? bound_stop : p.stop_time;
+        const SchedClock clock(p.sample_rate);
+        char* d = static_cast<char*>(p.dst);
+        switch (p.kind) {
+            case SCHED_OSC:
+            case SCHED_OSC_AR:
+            case SCHED_META_OSC: {
+                const OscStart s = osc_start(clock, start, p.incr, p.flag != 0);
+                const int64_t n_stop = osc_stop_frame(clock, stop);
+                if (p.kind == SCHED_META_OSC) {
+                    reinterpret_cast<MetaInst*>(d)->n_first = s.n_first;
+                    reinterpret_cast<MetaInst*>(d)->n_stop = n_stop;
+                    break;
+                }
+                OscInst* o = p.kind == SCHED_OSC_AR ? &reinterpret_cast<OscArInst*>(d)->base : reinterpret_cast<OscInst*>(d);
+                o->n_first = s.n_first;
+                o->n_stop = n_stop;
+                o->phase0 = s.phase0;
+                if (p.kind == SCHED_OSC_AR) reinterpret_cast<OscArInst*>(d)->start_ratio = s.start_ratio;
+                break;
+            }
+            case SCHED_CONST:
+            case SCHED_META_CONST: {
+                const int64_t n_first = clock.first_frame_at_or_after(start);
+                const int64_t n_stop = stop < 1e300 ? clock.first_frame_at_or_after(stop) : SCHED_NEVER;
+                if (p.kind == SCHED_META_CONST) {
+                    reinterpret_cast<MetaInst*>(d)->n_first = n_first;
+                    reinterpret_cast<MetaInst*>(d)->n_stop = n_stop;
+                } else {
+                    reinterpret_cast<ConstInst*>(d)->n_first = n_first;
+                    reinterpret_cast<ConstInst*>(d)->n_stop = n_stop;
+                }
+                break;
+            }
+            case SCHED_ABSN_BOUND: {
+                AbsnBoundInst* r = reinterpret_cast<AbsnBoundInst*>(d);
+                const int64_t q = absn_start_quantum(clock, start);
+                const bool aligned = start <= clock.block_time(q) && p.offset == 0.;
+                const AbsnStart st = absn_start(clock, start, stop);
+                r->s.n_first = st.n_first;
+                r->s.n_stop = st.n_stop;
+                r->start_delta = st.t_first - st.start;
+                r->n_start = q * 128;
+                r->fast_end = absn_fast_end(clock, p.lq, q * 128, p.duration);
+                r->fast_ok = aligned && p.flag && stop > 1e300;
+                break;
+            }
+            case SCHED_ABSN_SERIAL:
+                reinterpret_cast<AbsnSerialInst*>(d)->start_time = start;
+                reinterpret_cast<AbsnSerialInst*>(d)->stop_time = stop;
+                break;
+        }
+    }
+}
+
 // Host emulation of the transforms above with the SAME butterfly, index and twiddle code (tests/test_conv_fft_host.py pins them against
 // numpy on a machine without a GPU).  mode 0: complex forward, natural -> position order; 1: complex inverse, position -> natural order
 // (unnormalised); 2: 2B reals -> B packed bins in position order; 3: B packed bins -> 2B reals (scaled by 1 / 2B).  data: 2B floats in place.
@@ -5141,6 +5209,7 @@ void launch_bind_value_curves(const ValueCurveBindItem* d, int n, int64_t max_le
     const int64_t bx = std::max<int64_t>(1, std::min<int64_t>((max_len + VC_TILE - 1) / VC_TILE, 65535));
     k_bind_value_curves<<<dim3((unsigned)bx, (unsigned)std::min(n, 65535)), 256, 0, s>>>(d, n);
 }
+void launch_bind_schedules(const SchedBindItem* d, int n, cudaStream_t s) { k_bind_schedules<<<(unsigned)((n + 127) / 128), 128, 0, s>>>(d, n); }
 void launch_conv_ir_fft(const float* ir, int64_t ir_len, int64_t ir_stride, float2* h, int S, int channels, cudaStream_t s) {
     conv_configure();
     k_conv_ir_fft<<<dim3((unsigned)S, (unsigned)channels), CV_THREADS, CV_SMEM_ELEMS * sizeof(float2), s>>>(ir, ir_len, ir_stride, h, S);

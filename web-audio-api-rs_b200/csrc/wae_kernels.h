@@ -95,7 +95,144 @@ WAE_HD AbsnSlowDerived absn_slow_derive(double dt, double computed_rate, double 
     return d;
 }
 
-void upload_twiddles();                          // convolver FFT tables (computed in wae_kernels.cu, f64 -> f32)
+// ---- Sample-accurate scheduling of AudioScheduledSourceNodes, in f64 without transcendentals: one source for the planner (host, times
+// given when the graph is built) and for k_bind_schedules (device, times bound from device memory, wae_batch_bind_schedules).  The build
+// compiles without FMA contraction on both sides, so equal times give bit-equal frames and phases.
+constexpr int64_t SCHED_NEVER = 0x7fffffffffffffffll;
+WAE_HD bool almost_equal(double x, double y) {  // `almost` crate 0.2: absolute or relative sqrt(eps)
+    if (x == y) return true;
+    const double tol = 1.4901161193847656e-8;
+    const double d = fabs(y - x), m = fabs(x) < fabs(y) ? fabs(y) : fabs(x);
+    return d <= tol || d <= m * tol;
+}
+// The reference walks quanta (current_time = frame / sample_rate, src/render/thread.rs:357-360) and, inside the quantum that contains a
+// start/stop time, accumulates `current_time += dt` per frame (oscillator.rs:511-557, constant_source.rs:231-246).
+// first_frame_at_or_after(T) returns the first frame whose accumulated time is >= T, reproducing that walk.
+struct SchedClock {
+    double sample_rate, dt;
+    WAE_HD explicit SchedClock(float sr) : sample_rate((double)sr), dt(1. / (double)sr) {}
+    WAE_HD double block_time(int64_t q) const { return (double)(q * 128) / sample_rate; }
+    WAE_HD double next_block_time(int64_t q) const { return block_time(q) + dt * 128.; }
+    // first quantum whose next_block_time is > T (i.e. the node is not skipped by `T >= next_block_time`)
+    WAE_HD int64_t quantum_containing(double T) const {
+        if (!(T < 1e15)) return SCHED_NEVER / 256;
+        int64_t q = (int64_t)floor(T * sample_rate / 128.) - 2;
+        if (q < 0) q = 0;
+        while (!(T < next_block_time(q))) q++;
+        return q;
+    }
+    // returns frame index; *time_out = accumulated time of that frame
+    WAE_HD int64_t first_frame_at_or_after(double T, double* time_out = nullptr) const {
+        int64_t q = quantum_containing(T);
+        if (q >= SCHED_NEVER / 512) return SCHED_NEVER;
+        double t = block_time(q);
+        for (int i = 0; i < 128; i++) {
+            if (t >= T) {
+                if (time_out) *time_out = t;
+                return q * 128 + i;
+            }
+            t += dt;
+        }
+        if (time_out) *time_out = block_time(q + 1);
+        return (q + 1) * 128;
+    }
+};
+// OscillatorNode (oscillator.rs:391-428,511-540): the first rendered frame and its phase (`incr` = computed frequency / sample rate), and
+// the sub-sample start (t_first - start) / dt that the a-rate kernel adds its own increment with
+struct OscStart {
+    int64_t n_first;
+    double phase0, start_ratio;
+};
+WAE_HD OscStart osc_start(const SchedClock& clock, double start_time, double incr, bool outside_nyquist) {
+    OscStart r{0, 0., 0.};
+    const int64_t q = clock.quantum_containing(start_time);
+    double start = start_time;
+    if (start < clock.block_time(q)) start = clock.block_time(q);  // "prevent scheduling in the past"
+    double cur = clock.block_time(q);  // the accumulated per-frame clock of that quantum
+    int i = 0;
+    for (; i < 128; i++) {
+        if (!(cur < start)) break;
+        cur += clock.dt;
+    }
+    r.n_first = q * 128 + i;
+    if (i < 128 && cur > start) {
+        const double ratio = (cur - start) / clock.dt;
+        r.start_ratio = ratio;
+        double ph = incr * ratio;
+        if (outside_nyquist) {
+            ph = fmod(ph, 1.);
+            if (ph < 0.) ph += 1.;
+        } else {
+            ph = ph >= 1. ? ph - 1. : (ph < 0. ? ph + 1. : ph);  // unroll_phase
+        }
+        r.phase0 = ph;
+    }
+    return r;
+}
+WAE_HD int64_t osc_stop_frame(const SchedClock& clock, double stop_time) {
+    if (!(stop_time < 1e300)) return SCHED_NEVER;
+    const int64_t qs = clock.quantum_containing(stop_time);
+    return stop_time <= clock.block_time(qs) ? qs * 128 : clock.first_frame_at_or_after(stop_time);
+}
+// AudioBufferSourceNode: the quantum its start time falls in.  A start time that IS the next block boundary but compares below
+// next_block_time by one rounding: the reference goes through one all-silent slow-track quantum, then aligns (audio_buffer_source.rs:521-523)
+WAE_HD int64_t absn_start_quantum(const SchedClock& clock, double start_time) {
+    int64_t q = clock.quantum_containing(start_time);
+    if (start_time > clock.block_time(q) && start_time == clock.block_time(q + 1)) q = q + 1;
+    return q;
+}
+// the slow track's first playing frame: current_time = block_time + i * dt (:648), sticky within almost::equal (:652-654); the first
+// frame with current_time >= stop_time (:663)
+struct AbsnStart {
+    int64_t n_first, n_stop;
+    double t_first, start;  // the time of frame n_first, the start time (snapped to it when almost equal)
+};
+WAE_HD AbsnStart absn_start(const SchedClock& clock, double start_time, double stop_time) {
+    AbsnStart r{-1, SCHED_NEVER, 0., start_time};
+    int64_t qq = clock.quantum_containing(r.start);
+    for (int guard = 0; guard < 3 && r.n_first < 0; guard++, qq++) {
+        const double bt0 = clock.block_time(qq);
+        for (int i = 0; i < 128; i++) {
+            const double t = bt0 + (double)i * clock.dt;
+            if (almost_equal(t, r.start)) r.start = t;
+            if (!(t < r.start)) {
+                r.n_first = qq * 128 + i;
+                r.t_first = t;
+                break;
+            }
+        }
+    }
+    if (r.n_first < 0) r.n_first = qq * 128;
+    if (stop_time < 1e300) {
+        const int64_t qs = clock.quantum_containing(stop_time);
+        int64_t ns = (qs + 1) * 128;
+        const double bt0 = clock.block_time(qs);
+        for (int i = 0; i < 128; i++)
+            if (bt0 + (double)i * clock.dt >= stop_time) {
+                ns = qs * 128 + i;
+                break;
+            }
+        r.n_stop = ns;
+    }
+    return r;
+}
+// the fast track of a non-looping source: the frame after the quantum in which it has `ended`.  The reference accumulates
+// buffer_time += block_duration and stops once it reaches the buffer's duration (audio_buffer_source.rs:609,826-838) — replayed, not
+// divided.  lq: the render length the walk stops after.
+WAE_HD int64_t absn_fast_end(const SchedClock& clock, int64_t lq, int64_t n_start, double duration) {
+    const double block_duration = clock.dt * 128.;
+    const int64_t max_q = (lq - n_start) / 128 + 2;
+    int64_t played = 0;
+    double bt = 0.;
+    while (played < max_q) {
+        bt += block_duration;
+        played++;
+        if (bt >= duration) break;
+    }
+    return n_start + played * 128;
+}
+
+void upload_twiddles();                         // convolver FFT tables (computed in wae_kernels.cu, f64 -> f32)
 void conv_fft_selftest(float* data, int mode);   // host emulation of the convolver transforms (wae_selftest_conv_fft)
 void launch_oscillator(const OscInst* d, int n, ChunkInfo ci, cudaStream_t s);
 void launch_constant(const ConstInst* d, int n, ChunkInfo ci, cudaStream_t s);
@@ -155,6 +292,8 @@ void launch_bind_waves(const WaveBindItem* d, int n, int max_len, bool any_norma
 void launch_bind_iir(const IirBindItem* d, int n, cudaStream_t s);
 // a bind of n param value curves (k_bind_value_curves): each item's values copied bit for bit, max_len = the longest
 void launch_bind_value_curves(const ValueCurveBindItem* d, int n, int64_t max_len, cudaStream_t s);
+// a bind of n start / stop times (k_bind_schedules, one thread per item): clamped, then every patch entry of each item re-derived
+void launch_bind_schedules(const SchedBindItem* d, int n, cudaStream_t s);
 void launch_conv_ir_fft(const float* ir, int64_t ir_len, int64_t ir_stride, float2* h, int S, int channels, cudaStream_t s);
 
 }  // namespace wae
