@@ -510,16 +510,18 @@ WAE_API wae_status wae_buffer_source_set_device_input(wae_graph* graph, wae_node
 typedef struct wae_source_binding {
     uint32_t graph_index;    /* caller's index, as wae_batch_fetch_graph (also for wae_batch_prepare_many batches) */
     wae_node_id node;        /* a node declared with wae_buffer_source_set_device_input */
-    const float* pcm;        /* device memory on the engine's GPU: channel c is `length` floats at pcm + c * channel_stride */
-    uint64_t channel_stride; /* floats, >= the declared length; any alignment */
+    const float* pcm;        /* device memory on the engine's GPU, 4-byte aligned: channel c is `length` floats at
+                                pcm + c * channel_stride */
+    uint64_t channel_stride; /* floats, >= the declared length; channels need no 16-byte alignment */
 } wae_source_binding;
 
 /* Copies the audio into the batch's source slab, asynchronously on the engine stream, after the work already queued on `stream`
  * (a cudaStream_t of the engine's device, or cudaStreamLegacy for the legacy default stream, or cudaStreamPerThread; NULL = no extra
  * ordering: the engine stream is non-blocking and does NOT wait for the legacy default stream by itself).  All-or-nothing: every item
  * is validated before anything is enqueued.  Bound audio stays until it is bound again; runs never alter it.  A device input that is
- * never started renders silence and reads nothing: binding it is validated and copies nothing.  WAE_INVALID_ARGUMENT: `pcm` is not
- * device (or managed) memory of the engine's GPU, or the extent [pcm, pcm + (channels - 1) * channel_stride + length) does not lie
+ * never started renders silence and reads nothing: binding it is validated and copies nothing.  WAE_INVALID_ARGUMENT: `pcm` is null,
+ * not 4-byte aligned or not device (or managed) memory of the engine's GPU, or the extent
+ * [pcm, pcm + (channels - 1) * channel_stride + length) does not lie
  * inside one allocation, or channel_stride is below the declared length, or one (graph, node) is named twice in the call.
  * WAE_INVALID_STATE: graph_index out of range, or the node is not a device input.
  * wae_batch_run, wae_batch_run_group and wae_batch_run_pipelined answer WAE_INVALID_STATE while a device input of the batch has never
@@ -551,14 +553,15 @@ typedef struct wae_param_binding {
     uint32_t graph_index;  /* caller's index, as wae_batch_fetch_graph */
     wae_node_id node;      /* the param's node */
     uint32_t param_index;  /* declared with wae_param_set_device_value */
-    const float* value;    /* one float of device (or managed) memory on the engine's GPU */
+    const float* value;    /* one float of device (or managed) memory on the engine's GPU, 4-byte aligned */
 } wae_param_binding;
 
 /* Reads the values on the device, asynchronously on the engine stream after the work already queued on `stream` (as
  * wae_batch_bind_sources), and re-derives every planned record they reach (filter coefficients and scan constants, gain products,
  * panner gains, compressor settings) in every render segment.  All-or-nothing: every item is validated before anything is enqueued.
- * Bound values stay until they are bound again.  WAE_INVALID_ARGUMENT: `value` is not device (or managed) memory of the engine's GPU or
- * its 4 bytes are not in one allocation, or one param is named twice in the call.  WAE_INVALID_STATE: graph_index out of range, or the
+ * Bound values stay until they are bound again.  WAE_INVALID_ARGUMENT: `value` is null, not 4-byte aligned, not device (or managed)
+ * memory of the engine's GPU or its 4 bytes are not in one allocation, or one param is named twice in the call.  WAE_INVALID_STATE:
+ * graph_index out of range, or the
  * param was not declared.  wae_batch_run, wae_batch_run_group and wae_batch_run_pipelined answer WAE_INVALID_STATE while a declared
  * param of the batch has never been bound. */
 WAE_API wae_status wae_batch_bind_params(wae_batch* batch, const wae_param_binding* items, uint32_t n, void* stream);
@@ -580,13 +583,15 @@ WAE_API wae_status wae_convolver_set_device_response(wae_graph* graph, wae_node_
 typedef struct wae_response_binding {
     uint32_t graph_index;    /* caller's index, as wae_batch_fetch_graph */
     wae_node_id node;        /* declared with wae_convolver_set_device_response */
-    const float* pcm;        /* device memory of the engine's GPU: channel c is `length` floats at pcm + c * channel_stride */
-    uint64_t channel_stride; /* floats, >= the declared length; any alignment */
+    const float* pcm;        /* device memory of the engine's GPU, 4-byte aligned: channel c is `length` floats at
+                                pcm + c * channel_stride */
+    uint64_t channel_stride; /* floats, >= the declared length; channels need no 16-byte alignment */
 } wae_response_binding;
 
 /* Normalises, trims and transforms the responses on the device, asynchronously on the engine stream after the work already queued on
  * `stream` (as wae_batch_bind_sources).  All-or-nothing: every item is validated before anything is enqueued.  A bound response stays
- * until it is bound again.  WAE_INVALID_ARGUMENT: `pcm` is not device (or managed) memory of the engine's GPU, the extent does not lie
+ * until it is bound again.  WAE_INVALID_ARGUMENT: `pcm` is null, not 4-byte aligned or not device (or managed) memory of the engine's
+ * GPU, the extent does not lie
  * in one allocation, channel_stride is below the declared length, one (graph, node) is named twice in the call, or the call has more
  * than 65535 items that the batch renders.  WAE_INVALID_STATE:
  * graph_index out of range, or the node was not declared.  wae_batch_run, wae_batch_run_group and wae_batch_run_pipelined answer
@@ -607,12 +612,13 @@ WAE_API wae_status wae_wave_shaper_set_device_curve(wae_graph* graph, wae_node_i
 typedef struct wae_curve_binding {
     uint32_t graph_index;   /* caller's index, as wae_batch_fetch_graph */
     wae_node_id node;       /* declared with wae_wave_shaper_set_device_curve */
-    const float* curve;     /* device memory of the engine's GPU: `length` floats, any alignment */
+    const float* curve;     /* device memory of the engine's GPU: `length` floats, 4-byte aligned */
 } wae_curve_binding;
 
 /* Copies the curves into the batch, asynchronously on the engine stream after the work already queued on `stream` (as
  * wae_batch_bind_sources).  The values are used bit for bit, NaN and infinities included.  All-or-nothing: every item is validated before
- * anything is enqueued.  A bound curve stays until it is bound again.  WAE_INVALID_ARGUMENT: `curve` is null or not device (or managed)
+ * anything is enqueued.  A bound curve stays until it is bound again.  WAE_INVALID_ARGUMENT: `curve` is null, not 4-byte aligned or
+ * not device (or managed)
  * memory of the engine's GPU, [curve, curve + length) does not lie in one allocation, or one (graph, node) is named twice in the call.
  * WAE_INVALID_STATE: graph_index out of range, or the node was not declared.  wae_batch_run, wae_batch_run_group and
  * wae_batch_run_pipelined answer WAE_INVALID_STATE while a declared curve of the batch has never been bound. */
@@ -634,14 +640,15 @@ WAE_API wae_status wae_oscillator_set_device_periodic_wave(wae_graph* graph, wae
 typedef struct wae_periodic_wave_binding {
     uint32_t graph_index;   /* caller's index, as wae_batch_fetch_graph */
     wae_node_id node;       /* declared with wae_oscillator_set_device_periodic_wave */
-    const float* real;      /* device memory of the engine's GPU: `coefficients` floats, or NULL (= zeros) */
+    const float* real;      /* device memory of the engine's GPU: `coefficients` floats, 4-byte aligned, or NULL (= zeros) */
     const float* imag;      /* likewise; not both NULL */
 } wae_periodic_wave_binding;
 
 /* Synthesises the wavetables into the batch, asynchronously on the engine stream after the work already queued on `stream` (as
  * wae_batch_bind_sources).  real[0] and imag[0] (DC) are ignored, as PeriodicWave ignores them.  All-or-nothing: every item is validated
  * before anything is enqueued.  A bound wave stays until it is bound again.  WAE_INVALID_ARGUMENT: `real` and `imag` are both null, one
- * of them is not device (or managed) memory of the engine's GPU or does not hold `coefficients` floats in one allocation, or one
+ * of them is not 4-byte aligned, not device (or managed) memory of the engine's GPU or does not hold `coefficients` floats in one
+ * allocation, or one
  * (graph, node) is named twice in the call.  WAE_INVALID_STATE: graph_index out of range, or the node was not declared.  wae_batch_run,
  * wae_batch_run_group and wae_batch_run_pipelined answer WAE_INVALID_STATE while a declared wave of the batch has never been bound. */
 WAE_API wae_status wae_batch_bind_periodic_waves(wae_batch* batch, const wae_periodic_wave_binding* items, uint32_t n, void* stream);

@@ -840,8 +840,7 @@ class Batch:
         graphs (graphs built the same way share ids) or one per graph.  One call, ordered after torch's current stream (its default
         stream included); the copy runs on the engine stream, and the tensor's memory is kept from reuse until it has (record_stream)."""
         items, n = self._pcm_items("bind_sources", "pcm", nodes, pcm, graphs, "_device_inputs", B.SourceBinding)
-        self.api.check(self.api.batch_bind_sources(self.handle, items, n, C.c_void_p(self._torch_stream_handle())))
-        self._keep_until_read(pcm)
+        self._bind(self.api.batch_bind_sources, items, n, pcm)
 
     def bind_responses(self, nodes, ir, graphs=None):
         """wae_batch_bind_responses: ir[k] ([channels][length] of a float32 CUDA tensor [n][channels][length], unit stride on the last
@@ -849,8 +848,7 @@ class Batch:
         (default: 0..n-1).  `nodes` as for bind_sources.  One call, ordered after torch's current stream; the response is normalised,
         trimmed and transformed on the engine stream, and the tensor's memory is kept from reuse until it has been read."""
         items, n = self._pcm_items("bind_responses", "ir", nodes, ir, graphs, "_device_responses", B.ResponseBinding)
-        self.api.check(self.api.batch_bind_responses(self.handle, items, n, C.c_void_p(self._torch_stream_handle())))
-        self._keep_until_read(ir)
+        self._bind(self.api.batch_bind_responses, items, n, ir)
 
     def bind_curves(self, nodes, curves, graphs=None):
         """wae_batch_bind_curves: curves[k] (a row of a float32 CUDA tensor [n][length], unit stride on the last dimension) becomes the
@@ -873,8 +871,7 @@ class Batch:
                 raise B.WaeError(1, f"bind_curves: curves[{k}] has {curves.shape[1]} points, node {nid} of graph {g} was declared with "
                                     f"{declared}")
             items[k] = B.CurveBinding(g, int(nid), C.cast(C.c_void_p(base + 4 * k * curves.stride(0)), B.c_float_p))
-        self.api.check(self.api.batch_bind_curves(self.handle, items, n, C.c_void_p(self._torch_stream_handle())))
-        self._keep_until_read(curves)
+        self._bind(self.api.batch_bind_curves, items, n, curves)
 
     def bind_periodic_waves(self, nodes, real, imag=None, graphs=None):
         """wae_batch_bind_periodic_waves: real[k] and imag[k] (rows of float32 CUDA tensors [n][coefficients], unit stride on the last
@@ -906,9 +903,7 @@ class Batch:
                 raise B.WaeError(1, f"bind_periodic_waves: row {k} has {count} coefficients, node {nid} of graph {g} was declared "
                                     f"with {declared}")
             items[k] = B.PeriodicWaveBinding(g, int(nid), row(real, k), row(imag, k))
-        self.api.check(self.api.batch_bind_periodic_waves(self.handle, items, n, C.c_void_p(self._torch_stream_handle())))
-        for t in given:
-            self._keep_until_read(t)
+        self._bind(self.api.batch_bind_periodic_waves, items, n, *given)
 
     def bind_iir_coefficients(self, nodes, feedforward, feedback, graphs=None):
         """wae_batch_bind_iir_coefficients: feedforward[k] and feedback[k] (rows of float64 CUDA tensors [n][nff] and [n][nfb], unit
@@ -936,9 +931,7 @@ class Batch:
                 raise B.WaeError(1, f"bind_iir_coefficients: row {k} has {feedforward.shape[1]} feedforward and {feedback.shape[1]} "
                                     f"feedback coefficients, node {nid} of graph {g} was declared with {declared[0]} and {declared[1]}")
             items[k] = B.IirBinding(g, int(nid), row(feedforward, k), row(feedback, k))
-        self.api.check(self.api.batch_bind_iir_coefficients(self.handle, items, n, C.c_void_p(self._torch_stream_handle())))
-        self._keep_until_read(feedforward)
-        self._keep_until_read(feedback)
+        self._bind(self.api.batch_bind_iir_coefficients, items, n, feedforward, feedback)
 
     def bind_value_curves(self, params, values, graphs=None):
         """wae_batch_bind_value_curves: values[j][i] (a float32 CUDA tensor [n][length] per param, unit stride on the last dimension)
@@ -957,9 +950,7 @@ class Batch:
         n = tensors[0].shape[0] if tensors else 0
         if any(t.shape[0] != n for t in tensors):
             raise B.WaeError(1, "bind_value_curves: the tensors differ in their number of rows")
-        graphs = list(range(n)) if graphs is None else [int(g) for g in graphs]
-        if len(graphs) != n:
-            raise B.WaeError(1, f"bind_value_curves: {n} rows for {len(graphs)} graphs")
+        graphs = self._graphs("bind_value_curves", graphs, n, "rows")
         if n and any(t.stride(1) != 1 for t in tensors):
             raise B.WaeError(1, "bind_value_curves: the values of a curve must be contiguous (unit stride on the last dimension)")
         items = (B.ValueCurveBinding * max(n * len(params), 1))()
@@ -968,8 +959,6 @@ class Batch:
                 raise B.WaeError(2, "bind_value_curves: AudioListener params are not bound from device memory")
             key = (int(prm._node), int(prm._index))
             for i, g in enumerate(graphs):
-                if not 0 <= g < self.n:
-                    raise B.WaeError(2, f"bind_value_curves: graph index {g} is out of range")
                 declared = self.contexts[g]._device_value_curves.get(key)
                 # (the tensor's own shape: the library checks only the CUDA allocation, which may hold several tensors)
                 if declared is not None and t.shape[1] != declared:
@@ -977,9 +966,7 @@ class Batch:
                                         f"graph {g} was declared with {declared}")
                 ptr = C.cast(C.c_void_p(t.data_ptr() + 4 * i * t.stride(0)), B.c_float_p)
                 items[j * n + i] = B.ValueCurveBinding(g, key[0], key[1], ptr)
-        self.api.check(self.api.batch_bind_value_curves(self.handle, items, n * len(params), C.c_void_p(self._torch_stream_handle())))
-        for t in tensors:
-            self._keep_until_read(t)
+        self._bind(self.api.batch_bind_value_curves, items, n * len(params), *tensors)
 
     def bind_schedules(self, nodes, starts, stops=None, graphs=None):
         """wae_batch_bind_schedules: starts[i] (and stops[i]) become the start (and stop) times of the scheduled source `nodes` (declared
@@ -997,12 +984,8 @@ class Batch:
             raise B.WaeError(1, f"bind_schedules: starts is {list(starts.shape)} for {k} node(s): [n] for one node, [n][k] for a list")
         if stops is not None and stops.shape != starts.shape:
             raise B.WaeError(1, f"bind_schedules: stops is {list(stops.shape)}, starts {list(starts.shape)}")
-        graphs = list(range(n)) if graphs is None else [int(g) for g in graphs]
-        if len(graphs) != n:
-            raise B.WaeError(1, f"bind_schedules: {n} rows for {len(graphs)} graphs")
+        graphs = self._graphs("bind_schedules", graphs, n, "rows")
         for g in graphs:
-            if not 0 <= g < self.n:
-                raise B.WaeError(2, f"bind_schedules: graph index {g} is out of range")
             for nid in ids:
                 declared = self.contexts[g]._device_schedules.get(nid)
                 if declared is not None and declared != (stops is not None):
@@ -1017,23 +1000,27 @@ class Batch:
         for i, g in enumerate(graphs):
             for j, nid in enumerate(ids):
                 items[i * k + j] = B.ScheduleBinding(g, nid, C.cast(C.c_void_p(base + 8 * width * (i * k + j)), B.c_double_p))
-        self.api.check(self.api.batch_bind_schedules(self.handle, items, n * k, C.c_void_p(self._torch_stream_handle())))
-        self._keep_until_read(times)
+        self._bind(self.api.batch_bind_schedules, items, n * k, times)
+
+    def _graphs(self, fn, graphs, n, rows, ids=None):
+        """The graph indices of n rows of binding items: `graphs` (default 0..n-1), each in range; `ids`: the node ids of the rows, whose
+        count is checked with the graphs'."""
+        graphs = list(range(n)) if graphs is None else [int(g) for g in graphs]
+        if len(graphs) != n or (ids is not None and len(ids) != n):
+            raise B.WaeError(1, f"{fn}: {n} {rows} for {len(graphs)} graphs" + ("" if ids is None else f" and {len(ids)} nodes"))
+        for g in graphs:
+            if not 0 <= g < self.n:
+                raise B.WaeError(2, f"{fn}: graph index {g} is out of range")
+        return graphs
 
     def _graphs_and_nodes(self, fn, nodes, graphs, n):
         """The graph index and node id of each of n binding items: `graphs` (default 0..n-1), `nodes` one node (or id) for all graphs or
         one per graph."""
-        graphs = list(range(n)) if graphs is None else [int(g) for g in graphs]
         if isinstance(nodes, (list, tuple)):
             ids = [getattr(x, "id", x) for x in nodes]
         else:
             ids = [getattr(nodes, "id", nodes)] * n
-        if len(graphs) != n or len(ids) != n:
-            raise B.WaeError(1, f"{fn}: {n} tensors for {len(graphs)} graphs and {len(ids)} nodes")
-        for g in graphs:
-            if not 0 <= g < self.n:
-                raise B.WaeError(2, f"{fn}: graph index {g} is out of range")
-        return graphs, ids
+        return self._graphs(fn, graphs, n, "tensors", ids), ids
 
     def _pcm_items(self, fn, arg, nodes, pcm, graphs, declarations, Struct):
         """The binding items (graph index, node, device pointer, channel stride) of bind_sources / bind_responses: `declarations` names
@@ -1042,13 +1029,7 @@ class Batch:
         if not (isinstance(pcm, torch.Tensor) and pcm.is_cuda and pcm.dtype == torch.float32 and pcm.dim() == 3):
             raise B.WaeError(1, f"{fn}: {arg} must be a float32 CUDA tensor [n][channels][length]")
         n = pcm.shape[0]
-        graphs = list(range(n)) if graphs is None else [int(g) for g in graphs]
-        if isinstance(nodes, (list, tuple)):
-            ids = [getattr(x, "id", x) for x in nodes]
-        else:
-            ids = [getattr(nodes, "id", nodes)] * n
-        if len(graphs) != n or len(ids) != n:
-            raise B.WaeError(1, f"{fn}: {n} tensors for {len(graphs)} graphs and {len(ids)} nodes")
+        graphs, ids = self._graphs_and_nodes(fn, nodes, graphs, n)
         if n and pcm.stride(2) != 1:
             raise B.WaeError(1, f"{fn}: the frames of a channel must be contiguous (unit stride on the last dimension)")
         items = (Struct * max(n, 1))()
@@ -1056,8 +1037,6 @@ class Batch:
         # (torch may give the channel dimension of a one-channel tensor any stride: only channel 0 is read then)
         channel_stride = pcm.stride(1) if pcm.shape[1] > 1 else pcm.shape[2]
         for k, (g, nid) in enumerate(zip(graphs, ids)):
-            if not 0 <= g < self.n:
-                raise B.WaeError(2, f"{fn}: graph index {g} is out of range")
             declared = getattr(self.contexts[g], declarations).get(int(nid))
             # the library checks the CUDA allocation; torch's caching allocator may hold several tensors in one, so the tensor's own
             # shape is checked here
@@ -1066,6 +1045,13 @@ class Batch:
                                     f"[{declared[0]}][{declared[1]}]")
             items[k] = Struct(g, int(nid), C.cast(C.c_void_p(base + 4 * k * pcm.stride(0)), B.c_float_p), channel_stride)
         return items, n
+
+    def _bind(self, fn, items, n, *tensors):
+        """One call of the bind entry point `fn`, ordered after torch's current stream; the bound tensors are kept from reuse until the
+        engine stream has read them."""
+        self.api.check(fn(self.handle, items, n, C.c_void_p(self._torch_stream_handle())))
+        for t in tensors:
+            self._keep_until_read(t)
 
     def _keep_until_read(self, t):
         """Keeps torch's caching allocator from reusing a bound tensor's memory before the engine stream has read it.  The tensor is
@@ -1090,22 +1076,17 @@ class Batch:
         n, k = v2.shape
         if k != len(params):
             raise B.WaeError(1, f"bind_params: {k} value columns for {len(params)} params")
-        graphs = list(range(n)) if graphs is None else [int(g) for g in graphs]
-        if len(graphs) != n:
-            raise B.WaeError(1, f"bind_params: {n} value rows for {len(graphs)} graphs")
+        graphs = self._graphs("bind_params", graphs, n, "value rows")
         items = (B.ParamBinding * max(n * k, 1))()
         base = v2.data_ptr()
         s0, s1 = v2.stride()
         for i, g in enumerate(graphs):
-            if not 0 <= g < self.n:
-                raise B.WaeError(2, f"bind_params: graph index {g} is out of range")
             for j, prm in enumerate(params):
                 if prm._node == "listener":
                     raise B.WaeError(2, "bind_params: AudioListener params are not bound from device memory")
                 ptr = C.cast(C.c_void_p(base + 4 * (i * s0 + j * s1)), B.c_float_p)
                 items[i * k + j] = B.ParamBinding(g, int(prm._node), int(prm._index), ptr)
-        self.api.check(self.api.batch_bind_params(self.handle, items, n * k, C.c_void_p(self._torch_stream_handle())))
-        self._keep_until_read(values)
+        self._bind(self.api.batch_bind_params, items, n * k, values)
 
     def output_tensor(self, i=None):
         """Zero-copy torch view of the rendered output on the device: [n][channels][length] for a batch of one shape, [channels_i][length_i]

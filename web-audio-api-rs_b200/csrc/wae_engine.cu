@@ -359,6 +359,25 @@ struct StageBuild {
             default: return 0;
         }
     }
+    size_t record_bytes() const {  // size of one record of that table
+        switch (kind) {
+            case S_OSC: return sizeof(OscInst);
+            case S_OSC_AR: return sizeof(OscArInst);
+            case S_CONST: return sizeof(ConstInst);
+            case S_IIR: return sizeof(IirInst);
+            case S_SHAPER_OS: return sizeof(ShaperOsInst);
+            case S_CHAIN: case S_VSUM: return sizeof(ChainInst);
+            case S_BIQUAD: return sizeof(BiquadInst);
+            case S_BIQUAD_AR: return sizeof(BiquadArInst);
+            case S_GAIN: return sizeof(GainInst);
+            case S_SPAN: return sizeof(SPanInst);
+            case S_COMP: return sizeof(CompInst);
+            case S_META: return sizeof(MetaInst);
+            case S_ABSN_SERIAL: return sizeof(AbsnSerialInst);
+            case S_ABSN_BOUND: return sizeof(AbsnBoundInst);
+            default: return 0;
+        }
+    }
 };
 using PatchRec = StageBuild::PatchRec;
 
@@ -389,6 +408,151 @@ struct AnalyserRec {
     bool computed;      // frequency data already computed for the end-of-render time (analysis.rs:353-361)
     double min_db, max_db;
     int64_t lq;         // frames the graph renders (its own length padded to whole quanta): the ring's write index after the render
+};
+
+// One kind of input a prepared batch takes from device memory, as messages name it
+struct BindKind {
+    const char* noun;     // one declaration, in the messages of runs that wait for it
+    const char* plural;   // a graph's declarations, in the refusals of one-shot renders
+    const char* declare;  // the call that declares one
+    const char* bind;     // the call that binds them
+    uint32_t wae_graph::*count;  // the graph's number of declarations
+};
+enum { BK_SOURCES, BK_PARAMS, BK_RESPONSES, BK_CURVES, BK_WAVES, BK_IIRS, BK_VALUE_CURVES, BK_SCHEDULES, BK_COUNT };
+const BindKind kBindKinds[BK_COUNT] = {
+    {"device input", "device inputs", "wae_buffer_source_set_device_input", "wae_batch_bind_sources", &wae_graph::device_inputs},
+    {"param bound from device memory", "params bound from device memory", "wae_param_set_device_value", "wae_batch_bind_params",
+     &wae_graph::device_params},
+    {"response bound from device memory", "convolver responses bound from device memory", "wae_convolver_set_device_response",
+     "wae_batch_bind_responses", &wae_graph::device_responses},
+    {"curve bound from device memory", "WaveShaper curves bound from device memory", "wae_wave_shaper_set_device_curve",
+     "wae_batch_bind_curves", &wae_graph::device_curves},
+    {"periodic wave bound from device memory", "periodic waves bound from device memory", "wae_oscillator_set_device_periodic_wave",
+     "wae_batch_bind_periodic_waves", &wae_graph::device_waves},
+    {"IIR coefficients bound from device memory", "IIR coefficients bound from device memory", "wae_iir_filter_set_device_coefficients",
+     "wae_batch_bind_iir_coefficients", &wae_graph::device_iirs},
+    {"value curve bound from device memory", "value curves bound from device memory", "wae_param_set_device_value_curve",
+     "wae_batch_bind_value_curves", &wae_graph::device_value_curves},
+    {"schedule bound from device memory", "schedules bound from device memory", "wae_source_set_device_schedule", "wae_batch_bind_schedules",
+     &wae_graph::device_schedules},
+};
+
+// The name of a declaration: (batch position, node, param index); kinds declared on a node take kNodeLevel as param index
+constexpr uint32_t kNodeLevel = UINT32_MAX;
+struct BindKey {
+    uint32_t graph;
+    wae_node_id node;
+    uint32_t param;
+    bool operator<(const BindKey& o) const { return std::tie(graph, node, param) < std::tie(o.graph, o.node, o.param); }
+};
+
+// The declarations of one kind, whatever each holds.  A declaration is bound once a bind has named it; runs wait for the unbound ones.
+struct BindTable {
+    const BindKind* kind;
+    std::vector<BindKey> keys;  // [declaration]
+    std::vector<char> bound;
+    std::map<BindKey, size_t> index;  // key -> declaration
+    size_t unbound = 0;
+    static constexpr size_t npos = SIZE_MAX;
+    explicit BindTable(const BindKind& k) : kind(&k) {}
+    size_t find(const BindKey& key) const {
+        auto it = index.find(key);
+        return it == index.end() ? npos : it->second;
+    }
+    void set_bound(size_t k, bool is_bound) {
+        if (bound[k] == (char)is_bound) return;
+        bound[k] = is_bound;
+        if (is_bound) unbound--;
+        else unbound++;
+    }
+};
+
+// The declarations of one kind with what a bind writes for each (`D`: slot pointers, spectra, curve or wavetable memory, a range of
+// patch entries, windows).  The planner adds the ones it gives memory, under wae_batch::mu; seal() then puts them in key order and
+// appends the declared ones the planner never reached.  Those are bound from the start: binding one is validated and writes nothing,
+// and runs do not wait for it.
+template <typename D>
+struct Bindings : BindTable {
+    std::vector<D> data;  // [declaration]
+    using BindTable::BindTable;
+    void add(const BindKey& key, const D& d, bool is_bound = false) {
+        index[key] = keys.size();
+        keys.push_back(key);
+        data.push_back(d);
+        bound.push_back(is_bound);
+        unbound += is_bound ? 0 : 1;
+    }
+    // `visit(j, nodes, node, declare)` calls declare(key, d) for each declaration of `node` (of `nodes`: graph j's own nodes or an
+    // epoch's copy of them), declare(key, d, false) for one runs wait for whether or not the planner reached it
+    template <typename Visit>
+    void seal(wae_graph* const* graphs, uint32_t n_graphs, Visit&& visit) {
+        std::vector<size_t> perm(keys.size());
+        for (size_t k = 0; k < perm.size(); k++) perm[k] = k;
+        std::sort(perm.begin(), perm.end(), [&](size_t x, size_t y) { return keys[x] < keys[y]; });
+        Bindings sorted(*kind);
+        for (size_t k : perm) sorted.add(keys[k], data[k], bound[k]);
+        *this = std::move(sorted);
+        auto declare = [&](const BindKey& key, const D& d, bool is_bound = true) {
+            if (!index.count(key)) add(key, d, is_bound);
+        };
+        for (uint32_t j = 0; j < n_graphs; j++) {
+            if (!(graphs[j]->*kind->count)) continue;
+            for (const auto& kv : graphs[j]->nodes) visit(j, graphs[j]->nodes, kv.second, declare);
+            for (const auto& ep : graphs[j]->epochs)
+                for (const auto& kv : ep.nodes) visit(j, ep.nodes, kv.second, declare);
+        }
+    }
+};
+
+// a patch entry of the declaration (graph, node) of a kind declared on a node, its device addresses set
+template <typename P>
+struct PatchEntry {
+    uint32_t graph;  // batch position
+    wae_node_id node;
+    P p;
+};
+
+// What the binds write, per kind
+struct DevInput {  // wae_buffer_source_set_device_input: the slot in its group's slab
+    float* slot;   // [channels][stride]
+    uint32_t channels;
+    uint64_t length, stride;
+};
+struct DevResponse {  // wae_convolver_set_device_response: the spectra the planner made
+    float2* h;        // [channels][S + WAE_CONV_H_PAD][WAE_CONV_SPEC]
+    uint32_t channels;
+    uint64_t length;
+    int S;
+    bool normalize;
+    float sample_rate;
+};
+struct DevCurve {  // wae_wave_shaper_set_device_curve: the curve memory the planner made (zeroed, never in the upload slabs)
+    float* d;      // [length rounded up to 4]
+    uint32_t length;
+    int32_t p0, p1;  // its entries in d_curve_patches
+};
+struct DevWave {  // wae_oscillator_set_device_periodic_wave: the wavetable memory the planner made (zeroed, never in the upload slabs)
+    float* d;     // [table_len]
+    uint32_t coefficients, table_len;
+    bool normalize;
+};
+struct DevIir {  // wae_iir_filter_set_device_coefficients: the entries of every record its coefficients reach
+    uint32_t nff, nfb;
+    int32_t p0, p1;  // in d_iir_patches
+};
+struct DevSchedule {  // wae_source_set_device_schedule: the windows and the entries of every record the times reach
+    bool bind_stop;
+    double lo[2], hi[2];
+    int32_t p0, p1;  // in d_sched_patches
+};
+struct DevValueCurve {  // wae_param_set_device_value_curve: the param's curve pool (ParamInst::curves, made by the planner) and where
+    float* pool;        // the declared values lie in it
+    int32_t values_off;
+    uint32_t length;
+};
+struct DevParam {  // wae_param_set_device_value: the value slot is the declaration's index
+    uint32_t pid;  // the param's node id
+    ParamSlotInfo info;
 };
 
 }  // namespace
@@ -440,23 +604,19 @@ struct wae_batch {
         cudaEvent_t ev_h2d = nullptr, ev_done = nullptr;
     };
     std::vector<Group> groups;
-    // wae_buffer_source_set_device_input: the slot of each device input in its group's slab, filled by wae_batch_bind_sources
-    struct DevInput {
-        uint32_t graph;  // batch position
-        wae_node_id node;
-        float* slot;     // [channels][stride]
-        uint32_t channels;
-        uint64_t length, stride;
-        bool bound;
-    };
-    std::vector<DevInput> dev_inputs;
-    std::map<std::pair<uint32_t, wae_node_id>, size_t> dev_index;  // (batch position, node) -> dev_inputs
-    size_t dev_unbound = 0;
+    // the declarations of the inputs bound from device memory, one table per kind
+    Bindings<DevInput> sources{kBindKinds[BK_SOURCES]};
+    Bindings<DevParam> params{kBindKinds[BK_PARAMS]};
+    Bindings<DevResponse> responses{kBindKinds[BK_RESPONSES]};
+    Bindings<DevCurve> curves{kBindKinds[BK_CURVES]};
+    Bindings<DevWave> waves{kBindKinds[BK_WAVES]};
+    Bindings<DevIir> iirs{kBindKinds[BK_IIRS]};
+    Bindings<DevValueCurve> value_curves{kBindKinds[BK_VALUE_CURVES]};
+    Bindings<DevSchedule> schedules{kBindKinds[BK_SCHEDULES]};
     // The item table of a bind is staged in page-locked memory (a copy from pageable memory would wait for the engine stream first) and
     // copied to d_bind, which the next bind may overwrite at once (its copy is queued behind this bind's kernel on the same stream).  A
     // staging buffer is reused once its copy has run (its event has completed); while all are in flight a new one is made, so a bind
     // does not wait on the host for runs queued before it (up to kMaxBindStages staging buffers; then the bind waits for the first one that fits).
-    // wae_batch_bind_params uses the same staging buffers and device table for its items.
     struct BindStage {
         void* h;
         size_t cap;      // bytes
@@ -466,114 +626,16 @@ struct wae_batch {
     std::vector<BindStage> bind_stages;
     void* d_bind = nullptr;
     size_t bind_cap = 0;  // bytes
-    // wae_param_set_device_value: one value slot per declared param of the batch (batch position, node, param index), and the patch
-    // entries of every record a bound value reaches (re-derived by k_derive_params after each wae_batch_bind_params)
-    struct BoundParam {
-        uint32_t graph;  // batch position
-        wae_node_id node;
-        uint32_t param_index;
-        bool bound;
-    };
-    std::vector<BoundParam> bound_params;  // [slot]
-    std::map<std::tuple<uint32_t, wae_node_id, uint32_t>, int32_t> param_slot;
-    size_t params_unbound = 0;
+    // wae_batch_bind_params: the value of each slot and the patch entries of every record a bound value reaches (re-derived by
+    // k_derive_params after each bind)
     ParamSlotInfo* d_slot_info = nullptr;
     float* d_values = nullptr;
     ParamPatch* d_patches = nullptr;
     int n_patches = 0;
-    // wae_convolver_set_device_response: the spectra of each declared response (made by the planner), rewritten by
-    // wae_batch_bind_responses.  A declared response the planner never reached (its convolver renders nothing) has no spectra: binding it
-    // is validated and writes nothing.
-    struct DevResponse {
-        uint32_t graph;  // batch position
-        wae_node_id node;
-        float2* h;       // [channels][S + WAE_CONV_H_PAD][WAE_CONV_SPEC]
-        uint32_t channels;
-        uint64_t length;
-        int S;
-        bool normalize;
-        float sample_rate;
-        bool bound;
-    };
-    std::vector<DevResponse> responses;
-    std::map<std::pair<uint32_t, wae_node_id>, size_t> response_index;  // (batch position, node) -> responses
-    size_t responses_unbound = 0;
-    // wae_wave_shaper_set_device_curve: the curve memory of each declared curve (made by the planner, zeroed, never in the upload slabs)
-    // and the range of its patch entries in d_curve_patches, both rewritten by wae_batch_bind_curves.  A declared curve the planner never
-    // reached has no memory: binding it is validated and writes nothing.
-    struct DevCurve {
-        uint32_t graph;  // batch position
-        wae_node_id node;
-        float* d;        // [length rounded up to 4]
-        uint32_t length;
-        int32_t p0, p1;  // its entries in d_curve_patches
-        bool bound;
-    };
-    std::vector<DevCurve> curves;
-    std::map<std::pair<uint32_t, wae_node_id>, size_t> curve_index;  // (batch position, node) -> curves
-    size_t curves_unbound = 0;
+    // the patch entries of declared curves, IIR filters and schedules, each declaration's a contiguous range
     CurvePatch* d_curve_patches = nullptr;
-    // wae_oscillator_set_device_periodic_wave: the wavetable memory of each declared wave (made by the planner, zeroed, never in the
-    // upload slabs), rewritten by wae_batch_bind_periodic_waves.  A declared wave the planner never reached has no memory: binding it is
-    // validated and writes nothing.
-    struct DevWave {
-        uint32_t graph;  // batch position
-        wae_node_id node;
-        float* d;        // [table_len]
-        uint32_t coefficients, table_len;
-        bool normalize;
-        bool bound;
-    };
-    std::vector<DevWave> waves;
-    std::map<std::pair<uint32_t, wae_node_id>, size_t> wave_index;  // (batch position, node) -> waves
-    size_t waves_unbound = 0;
-    // wae_iir_filter_set_device_coefficients: the range of each declared filter's patch entries in d_iir_patches (every record its
-    // coefficients reach), rewritten by wae_batch_bind_iir_coefficients.  A declared filter the planner never reached has none: binding it
-    // is validated and writes nothing, and runs do not wait for it.
-    struct DevIir {
-        uint32_t graph;  // batch position
-        wae_node_id node;
-        uint32_t nff, nfb;
-        int32_t p0, p1;  // its entries in d_iir_patches
-        bool bound;
-    };
-    std::vector<DevIir> iirs;
-    std::map<std::pair<uint32_t, wae_node_id>, size_t> iir_index;  // (batch position, node) -> iirs
-    size_t iirs_unbound = 0;
     IirPatch* d_iir_patches = nullptr;
-    // wae_source_set_device_schedule: the windows of each declared source and the range of its patch entries in d_sched_patches (every
-    // record its times reach), rewritten by wae_batch_bind_schedules.  A declared source the planner never reached has none: binding it is
-    // validated and writes nothing, and runs do not wait for it.
-    struct DevSchedule {
-        uint32_t graph;  // batch position
-        wae_node_id node;
-        bool bind_stop;
-        double lo[2], hi[2];
-        int32_t p0, p1;  // its entries in d_sched_patches
-        bool bound;
-    };
-    std::vector<DevSchedule> schedules;
-    std::map<std::pair<uint32_t, wae_node_id>, size_t> schedule_index;  // (batch position, node) -> schedules
-    size_t schedules_unbound = 0;
     SchedPatch* d_sched_patches = nullptr;
-    // wae_param_set_device_value_curve: the curve pool of each declared param (ParamInst::curves: made by the planner, zeroed, the param's
-    // host curves copied in once, never in the upload slabs) and where the declared values lie in it, rewritten by
-    // wae_batch_bind_value_curves.  A declared param the planner never lowered has no pool: binding it is validated and writes nothing,
-    // and runs do not wait for it.
-    struct DevValueCurve {
-        uint32_t graph;  // batch position
-        uint32_t pid;    // the param's node id
-        wae_node_id node;
-        uint32_t param_index;
-        float* pool;
-        int32_t values_off;
-        uint32_t length;
-        bool bound;
-    };
-    std::vector<DevValueCurve> value_curves;
-    std::map<std::pair<uint32_t, uint32_t>, size_t> value_curve_pool;  // (batch position, param id) -> value_curves, while planning
-    std::map<std::tuple<uint32_t, wae_node_id, uint32_t>, size_t> value_curve_index;  // (batch position, node, param index) -> value_curves
-    size_t value_curves_unbound = 0;
     cudaEvent_t ev_bind = nullptr;  // orders a bind after the caller's stream
     // OfflineAudioContext::suspend_sync: a group's render is cut at the suspend frames of its graphs (graphs with different
     // suspend points are put in different groups); every segment has its own plan, node state is shared between the plans
@@ -1222,7 +1284,7 @@ struct Planner {
     bool device_response_spectra(const Node& n, int S, IrSpectra& spec);
     const float* device_curve(const Node& n);
     float* device_wave(const Node& n);
-    float* device_value_curve(uint32_t pid, const Param& prm, const ParamTimeline& tl);
+    float* device_value_curve(const Param& prm, const ParamTimeline& tl);
     // a patch entry of the declared curve of node `n` for the int32 field `off` bytes into the last record of stage `s`
     void add_curve_patch(StageBuild& s, const Node& n, uint32_t off, int32_t keeps, int32_t other) {
         s.curve_patches.push_back(StageBuild::CurvePatchRec{gi, n.id, (int32_t)s.records() - 1, off, keeps, other});
@@ -1815,8 +1877,7 @@ bool Planner::device_response_spectra(const Node& n, int S, IrSpectra& spec) {
     b->asset_bytes += (size_t)ir_ch * (S + WAE_CONV_H_PAD) * WAE_CONV_SPEC * 8;
     (*ir_cache)[key] = spec;
     if (!dry)
-        b->responses.push_back(wae_batch::DevResponse{key_graph, n.id, spec.h, (uint32_t)ir_ch, (uint64_t)ir.length(), S, n.normalize,
-                                                      ir.sample_rate, false});
+        b->responses.add({key_graph, n.id, kNodeLevel}, DevResponse{spec.h, (uint32_t)ir_ch, (uint64_t)ir.length(), S, n.normalize, ir.sample_rate});
     return true;
 }
 
@@ -1826,16 +1887,15 @@ bool Planner::device_response_spectra(const Node& n, int S, IrSpectra& spec) {
 const float* Planner::device_curve(const Node& n) {
     if (dry) return reinterpret_cast<const float*>(uintptr_t(256));
     std::lock_guard<std::recursive_mutex> lk(b->mu);
-    auto it = b->curve_index.find({gi, n.id});
-    if (it != b->curve_index.end()) return b->curves[it->second].d;
+    const size_t k = b->curves.find({gi, n.id, kNodeLevel});
+    if (k != BindTable::npos) return b->curves.data[k].d;
     float* d = b->dalloc<float>((size_t)(n.device_curve + 3) / 4 * 4, true);
     if (!d) {
         bail(WAE_OUT_OF_MEMORY, "out of device memory (WaveShaper curve)");
         return nullptr;
     }
     b->asset_bytes += (size_t)(n.device_curve + 3) / 4 * 16;
-    b->curve_index[{gi, n.id}] = b->curves.size();
-    b->curves.push_back(wae_batch::DevCurve{gi, n.id, d, n.device_curve, 0, 0, false});
+    b->curves.add({gi, n.id, kNodeLevel}, DevCurve{d, n.device_curve, 0, 0});
     return d;
 }
 
@@ -1845,28 +1905,29 @@ const float* Planner::device_curve(const Node& n) {
 float* Planner::device_wave(const Node& n) {
     if (dry) return reinterpret_cast<float*>(uintptr_t(256));
     std::lock_guard<std::recursive_mutex> lk(b->mu);
-    auto it = b->wave_index.find({gi, n.id});
-    if (it != b->wave_index.end()) return b->waves[it->second].d;
+    const size_t k = b->waves.find({gi, n.id, kNodeLevel});
+    if (k != BindTable::npos) return b->waves.data[k].d;
     float* d = b->dalloc<float>((size_t)n.device_wave_len, true);
     if (!d) {
         bail(WAE_OUT_OF_MEMORY, "out of device memory (periodic wave)");
         return nullptr;
     }
     b->asset_bytes += (size_t)n.device_wave_len * sizeof(float);
-    b->wave_index[{gi, n.id}] = b->waves.size();
-    b->waves.push_back(wae_batch::DevWave{gi, n.id, d, n.device_wave, n.device_wave_len, n.device_wave_normalize, false});
+    b->waves.add({gi, n.id, kNodeLevel}, DevWave{d, n.device_wave, n.device_wave_len, n.device_wave_normalize});
     return d;
 }
 
 // The curve pool of a param with a value curve bound from device memory: one zeroed allocation per (batch graph, param), outside the
 // upload slabs (nothing but wae_batch_bind_value_curves writes the declared values), shared by every suspend segment.  The declared event
 // is the param's last, so its values are the last `device_curve` of the pool; the param's other curves are copied in once.  The sizing
-// pass gets the placeholder an uploaded pool gets, so that plan digests stay comparable.
-float* Planner::device_value_curve(uint32_t pid, const Param& prm, const ParamTimeline& tl) {
+// pass gets the placeholder an uploaded pool gets, so that plan digests stay comparable.  The pool is found by the (node, param index) the
+// param was declared through.
+float* Planner::device_value_curve(const Param& prm, const ParamTimeline& tl) {
     if (dry) return reinterpret_cast<float*>(uintptr_t(256));
     std::lock_guard<std::recursive_mutex> lk(b->mu);
-    auto it = b->value_curve_pool.find({gi, pid});
-    if (it != b->value_curve_pool.end()) return b->value_curves[it->second].pool;
+    const BindKey key{gi, prm.device_curve_node, prm.device_curve_index};
+    const size_t k = b->value_curves.find(key);
+    if (k != BindTable::npos) return b->value_curves.data[k].pool;
     const size_t host_part = tl.curves.size() - prm.device_curve;
     float* d = b->dalloc<float>((tl.curves.size() + 3) / 4 * 4, true);
     if (!d || (host_part && cudaMemcpyAsync(d, tl.curves.data(), host_part * sizeof(float), cudaMemcpyHostToDevice, b->engine->stream) !=
@@ -1875,8 +1936,7 @@ float* Planner::device_value_curve(uint32_t pid, const Param& prm, const ParamTi
         return nullptr;
     }
     b->asset_bytes += (tl.curves.size() + 3) / 4 * 16;
-    b->value_curve_pool[{gi, pid}] = b->value_curves.size();
-    b->value_curves.push_back(wae_batch::DevValueCurve{gi, pid, 0, 0, d, (int32_t)host_part, prm.device_curve, false});
+    b->value_curves.add(key, DevValueCurve{d, (int32_t)host_part, prm.device_curve});
     return d;
 }
 
@@ -2039,7 +2099,7 @@ bool Planner::lower_param(uint32_t id, Node& n, PNode& p) {
     pi.events = tl.events.empty() ? nullptr : upload(tl.events);
     // (a value curve bound from device memory: the pool of its own the bind writes into)
     if (n.param.device_curve) {
-        if (!(pi.curves = device_value_curve(id, n.param, tl))) return false;
+        if (!(pi.curves = device_value_curve(n.param, tl))) return false;
     } else {
         pi.curves = tl.curves.empty() ? nullptr : upload(tl.curves);
     }
@@ -3747,24 +3807,9 @@ struct GroupPlan {  // result of phase B for one group
     int code = WAE_OK;
     std::string error;
     std::vector<std::pair<uint32_t, ParamPatch>> patches;  // (batch position, entry): device addresses set, operands still param ids
-    struct CurveEntry {
-        uint32_t graph;  // batch position
-        wae_node_id node;
-        CurvePatch p;    // device address set
-    };
-    std::vector<CurveEntry> curve_patches;
-    struct IirEntry {
-        uint32_t graph;  // batch position
-        wae_node_id node;
-        IirPatch p;      // device addresses set
-    };
-    std::vector<IirEntry> iir_patches;
-    struct SchedEntry {
-        uint32_t graph;  // batch position
-        wae_node_id node;
-        SchedPatch p;    // device address set
-    };
-    std::vector<SchedEntry> sched_patches;
+    std::vector<PatchEntry<CurvePatch>> curve_patches;
+    std::vector<PatchEntry<IirPatch>> iir_patches;
+    std::vector<PatchEntry<SchedPatch>> sched_patches;
 };
 
 static int64_t padded_length(const wae_graph* g) { return (int64_t)((g->length + 127) / 128 * 128); }
@@ -4354,62 +4399,35 @@ static void prep_plan_group(wae_batch* b, wae_graph* const* graphs, int k, PrepS
                 if (!st.d_a) return oom("stage tables");
                 gp.stages.push_back(st);
             }
-            if (st.n > 0 && !s.patches.empty()) {  // patch entries: the device addresses of the fields they re-derive
-                size_t rec_size = 0, rec2_size = 0;
-                switch (s.kind) {
-                    case S_CHAIN: case S_VSUM: rec_size = sizeof(ChainInst); rec2_size = sizeof(ScanCoef); break;
-                    case S_BIQUAD: rec_size = sizeof(BiquadInst); break;
-                    case S_BIQUAD_AR: rec_size = sizeof(BiquadArInst); break;
-                    case S_GAIN: rec_size = sizeof(GainInst); break;
-                    case S_SPAN: rec_size = sizeof(SPanInst); rec2_size = sizeof(float2); break;
-                    case S_COMP: rec_size = sizeof(CompInst); break;
-                    case S_META: rec_size = sizeof(MetaInst); break;
-                    case S_ABSN_SERIAL: rec_size = sizeof(AbsnSerialInst); break;
-                    case S_ABSN_BOUND: rec_size = sizeof(AbsnBoundInst); break;
-                }
+            if (st.n > 0) {  // patch entries: the device addresses of the fields they set
+                const size_t rec_size = s.record_bytes();
+                auto rec = [&](int32_t k) { return static_cast<char*>(st.d_a) + (size_t)k * rec_size; };
+                // params: the field and the scan constants (S_CHAIN / S_VSUM) or stereo gains (S_SPAN) it re-derives
+                const size_t rec2_size = s.kind == S_SPAN ? sizeof(float2) : sizeof(ScanCoef);
                 for (const PatchRec& pr : s.patches) {
                     ParamPatch p = pr.p;
-                    p.dst = static_cast<char*>(st.d_a) + (size_t)pr.rec * rec_size + pr.off;
+                    p.dst = rec(pr.rec) + pr.off;
                     p.dst2 = pr.rec2 >= 0 ? static_cast<char*>(st.d_b) + (size_t)pr.rec2 * rec2_size : nullptr;
                     gp.patches.push_back({pr.graph, p});
                 }
-            }
-            if (st.n > 0) {  // patch entries of curves bound from device memory: the device addresses of the int32 fields they set
-                const size_t rec_size = s.kind == S_META ? sizeof(MetaInst) : s.kind == S_SHAPER_OS ? sizeof(ShaperOsInst) : sizeof(ChainInst);
-                for (const auto& cp : s.curve_patches) {
-                    int32_t* dst = reinterpret_cast<int32_t*>(static_cast<char*>(st.d_a) + (size_t)cp.rec * rec_size + cp.off);
-                    gp.curve_patches.push_back({cp.graph, cp.node, CurvePatch{dst, cp.keeps, cp.other}});
-                }
-                // patch entries of IIR coefficients bound from device memory: the coefficient fields of the IirInst or ChainBiquad, and
-                // the biquad's scan constants where they were built
+                for (const auto& cp : s.curve_patches)  // curves: the int32 field
+                    gp.curve_patches.push_back({cp.graph, cp.node, CurvePatch{reinterpret_cast<int32_t*>(rec(cp.rec) + cp.off), cp.keeps, cp.other}});
+                // IIR coefficients: the coefficient fields of the IirInst or ChainBiquad, and the biquad's scan constants where they were built
                 for (const auto& ip : s.iir_patches) {
                     IirPatch p{};
                     if (ip.bq < 0) {
-                        IirInst* r = static_cast<IirInst*>(st.d_a) + ip.rec;
-                        p.b = reinterpret_cast<double*>(reinterpret_cast<char*>(r) + offsetof(IirInst, b));
-                        p.a = reinterpret_cast<double*>(reinterpret_cast<char*>(r) + offsetof(IirInst, a));
+                        p.b = reinterpret_cast<double*>(rec(ip.rec) + offsetof(IirInst, b));
+                        p.a = reinterpret_cast<double*>(rec(ip.rec) + offsetof(IirInst, a));
                     } else {
-                        ChainInst* r = static_cast<ChainInst*>(st.d_a) + ip.rec;
-                        p.b = reinterpret_cast<double*>(reinterpret_cast<char*>(r) + offsetof(ChainInst, bq) + (size_t)ip.bq * sizeof(ChainBiquad) +
+                        p.b = reinterpret_cast<double*>(rec(ip.rec) + offsetof(ChainInst, bq) + (size_t)ip.bq * sizeof(ChainBiquad) +
                                                         offsetof(ChainBiquad, b0));
                         if (ip.scan >= 0 && (size_t)ip.scan < s.scan_coef.size()) p.scan = static_cast<ScanCoef*>(st.d_b) + ip.scan;
                     }
                     gp.iir_patches.push_back({ip.graph, ip.node, p});
                 }
-                // patch entries of schedules bound from device memory: the record whose fields the times reach
-                size_t sched_rec_size = 0;
-                switch (s.kind) {
-                    case S_CHAIN: case S_VSUM: sched_rec_size = sizeof(ChainInst); break;
-                    case S_OSC: sched_rec_size = sizeof(OscInst); break;
-                    case S_OSC_AR: sched_rec_size = sizeof(OscArInst); break;
-                    case S_CONST: sched_rec_size = sizeof(ConstInst); break;
-                    case S_META: sched_rec_size = sizeof(MetaInst); break;
-                    case S_ABSN_BOUND: sched_rec_size = sizeof(AbsnBoundInst); break;
-                    case S_ABSN_SERIAL: sched_rec_size = sizeof(AbsnSerialInst); break;
-                }
-                for (const auto& sp : s.sched_patches) {
+                for (const auto& sp : s.sched_patches) {  // schedules: the record whose fields the times reach
                     SchedPatch p = sp.p;
-                    p.dst = static_cast<char*>(st.d_a) + (size_t)sp.rec * sched_rec_size + sp.off;
+                    p.dst = rec(sp.rec) + sp.off;
                     gp.sched_patches.push_back({sp.graph, sp.node, p});
                 }
             }
@@ -4437,304 +4455,119 @@ static wae_status enqueue_source_copies(wae_batch* b, wae_batch::Group& grp, cud
     return WAE_OK;
 }
 
-// The device inputs of the batch (`graphs` in batch order): the slots of the planned groups, all unbound, then the declared device
-// inputs the planner gave no slot (a source that is never started renders silence without reading its buffer): binding one is
-// validated like any other and copies nothing, and runs do not wait for it — it behaves like a node given an AudioBuffer of that shape.
+// The device inputs of the batch (`graphs` in batch order): the slots of the planned groups, then the declared ones the planner gave no
+// slot (a source that is never started renders silence without reading its buffer), which behave like a node given an AudioBuffer of
+// that shape.
 static void record_device_inputs(wae_batch* b, wae_graph* const* graphs, uint32_t n_graphs) {
     for (auto& grp : b->groups)
         for (auto& sc : grp.src_copies)
             if (sc.buf->device_input) {
                 grp.has_device_inputs = true;
-                b->dev_index[{sc.graph, sc.node}] = b->dev_inputs.size();
-                b->dev_inputs.push_back(wae_batch::DevInput{sc.graph, sc.node, grp.d_src + sc.offset, (uint32_t)sc.buf->channels.size(),
-                                                            (uint64_t)sc.buf->length(), (uint64_t)sc.buf->stride, false});
+                b->sources.add({sc.graph, sc.node, kNodeLevel}, DevInput{grp.d_src + sc.offset, (uint32_t)sc.buf->channels.size(),
+                                                                         (uint64_t)sc.buf->length(), (uint64_t)sc.buf->stride});
             }
-    b->dev_unbound = b->dev_inputs.size();
-    for (uint32_t j = 0; j < n_graphs; j++) {
-        if (!graphs[j]->device_inputs) continue;
-        auto scan = [&](const NodeMap& nodes) {
-            for (const auto& kv : nodes) {
-                const Node& nd = kv.second;
-                if (nd.kind != K_ABSN || !nd.buffer || !nd.buffer->device_input || b->dev_index.count({j, nd.id})) continue;
-                b->dev_index[{j, nd.id}] = b->dev_inputs.size();
-                b->dev_inputs.push_back(wae_batch::DevInput{j, nd.id, nullptr, (uint32_t)nd.buffer->channels.size(), (uint64_t)nd.buffer->length(),
-                                                            (uint64_t)nd.buffer->stride, true});
-            }
-        };
-        scan(graphs[j]->nodes);
-        for (const auto& ep : graphs[j]->epochs) scan(ep.nodes);
-    }
+    b->sources.seal(graphs, n_graphs, [](uint32_t j, const NodeMap&, const Node& nd, auto& declare) {
+        if (nd.kind == K_ABSN && nd.buffer && nd.buffer->device_input)
+            declare({j, nd.id, kNodeLevel},
+                    DevInput{nullptr, (uint32_t)nd.buffer->channels.size(), (uint64_t)nd.buffer->length(), (uint64_t)nd.buffer->stride});
+    });
 }
 
-// The declared responses of the batch (`graphs` in batch order), after planning: the ones the planner gave spectra, all unbound, then
-// the declared ones it never reached, which binding validates and writes nothing to, and which runs do not wait for.
-static void record_responses(wae_batch* b, wae_graph* const* graphs, uint32_t n_graphs) {
-    std::sort(b->responses.begin(), b->responses.end(),
-              [](const wae_batch::DevResponse& x, const wae_batch::DevResponse& y) { return std::tie(x.graph, x.node) < std::tie(y.graph, y.node); });
-    for (size_t k = 0; k < b->responses.size(); k++) b->response_index[{b->responses[k].graph, b->responses[k].node}] = k;
-    b->responses_unbound = b->responses.size();
-    for (uint32_t j = 0; j < n_graphs; j++) {
-        if (!graphs[j]->device_responses) continue;
-        auto scan = [&](const NodeMap& nodes) {
-            for (const auto& kv : nodes) {
-                const Node& nd = kv.second;
-                if (nd.kind != K_CONV || !nd.buffer || !nd.buffer->device_input || b->response_index.count({j, nd.id})) continue;
-                b->response_index[{j, nd.id}] = b->responses.size();
-                b->responses.push_back(wae_batch::DevResponse{j, nd.id, nullptr, (uint32_t)nd.buffer->channels.size(), (uint64_t)nd.buffer->length(),
-                                                              0, nd.normalize, nd.buffer->sample_rate, true});
-            }
-        };
-        scan(graphs[j]->nodes);
-        for (const auto& ep : graphs[j]->epochs) scan(ep.nodes);
-    }
-}
-
-// The declared curves of the batch (`graphs` in batch order), after planning: the ones the planner gave memory, all unbound, with their
-// patch entries gathered per curve and uploaded (from `patches`, which the caller keeps alive until the stream has been synchronised);
-// then the declared ones it never reached, which binding validates and writes nothing to, and which runs do not wait for.
-static wae_status record_curves(wae_batch* b, wae_graph* const* graphs, uint32_t n_graphs, const std::vector<GroupPlan>& gps,
-                                std::vector<CurvePatch>& patches) {
-    std::sort(b->curves.begin(), b->curves.end(),
-              [](const wae_batch::DevCurve& x, const wae_batch::DevCurve& y) { return std::tie(x.graph, x.node) < std::tie(y.graph, y.node); });
-    b->curve_index.clear();
-    for (size_t k = 0; k < b->curves.size(); k++) b->curve_index[{b->curves[k].graph, b->curves[k].node}] = k;
-    b->curves_unbound = b->curves.size();
-    std::vector<std::vector<CurvePatch>> per(b->curves.size());
+// The patch entries of the planned groups (`entries` of each GroupPlan) gathered per declaration of `t`, each declaration's range [p0, p1)
+// set, and uploaded to *d (from `patches`, which the caller keeps alive until the stream has been synchronised).  Runs wait for a
+// declaration with entries.
+extern "C++" {
+template <typename D, typename P>
+static wae_status gather_patches(wae_batch* b, Bindings<D>& t, const std::vector<GroupPlan>& gps,
+                                 std::vector<PatchEntry<P>> GroupPlan::*entries, std::vector<P>& patches, P** d) {
+    std::vector<std::vector<P>> per(t.keys.size());
     for (const auto& gp : gps)
-        for (const auto& e : gp.curve_patches) per[b->curve_index.at({e.graph, e.node})].push_back(e.p);
+        for (const auto& e : gp.*entries) per[t.index.at({e.graph, e.node, kNodeLevel})].push_back(e.p);
     for (size_t k = 0; k < per.size(); k++) {
-        b->curves[k].p0 = (int32_t)patches.size();
+        t.data[k].p0 = (int32_t)patches.size();
         patches.insert(patches.end(), per[k].begin(), per[k].end());
-        b->curves[k].p1 = (int32_t)patches.size();
+        t.data[k].p1 = (int32_t)patches.size();
+        if (!per[k].empty()) t.set_bound(k, false);
     }
-    if (!patches.empty() && !(b->d_curve_patches = b->dupload_now(patches)))
-        return fail(WAE_OUT_OF_MEMORY, "out of device memory (curve patch entries)");
-    for (uint32_t j = 0; j < n_graphs; j++) {
-        if (!graphs[j]->device_curves) continue;
-        auto scan = [&](const NodeMap& nodes) {
-            for (const auto& kv : nodes) {
-                const Node& nd = kv.second;
-                if (nd.kind != K_SHAPER || !nd.device_curve || b->curve_index.count({j, nd.id})) continue;
-                b->curve_index[{j, nd.id}] = b->curves.size();
-                b->curves.push_back(wae_batch::DevCurve{j, nd.id, nullptr, nd.device_curve, 0, 0, true});
-            }
-        };
-        scan(graphs[j]->nodes);
-        for (const auto& ep : graphs[j]->epochs) scan(ep.nodes);
-    }
+    if (!patches.empty() && !(*d = b->dupload_now(patches)))
+        return fail(WAE_OUT_OF_MEMORY, std::string("out of device memory (patch entries of ") + t.kind->bind + ")");
     return WAE_OK;
 }
+}  // extern "C++"
 
-// The declared periodic waves of the batch (`graphs` in batch order), after planning: the ones the planner gave memory, all unbound; then
-// the declared ones it never reached (never started, pruned), which binding validates and writes nothing to, and which runs do not wait for.
-static void record_waves(wae_batch* b, wae_graph* const* graphs, uint32_t n_graphs) {
-    std::sort(b->waves.begin(), b->waves.end(),
-              [](const wae_batch::DevWave& x, const wae_batch::DevWave& y) { return std::tie(x.graph, x.node) < std::tie(y.graph, y.node); });
-    b->wave_index.clear();
-    for (size_t k = 0; k < b->waves.size(); k++) b->wave_index[{b->waves[k].graph, b->waves[k].node}] = k;
-    b->waves_unbound = b->waves.size();
-    for (uint32_t j = 0; j < n_graphs; j++) {
-        if (!graphs[j]->device_waves) continue;
-        auto scan = [&](const NodeMap& nodes) {
-            for (const auto& kv : nodes) {
-                const Node& nd = kv.second;
-                if (nd.kind != K_OSC || !nd.device_wave || b->wave_index.count({j, nd.id})) continue;
-                b->wave_index[{j, nd.id}] = b->waves.size();
-                b->waves.push_back(
-                    wae_batch::DevWave{j, nd.id, nullptr, nd.device_wave, nd.device_wave_len, nd.device_wave_normalize, true});
-            }
-        };
-        scan(graphs[j]->nodes);
-        for (const auto& ep : graphs[j]->epochs) scan(ep.nodes);
-    }
+// The declared responses, curves, periodic waves, IIR filters, schedules and value curves of the batch (`graphs` in batch order), after
+// planning.  Runs wait for the ones the planner gave memory or patch entries; the patch entries are uploaded from the vectors passed,
+// which the caller keeps alive until the stream has been synchronised.
+static wae_status record_declarations(wae_batch* b, wae_graph* const* graphs, uint32_t n_graphs, const std::vector<GroupPlan>& gps,
+                                      std::vector<CurvePatch>& curve_patches, std::vector<IirPatch>& iir_patches,
+                                      std::vector<SchedPatch>& sched_patches) {
+    b->responses.seal(graphs, n_graphs, [](uint32_t j, const NodeMap&, const Node& nd, auto& declare) {
+        if (nd.kind == K_CONV && nd.buffer && nd.buffer->device_input)
+            declare({j, nd.id, kNodeLevel}, DevResponse{nullptr, (uint32_t)nd.buffer->channels.size(), (uint64_t)nd.buffer->length(), 0,
+                                                        nd.normalize, nd.buffer->sample_rate});
+    });
+    b->curves.seal(graphs, n_graphs, [](uint32_t j, const NodeMap&, const Node& nd, auto& declare) {
+        if (nd.kind == K_SHAPER && nd.device_curve) declare({j, nd.id, kNodeLevel}, DevCurve{nullptr, nd.device_curve, 0, 0});
+    });
+    b->waves.seal(graphs, n_graphs, [](uint32_t j, const NodeMap&, const Node& nd, auto& declare) {
+        if (nd.kind == K_OSC && nd.device_wave)
+            declare({j, nd.id, kNodeLevel}, DevWave{nullptr, nd.device_wave, nd.device_wave_len, nd.device_wave_normalize});
+    });
+    b->iirs.seal(graphs, n_graphs, [](uint32_t j, const NodeMap&, const Node& nd, auto& declare) {
+        if (nd.kind == K_IIR && nd.device_iir)
+            declare({j, nd.id, kNodeLevel}, DevIir{(uint32_t)nd.feedforward.size(), (uint32_t)nd.feedback.size(), 0, 0});
+    });
+    b->schedules.seal(graphs, n_graphs, [](uint32_t j, const NodeMap&, const Node& nd, auto& declare) {
+        if (nd.device_schedule)
+            declare({j, nd.id, kNodeLevel},
+                    DevSchedule{nd.sched_stop, {nd.sched_lo[0], nd.sched_lo[1]}, {nd.sched_hi[0], nd.sched_hi[1]}, 0, 0});
+    });
+    b->value_curves.seal(graphs, n_graphs, [](uint32_t j, const NodeMap&, const Node& nd, auto& declare) {
+        if (nd.kind == K_PARAM && nd.param.device_curve)
+            declare({j, nd.param.device_curve_node, nd.param.device_curve_index}, DevValueCurve{nullptr, 0, nd.param.device_curve});
+    });
+    wae_status st = gather_patches(b, b->curves, gps, &GroupPlan::curve_patches, curve_patches, &b->d_curve_patches);
+    if (st == WAE_OK) st = gather_patches(b, b->iirs, gps, &GroupPlan::iir_patches, iir_patches, &b->d_iir_patches);
+    if (st == WAE_OK) st = gather_patches(b, b->schedules, gps, &GroupPlan::sched_patches, sched_patches, &b->d_sched_patches);
+    return st;
 }
 
-// The declared IIR filters of the batch (`graphs` in batch order, each in graph and node order), after planning, with the patch
-// entries of the planned groups gathered per filter and uploaded (from `patches`, which the caller keeps alive until the stream has been
-// synchronised).  The ones the planner reached are unbound; the ones it never reached have no entries: binding them is validated and
-// writes nothing, and runs do not wait for them.
-static wae_status record_iirs(wae_batch* b, wae_graph* const* graphs, uint32_t n_graphs, const std::vector<GroupPlan>& gps,
-                              std::vector<IirPatch>& patches) {
-    for (uint32_t j = 0; j < n_graphs; j++) {
-        if (!graphs[j]->device_iirs) continue;
-        auto scan = [&](const NodeMap& nodes) {
-            for (const auto& kv : nodes) {
-                const Node& nd = kv.second;
-                if (nd.kind != K_IIR || !nd.device_iir || b->iir_index.count({j, nd.id})) continue;
-                b->iir_index[{j, nd.id}] = b->iirs.size();
-                b->iirs.push_back(wae_batch::DevIir{j, nd.id, (uint32_t)nd.feedforward.size(), (uint32_t)nd.feedback.size(), 0, 0, false});
-            }
-        };
-        scan(graphs[j]->nodes);
-        for (const auto& ep : graphs[j]->epochs) scan(ep.nodes);
-    }
-    std::vector<std::vector<IirPatch>> per(b->iirs.size());
-    for (const auto& gp : gps)
-        for (const auto& e : gp.iir_patches) per[b->iir_index.at({e.graph, e.node})].push_back(e.p);
-    b->iirs_unbound = 0;
-    for (size_t k = 0; k < per.size(); k++) {
-        wae_batch::DevIir& d = b->iirs[k];
-        d.p0 = (int32_t)patches.size();
-        patches.insert(patches.end(), per[k].begin(), per[k].end());
-        d.p1 = (int32_t)patches.size();
-        d.bound = d.p0 == d.p1;  // (never reached: nothing to wait for)
-        b->iirs_unbound += d.bound ? 0 : 1;
-    }
-    if (!patches.empty() && !(b->d_iir_patches = b->dupload_now(patches)))
-        return fail(WAE_OUT_OF_MEMORY, "out of device memory (IIR patch entries)");
-    return WAE_OK;
-}
-
-// The declared schedules of the batch (`graphs` in batch order, each in graph and node order), after planning, with the patch entries of
-// the planned groups gathered per source and uploaded (from `patches`, which the caller keeps alive until the stream has been
-// synchronised).  The ones the planner reached are unbound; the ones it never reached have no entries: binding them is validated and
-// writes nothing, and runs do not wait for them.
-static wae_status record_schedules(wae_batch* b, wae_graph* const* graphs, uint32_t n_graphs, const std::vector<GroupPlan>& gps,
-                                   std::vector<SchedPatch>& patches) {
-    for (uint32_t j = 0; j < n_graphs; j++) {
-        if (!graphs[j]->device_schedules) continue;
-        for (const auto& kv : graphs[j]->nodes) {  // (a graph with a declaration has no suspend point)
-            const Node& nd = kv.second;
-            if (!nd.device_schedule || b->schedule_index.count({j, nd.id})) continue;
-            b->schedule_index[{j, nd.id}] = b->schedules.size();
-            b->schedules.push_back(wae_batch::DevSchedule{j, nd.id, nd.sched_stop, {nd.sched_lo[0], nd.sched_lo[1]},
-                                                          {nd.sched_hi[0], nd.sched_hi[1]}, 0, 0, false});
-        }
-    }
-    std::vector<std::vector<SchedPatch>> per(b->schedules.size());
-    for (const auto& gp : gps)
-        for (const auto& e : gp.sched_patches) per[b->schedule_index.at({e.graph, e.node})].push_back(e.p);
-    b->schedules_unbound = 0;
-    for (size_t k = 0; k < per.size(); k++) {
-        wae_batch::DevSchedule& d = b->schedules[k];
-        d.p0 = (int32_t)patches.size();
-        patches.insert(patches.end(), per[k].begin(), per[k].end());
-        d.p1 = (int32_t)patches.size();
-        d.bound = d.p0 == d.p1;  // (never reached: nothing to wait for)
-        b->schedules_unbound += d.bound ? 0 : 1;
-    }
-    if (!patches.empty() && !(b->d_sched_patches = b->dupload_now(patches)))
-        return fail(WAE_OUT_OF_MEMORY, "out of device memory (schedule patch entries)");
-    return WAE_OK;
-}
-
-// The declared value curves of the batch (`graphs` in batch order), after planning: each named by the (node, param index) it was declared
-// through, the ones the planner gave a pool unbound, in graph, node and param order; then the declared ones it never lowered, which
-// binding validates and writes nothing to, and which runs do not wait for.
-static void record_value_curves(wae_batch* b, wae_graph* const* graphs, uint32_t n_graphs) {
-    std::vector<wae_batch::DevValueCurve> never;
-    for (uint32_t j = 0; j < n_graphs; j++) {
-        if (!graphs[j]->device_value_curves) continue;
-        auto scan = [&](const NodeMap& nodes) {
-            for (const auto& kv : nodes) {
-                const Node& nd = kv.second;
-                if (nd.kind != K_PARAM || !nd.param.device_curve) continue;
-                auto pi = b->value_curve_pool.find({j, nd.id});
-                if (pi != b->value_curve_pool.end()) {
-                    b->value_curves[pi->second].node = nd.param.device_curve_node;
-                    b->value_curves[pi->second].param_index = nd.param.device_curve_index;
-                } else if (std::none_of(never.begin(), never.end(), [&](const wae_batch::DevValueCurve& d) { return d.graph == j && d.pid == nd.id; })) {
-                    never.push_back(wae_batch::DevValueCurve{j, nd.id, nd.param.device_curve_node, nd.param.device_curve_index, nullptr, 0,
-                                                             nd.param.device_curve, true});
-                }
-            }
-        };
-        scan(graphs[j]->nodes);
-        for (const auto& ep : graphs[j]->epochs) scan(ep.nodes);
-    }
-    auto by_name = [](const wae_batch::DevValueCurve& x, const wae_batch::DevValueCurve& y) {
-        return std::tie(x.graph, x.node, x.param_index) < std::tie(y.graph, y.node, y.param_index);
-    };
-    std::sort(b->value_curves.begin(), b->value_curves.end(), by_name);
-    b->value_curves_unbound = b->value_curves.size();
-    b->value_curves.insert(b->value_curves.end(), never.begin(), never.end());
-    b->value_curve_pool.clear();
-    for (size_t k = 0; k < b->value_curves.size(); k++) {
-        const auto& d = b->value_curves[k];
-        b->value_curve_index[{d.graph, d.node, d.param_index}] = k;
-    }
-}
-
-// runs of a batch need every device input, param, response, curve, periodic wave, IIR coefficient set, value curve and schedule bound once
+// runs of a batch need every declaration they read bound once; the first unbound one is named, kind by kind in this order
 static wae_status check_bound(wae_batch* b) {
     if (!b) return fail(WAE_INVALID_ARGUMENT, "null batch");
-    for (size_t k = 0; b->schedules_unbound && k < b->schedules.size(); k++)
-        if (const auto& d = b->schedules[k]; !d.bound) {
-            const uint32_t caller = b->order.empty() ? d.graph : b->order[d.graph];
-            return fail(WAE_INVALID_STATE, "schedule bound from device memory never bound: graph " + std::to_string(caller) + ", node " +
-                                               std::to_string(d.node) + " (wae_batch_bind_schedules)");
-        }
-    for (size_t k = 0; b->value_curves_unbound && k < b->value_curves.size(); k++)
-        if (const auto& d = b->value_curves[k]; !d.bound) {
-            const uint32_t caller = b->order.empty() ? d.graph : b->order[d.graph];
-            return fail(WAE_INVALID_STATE, "value curve bound from device memory never bound: graph " + std::to_string(caller) + ", node " +
-                                               std::to_string(d.node) + ", param " + std::to_string(d.param_index) +
-                                               " (wae_batch_bind_value_curves)");
-        }
-    for (size_t k = 0; b->iirs_unbound && k < b->iirs.size(); k++)
-        if (const auto& d = b->iirs[k]; !d.bound) {
-            const uint32_t caller = b->order.empty() ? d.graph : b->order[d.graph];
-            return fail(WAE_INVALID_STATE, "IIR coefficients bound from device memory never bound: graph " + std::to_string(caller) +
-                                               ", node " + std::to_string(d.node) + " (wae_batch_bind_iir_coefficients)");
-        }
-    for (size_t k = 0; b->waves_unbound && k < b->waves.size(); k++)
-        if (const auto& d = b->waves[k]; !d.bound) {
-            const uint32_t caller = b->order.empty() ? d.graph : b->order[d.graph];
-            return fail(WAE_INVALID_STATE, "periodic wave bound from device memory never bound: graph " + std::to_string(caller) +
-                                               ", node " + std::to_string(d.node) + " (wae_batch_bind_periodic_waves)");
-        }
-    for (size_t k = 0; b->curves_unbound && k < b->curves.size(); k++)
-        if (const auto& d = b->curves[k]; !d.bound) {
-            const uint32_t caller = b->order.empty() ? d.graph : b->order[d.graph];
-            return fail(WAE_INVALID_STATE, "curve bound from device memory never bound: graph " + std::to_string(caller) + ", node " +
-                                               std::to_string(d.node) + " (wae_batch_bind_curves)");
-        }
-    for (size_t k = 0; b->responses_unbound && k < b->responses.size(); k++)
-        if (const auto& d = b->responses[k]; !d.bound) {
-            const uint32_t caller = b->order.empty() ? d.graph : b->order[d.graph];
-            return fail(WAE_INVALID_STATE, "response bound from device memory never bound: graph " + std::to_string(caller) + ", node " +
-                                               std::to_string(d.node) + " (wae_batch_bind_responses)");
-        }
-    for (size_t k = 0; b->dev_unbound && k < b->dev_inputs.size(); k++)
-        if (const auto& d = b->dev_inputs[k]; !d.bound) {
-            const uint32_t caller = b->order.empty() ? d.graph : b->order[d.graph];
-            return fail(WAE_INVALID_STATE, "device input never bound: graph " + std::to_string(caller) + ", node " + std::to_string(d.node) +
-                                               " (wae_batch_bind_sources)");
-        }
-    if (b->params_unbound == 0) return WAE_OK;
-    for (auto& d : b->bound_params)
-        if (!d.bound) {
-            const uint32_t caller = b->order.empty() ? d.graph : b->order[d.graph];
-            return fail(WAE_INVALID_STATE, "param bound from device memory never bound: graph " + std::to_string(caller) + ", node " +
-                                               std::to_string(d.node) + ", param " + std::to_string(d.param_index) + " (wae_batch_bind_params)");
-        }
+    const BindTable* const kinds[] = {&b->schedules, &b->value_curves, &b->iirs, &b->waves, &b->curves, &b->responses, &b->sources, &b->params};
+    for (const BindTable* t : kinds)
+        for (size_t k = 0; t->unbound && k < t->keys.size(); k++)
+            if (!t->bound[k]) {
+                const BindKey& key = t->keys[k];
+                const uint32_t caller = b->order.empty() ? key.graph : b->order[key.graph];
+                return fail(WAE_INVALID_STATE, std::string(t->kind->noun) + " never bound: graph " + std::to_string(caller) + ", node " +
+                                                   std::to_string(key.node) + (key.param == kNodeLevel ? "" : ", param " + std::to_string(key.param)) +
+                                                   " (" + t->kind->bind + ")");
+            }
     return WAE_OK;
 }
 
-// The value slots of the params declared with wae_param_set_device_value (`graphs` in batch order: one slot per param, in graph and node
-// order) and the patch entries of the planned groups, their operands renumbered from param ids to slots; both uploaded (from `info` and
-// `patches`, which the caller keeps alive until the stream has been synchronised).
+// The value slots of the params declared with wae_param_set_device_value (`graphs` in batch order: one slot per param, in graph, node and
+// param order; runs wait for every one, reached by the planner or not) and the patch entries of the planned groups, their operands
+// renumbered from param ids to slots; both uploaded (from `info` and `patches`, which the caller keeps alive until the stream has been
+// synchronised).
 static wae_status record_params(wae_batch* b, wae_graph* const* graphs, uint32_t n_graphs, std::vector<GroupPlan>& gps,
                                 std::vector<ParamSlotInfo>& info, std::vector<ParamPatch>& patches) {
-    std::unordered_map<uint64_t, int32_t> slot_of;  // (batch position << 32 | param id) -> slot
-    for (uint32_t j = 0; j < n_graphs; j++) {
-        if (!graphs[j]->device_params) continue;
-        for (const auto& kv : graphs[j]->nodes) {
-            const Node& nd = kv.second;
-            if (nd.kind == K_PARAM) continue;
-            for (uint32_t i = 0; i < nd.params.size(); i++) {
-                const Param& prm = graphs[j]->nodes.at(nd.params[i]).param;
-                if (!prm.device_bound) continue;
-                const int32_t slot = (int32_t)b->bound_params.size();
-                slot_of[(uint64_t)j << 32 | nd.params[i]] = slot;
-                b->param_slot[{j, nd.id, i}] = slot;
-                b->bound_params.push_back(wae_batch::BoundParam{j, nd.id, i, false});
-                info.push_back(ParamSlotInfo{prm.device_lo, prm.device_hi, prm.default_value, 0});
-            }
+    b->params.seal(graphs, n_graphs, [](uint32_t j, const NodeMap& nodes, const Node& nd, auto& declare) {
+        if (nd.kind == K_PARAM) return;
+        for (uint32_t i = 0; i < nd.params.size(); i++) {
+            const Param& prm = nodes.at(nd.params[i]).param;
+            if (prm.device_bound)
+                declare({j, nd.id, i}, DevParam{nd.params[i], ParamSlotInfo{prm.device_lo, prm.device_hi, prm.default_value, 0}}, false);
         }
+    });
+    if (b->params.keys.empty()) return WAE_OK;
+    std::unordered_map<uint64_t, int32_t> slot_of;  // (batch position << 32 | param id) -> slot
+    for (size_t k = 0; k < b->params.keys.size(); k++) {
+        slot_of[(uint64_t)b->params.keys[k].graph << 32 | b->params.data[k].pid] = (int32_t)k;
+        info.push_back(b->params.data[k].info);
     }
-    if (info.empty()) return WAE_OK;
-    b->params_unbound = info.size();
     for (auto& gp : gps)
         for (auto& gpp : gp.patches) {
             ParamPatch p = gpp.second;
@@ -4811,17 +4644,12 @@ static wae_status prepare_impl(wae_engine* eng, wae_graph* const* graphs, uint32
             return cs;
         }
     }
-    record_responses(b, graphs, n_graphs);
-    record_waves(b, graphs, n_graphs);
-    record_value_curves(b, graphs, n_graphs);
     std::vector<CurvePatch> curve_patches;
     std::vector<IirPatch> iir_patches;
     std::vector<SchedPatch> sched_patches;
     std::vector<ParamSlotInfo> slot_info;
     std::vector<ParamPatch> patches;
-    st = record_curves(b, graphs, n_graphs, gps, curve_patches);
-    if (st == WAE_OK) st = record_iirs(b, graphs, n_graphs, gps, iir_patches);
-    if (st == WAE_OK) st = record_schedules(b, graphs, n_graphs, gps, sched_patches);
+    st = record_declarations(b, graphs, n_graphs, gps, curve_patches, iir_patches, sched_patches);
     if (st == WAE_OK) st = record_params(b, graphs, n_graphs, gps, slot_info, patches);
     if (st != WAE_OK) {
         wae_batch_destroy(b);
@@ -5181,9 +5009,12 @@ WAE_API wae_status wae_batch_run_pipelined(wae_batch* b, float* host_out) {
 struct BindExtents {
     int device;
     std::map<uintptr_t, size_t> known;  // base -> bytes of allocations of the engine's GPU looked up so far
-    // `what`: the pointer's name in the messages; `overrun`: the message when the extent runs past the end of its allocation
-    wae_status check(const void* ptr, uint64_t bytes, const char* what, const char* overrun) {
+    // `what`: the pointer's name in the messages; `align`: the alignment the bind kernel's loads need; `overrun`: the message when the
+    // extent runs past the end of its allocation
+    wae_status check(const void* ptr, size_t align, uint64_t bytes, const char* what, const char* overrun) {
         const uintptr_t p = (uintptr_t)ptr;
+        if (!ptr) return fail(WAE_INVALID_ARGUMENT, std::string("bind: null ") + what);
+        if (p % align) return fail(WAE_INVALID_ARGUMENT, std::string("bind: ") + what + " is not " + std::to_string(align) + "-byte aligned");
         auto it = known.upper_bound(p);
         if (it != known.begin() && p - std::prev(it)->first < std::prev(it)->second) {
             --it;
@@ -5279,413 +5110,223 @@ static wae_status stage_bind_table(wae_batch* b, const void* table, size_t bytes
     return WAE_OK;
 }
 
-WAE_API wae_status wae_batch_bind_sources(wae_batch* b, const wae_source_binding* items, uint32_t n, void* stream) {
+extern "C++" {
+template <typename Item>
+static uint32_t param_of(const Item&) { return kNodeLevel; }
+static uint32_t param_of(const wae_param_binding& it) { return it.param_index; }
+static uint32_t param_of(const wae_value_curve_binding& it) { return it.param_index; }
+
+// The steps every wae_batch_bind_* shares.  Every item is validated before anything is enqueued: its graph index, its declaration in
+// `table`, then `check(it, d, k, extents, rows)`, which checks the kind's pointers against declaration k (`d`) and appends the device
+// item, or nothing for a declaration the planner never reached.  `launch(rows_on_device, rows)` enqueues the kind's kernel.
+template <typename Row, typename Item, typename D, typename Check, typename Launch>
+static wae_status bind_items(wae_batch* b, Bindings<D> wae_batch::*table, const Item* items, uint32_t n, void* stream, Check&& check,
+                             Launch&& launch) {
     if (!b || (n && !items)) return fail(WAE_INVALID_ARGUMENT, "null batch / items");
     if (n == 0) return WAE_OK;
     CUDA_TRY(cudaSetDevice(b->engine->device));
-    // every item is validated before anything is enqueued
-    std::vector<BindItem> table;
-    std::vector<size_t> slot_of;
-    std::vector<char> named(b->dev_inputs.size(), 0);
+    Bindings<D>& t = b->*table;
+    std::vector<Row> rows;
+    std::vector<char> named(t.keys.size(), 0);
     BindExtents extents{b->engine->device, {}};
-    int64_t max_vec = 0;
-    int max_ch = 0;
     for (uint32_t i = 0; i < n; i++) {
-        const wae_source_binding& it = items[i];
+        const Item& it = items[i];
         if (it.graph_index >= b->n_graphs)
             return fail(WAE_INVALID_STATE, "bind: graph index " + std::to_string(it.graph_index) + " is out of range");
-        auto di = b->dev_index.find({b->batch_pos(it.graph_index), it.node});
-        if (di == b->dev_index.end())
-            return fail(WAE_INVALID_STATE, "bind: node " + std::to_string(it.node) + " of graph " + std::to_string(it.graph_index) +
-                                               " is not a device input (wae_buffer_source_set_device_input)");
-        const size_t k = di->second;
-        if (named[k]++)  // (two items of one launch writing one slot: which one lands would be undefined)
-            return fail(WAE_INVALID_ARGUMENT, "bind: node " + std::to_string(it.node) + " of graph " + std::to_string(it.graph_index) +
-                                                  " is named twice in one call");
-        const wae_batch::DevInput& d = b->dev_inputs[k];
-        if (!it.pcm) return fail(WAE_INVALID_ARGUMENT, "bind: null pcm");
-        if (it.channel_stride < d.length)
-            return fail(WAE_INVALID_ARGUMENT, "bind: channel_stride " + std::to_string(it.channel_stride) + " is below the declared length " +
-                                                  std::to_string(d.length));
-        if (it.channel_stride > (UINT64_MAX / 4 - d.length) / WAE_MAX_CHANNELS)
-            return fail(WAE_INVALID_ARGUMENT, "bind: channel_stride runs past the end of its allocation");
-        wae_status st = extents.check(it.pcm, ((uint64_t)(d.channels - 1) * it.channel_stride + d.length) * sizeof(float), "pcm",
-                                      "[pcm, pcm + (channels - 1) * channel_stride + length) runs past the end of its allocation");
+        const BindKey key{b->batch_pos(it.graph_index), it.node, param_of(it)};
+        auto name = [&] {
+            return (key.param == kNodeLevel ? std::string() : "param " + std::to_string(key.param) + " of ") + "node " +
+                   std::to_string(it.node) + " of graph " + std::to_string(it.graph_index);
+        };
+        const size_t k = t.find(key);
+        if (k == BindTable::npos) return fail(WAE_INVALID_STATE, "bind: " + name() + " was not declared with " + t.kind->declare);
+        if (named[k]++)  // (two items of one launch writing one declaration's memory: which one lands would be undefined)
+            return fail(WAE_INVALID_ARGUMENT, "bind: " + name() + " is named twice in one call");
+        wae_status st = check(it, t.data[k], k, extents, rows);
         if (st != WAE_OK) return st;
-        if (!d.slot) continue;  // declared, never rendered: nothing to copy
-        table.push_back(BindItem{d.slot, it.pcm, (int64_t)d.stride, (int64_t)it.channel_stride, (int64_t)d.length, (int32_t)d.channels, 0});
-        slot_of.push_back(k);
-        max_vec = std::max<int64_t>(max_vec, (int64_t)d.stride / 4);
-        max_ch = std::max<int>(max_ch, (int)d.channels);
     }
-    const size_t m = table.size();
-    if (m == 0) return WAE_OK;
-    wae_status st = bind_after(b, stream);
-    if (st == WAE_OK) st = stage_bind_table(b, table.data(), m * sizeof(BindItem));
-    if (st != WAE_OK) return st;
-    launch_bind_sources(static_cast<const BindItem*>(b->d_bind), (int)m, max_vec, max_ch, b->engine->stream);
-    cudaError_t le = cudaGetLastError();
-    if (le != cudaSuccess) return fail(WAE_CUDA_ERROR, std::string("bind: ") + cudaGetErrorString(le));
-    for (size_t k : slot_of)
-        if (!b->dev_inputs[k].bound) {
-            b->dev_inputs[k].bound = true;
-            b->dev_unbound--;
-        }
+    if (!rows.empty()) {
+        wae_status st = bind_after(b, stream);
+        if (st == WAE_OK) st = stage_bind_table(b, rows.data(), rows.size() * sizeof(Row));
+        if (st != WAE_OK) return st;
+        launch(static_cast<Row*>(b->d_bind), rows);
+        cudaError_t le = cudaGetLastError();
+        if (le != cudaSuccess) return fail(WAE_CUDA_ERROR, std::string("bind: ") + cudaGetErrorString(le));
+    }
+    for (size_t k = 0; t.unbound && k < named.size(); k++)
+        if (named[k]) t.set_bound(k, true);
     return WAE_OK;
+}
+}  // extern "C++"
+
+WAE_API wae_status wae_batch_bind_sources(wae_batch* b, const wae_source_binding* items, uint32_t n, void* stream) {
+    return bind_items<BindItem>(
+        b, &wae_batch::sources, items, n, stream,
+        [](const wae_source_binding& it, const DevInput& d, size_t, BindExtents& extents, auto& rows) -> wae_status {
+            if (it.channel_stride < d.length)
+                return fail(WAE_INVALID_ARGUMENT, "bind: channel_stride " + std::to_string(it.channel_stride) + " is below the declared length " +
+                                                      std::to_string(d.length));
+            if (it.channel_stride > (UINT64_MAX / 4 - d.length) / WAE_MAX_CHANNELS)
+                return fail(WAE_INVALID_ARGUMENT, "bind: channel_stride runs past the end of its allocation");
+            wae_status st = extents.check(it.pcm, alignof(float), ((uint64_t)(d.channels - 1) * it.channel_stride + d.length) * sizeof(float), "pcm",
+                                          "[pcm, pcm + (channels - 1) * channel_stride + length) runs past the end of its allocation");
+            if (st == WAE_OK && d.slot)
+                rows.push_back(BindItem{d.slot, it.pcm, (int64_t)d.stride, (int64_t)it.channel_stride, (int64_t)d.length, (int32_t)d.channels, 0});
+            return st;
+        },
+        [b](const BindItem* dev, const std::vector<BindItem>& rows) {
+            int64_t max_vec = 0;
+            int max_ch = 0;
+            for (const BindItem& r : rows) {
+                max_vec = std::max<int64_t>(max_vec, r.stride / 4);
+                max_ch = std::max<int>(max_ch, r.channels);
+            }
+            launch_bind_sources(dev, (int)rows.size(), max_vec, max_ch, b->engine->stream);
+        });
 }
 
 WAE_API wae_status wae_batch_bind_params(wae_batch* b, const wae_param_binding* items, uint32_t n, void* stream) {
-    if (!b || (n && !items)) return fail(WAE_INVALID_ARGUMENT, "null batch / items");
-    if (n == 0) return WAE_OK;
-    CUDA_TRY(cudaSetDevice(b->engine->device));
-    // every item is validated before anything is enqueued
-    std::vector<ParamBindItem> table;
-    std::vector<char> named(b->bound_params.size(), 0);
-    BindExtents extents{b->engine->device, {}};
-    for (uint32_t i = 0; i < n; i++) {
-        const wae_param_binding& it = items[i];
-        if (it.graph_index >= b->n_graphs)
-            return fail(WAE_INVALID_STATE, "bind: graph index " + std::to_string(it.graph_index) + " is out of range");
-        auto si = b->param_slot.find(std::make_tuple(b->batch_pos(it.graph_index), it.node, it.param_index));
-        const std::string name = "param " + std::to_string(it.param_index) + " of node " + std::to_string(it.node) + " of graph " +
-                                 std::to_string(it.graph_index);
-        if (si == b->param_slot.end())
-            return fail(WAE_INVALID_STATE, "bind: " + name + " is not bound from device memory (wae_param_set_device_value)");
-        if (named[si->second]++) return fail(WAE_INVALID_ARGUMENT, "bind: " + name + " is named twice in one call");
-        if (!it.value) return fail(WAE_INVALID_ARGUMENT, "bind: null value");
-        wae_status st = extents.check(it.value, sizeof(float), "value", "the value's 4 bytes run past the end of its allocation");
-        if (st != WAE_OK) return st;
-        table.push_back(ParamBindItem{it.value, si->second, 0});
-    }
-    wae_status st = bind_after(b, stream);
-    if (st == WAE_OK) st = stage_bind_table(b, table.data(), table.size() * sizeof(ParamBindItem));
-    if (st != WAE_OK) return st;
-    launch_bind_params(static_cast<const ParamBindItem*>(b->d_bind), (int)table.size(), b->d_slot_info, b->d_values, b->d_patches, b->n_patches,
-                       b->engine->stream);
-    cudaError_t le = cudaGetLastError();
-    if (le != cudaSuccess) return fail(WAE_CUDA_ERROR, std::string("bind: ") + cudaGetErrorString(le));
-    for (const ParamBindItem& t : table)
-        if (!b->bound_params[t.slot].bound) {
-            b->bound_params[t.slot].bound = true;
-            b->params_unbound--;
-        }
-    return WAE_OK;
+    return bind_items<ParamBindItem>(
+        b, &wae_batch::params, items, n, stream,
+        [](const wae_param_binding& it, const DevParam&, size_t slot, BindExtents& extents, auto& rows) -> wae_status {
+            wae_status st = extents.check(it.value, alignof(float), sizeof(float), "value", "the value's 4 bytes run past the end of its allocation");
+            if (st == WAE_OK) rows.push_back(ParamBindItem{it.value, (int32_t)slot, 0});
+            return st;
+        },
+        [b](const ParamBindItem* dev, const std::vector<ParamBindItem>& rows) {
+            launch_bind_params(dev, (int)rows.size(), b->d_slot_info, b->d_values, b->d_patches, b->n_patches, b->engine->stream);
+        });
 }
 
 // The spectra are rewritten in full on the engine stream: runs queued before the bind have read the previous ones by then.
 WAE_API wae_status wae_batch_bind_responses(wae_batch* b, const wae_response_binding* items, uint32_t n, void* stream) {
-    if (!b || (n && !items)) return fail(WAE_INVALID_ARGUMENT, "null batch / items");
-    if (n == 0) return WAE_OK;
-    CUDA_TRY(cudaSetDevice(b->engine->device));
-    // every item is validated before anything is enqueued
-    std::vector<RespBindItem> table;
-    std::vector<size_t> resp_of;
-    std::vector<char> named(b->responses.size(), 0);
-    BindExtents extents{b->engine->device, {}};
-    int64_t max_len = 0;
-    int max_S = 0, max_ch = 0;
-    bool any_normalize = false;
-    for (uint32_t i = 0; i < n; i++) {
-        const wae_response_binding& it = items[i];
-        if (it.graph_index >= b->n_graphs)
-            return fail(WAE_INVALID_STATE, "bind: graph index " + std::to_string(it.graph_index) + " is out of range");
-        auto ri = b->response_index.find({b->batch_pos(it.graph_index), it.node});
-        if (ri == b->response_index.end())
-            return fail(WAE_INVALID_STATE, "bind: node " + std::to_string(it.node) + " of graph " + std::to_string(it.graph_index) +
-                                               " is not a response bound from device memory (wae_convolver_set_device_response)");
-        const size_t k = ri->second;
-        if (named[k]++)  // (two items of one launch writing one set of spectra: which one lands would be undefined)
-            return fail(WAE_INVALID_ARGUMENT, "bind: node " + std::to_string(it.node) + " of graph " + std::to_string(it.graph_index) +
-                                                  " is named twice in one call");
-        const wae_batch::DevResponse& d = b->responses[k];
-        if (!it.pcm) return fail(WAE_INVALID_ARGUMENT, "bind: null pcm");
-        if (it.channel_stride < d.length)
-            return fail(WAE_INVALID_ARGUMENT, "bind: channel_stride " + std::to_string(it.channel_stride) + " is below the declared length " +
-                                                  std::to_string(d.length));
-        if (it.channel_stride > (UINT64_MAX / 4 - d.length) / 4)
-            return fail(WAE_INVALID_ARGUMENT, "bind: channel_stride runs past the end of its allocation");
-        wae_status st = extents.check(it.pcm, ((uint64_t)(d.channels - 1) * it.channel_stride + d.length) * sizeof(float), "pcm",
-                                      "[pcm, pcm + (channels - 1) * channel_stride + length) runs past the end of its allocation");
-        if (st != WAE_OK) return st;
-        if (!d.h) continue;  // declared, never rendered: nothing to write
-        RespBindItem r{};
-        r.src = it.pcm;
-        r.h = d.h;
-        r.src_stride = (int64_t)it.channel_stride;
-        r.len = (int64_t)d.length;
-        r.sample_rate = d.sample_rate;
-        r.channels = (int32_t)d.channels;
-        r.S = d.S;
-        r.normalize = d.normalize ? 1 : 0;
-        r.scale = 1.f;
-        table.push_back(r);
-        resp_of.push_back(k);
-        max_len = std::max<int64_t>(max_len, r.len);
-        max_S = std::max(max_S, d.S);
-        max_ch = std::max(max_ch, (int)d.channels);
-        any_normalize |= d.normalize;
-    }
-    const size_t m = table.size();
-    if (m == 0) return WAE_OK;
-    if (m > 65535) return fail(WAE_INVALID_ARGUMENT, "bind: more than 65535 responses in one call");
-    wae_status st = bind_after(b, stream);
-    if (st == WAE_OK) st = stage_bind_table(b, table.data(), m * sizeof(RespBindItem));
-    if (st != WAE_OK) return st;
-    launch_bind_responses(static_cast<RespBindItem*>(b->d_bind), (int)m, any_normalize, max_len, max_S, max_ch, b->engine->stream);
-    cudaError_t le = cudaGetLastError();
-    if (le != cudaSuccess) return fail(WAE_CUDA_ERROR, std::string("bind: ") + cudaGetErrorString(le));
-    for (size_t k : resp_of)
-        if (!b->responses[k].bound) {
-            b->responses[k].bound = true;
-            b->responses_unbound--;
-        }
-    return WAE_OK;
+    return bind_items<RespBindItem>(
+        b, &wae_batch::responses, items, n, stream,
+        [](const wae_response_binding& it, const DevResponse& d, size_t, BindExtents& extents, auto& rows) -> wae_status {
+            if (it.channel_stride < d.length)
+                return fail(WAE_INVALID_ARGUMENT, "bind: channel_stride " + std::to_string(it.channel_stride) + " is below the declared length " +
+                                                      std::to_string(d.length));
+            if (it.channel_stride > (UINT64_MAX / 4 - d.length) / 4)
+                return fail(WAE_INVALID_ARGUMENT, "bind: channel_stride runs past the end of its allocation");
+            wae_status st = extents.check(it.pcm, alignof(float), ((uint64_t)(d.channels - 1) * it.channel_stride + d.length) * sizeof(float), "pcm",
+                                          "[pcm, pcm + (channels - 1) * channel_stride + length) runs past the end of its allocation");
+            if (st != WAE_OK || !d.h) return st;
+            if (rows.size() == 65535)  // (the launch's grid)
+                return fail(WAE_INVALID_ARGUMENT, "bind: more than 65535 responses in one call");
+            RespBindItem r{};
+            r.src = it.pcm;
+            r.h = d.h;
+            r.src_stride = (int64_t)it.channel_stride;
+            r.len = (int64_t)d.length;
+            r.sample_rate = d.sample_rate;
+            r.channels = (int32_t)d.channels;
+            r.S = d.S;
+            r.normalize = d.normalize ? 1 : 0;
+            r.scale = 1.f;
+            rows.push_back(r);
+            return WAE_OK;
+        },
+        [b](RespBindItem* dev, const std::vector<RespBindItem>& rows) {
+            int64_t max_len = 0;
+            int max_S = 0, max_ch = 0;
+            bool any_normalize = false;
+            for (const RespBindItem& r : rows) {
+                max_len = std::max<int64_t>(max_len, r.len);
+                max_S = std::max(max_S, r.S);
+                max_ch = std::max(max_ch, (int)r.channels);
+                any_normalize |= r.normalize != 0;
+            }
+            launch_bind_responses(dev, (int)rows.size(), any_normalize, max_len, max_S, max_ch, b->engine->stream);
+        });
 }
 
 // The curve memory and the patched fields are rewritten on the engine stream: runs queued before the bind have read the previous ones.
 WAE_API wae_status wae_batch_bind_curves(wae_batch* b, const wae_curve_binding* items, uint32_t n, void* stream) {
-    if (!b || (n && !items)) return fail(WAE_INVALID_ARGUMENT, "null batch / items");
-    if (n == 0) return WAE_OK;
-    CUDA_TRY(cudaSetDevice(b->engine->device));
-    // every item is validated before anything is enqueued
-    std::vector<CurveBindItem> table;
-    std::vector<size_t> curve_of;
-    std::vector<char> named(b->curves.size(), 0);
-    BindExtents extents{b->engine->device, {}};
-    for (uint32_t i = 0; i < n; i++) {
-        const wae_curve_binding& it = items[i];
-        if (it.graph_index >= b->n_graphs)
-            return fail(WAE_INVALID_STATE, "bind: graph index " + std::to_string(it.graph_index) + " is out of range");
-        auto ci = b->curve_index.find({b->batch_pos(it.graph_index), it.node});
-        if (ci == b->curve_index.end())
-            return fail(WAE_INVALID_STATE, "bind: node " + std::to_string(it.node) + " of graph " + std::to_string(it.graph_index) +
-                                               " is not a curve bound from device memory (wae_wave_shaper_set_device_curve)");
-        const size_t k = ci->second;
-        if (named[k]++)  // (two items of one launch writing one curve: which one lands would be undefined)
-            return fail(WAE_INVALID_ARGUMENT, "bind: node " + std::to_string(it.node) + " of graph " + std::to_string(it.graph_index) +
-                                                  " is named twice in one call");
-        const wae_batch::DevCurve& d = b->curves[k];
-        if (!it.curve) return fail(WAE_INVALID_ARGUMENT, "bind: null curve");
-        wae_status st = extents.check(it.curve, (uint64_t)d.length * sizeof(float), "curve",
-                                      "[curve, curve + length) runs past the end of its allocation");
-        if (st != WAE_OK) return st;
-        if (!d.d) continue;  // declared, never rendered: nothing to write
-        table.push_back(CurveBindItem{it.curve, d.d, b->d_curve_patches + d.p0, (int32_t)d.length, d.p1 - d.p0});
-        curve_of.push_back(k);
-    }
-    if (table.empty()) return WAE_OK;
-    wae_status st = bind_after(b, stream);
-    if (st == WAE_OK) st = stage_bind_table(b, table.data(), table.size() * sizeof(CurveBindItem));
-    if (st != WAE_OK) return st;
-    launch_bind_curves(static_cast<const CurveBindItem*>(b->d_bind), (int)table.size(), b->engine->stream);
-    cudaError_t le = cudaGetLastError();
-    if (le != cudaSuccess) return fail(WAE_CUDA_ERROR, std::string("bind: ") + cudaGetErrorString(le));
-    for (size_t k : curve_of)
-        if (!b->curves[k].bound) {
-            b->curves[k].bound = true;
-            b->curves_unbound--;
-        }
-    return WAE_OK;
+    return bind_items<CurveBindItem>(
+        b, &wae_batch::curves, items, n, stream,
+        [b](const wae_curve_binding& it, const DevCurve& d, size_t, BindExtents& extents, auto& rows) -> wae_status {
+            wae_status st = extents.check(it.curve, alignof(float), (uint64_t)d.length * sizeof(float), "curve",
+                                          "[curve, curve + length) runs past the end of its allocation");
+            if (st == WAE_OK && d.d) rows.push_back(CurveBindItem{it.curve, d.d, b->d_curve_patches + d.p0, (int32_t)d.length, d.p1 - d.p0});
+            return st;
+        },
+        [b](const CurveBindItem* dev, const std::vector<CurveBindItem>& rows) { launch_bind_curves(dev, (int)rows.size(), b->engine->stream); });
 }
 
 // The wavetables are rewritten on the engine stream: runs queued before the bind have read the previous ones.
 WAE_API wae_status wae_batch_bind_periodic_waves(wae_batch* b, const wae_periodic_wave_binding* items, uint32_t n, void* stream) {
-    if (!b || (n && !items)) return fail(WAE_INVALID_ARGUMENT, "null batch / items");
-    if (n == 0) return WAE_OK;
-    CUDA_TRY(cudaSetDevice(b->engine->device));
-    // every item is validated before anything is enqueued
-    std::vector<WaveBindItem> table;
-    std::vector<size_t> wave_of;
-    std::vector<char> named(b->waves.size(), 0);
-    BindExtents extents{b->engine->device, {}};
-    int max_len = 0;
-    bool any_normalize = false;
-    for (uint32_t i = 0; i < n; i++) {
-        const wae_periodic_wave_binding& it = items[i];
-        if (it.graph_index >= b->n_graphs)
-            return fail(WAE_INVALID_STATE, "bind: graph index " + std::to_string(it.graph_index) + " is out of range");
-        auto wi = b->wave_index.find({b->batch_pos(it.graph_index), it.node});
-        if (wi == b->wave_index.end())
-            return fail(WAE_INVALID_STATE, "bind: node " + std::to_string(it.node) + " of graph " + std::to_string(it.graph_index) +
-                                               " is not a periodic wave bound from device memory (wae_oscillator_set_device_periodic_wave)");
-        const size_t k = wi->second;
-        if (named[k]++)  // (two items of one launch writing one wavetable: which one lands would be undefined)
-            return fail(WAE_INVALID_ARGUMENT, "bind: node " + std::to_string(it.node) + " of graph " + std::to_string(it.graph_index) +
-                                                  " is named twice in one call");
-        const wae_batch::DevWave& d = b->waves[k];
-        if (!it.real && !it.imag) return fail(WAE_INVALID_ARGUMENT, "bind: null real and imag");
-        const uint64_t bytes = (uint64_t)d.coefficients * sizeof(float);
-        for (const float* p : {it.real, it.imag}) {
-            if (!p) continue;
-            wae_status st = extents.check(p, bytes, p == it.real ? "real" : "imag",
-                                          "[coefficients, coefficients + count) runs past the end of its allocation");
-            if (st != WAE_OK) return st;
-        }
-        if (!d.d) continue;  // declared, never rendered: nothing to write
-        table.push_back(WaveBindItem{it.real, it.imag, d.d, (int32_t)d.coefficients, (int32_t)d.table_len, d.normalize ? 1 : 0, 0});
-        max_len = std::max(max_len, (int)d.table_len);
-        any_normalize = any_normalize || d.normalize;
-        wave_of.push_back(k);
-    }
-    if (table.empty()) return WAE_OK;
-    wae_status st = bind_after(b, stream);
-    if (st == WAE_OK) st = stage_bind_table(b, table.data(), table.size() * sizeof(WaveBindItem));
-    if (st != WAE_OK) return st;
-    launch_bind_waves(static_cast<const WaveBindItem*>(b->d_bind), (int)table.size(), max_len, any_normalize, b->engine->stream);
-    cudaError_t le = cudaGetLastError();
-    if (le != cudaSuccess) return fail(WAE_CUDA_ERROR, std::string("bind: ") + cudaGetErrorString(le));
-    for (size_t k : wave_of)
-        if (!b->waves[k].bound) {
-            b->waves[k].bound = true;
-            b->waves_unbound--;
-        }
-    return WAE_OK;
+    return bind_items<WaveBindItem>(
+        b, &wae_batch::waves, items, n, stream,
+        [](const wae_periodic_wave_binding& it, const DevWave& d, size_t, BindExtents& extents, auto& rows) -> wae_status {
+            if (!it.real && !it.imag) return fail(WAE_INVALID_ARGUMENT, "bind: null real and imag");
+            const uint64_t bytes = (uint64_t)d.coefficients * sizeof(float);
+            for (const float* p : {it.real, it.imag}) {
+                if (!p) continue;
+                wae_status st = extents.check(p, alignof(float), bytes, p == it.real ? "real" : "imag",
+                                              "[coefficients, coefficients + count) runs past the end of its allocation");
+                if (st != WAE_OK) return st;
+            }
+            if (d.d) rows.push_back(WaveBindItem{it.real, it.imag, d.d, (int32_t)d.coefficients, (int32_t)d.table_len, d.normalize ? 1 : 0, 0});
+            return WAE_OK;
+        },
+        [b](const WaveBindItem* dev, const std::vector<WaveBindItem>& rows) {
+            int max_len = 0;
+            bool any_normalize = false;
+            for (const WaveBindItem& r : rows) {
+                max_len = std::max(max_len, (int)r.len);
+                any_normalize = any_normalize || r.normalize != 0;
+            }
+            launch_bind_waves(dev, (int)rows.size(), max_len, any_normalize, b->engine->stream);
+        });
 }
 
 // The coefficient fields are rewritten on the engine stream: runs queued before the bind have read the previous ones.
 WAE_API wae_status wae_batch_bind_iir_coefficients(wae_batch* b, const wae_iir_binding* items, uint32_t n, void* stream) {
-    if (!b || (n && !items)) return fail(WAE_INVALID_ARGUMENT, "null batch / items");
-    if (n == 0) return WAE_OK;
-    CUDA_TRY(cudaSetDevice(b->engine->device));
-    // every item is validated before anything is enqueued
-    std::vector<IirBindItem> table;
-    std::vector<size_t> iir_of;
-    std::vector<char> named(b->iirs.size(), 0);
-    BindExtents extents{b->engine->device, {}};
-    for (uint32_t i = 0; i < n; i++) {
-        const wae_iir_binding& it = items[i];
-        if (it.graph_index >= b->n_graphs)
-            return fail(WAE_INVALID_STATE, "bind: graph index " + std::to_string(it.graph_index) + " is out of range");
-        auto ii = b->iir_index.find({b->batch_pos(it.graph_index), it.node});
-        if (ii == b->iir_index.end())
-            return fail(WAE_INVALID_STATE, "bind: node " + std::to_string(it.node) + " of graph " + std::to_string(it.graph_index) +
-                                               " is not an IIR filter bound from device memory (wae_iir_filter_set_device_coefficients)");
-        const size_t k = ii->second;
-        if (named[k]++)  // (two items of one launch writing one filter's records: which one lands would be undefined)
-            return fail(WAE_INVALID_ARGUMENT, "bind: node " + std::to_string(it.node) + " of graph " + std::to_string(it.graph_index) +
-                                                  " is named twice in one call");
-        const wae_batch::DevIir& d = b->iirs[k];
-        if (!it.feedforward || !it.feedback) return fail(WAE_INVALID_ARGUMENT, "bind: null feedforward / feedback");
-        if (((uintptr_t)it.feedforward | (uintptr_t)it.feedback) % alignof(double))
-            return fail(WAE_INVALID_ARGUMENT, "bind: feedforward / feedback is not 8-byte aligned");
-        wae_status st = extents.check(it.feedforward, (uint64_t)d.nff * sizeof(double), "feedforward",
-                                      "[feedforward, feedforward + count) runs past the end of its allocation");
-        if (st == WAE_OK)
-            st = extents.check(it.feedback, (uint64_t)d.nfb * sizeof(double), "feedback",
-                               "[feedback, feedback + count) runs past the end of its allocation");
-        if (st != WAE_OK) return st;
-        if (d.p0 == d.p1) continue;  // declared, never rendered: nothing to write
-        table.push_back(IirBindItem{it.feedforward, it.feedback, b->d_iir_patches + d.p0, (int32_t)d.nff, (int32_t)d.nfb, d.p1 - d.p0, 0});
-        iir_of.push_back(k);
-    }
-    if (table.empty()) return WAE_OK;
-    wae_status st = bind_after(b, stream);
-    if (st == WAE_OK) st = stage_bind_table(b, table.data(), table.size() * sizeof(IirBindItem));
-    if (st != WAE_OK) return st;
-    launch_bind_iir(static_cast<const IirBindItem*>(b->d_bind), (int)table.size(), b->engine->stream);
-    cudaError_t le = cudaGetLastError();
-    if (le != cudaSuccess) return fail(WAE_CUDA_ERROR, std::string("bind: ") + cudaGetErrorString(le));
-    for (size_t k : iir_of)
-        if (!b->iirs[k].bound) {
-            b->iirs[k].bound = true;
-            b->iirs_unbound--;
-        }
-    return WAE_OK;
+    return bind_items<IirBindItem>(
+        b, &wae_batch::iirs, items, n, stream,
+        [b](const wae_iir_binding& it, const DevIir& d, size_t, BindExtents& extents, auto& rows) -> wae_status {
+            wae_status st = extents.check(it.feedforward, alignof(double), (uint64_t)d.nff * sizeof(double), "feedforward",
+                                          "[feedforward, feedforward + count) runs past the end of its allocation");
+            if (st == WAE_OK)
+                st = extents.check(it.feedback, alignof(double), (uint64_t)d.nfb * sizeof(double), "feedback",
+                                   "[feedback, feedback + count) runs past the end of its allocation");
+            if (st == WAE_OK && d.p0 != d.p1)
+                rows.push_back(IirBindItem{it.feedforward, it.feedback, b->d_iir_patches + d.p0, (int32_t)d.nff, (int32_t)d.nfb, d.p1 - d.p0, 0});
+            return st;
+        },
+        [b](const IirBindItem* dev, const std::vector<IirBindItem>& rows) { launch_bind_iir(dev, (int)rows.size(), b->engine->stream); });
 }
 
 // The schedule fields are rewritten on the engine stream: runs queued before the bind have read the previous ones.
 WAE_API wae_status wae_batch_bind_schedules(wae_batch* b, const wae_schedule_binding* items, uint32_t n, void* stream) {
-    if (!b || (n && !items)) return fail(WAE_INVALID_ARGUMENT, "null batch / items");
-    if (n == 0) return WAE_OK;
-    CUDA_TRY(cudaSetDevice(b->engine->device));
-    // every item is validated before anything is enqueued
-    std::vector<SchedBindItem> table;
-    std::vector<size_t> schedule_of;
-    std::vector<char> named(b->schedules.size(), 0);
-    BindExtents extents{b->engine->device, {}};
-    for (uint32_t i = 0; i < n; i++) {
-        const wae_schedule_binding& it = items[i];
-        if (it.graph_index >= b->n_graphs)
-            return fail(WAE_INVALID_STATE, "bind: graph index " + std::to_string(it.graph_index) + " is out of range");
-        auto si = b->schedule_index.find({b->batch_pos(it.graph_index), it.node});
-        const std::string name = "node " + std::to_string(it.node) + " of graph " + std::to_string(it.graph_index);
-        if (si == b->schedule_index.end())
-            return fail(WAE_INVALID_STATE, "bind: " + name + " has no schedule bound from device memory (wae_source_set_device_schedule)");
-        const size_t k = si->second;
-        if (named[k]++)  // (two items of one launch writing one source's records: which one lands would be undefined)
-            return fail(WAE_INVALID_ARGUMENT, "bind: " + name + " is named twice in one call");
-        const wae_batch::DevSchedule& d = b->schedules[k];
-        if (!it.times) return fail(WAE_INVALID_ARGUMENT, "bind: null times");
-        if ((uintptr_t)it.times % alignof(double)) return fail(WAE_INVALID_ARGUMENT, "bind: times is not 8-byte aligned");
-        wae_status st = extents.check(it.times, (d.bind_stop ? 2 : 1) * sizeof(double), "times",
-                                      "[times, times + count) runs past the end of its allocation");
-        if (st != WAE_OK) return st;
-        if (d.p0 == d.p1) continue;  // declared, never rendered: nothing to write
-        table.push_back(SchedBindItem{it.times, b->d_sched_patches + d.p0, {d.lo[0], d.lo[1]}, {d.hi[0], d.hi[1]}, d.p1 - d.p0, d.bind_stop ? 1 : 0});
-        schedule_of.push_back(k);
-    }
-    if (table.empty()) return WAE_OK;
-    wae_status st = bind_after(b, stream);
-    if (st == WAE_OK) st = stage_bind_table(b, table.data(), table.size() * sizeof(SchedBindItem));
-    if (st != WAE_OK) return st;
-    launch_bind_schedules(static_cast<const SchedBindItem*>(b->d_bind), (int)table.size(), b->engine->stream);
-    cudaError_t le = cudaGetLastError();
-    if (le != cudaSuccess) return fail(WAE_CUDA_ERROR, std::string("bind: ") + cudaGetErrorString(le));
-    for (size_t k : schedule_of)
-        if (!b->schedules[k].bound) {
-            b->schedules[k].bound = true;
-            b->schedules_unbound--;
-        }
-    return WAE_OK;
+    return bind_items<SchedBindItem>(
+        b, &wae_batch::schedules, items, n, stream,
+        [b](const wae_schedule_binding& it, const DevSchedule& d, size_t, BindExtents& extents, auto& rows) -> wae_status {
+            wae_status st = extents.check(it.times, alignof(double), (d.bind_stop ? 2 : 1) * sizeof(double), "times",
+                                          "[times, times + count) runs past the end of its allocation");
+            if (st == WAE_OK && d.p0 != d.p1)
+                rows.push_back(SchedBindItem{it.times, b->d_sched_patches + d.p0, {d.lo[0], d.lo[1]}, {d.hi[0], d.hi[1]}, d.p1 - d.p0,
+                                             d.bind_stop ? 1 : 0});
+            return st;
+        },
+        [b](const SchedBindItem* dev, const std::vector<SchedBindItem>& rows) { launch_bind_schedules(dev, (int)rows.size(), b->engine->stream); });
 }
 
 // The declared values are rewritten on the engine stream: runs queued before the bind have read the previous ones.
 WAE_API wae_status wae_batch_bind_value_curves(wae_batch* b, const wae_value_curve_binding* items, uint32_t n, void* stream) {
-    if (!b || (n && !items)) return fail(WAE_INVALID_ARGUMENT, "null batch / items");
-    if (n == 0) return WAE_OK;
-    CUDA_TRY(cudaSetDevice(b->engine->device));
-    // every item is validated before anything is enqueued
-    std::vector<ValueCurveBindItem> table;
-    std::vector<size_t> curve_of;
-    std::vector<char> named(b->value_curves.size(), 0);
-    BindExtents extents{b->engine->device, {}};
-    int64_t max_len = 0;
-    for (uint32_t i = 0; i < n; i++) {
-        const wae_value_curve_binding& it = items[i];
-        if (it.graph_index >= b->n_graphs)
-            return fail(WAE_INVALID_STATE, "bind: graph index " + std::to_string(it.graph_index) + " is out of range");
-        auto ci = b->value_curve_index.find(std::make_tuple(b->batch_pos(it.graph_index), it.node, it.param_index));
-        const std::string name = "param " + std::to_string(it.param_index) + " of node " + std::to_string(it.node) + " of graph " +
-                                 std::to_string(it.graph_index);
-        if (ci == b->value_curve_index.end())
-            return fail(WAE_INVALID_STATE, "bind: " + name + " has no value curve bound from device memory (wae_param_set_device_value_curve)");
-        const size_t k = ci->second;
-        if (named[k]++)  // (two items of one launch writing one curve: which one lands would be undefined)
-            return fail(WAE_INVALID_ARGUMENT, "bind: " + name + " is named twice in one call");
-        const wae_batch::DevValueCurve& d = b->value_curves[k];
-        if (!it.values) return fail(WAE_INVALID_ARGUMENT, "bind: null values");
-        if ((uintptr_t)it.values % alignof(float)) return fail(WAE_INVALID_ARGUMENT, "bind: values is not 4-byte aligned");
-        wae_status st = extents.check(it.values, (uint64_t)d.length * sizeof(float), "values",
-                                      "[values, values + length) runs past the end of its allocation");
-        if (st != WAE_OK) return st;
-        if (!d.pool) continue;  // declared, never rendered: nothing to write
-        table.push_back(ValueCurveBindItem{it.values, d.pool + d.values_off, (int32_t)d.length, 0});
-        max_len = std::max<int64_t>(max_len, d.length);
-        curve_of.push_back(k);
-    }
-    if (table.empty()) return WAE_OK;
-    wae_status st = bind_after(b, stream);
-    if (st == WAE_OK) st = stage_bind_table(b, table.data(), table.size() * sizeof(ValueCurveBindItem));
-    if (st != WAE_OK) return st;
-    launch_bind_value_curves(static_cast<const ValueCurveBindItem*>(b->d_bind), (int)table.size(), max_len, b->engine->stream);
-    cudaError_t le = cudaGetLastError();
-    if (le != cudaSuccess) return fail(WAE_CUDA_ERROR, std::string("bind: ") + cudaGetErrorString(le));
-    for (size_t k : curve_of)
-        if (!b->value_curves[k].bound) {
-            b->value_curves[k].bound = true;
-            b->value_curves_unbound--;
-        }
-    return WAE_OK;
+    return bind_items<ValueCurveBindItem>(
+        b, &wae_batch::value_curves, items, n, stream,
+        [](const wae_value_curve_binding& it, const DevValueCurve& d, size_t, BindExtents& extents, auto& rows) -> wae_status {
+            wae_status st = extents.check(it.values, alignof(float), (uint64_t)d.length * sizeof(float), "values",
+                                          "[values, values + length) runs past the end of its allocation");
+            if (st == WAE_OK && d.pool) rows.push_back(ValueCurveBindItem{it.values, d.pool + d.values_off, (int32_t)d.length, 0});
+            return st;
+        },
+        [b](const ValueCurveBindItem* dev, const std::vector<ValueCurveBindItem>& rows) {
+            int64_t max_len = 0;
+            for (const ValueCurveBindItem& r : rows) max_len = std::max<int64_t>(max_len, r.n);
+            launch_bind_value_curves(dev, (int)rows.size(), max_len, b->engine->stream);
+        });
 }
 
 WAE_API wae_status wae_batch_sync(wae_batch* b) {
@@ -6136,34 +5777,13 @@ WAE_API wae_status wae_selftest_conv_fft(float* data, uint32_t mode) {
     return WAE_OK;
 }
 
-// a one-shot call renders the graphs before a caller could bind anything to their device inputs or device-bound params
+// a one-shot call renders the graphs before a caller could bind anything to their declarations
 static wae_status refuse_device_inputs(wae_graph* const* graphs, uint32_t n_graphs) {
-    for (uint32_t i = 0; graphs && i < n_graphs; i++) {
-        if (graphs[i] && graphs[i]->device_inputs)
-            return fail(WAE_INVALID_STATE, "graph " + std::to_string(i) + " has device inputs: render it with wae_batch_prepare (or _prepare_many), "
-                                           "wae_batch_bind_sources and wae_batch_run");
-        if (graphs[i] && graphs[i]->device_params)
-            return fail(WAE_INVALID_STATE, "graph " + std::to_string(i) + " has params bound from device memory: render it with wae_batch_prepare "
-                                           "(or _prepare_many), wae_batch_bind_params and wae_batch_run");
-        if (graphs[i] && graphs[i]->device_responses)
-            return fail(WAE_INVALID_STATE, "graph " + std::to_string(i) + " has convolver responses bound from device memory: render it with "
-                                           "wae_batch_prepare (or _prepare_many), wae_batch_bind_responses and wae_batch_run");
-        if (graphs[i] && graphs[i]->device_curves)
-            return fail(WAE_INVALID_STATE, "graph " + std::to_string(i) + " has WaveShaper curves bound from device memory: render it with "
-                                           "wae_batch_prepare (or _prepare_many), wae_batch_bind_curves and wae_batch_run");
-        if (graphs[i] && graphs[i]->device_waves)
-            return fail(WAE_INVALID_STATE, "graph " + std::to_string(i) + " has periodic waves bound from device memory: render it with "
-                                           "wae_batch_prepare (or _prepare_many), wae_batch_bind_periodic_waves and wae_batch_run");
-        if (graphs[i] && graphs[i]->device_iirs)
-            return fail(WAE_INVALID_STATE, "graph " + std::to_string(i) + " has IIR coefficients bound from device memory: render it with "
-                                           "wae_batch_prepare (or _prepare_many), wae_batch_bind_iir_coefficients and wae_batch_run");
-        if (graphs[i] && graphs[i]->device_value_curves)
-            return fail(WAE_INVALID_STATE, "graph " + std::to_string(i) + " has value curves bound from device memory: render it with "
-                                           "wae_batch_prepare (or _prepare_many), wae_batch_bind_value_curves and wae_batch_run");
-        if (graphs[i] && graphs[i]->device_schedules)
-            return fail(WAE_INVALID_STATE, "graph " + std::to_string(i) + " has schedules bound from device memory: render it with "
-                                           "wae_batch_prepare (or _prepare_many), wae_batch_bind_schedules and wae_batch_run");
-    }
+    for (uint32_t i = 0; graphs && i < n_graphs; i++)
+        for (const BindKind& kind : kBindKinds)
+            if (graphs[i] && graphs[i]->*kind.count)
+                return fail(WAE_INVALID_STATE, "graph " + std::to_string(i) + " has " + kind.plural + ": render it with wae_batch_prepare " +
+                                                   "(or _prepare_many), " + kind.bind + " and wae_batch_run");
     return WAE_OK;
 }
 
