@@ -533,17 +533,25 @@ WAE_API wae_status wae_batch_bind_sources(wae_batch* batch, const wae_source_bin
  * prepared batch renders any number of parameter sets (EQ, gain, pan, compressor settings drawn on the GPU) without being built and
  * planned again.  The param renders as a constant for the whole render, as a param with only a value does.  param_index numbers the
  * params as wae_param_event_push does.  Bindable: GainNode gain; BiquadFilterNode q, detune, frequency, gain (0..3); StereoPannerNode
- * pan; DynamicsCompressorNode attack, knee, ratio, release, threshold (0..4); AudioBufferSourceNode detune, playbackRate (0, 1).  A
+ * pan; DynamicsCompressorNode attack, knee, ratio, release, threshold (0..4); AudioBufferSourceNode detune, playbackRate (0, 1);
+ * OscillatorNode frequency, detune (0, 1).  A
  * bound value is clamped to [max(lo, minValue), min(hi, maxValue)], as AudioParam::set_value clamps to [minValue, maxValue].  The range
  * decides what is planned, never the value: a GainNode whose range excludes |gain| <= 1e-6 can never answer with silence, so its output
  * keeps the layout of its input.  An AudioBufferSourceNode's two ranges give the computed rates rate * 2^(detune / 1200) it may play
  * at: a source that does not loop, whose other param is not automated and whose rates are all > 0 is rendered time-parallel (give
  * detune a range: the default one allows a rate of 0), its output has a constant layout only when the clip lasts to the end of the
- * render at the highest rate; any other source takes the serial renderer, which is right for every value but slow.
+ * render at the highest rate; any other source takes the serial renderer, which is right for every value but slow.  An
+ * OscillatorNode keeps its fused path (k_chain, k_voice_sum) when every computed frequency frequency * 2^(detune / 1200) its ranges allow
+ * (the other param's range, or its current value when it is not declared) lies in (0, sampleRate / 2); a range that allows any other
+ * frequency answers WAE_UNSUPPORTED (bind such a pitch with wae_param_set_device_value_curve).  The rule is not needed while the other
+ * param is automated or driven at audio rate.  The other param may change after the declaration, so wae_batch_prepare and wae_batch_plan
+ * check the rule again and answer WAE_UNSUPPORTED, naming the graph and the node, when it no longer holds.  With a start time declared as
+ * well (wae_source_set_device_schedule) the two binds may come in either order.
  * Deviation: a non-finite bound value renders as the param's default value (the reference panics on a non-finite set_value, which a
- * device bind cannot do; this is its rule for a NaN computed value).
+ * device bind cannot do; this is its rule for a NaN computed value); an oscillator's frequency and detune take the default clamped to the
+ * declared range.
  * WAE_INVALID_ARGUMENT: lo > hi, a non-finite bound, or a range outside [minValue, maxValue].  WAE_UNSUPPORTED: another node kind or
- * param.  WAE_INVALID_STATE: the param has automation events or an audio-rate input, is declared twice, or the graph already has a
+ * param, or an oscillator pitch range that breaks the rule above.  WAE_INVALID_STATE: the param has automation events or an audio-rate input, is declared twice, or the graph already has a
  * suspend point; after the declaration, events (set_value included, also from a suspend callback) and wae_connect_param to it answer
  * WAE_INVALID_STATE.  wae_render_batch and wae_render_many answer WAE_INVALID_STATE on graphs with such params; wae_batch_plan plans
  * them with the param's current value clamped to the range. */

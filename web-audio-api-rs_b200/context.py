@@ -146,7 +146,9 @@ class AudioParam:
     def set_device_value(self, lo=None, hi=None):
         """wae_param_set_device_value (product only): the param's value is supplied per run from device memory by Batch.bind_params,
         clamped to [lo, hi] within [minValue, maxValue] (default: the whole range).  It renders as a constant over the render; until
-        bound, the batch is planned with the current value clamped to the range."""
+        bound, the batch is planned with the current value clamped to the range.  An OscillatorNode's frequency and detune need a range
+        whose computed frequencies (with the other param's range or value) all lie in (0, sampleRate / 2), so the whole range is refused
+        (WaeError status 4): bind a wider pitch with set_device_value_curve."""
         api = self._ctx._api
         if not api.is_product:
             raise B.WaeError(3, "params bound from device memory are a feature of the GPU engine")
@@ -1065,9 +1067,10 @@ class Batch:
 
     def bind_params(self, params, values, graphs=None):
         """wae_batch_bind_params: values[i][j] (a float32 CUDA tensor [n][k], or [n] for one param) becomes the value of params[j] in
-        context graphs[i] (default: 0..n-1).  `params`: AudioParams declared with set_device_value, one per column; a param of a context
-        built like the others shares its node id and index, so the params of context 0 name those of every context.  One call, ordered
-        after torch's current stream; the values are read on the engine stream, and the tensor is kept from reuse until they have been."""
+        context graphs[i] (default: 0..n-1).  `params`: AudioParams declared with set_device_value, one per column (an oscillator's
+        frequency / detune included: the bind re-derives its phase fields); a param of a context built like the others shares its node id
+        and index, so the params of context 0 name those of every context.  One call, ordered after torch's current stream; the values
+        are read on the engine stream, and the tensor is kept from reuse until they have been."""
         import torch
         if not (isinstance(values, torch.Tensor) and values.is_cuda and values.dtype == torch.float32 and values.dim() in (1, 2)):
             raise B.WaeError(1, "bind_params: values must be a float32 CUDA tensor [n] or [n][k]")

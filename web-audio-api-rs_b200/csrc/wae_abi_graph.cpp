@@ -601,7 +601,8 @@ WAE_API wae_status wae_connect_param(wae_graph* g, wae_node_id from, uint32_t ou
 
 // Params whose value stays constant over the render, so that a per-run value can be re-derived into the planned records (a GainNode's
 // gain, a BiquadFilterNode's four, a StereoPannerNode's pan, a DynamicsCompressorNode's five, an AudioBufferSourceNode's detune and
-// playbackRate: the planner picks the source's playback path from the declared range)
+// playbackRate: the planner picks the source's playback path from the declared range; an OscillatorNode's frequency and detune, whose
+// computed frequencies the range keeps inside (0, sampleRate / 2): see osc_pitch_allowed)
 static bool device_value_supported(Kind kind, uint32_t param_index) {
     switch (kind) {
         case K_GAIN: return param_index == 0;
@@ -609,8 +610,28 @@ static bool device_value_supported(Kind kind, uint32_t param_index) {
         case K_SPANNER: return param_index == 0;
         case K_COMP: return param_index < 5;
         case K_ABSN: return param_index < 2;
+        case K_OSC: return param_index < 2;
         default: return false;
     }
+}
+
+// An oscillator's frequency (index 0) or detune (1) declared over [lo, hi]: the computed frequencies it allows, with the other param's
+// declared range or current value, must all lie inside (0, sampleRate / 2), so that the planner's choice of path holds for every bound
+// value.  Not needed while the other param is automated or driven at audio rate: the a-rate kernel takes the bound value raw.  The
+// planner checks the rule again when it lowers the node (the other param may change after this call).
+static bool osc_pitch_allowed(const wae_graph* g, const Node& n, uint32_t param_index, float lo, float hi, std::string& range) {
+    const Param& other = g->nodes.at(n.params[1 - param_index]).param;
+    if (!other.constant()) return true;
+    for (const auto& kv : g->nodes)
+        for (const Edge& e : kv.second.outgoing)
+            if (e.other_id == n.params[1 - param_index]) return true;
+    const float olo = other.device_bound ? other.device_lo : other.constant_value();
+    const float ohi = other.device_bound ? other.device_hi : other.constant_value();
+    const float f_lo = param_index == 0 ? lo : olo, f_hi = param_index == 0 ? hi : ohi;
+    const float d_lo = param_index == 1 ? lo : olo, d_hi = param_index == 1 ? hi : ohi;
+    range = "frequency [" + std::to_string(f_lo) + ", " + std::to_string(f_hi) + "] Hz, detune [" + std::to_string(d_lo) + ", " +
+            std::to_string(d_hi) + "] cents";
+    return hostmath::osc_pitch_inside(f_lo, f_hi, d_lo, d_hi, (double)g->sample_rate);
 }
 
 WAE_API wae_status wae_param_set_device_value(wae_graph* g, wae_node_id node, uint32_t param_index, float lo, float hi) {
@@ -622,8 +643,8 @@ WAE_API wae_status wae_param_set_device_value(wae_graph* g, wae_node_id node, ui
     if (!device_value_supported(n->kind, param_index))
         return fail(WAE_UNSUPPORTED, "param " + std::to_string(param_index) + " of node " + std::to_string(node) +
                                          " cannot be bound from device memory (GainNode gain, BiquadFilterNode q / detune / frequency / gain, "
-                                         "StereoPannerNode pan, DynamicsCompressorNode params and AudioBufferSourceNode detune / "
-                                         "playbackRate can)");
+                                         "StereoPannerNode pan, DynamicsCompressorNode params, AudioBufferSourceNode detune / "
+                                         "playbackRate and OscillatorNode frequency / detune can)");
     const uint32_t pid = n->params[param_index];
     Param& p = g->nodes.at(pid).param;
     if (p.device_bound) return fail(WAE_INVALID_STATE, "InvalidStateError - the param is already bound from device memory");
@@ -635,6 +656,11 @@ WAE_API wae_status wae_param_set_device_value(wae_graph* g, wae_node_id node, ui
             if (e.other_id == pid) return fail(WAE_INVALID_STATE, "InvalidStateError - the param has an audio-rate input (connect_param)");
     const float l = std::max(lo, p.min_value), h = std::min(hi, p.max_value);
     if (l > h) return fail(WAE_INVALID_ARGUMENT, "device value range lies outside the param's [minValue, maxValue]");
+    std::string range;
+    if (n->kind == K_OSC && !osc_pitch_allowed(g, *n, param_index, l, h, range))
+        return fail(WAE_UNSUPPORTED, "OscillatorNode " + std::to_string(node) + ": " + range + " allow computed frequencies outside (0, " +
+                                         std::to_string(g->sample_rate / 2.f) + ") Hz; a pitch bound from device memory must stay inside "
+                                         "it (bind a wider pitch as a value curve: wae_param_set_device_value_curve)");
     p.device_bound = true;
     p.device_lo = l;
     p.device_hi = h;

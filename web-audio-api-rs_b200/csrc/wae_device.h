@@ -617,11 +617,11 @@ enum SchedKind : int32_t {
 struct SchedPatch {
     void* dst;            // the record
     int32_t kind;
-    int32_t flag;         // SCHED_OSC*: outside Nyquist; SCHED_ABSN_BOUND: fast_ok but for the start and stop (sampling ratio 1, default
-                          // loop points, no duration)
+    int32_t flag;         // SCHED_ABSN_BOUND: fast_ok but for the start and stop (sampling ratio 1, default loop points, no duration)
     float sample_rate;    // the graph's (the clock)
     int32_t pad;
-    double incr;          // SCHED_OSC*: the phase increment per frame
+    double* start_out;    // SCHED_OSC of an oscillator whose pitch is bound from device memory: the clamped start is also written here,
+                          // where its PATCH_OSC entry reads it (nullptr: none).  SCHED_OSC* take the phase increment from the record.
     double offset;        // SCHED_ABSN_BOUND: start(when, offset)
     double duration;      // SCHED_ABSN_BOUND: the buffer's duration
     double stop_time;     // the planned stop time, taken when the stop is not bound (>= 1e300: none)
@@ -653,12 +653,14 @@ enum PatchKind : int32_t {
     PATCH_BIQUAD = 2,  // operands q, detune, frequency, gain: double *dst = b0, b1, b2, a1, a2; ScanCoef *dst2 (k_chain) or nullptr
     PATCH_SPAN = 3,    // operand pan: float *dst = pan, float2 *dst2 = the stereo gains for n input channels
     PATCH_RAW = 4,     // float *dst = operand 0
+    PATCH_OSC = 5,     // operands frequency, detune: OscInst *dst = incr, inv_incr, outside_nyquist, and phase0 from the start time at
+                       // const double *dst2 (the planned one, or the slot a bound schedule writes: SchedPatch::start_out)
 };
 constexpr int PATCH_OPS = 8;
 struct ParamPatch {
     int32_t kind;
     int32_t n;          // PATCH_GAIN / PATCH_META: operands; PATCH_BIQUAD: filter type; PATCH_SPAN: input channels
-    float sample_rate;  // PATCH_BIQUAD
+    float sample_rate;  // PATCH_BIQUAD, PATCH_OSC
     int32_t pad;
     void* dst;
     void* dst2;

@@ -1016,8 +1016,9 @@ struct Planner {
         int phase = 0;  // 0: before biquad A, 1: after A, 3: after B, 5: after the shaper (canonical chain order)
         int cls = 0;    // scheduling class of the node that opened the chain (see stage())
         Lay lay;        // layout of the chain's output over time (the kernel writes the track when it is not constant)
-        // params bound from device memory: biquad k's patch entries (rec2 = k until the chain is emitted), and per gain slot the factors
-        // folded into it since the first bound one (gain_fold[s].p.n == 0: the slot has none)
+        // params bound from device memory: the source oscillator's PATCH_OSC entry and biquad k's patch entries (rec2 = k until the
+        // chain is emitted), and per gain slot the factors folded into it since the first bound one (gain_fold[s].p.n == 0: the slot
+        // has none)
         std::vector<PatchRec> patches;
         PatchRec gain_fold[4] = {};
         // a shaper whose curve is bound from device memory: the entry of shaper_keeps_silence (rec / off set when the chain is emitted)
@@ -1243,8 +1244,13 @@ struct Planner {
     // a chain's patch entries for its record at index `rec` of stage `s` (emit_chain, sum_voices)
     static void chain_patches(StageBuild& s, const PendingChain& pc, int32_t rec) {
         for (PatchRec r : pc.patches) {
-            const int k = r.rec2;
             r.rec = rec;
+            if (r.p.kind == PATCH_OSC) {  // the source oscillator's pitch
+                r.off = (uint32_t)offsetof(ChainInst, osc);
+                s.patches.push_back(r);
+                continue;
+            }
+            const int k = r.rec2;
             r.rec2 = pc.inst.bq[k].coef;
             r.off = (uint32_t)(offsetof(ChainInst, bq) + (size_t)k * sizeof(ChainBiquad) + offsetof(ChainBiquad, b0));
             s.patches.push_back(r);
@@ -2362,14 +2368,35 @@ bool Planner::lower_osc(NodeCtx& nc) {
     }
     // a schedule bound from device memory: the fields the times reach are re-derived by the bind (planned with the windows' low ends)
     SchedPatch sched{};
-    if (n.device_schedule) {
-        sched = sched_entry(n, nc.dyn_params ? SCHED_OSC_AR : SCHED_OSC);
-        sched.incr = o.incr;
-        sched.flag = o.outside_nyquist;
-    }
+    if (n.device_schedule) sched = sched_entry(n, nc.dyn_params ? SCHED_OSC_AR : SCHED_OSC);
     SchedPatch meta_sched = sched;
     meta_sched.kind = SCHED_META_OSC;
     const SchedPatch* track_sched = n.device_schedule ? &meta_sched : nullptr;
+    // frequency / detune bound from device memory, planned with their placeholders.  With the other param automated the a-rate kernel
+    // takes the bound value raw (PATCH_RAW into f_val / d_val).  Otherwise the declared ranges keep every computed frequency inside
+    // (0, Nyquist), so the path and OscInst::fast hold for every value, and a PATCH_OSC entry re-derives the phase fields per bind: from
+    // the planned start time, or from the slot a bound schedule writes its start into.
+    const bool pitch_bound = pf.bound >= 0 || pd.bound >= 0;
+    PatchRec pitch = patch(PATCH_OSC, 2);
+    if (pitch_bound && !nc.dyn_params) {
+        const double f_lo = pf.bound >= 0 ? pf.lo : freq, f_hi = pf.bound >= 0 ? pf.hi : freq;
+        const double d_lo = pd.bound >= 0 ? pd.lo : detune, d_hi = pd.bound >= 0 ? pd.hi : detune;
+        if (!hm::osc_pitch_inside(f_lo, f_hi, d_lo, d_hi, sr)) {
+            const uint32_t caller = b->order.empty() ? gi : b->order[gi];
+            return bail(WAE_UNSUPPORTED, "graph " + std::to_string(caller) + ", OscillatorNode " + std::to_string(n.id) +
+                                             ": the pitch bound from device memory allows computed frequencies outside (0, sampleRate / 2) "
+                                             "with frequency [" + std::to_string(f_lo) + ", " + std::to_string(f_hi) + "] Hz and detune [" +
+                                             std::to_string(d_lo) + ", " + std::to_string(d_hi) +
+                                             "] cents (bind a wider pitch as a value curve: wae_param_set_device_value_curve)");
+        }
+        operand(pitch, 0, pf, freq);
+        operand(pitch, 1, pd, detune);
+        pitch.p.sample_rate = g->sample_rate;
+        double* start = upload(std::vector<double>{n.start_time});
+        if (!start) return bail(WAE_OUT_OF_MEMORY, "out of device memory (oscillator start time)");
+        pitch.p.dst2 = start;
+        if (n.device_schedule) sched.start_out = start;
+    }
     if (n.type == WAE_OSC_CUSTOM && n.device_wave) {  // a wave bound from device memory: planned as a host wave of its length
         o.table = device_wave(n);
         o.table_len = (int)n.device_wave_len;
@@ -2398,17 +2425,27 @@ bool Planner::lower_osc(NodeCtx& nc) {
         StageBuild& sb = stage(nc.L, S_OSC_AR);
         sb.osc_ar.push_back(oa);
         if (n.device_schedule) add_sched_patch(sb, n, sched);
+        const PRef* refs[2] = {&pf, &pd};
+        const size_t offs[2] = {offsetof(OscArInst, f_val), offsetof(OscArInst, d_val)};
+        for (int i = 0; i < 2; i++)
+            if (refs[i]->bound >= 0) {
+                PatchRec r = patch(PATCH_RAW, 1);
+                operand(r, 0, *refs[i], refs[i]->v);
+                add_patch(sb, r, (uint32_t)offs[i]);
+            }
     } else if (nc.fuse_n) {
         PendingChain pc = source_chain(CHAIN_SRC_OSC, 1);
         pc.inst.osc = o;
         pc.lay = source_lay(o.n_first, o.n_stop, 1, n.device_schedule);
         if (n.device_schedule) pc.sched_patches.push_back(StageBuild::SchedPatchRec{gi, n.id, -1, (uint32_t)offsetof(ChainInst, osc), sched});
+        if (pitch_bound) pc.patches.push_back(pitch);  // (rec / off set when the chain is emitted)
         return finish_chain(nc, std::move(pc));
     } else {
         o.out = source_out(nc, o.n_first, o.n_stop, 1, track_sched);
         StageBuild& sb = stage(nc.L, S_OSC);
         sb.osc.push_back(o);
         if (n.device_schedule) add_sched_patch(sb, n, sched);
+        if (pitch_bound) add_patch(sb, pitch, 0);
     }
     return true;
 }
@@ -4402,12 +4439,13 @@ static void prep_plan_group(wae_batch* b, wae_graph* const* graphs, int k, PrepS
             if (st.n > 0) {  // patch entries: the device addresses of the fields they set
                 const size_t rec_size = s.record_bytes();
                 auto rec = [&](int32_t k) { return static_cast<char*>(st.d_a) + (size_t)k * rec_size; };
-                // params: the field and the scan constants (S_CHAIN / S_VSUM) or stereo gains (S_SPAN) it re-derives
+                // params: the field and the scan constants (S_CHAIN / S_VSUM) or stereo gains (S_SPAN) it re-derives (PATCH_OSC: dst2 is
+                // the start time's address, set by the planner)
                 const size_t rec2_size = s.kind == S_SPAN ? sizeof(float2) : sizeof(ScanCoef);
                 for (const PatchRec& pr : s.patches) {
                     ParamPatch p = pr.p;
                     p.dst = rec(pr.rec) + pr.off;
-                    p.dst2 = pr.rec2 >= 0 ? static_cast<char*>(st.d_b) + (size_t)pr.rec2 * rec2_size : nullptr;
+                    if (pr.rec2 >= 0) p.dst2 = static_cast<char*>(st.d_b) + (size_t)pr.rec2 * rec2_size;
                     gp.patches.push_back({pr.graph, p});
                 }
                 for (const auto& cp : s.curve_patches)  // curves: the int32 field
@@ -4558,8 +4596,11 @@ static wae_status record_params(wae_batch* b, wae_graph* const* graphs, uint32_t
         if (nd.kind == K_PARAM) return;
         for (uint32_t i = 0; i < nd.params.size(); i++) {
             const Param& prm = nodes.at(nd.params[i]).param;
-            if (prm.device_bound)
-                declare({j, nd.id, i}, DevParam{nd.params[i], ParamSlotInfo{prm.device_lo, prm.device_hi, prm.default_value, 0}}, false);
+            if (!prm.device_bound) continue;
+            // a non-finite value takes the default value; an oscillator's pitch takes it clamped to the range, which keeps the bound
+            // pitch inside the range its plan was checked for
+            const float def = nd.kind == K_OSC ? std::min(std::max(prm.default_value, prm.device_lo), prm.device_hi) : prm.default_value;
+            declare({j, nd.id, i}, DevParam{nd.params[i], ParamSlotInfo{prm.device_lo, prm.device_hi, def, 0}}, false);
         }
     });
     if (b->params.keys.empty()) return WAE_OK;

@@ -91,6 +91,16 @@ inline BiquadCoefs biquad_coefs(int type, double sample_rate, double f0, double 
 // get_computed_freq, src/node/biquad_filter.rs:393-399 (f32)
 inline float biquad_computed_freq(float freq, float detune) { return detune != 0.f ? freq * exp2f(detune / 1200.f) : freq; }
 
+// An OscillatorNode whose frequency and detune are bound from device memory: every computed frequency f * 2^(d / 1200)
+// (oscillator.rs:30-32) that f in [f_lo, f_hi], d in [d_lo, d_hi] allow lies inside (0, sample_rate / 2).  Then every value renders on
+// the path the planner picks from one of them (inside Nyquist, OscInst::fast the same).  The product is monotone in both once f > 0, so
+// the corners decide.  The top keeps a relative margin of a few ulps below Nyquist: the device's exp2 may round its last bit the other
+// way than glibc's.
+inline bool osc_pitch_inside(double f_lo, double f_hi, double d_lo, double d_hi, double sample_rate) {
+    const double lo = f_lo * std::exp2(d_lo / 1200.), hi = f_hi * std::exp2(d_hi / 1200.);
+    return f_lo > 0. && lo > 0. && hi < sample_rate / 2. * (1. - 8. * std::numeric_limits<double>::epsilon());
+}
+
 // sine table, src/node/oscillator.rs:16-28
 inline std::vector<float> sine_table() {
     std::vector<float> t(2048);

@@ -4610,18 +4610,23 @@ __global__ void __launch_bounds__(128) k_bind_schedules(const SchedBindItem* __r
             case SCHED_OSC:
             case SCHED_OSC_AR:
             case SCHED_META_OSC: {
-                const OscStart s = osc_start(clock, start, p.incr, p.flag != 0);
+                // the phase increment is the record's own: planned, or re-derived by the oscillator's pitch bound from device memory
+                // (PATCH_OSC), which reads the start written to start_out — either bind sees the other's current value
+                OscInst* o = p.kind == SCHED_META_OSC ? nullptr
+                             : p.kind == SCHED_OSC_AR ? &reinterpret_cast<OscArInst*>(d)->base
+                                                      : reinterpret_cast<OscInst*>(d);
+                const OscStart s = osc_start(clock, start, o ? o->incr : 0., o && o->outside_nyquist != 0);
                 const int64_t n_stop = osc_stop_frame(clock, stop);
-                if (p.kind == SCHED_META_OSC) {
+                if (!o) {
                     reinterpret_cast<MetaInst*>(d)->n_first = s.n_first;
                     reinterpret_cast<MetaInst*>(d)->n_stop = n_stop;
                     break;
                 }
-                OscInst* o = p.kind == SCHED_OSC_AR ? &reinterpret_cast<OscArInst*>(d)->base : reinterpret_cast<OscInst*>(d);
                 o->n_first = s.n_first;
                 o->n_stop = n_stop;
                 o->phase0 = s.phase0;
                 if (p.kind == SCHED_OSC_AR) reinterpret_cast<OscArInst*>(d)->start_ratio = s.start_ratio;
+                if (p.start_out) *p.start_out = start;
                 break;
             }
             case SCHED_CONST:
@@ -4883,6 +4888,20 @@ __global__ void __launch_bounds__(64) k_derive_params(const ParamPatch* __restri
             const float x = p.n == 1 ? (pan + 1.f) * 0.5f : (pan <= 0.f ? pan + 1.f : pan);
             *static_cast<float*>(p.dst) = pan;
             *static_cast<float2*>(p.dst2) = make_float2(sinf((1.f - x) * PI32 / 2.f), sinf(x * PI32 / 2.f));
+            break;
+        }
+        case PATCH_OSC: {  // Planner::lower_osc's f64 expressions (OscInst::fast stays the planner's: the declared range keeps it)
+            const float freq = patch_op(p, 0, values), detune = patch_op(p, 1, values);
+            const double sr = (double)p.sample_rate;
+            const double computed_freq = (double)freq * exp2((double)detune / 1200.);  // oscillator.rs:30-32
+            OscInst* o = static_cast<OscInst*>(p.dst);
+            const double incr = computed_freq / sr;
+            const bool outside = fabs(computed_freq) >= sr / 2.;
+            o->incr = incr;
+            o->inv_incr = incr != 0. ? 1. / incr : 0.;
+            o->outside_nyquist = outside;
+            const double start = *static_cast<const double*>(p.dst2);
+            o->phase0 = start < 1e300 ? osc_start(SchedClock(p.sample_rate), start, incr, outside).phase0 : 0.;
             break;
         }
         default: *static_cast<float*>(p.dst) = patch_op(p, 0, values); break;
