@@ -534,7 +534,8 @@ WAE_API wae_status wae_batch_bind_sources(wae_batch* batch, const wae_source_bin
  * planned again.  The param renders as a constant for the whole render, as a param with only a value does.  param_index numbers the
  * params as wae_param_event_push does.  Bindable: GainNode gain; BiquadFilterNode q, detune, frequency, gain (0..3); StereoPannerNode
  * pan; DynamicsCompressorNode attack, knee, ratio, release, threshold (0..4); AudioBufferSourceNode detune, playbackRate (0, 1);
- * OscillatorNode frequency, detune (0, 1).  A
+ * OscillatorNode frequency, detune (0, 1); PannerNode positionX/Y/Z, orientationX/Y/Z (0..5); the AudioListener's positionX/Y/Z,
+ * forwardX/Y/Z, upX/Y/Z (0..8, addressed as node 1: declaring one creates the listener, as wae_connect_param does).  A
  * bound value is clamped to [max(lo, minValue), min(hi, maxValue)], as AudioParam::set_value clamps to [minValue, maxValue].  The range
  * decides what is planned, never the value: a GainNode whose range excludes |gain| <= 1e-6 can never answer with silence, so its output
  * keeps the layout of its input.  An AudioBufferSourceNode's two ranges give the computed rates rate * 2^(detune / 1200) it may play
@@ -546,12 +547,19 @@ WAE_API wae_status wae_batch_bind_sources(wae_batch* batch, const wae_source_bin
  * frequency answers WAE_UNSUPPORTED (bind such a pitch with wae_param_set_device_value_curve).  The rule is not needed while the other
  * param is automated or driven at audio rate.  The other param may change after the declaration, so wae_batch_prepare and wae_batch_plan
  * check the rule again and answer WAE_UNSUPPORTED, naming the graph and the node, when it no longer holds.  With a start time declared as
- * well (wae_source_set_device_schedule) the two binds may come in either order.
+ * well (wae_source_set_device_schedule) the two binds may come in either order.  A PannerNode whose position, orientation or listener is
+ * declared keeps the lowering of its placeholder (equal-power or HRTF, static or moving when another of its 15 spatial params is
+ * automated).  Its range, and a listener param's, must lie inside [-1e9, 1e9], where the f32 spatial math (squared differences, the
+ * cross product of forward and up) stays finite; a wider range, the default one included, answers WAE_UNSUPPORTED.  A static HRTF panner
+ * lowered to a convolver gets response spectra of its own (2 x 24 x 8192 float2, 3 MiB), which every
+ * wae_batch_bind_params rewrites.  A listener param reaches every panner of its graph; in a graph without a panner it is validated and
+ * reaches nothing, and runs still wait for its bind.  Bound spatial math runs on the device (acosf, sinf / cosf, pow), which may round the
+ * last bit differently from the host: near a face of the HRIR sphere the device may pick the neighbouring triangle.
  * Deviation: a non-finite bound value renders as the param's default value (the reference panics on a non-finite set_value, which a
  * device bind cannot do; this is its rule for a NaN computed value); an oscillator's frequency and detune take the default clamped to the
  * declared range.
  * WAE_INVALID_ARGUMENT: lo > hi, a non-finite bound, or a range outside [minValue, maxValue].  WAE_UNSUPPORTED: another node kind or
- * param, or an oscillator pitch range that breaks the rule above.  WAE_INVALID_STATE: the param has automation events or an audio-rate input, is declared twice, or the graph already has a
+ * param, an oscillator pitch range that breaks the rule above, or a spatial range beyond [-1e9, 1e9].  WAE_INVALID_STATE: the param has automation events or an audio-rate input, is declared twice, or the graph already has a
  * suspend point; after the declaration, events (set_value included, also from a suspend callback) and wae_connect_param to it answer
  * WAE_INVALID_STATE.  wae_render_batch and wae_render_many answer WAE_INVALID_STATE on graphs with such params; wae_batch_plan plans
  * them with the param's current value clamped to the range. */
@@ -569,8 +577,10 @@ typedef struct wae_param_binding {
  * panner gains, compressor settings) in every render segment.  All-or-nothing: every item is validated before anything is enqueued.
  * Bound values stay until they are bound again.  WAE_INVALID_ARGUMENT: `value` is null, not 4-byte aligned, not device (or managed)
  * memory of the engine's GPU or its 4 bytes are not in one allocation, or one param is named twice in the call.  WAE_INVALID_STATE:
- * graph_index out of range, or the
- * param was not declared.  wae_batch_run, wae_batch_run_group and wae_batch_run_pipelined answer WAE_INVALID_STATE while a declared
+ * graph_index out of range, the param was not declared, or the batch has HRTF panners whose source or listener is bound and
+ * wae_engine_set_hrir_sphere has replaced the sphere since the batch was prepared (nothing is enqueued: prepare the batch again).  The
+ * spatial values re-derive each static panner's direction and gains, and for HRTF its triangle, weights and, for one lowered to a
+ * convolver, its blended response and spectra.  wae_batch_run, wae_batch_run_group and wae_batch_run_pipelined answer WAE_INVALID_STATE while a declared
  * param of the batch has never been bound. */
 WAE_API wae_status wae_batch_bind_params(wae_batch* batch, const wae_param_binding* items, uint32_t n, void* stream);
 

@@ -148,15 +148,16 @@ class AudioParam:
         clamped to [lo, hi] within [minValue, maxValue] (default: the whole range).  It renders as a constant over the render; until
         bound, the batch is planned with the current value clamped to the range.  An OscillatorNode's frequency and detune need a range
         whose computed frequencies (with the other param's range or value) all lie in (0, sampleRate / 2), so the whole range is refused
-        (WaeError status 4): bind a wider pitch with set_device_value_curve."""
+        (WaeError status 4): bind a wider pitch with set_device_value_curve.  A PannerNode's position and orientation and the
+        AudioListener's position, forward and up are bindable too, over a range inside [-1e9, 1e9] (a wider one, the default
+        included, is refused with status 4): a static panner keeps its static lowering (HRTF as a convolver included), and the bind
+        re-derives its direction, gains and HRTF response."""
         api = self._ctx._api
         if not api.is_product:
             raise B.WaeError(3, "params bound from device memory are a feature of the GPU engine")
-        if self._node == "listener":
-            raise B.WaeError(4, "AudioListener params cannot be bound from device memory")
         lo = -3.4028234663852886e38 if lo is None else float(lo)
         hi = 3.4028234663852886e38 if hi is None else float(hi)
-        api.check(api.param_set_device_value(self._ctx._g, self._node, self._index, lo, hi))
+        api.check(api.param_set_device_value(self._ctx._g, 1 if self._node == "listener" else self._node, self._index, lo, hi))
         return self
 
     def set_device_value_curve(self, length, start_time, duration):
@@ -938,8 +939,8 @@ class Batch:
     def bind_value_curves(self, params, values, graphs=None):
         """wae_batch_bind_value_curves: values[j][i] (a float32 CUDA tensor [n][length] per param, unit stride on the last dimension)
         becomes the curve of params[j] (declared with set_device_value_curve) in context graphs[i] (default: 0..n-1).  `params`: one
-        AudioParam or a list; a param of a context built like the others shares its node id and index, so the params of context 0 name
-        those of every context.  `values`: one tensor, or a list of tensors, one per param.  One call, ordered after torch's current
+        AudioParam or a list (AudioListener params are not bound as curves); a param of a context built like the others shares its node
+        id and index, so the params of context 0 name those of every context.  `values`: one tensor, or a list of tensors, one per param.  One call, ordered after torch's current
         stream; the values are copied on the engine stream, and the tensors' memory is kept from reuse until they have been."""
         import torch
         params = list(params) if isinstance(params, (list, tuple)) else [params]
@@ -1068,8 +1069,9 @@ class Batch:
     def bind_params(self, params, values, graphs=None):
         """wae_batch_bind_params: values[i][j] (a float32 CUDA tensor [n][k], or [n] for one param) becomes the value of params[j] in
         context graphs[i] (default: 0..n-1).  `params`: AudioParams declared with set_device_value, one per column (an oscillator's
-        frequency / detune included: the bind re-derives its phase fields); a param of a context built like the others shares its node id
-        and index, so the params of context 0 name those of every context.  One call, ordered after torch's current stream; the values
+        frequency / detune included: the bind re-derives its phase fields; a PannerNode's position / orientation and the AudioListener's
+        position / forward / up included: the bind re-derives the panner's direction, gains and HRTF response); a param of a context built
+        like the others shares its node id and index, so the params of context 0 name those of every context.  One call, ordered after torch's current stream; the values
         are read on the engine stream, and the tensor is kept from reuse until they have been."""
         import torch
         if not (isinstance(values, torch.Tensor) and values.is_cuda and values.dtype == torch.float32 and values.dim() in (1, 2)):
@@ -1085,10 +1087,9 @@ class Batch:
         s0, s1 = v2.stride()
         for i, g in enumerate(graphs):
             for j, prm in enumerate(params):
-                if prm._node == "listener":
-                    raise B.WaeError(2, "bind_params: AudioListener params are not bound from device memory")
                 ptr = C.cast(C.c_void_p(base + 4 * (i * s0 + j * s1)), B.c_float_p)
-                items[i * k + j] = B.ParamBinding(g, int(prm._node), int(prm._index), ptr)
+                node = 1 if prm._node == "listener" else int(prm._node)
+                items[i * k + j] = B.ParamBinding(g, node, int(prm._index), ptr)
         self._bind(self.api.batch_bind_params, items, n * k, values)
 
     def output_tensor(self, i=None):

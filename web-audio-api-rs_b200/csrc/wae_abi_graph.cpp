@@ -602,7 +602,8 @@ WAE_API wae_status wae_connect_param(wae_graph* g, wae_node_id from, uint32_t ou
 // Params whose value stays constant over the render, so that a per-run value can be re-derived into the planned records (a GainNode's
 // gain, a BiquadFilterNode's four, a StereoPannerNode's pan, a DynamicsCompressorNode's five, an AudioBufferSourceNode's detune and
 // playbackRate: the planner picks the source's playback path from the declared range; an OscillatorNode's frequency and detune, whose
-// computed frequencies the range keeps inside (0, sampleRate / 2): see osc_pitch_allowed)
+// computed frequencies the range keeps inside (0, sampleRate / 2): see osc_pitch_allowed; a PannerNode's position and orientation and the
+// AudioListener's position, forward and up: no lowering decision reads their values, and kSpatialBound keeps their arithmetic finite)
 static bool device_value_supported(Kind kind, uint32_t param_index) {
     switch (kind) {
         case K_GAIN: return param_index == 0;
@@ -611,6 +612,8 @@ static bool device_value_supported(Kind kind, uint32_t param_index) {
         case K_COMP: return param_index < 5;
         case K_ABSN: return param_index < 2;
         case K_OSC: return param_index < 2;
+        case K_PANNER: return param_index < 6;
+        case K_LISTENER: return param_index < 9;
         default: return false;
     }
 }
@@ -634,8 +637,16 @@ static bool osc_pitch_allowed(const wae_graph* g, const Node& n, uint32_t param_
     return hostmath::osc_pitch_inside(f_lo, f_hi, d_lo, d_hi, (double)g->sample_rate);
 }
 
+// A spatial param (a PannerNode's position / orientation, the AudioListener's position / forward / up) bound from device memory must keep
+// its values inside [-kSpatialBound, kSpatialBound].  The spatial math is f32 (wae_spatial.h): it squares source - listener differences
+// (up to 2 x the bound per axis) and the cross product of forward and up (up to 2 x bound^2 per axis), and 12 x (1e9)^4 = 1.2e37 still lies
+// below FLT_MAX; wider values overflow to inf and the direction and gains the bind derives turn into NaN.  Metres, or unit vectors: a scene
+// never comes near it, and the default range (the whole f32 line) is refused.
+constexpr float kSpatialBound = 1e9f;
+
 WAE_API wae_status wae_param_set_device_value(wae_graph* g, wae_node_id node, uint32_t param_index, float lo, float hi) {
     if (!g) return fail(WAE_INVALID_ARGUMENT, "null graph");
+    if (node == 1) g->ensure_listener();  // BaseAudioContext::listener() creates it on first access (context/mod.rs)
     Node* n = g->nodes.get(node);
     if (!n || n->kind == K_PARAM || param_index >= n->params.size()) return fail(WAE_INVALID_ARGUMENT, "unknown param");
     if (!std::isfinite(lo) || !std::isfinite(hi) || lo > hi)
@@ -644,7 +655,8 @@ WAE_API wae_status wae_param_set_device_value(wae_graph* g, wae_node_id node, ui
         return fail(WAE_UNSUPPORTED, "param " + std::to_string(param_index) + " of node " + std::to_string(node) +
                                          " cannot be bound from device memory (GainNode gain, BiquadFilterNode q / detune / frequency / gain, "
                                          "StereoPannerNode pan, DynamicsCompressorNode params, AudioBufferSourceNode detune / "
-                                         "playbackRate and OscillatorNode frequency / detune can)");
+                                         "playbackRate, OscillatorNode frequency / detune, PannerNode position / orientation (0..5) and "
+                                         "AudioListener position / forward / up (node 1, 0..8) can)");
     const uint32_t pid = n->params[param_index];
     Param& p = g->nodes.at(pid).param;
     if (p.device_bound) return fail(WAE_INVALID_STATE, "InvalidStateError - the param is already bound from device memory");
@@ -661,6 +673,10 @@ WAE_API wae_status wae_param_set_device_value(wae_graph* g, wae_node_id node, ui
         return fail(WAE_UNSUPPORTED, "OscillatorNode " + std::to_string(node) + ": " + range + " allow computed frequencies outside (0, " +
                                          std::to_string(g->sample_rate / 2.f) + ") Hz; a pitch bound from device memory must stay inside "
                                          "it (bind a wider pitch as a value curve: wae_param_set_device_value_curve)");
+    if ((n->kind == K_PANNER || n->kind == K_LISTENER) && (l < -kSpatialBound || h > kSpatialBound))
+        return fail(WAE_UNSUPPORTED, std::string(n->kind == K_PANNER ? "PannerNode " + std::to_string(node) : std::string("AudioListener")) +
+                                         " param " + std::to_string(param_index) + ": a spatial value bound from device memory must lie "
+                                         "inside [-1e9, 1e9] (the f32 spatial math overflows beyond it); declare a narrower range");
     p.device_bound = true;
     p.device_lo = l;
     p.device_hi = h;

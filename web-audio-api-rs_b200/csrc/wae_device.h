@@ -668,4 +668,28 @@ struct ParamPatch {
     float val[PATCH_OPS];
 };
 
+// A spatial entry: one static panner whose source or listener is bound from device memory (panner params 0..5, listener params 0..8),
+// re-derived by k_derive_spatial after k_derive_params.  Operand i (the 15 spatial params in SpatialTracks order) is slot[i] (>= 0) or
+// the constant val[i].
+enum SpatialKind : int32_t {
+    SPATIAL_PAN = 0,   // PanInst *dst = azimuth, dist_gain, cone_gain (S_PAN)
+    SPATIAL_SEL = 1,   // HrtfSel *dst = triangle, weights, gain (HrtfInst::static_sel)
+    SPATIAL_RESP = 2,  // HrtfSel *dst as SPATIAL_SEL, then the blended pair into resp [2][taps] (k_spatial_blend), which k_resp_fft
+                       // transforms into the node's spectra
+};
+struct SpatialPatch {
+    int32_t kind;
+    int32_t n_faces;         // SPATIAL_SEL / SPATIAL_RESP: the sphere's faces
+    void* dst;
+    const float* pos;        // sphere vertices [v][3]
+    const uint32_t* tri;     // sphere faces
+    const float* ir;         // SPATIAL_RESP: the sphere's responses at the context rate [v][2][taps]
+    float* resp;             // SPATIAL_RESP: the blended pair [2][taps]
+    int32_t taps;
+    float correction;        // SPATIAL_RESP: 2 for a two-channel input (panner.rs:805-812)
+    spatial::PanModel model;
+    int32_t slot[15];
+    float val[15];
+};
+
 }  // namespace wae

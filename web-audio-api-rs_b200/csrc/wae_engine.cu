@@ -121,6 +121,7 @@ struct wae_engine {
     float* d_sphere_ir = nullptr;
     float* d_sphere_pos = nullptr;
     uint32_t* d_sphere_tri = nullptr;
+    uint64_t sphere_gen = 0;  // counts the spheres wae_engine_set_hrir_sphere installed (a bind checks that its batch's is still there)
     struct RateSphere {  // the sphere's responses resampled to a context rate (HrirSphere::new of the crate), built on first use
         float* d_ir = nullptr;
         uint32_t taps = 0;
@@ -340,7 +341,22 @@ struct StageBuild {
         SchedPatch p;    // dst set when the tables are uploaded
     };
     std::vector<SchedPatchRec> sched_patches;
-    size_t records() const {  // size of the table patch entries point into
+    // Spatial entries of static panners whose source or listener is bound from device memory (wae_param_set_device_value): record `rec`
+    // of this stage's table (S_PAN: PanInst, S_HRTF: HrtfInst), `off` bytes into it, or -1 for an HRTF panner lowered to a convolver,
+    // whose entry's dst / resp the planner sets and whose bind also rewrites the spectra `spec` of `S` partitions.  Operands name their
+    // param by node id (p.slot) until the batch numbers its value slots.
+    struct SpatialPatchRec {
+        SpatialPatch p;
+        uint32_t graph;  // batch position
+        int32_t rec;
+        uint32_t off;
+        float2* spec;
+        int32_t S;
+    };
+    std::vector<SpatialPatchRec> spatial;
+    size_t spatial_records() const { return kind == S_PAN ? pan.size() : kind == S_HRTF ? hrtf.size() : 0; }
+    // size of the table patch entries point into (S_HRTF: the selection records of its moving panners, the stage's second table)
+    size_t records() const {
         switch (kind) {
             case S_OSC: return osc.size();
             case S_OSC_AR: return osc_ar.size();
@@ -356,6 +372,8 @@ struct StageBuild {
             case S_META: return meta.size();
             case S_ABSN_SERIAL: return absn_serial.size();
             case S_ABSN_BOUND: return absn_bound.size();
+            case S_PAN_DYN: return pan_dyn.size();
+            case S_HRTF: return hrtf_sel.size();
             default: return 0;
         }
     }
@@ -375,6 +393,8 @@ struct StageBuild {
             case S_META: return sizeof(MetaInst);
             case S_ABSN_SERIAL: return sizeof(AbsnSerialInst);
             case S_ABSN_BOUND: return sizeof(AbsnBoundInst);
+            case S_PAN_DYN: return sizeof(PanDynInst);
+            case S_HRTF: return sizeof(HrtfSelInst);
             default: return 0;
         }
     }
@@ -632,6 +652,14 @@ struct wae_batch {
     float* d_values = nullptr;
     ParamPatch* d_patches = nullptr;
     int n_patches = 0;
+    // and the spatial entries of its static panners (re-derived by k_derive_spatial after k_derive_params), with the transform items of
+    // those lowered to a convolver (k_resp_fft).  Entries with HRTF read the engine's sphere of generation sphere_gen.
+    SpatialPatch* d_spatial = nullptr;
+    int n_spatial = 0;
+    RespBindItem* d_spatial_resp = nullptr;
+    int n_spatial_resp = 0, spatial_max_taps = 0, spatial_max_S = 0;
+    bool spatial_sphere = false;
+    uint64_t sphere_gen = 0;
     // the patch entries of declared curves, IIR filters and schedules, each declaration's a contiguous range
     CurvePatch* d_curve_patches = nullptr;
     IirPatch* d_iir_patches = nullptr;
@@ -1241,6 +1269,35 @@ struct Planner {
         r.off = off;
         s.patches.push_back(r);
     }
+    // the spatial entry of a static panner of this graph; operand i is pr[i] (its id when bound, else its planned value)
+    using SpatialPatchRec = StageBuild::SpatialPatchRec;
+    SpatialPatchRec spatial_entry(int kind, const PRef* pr, const spatial::PanModel& model) const {
+        SpatialPatchRec r{};
+        r.p.kind = kind;
+        r.p.model = model;
+        for (int i = 0; i < 15; i++) {
+            r.p.slot[i] = pr[i].bound;
+            r.p.val[i] = pr[i].v;
+        }
+        r.graph = gi;
+        r.rec = -1;
+        return r;
+    }
+    // records spatial entry `r` for the last record of stage `s` (S_PAN / S_HRTF), `off` bytes into it
+    static void add_spatial(StageBuild& s, SpatialPatchRec r, uint32_t off) {
+        r.rec = (int32_t)s.spatial_records() - 1;
+        r.off = off;
+        s.spatial.push_back(r);
+    }
+    // a moving panner: its bound params are taken raw, PATCH_RAW into SpatialTracks::value of the last record of `s`, `off` bytes into it
+    void raw_spatial_patches(StageBuild& s, const PRef* pr, size_t off) const {
+        for (int i = 0; i < 15; i++)
+            if (pr[i].bound >= 0) {
+                PatchRec r = patch(PATCH_RAW, 1);
+                operand(r, 0, pr[i], pr[i].v);
+                add_patch(s, r, (uint32_t)(off + offsetof(SpatialTracks, value) + (size_t)i * sizeof(float)));
+            }
+    }
     // a chain's patch entries for its record at index `rec` of stage `s` (emit_chain, sum_voices)
     static void chain_patches(StageBuild& s, const PendingChain& pc, int32_t rec) {
         for (PatchRec r : pc.patches) {
@@ -1285,9 +1342,11 @@ struct Planner {
     bool plan_graph(wae_graph* graph, uint32_t graph_index);
     // ir_override: the response of a STATIC HRTF panner (blended, gain folded in): no normalisation, no trimming of small trailing taps;
     // a two-channel input is mixed down to mono by the forward transform's loads (ConvInput::in_channel = -1)
-    bool plan_convolver(PNode& pn, int level, const BufRef* dest = nullptr, int64_t dest_limit = -1, const PcmBuffer* ir_override = nullptr);
+    bool plan_convolver(PNode& pn, int level, const BufRef* dest = nullptr, int64_t dest_limit = -1, const PcmBuffer* ir_override = nullptr,
+                        const IrSpectra* fixed = nullptr);
     bool ir_spectra(const PcmBuffer& ir, float scale, const std::vector<std::vector<float>>& scaled, int Smax, IrSpectra& spec);
     bool device_response_spectra(const Node& n, int S, IrSpectra& spec);
+    bool bound_panner_spectra(const Node& n, int S, IrSpectra& spec);
     const float* device_curve(const Node& n);
     float* device_wave(const Node& n);
     float* device_value_curve(const Param& prm, const ParamTimeline& tl);
@@ -1475,9 +1534,9 @@ struct Planner {
     bool lower_panner(NodeCtx& nc);
     bool hrir_at_rate(HrirAtRate& hr);
     HrtfSel static_hrtf_sel(const spatial::SpatialParams& sp0) const;
-    bool panner_hrtf_conv(NodeCtx& nc, const spatial::SpatialParams& sp0, const HrirAtRate& hr);
+    bool panner_hrtf_conv(NodeCtx& nc, const spatial::SpatialParams& sp0, const HrirAtRate& hr, const PRef* pr, const spatial::PanModel& model);
     bool panner_hrtf_fir(NodeCtx& nc, const spatial::SpatialParams& sp0, const HrirAtRate& hr, bool moving, const SpatialTracks& tr,
-                         const spatial::PanModel& model);
+                         const spatial::PanModel& model, const PRef* pr);
     bool lower_delay_writer(NodeCtx& nc);
     bool lower_delay_reader(NodeCtx& nc);
     bool lower_compressor(NodeCtx& nc);
@@ -1580,14 +1639,14 @@ static void append_vec(std::vector<T>& d, std::vector<T>& s) {
 }
 static void merge_builds(Builds& dst, Builds& src) {
     struct Base {
-        size_t mix_edges = 0, scan = 0, chain = 0, conv_in = 0, records = 0;
+        size_t mix_edges = 0, scan = 0, chain = 0, conv_in = 0, records = 0, spatial = 0;
     };
     std::map<std::pair<int, int>, Base> base;  // table sizes of `dst` before anything of `src` is appended
     for (auto& kv : src) {
         auto it = dst.find(kv.first);
         if (it != dst.end())
             base[kv.first] = Base{it->second.mix_edges.size(), it->second.n_scan_coef, it->second.chain.size(), it->second.conv_in.size(),
-                                  it->second.records()};
+                                  it->second.records(), it->second.spatial_records()};
         else base[kv.first] = Base{};
     }
     for (auto& kv : src) {
@@ -1599,6 +1658,8 @@ static void merge_builds(Builds& dst, Builds& src) {
         }
         for (auto& cp : s.curve_patches) cp.rec += (int32_t)bs.records;
         for (auto& sp : s.sched_patches) sp.rec += (int32_t)bs.records;
+        for (auto& sp : s.spatial)
+            if (sp.rec >= 0) sp.rec += (int32_t)bs.spatial;
         for (auto& ip : s.iir_patches) {
             ip.rec += (int32_t)bs.records;
             if (ip.scan >= 0) ip.scan += (int32_t)bs.scan;
@@ -1635,6 +1696,7 @@ static void merge_builds(Builds& dst, Builds& src) {
         append_vec(d.curve_patches, s.curve_patches);
         append_vec(d.iir_patches, s.iir_patches);
         append_vec(d.sched_patches, s.sched_patches);
+        append_vec(d.spatial, s.spatial);
         d.n_scan_coef += s.n_scan_coef;
         d.max_ch = std::max(d.max_ch, s.max_ch);
     }
@@ -1661,7 +1723,7 @@ static ScanCoef make_scan_coef(const hm::BiquadCoefs& c) {
     return sc;
 }
 
-bool Planner::plan_convolver(PNode& pn, int level, const BufRef* dest, int64_t dest_limit, const PcmBuffer* ir_override) {
+bool Planner::plan_convolver(PNode& pn, int level, const BufRef* dest, int64_t dest_limit, const PcmBuffer* ir_override, const IrSpectra* fixed) {
     Node& n = *pn.n;
     int in_ch = pn.in_ch[0];
     const bool mono_mix = ir_override && in_ch == 2;
@@ -1681,6 +1743,8 @@ bool Planner::plan_convolver(PNode& pn, int level, const BufRef* dest, int64_t d
     // a response bound from device memory (wae_convolver_set_device_response): planned as an untrimmed response of the declared length;
     // the bind normalises, trims and transforms it on the device
     const bool declared = !ir_override && ir.device_input;
+    // `fixed`: spectra made by the caller (an HRTF panner whose position is bound from device memory), of fixed->S partitions whatever
+    // the response holds; the bind writes them
     // normalize_buffer, src/node/convolver.rs:16-53 (f32, channel by channel)
     float scale = 1.f;
     if (n.normalize && !ir_override && !declared) {
@@ -1700,15 +1764,15 @@ bool Planner::plan_convolver(PNode& pn, int level, const BufRef* dest, int64_t d
     // convolvers: one per IR channel, a mono IR is duplicated (convolver.rs:289-293)
     int n_conv = std::max(ir_ch, 2);
     // trailing samples below 1e-6 are ignored by fft-convolver's init
-    std::vector<std::vector<float>> scaled(declared ? 0 : ir_ch);
+    std::vector<std::vector<float>> scaled(declared || fixed ? 0 : ir_ch);
     size_t trimmed_len = declared ? ir_len : 0;
-    for (int c = 0; c < (declared ? 0 : ir_ch); c++) {
+    for (int c = 0; c < (declared || fixed ? 0 : ir_ch); c++) {
         scaled[c].resize(ir_len);
         for (size_t i = 0; i < ir_len; i++) scaled[c][i] = ir.channels[c][i] * scale;
     }
     // per-channel trimmed length (each FFTConvolver trims its own IR); use per channel S
-    std::vector<int> S(ir_ch, declared ? (int)((ir_len + WAE_CONV_BLOCK - 1) / WAE_CONV_BLOCK) : 0);
-    for (int c = 0; c < (declared ? 0 : ir_ch); c++) {
+    std::vector<int> S(ir_ch, declared ? (int)((ir_len + WAE_CONV_BLOCK - 1) / WAE_CONV_BLOCK) : fixed ? fixed->S : 0);
+    for (int c = 0; c < (declared || fixed ? 0 : ir_ch); c++) {
         size_t m = ir_len;
         while (!ir_override && m > 0 && std::fabs(scaled[c][m - 1]) < 0.000001f) m--;
         while (ir_override && m > 0 && scaled[c][m - 1] == 0.f) m--;  // (exact zeros only)
@@ -1769,7 +1833,8 @@ bool Planner::plan_convolver(PNode& pn, int level, const BufRef* dest, int64_t d
         return true;
     }
     IrSpectra spec;
-    if (!(declared ? device_response_spectra(n, Smax, spec) : ir_spectra(ir, scale, scaled, Smax, spec))) return false;
+    if (fixed) spec = *fixed;
+    else if (!(declared ? device_response_spectra(n, Smax, spec) : ir_spectra(ir, scale, scaled, Smax, spec))) return false;
     // inputs: one spectra ring per input channel
     StageBuild& fs = stage(level, S_CONV_FFT);
     int blocks_per_chunk = (int)((b->chunk + WAE_CONV_BLOCK - 1) / WAE_CONV_BLOCK);
@@ -1884,6 +1949,27 @@ bool Planner::device_response_spectra(const Node& n, int S, IrSpectra& spec) {
     (*ir_cache)[key] = spec;
     if (!dry)
         b->responses.add({key_graph, n.id, kNodeLevel}, DevResponse{spec.h, (uint32_t)ir_ch, (uint64_t)ir.length(), S, n.normalize, ir.sample_rate});
+    return true;
+}
+
+// The spectra of an HRTF panner lowered to a convolver whose source or listener is bound from device memory: one zeroed
+// [2][S + WAE_CONV_H_PAD][WAE_CONV_SPEC] allocation per (batch graph, node), never shared by content, that wae_batch_bind_params rewrites
+// in full on every bind (the padding partitions stay zero)
+bool Planner::bound_panner_spectra(const Node& n, int S, IrSpectra& spec) {
+    const uint64_t tag[3] = {0x70616e6e6572ull /* "panner" */, key_graph, n.id};
+    const uint64_t key = fnv1a(tag, sizeof(tag));
+    std::unique_lock<std::recursive_mutex> ir_lock(b->mu);
+    auto it = ir_cache->find(key);
+    if (it != ir_cache->end()) {
+        spec = it->second;
+        return true;
+    }
+    spec.S = S;
+    spec.channels = 2;
+    spec.h = dry ? reinterpret_cast<float2*>(uintptr_t(256)) : b->dalloc<float2>((size_t)2 * (S + WAE_CONV_H_PAD) * WAE_CONV_SPEC, true);
+    if (!spec.h) return bail(WAE_OUT_OF_MEMORY, "out of device memory (HRTF spectra)");
+    b->asset_bytes += (size_t)2 * (S + WAE_CONV_H_PAD) * WAE_CONV_SPEC * 8;
+    (*ir_cache)[key] = spec;
     return true;
 }
 
@@ -3103,11 +3189,15 @@ bool Planner::lower_stereo_panner(NodeCtx& nc) {
 bool Planner::lower_panner(NodeCtx& nc) {
     Node& n = nc.n; PNode& p = nc.p; const Lay& in0 = nc.in0;
     // the 15 spatial params (panner.rs:714-780): 6 of the node, 9 of the AudioListener (graph ids 2..10)
+    // Params bound from device memory (source position / orientation, listener pose) are planned with their placeholders: no lowering
+    // decision reads a value.  A moving panner takes them raw (PATCH_RAW), a static one gets a spatial entry that re-derives what the
+    // values decide (SpatialPatch).
     PRef pr[15];
-    bool moving = false;
+    bool moving = false, bound = false;
     for (int i = 0; i < 15; i++) {
         pr[i] = param_ref(i < 6 ? n.params[i] : (uint32_t)(2 + i - 6));
         moving = moving || pr[i].dyn;
+        bound = bound || pr[i].bound >= 0;
     }
     int ch = p.in_ch[0];
     // (a static HRTF panner with a constant-layout input is lowered to the convolver kernels, which take their own output buffer)
@@ -3137,8 +3227,8 @@ bool Planner::lower_panner(NodeCtx& nc) {
     if (n.panning_model == WAE_PANNING_HRTF) {  // panner.rs:781-830
         HrirAtRate hr;
         if (!hrir_at_rate(hr)) return false;
-        if (hrtf_as_conv) return panner_hrtf_conv(nc, sp0, hr);
-        return panner_hrtf_fir(nc, sp0, hr, moving, tr, model);
+        if (hrtf_as_conv) return panner_hrtf_conv(nc, sp0, hr, bound ? pr : nullptr, model);
+        return panner_hrtf_fir(nc, sp0, hr, moving, tr, model, bound ? pr : nullptr);
     }
     if (moving) {
         PanDynInst d{};
@@ -3147,7 +3237,9 @@ bool Planner::lower_panner(NodeCtx& nc) {
         d.sp = tr;
         d.model = model;
         d.in_ch = ch;
-        stage(nc.L, S_PAN_DYN).pan_dyn.push_back(d);
+        StageBuild& ds = stage(nc.L, S_PAN_DYN);
+        ds.pan_dyn.push_back(d);
+        if (bound) raw_spatial_patches(ds, pr, offsetof(PanDynInst, sp));
         return true;
     }
     PanInst pi{};
@@ -3157,7 +3249,9 @@ bool Planner::lower_panner(NodeCtx& nc) {
     pi.azimuth = sp0.azimuth;
     pi.dist_gain = sp0.dist_gain;
     pi.cone_gain = sp0.cone_gain;
-    stage(nc.L, S_PAN).pan.push_back(pi);
+    StageBuild& ps = stage(nc.L, S_PAN);
+    ps.pan.push_back(pi);
+    if (bound) add_spatial(ps, spatial_entry(SPATIAL_PAN, pr, model), 0);
     return true;
 }
 
@@ -3208,13 +3302,42 @@ HrtfSel Planner::static_hrtf_sel(const spatial::SpatialParams& sp0) const {
 // panner.rs:805-812) folded in; a two-channel input is mixed down to mono by the forward transform's loads; one
 // partition, so the product is formed inside the inverse transform — instead of 2 x taps multiply-adds per output
 // frame in k_hrtf_fir.  WAE_HRTF_FFT=0: keep the FIR kernel.
-bool Planner::panner_hrtf_conv(NodeCtx& nc, const spatial::SpatialParams& sp0, const HrirAtRate& hr) {
+// `pr` (source or listener bound from device memory): planned with ceil(taps / WAE_CONV_BLOCK) partitions whatever the placeholder's
+// response holds, into spectra of the node's own; a SPATIAL_RESP entry re-derives the triangle, blends the pair into a [2][taps]
+// scratch of its own and transforms it on every bind.
+bool Planner::panner_hrtf_conv(NodeCtx& nc, const spatial::SpatialParams& sp0, const HrirAtRate& hr, const PRef* pr,
+                               const spatial::PanModel& model) {
     const uint32_t taps = hr.taps;
     const int ch = nc.p.in_ch[0];
-    const HrtfSel sel = static_hrtf_sel(sp0);
     PcmBuffer resp;
     if (!resp.allocate(2, taps, false)) return bail(WAE_OUT_OF_MEMORY, "out of host memory (hrtf response)");
     const float corr = ch == 2 ? 2.f : 1.f;  // overall_gain_correction of a two-channel input (panner.rs:805-812)
+    resp.sample_rate = (float)hr.sr;
+    if (pr) {
+        IrSpectra spec;
+        const int S = (int)((taps + WAE_CONV_BLOCK - 1) / WAE_CONV_BLOCK);
+        if (!bound_panner_spectra(nc.n, S, spec) || !plan_convolver(nc.p, nc.L, nullptr, -1, &resp, &spec)) return false;
+        if (dry) return true;
+        SpatialPatchRec r = spatial_entry(SPATIAL_RESP, pr, model);
+        r.p.pos = eng->d_sphere_pos;
+        r.p.tri = eng->d_sphere_tri;
+        r.p.n_faces = (int32_t)(eng->sphere->tri.size() / 3);
+        r.p.ir = hr.d_ir;
+        r.p.taps = (int32_t)taps;
+        r.p.correction = corr;
+        const size_t sel_floats = sizeof(HrtfSel) / sizeof(float);
+        std::lock_guard<std::recursive_mutex> lk(b->mu);  // (groups are planned on worker threads)
+        float* scratch = b->dalloc<float>((size_t)2 * taps + sel_floats, true);  // the pair, then the selection
+        if (!scratch) return bail(WAE_OUT_OF_MEMORY, "out of device memory (hrtf response)");
+        b->asset_bytes += ((size_t)2 * taps + sel_floats) * sizeof(float);
+        r.p.resp = scratch;
+        r.p.dst = scratch + (size_t)2 * taps;
+        r.spec = spec.h;
+        r.S = S;
+        stage(nc.L, S_CONV_FFT).spatial.push_back(r);
+        return true;
+    }
+    const HrtfSel sel = static_hrtf_sel(sp0);
     const float* A = hr.h_ir + (size_t)sel.v[0] * 2 * taps;
     const float* B = hr.h_ir + (size_t)sel.v[1] * 2 * taps;
     const float* C = hr.h_ir + (size_t)sel.v[2] * 2 * taps;
@@ -3224,12 +3347,11 @@ bool Planner::panner_hrtf_conv(NodeCtx& nc, const spatial::SpatialParams& sp0, c
         resp.channels[0].p[k] = corr * (l * sel.gain);
         resp.channels[1].p[k] = corr * (r * sel.gain);
     }
-    resp.sample_rate = (float)hr.sr;
     return plan_convolver(nc.p, nc.L, nullptr, -1, &resp);
 }
 
 bool Planner::panner_hrtf_fir(NodeCtx& nc, const spatial::SpatialParams& sp0, const HrirAtRate& hr, bool moving, const SpatialTracks& tr,
-                              const spatial::PanModel& model) {
+                              const spatial::PanModel& model, const PRef* pr) {
     PNode& p = nc.p;
     const HrirSphere* sph = eng->sphere;
     const int ch = p.in_ch[0];
@@ -3261,10 +3383,18 @@ bool Planner::panner_hrtf_fir(NodeCtx& nc, const spatial::SpatialParams& sp0, co
         if (!si.sel) return bail(WAE_OUT_OF_MEMORY, "out of device memory (hrtf selection)");
         h.sel = si.sel;
         hs.hrtf_sel.push_back(si);
+        if (pr) raw_spatial_patches(hs, pr, offsetof(HrtfSelInst, sp));
     } else {
         h.static_sel = static_hrtf_sel(sp0);
     }
     hs.hrtf.push_back(h);
+    if (pr && !moving) {  // (the sphere operands: the ones a moving panner's HrtfSelInst holds)
+        SpatialPatchRec r = spatial_entry(SPATIAL_SEL, pr, model);
+        r.p.pos = eng->d_sphere_pos;
+        r.p.tri = eng->d_sphere_tri;
+        r.p.n_faces = (int32_t)(sph->tri.size() / 3);
+        add_spatial(hs, r, (uint32_t)offsetof(HrtfInst, static_sel));
+    }
     return true;
 }
 
@@ -3743,6 +3873,7 @@ WAE_API wae_status wae_engine_set_hrir_sphere(wae_engine* eng, const void* data,
     delete eng->sphere;
     eng->sphere = sp;
     eng->d_sphere_ir = d;
+    eng->sphere_gen++;
     return WAE_OK;
 }
 
@@ -3847,6 +3978,7 @@ struct GroupPlan {  // result of phase B for one group
     std::vector<PatchEntry<CurvePatch>> curve_patches;
     std::vector<PatchEntry<IirPatch>> iir_patches;
     std::vector<PatchEntry<SchedPatch>> sched_patches;
+    std::vector<StageBuild::SpatialPatchRec> spatial;  // device addresses set, operands still param ids
 };
 
 static int64_t padded_length(const wae_graph* g) { return (int64_t)((g->length + 127) / 128 * 128); }
@@ -4442,9 +4574,10 @@ static void prep_plan_group(wae_batch* b, wae_graph* const* graphs, int k, PrepS
                 // params: the field and the scan constants (S_CHAIN / S_VSUM) or stereo gains (S_SPAN) it re-derives (PATCH_OSC: dst2 is
                 // the start time's address, set by the planner)
                 const size_t rec2_size = s.kind == S_SPAN ? sizeof(float2) : sizeof(ScanCoef);
+                char* const param_table = static_cast<char*>(s.kind == S_HRTF ? st.d_b : st.d_a);  // (see StageBuild::records)
                 for (const PatchRec& pr : s.patches) {
                     ParamPatch p = pr.p;
-                    p.dst = rec(pr.rec) + pr.off;
+                    p.dst = param_table + (size_t)pr.rec * rec_size + pr.off;
                     if (pr.rec2 >= 0) p.dst2 = static_cast<char*>(st.d_b) + (size_t)pr.rec2 * rec2_size;
                     gp.patches.push_back({pr.graph, p});
                 }
@@ -4467,6 +4600,11 @@ static void prep_plan_group(wae_batch* b, wae_graph* const* graphs, int k, PrepS
                     SchedPatch p = sp.p;
                     p.dst = rec(sp.rec) + sp.off;
                     gp.sched_patches.push_back({sp.graph, sp.node, p});
+                }
+                for (StageBuild::SpatialPatchRec sp : s.spatial) {  // static panners: the PanInst or HrtfInst::static_sel they re-derive
+                    if (sp.rec >= 0)
+                        sp.p.dst = static_cast<char*>(st.d_a) + (size_t)sp.rec * (s.kind == S_PAN ? sizeof(PanInst) : sizeof(HrtfInst)) + sp.off;
+                    gp.spatial.push_back(sp);
                 }
             }
         }
@@ -4589,9 +4727,10 @@ static wae_status check_bound(wae_batch* b) {
 // The value slots of the params declared with wae_param_set_device_value (`graphs` in batch order: one slot per param, in graph, node and
 // param order; runs wait for every one, reached by the planner or not) and the patch entries of the planned groups, their operands
 // renumbered from param ids to slots; both uploaded (from `info` and `patches`, which the caller keeps alive until the stream has been
-// synchronised).
+// synchronised).  The spatial entries and their transform items likewise (`spatial`, `resp`).
 static wae_status record_params(wae_batch* b, wae_graph* const* graphs, uint32_t n_graphs, std::vector<GroupPlan>& gps,
-                                std::vector<ParamSlotInfo>& info, std::vector<ParamPatch>& patches) {
+                                std::vector<ParamSlotInfo>& info, std::vector<ParamPatch>& patches, std::vector<SpatialPatch>& spatial,
+                                std::vector<RespBindItem>& resp) {
     b->params.seal(graphs, n_graphs, [](uint32_t j, const NodeMap& nodes, const Node& nd, auto& declare) {
         if (nd.kind == K_PARAM) return;
         for (uint32_t i = 0; i < nd.params.size(); i++) {
@@ -4616,6 +4755,33 @@ static wae_status record_params(wae_batch* b, wae_graph* const* graphs, uint32_t
                 if (p.slot[i] >= 0) p.slot[i] = slot_of.at((uint64_t)gpp.first << 32 | (uint32_t)p.slot[i]);
             patches.push_back(p);
         }
+    for (auto& gp : gps)
+        for (const auto& sr : gp.spatial) {
+            SpatialPatch p = sr.p;
+            for (int i = 0; i < 15; i++)
+                if (p.slot[i] >= 0) p.slot[i] = slot_of.at((uint64_t)sr.graph << 32 | (uint32_t)p.slot[i]);
+            spatial.push_back(p);
+            b->spatial_sphere = b->spatial_sphere || p.kind != SPATIAL_PAN;
+            if (p.kind != SPATIAL_RESP) continue;
+            RespBindItem it{};  // the blended pair, untrimmed, scale 1: the transform panner_hrtf_conv's host path runs
+            it.src = p.resp;
+            it.h = sr.spec;
+            it.src_stride = it.len = p.taps;
+            it.channels = 2;
+            it.S = sr.S;
+            it.scale = 1.f;
+            it.m[0] = it.m[1] = p.taps;
+            resp.push_back(it);
+            b->spatial_max_taps = std::max(b->spatial_max_taps, p.taps);
+            b->spatial_max_S = std::max(b->spatial_max_S, sr.S);
+        }
+    b->sphere_gen = b->engine->sphere_gen;
+    b->n_spatial = (int)spatial.size();
+    b->n_spatial_resp = (int)resp.size();
+    b->d_spatial = spatial.empty() ? nullptr : b->dupload_now(spatial);
+    b->d_spatial_resp = resp.empty() ? nullptr : b->dupload_now(resp);
+    if ((!spatial.empty() && !b->d_spatial) || (!resp.empty() && !b->d_spatial_resp))
+        return fail(WAE_OUT_OF_MEMORY, "out of device memory (spatial entries)");
     b->d_slot_info = b->dupload_now(info);
     b->d_values = b->dalloc<float>(info.size(), true);
     b->n_patches = (int)patches.size();
@@ -4690,8 +4856,10 @@ static wae_status prepare_impl(wae_engine* eng, wae_graph* const* graphs, uint32
     std::vector<SchedPatch> sched_patches;
     std::vector<ParamSlotInfo> slot_info;
     std::vector<ParamPatch> patches;
+    std::vector<SpatialPatch> spatial;
+    std::vector<RespBindItem> spatial_resp;
     st = record_declarations(b, graphs, n_graphs, gps, curve_patches, iir_patches, sched_patches);
-    if (st == WAE_OK) st = record_params(b, graphs, n_graphs, gps, slot_info, patches);
+    if (st == WAE_OK) st = record_params(b, graphs, n_graphs, gps, slot_info, patches, spatial, spatial_resp);
     if (st != WAE_OK) {
         wae_batch_destroy(b);
         return st;
@@ -5227,6 +5395,9 @@ WAE_API wae_status wae_batch_bind_sources(wae_batch* b, const wae_source_binding
 }
 
 WAE_API wae_status wae_batch_bind_params(wae_batch* b, const wae_param_binding* items, uint32_t n, void* stream) {
+    if (b && n && b->spatial_sphere && b->sphere_gen != b->engine->sphere_gen)  // (its records point into the freed sphere)
+        return fail(WAE_INVALID_STATE, "bind: the batch's HRTF panners were prepared with an HRIR sphere that wae_engine_set_hrir_sphere has "
+                                       "since replaced; prepare the batch again");
     return bind_items<ParamBindItem>(
         b, &wae_batch::params, items, n, stream,
         [](const wae_param_binding& it, const DevParam&, size_t slot, BindExtents& extents, auto& rows) -> wae_status {
@@ -5236,6 +5407,9 @@ WAE_API wae_status wae_batch_bind_params(wae_batch* b, const wae_param_binding* 
         },
         [b](const ParamBindItem* dev, const std::vector<ParamBindItem>& rows) {
             launch_bind_params(dev, (int)rows.size(), b->d_slot_info, b->d_values, b->d_patches, b->n_patches, b->engine->stream);
+            if (b->n_spatial > 0)
+                launch_derive_spatial(b->d_spatial, b->n_spatial, b->d_values, b->d_spatial_resp, b->n_spatial_resp, b->spatial_max_taps,
+                                      b->spatial_max_S, b->engine->stream);
         });
 }
 

@@ -4908,6 +4908,46 @@ __global__ void __launch_bounds__(64) k_derive_params(const ParamPatch* __restri
     }
 }
 
+// step 3 (batches with spatial entries): what a static panner derives from its 15 spatial params, with the functions the planner
+// runs on the host (Planner::lower_panner, static_hrtf_sel) and k_hrtf_sel runs per quantum.  One thread per entry, as k_hrtf_sel.
+__global__ void __launch_bounds__(64) k_derive_spatial(const SpatialPatch* __restrict__ patches, int n, const float* __restrict__ values) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const SpatialPatch& p = patches[i];
+    float v[15];
+    for (int k = 0; k < 15; k++) v[k] = p.slot[k] >= 0 ? values[p.slot[k]] : p.val[k];
+    const spatial::SpatialParams sp = spatial::spatial_params(p.model, v);
+    if (p.kind == SPATIAL_PAN) {
+        PanInst* o = static_cast<PanInst*>(p.dst);
+        o->azimuth = sp.azimuth;
+        o->dist_gain = sp.dist_gain;
+        o->cone_gain = sp.cone_gain;
+        return;
+    }
+    float proj[3];
+    spatial::projected_source(sp, proj);
+    const float dir[3] = {proj[0], proj[2], proj[1]};  // HrtfState::process swaps y / z (panner.rs:248-252)
+    HrtfSel s{{0, 0, 0}, {0.f, 0.f, 0.f}, sp.cone_gain * sp.dist_gain, 0.f};
+    spatial::hrir_locate(p.pos, p.tri, p.n_faces, dir, s.v, s.w);  // no face: all-zero weights (silence)
+    *static_cast<HrtfSel*>(p.dst) = s;
+}
+
+// step 4 (SPATIAL_RESP entries): the blended pair of panner_hrtf_conv, corr * (((A * w0 + B * w1) + C * w2) * gain) in its f32
+// operations and order (no contraction).  grid: (tap blocks, entries)
+__global__ void __launch_bounds__(256) k_spatial_blend(const SpatialPatch* __restrict__ patches) {
+    const SpatialPatch& p = patches[blockIdx.y];
+    if (p.kind != SPATIAL_RESP) return;
+    const HrtfSel s = *static_cast<const HrtfSel*>(p.dst);
+    const int taps = p.taps;
+    const float* A = p.ir + (size_t)s.v[0] * 2 * taps;
+    const float* B = p.ir + (size_t)s.v[1] * 2 * taps;
+    const float* C = p.ir + (size_t)s.v[2] * 2 * taps;
+    for (int k = blockIdx.x * blockDim.x + threadIdx.x; k < 2 * taps; k += gridDim.x * blockDim.x) {  // (left taps, then right)
+        const float x = __fadd_rn(__fadd_rn(__fmul_rn(__ldg(A + k), s.w[0]), __fmul_rn(__ldg(B + k), s.w[1])), __fmul_rn(__ldg(C + k), s.w[2]));
+        p.resp[k] = __fmul_rn(p.correction, __fmul_rn(x, s.gain));
+    }
+}
+
 // ---------------------------------------------------------------------------------------------------------
 // launchers
 // ---------------------------------------------------------------------------------------------------------
@@ -5208,6 +5248,16 @@ void launch_bind_params(const ParamBindItem* d, int n, const ParamSlotInfo* info
                         cudaStream_t s) {
     k_bind_params<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(d, n, info, values);
     if (n_patches > 0) k_derive_params<<<(unsigned)((n_patches + 63) / 64), 64, 0, s>>>(patches, n_patches, values);
+}
+void launch_derive_spatial(const SpatialPatch* patches, int n, const float* values, const RespBindItem* resp, int n_resp, int max_taps,
+                           int max_S, cudaStream_t s) {
+    k_derive_spatial<<<(unsigned)((n + 63) / 64), 64, 0, s>>>(patches, n, values);
+    if (n_resp == 0) return;
+    conv_configure();
+    const unsigned bx = (unsigned)std::max(1, std::min((2 * max_taps + 255) / 256, 64));
+    for (int k = 0; k < n; k += 65535) k_spatial_blend<<<dim3(bx, (unsigned)std::min(n - k, 65535)), 256, 0, s>>>(patches + k);
+    for (int k = 0; k < n_resp; k += 65535)  // (the transform of wae_batch_bind_responses: scale 1, untrimmed)
+        k_resp_fft<<<dim3((unsigned)max_S, 2, (unsigned)std::min(n_resp - k, 65535)), CV_THREADS, CV_SMEM_ELEMS * sizeof(float2), s>>>(resp + k);
 }
 void launch_bind_responses(RespBindItem* d, int n, bool any_normalize, int64_t max_len, int max_S, int max_ch, cudaStream_t s) {
     conv_configure();

@@ -280,6 +280,10 @@ void launch_bind_sources(const BindItem* d, int n, int64_t max_vec, int max_ch, 
 // a bind of n param values into their slots (k_bind_params), then every patch entry of the batch re-derived from the slots (k_derive_params)
 void launch_bind_params(const ParamBindItem* d, int n, const ParamSlotInfo* info, float* values, const ParamPatch* patches, int n_patches,
                         cudaStream_t s);
+// after a param bind, the n spatial entries of the batch re-derived from the slots (k_derive_spatial); then the blended pair of each
+// SPATIAL_RESP entry (k_spatial_blend) and its spectra (k_resp_fft over `resp`, one item per such entry); max_* over those entries
+void launch_derive_spatial(const SpatialPatch* patches, int n, const float* values, const RespBindItem* resp, int n_resp, int max_taps,
+                           int max_S, cudaStream_t s);
 // a bind of n convolver responses: the power of the normalising items (k_resp_power, when any_normalize), the trimmed lengths
 // (k_resp_trim), the spectra (k_resp_fft); max_* over the items
 void launch_bind_responses(RespBindItem* d, int n, bool any_normalize, int64_t max_len, int max_S, int max_ch, cudaStream_t s);
