@@ -737,7 +737,7 @@ WAE_API wae_status wae_batch_bind_value_curves(wae_batch* batch, const wae_value
  * time) is supplied per run from device memory (wae_batch_bind_schedules), so that one prepared batch renders any number of event
  * onsets, note sequences or onset jitters without being built and planned again.  The `when` given to wae_source_start becomes a
  * placeholder (as does the stop time with `bind_stop`); an AudioBufferSourceNode's offset and duration stay the ones given to
- * wae_source_start.  A bound time is clamped to its window [lo, hi] (a NaN becomes lo); the reference panics on a negative or non-finite
+ * wae_source_start unless wae_buffer_source_set_device_offset declares them too.  A bound time is clamped to its window [lo, hi] (a NaN becomes lo); the reference panics on a negative or non-finite
  * `when`, which a bind on the device cannot do.  The source is always planned with a gated output layout, and its path never depends on
  * the bound times: a non-looping AudioBufferSourceNode whose computed playback rates are all > 0 and not automated takes the bound slow
  * track (k_buffer_source_slow(bound), which plays a rate of 1 from an aligned start 1:1), every other one the serial kernel.  A declared
@@ -749,16 +749,28 @@ WAE_API wae_status wae_batch_bind_value_curves(wae_batch* batch, const wae_value
 WAE_API wae_status wae_source_set_device_schedule(wae_graph* graph, wae_node_id node, double start_lo, double start_hi, int32_t bind_stop,
                                                   double stop_lo, double stop_hi);
 
+/* Extends the schedule declaration of an AudioBufferSourceNode with the `offset` of start_at_with_offset_and_duration (and, with
+ * `bind_duration`, its `duration`), supplied per run by wae_batch_bind_schedules, so that one prepared batch plays any excerpt of a long
+ * clip.  A caller who only wants a per-run offset declares the start window [when, when].  The offset (and duration) given to
+ * wae_source_start become placeholders: the windows' low ends, and the plan is the one of a source started with them.  A bound value is
+ * clamped to its window (a NaN becomes lo); the reference panics on a negative or non-finite offset or duration.  The playback path is the
+ * declared schedule's (see above); an offset of 0 from an aligned start still plays 1:1 at a rate of 1, a declared duration never does.
+ * WAE_INVALID_ARGUMENT: not an AudioBufferSourceNode, a window that is not finite with 0 <= lo <= hi.  WAE_INVALID_STATE: the node's
+ * schedule has not been declared with wae_source_set_device_schedule, or a second declaration. */
+WAE_API wae_status wae_buffer_source_set_device_offset(wae_graph* graph, wae_node_id node, double offset_lo, double offset_hi,
+                                                       int32_t bind_duration, double duration_lo, double duration_hi);
+
 typedef struct wae_schedule_binding {
     uint32_t graph_index;  /* caller's index, as wae_batch_fetch_graph */
     wae_node_id node;      /* declared with wae_source_set_device_schedule */
-    const double* times;   /* device memory of the engine's GPU, 8-byte aligned: times[0] = start, times[1] = stop (declared bind_stop) */
+    const double* times;   /* device memory of the engine's GPU, 8-byte aligned: the row start, [stop], [offset], [duration], holding
+                              only what was declared (bind_stop; wae_buffer_source_set_device_offset, bind_duration) */
 } wae_schedule_binding;
 
 /* Writes the times into the batch, asynchronously on the engine stream after the work already queued on `stream` (as
  * wae_batch_bind_sources).  All-or-nothing: every item is validated before anything is enqueued.  A bound schedule stays until it is
  * bound again.  WAE_INVALID_ARGUMENT: `times` is null, not 8-byte aligned or not device (or managed) memory of the engine's GPU, the
- * declared times do not lie in one allocation, or one node is named twice in the call.  WAE_INVALID_STATE: graph_index out of range, or
+ * declared row does not lie in one allocation, or one node is named twice in the call.  WAE_INVALID_STATE: graph_index out of range, or
  * the node has no declaration.  wae_batch_run, wae_batch_run_group and wae_batch_run_pipelined answer WAE_INVALID_STATE while a declared
  * schedule of the batch has never been bound (a declared source the batch never renders needs no bind). */
 WAE_API wae_status wae_batch_bind_schedules(wae_batch* batch, const wae_schedule_binding* items, uint32_t n, void* stream);

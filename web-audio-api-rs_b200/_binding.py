@@ -155,7 +155,7 @@ class ValueCurveBinding(C.Structure):
 
 
 class ScheduleBinding(C.Structure):
-    """wae_schedule_binding: the device start (and stop) time of one declared scheduled source of a prepared batch
+    """wae_schedule_binding: the device row start, [stop], [offset], [duration] of one declared scheduled source of a prepared batch
     (wae_batch_bind_schedules)."""
     _fields_ = [("graph_index", C.c_uint32), ("node", C.c_uint32), ("times", c_double_p)]
 
@@ -205,7 +205,7 @@ WAE_SYMBOLS = [
     "wae_oscillator_set_device_periodic_wave", "wae_batch_bind_periodic_waves",
     "wae_iir_filter_set_device_coefficients", "wae_batch_bind_iir_coefficients",
     "wae_param_set_device_value_curve", "wae_batch_bind_value_curves",
-    "wae_source_set_device_schedule", "wae_batch_bind_schedules",
+    "wae_source_set_device_schedule", "wae_batch_bind_schedules", "wae_buffer_source_set_device_offset",
 ]
 
 
@@ -330,6 +330,7 @@ class Api:
             # start / stop times bound from device memory
             f("source_set_device_schedule", C.c_int32, [gp, C.c_uint32, C.c_double, C.c_double, C.c_int32, C.c_double, C.c_double])
             f("batch_bind_schedules", C.c_int32, [C.c_void_p, C.POINTER(ScheduleBinding), C.c_uint32, C.c_void_p])
+            f("buffer_source_set_device_offset", C.c_int32, [gp, C.c_uint32, C.c_double, C.c_double, C.c_int32, C.c_double, C.c_double])
         else:
             f("graph_create", C.c_int32, [C.c_uint32, C.c_uint64, C.c_float, C.POINTER(C.c_void_p)])
             f("render", C.c_int32, [gp, c_float_p])

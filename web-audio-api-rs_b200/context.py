@@ -277,7 +277,7 @@ class AudioScheduledSourceNode(AudioNode):
         s_lo, s_hi = (float(x) for x in start)
         t_lo, t_hi = (0.0, 0.0) if stop is None else (float(x) for x in stop)
         api.check(api.source_set_device_schedule(self._ctx._g, self.id, s_lo, s_hi, 0 if stop is None else 1, t_lo, t_hi))
-        self._ctx._device_schedules[self.id] = stop is not None
+        self._ctx._device_schedules[self.id] = (stop is not None, False, False)
         return self
 
 
@@ -333,6 +333,24 @@ class AudioBufferSourceNode(AudioScheduledSourceNode):
     def start_at_with_offset_and_duration(self, start, offset, duration):
         api = self._ctx._api
         api.check(api.source_start(self._ctx._g, self.id, start, offset, duration))
+
+    def set_device_schedule(self, start, stop=None, offset=None, duration=None):
+        """As for every scheduled source; given `offset` = (lo, hi) (and `duration` = (lo, hi)), the offset (and duration) of
+        start_at_with_offset_and_duration are supplied by Batch.bind_schedules as well (wae_buffer_source_set_device_offset).  A
+        duration is declared together with an offset."""
+        if duration is not None and offset is None:
+            raise B.WaeError(1, "set_device_schedule: a duration window needs an offset window")
+        o_lo, o_hi = (0.0, 0.0) if offset is None else (float(x) for x in offset)
+        d_lo, d_hi = (0.0, 0.0) if duration is None else (float(x) for x in duration)
+        # (checked before the start is declared, so that a refused call declares nothing)
+        if not all(math.isfinite(lo) and math.isfinite(hi) and 0.0 <= lo <= hi for lo, hi in ((o_lo, o_hi), (d_lo, d_hi))):
+            raise B.WaeError(1, "RangeError - an offset / duration window must be finite with 0 <= lo <= hi")
+        super().set_device_schedule(start, stop)
+        if offset is not None:
+            api = self._ctx._api
+            api.check(api.buffer_source_set_device_offset(self._ctx._g, self.id, o_lo, o_hi, 0 if duration is None else 1, d_lo, d_hi))
+            self._ctx._device_schedules[self.id] = (stop is not None, True, duration is not None)
+        return self
 
 
 def _response_arrays(frequency_hz):
@@ -971,32 +989,39 @@ class Batch:
                 items[j * n + i] = B.ValueCurveBinding(g, key[0], key[1], ptr)
         self._bind(self.api.batch_bind_value_curves, items, n * len(params), *tensors)
 
-    def bind_schedules(self, nodes, starts, stops=None, graphs=None):
+    def bind_schedules(self, nodes, starts, stops=None, offsets=None, durations=None, graphs=None):
         """wae_batch_bind_schedules: starts[i] (and stops[i]) become the start (and stop) times of the scheduled source `nodes` (declared
-        with set_device_schedule) in context graphs[i] (default: 0..n-1).  `starts` / `stops`: float64 CUDA tensors [n] for one node, or
-        [n][k] for a list of k nodes; `stops` is given exactly when the nodes were declared with a stop window.  One call, ordered after
-        torch's current stream; the times are read on the engine stream, and their memory is kept from reuse until they have been."""
+        with set_device_schedule) in context graphs[i] (default: 0..n-1), and offsets[i] (and durations[i]) the offset (and duration) of
+        an AudioBufferSourceNode declared with them.  Each is a float64 CUDA tensor [n] for one node, or [n][k] for a list of k nodes;
+        `stops`, `offsets` and `durations` are given exactly when the nodes were declared with those windows.  One call, ordered after
+        torch's current stream; the values are read on the engine stream, and their memory is kept from reuse until they have been."""
         import torch
-        for t in (starts,) if stops is None else (starts, stops):
+        cols = {"stops": stops, "offsets": offsets, "durations": durations}
+        for t in [starts] + [t for t in cols.values() if t is not None]:
             if not (isinstance(t, torch.Tensor) and t.is_cuda and t.dtype == torch.float64 and t.dim() in (1, 2)):
-                raise B.WaeError(1, "bind_schedules: starts / stops must be float64 CUDA tensors [n] or [n][k]")
+                raise B.WaeError(1, "bind_schedules: starts / stops / offsets / durations must be float64 CUDA tensors [n] or [n][k]")
         many = isinstance(nodes, (list, tuple))
         ids = [int(getattr(x, "id", x)) for x in nodes] if many else [int(getattr(nodes, "id", nodes))]
         n, k = starts.shape[0], len(ids)
         if (starts.dim() == 2) != many or (many and starts.shape[1] != k):
             raise B.WaeError(1, f"bind_schedules: starts is {list(starts.shape)} for {k} node(s): [n] for one node, [n][k] for a list")
-        if stops is not None and stops.shape != starts.shape:
-            raise B.WaeError(1, f"bind_schedules: stops is {list(stops.shape)}, starts {list(starts.shape)}")
+        for name, t in cols.items():
+            if t is not None and t.shape != starts.shape:
+                raise B.WaeError(1, f"bind_schedules: {name} is {list(t.shape)}, starts {list(starts.shape)}")
         graphs = self._graphs("bind_schedules", graphs, n, "rows")
+        given = tuple(t is not None for t in cols.values())
         for g in graphs:
             for nid in ids:
                 declared = self.contexts[g]._device_schedules.get(nid)
-                if declared is not None and declared != (stops is not None):
-                    raise B.WaeError(1, f"bind_schedules: node {nid} of graph {g} was declared {'with' if declared else 'without'} a stop "
-                                        f"window, stops is {'missing' if declared else 'given'}")
-        # one item reads [start, stop] from adjacent memory: the times are packed on torch's current stream
-        s = starts.reshape(n, k)
-        times = (s if stops is None else torch.stack([s, stops.reshape(n, k)], dim=2)).reshape(n, k, -1).contiguous()
+                if declared is None:
+                    continue
+                for name, what, d, h in zip(cols, ("a stop", "an offset", "a duration"), declared, given):
+                    if d != h:
+                        raise B.WaeError(1, f"bind_schedules: node {nid} of graph {g} was declared {'with' if d else 'without'} {what} "
+                                            f"window, {name} is {'missing' if d else 'given'}")
+        # one item reads its row start, [stop], [offset], [duration] from adjacent memory: the values are packed on torch's current stream
+        rest = [t.reshape(n, k) for t in cols.values() if t is not None]
+        times = (torch.stack([starts.reshape(n, k)] + rest, dim=2) if rest else starts.reshape(n, k, 1)).contiguous()
         width = times.shape[2]
         items = (B.ScheduleBinding * max(n * k, 1))()
         base = times.data_ptr()

@@ -1046,6 +1046,34 @@ WAE_API wae_status wae_source_set_device_schedule(wae_graph* g, wae_node_id node
     return WAE_OK;
 }
 
+// Extends the schedule declaration of an AudioBufferSourceNode with its offset (and with bind_duration its duration): placeholders
+// written per run by wae_batch_bind_schedules, planned at the windows' low ends like the start time.  A declared schedule already takes
+// the bound slow track or the serial kernel, whose records hold the offset and duration the bind rewrites.
+WAE_API wae_status wae_buffer_source_set_device_offset(wae_graph* g, wae_node_id node, double offset_lo, double offset_hi, int32_t bind_duration,
+                                                       double duration_lo, double duration_hi) {
+    if (!g) return fail(WAE_INVALID_ARGUMENT, "null graph");
+    Node* n = g->nodes.get(node);
+    if (!n || n->kind != K_ABSN) return fail(WAE_INVALID_ARGUMENT, "not an AudioBufferSourceNode");
+    auto window = [](double lo, double hi) { return std::isfinite(lo) && std::isfinite(hi) && 0. <= lo && lo <= hi; };
+    if (!window(offset_lo, offset_hi) || (bind_duration && !window(duration_lo, duration_hi)))
+        return fail(WAE_INVALID_ARGUMENT, "RangeError - an offset / duration window must be finite with 0 <= lo <= hi");
+    if (!n->device_schedule)
+        return fail(WAE_INVALID_STATE, "InvalidStateError - the start time is not bound from device memory (wae_source_set_device_schedule)");
+    if (n->sched_offset)
+        return fail(WAE_INVALID_STATE, "InvalidStateError - the offset is already bound from device memory (wae_buffer_source_set_device_offset)");
+    n->sched_offset = true;
+    n->sched_duration = bind_duration != 0;
+    n->offset = offset_lo;
+    n->sched_lo[2] = offset_lo;
+    n->sched_hi[2] = offset_hi;
+    if (bind_duration) {
+        n->duration = duration_lo;
+        n->sched_lo[3] = duration_lo;
+        n->sched_hi[3] = duration_hi;
+    }
+    return WAE_OK;
+}
+
 WAE_API wae_status wae_oscillator_set_type(wae_graph* g, wae_node_id node, uint32_t type) {
     auto ni = g->nodes.find(node);
     if (ni == g->nodes.end() || ni->second.kind != K_OSC) return fail(WAE_INVALID_ARGUMENT, "not an oscillator");

@@ -622,17 +622,22 @@ struct SchedPatch {
     int32_t pad;
     double* start_out;    // SCHED_OSC of an oscillator whose pitch is bound from device memory: the clamped start is also written here,
                           // where its PATCH_OSC entry reads it (nullptr: none).  SCHED_OSC* take the phase increment from the record.
-    double offset;        // SCHED_ABSN_BOUND: start(when, offset)
+    double offset;        // SCHED_ABSN_BOUND: start(when, offset), taken when the offset is not bound
     double duration;      // SCHED_ABSN_BOUND: the buffer's duration
     double stop_time;     // the planned stop time, taken when the stop is not bound (>= 1e300: none)
     int64_t lq;           // SCHED_ABSN_BOUND: the render length of the plan (absn_fast_end)
 };
+enum SchedBinds : int32_t {  // the declared values after the start, in the order they follow it in the caller's row
+    SCHED_BIND_STOP = 1,
+    SCHED_BIND_OFFSET = 2,    // AudioBufferSourceNode: start(when, offset)
+    SCHED_BIND_DURATION = 4,  // AudioBufferSourceNode: start(when, offset, duration)
+};
 struct SchedBindItem {
-    const double* times;        // caller's [start] or [start, stop] (8 B aligned)
+    const double* times;        // caller's row: start, [stop], [offset], [duration] (8 B aligned)
     const SchedPatch* patches;  // the node's entries
-    double lo[2], hi[2];        // the declared windows the times are clamped to (a NaN becomes lo)
+    double lo[4], hi[4];        // the declared windows the values are clamped to (a NaN becomes lo): start, stop, offset, duration
     int32_t n_patches;
-    int32_t bind_stop;
+    int32_t binds;              // SchedBinds
 };
 
 // ---- wae_batch_bind_params: per-run values of params planned as constants ------------------------------------------------------

@@ -560,9 +560,9 @@ struct DevIir {  // wae_iir_filter_set_device_coefficients: the entries of every
     uint32_t nff, nfb;
     int32_t p0, p1;  // in d_iir_patches
 };
-struct DevSchedule {  // wae_source_set_device_schedule: the windows and the entries of every record the times reach
-    bool bind_stop;
-    double lo[2], hi[2];
+struct DevSchedule {  // wae_source_set_device_schedule (+ wae_buffer_source_set_device_offset): the windows and the entries of every
+    int32_t binds;    // record the values reach; SchedBinds
+    double lo[4], hi[4];
     int32_t p0, p1;  // in d_sched_patches
 };
 struct DevValueCurve {  // wae_param_set_device_value_curve: the param's curve pool (ParamInst::curves, made by the planner) and where
@@ -4694,9 +4694,14 @@ static wae_status record_declarations(wae_batch* b, wae_graph* const* graphs, ui
             declare({j, nd.id, kNodeLevel}, DevIir{(uint32_t)nd.feedforward.size(), (uint32_t)nd.feedback.size(), 0, 0});
     });
     b->schedules.seal(graphs, n_graphs, [](uint32_t j, const NodeMap&, const Node& nd, auto& declare) {
-        if (nd.device_schedule)
-            declare({j, nd.id, kNodeLevel},
-                    DevSchedule{nd.sched_stop, {nd.sched_lo[0], nd.sched_lo[1]}, {nd.sched_hi[0], nd.sched_hi[1]}, 0, 0});
+        if (nd.device_schedule) {
+            DevSchedule d{(nd.sched_stop ? SCHED_BIND_STOP : 0) | (nd.sched_offset ? SCHED_BIND_OFFSET : 0) |
+                              (nd.sched_duration ? SCHED_BIND_DURATION : 0),
+                          {}, {}, 0, 0};
+            std::copy(nd.sched_lo, nd.sched_lo + 4, d.lo);
+            std::copy(nd.sched_hi, nd.sched_hi + 4, d.hi);
+            declare({j, nd.id, kNodeLevel}, d);
+        }
     });
     b->value_curves.seal(graphs, n_graphs, [](uint32_t j, const NodeMap&, const Node& nd, auto& declare) {
         if (nd.kind == K_PARAM && nd.param.device_curve)
@@ -5517,11 +5522,15 @@ WAE_API wae_status wae_batch_bind_schedules(wae_batch* b, const wae_schedule_bin
     return bind_items<SchedBindItem>(
         b, &wae_batch::schedules, items, n, stream,
         [b](const wae_schedule_binding& it, const DevSchedule& d, size_t, BindExtents& extents, auto& rows) -> wae_status {
-            wae_status st = extents.check(it.times, alignof(double), (d.bind_stop ? 2 : 1) * sizeof(double), "times",
+            const int count = 1 + __builtin_popcount((unsigned)d.binds);
+            wae_status st = extents.check(it.times, alignof(double), count * sizeof(double), "times",
                                           "[times, times + count) runs past the end of its allocation");
-            if (st == WAE_OK && d.p0 != d.p1)
-                rows.push_back(SchedBindItem{it.times, b->d_sched_patches + d.p0, {d.lo[0], d.lo[1]}, {d.hi[0], d.hi[1]}, d.p1 - d.p0,
-                                             d.bind_stop ? 1 : 0});
+            if (st == WAE_OK && d.p0 != d.p1) {
+                SchedBindItem r{it.times, b->d_sched_patches + d.p0, {}, {}, d.p1 - d.p0, d.binds};
+                std::copy(d.lo, d.lo + 4, r.lo);
+                std::copy(d.hi, d.hi + 4, r.hi);
+                rows.push_back(r);
+            }
             return st;
         },
         [b](const SchedBindItem* dev, const std::vector<SchedBindItem>& rows) { launch_bind_schedules(dev, (int)rows.size(), b->engine->stream); });

@@ -152,9 +152,11 @@ struct Node {
     // wae_source_set_device_schedule: the start time (and, with sched_stop, the stop time) is written per run by wae_batch_bind_schedules,
     // clamped to [sched_lo, sched_hi] (index 0: start, 1: stop).  start_time / stop_time hold the windows' low ends: the plan is made
     // with them, always with a gated output layout, so no planning decision depends on the bound times.
+    // wae_buffer_source_set_device_offset extends the declaration of an AudioBufferSourceNode with its offset (index 2) and, with
+    // sched_duration, its duration (index 3); offset / duration hold those windows' low ends.
     bool device_schedule = false;
-    bool sched_stop = false;
-    double sched_lo[2] = {0., 0.}, sched_hi[2] = {0., 0.};
+    bool sched_stop = false, sched_offset = false, sched_duration = false;
+    double sched_lo[4] = {0., 0., 0., 0.}, sched_hi[4] = {0., 0., 0., 0.};
     bool loop = false;
     double loop_start = 0., loop_end = 0.;
     double max_delay_time = 1.;

@@ -4593,17 +4593,22 @@ __global__ void __launch_bounds__(256) k_bind_value_curves(const ValueCurveBindI
 // ---- wae_batch_bind_schedules: one thread per item -----------------------------------------------------------------------------------
 // The times are clamped to their windows, then every record field they reach is derived with the planner's functions (wae_kernels.h):
 // f64 without transcendentals or contraction, so each field gets the bits a host-built plan of those times holds.  The frame walks are
-// sequential (the slow track's start is sticky within almost_equal) and run once per bind.
+// sequential (the slow track's start is sticky within almost_equal) and run once per bind.  A bound offset / duration of a buffer source
+// is written raw: the render kernels derive the playhead from them on every run.
 DEVI double sched_clamp(double v, double lo, double hi) { return v != v ? lo : (v < lo ? lo : (v > hi ? hi : v)); }
 __global__ void __launch_bounds__(128) k_bind_schedules(const SchedBindItem* __restrict__ items, int n_items) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n_items) return;
     const SchedBindItem it = items[i];
-    const double start = sched_clamp(it.times[0], it.lo[0], it.hi[0]);
-    const double bound_stop = it.bind_stop ? sched_clamp(it.times[1], it.lo[1], it.hi[1]) : 0.;
+    const bool bind_stop = it.binds & SCHED_BIND_STOP, bind_offset = it.binds & SCHED_BIND_OFFSET, bind_duration = it.binds & SCHED_BIND_DURATION;
+    int col = 0;  // the row holds only what was declared
+    const double start = sched_clamp(it.times[col++], it.lo[0], it.hi[0]);
+    const double bound_stop = bind_stop ? sched_clamp(it.times[col++], it.lo[1], it.hi[1]) : 0.;
+    const double bound_offset = bind_offset ? sched_clamp(it.times[col++], it.lo[2], it.hi[2]) : 0.;
+    const double bound_duration = bind_duration ? sched_clamp(it.times[col], it.lo[3], it.hi[3]) : 0.;
     for (int k = 0; k < it.n_patches; k++) {
         const SchedPatch p = it.patches[k];
-        const double stop = it.bind_stop ? bound_stop : p.stop_time;
+        const double stop = bind_stop ? bound_stop : p.stop_time;
         const SchedClock clock(p.sample_rate);
         char* d = static_cast<char*>(p.dst);
         switch (p.kind) {
@@ -4644,21 +4649,28 @@ __global__ void __launch_bounds__(128) k_bind_schedules(const SchedBindItem* __r
             }
             case SCHED_ABSN_BOUND: {
                 AbsnBoundInst* r = reinterpret_cast<AbsnBoundInst*>(d);
+                const double offset = bind_offset ? bound_offset : p.offset;
                 const int64_t q = absn_start_quantum(clock, start);
-                const bool aligned = start <= clock.block_time(q) && p.offset == 0.;
+                const bool aligned = start <= clock.block_time(q) && offset == 0.;
                 const AbsnStart st = absn_start(clock, start, stop);
                 r->s.n_first = st.n_first;
                 r->s.n_stop = st.n_stop;
                 r->start_delta = st.t_first - st.start;
                 r->n_start = q * 128;
                 r->fast_end = absn_fast_end(clock, p.lq, q * 128, p.duration);
-                r->fast_ok = aligned && p.flag && stop > 1e300;
+                r->fast_ok = aligned && p.flag && stop > 1e300;  // (flag is 0 for a declared duration: it is finite)
+                if (bind_offset) r->offset = bound_offset;
+                if (bind_duration) r->s.duration = bound_duration;
                 break;
             }
-            case SCHED_ABSN_SERIAL:
-                reinterpret_cast<AbsnSerialInst*>(d)->start_time = start;
-                reinterpret_cast<AbsnSerialInst*>(d)->stop_time = stop;
+            case SCHED_ABSN_SERIAL: {
+                AbsnSerialInst* r = reinterpret_cast<AbsnSerialInst*>(d);
+                r->start_time = start;
+                r->stop_time = stop;
+                if (bind_offset) r->offset = bound_offset;
+                if (bind_duration) r->duration = bound_duration;
                 break;
+            }
         }
     }
 }

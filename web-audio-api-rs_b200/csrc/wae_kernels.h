@@ -296,7 +296,8 @@ void launch_bind_waves(const WaveBindItem* d, int n, int max_len, bool any_norma
 void launch_bind_iir(const IirBindItem* d, int n, cudaStream_t s);
 // a bind of n param value curves (k_bind_value_curves): each item's values copied bit for bit, max_len = the longest
 void launch_bind_value_curves(const ValueCurveBindItem* d, int n, int64_t max_len, cudaStream_t s);
-// a bind of n start / stop times (k_bind_schedules, one thread per item): clamped, then every patch entry of each item re-derived
+// a bind of n schedules (start, [stop], [offset], [duration]; k_bind_schedules, one thread per item): clamped, then every patch entry of
+// each item re-derived
 void launch_bind_schedules(const SchedBindItem* d, int n, cudaStream_t s);
 void launch_conv_ir_fft(const float* ir, int64_t ir_len, int64_t ir_stride, float2* h, int S, int channels, cudaStream_t s);
 
