@@ -286,9 +286,12 @@ struct DelayInst {
     int32_t pad;
 };
 
+// slots of CompInst::meta_ring: more than the look-ahead of quanta at the highest sample rate (37 at 768 kHz), a power of two
+constexpr int COMP_META_RING = 64;
+
 struct CompInst {
     BufRef in, out;
-    uint8_t* meta_ring;  // dynamic input layout: the layout bytes of the quanta inside the look-ahead ring ([8], index = quantum & 7)
+    uint8_t* meta_ring;  // dynamic input layout: the layout bytes of the quanta inside the look-ahead ring ([COMP_META_RING], index = quantum & (COMP_META_RING - 1))
     float* ring;         // [ch][ring_len] input history
     float* state;        // [0] = prev_detector_value, [1] = last reduction (dB)
     uint32_t ring_len;   // power of two

@@ -3491,10 +3491,12 @@ bool Planner::lower_compressor(NodeCtx& nc) {
     c.ch = ch;
     int ring_size = (int)std::ceil(g->sample_rate * 0.006f / 128.f) + 1;  // dynamics_compressor.rs:250-255
     c.delay_frames = (ring_size - 1) * 128;
+    // (the layout ring holds the look-ahead's quanta and the one being written: 38 slots at the highest sample rate the ABI takes)
+    if (ring_size > COMP_META_RING) return bail(WAE_UNSUPPORTED, "compressor look-ahead longer than its layout ring");
     c.ring_len = next_pow2((uint64_t)c.delay_frames + 128);
     c.ring = alloc<float>((size_t)ch * c.ring_len, true, true);
     c.state = alloc<float>(2, true, true);
-    c.meta_ring = alloc<uint8_t>(8, true, true);
+    c.meta_ring = alloc<uint8_t>(COMP_META_RING, true, true);
     if (!c.ring || !c.state || !c.meta_ring) return bail(WAE_OUT_OF_MEMORY, "out of device memory (compressor)");
     // the look-ahead ring starts out silent and hands on the layout of the quantum it delays (dynamics_compressor.rs:340-349,452-468)
     out_dynamic(nc, Lay{1, in0.hi, in0.nlo, in0.nhi, true});

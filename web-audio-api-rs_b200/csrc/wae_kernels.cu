@@ -3303,9 +3303,9 @@ __global__ void __launch_bounds__(32) k_compressor(const CompInst* __restrict__ 
             const int64_t q_abs = (ci.f0 + n) >> 7;
             cur_silent = buf_silent(q.in, q.ch, qi);
             cur_ch = buf_count(q.in, q.ch, qi);
-            q.meta_ring[q_abs & 7] = (uint8_t)(cur_ch | (cur_silent ? WAE_META_SILENT : 0));
+            q.meta_ring[q_abs & (COMP_META_RING - 1)] = (uint8_t)(cur_ch | (cur_silent ? WAE_META_SILENT : 0));
             uint8_t dm = (uint8_t)(1 | WAE_META_SILENT);  // the ring starts out as silent quanta (:340-349)
-            if (q_abs - D >= 0) dm = q.meta_ring[(q_abs - D) & 7];
+            if (q_abs - D >= 0) dm = q.meta_ring[(q_abs - D) & (COMP_META_RING - 1)];
             out_silent = (dm & WAE_META_SILENT) != 0;
             out_ch = out_silent ? 1 : (dm & 0x3f);
             if (q.out.meta) meta_put_all(q.out, q.ch, qi, out_ch, out_silent);
@@ -3319,8 +3319,10 @@ __global__ void __launch_bounds__(32) k_compressor(const CompInst* __restrict__ 
             thr = knee > 0.f ? threshold + knee / 2.f : threshold;
             half_knee = knee / 2.f;
             knee_partial = (1.f / ratio - 1.f) / (2.f * knee);
-            attack_tau = expf(-1.f / (attack * q.sample_rate));
-            release_tau = expf(-1.f / (release * q.sample_rate));
+            // correctly rounded, as the reference's f32 exp: at high rates 1 - tau is only a few hundred ulps, so expf's error of up
+            // to one ulp would change the detector's attack / release rate by up to 1 %
+            attack_tau = (float)exp((double)(-1.f / (attack * q.sample_rate)));
+            release_tau = (float)exp((double)(-1.f / (release * q.sample_rate)));
             const float full_range_gain = thr + (-thr / ratio);
             const float full_range_makeup = 1.f / db_to_lin(full_range_gain);
             makeup_gain = lin_to_db(powf(full_range_makeup, 0.6f));
