@@ -740,7 +740,8 @@ WAE_API wae_status wae_batch_bind_value_curves(wae_batch* batch, const wae_value
  * wae_source_start unless wae_buffer_source_set_device_offset declares them too.  A bound time is clamped to its window [lo, hi] (a NaN becomes lo); the reference panics on a negative or non-finite
  * `when`, which a bind on the device cannot do.  The source is always planned with a gated output layout, and its path never depends on
  * the bound times: a non-looping AudioBufferSourceNode whose computed playback rates are all > 0 and not automated takes the bound slow
- * track (k_buffer_source_slow(bound), which plays a rate of 1 from an aligned start 1:1), every other one the serial kernel.  A declared
+ * track (k_buffer_source_slow(bound), which plays a rate of 1 from an aligned start 1:1), a looping one the path of its loop declaration
+ * (wae_buffer_source_set_device_loop), every other one the serial kernel.  A declared
  * source is never fused into k_chain.
  * WAE_INVALID_ARGUMENT: not a scheduled source node, a window that is not finite with 0 <= lo <= hi.  WAE_INVALID_STATE: a source that
  * has not been started, a second declaration, or a graph with a suspend point.  After the declaration, wae_source_start / wae_source_stop
@@ -774,6 +775,40 @@ typedef struct wae_schedule_binding {
  * the node has no declaration.  wae_batch_run, wae_batch_run_group and wae_batch_run_pipelined answer WAE_INVALID_STATE while a declared
  * schedule of the batch has never been bound (a declared source the batch never renders needs no bind). */
 WAE_API wae_status wae_batch_bind_schedules(wae_batch* batch, const wae_schedule_binding* items, uint32_t n, void* stream);
+
+/* ---- Loop points of AudioBufferSourceNodes bound from device memory ----------------------------------------------------------------
+ * Declares that the loopStart and loopEnd of a looping AudioBufferSourceNode are supplied per run from device memory
+ * (wae_batch_bind_loops), so that one prepared batch loops any region of its clip without being built and planned again.  Both are
+ * declared together: a caller who wants only one pins the other with a window [v, v].  The current loop_start / loop_end become
+ * placeholders, the windows' low ends: the plan is the one of a source built with them.  A bound value is clamped to its window (a NaN
+ * becomes lo); the reference stores any f64.  The reference's clamp_loop_boundaries and actual-loop-point rules then apply on the device.
+ * The playback path is decided from the windows and the declared rates, never from the bound values: a source whose computed playback
+ * rates are all > 0 and not automated, whose shortest possible loop is longer than four output frames at the top rate, and whose
+ * playhead table fits 65536 segments, takes the bound slow track (k_buffer_source_slow(bound)), whose table is derived on the device
+ * after each bind; every other one the serial kernel.  A looping source with a bound playbackRate / detune or a bound schedule but no
+ * loop declaration stays on the serial kernel: to put it on the bound slow track, declare its loop with one-point windows [ls, ls],
+ * [le, le].
+ * WAE_INVALID_ARGUMENT: not an AudioBufferSourceNode, a window that is not finite with 0 <= lo <= hi.  WAE_INVALID_STATE: the node's
+ * `loop` is false, a second declaration, or a graph with a suspend point.  After the declaration, wae_node_set_attribute with
+ * WAE_ATTR_LOOP / _LOOP_START / _LOOP_END on the node and wae_graph_suspend on the graph answer WAE_INVALID_STATE.  wae_render_batch and
+ * wae_render_many answer WAE_INVALID_STATE on graphs with declarations; wae_batch_plan plans them. */
+WAE_API wae_status wae_buffer_source_set_device_loop(wae_graph* graph, wae_node_id node, double start_lo, double start_hi, double end_lo,
+                                                     double end_hi);
+
+typedef struct wae_loop_binding {
+    uint32_t graph_index;  /* caller's index, as wae_batch_fetch_graph */
+    wae_node_id node;      /* declared with wae_buffer_source_set_device_loop */
+    const double* points;  /* device memory of the engine's GPU, 8-byte aligned: the row loop_start, loop_end */
+} wae_loop_binding;
+
+/* Writes the loop points into the batch, asynchronously on the engine stream after the work already queued on `stream` (as
+ * wae_batch_bind_sources).  All-or-nothing: every item is validated before anything is enqueued.  Bound loop points stay until they are
+ * bound again.  WAE_INVALID_ARGUMENT: `points` is null, not 8-byte aligned or not device (or managed) memory of the engine's GPU, the row
+ * does not lie in one allocation, or one node is named twice in the call.  WAE_INVALID_STATE: graph_index out of range, or the node has
+ * no declaration.  wae_batch_run, wae_batch_run_group and wae_batch_run_pipelined answer WAE_INVALID_STATE while declared loop points of
+ * the batch have never been bound (a declared source the batch never renders needs no bind).  wae_batch_sync answers WAE_CUDA_ERROR if a
+ * playhead table derived on the device ever needed more segments than were planned for it (a defect: the render is wrong). */
+WAE_API wae_status wae_batch_bind_loops(wae_batch* batch, const wae_loop_binding* items, uint32_t n, void* stream);
 
 /* PeriodicWave::new(context, PeriodicWaveOptions { real, imag, disable_normalization }) (src/periodic_wave.rs:104-209): fills `table`
  * (PERIODIC_WAVE_TABLE_LENGTH = 8192 in the reference) with the wavetable an OscillatorNode of type Custom plays.  `real` / `imag` may be

@@ -160,6 +160,12 @@ class ScheduleBinding(C.Structure):
     _fields_ = [("graph_index", C.c_uint32), ("node", C.c_uint32), ("times", c_double_p)]
 
 
+class LoopBinding(C.Structure):
+    """wae_loop_binding: the device row loop_start, loop_end of one declared looping AudioBufferSourceNode of a prepared batch
+    (wae_batch_bind_loops)."""
+    _fields_ = [("graph_index", C.c_uint32), ("node", C.c_uint32), ("points", c_double_p)]
+
+
 STATUS_NAMES = {0: "OK", 1: "INVALID_ARGUMENT", 2: "INVALID_STATE", 3: "NOT_SUPPORTED", 4: "UNSUPPORTED",
                 5: "CUDA_ERROR", 6: "OUT_OF_MEMORY", 7: "NO_DEVICE"}
 
@@ -206,6 +212,7 @@ WAE_SYMBOLS = [
     "wae_iir_filter_set_device_coefficients", "wae_batch_bind_iir_coefficients",
     "wae_param_set_device_value_curve", "wae_batch_bind_value_curves",
     "wae_source_set_device_schedule", "wae_batch_bind_schedules", "wae_buffer_source_set_device_offset",
+    "wae_buffer_source_set_device_loop", "wae_batch_bind_loops",
 ]
 
 
@@ -331,6 +338,9 @@ class Api:
             f("source_set_device_schedule", C.c_int32, [gp, C.c_uint32, C.c_double, C.c_double, C.c_int32, C.c_double, C.c_double])
             f("batch_bind_schedules", C.c_int32, [C.c_void_p, C.POINTER(ScheduleBinding), C.c_uint32, C.c_void_p])
             f("buffer_source_set_device_offset", C.c_int32, [gp, C.c_uint32, C.c_double, C.c_double, C.c_int32, C.c_double, C.c_double])
+            # loop points bound from device memory
+            f("buffer_source_set_device_loop", C.c_int32, [gp, C.c_uint32, C.c_double, C.c_double, C.c_double, C.c_double])
+            f("batch_bind_loops", C.c_int32, [C.c_void_p, C.POINTER(LoopBinding), C.c_uint32, C.c_void_p])
         else:
             f("graph_create", C.c_int32, [C.c_uint32, C.c_uint64, C.c_float, C.POINTER(C.c_void_p)])
             f("render", C.c_int32, [gp, c_float_p])

@@ -352,6 +352,19 @@ class AudioBufferSourceNode(AudioScheduledSourceNode):
             self._ctx._device_schedules[self.id] = (stop is not None, True, duration is not None)
         return self
 
+    def set_device_loop(self, start, end):
+        """wae_buffer_source_set_device_loop (product only): the loopStart and loopEnd of this looping source are supplied by
+        Batch.bind_loops from device memory before each run, clamped to the windows `start` = (lo, hi) and `end` = (lo, hi).  Pin one of
+        them with a one-point window.  The node takes no further set_loop / set_loop_start / set_loop_end."""
+        api = self._ctx._api
+        if not api.is_product:
+            raise B.WaeError(3, "loop points bound from device memory are a feature of the GPU engine")
+        s_lo, s_hi = (float(x) for x in start)
+        e_lo, e_hi = (float(x) for x in end)
+        api.check(api.buffer_source_set_device_loop(self._ctx._g, self.id, s_lo, s_hi, e_lo, e_hi))
+        self._ctx._device_loops.add(self.id)
+        return self
+
 
 def _response_arrays(frequency_hz):
     f = np.ascontiguousarray(frequency_hz, dtype=np.float32)
@@ -549,6 +562,7 @@ class OfflineAudioContext:
         self._device_iirs = {}  # node id -> (feedforward count, feedback count) declared with set_device_coefficients
         self._device_value_curves = {}  # (node id, param index) -> length declared with set_device_value_curve
         self._device_schedules = {}  # node id -> whether set_device_schedule declared the stop time too
+        self._device_loops = set()  # ids of the nodes declared with set_device_loop
 
     def __del__(self):
         try:
@@ -1029,6 +1043,32 @@ class Batch:
             for j, nid in enumerate(ids):
                 items[i * k + j] = B.ScheduleBinding(g, nid, C.cast(C.c_void_p(base + 8 * width * (i * k + j)), B.c_double_p))
         self._bind(self.api.batch_bind_schedules, items, n * k, times)
+
+    def bind_loops(self, nodes, starts, ends, graphs=None):
+        """wae_batch_bind_loops: starts[i] and ends[i] become the loopStart and loopEnd of the AudioBufferSourceNode `nodes` (declared
+        with set_device_loop) in context graphs[i] (default: 0..n-1).  Each is a float64 CUDA tensor [n] for one node, or [n][k] for a
+        list of k nodes.  One call, ordered after torch's current stream; the values are read on the engine stream, and their memory is
+        kept from reuse until they have been."""
+        import torch
+        for t in (starts, ends):
+            if not (isinstance(t, torch.Tensor) and t.is_cuda and t.dtype == torch.float64 and t.dim() in (1, 2)):
+                raise B.WaeError(1, "bind_loops: starts / ends must be float64 CUDA tensors [n] or [n][k]")
+        many = isinstance(nodes, (list, tuple))
+        ids = [int(getattr(x, "id", x)) for x in nodes] if many else [int(getattr(nodes, "id", nodes))]
+        n, k = starts.shape[0], len(ids)
+        if (starts.dim() == 2) != many or (many and starts.shape[1] != k):
+            raise B.WaeError(1, f"bind_loops: starts is {list(starts.shape)} for {k} node(s): [n] for one node, [n][k] for a list")
+        if ends.shape != starts.shape:
+            raise B.WaeError(1, f"bind_loops: ends is {list(ends.shape)}, starts {list(starts.shape)}")
+        graphs = self._graphs("bind_loops", graphs, n, "rows")
+        # one item reads its row loop_start, loop_end from adjacent memory: the values are packed on torch's current stream
+        points = torch.stack([starts.reshape(n, k), ends.reshape(n, k)], dim=2).contiguous()
+        items = (B.LoopBinding * max(n * k, 1))()
+        base = points.data_ptr()
+        for i, g in enumerate(graphs):
+            for j, nid in enumerate(ids):
+                items[i * k + j] = B.LoopBinding(g, nid, C.cast(C.c_void_p(base + 16 * (i * k + j)), B.c_double_p))
+        self._bind(self.api.batch_bind_loops, items, n * k, points)
 
     def _graphs(self, fn, graphs, n, rows, ids=None):
         """The graph indices of n rows of binding items: `graphs` (default 0..n-1), each in range; `ids`: the node ids of the rows, whose

@@ -699,6 +699,8 @@ WAE_API wae_status wae_graph_suspend(wae_graph* g, double suspend_time) {
     if (quantum >= total) return fail(WAE_INVALID_STATE, "InvalidStateError - cannot suspend after the end of the rendering");
     if (g->device_schedules)  // (sources are planned per render segment from their start time)
         return fail(WAE_INVALID_STATE, "InvalidStateError - the graph has schedules bound from device memory (wae_source_set_device_schedule)");
+    if (g->device_loops)  // (the reference allows loop changes after start, which suspend points do not lower)
+        return fail(WAE_INVALID_STATE, "InvalidStateError - the graph has loop points bound from device memory (wae_buffer_source_set_device_loop)");
     g->epochs.push_back(wae_graph::Epoch{quantum * 128, g->nodes});
     return WAE_OK;
 }
@@ -1074,6 +1076,32 @@ WAE_API wae_status wae_buffer_source_set_device_offset(wae_graph* g, wae_node_id
     return WAE_OK;
 }
 
+// loopStart and loopEnd become placeholders (the windows' low ends), written per run by wae_batch_bind_loops clamped to their windows.
+// The planner decides the playback path from the windows (and the declared rates), never from the bound values.
+WAE_API wae_status wae_buffer_source_set_device_loop(wae_graph* g, wae_node_id node, double start_lo, double start_hi, double end_lo,
+                                                     double end_hi) {
+    if (!g) return fail(WAE_INVALID_ARGUMENT, "null graph");
+    Node* n = g->nodes.get(node);
+    if (!n || n->kind != K_ABSN) return fail(WAE_INVALID_ARGUMENT, "not an AudioBufferSourceNode");
+    auto window = [](double lo, double hi) { return std::isfinite(lo) && std::isfinite(hi) && 0. <= lo && lo <= hi; };
+    if (!window(start_lo, start_hi) || !window(end_lo, end_hi))
+        return fail(WAE_INVALID_ARGUMENT, "RangeError - a loop window must be finite with 0 <= lo <= hi");
+    if (!n->loop) return fail(WAE_INVALID_STATE, "InvalidStateError - the source does not loop (set_loop)");
+    if (n->device_loop)
+        return fail(WAE_INVALID_STATE, "InvalidStateError - the loop points are already bound from device memory (wae_buffer_source_set_device_loop)");
+    if (!g->epochs.empty())
+        return fail(WAE_INVALID_STATE, "InvalidStateError - loop points are bound from device memory in a graph with a suspend point");
+    n->device_loop = true;
+    n->loop_start = start_lo;
+    n->loop_end = end_lo;
+    n->loop_lo[0] = start_lo;
+    n->loop_hi[0] = start_hi;
+    n->loop_lo[1] = end_lo;
+    n->loop_hi[1] = end_hi;
+    g->device_loops++;
+    return WAE_OK;
+}
+
 WAE_API wae_status wae_oscillator_set_type(wae_graph* g, wae_node_id node, uint32_t type) {
     auto ni = g->nodes.find(node);
     if (ni == g->nodes.end() || ni->second.kind != K_OSC) return fail(WAE_INVALID_ARGUMENT, "not an oscillator");
@@ -1348,6 +1376,8 @@ WAE_API wae_status wae_node_set_attribute(wae_graph* g, wae_node_id node, uint32
             // engine are planned per segment from the start time, so a change at a suspend point of a started source is refused
             if (!g->epochs.empty() && n.has_start)
                 return fail(WAE_UNSUPPORTED, "changing the loop attributes of a started AudioBufferSourceNode at a suspend point is not lowered to the GPU");
+            if (n.device_loop)
+                return fail(WAE_INVALID_STATE, "InvalidStateError - the loop points are bound from device memory (wae_buffer_source_set_device_loop)");
             if (attribute == WAE_ATTR_LOOP) n.loop = value != 0.;
             else if (attribute == WAE_ATTR_LOOP_START) n.loop_start = value;
             else n.loop_end = value;

@@ -98,7 +98,8 @@ struct AbsnSlowInst {
 // positive computed rates (k_buffer_source_slow<true>).  The record holds what does not depend on the rate; each run derives the rest
 // from `rate` and `detune` (patched by wae_batch_bind_params) with absn_slow_derive, the planner's own expressions.
 struct AbsnBoundInst {
-    AbsnSlowInst s;        // step, offset0, elapsed0 and the segment table are derived per run (one segment: the source does not loop)
+    AbsnSlowInst s;        // step, offset0, elapsed0 are derived per run; the segment table too (one segment) unless s.loop, whose
+                           // table k_absn_loop_schedule derives after each bind that reaches it (loop points bound from device memory)
     double dt;             // the planner clock's frame duration
     double offset;         // start(when, offset): the requested offset
     double start_delta;    // t_first - start: the first playing frame's time after the start time
@@ -641,6 +642,34 @@ struct SchedBindItem {
     double lo[4], hi[4];        // the declared windows the values are clamped to (a NaN becomes lo): start, stop, offset, duration
     int32_t n_patches;
     int32_t binds;              // SchedBinds
+};
+
+// ---- wae_batch_bind_loops: caller loop points -> the records of a declared looping AudioBufferSourceNode ------------------------------
+enum LoopKind : int32_t {
+    LOOP_BOUND = 0,   // AbsnBoundInst: s.loop_start / s.loop_end = the actual loop points (k_absn_loop_schedule then walks its table)
+    LOOP_SERIAL = 1,  // AbsnSerialInst: loop_start / loop_end after clamp_loop_boundaries (the kernel takes them as they are)
+};
+struct LoopPatch {
+    void* dst;               // the record
+    int32_t kind;
+    int32_t pad;
+    double buffer_duration;  // of the source's buffer (clamp_loop_boundaries)
+};
+struct LoopBindItem {
+    const double* points;     // caller's row: loop_start, loop_end (8 B aligned)
+    const LoopPatch* patches;  // the node's entries
+    double lo[2], hi[2];       // the declared windows the values are clamped to (a NaN becomes lo): start, end
+    int32_t n_patches;
+    int32_t pad;
+};
+// A looping record of the bound slow track whose playhead table is derived on the device (k_absn_loop_schedule, one thread per walk)
+// from its loop points, rate, detune, start, offset and duration, into the table the record points at (s.seg_n / s.seg_bt, `cap`
+// segments).  `lq`: the frames its group renders.
+struct LoopWalk {
+    AbsnBoundInst* rec;
+    int64_t lq;
+    int32_t cap;
+    int32_t pad;
 };
 
 // ---- wae_batch_bind_params: per-run values of params planned as constants ------------------------------------------------------

@@ -341,6 +341,21 @@ struct StageBuild {
         SchedPatch p;    // dst set when the tables are uploaded
     };
     std::vector<SchedPatchRec> sched_patches;
+    // Patch entries of loop points bound from device memory (wae_buffer_source_set_device_loop): record `rec` of this stage's table
+    // (S_ABSN_BOUND / S_ABSN_SERIAL); and the looping S_ABSN_BOUND records whose playhead tables are derived on the device
+    struct LoopPatchRec {
+        uint32_t graph;  // batch position
+        wae_node_id node;
+        int32_t rec;
+        LoopPatch p;     // dst set when the tables are uploaded
+    };
+    std::vector<LoopPatchRec> loop_patches;
+    struct LoopWalkRec {
+        int32_t rec;
+        int32_t cap;
+        int64_t lq;
+    };
+    std::vector<LoopWalkRec> loop_walks;
     // Spatial entries of static panners whose source or listener is bound from device memory (wae_param_set_device_value): record `rec`
     // of this stage's table (S_PAN: PanInst, S_HRTF: HrtfInst), `off` bytes into it, or -1 for an HRTF panner lowered to a convolver,
     // whose entry's dst / resp the planner sets and whose bind also rewrites the spectra `spec` of `S` partitions.  Operands name their
@@ -438,7 +453,7 @@ struct BindKind {
     const char* bind;     // the call that binds them
     uint32_t wae_graph::*count;  // the graph's number of declarations
 };
-enum { BK_SOURCES, BK_PARAMS, BK_RESPONSES, BK_CURVES, BK_WAVES, BK_IIRS, BK_VALUE_CURVES, BK_SCHEDULES, BK_COUNT };
+enum { BK_SOURCES, BK_PARAMS, BK_RESPONSES, BK_CURVES, BK_WAVES, BK_IIRS, BK_VALUE_CURVES, BK_SCHEDULES, BK_LOOPS, BK_COUNT };
 const BindKind kBindKinds[BK_COUNT] = {
     {"device input", "device inputs", "wae_buffer_source_set_device_input", "wae_batch_bind_sources", &wae_graph::device_inputs},
     {"param bound from device memory", "params bound from device memory", "wae_param_set_device_value", "wae_batch_bind_params",
@@ -455,6 +470,8 @@ const BindKind kBindKinds[BK_COUNT] = {
      "wae_batch_bind_value_curves", &wae_graph::device_value_curves},
     {"schedule bound from device memory", "schedules bound from device memory", "wae_source_set_device_schedule", "wae_batch_bind_schedules",
      &wae_graph::device_schedules},
+    {"loop points bound from device memory", "loop points bound from device memory", "wae_buffer_source_set_device_loop",
+     "wae_batch_bind_loops", &wae_graph::device_loops},
 };
 
 // The name of a declaration: (batch position, node, param index); kinds declared on a node take kNodeLevel as param index
@@ -565,6 +582,10 @@ struct DevSchedule {  // wae_source_set_device_schedule (+ wae_buffer_source_set
     double lo[4], hi[4];
     int32_t p0, p1;  // in d_sched_patches
 };
+struct DevLoop {         // wae_buffer_source_set_device_loop: the windows and the entries of every record the loop points reach
+    double lo[2], hi[2];
+    int32_t p0, p1;  // in d_loop_patches
+};
 struct DevValueCurve {  // wae_param_set_device_value_curve: the param's curve pool (ParamInst::curves, made by the planner) and where
     float* pool;        // the declared values lie in it
     int32_t values_off;
@@ -633,6 +654,7 @@ struct wae_batch {
     Bindings<DevIir> iirs{kBindKinds[BK_IIRS]};
     Bindings<DevValueCurve> value_curves{kBindKinds[BK_VALUE_CURVES]};
     Bindings<DevSchedule> schedules{kBindKinds[BK_SCHEDULES]};
+    Bindings<DevLoop> loops{kBindKinds[BK_LOOPS]};
     // The item table of a bind is staged in page-locked memory (a copy from pageable memory would wait for the engine stream first) and
     // copied to d_bind, which the next bind may overwrite at once (its copy is queued behind this bind's kernel on the same stream).  A
     // staging buffer is reused once its copy has run (its event has completed); while all are in flight a new one is made, so a bind
@@ -664,6 +686,12 @@ struct wae_batch {
     CurvePatch* d_curve_patches = nullptr;
     IirPatch* d_iir_patches = nullptr;
     SchedPatch* d_sched_patches = nullptr;
+    LoopPatch* d_loop_patches = nullptr;
+    // the looping bound slow-track records whose playhead tables k_absn_loop_schedule derives after every bind of loop points, params or
+    // schedules (their inputs); d_loop_overflow: set by a walk that outgrew its table (reported by wae_batch_sync)
+    LoopWalk* d_loop_walks = nullptr;
+    int n_loop_walks = 0;
+    int* d_loop_overflow = nullptr;
     cudaEvent_t ev_bind = nullptr;  // orders a bind after the caller's stream
     // OfflineAudioContext::suspend_sync: a group's render is cut at the suspend frames of its graphs (graphs with different
     // suspend points are put in different groups); every segment has its own plan, node state is shared between the plans
@@ -1518,8 +1546,8 @@ struct Planner {
     bool absn_silent(NodeCtx& nc);
     bool absn_serial(NodeCtx& nc, const AbsnPlay& s, const PRef& pdet, const PRef& prate);
     bool absn_slow(NodeCtx& nc, const AbsnPlay& s);
-    bool absn_bound(NodeCtx& nc, const AbsnPlay& s, const PRef& pdet, const PRef& prate, int64_t q, bool aligned, double rate_hi);
-    void absn_schedule(const AbsnSlowInst& a, int64_t n_first, double off, std::vector<int64_t>& seg_n, std::vector<double>& seg_bt) const;
+    bool absn_bound(NodeCtx& nc, const AbsnPlay& s, const PRef& pdet, const PRef& prate, int64_t q, bool aligned, double rate_hi,
+                    int32_t loop_cap);
     bool absn_fast(NodeCtx& nc, const AbsnPlay& s, int64_t q, bool fused);
     bool lower_biquad(NodeCtx& nc);
     bool lower_iir(NodeCtx& nc);
@@ -1658,6 +1686,8 @@ static void merge_builds(Builds& dst, Builds& src) {
         }
         for (auto& cp : s.curve_patches) cp.rec += (int32_t)bs.records;
         for (auto& sp : s.sched_patches) sp.rec += (int32_t)bs.records;
+        for (auto& lp : s.loop_patches) lp.rec += (int32_t)bs.records;
+        for (auto& lw : s.loop_walks) lw.rec += (int32_t)bs.records;
         for (auto& sp : s.spatial)
             if (sp.rec >= 0) sp.rec += (int32_t)bs.spatial;
         for (auto& ip : s.iir_patches) {
@@ -1696,6 +1726,8 @@ static void merge_builds(Builds& dst, Builds& src) {
         append_vec(d.curve_patches, s.curve_patches);
         append_vec(d.iir_patches, s.iir_patches);
         append_vec(d.sched_patches, s.sched_patches);
+        append_vec(d.loop_patches, s.loop_patches);
+        append_vec(d.loop_walks, s.loop_walks);
         append_vec(d.spatial, s.spatial);
         d.n_scan_coef += s.n_scan_coef;
         d.max_ch = std::max(d.max_ch, s.max_ch);
@@ -2570,6 +2602,28 @@ bool Planner::lower_const(NodeCtx& nc) {
     return true;
 }
 
+// A looping source whose loop points are bound from device memory, on the bound slow track: the capacity of its playhead table (segments),
+// or 0 when its windows and computed rates [rate_lo, rate_hi] do not allow the track.  Decided from the declared ranges only.
+//  - The shortest actual loop the windows allow is min(end_lo, duration) - min(start_hi, duration) (clamp_loop_boundaries); it must be
+//    longer than four output frames at the top rate (the host rule of a built loop), so no frame wraps twice.  Overlapping windows fail.
+//  - A step at the lowest rate wider than two snap zones (almost::equal around a loop point: < 3e-8 (1 + duration)) lets at most one
+//    frame per pass be snapped without a wrap.
+//  - Over `frames` frames the playhead advances at most frames * dt * rate_hi; each wrap takes back at least the shortest loop, so it
+//    wraps at most W = floor(frames * dt * rate_hi / shortest) + 1 times.  Every segment is a wrap or a snap, and a snap without a wrap
+//    happens once, on the way into the loop: at most W + 2 segments with the first.  The capacity is 2 (W + 1) + 4, which also covers the
+//    rounding of the device's exp2 and the snaps' own displacement of the playhead.
+constexpr int32_t kLoopSegmentsMax = 1 << 16;  // per record: 1 MiB of table
+static int32_t absn_loop_capacity(const Node& n, double duration, double dt, double rate_lo, double rate_hi, int64_t frames) {
+    const double max_start = std::min(n.loop_hi[0], duration);
+    const double min_end = n.loop_lo[1] > duration ? duration : n.loop_lo[1];
+    const double shortest = min_end - max_start;
+    if (!(shortest > 4. * dt * rate_hi)) return 0;
+    if (!(dt * rate_lo > 6.0e-8 * (1. + duration))) return 0;
+    const double wraps = std::floor((double)frames * dt * rate_hi / shortest) + 1.;
+    const double cap = 2. * (wraps + 1.) + 4.;
+    return cap > (double)kLoopSegmentsMax ? 0 : (int32_t)cap;
+}
+
 bool Planner::lower_absn(NodeCtx& nc) {
     Node& n = nc.n;
     const double sr = (double)g->sample_rate;
@@ -2588,21 +2642,28 @@ bool Planner::lower_absn(NodeCtx& nc) {
     const int64_t q = absn_start_quantum(clock, n.start_time);
     bool aligned = (n.start_time <= clock.block_time(q)) && n.offset == 0.;  // start in the past snaps to the block
     // (a schedule bound from device memory: the start may fall anywhere, the bound slow track or the serial kernel plays it)
-    bool fast = !rate_automated && !rate_bound && !n.device_schedule && aligned && (double)pb.sample_rate / sr == 1. && computed_rate == 1. &&
+    bool fast = !rate_automated && !rate_bound && !n.device_schedule && !n.device_loop && aligned && (double)pb.sample_rate / sr == 1. && computed_rate == 1. &&
                 ls == 0. && le == duration && n.duration > 1e300 && n.stop_time > 1e300;
     // everything the closed-form tracks do not cover runs the renderer's own frame loop (one warp per source)
     bool serial = rate_automated || (!fast && !(computed_rate > 0.)) || (n.device_schedule && n.loop);
     // playbackRate / detune bound from device memory: the path follows from the computed rates their declared ranges allow (the low
     // corner's exp2 underflows to 0 far enough below 0 cents), never from the value.  A non-looping source whose rates are all positive
     // takes the bound slow track; the serial kernel is right for every other value.
-    double rate_hi = computed_rate;
+    double rate_lo = computed_rate, rate_hi = computed_rate;
     if (rate_bound) {
         const bool br = prate.bound >= 0, bd = pdet.bound >= 0;
-        const double rate_lo = (double)(br ? prate.lo : rate) * std::exp2((double)(bd ? pdet.lo : detune) / 1200.);
+        rate_lo = (double)(br ? prate.lo : rate) * std::exp2((double)(bd ? pdet.lo : detune) / 1200.);
         rate_hi = (double)(br ? prate.hi : rate) * std::exp2((double)(bd ? pdet.hi : detune) / 1200.);
         serial = rate_automated || n.loop || !(rate_lo > 0.);
     }
-    if (!fast && !serial && n.loop) {
+    // loop points bound from device memory: the bound slow track when the windows and the rates allow a playhead table of bounded size
+    // (absn_loop_capacity), else the serial kernel
+    int32_t loop_cap = 0;
+    if (n.device_loop) {
+        loop_cap = rate_automated || !(rate_lo > 0.) ? 0 : absn_loop_capacity(n, duration, clock.dt, rate_lo, rate_hi, lq);
+        serial = loop_cap == 0;
+    }
+    if (!fast && !serial && n.loop && !n.device_loop) {
         const bool custom = ls >= 0. && le > 0. && ls < le;
         const double loop_len = custom ? le - ls : duration;
         if (!(loop_len > 4. * clock.dt * computed_rate)) serial = true;  // loop shorter than four output frames
@@ -2630,7 +2691,7 @@ bool Planner::lower_absn(NodeCtx& nc) {
     }
     const AbsnPlay s{&pb, d_buf, len, stride, ch, duration, ls, le, computed_rate};
     if (serial) return absn_serial(nc, s, pdet, prate);
-    if (rate_bound || n.device_schedule) return absn_bound(nc, s, pdet, prate, q, aligned, rate_hi);
+    if (rate_bound || n.device_schedule || n.device_loop) return absn_bound(nc, s, pdet, prate, q, aligned, rate_hi, loop_cap);
     if (!fast) return absn_slow(nc, s);
     return absn_fast(nc, s, q, fused);
 }
@@ -2682,6 +2743,8 @@ bool Planner::absn_serial(NodeCtx& nc, const AbsnPlay& s, const PRef& pdet, cons
             add_patch(sb, r, (uint32_t)offs[i]);
         }
     if (n.device_schedule) add_sched_patch(sb, n, sched_entry(n, SCHED_ABSN_SERIAL));  // (the raw start / stop times)
+    if (n.device_loop)  // (the loop points after clamp_loop_boundaries)
+        sb.loop_patches.push_back(StageBuild::LoopPatchRec{gi, n.id, (int32_t)sb.records() - 1, LoopPatch{nullptr, LOOP_SERIAL, 0, s.duration}});
     algorithmic_bytes += (uint64_t)s.ch * 4ull * (uint64_t)std::min<int64_t>(lq, (int64_t)s.len);
     return true;
 }
@@ -2719,11 +2782,20 @@ bool Planner::absn_slow(NodeCtx& nc, const AbsnPlay& s) {
     a.step = d.step;
     a.offset0 = d.offset0;
     a.elapsed0 = d.elapsed0;
-    const double off = d.offset0;
-    std::vector<int64_t> seg_n{n_first};
-    std::vector<double> seg_bt{off};
-    if (n.loop && off < a.loop_end) absn_schedule(a, n_first, off, seg_n, seg_bt);
-    a.n_seg = (int32_t)seg_n.size();
+    std::vector<int64_t> seg_n(64);
+    std::vector<double> seg_bt(64);
+    int32_t n_seg = 1;
+    seg_n[0] = n_first;
+    seg_bt[0] = d.offset0;
+    const int64_t n_end = std::min<int64_t>(lq, a.n_stop);
+    while (n.loop && (n_seg = absn_loop_segments(a.loop_start, a.loop_end, d.step, n_first, n_end, d.offset0, seg_n.data(), seg_bt.data(),
+                                                 (int32_t)seg_n.size())) < 0) {
+        seg_n.resize(seg_n.size() * 4);
+        seg_bt.resize(seg_bt.size() * 4);
+    }
+    seg_n.resize(n_seg);
+    seg_bt.resize(n_seg);
+    a.n_seg = n_seg;
     a.seg_n = upload(seg_n);
     a.seg_bt = upload(seg_bt);
     // layout: silent before the quantum of the first playing frame and after the quantum in which the source ends
@@ -2736,7 +2808,8 @@ bool Planner::absn_slow(NodeCtx& nc, const AbsnPlay& s) {
 
 // ---- playbackRate / detune bound from device memory, a non-looping source whose declared rates are all positive: the slow track's
 // constants that do not depend on the rate, and the bound values (PATCH_RAW); k_buffer_source_slow<true> derives the rest per run
-bool Planner::absn_bound(NodeCtx& nc, const AbsnPlay& s, const PRef& pdet, const PRef& prate, int64_t q, bool aligned, double rate_hi) {
+bool Planner::absn_bound(NodeCtx& nc, const AbsnPlay& s, const PRef& pdet, const PRef& prate, int64_t q, bool aligned, double rate_hi,
+                         int32_t loop_cap) {
     Node& n = nc.n;
     const double sr = (double)g->sample_rate;
     AbsnBoundInst r{};
@@ -2758,8 +2831,24 @@ bool Planner::absn_bound(NodeCtx& nc, const AbsnPlay& s, const PRef& pdet, const
     r.start_delta = st.t_first - st.start;
     r.n_start = q * 128;
     r.fast_end = absn_fast_end(clock, lq, r.n_start, s.duration);
-    const bool fast_shape = (double)s.pb->sample_rate / sr == 1. && s.ls == 0. && s.le == s.duration && n.duration > 1e300;
+    const bool fast_shape = (double)s.pb->sample_rate / sr == 1. && s.ls == 0. && s.le == s.duration && n.duration > 1e300 && !n.device_loop;
     r.fast_ok = aligned && fast_shape && n.stop_time > 1e300;
+    if (n.device_loop) {  // the placeholders' actual loop points and a table of loop_cap segments, both rewritten by the binds
+        const AbsnLoopPoints lp = absn_loop_points(n.loop_start, n.loop_end, s.duration);
+        a.loop = 1;
+        a.loop_start = lp.actual_start;
+        a.loop_end = lp.actual_end;
+        a.n_seg = 1;
+        if (dry) {
+            a.seg_n = reinterpret_cast<const int64_t*>(uintptr_t(256));
+            a.seg_bt = reinterpret_cast<const double*>(uintptr_t(256));
+        } else {
+            a.seg_n = b->dalloc<int64_t>((size_t)loop_cap, true);
+            a.seg_bt = b->dalloc<double>((size_t)loop_cap, true);
+            if (!a.seg_n || !a.seg_bt) return bail(WAE_OUT_OF_MEMORY, "out of device memory (loop playhead table)");
+            b->asset_bytes += (size_t)loop_cap * (sizeof(int64_t) + sizeof(double));
+        }
+    }
     r.rate = prate.v;
     r.detune = pdet.v;
     // The one decision the range drives: a constant layout only when the source plays to the end of the render at every rate it allows.
@@ -2767,8 +2856,10 @@ bool Planner::absn_bound(NodeCtx& nc, const AbsnPlay& s, const PRef& pdet, const
     const AbsnSlowDerived top = absn_slow_derive(clock.dt, rate_hi, n.offset, r.start_delta, s.duration, n.duration, false, s.duration, a.n_first,
                                                  a.n_stop);
     const int64_t margin = (pdet.bound >= 0 || pdet.v != 0.f) ? 128 : 0;
-    // (a schedule bound from device memory is always gated)
-    const bool fixed = !n.device_schedule && a.n_first <= 0 && top.n_end >= glq + margin && !(r.fast_ok && r.fast_end < glq);
+    // (a schedule bound from device memory is always gated; a looping source never reaches the end of its buffer, so it plays to the
+    // end of the render unless it stops or has a duration)
+    const bool fixed = n.device_loop ? !n.device_schedule && a.n_first <= 0 && n.stop_time > 1e300 && n.duration > 1e300
+                                     : !n.device_schedule && a.n_first <= 0 && top.n_end >= glq + margin && !(r.fast_ok && r.fast_end < glq);
     out_dynamic(nc, fixed ? Lay::fixed(s.ch) : Lay::gated(s.ch));  // (gated: the kernel writes the layout track)
     a.out = nc.p.out_buf[0];
     StageBuild& sb = stage(nc.L, S_ABSN_BOUND);
@@ -2780,6 +2871,11 @@ bool Planner::absn_bound(NodeCtx& nc, const AbsnPlay& s, const PRef& pdet, const
         sp.duration = s.duration;
         add_sched_patch(sb, n, sp);
     }
+    if (n.device_loop) {
+        const int32_t rec = (int32_t)sb.records() - 1;
+        sb.loop_patches.push_back(StageBuild::LoopPatchRec{gi, n.id, rec, LoopPatch{nullptr, LOOP_BOUND, 0, s.duration}});
+        sb.loop_walks.push_back(StageBuild::LoopWalkRec{rec, loop_cap, lq});
+    }
     const PRef* refs[2] = {&pdet, &prate};
     const size_t offs[2] = {offsetof(AbsnBoundInst, detune), offsetof(AbsnBoundInst, rate)};
     for (int i = 0; i < 2; i++)
@@ -2790,46 +2886,6 @@ bool Planner::absn_bound(NodeCtx& nc, const AbsnPlay& s, const PRef& pdet, const
         }
     algorithmic_bytes += (uint64_t)s.ch * 4ull * (uint64_t)std::min<int64_t>(lq, (int64_t)s.len);
     return true;
-}
-
-// playhead schedule of a looping slow-track source: walk the reference's per-frame bookkeeping (:730-770) from event to event — a
-// frame where buffer_time is snapped to a loop point (almost::equal) or wrapped starts a new segment
-void Planner::absn_schedule(const AbsnSlowInst& a, int64_t n_first, double off, std::vector<int64_t>& seg_n, std::vector<double>& seg_bt) const {
-    const double ls2 = a.loop_start, le2 = a.loop_end, len2 = le2 - ls2, step = a.step;
-    const int64_t n_end = std::min<int64_t>(lq, a.n_stop);
-    int64_t m = 0;   // frames since n_first
-    double v = off;  // buffer_time of frame m
-    bool entered = false;
-    auto tz = [&](double x) { return 3.0e-8 * (1.0 + std::fabs(x)); };  // a little wider than almost::equal
-    while (n_first + m < n_end) {
-        // frames until the playhead can touch the tolerance zone of a loop point
-        double to_ls = v < ls2 - tz(ls2) ? (ls2 - tz(ls2) - v) / step : 0.;
-        double to_le = v < le2 - tz(le2) ? (le2 - tz(le2) - v) / step : 0.;
-        double skip = (!entered && to_ls > 0.) ? std::min(to_ls, to_le) : to_le;
-        int64_t adv = (int64_t)std::floor(skip);
-        if (adv > 0) {
-            v += (double)adv * step;
-            m += adv;
-            continue;
-        }
-        // exact per-frame logic of the reference
-        double w = v;
-        if (almost_equal(w, le2)) w = le2;
-        if (almost_equal(w, ls2)) w = ls2;
-        if (!entered && w >= ls2) entered = true;
-        if (entered) {
-            while (w >= le2) w -= len2;
-            while (w < ls2) w += len2;
-        }
-        if (w != v && n_first + m > seg_n.back()) {
-            seg_n.push_back(n_first + m);
-            seg_bt.push_back(w);
-        } else if (w != v) {
-            seg_bt.back() = w;
-        }
-        v = w + step;
-        m += 1;
-    }
 }
 
 // fast track: the buffer played 1:1 from a block boundary (a chain source when it fuses)
@@ -3980,6 +4036,8 @@ struct GroupPlan {  // result of phase B for one group
     std::vector<PatchEntry<CurvePatch>> curve_patches;
     std::vector<PatchEntry<IirPatch>> iir_patches;
     std::vector<PatchEntry<SchedPatch>> sched_patches;
+    std::vector<PatchEntry<LoopPatch>> loop_patches;
+    std::vector<LoopWalk> loop_walks;
     std::vector<StageBuild::SpatialPatchRec> spatial;  // device addresses set, operands still param ids
 };
 
@@ -4603,6 +4661,13 @@ static void prep_plan_group(wae_batch* b, wae_graph* const* graphs, int k, PrepS
                     p.dst = rec(sp.rec) + sp.off;
                     gp.sched_patches.push_back({sp.graph, sp.node, p});
                 }
+                for (const auto& lp : s.loop_patches) {  // loop points: the record
+                    LoopPatch p = lp.p;
+                    p.dst = rec(lp.rec);
+                    gp.loop_patches.push_back({lp.graph, lp.node, p});
+                }
+                for (const auto& lw : s.loop_walks)
+                    gp.loop_walks.push_back(LoopWalk{reinterpret_cast<AbsnBoundInst*>(rec(lw.rec)), lw.lq, lw.cap, 0});
                 for (StageBuild::SpatialPatchRec sp : s.spatial) {  // static panners: the PanInst or HrtfInst::static_sel they re-derive
                     if (sp.rec >= 0)
                         sp.p.dst = static_cast<char*>(st.d_a) + (size_t)sp.rec * (s.kind == S_PAN ? sizeof(PanInst) : sizeof(HrtfInst)) + sp.off;
@@ -4678,7 +4743,8 @@ static wae_status gather_patches(wae_batch* b, Bindings<D>& t, const std::vector
 // which the caller keeps alive until the stream has been synchronised.
 static wae_status record_declarations(wae_batch* b, wae_graph* const* graphs, uint32_t n_graphs, const std::vector<GroupPlan>& gps,
                                       std::vector<CurvePatch>& curve_patches, std::vector<IirPatch>& iir_patches,
-                                      std::vector<SchedPatch>& sched_patches) {
+                                      std::vector<SchedPatch>& sched_patches, std::vector<LoopPatch>& loop_patches,
+                                      std::vector<LoopWalk>& loop_walks) {
     b->responses.seal(graphs, n_graphs, [](uint32_t j, const NodeMap&, const Node& nd, auto& declare) {
         if (nd.kind == K_CONV && nd.buffer && nd.buffer->device_input)
             declare({j, nd.id, kNodeLevel}, DevResponse{nullptr, (uint32_t)nd.buffer->channels.size(), (uint64_t)nd.buffer->length(), 0,
@@ -4709,16 +4775,28 @@ static wae_status record_declarations(wae_batch* b, wae_graph* const* graphs, ui
         if (nd.kind == K_PARAM && nd.param.device_curve)
             declare({j, nd.param.device_curve_node, nd.param.device_curve_index}, DevValueCurve{nullptr, 0, nd.param.device_curve});
     });
+    b->loops.seal(graphs, n_graphs, [](uint32_t j, const NodeMap&, const Node& nd, auto& declare) {
+        if (nd.kind == K_ABSN && nd.device_loop)
+            declare({j, nd.id, kNodeLevel}, DevLoop{{nd.loop_lo[0], nd.loop_lo[1]}, {nd.loop_hi[0], nd.loop_hi[1]}, 0, 0});
+    });
     wae_status st = gather_patches(b, b->curves, gps, &GroupPlan::curve_patches, curve_patches, &b->d_curve_patches);
     if (st == WAE_OK) st = gather_patches(b, b->iirs, gps, &GroupPlan::iir_patches, iir_patches, &b->d_iir_patches);
     if (st == WAE_OK) st = gather_patches(b, b->schedules, gps, &GroupPlan::sched_patches, sched_patches, &b->d_sched_patches);
+    if (st == WAE_OK) st = gather_patches(b, b->loops, gps, &GroupPlan::loop_patches, loop_patches, &b->d_loop_patches);
+    for (const auto& gp : gps) loop_walks.insert(loop_walks.end(), gp.loop_walks.begin(), gp.loop_walks.end());
+    if (st == WAE_OK && !loop_walks.empty()) {
+        b->n_loop_walks = (int)loop_walks.size();
+        b->d_loop_walks = b->dupload_now(loop_walks);
+        b->d_loop_overflow = b->dalloc<int>(1, true);
+        if (!b->d_loop_walks || !b->d_loop_overflow) st = fail(WAE_OUT_OF_MEMORY, "out of device memory (loop playhead tables)");
+    }
     return st;
 }
 
 // runs of a batch need every declaration they read bound once; the first unbound one is named, kind by kind in this order
 static wae_status check_bound(wae_batch* b) {
     if (!b) return fail(WAE_INVALID_ARGUMENT, "null batch");
-    const BindTable* const kinds[] = {&b->schedules, &b->value_curves, &b->iirs, &b->waves, &b->curves, &b->responses, &b->sources, &b->params};
+    const BindTable* const kinds[] = {&b->loops, &b->schedules, &b->value_curves, &b->iirs, &b->waves, &b->curves, &b->responses, &b->sources, &b->params};
     for (const BindTable* t : kinds)
         for (size_t k = 0; t->unbound && k < t->keys.size(); k++)
             if (!t->bound[k]) {
@@ -4861,11 +4939,13 @@ static wae_status prepare_impl(wae_engine* eng, wae_graph* const* graphs, uint32
     std::vector<CurvePatch> curve_patches;
     std::vector<IirPatch> iir_patches;
     std::vector<SchedPatch> sched_patches;
+    std::vector<LoopPatch> loop_patches;
+    std::vector<LoopWalk> loop_walks;
     std::vector<ParamSlotInfo> slot_info;
     std::vector<ParamPatch> patches;
     std::vector<SpatialPatch> spatial;
     std::vector<RespBindItem> spatial_resp;
-    st = record_declarations(b, graphs, n_graphs, gps, curve_patches, iir_patches, sched_patches);
+    st = record_declarations(b, graphs, n_graphs, gps, curve_patches, iir_patches, sched_patches, loop_patches, loop_walks);
     if (st == WAE_OK) st = record_params(b, graphs, n_graphs, gps, slot_info, patches, spatial, spatial_resp);
     if (st != WAE_OK) {
         wae_batch_destroy(b);
@@ -5326,6 +5406,13 @@ static wae_status stage_bind_table(wae_batch* b, const void* table, size_t bytes
     return WAE_OK;
 }
 
+// The playhead tables of the batch's looping bound slow-track records, from the values the binds have written so far.  Every bind that
+// writes one of their inputs (loop points, params, schedules) ends with it on the engine stream, so every later run reads tables that
+// follow the latest binds, with no work per run and no host synchronisation.
+static void derive_loop_tables(wae_batch* b) {
+    if (b->n_loop_walks > 0) launch_absn_loop_schedule(b->d_loop_walks, b->n_loop_walks, b->d_loop_overflow, b->engine->stream);
+}
+
 extern "C++" {
 template <typename Item>
 static uint32_t param_of(const Item&) { return kNodeLevel; }
@@ -5417,6 +5504,7 @@ WAE_API wae_status wae_batch_bind_params(wae_batch* b, const wae_param_binding* 
             if (b->n_spatial > 0)
                 launch_derive_spatial(b->d_spatial, b->n_spatial, b->d_values, b->d_spatial_resp, b->n_spatial_resp, b->spatial_max_taps,
                                       b->spatial_max_S, b->engine->stream);
+            derive_loop_tables(b);  // (a bound playbackRate / detune moves the loop wraps)
         });
 }
 
@@ -5535,7 +5623,27 @@ WAE_API wae_status wae_batch_bind_schedules(wae_batch* b, const wae_schedule_bin
             }
             return st;
         },
-        [b](const SchedBindItem* dev, const std::vector<SchedBindItem>& rows) { launch_bind_schedules(dev, (int)rows.size(), b->engine->stream); });
+        [b](const SchedBindItem* dev, const std::vector<SchedBindItem>& rows) {
+            launch_bind_schedules(dev, (int)rows.size(), b->engine->stream);
+            derive_loop_tables(b);  // (a bound start, offset, stop or duration moves the loop wraps)
+        });
+}
+
+// The loop points are rewritten on the engine stream: runs queued before the bind have read the previous ones.
+WAE_API wae_status wae_batch_bind_loops(wae_batch* b, const wae_loop_binding* items, uint32_t n, void* stream) {
+    return bind_items<LoopBindItem>(
+        b, &wae_batch::loops, items, n, stream,
+        [b](const wae_loop_binding& it, const DevLoop& d, size_t, BindExtents& extents, auto& rows) -> wae_status {
+            wae_status st = extents.check(it.points, alignof(double), 2 * sizeof(double), "points",
+                                          "[points, points + 2) runs past the end of its allocation");
+            if (st == WAE_OK && d.p0 != d.p1)
+                rows.push_back(LoopBindItem{it.points, b->d_loop_patches + d.p0, {d.lo[0], d.lo[1]}, {d.hi[0], d.hi[1]}, d.p1 - d.p0, 0});
+            return st;
+        },
+        [b](const LoopBindItem* dev, const std::vector<LoopBindItem>& rows) {
+            launch_bind_loops(dev, (int)rows.size(), b->engine->stream);
+            derive_loop_tables(b);
+        });
 }
 
 // The declared values are rewritten on the engine stream: runs queued before the bind have read the previous ones.
@@ -5558,6 +5666,12 @@ WAE_API wae_status wae_batch_bind_value_curves(wae_batch* b, const wae_value_cur
 WAE_API wae_status wae_batch_sync(wae_batch* b) {
     CUDA_TRY(cudaSetDevice(b->engine->device));
     CUDA_TRY(cudaStreamSynchronize(b->engine->stream));
+    if (b->d_loop_overflow) {
+        int overflow = 0;
+        CUDA_TRY(cudaMemcpy(&overflow, b->d_loop_overflow, sizeof overflow, cudaMemcpyDeviceToHost));
+        if (overflow)
+            return fail(WAE_CUDA_ERROR, "a loop playhead table derived on the device needed more segments than were planned for it (a defect)");
+    }
     float ms = 0.f;
     if (cudaEventElapsedTime(&ms, b->ev0, b->ev1) == cudaSuccess) b->stats.last_run_ms = ms;
     else cudaGetLastError();

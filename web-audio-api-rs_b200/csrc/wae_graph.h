@@ -159,6 +159,10 @@ struct Node {
     double sched_lo[4] = {0., 0., 0., 0.}, sched_hi[4] = {0., 0., 0., 0.};
     bool loop = false;
     double loop_start = 0., loop_end = 0.;
+    // wae_buffer_source_set_device_loop: loop_start / loop_end are written per run by wae_batch_bind_loops, clamped to [loop_lo, loop_hi]
+    // (index 0: start, 1: end); loop_start / loop_end hold the windows' low ends, which the plan is made with
+    bool device_loop = false;
+    double loop_lo[2] = {0., 0.}, loop_hi[2] = {0., 0.};
     double max_delay_time = 1.;
     uint32_t delay_peer = 0;  // writer <-> reader
     // panner
@@ -284,6 +288,7 @@ struct wae_graph {
     uint32_t device_iirs = 0;       // IIRFilterNodes declared with wae_iir_filter_set_device_coefficients
     uint32_t device_value_curves = 0;  // AudioParams declared with wae_param_set_device_value_curve
     uint32_t device_schedules = 0;     // scheduled sources declared with wae_source_set_device_schedule
+    uint32_t device_loops = 0;         // AudioBufferSourceNodes declared with wae_buffer_source_set_device_loop
 
     uint32_t create_param(uint32_t owner, float def, float mn, float mx, bool a_rate, float initial, bool send_set_value = true,
                           bool fixed_id = false, uint32_t id = 0, bool constrained = false);

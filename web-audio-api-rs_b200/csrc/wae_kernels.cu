@@ -262,16 +262,18 @@ DEVI void absn_bound_tiles(const AbsnBoundInst& r, int n0, const ChunkInfo& ci) 
     if (threadIdx.x == 0) {
         AbsnSlowInst o = r.s;
         const double computed_rate = (double)r.rate * exp2((double)r.detune / 1200.);
-        const AbsnSlowDerived d = absn_slow_derive(r.dt, computed_rate, r.offset, r.start_delta, o.buffer_duration, o.duration, false, o.loop_end,
-                                                   o.n_first, o.n_stop);
+        const AbsnSlowDerived d = absn_slow_derive(r.dt, computed_rate, r.offset, r.start_delta, o.buffer_duration, o.duration, o.loop != 0,
+                                                   o.loop_end, o.n_first, o.n_stop);
         o.step = d.step;
         o.offset0 = d.offset0;
         o.elapsed0 = d.elapsed0;
-        o.n_seg = 1;
-        o.seg_n = &s_seg_n;
-        o.seg_bt = &s_seg_bt;
-        s_seg_n = o.n_first;
-        s_seg_bt = d.offset0;
+        if (!o.loop) {  // (a looping record reads the table k_absn_loop_schedule derived from the same values)
+            o.n_seg = 1;
+            o.seg_n = &s_seg_n;
+            o.seg_bt = &s_seg_bt;
+            s_seg_n = o.n_first;
+            s_seg_bt = d.offset0;
+        }
         const bool fast = r.fast_ok && computed_rate == 1.;
         s_fast = fast;
         s_first = fast ? r.n_start : o.n_first;
@@ -4677,6 +4679,54 @@ __global__ void __launch_bounds__(128) k_bind_schedules(const SchedBindItem* __r
     }
 }
 
+// ---- wae_batch_bind_loops: one thread per item -----------------------------------------------------------------------------------------
+// The loop points are clamped to their windows, then clamp_loop_boundaries and the actual-loop-points rule are applied with the planner's
+// function (absn_loop_points).  A bound slow-track record takes the actual loop points; its table is derived by k_absn_loop_schedule,
+// launched right after this kernel.
+__global__ void __launch_bounds__(128) k_bind_loops(const LoopBindItem* __restrict__ items, int n_items) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n_items) return;
+    const LoopBindItem it = items[i];
+    const double ls = sched_clamp(it.points[0], it.lo[0], it.hi[0]);
+    const double le = sched_clamp(it.points[1], it.lo[1], it.hi[1]);
+    for (int k = 0; k < it.n_patches; k++) {
+        const LoopPatch p = it.patches[k];
+        const AbsnLoopPoints lp = absn_loop_points(ls, le, p.buffer_duration);
+        if (p.kind == LOOP_BOUND) {
+            AbsnBoundInst* r = static_cast<AbsnBoundInst*>(p.dst);
+            r->s.loop_start = lp.actual_start;
+            r->s.loop_end = lp.actual_end;
+        } else {
+            AbsnSerialInst* r = static_cast<AbsnSerialInst*>(p.dst);
+            r->loop_start = lp.start;
+            r->loop_end = lp.end;
+        }
+    }
+}
+
+// ---- The playhead tables of looping bound slow-track records: one thread per record.  step / offset0 from the record's (bound or
+// planned) rate, detune, start, offset and duration exactly as absn_bound_tiles derives them, then the planner's walk
+// (absn_loop_segments) into the record's table.  A walk that needs more than the planned capacity is a planner defect: the table keeps
+// its first `cap` segments and *overflow is set, which wae_batch_sync reports.
+__global__ void __launch_bounds__(128) k_absn_loop_schedule(const LoopWalk* __restrict__ walks, int n, int* overflow) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const LoopWalk w = walks[i];
+    AbsnBoundInst& r = *w.rec;
+    const AbsnSlowInst& o = r.s;
+    const double computed_rate = (double)r.rate * exp2((double)r.detune / 1200.);
+    const AbsnSlowDerived d = absn_slow_derive(r.dt, computed_rate, r.offset, r.start_delta, o.buffer_duration, o.duration, true, o.loop_end,
+                                               o.n_first, o.n_stop);
+    const int64_t n_end = o.n_stop < w.lq ? o.n_stop : w.lq;
+    int32_t k = absn_loop_segments(o.loop_start, o.loop_end, d.step, o.n_first, n_end, d.offset0, const_cast<int64_t*>(o.seg_n),
+                                   const_cast<double*>(o.seg_bt), w.cap);
+    if (k < 0) {
+        atomicExch(overflow, 1);
+        k = w.cap;
+    }
+    r.s.n_seg = k;
+}
+
 // Host emulation of the transforms above with the SAME butterfly, index and twiddle code (tests/test_conv_fft_host.py pins them against
 // numpy on a machine without a GPU).  mode 0: complex forward, natural -> position order; 1: complex inverse, position -> natural order
 // (unnormalised); 2: 2B reals -> B packed bins in position order; 3: B packed bins -> 2B reals (scaled by 1 / 2B).  data: 2B floats in place.
@@ -5293,6 +5343,10 @@ void launch_bind_value_curves(const ValueCurveBindItem* d, int n, int64_t max_le
     k_bind_value_curves<<<dim3((unsigned)bx, (unsigned)std::min(n, 65535)), 256, 0, s>>>(d, n);
 }
 void launch_bind_schedules(const SchedBindItem* d, int n, cudaStream_t s) { k_bind_schedules<<<(unsigned)((n + 127) / 128), 128, 0, s>>>(d, n); }
+void launch_bind_loops(const LoopBindItem* d, int n, cudaStream_t s) { k_bind_loops<<<(unsigned)((n + 127) / 128), 128, 0, s>>>(d, n); }
+void launch_absn_loop_schedule(const LoopWalk* d, int n, int* overflow, cudaStream_t s) {
+    k_absn_loop_schedule<<<(unsigned)((n + 127) / 128), 128, 0, s>>>(d, n, overflow);
+}
 void launch_conv_ir_fft(const float* ir, int64_t ir_len, int64_t ir_stride, float2* h, int S, int channels, cudaStream_t s) {
     conv_configure();
     k_conv_ir_fft<<<dim3((unsigned)S, (unsigned)channels), CV_THREADS, CV_SMEM_ELEMS * sizeof(float2), s>>>(ir, ir_len, ir_stride, h, S);

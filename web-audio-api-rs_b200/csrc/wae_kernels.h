@@ -232,6 +232,75 @@ WAE_HD int64_t absn_fast_end(const SchedClock& clock, int64_t lq, int64_t n_star
     return n_start + played * 128;
 }
 
+// The loop points a looping slow-track source plays (audio_buffer_source.rs:400-417 clamp_loop_boundaries, then the actual loop points
+// of :627-636): one source for the planner (host, loop points bound from device memory: the placeholders) and for k_bind_loops (device).
+struct AbsnLoopPoints {
+    double start, end;        // after clamp_loop_boundaries (AbsnSerialInst)
+    double actual_start, actual_end;  // the loop the slow track plays (AbsnSlowInst)
+};
+WAE_HD AbsnLoopPoints absn_loop_points(double loop_start, double loop_end, double buffer_duration) {
+    AbsnLoopPoints p;
+    p.start = loop_start < 0. ? 0. : (loop_start > buffer_duration ? buffer_duration : loop_start);
+    p.end = (loop_end <= 0. || loop_end > buffer_duration) ? buffer_duration : loop_end;
+    const bool custom = p.start >= 0. && p.end > 0. && p.start < p.end;
+    p.actual_start = custom ? p.start : 0.;
+    p.actual_end = custom ? p.end : buffer_duration;
+    return p;
+}
+
+// The playhead schedule of a looping slow-track source (AbsnSlowInst::seg_n / seg_bt): the reference's per-frame loop bookkeeping
+// (audio_buffer_source.rs:730-770) walked from event to event — a frame where buffer_time is snapped to a loop point (almost::equal) or
+// wrapped starts a new segment.  One source for the planner (host-built loop points) and for k_absn_loop_schedule (loop points bound from
+// device memory); the build compiles without FMA contraction on both sides, so equal inputs give bit-equal tables.  ls2 / le2: the actual
+// loop points; off: buffer_time at n_first (absn_slow_derive's offset0); frames [n_first, n_end) are walked.  Writes at most `cap` (>= 1)
+// segments and returns their number, or -1 when the walk needs more than `cap` (the first `cap` are written and valid).  A source that
+// starts at or past the loop end never enters the loop (:700-707): one segment.
+WAE_HD int32_t absn_loop_segments(double ls2, double le2, double step, int64_t n_first, int64_t n_end, double off, int64_t* seg_n,
+                                  double* seg_bt, int32_t cap) {
+    seg_n[0] = n_first;
+    seg_bt[0] = off;
+    int32_t k = 1;
+    if (!(off < le2)) return k;
+    const double len2 = le2 - ls2;
+    int64_t m = 0;   // frames since n_first
+    double v = off;  // buffer_time of frame m
+    bool entered = false;
+    auto tz = [](double x) { return 3.0e-8 * (1.0 + fabs(x)); };  // a little wider than almost::equal
+    while (n_first + m < n_end) {
+        // frames until the playhead can touch the tolerance zone of a loop point
+        const double to_ls = v < ls2 - tz(ls2) ? (ls2 - tz(ls2) - v) / step : 0.;
+        const double to_le = v < le2 - tz(le2) ? (le2 - tz(le2) - v) / step : 0.;
+        // (until the loop is entered, the loop start's zone is walked frame by frame too: a frame that lands in it is snapped to it)
+        const double skip = !entered ? (to_le < to_ls ? to_le : to_ls) : to_le;
+        const int64_t adv = (int64_t)floor(skip);
+        if (adv > 0) {
+            v += (double)adv * step;
+            m += adv;
+            continue;
+        }
+        // exact per-frame logic of the reference
+        double w = v;
+        if (almost_equal(w, le2)) w = le2;
+        if (almost_equal(w, ls2)) w = ls2;
+        if (!entered && w >= ls2) entered = true;
+        if (entered) {
+            while (w >= le2) w -= len2;
+            while (w < ls2) w += len2;
+        }
+        if (w != v && n_first + m > seg_n[k - 1]) {
+            if (k == cap) return -1;
+            seg_n[k] = n_first + m;
+            seg_bt[k] = w;
+            k++;
+        } else if (w != v) {
+            seg_bt[k - 1] = w;
+        }
+        v = w + step;
+        m += 1;
+    }
+    return k;
+}
+
 void upload_twiddles();                         // convolver FFT tables (computed in wae_kernels.cu, f64 -> f32)
 void conv_fft_selftest(float* data, int mode);   // host emulation of the convolver transforms (wae_selftest_conv_fft)
 void launch_oscillator(const OscInst* d, int n, ChunkInfo ci, cudaStream_t s);
@@ -299,6 +368,11 @@ void launch_bind_value_curves(const ValueCurveBindItem* d, int n, int64_t max_le
 // a bind of n schedules (start, [stop], [offset], [duration]; k_bind_schedules, one thread per item): clamped, then every patch entry of
 // each item re-derived
 void launch_bind_schedules(const SchedBindItem* d, int n, cudaStream_t s);
+// a bind of n loop-point pairs (k_bind_loops, one thread per item): clamped, then every patch entry of each item written
+void launch_bind_loops(const LoopBindItem* d, int n, cudaStream_t s);
+// the playhead tables of the n looping bound slow-track records of a batch (k_absn_loop_schedule, one thread per record); *overflow is
+// set when a walk needs more segments than its table holds
+void launch_absn_loop_schedule(const LoopWalk* d, int n, int* overflow, cudaStream_t s);
 void launch_conv_ir_fft(const float* ir, int64_t ir_len, int64_t ir_stride, float2* h, int S, int channels, cudaStream_t s);
 
 }  // namespace wae
