@@ -810,6 +810,24 @@ typedef struct wae_loop_binding {
  * playhead table derived on the device ever needed more segments than were planned for it (a defect: the render is wrong). */
 WAE_API wae_status wae_batch_bind_loops(wae_batch* batch, const wae_loop_binding* items, uint32_t n, void* stream);
 
+/* ---- Rendered PCM written to caller device memory ---------------------------------------------------------------------------------
+ * Points the rendered PCM of later runs at caller device memory instead of the batch's own buffer.  `out` takes the layout of that buffer:
+ * packed, graph j at the offset wae_batch_graph_output reports, [channels_j][length_j] f32; `floats` must be the out_floats of
+ * wae_batch_output_device_ptr.  The call is ordered after the work already queued on `stream` (as wae_batch_bind_sources) and rewrites the
+ * batch's output pointers on the engine stream; later wae_batch_run / wae_batch_run_group write `out`, every float of it (a graph whose
+ * destination has no input, or whose destination is muted in a cycle, renders zeros there, as in the batch's own buffer).  A null `out`
+ * with floats == 0 returns the batch to its own buffer, which a run into `out` leaves untouched.  The binding stays until it is changed.
+ * Runs are asynchronous on the engine stream (wae_engine_stream) and never wait for another stream by themselves, as for the batch's own
+ * buffer: a reader of `out` on another stream waits for the engine stream after the run, and a run into memory whose last render is still
+ * being read is ordered after that reader by the caller (binding again orders it after `stream`).  While it holds,
+ * wae_batch_output_device_ptr reports `out` and wae_batch_fetch / wae_batch_fetch_graph read it.  WAE_INVALID_ARGUMENT, with nothing
+ * changed: `out` is not 256-byte aligned (as cudaMalloc aligns the batch's own buffer; a torch allocation is, and so is a slice of it at
+ * a multiple of 64 floats), not device (or managed) memory of the engine's GPU or [out, out + floats) does not lie in one allocation,
+ * `floats` is not the batch's out_floats, or a null `out` comes with floats != 0.  WAE_INVALID_STATE: a graph of the batch connects its
+ * destination to another node (that node reads the batch's own buffer).  wae_batch_run_pipelined, which streams the batch's own buffer
+ * to host memory, answers WAE_INVALID_STATE while an output is bound.  wae_render_batch and wae_render_many are not affected. */
+WAE_API wae_status wae_batch_bind_output(wae_batch* batch, float* out, uint64_t floats, void* stream);
+
 /* PeriodicWave::new(context, PeriodicWaveOptions { real, imag, disable_normalization }) (src/periodic_wave.rs:104-209): fills `table`
  * (PERIODIC_WAVE_TABLE_LENGTH = 8192 in the reference) with the wavetable an OscillatorNode of type Custom plays.  `real` / `imag` may be
  * NULL (= zeros); both NULL = the sine default.  Host math, no engine needed. */

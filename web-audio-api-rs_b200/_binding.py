@@ -213,6 +213,7 @@ WAE_SYMBOLS = [
     "wae_param_set_device_value_curve", "wae_batch_bind_value_curves",
     "wae_source_set_device_schedule", "wae_batch_bind_schedules", "wae_buffer_source_set_device_offset",
     "wae_buffer_source_set_device_loop", "wae_batch_bind_loops",
+    "wae_batch_bind_output",
 ]
 
 
@@ -341,6 +342,8 @@ class Api:
             # loop points bound from device memory
             f("buffer_source_set_device_loop", C.c_int32, [gp, C.c_uint32, C.c_double, C.c_double, C.c_double, C.c_double])
             f("batch_bind_loops", C.c_int32, [C.c_void_p, C.POINTER(LoopBinding), C.c_uint32, C.c_void_p])
+            # rendered PCM written to caller device memory
+            f("batch_bind_output", C.c_int32, [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p])
         else:
             f("graph_create", C.c_int32, [C.c_uint32, C.c_uint64, C.c_float, C.POINTER(C.c_void_p)])
             f("render", C.c_int32, [gp, c_float_p])

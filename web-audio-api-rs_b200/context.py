@@ -780,7 +780,9 @@ class Batch:
         self.api.check(prepare(ctx0._backend.engine, arr, self.n, C.byref(h)))
         self.handle = h
         self._guard = None  # bind_sources: torch stream the bound tensors are recorded on
-        self._views_out = False  # output_tensor was called: runs are ordered after torch's current stream
+        self._views_out = False  # output_tensor was called: runs into the batch's own buffer are ordered after torch's current stream
+        self._out = None  # bind_output: the tensor runs write
+        self._out_viewed = False  # output_tensor handed out views of the bound tensor since it was bound: runs into it wait for torch
         self._backend = ctx0._backend
         self._backend.batches.add(self)
         for i, c in enumerate(contexts):
@@ -789,6 +791,7 @@ class Batch:
     def run(self):
         self._after_torch_readers()
         self.api.check(self.api.batch_run(self.handle))
+        self._out_written()
 
     def upload(self):
         self.api.check(self.api.batch_upload(self.handle))
@@ -814,6 +817,7 @@ class Batch:
         """render of ONE graph group, asynchronous on the engine stream (call the groups in order)"""
         self._after_torch_readers()
         self.api.check(self.api.batch_run_group(self.handle, k))
+        self._out_written()
 
     def run_pipelined(self, host_out_ptr):
         """H2D + render + D2H, overlapped per graph group; `host_out_ptr` = address of [n][ch][length] f32 (pinned)."""
@@ -863,9 +867,11 @@ class Batch:
         return torch.cuda.current_stream(self._device()).cuda_stream or 1  # 1 = cudaStreamLegacy
 
     def _after_torch_readers(self):
-        """A run overwrites the device output: once output_tensor views were handed out, order it after the work torch has queued so far
-        on its current stream (the readers of the last output)."""
-        if self._views_out:
+        """A run overwrites the device output: once output_tensor views of the buffer it writes were handed out, order it after the work
+        torch has queued so far on its current stream (the readers of the last output).  Views of another buffer do not hold a run into a
+        bound output up: bind_output ordered it after the work queued before the bind, and the readers of the other buffer may run while it
+        renders."""
+        if (self._views_out and self._out is None) or (self._out_viewed and self._out is not None):
             import torch
             self._engine_stream().wait_stream(torch.cuda.current_stream(self._device()))
 
@@ -1157,15 +1163,54 @@ class Batch:
                 items[i * k + j] = B.ParamBinding(g, node, int(prm._index), ptr)
         self._bind(self.api.batch_bind_params, items, n * k, values)
 
+    def bind_output(self, out):
+        """wae_batch_bind_output: later runs write the rendered PCM into `out`, a contiguous float32 CUDA tensor on the engine's device,
+        [n][channels][length] for a batch of one shape, else 1-D of the batch's output floats in the layout output_tensor(i) addresses.  The
+        call is ordered after torch's current stream; the tensor is kept while it is bound, and from reuse until the runs into it are done.
+        None: back to the batch's own buffer."""
+        import torch
+        if out is None:
+            self.api.check(self.api.batch_bind_output(self.handle, None, 0, C.c_void_p(self._torch_stream_handle())))
+            self._out, self._out_viewed = None, False
+            return
+        p, floats = C.c_void_p(), C.c_uint64()
+        self.api.check(self.api.batch_output_device_ptr(self.handle, C.byref(p), C.byref(floats)))
+        shape = (self.n, self.channels, self.length) if self._one_shape() else (floats.value,)
+        if not (isinstance(out, torch.Tensor) and out.is_cuda and out.dtype == torch.float32):
+            raise B.WaeError(1, "bind_output: out must be a float32 CUDA tensor")
+        if out.device != self._device():
+            raise B.WaeError(1, f"bind_output: out is on {out.device}, the batch renders on {self._device()}")
+        if tuple(out.shape) != shape or not out.is_contiguous():
+            raise B.WaeError(1, f"bind_output: out must be a contiguous tensor of shape {list(shape)}, not {list(out.shape)}")
+        self.api.check(self.api.batch_bind_output(self.handle, C.c_void_p(out.data_ptr()), floats.value,
+                                                  C.c_void_p(self._torch_stream_handle())))
+        self._out, self._out_viewed = out, False
+
+    def _out_written(self):
+        if self._out is not None:
+            self._keep_until_read(self._out)
+
+    def _one_shape(self):
+        return len({(c._channels, c._length) for c in self.contexts}) == 1
+
     def output_tensor(self, i=None):
         """Zero-copy torch view of the rendered output on the device: [n][channels][length] for a batch of one shape, [channels_i][length_i]
-        of context i.  The view keeps the batch alive; torch's current stream is made to wait for the engine stream first, and later
-        runs of the batch (which overwrite the view) wait for the work then queued on torch's current stream."""
+        of context i; while an output is bound (bind_output), views of that tensor.  The view keeps the batch alive; torch's current stream
+        is made to wait for the engine stream first (read a bound tensor through this call: it orders the read after the run), and later
+        runs of the batch into the same memory (which overwrite the view) wait for the work then queued on torch's current stream."""
         import torch
+        if self._out is not None:
+            self._out_viewed = True
+            torch.cuda.current_stream(self._device()).wait_stream(self._engine_stream())
+            if i is None:
+                if not self._one_shape():
+                    raise B.WaeError(2, "output_tensor: the contexts of this batch differ in shape; view one with output_tensor(i)")
+                return self._out
+            off, ch, length = self.graph_output(i)
+            return self._out.view(-1)[off:off + ch * length].view(ch, length)
         base, _ = self.device_ptr()
         if i is None:
-            shapes = {(c._channels, c._length) for c in self.contexts}
-            if len(shapes) != 1:
+            if not self._one_shape():
                 raise B.WaeError(2, "output_tensor: the contexts of this batch differ in shape; view one with output_tensor(i)")
             off, shape = 0, (self.n, self.channels, self.length)
         else:

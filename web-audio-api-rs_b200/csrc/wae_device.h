@@ -729,4 +729,11 @@ struct SpatialPatch {
     float val[15];
 };
 
+// An output entry: one planned record field that points into the batch's rendered PCM (the BufRef::p of a destination writer: k_mix,
+// k_mix_dyn, k_chain, k_voice_sum, k_conv_mac_ifft).  wae_batch_bind_output writes base + off into it (k_bind_output).
+struct OutPatch {
+    float** dst;
+    uint64_t off;  // floats from the start of the packed output
+};
+
 }  // namespace wae

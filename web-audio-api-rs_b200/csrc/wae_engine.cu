@@ -370,6 +370,36 @@ struct StageBuild {
     };
     std::vector<SpatialPatchRec> spatial;
     size_t spatial_records() const { return kind == S_PAN ? pan.size() : kind == S_HRTF ? hrtf.size() : 0; }
+    // Output entries (wae_batch_bind_output): the BufRef `off` bytes into record `rec` of this stage's destination-writer table (see
+    // out_records) is the rendered PCM of graph `graph`, `dest` floats into the packed output
+    struct OutPatchRec {
+        uint64_t dest;
+        int32_t rec;
+        uint32_t off;
+        uint32_t graph;  // batch position
+        uint32_t pad;
+    };
+    std::vector<OutPatchRec> out_patches;
+    size_t out_records() const {
+        switch (kind) {
+            case S_MIX: return mix.size();
+            case S_MIX_DYN: return mix_dyn.size();
+            case S_CHAIN: return chain.size();
+            case S_VSUM: return vgroups.size();
+            case S_CONV_MAC: case S_CONV_MAC_ACC: return conv_path.size();
+            default: return 0;
+        }
+    }
+    size_t out_record_bytes() const {
+        switch (kind) {
+            case S_MIX: return sizeof(MixInst);
+            case S_MIX_DYN: return sizeof(MixDynInst);
+            case S_CHAIN: return sizeof(ChainInst);
+            case S_VSUM: return sizeof(VoiceGroup);
+            case S_CONV_MAC: case S_CONV_MAC_ACC: return sizeof(ConvPath);
+            default: return 0;
+        }
+    }
     // size of the table patch entries point into (S_HRTF: the selection records of its moving panners, the stage's second table)
     size_t records() const {
         switch (kind) {
@@ -630,6 +660,7 @@ struct wae_batch {
         size_t stage0 = 0, stage1 = 0;  // stages [stage0, stage1) of `stages` (all segments)
         std::vector<std::pair<size_t, size_t>> seg_stages;  // per render segment: its stages
         std::vector<int64_t> seg_bounds;                    // 0 = b0 < b1 < ... < lq: the suspend frames of this group's graphs
+        std::vector<std::pair<size_t, size_t>> out_zero;    // (offset, floats) of the output no stage writes: zeroed when it is bound
         float* d_src = nullptr;         // device slab of source PCM
         float* h_src = nullptr;         // pinned host mirror, built on first use (wae_batch_upload / wae_batch_run_pipelined)
         struct SrcCopy {                // the PCM of one AudioBufferSourceNode inside the slab: planar [ch][stride], as PcmBuffer holds it
@@ -693,6 +724,13 @@ struct wae_batch {
     int n_loop_walks = 0;
     int* d_loop_overflow = nullptr;
     cudaEvent_t ev_bind = nullptr;  // orders a bind after the caller's stream
+    // wae_batch_bind_output: the output entries of every group and the caller's memory the runs write instead of d_out (nullptr: d_out).
+    // dest_reader: a graph (batch position) whose destination feeds another node, -1: none; its output cannot be bound.
+    OutPatch* d_out_patches = nullptr;
+    int n_out_patches = 0;
+    float* bound_out = nullptr;
+    int64_t dest_reader = -1;
+    float* out_ptr() const { return bound_out ? bound_out : d_out; }
     // OfflineAudioContext::suspend_sync: a group's render is cut at the suspend frames of its graphs (graphs with different
     // suspend points are put in different groups); every segment has its own plan, node state is shared between the plans
     // through `state_map` (graph, node, allocation sequence, salt)
@@ -1166,6 +1204,13 @@ struct Planner {
     int64_t lq = 0, glq = 0;
     // the graph's rendered PCM in the packed output: [channels][length], frames from `length` on are not written (limit)
     BufRef dest_ref() const { return BufRef{b->d_out + b->out_off[gi], (uint32_t)g->length, 1}; }
+    // the output entry of the last record of `s`'s destination-writer table, whose BufRef `off` bytes into it is dest_ref()
+    void add_out(StageBuild& s, size_t off) const {
+        s.out_patches.push_back(StageBuild::OutPatchRec{(uint64_t)b->out_off[gi], (int32_t)s.out_records() - 1, (uint32_t)off, gi, 0});
+    }
+    // a graph planned so far feeds its destination's output to another node, which reads the rendered PCM through a record the output
+    // entries do not cover: batch position, -1: none
+    int64_t dest_reader = -1;
     void begin_segment(int64_t f0, int64_t f1) {
         seg_start = f0;
         seg_end = f1;
@@ -1390,7 +1435,7 @@ struct Planner {
             if (e.other_index >= 0) k++;
         return k;
     }
-    void emit_chain(PendingChain& pc, int L);
+    StageBuild& emit_chain(PendingChain& pc, int L);  // (returns the stage the chain's record went to)
     bool materialize(uint32_t nid, bool may_alias = false);
     // can a node of this kind still be appended to the canonical chain gain, A, gain, B, gain, shaper, gain?
     static bool chain_accepts(const PendingChain& pc, Kind kind) {
@@ -1636,6 +1681,12 @@ static uint64_t digest_vec_skipping(const std::vector<T>& v, std::initializer_li
 template <typename T>
 static uint64_t digest_vec_without_end(const std::vector<T>& v, uint64_t h) { return digest_vec_skipping(v, {offsetof(T, end)}, h); }
 
+// (the output entries are not part of any record: the split sizing's self-check compares them on their own)
+static uint64_t digest_out_patches(const std::map<std::pair<int, int>, StageBuild>& builds) {
+    uint64_t h = 1469598103934665603ull;
+    for (auto& kv : builds) h = digest_vec(kv.second.out_patches, h);
+    return h;
+}
 static uint64_t digest_builds(const std::map<std::pair<int, int>, StageBuild>& builds, uint64_t h) {
     for (auto& kv : builds) {
         const StageBuild& s = kv.second;
@@ -1667,14 +1718,14 @@ static void append_vec(std::vector<T>& d, std::vector<T>& s) {
 }
 static void merge_builds(Builds& dst, Builds& src) {
     struct Base {
-        size_t mix_edges = 0, scan = 0, chain = 0, conv_in = 0, records = 0, spatial = 0;
+        size_t mix_edges = 0, scan = 0, chain = 0, conv_in = 0, records = 0, spatial = 0, out = 0;
     };
     std::map<std::pair<int, int>, Base> base;  // table sizes of `dst` before anything of `src` is appended
     for (auto& kv : src) {
         auto it = dst.find(kv.first);
         if (it != dst.end())
             base[kv.first] = Base{it->second.mix_edges.size(), it->second.n_scan_coef, it->second.chain.size(), it->second.conv_in.size(),
-                                  it->second.records(), it->second.spatial_records()};
+                                  it->second.records(), it->second.spatial_records(), it->second.out_records()};
         else base[kv.first] = Base{};
     }
     for (auto& kv : src) {
@@ -1690,6 +1741,7 @@ static void merge_builds(Builds& dst, Builds& src) {
         for (auto& lw : s.loop_walks) lw.rec += (int32_t)bs.records;
         for (auto& sp : s.spatial)
             if (sp.rec >= 0) sp.rec += (int32_t)bs.spatial;
+        for (auto& op : s.out_patches) op.rec += (int32_t)bs.out;
         for (auto& ip : s.iir_patches) {
             ip.rec += (int32_t)bs.records;
             if (ip.scan >= 0) ip.scan += (int32_t)bs.scan;
@@ -1729,6 +1781,7 @@ static void merge_builds(Builds& dst, Builds& src) {
         append_vec(d.loop_patches, s.loop_patches);
         append_vec(d.loop_walks, s.loop_walks);
         append_vec(d.spatial, s.spatial);
+        append_vec(d.out_patches, s.out_patches);
         d.n_scan_coef += s.n_scan_coef;
         d.max_ch = std::max(d.max_ch, s.max_ch);
     }
@@ -1916,7 +1969,9 @@ bool Planner::plan_convolver(PNode& pn, int level, const BufRef* dest, int64_t d
             if (!p.y) return bail(WAE_OUT_OF_MEMORY, "out of device memory (convolver output spectra)");
             b->arena_bytes += (size_t)blocks_per_chunk * WAE_CONV_SPEC * 8;
         }
-        stage(level, r.acc ? S_CONV_MAC_ACC : S_CONV_MAC).conv_path.push_back(p);
+        StageBuild& cs = stage(level, r.acc ? S_CONV_MAC_ACC : S_CONV_MAC);
+        cs.conv_path.push_back(p);
+        if (direct) add_out(cs, offsetof(ConvPath, out));
     }
     if (compact) {
         role(16);  // (16 .. 22, in this order)
@@ -2110,7 +2165,7 @@ Planner::PRef Planner::param_ref(uint32_t pid) {
 }
 
 // ---- chain fusion ---------------------------------------------------------------------------------------------------------
-void Planner::emit_chain(PendingChain& pc, int L) {
+StageBuild& Planner::emit_chain(PendingChain& pc, int L) {
     const int variant = pc.inst.src_kind * 6 + pc.inst.n_biquad * 2 + (pc.inst.has_shaper ? 1 : 0);
     const int consumer_cls = cur_cls;  // a chain is emitted while its consumer is planned, but runs with its own nodes' class
     cur_cls = pc.cls;
@@ -2122,6 +2177,7 @@ void Planner::emit_chain(PendingChain& pc, int L) {
     cs.max_ch = std::max(cs.max_ch, pc.ch);
     chain_patches(cs, pc, (int32_t)cs.chain.size());
     cs.chain.push_back(pc.inst);
+    return cs;
 }
 
 // may_alias: the consumer reads its input through chan() with any alignment (the convolver's forward transform): a pending chain that
@@ -2184,6 +2240,7 @@ bool Planner::mix(int level, const std::vector<PortRef>& edges, int ch, const Ch
         m.edge_offset = edge_offset;
         m.limit = limit;
         ms.mix_dyn.push_back(m);
+        if (to_dest) add_out(ms, offsetof(MixDynInst, out));
     } else {
         MixInst m{};
         m.out = out;
@@ -2193,6 +2250,7 @@ bool Planner::mix(int level, const std::vector<PortRef>& edges, int ch, const Ch
         m.edge_offset = edge_offset;
         m.limit = limit;
         ms.mix.push_back(m);
+        if (to_dest) add_out(ms, offsetof(MixInst, out));
     }
     return true;
 }
@@ -2436,6 +2494,7 @@ bool Planner::sum_voices(NodeCtx& nc, int port, int ch, int nb) {
         vs.chain.push_back(pc.inst);
     }
     vs.vgroups.push_back(vg);
+    if (nc.n.kind == K_DEST) add_out(vs, offsetof(VoiceGroup, out));
     nc.p.in_buf[port] = vg.out;
     return true;
 }
@@ -2451,11 +2510,14 @@ bool Planner::lower_dest(NodeCtx& nc) {
         pc.inst.out = fin;
         pc.inst.limit = (int64_t)g->length;
         pc.inst.out_dup = (pc.ch == 1 && g->channels == 2) ? 2 : 0;
-        emit_chain(pc, nc.L);
+        add_out(emit_chain(pc, nc.L), offsetof(ChainInst, out));
         node_table.at(nc.fuse_src).out_buf = {fin};
         p.in_buf[0] = fin;
     }
     p.out_buf = {p.in_buf[0]};
+    if (const std::vector<Edge>* outs = ord.edges.find(nc.id))
+        for (auto& e : *outs)
+            if (e.other_index >= 0 && dest_reader < 0) dest_reader = gi;
     algorithmic_bytes += (uint64_t)g->channels * g->length * 4;  // destination write, SURVEY §8(d)
     return true;
 }
@@ -4039,6 +4101,9 @@ struct GroupPlan {  // result of phase B for one group
     std::vector<PatchEntry<LoopPatch>> loop_patches;
     std::vector<LoopWalk> loop_walks;
     std::vector<StageBuild::SpatialPatchRec> spatial;  // device addresses set, operands still param ids
+    std::vector<OutPatch> out_patches;                 // device addresses set
+    std::vector<std::pair<size_t, size_t>> out_zero;   // (offset, floats) of the output no stage writes
+    int64_t dest_reader = -1;                          // see Planner::dest_reader
 };
 
 static int64_t padded_length(const wae_graph* g) { return (int64_t)((g->length + 127) / 128 * 128); }
@@ -4300,7 +4365,7 @@ static wae_status prep_begin(wae_engine* eng, wae_graph* const* graphs, uint32_t
             b->groups[k].graph_src_base.clear();
             Planner sizing(b, b->groups[k], ps, &b->groups[k].src_copies);
             const std::vector<int64_t>& bounds = b->groups[k].seg_bounds;
-            uint64_t serial_digest = 0;
+            uint64_t serial_digest = 0, serial_out_digest = 0;
             for (size_t sg = 0; sg + 1 < bounds.size(); sg++) {
                 sizing.begin_segment(bounds[sg], bounds[sg + 1]);
                 for (uint32_t i = b->groups[k].g0; i < b->groups[k].g1; i++) {
@@ -4318,7 +4383,10 @@ static wae_status prep_begin(wae_engine* eng, wae_graph* const* graphs, uint32_t
                     for (auto& kv : sizing.builds) kinds.push_back(kv.second.kind);
                     so[k].stage_lists.push_back(std::move(kinds));
                     if (plan_digest_wanted()) so[k].digest = digest_builds(sizing.builds, so[k].digest);
-                    if (check_split && one_segment) serial_digest = digest_builds(sizing.builds, 1469598103934665603ull);
+                    if (check_split && one_segment) {
+                        serial_digest = digest_builds(sizing.builds, 1469598103934665603ull);
+                        serial_out_digest = digest_out_patches(sizing.builds);
+                    }
                 }
             }
             b->groups[k].src_floats = sizing.src_cursor;
@@ -4336,7 +4404,8 @@ static wae_status prep_begin(wae_engine* eng, wae_graph* const* graphs, uint32_t
                 if (same) {  // with the runs started at their place in the slab the merged stage builds ARE the serial ones
                     RangeOut abs_out;
                     same = size_group_split(k, nullptr, (int)std::min<uint32_t>(n_in_group, 3u), abs_out, &b->groups[k].graph_src_base) &&
-                           abs_out.graph_base == b->groups[k].graph_src_base && digest_builds(abs_out.builds, 1469598103934665603ull) == serial_digest;
+                           abs_out.graph_base == b->groups[k].graph_src_base && digest_builds(abs_out.builds, 1469598103934665603ull) == serial_digest &&
+                           digest_out_patches(abs_out.builds) == serial_out_digest;
                 }
                 for (size_t c = 0; same && c < out.copies.size(); c++) {
                     const auto& x = out.copies[c];
@@ -4477,6 +4546,7 @@ static void prep_plan_group(wae_batch* b, wae_graph* const* graphs, int k, PrepS
             struct Run {
                 Builds builds;
                 uint64_t algorithmic_bytes = 0;
+                int64_t dest_reader = -1;
                 int code = WAE_OK;
                 std::string error;
             };
@@ -4497,6 +4567,7 @@ static void prep_plan_group(wae_batch* b, wae_graph* const* graphs, int k, PrepS
                 }
                 runs[t].builds = std::move(rp.builds);
                 runs[t].algorithmic_bytes = rp.algorithmic_bytes;
+                runs[t].dest_reader = rp.dest_reader;
             });
             for (auto& r : runs) {
                 if (r.code != WAE_OK) {
@@ -4506,6 +4577,7 @@ static void prep_plan_group(wae_batch* b, wae_graph* const* graphs, int k, PrepS
                 }
                 merge_builds(pl.builds, r.builds);
                 pl.algorithmic_bytes += r.algorithmic_bytes;
+                if (pl.dest_reader < 0) pl.dest_reader = r.dest_reader;
             }
         } else
         for (uint32_t i = grp.g0; i < grp.g1; i++) {
@@ -4673,10 +4745,26 @@ static void prep_plan_group(wae_batch* b, wae_graph* const* graphs, int k, PrepS
                         sp.p.dst = static_cast<char*>(st.d_a) + (size_t)sp.rec * (s.kind == S_PAN ? sizeof(PanInst) : sizeof(HrtfInst)) + sp.off;
                     gp.spatial.push_back(sp);
                 }
+                char* const out_table = static_cast<char*>(s.kind == S_VSUM ? st.d_c : st.d_a);  // (see StageBuild::out_records)
+                for (const auto& op : s.out_patches)  // destination writers: the BufRef::p of the rendered PCM
+                    gp.out_patches.push_back(
+                        OutPatch{reinterpret_cast<float**>(out_table + (size_t)op.rec * s.out_record_bytes() + op.off + offsetof(BufRef, p)), op.dest});
             }
+        }
+        // the frames of this segment of the graphs no stage writes: zeroed by every run into a bound output (the batch's own buffer
+        // keeps the zeros it was allocated with)
+        std::vector<char> written(grp.g1 - grp.g0, 0);
+        for (auto& kv : pl.builds)
+            for (const auto& op : kv.second.out_patches) written[op.graph - grp.g0] = 1;
+        for (uint32_t j = grp.g0; j < grp.g1; j++) {
+            const int64_t len = (int64_t)b->shape[j].second, f1 = std::min<int64_t>(pl.seg_end, len);
+            if (written[j - grp.g0] || f1 <= pl.seg_start) continue;
+            for (uint32_t c = 0; c < b->shape[j].first; c++)
+                gp.out_zero.push_back({b->out_off[j] + (size_t)c * (size_t)len + (size_t)pl.seg_start, (size_t)(f1 - pl.seg_start)});
         }
         gp.seg_ranges.push_back({seg_stage0, gp.stages.size()});
     }  // segments
+    gp.dest_reader = pl.dest_reader;
     b->flush_uploads();  // the group's tables, before anything of it is launched
 }
 
@@ -4686,6 +4774,8 @@ static void prep_append_group(wae_batch* b, int k, PrepState& ps, GroupPlan& gp)
     for (auto& r : gp.seg_ranges) grp.seg_stages.push_back({grp.stage0 + r.first, grp.stage0 + r.second});
     for (auto& st : gp.stages) b->stages.push_back(st);
     grp.stage1 = b->stages.size();
+    grp.out_zero = std::move(gp.out_zero);
+    if (b->dest_reader < 0 && gp.dest_reader >= 0) b->dest_reader = gp.dest_reader;
     ps.algorithmic_bytes += gp.algorithmic_bytes;
 }
 
@@ -4945,7 +5035,11 @@ static wae_status prepare_impl(wae_engine* eng, wae_graph* const* graphs, uint32
     std::vector<ParamPatch> patches;
     std::vector<SpatialPatch> spatial;
     std::vector<RespBindItem> spatial_resp;
-    st = record_declarations(b, graphs, n_graphs, gps, curve_patches, iir_patches, sched_patches, loop_patches, loop_walks);
+    std::vector<OutPatch> out_patches;
+    for (const auto& gp : gps) out_patches.insert(out_patches.end(), gp.out_patches.begin(), gp.out_patches.end());
+    b->n_out_patches = (int)out_patches.size();
+    if (!out_patches.empty() && !(b->d_out_patches = b->dupload_now(out_patches))) st = fail(WAE_OUT_OF_MEMORY, "out of device memory (output entries)");
+    if (st == WAE_OK) st = record_declarations(b, graphs, n_graphs, gps, curve_patches, iir_patches, sched_patches, loop_patches, loop_walks);
     if (st == WAE_OK) st = record_params(b, graphs, n_graphs, gps, slot_info, patches, spatial, spatial_resp);
     if (st != WAE_OK) {
         wae_batch_destroy(b);
@@ -5153,6 +5247,9 @@ WAE_API wae_status wae_batch_set_timing(wae_batch* b, uint32_t per_stage) {
 // renders one group (all its chunks, all its stages) on the engine stream
 static wae_status run_group(wae_batch* b, const wae_batch::Group& g) {
     cudaStream_t s = b->engine->stream;
+    // each run writes every float of a bound output: what no stage writes is zeroed first
+    if (b->bound_out)
+        for (const auto& z : g.out_zero) CUDA_TRY(cudaMemsetAsync(b->bound_out + z.first, 0, z.second * sizeof(float), s));
     // per-stage device time: one event between consecutive launches, recorded on the launching stream and read back in
     // wae_batch_sync (no host synchronisation inside the run)
     size_t e_prev = (size_t)-1;
@@ -5293,6 +5390,9 @@ static const char* kMixedPacked = "the graphs of this batch differ in shape: the
                                   "wae_batch_fetch_graph (or render with wae_render_many)";
 WAE_API wae_status wae_batch_run_pipelined(wae_batch* b, float* host_out) {
     if (b && b->mixed) return fail(WAE_INVALID_STATE, kMixedPacked);
+    if (b && b->bound_out)
+        return fail(WAE_INVALID_STATE, "wae_batch_run_pipelined streams the batch's own output buffer to host memory, and an output is bound "
+                                       "(wae_batch_bind_output): unbind it with a null output first, or run and fetch");
     wae_status st = check_bound(b);
     if (st != WAE_OK) return st;
     return run_pipelined(b, host_out, true);
@@ -5695,7 +5795,7 @@ WAE_API wae_status wae_batch_sync(wae_batch* b) {
 }
 
 WAE_API wae_status wae_batch_output_device_ptr(wae_batch* b, float** out_dev, uint64_t* out_floats) {
-    *out_dev = b->d_out;
+    *out_dev = b->out_ptr();
     *out_floats = (uint64_t)b->out_off[b->n_graphs];
     return WAE_OK;
 }
@@ -5716,7 +5816,7 @@ WAE_API wae_status wae_batch_fetch_graph(wae_batch* b, uint32_t graph_index, flo
     const uint32_t j = b->batch_pos(graph_index);
     CUDA_TRY(cudaSetDevice(b->engine->device));
     const size_t bytes = (b->out_off[j + 1] - b->out_off[j]) * sizeof(float);
-    if (bytes) CUDA_TRY(cudaMemcpyAsync(out, b->d_out + b->out_off[j], bytes, cudaMemcpyDeviceToHost, b->engine->stream));
+    if (bytes) CUDA_TRY(cudaMemcpyAsync(out, b->out_ptr() + b->out_off[j], bytes, cudaMemcpyDeviceToHost, b->engine->stream));
     CUDA_TRY(cudaStreamSynchronize(b->engine->stream));
     return WAE_OK;
 }
@@ -5725,8 +5825,37 @@ WAE_API wae_status wae_batch_fetch(wae_batch* b, float* host_out) {
     if (b && b->mixed) return fail(WAE_INVALID_STATE, kMixedPacked);
     CUDA_TRY(cudaSetDevice(b->engine->device));
     size_t bytes = (size_t)b->n_graphs * b->channels * b->length * sizeof(float);
-    CUDA_TRY(cudaMemcpyAsync(host_out, b->d_out, bytes, cudaMemcpyDeviceToHost, b->engine->stream));
+    CUDA_TRY(cudaMemcpyAsync(host_out, b->out_ptr(), bytes, cudaMemcpyDeviceToHost, b->engine->stream));
     CUDA_TRY(cudaStreamSynchronize(b->engine->stream));
+    return WAE_OK;
+}
+
+// Later runs write `out` ([out_floats] in the layout of the batch's own buffer) instead of that buffer: every output entry is rewritten on
+// the engine stream, after the work queued on `stream`.  A null `out` with 0 floats returns the batch to its own buffer.
+WAE_API wae_status wae_batch_bind_output(wae_batch* b, float* out, uint64_t floats, void* stream) {
+    if (!b) return fail(WAE_INVALID_ARGUMENT, "null batch");
+    const uint64_t n = (uint64_t)b->out_off[b->n_graphs];
+    CUDA_TRY(cudaSetDevice(b->engine->device));
+    if (!out) {
+        if (floats != 0) return fail(WAE_INVALID_ARGUMENT, "bind_output: a null output (unbind) takes 0 floats, not " + std::to_string(floats));
+    } else {
+        if (b->dest_reader >= 0)
+            return fail(WAE_INVALID_STATE, "bind_output: the destination of graph " +
+                                               std::to_string(b->order.empty() ? b->dest_reader : b->order[b->dest_reader]) +
+                                               " feeds another node, which reads the batch's own output buffer: its output cannot be bound");
+        if (floats != n)
+            return fail(WAE_INVALID_ARGUMENT, "bind_output: " + std::to_string(floats) + " floats given, the batch renders " + std::to_string(n));
+        // (256 bytes, as cudaMalloc aligns the batch's own buffer: the alignment every writer found at its graph's offset holds)
+        BindExtents extents{b->engine->device, {}};
+        wae_status st = extents.check(out, 256, n * sizeof(float), "output", "the output runs past the end of its allocation");
+        if (st != WAE_OK) return st;
+    }
+    wae_status st = bind_after(b, stream);
+    if (st != WAE_OK) return st;
+    if (b->n_out_patches > 0) launch_bind_output(b->d_out_patches, b->n_out_patches, out ? out : b->d_out, b->engine->stream);
+    cudaError_t le = cudaGetLastError();
+    if (le != cudaSuccess) return fail(WAE_CUDA_ERROR, std::string("bind_output: ") + cudaGetErrorString(le));
+    b->bound_out = out;
     return WAE_OK;
 }
 

@@ -4727,6 +4727,15 @@ __global__ void __launch_bounds__(128) k_absn_loop_schedule(const LoopWalk* __re
     r.s.n_seg = k;
 }
 
+// wae_batch_bind_output: every record field that points into the rendered PCM now points into `base` (the caller's memory or the batch's
+// own buffer), at the same offset
+__global__ void __launch_bounds__(128) k_bind_output(const OutPatch* __restrict__ entries, int n, float* base) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const OutPatch e = entries[i];
+    *e.dst = base + e.off;
+}
+
 // Host emulation of the transforms above with the SAME butterfly, index and twiddle code (tests/test_conv_fft_host.py pins them against
 // numpy on a machine without a GPU).  mode 0: complex forward, natural -> position order; 1: complex inverse, position -> natural order
 // (unnormalised); 2: 2B reals -> B packed bins in position order; 3: B packed bins -> 2B reals (scaled by 1 / 2B).  data: 2B floats in place.
@@ -5346,6 +5355,9 @@ void launch_bind_schedules(const SchedBindItem* d, int n, cudaStream_t s) { k_bi
 void launch_bind_loops(const LoopBindItem* d, int n, cudaStream_t s) { k_bind_loops<<<(unsigned)((n + 127) / 128), 128, 0, s>>>(d, n); }
 void launch_absn_loop_schedule(const LoopWalk* d, int n, int* overflow, cudaStream_t s) {
     k_absn_loop_schedule<<<(unsigned)((n + 127) / 128), 128, 0, s>>>(d, n, overflow);
+}
+void launch_bind_output(const OutPatch* d, int n, float* base, cudaStream_t s) {
+    k_bind_output<<<(unsigned)((n + 127) / 128), 128, 0, s>>>(d, n, base);
 }
 void launch_conv_ir_fft(const float* ir, int64_t ir_len, int64_t ir_stride, float2* h, int S, int channels, cudaStream_t s) {
     conv_configure();

@@ -373,6 +373,8 @@ void launch_bind_loops(const LoopBindItem* d, int n, cudaStream_t s);
 // the playhead tables of the n looping bound slow-track records of a batch (k_absn_loop_schedule, one thread per record); *overflow is
 // set when a walk needs more segments than its table holds
 void launch_absn_loop_schedule(const LoopWalk* d, int n, int* overflow, cudaStream_t s);
+// a bind of the output (k_bind_output, one thread per entry): base + off into each of the n output entries of a batch
+void launch_bind_output(const OutPatch* d, int n, float* base, cudaStream_t s);
 void launch_conv_ir_fft(const float* ir, int64_t ir_len, int64_t ir_stride, float2* h, int S, int channels, cudaStream_t s);
 
 }  // namespace wae
