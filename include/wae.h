@@ -507,6 +507,17 @@ WAE_API wae_status wae_batch_plan_quanta(wae_graph* const* graphs, uint32_t n_gr
 WAE_API wae_status wae_buffer_source_set_device_input(wae_graph* graph, wae_node_id node, uint32_t number_of_channels,
                                                       uint64_t length, float sample_rate);
 
+/* A device input read where the caller keeps it: validated and counted as wae_buffer_source_set_device_input (the same texts, the same
+ * "cannot assign buffer twice" rule against set_buffer and either declaration), but the batch gives it no slab memory and its bind
+ * copies no audio.  wae_batch_bind_sources records the item's `pcm` and `channel_stride` in every planned record that plays the node;
+ * later runs read that memory.  The contract differs from a copy: after a copy bind the caller may free or overwrite the tensor at once,
+ * after a reference bind it keeps the memory alive and unchanged for every run that reads it, until it binds other memory.  Writes to
+ * it are ordered by the caller: a write queued on another stream before a run is read by the run only if the engine stream waits for
+ * that stream, and a write after a run waits for the engine stream.  Several declarations may name the same memory; the memory must not
+ * overlap the output the runs write.  wae_render_batch and wae_render_many refuse graphs with such inputs as they refuse device inputs. */
+WAE_API wae_status wae_buffer_source_set_device_input_by_reference(wae_graph* graph, wae_node_id node, uint32_t number_of_channels,
+                                                                   uint64_t length, float sample_rate);
+
 typedef struct wae_source_binding {
     uint32_t graph_index;    /* caller's index, as wae_batch_fetch_graph (also for wae_batch_prepare_many batches) */
     wae_node_id node;        /* a node declared with wae_buffer_source_set_device_input */
@@ -524,6 +535,10 @@ typedef struct wae_source_binding {
  * [pcm, pcm + (channels - 1) * channel_stride + length) does not lie
  * inside one allocation, or channel_stride is below the declared length, or one (graph, node) is named twice in the call.
  * WAE_INVALID_STATE: graph_index out of range, or the node is not a device input.
+ * An input declared with wae_buffer_source_set_device_input_by_reference is not copied: the bind writes `pcm` and `channel_stride` into
+ * the batch's records (one small kernel on the engine stream, no host synchronisation), and runs read the caller's memory.  One call
+ * may mix copied and referenced items.  A referenced extent that overlaps the batch's own output buffer or the output bound with
+ * wae_batch_bind_output answers WAE_INVALID_ARGUMENT.
  * wae_batch_run, wae_batch_run_group and wae_batch_run_pipelined answer WAE_INVALID_STATE while a device input of the batch has never
  * been bound. */
 WAE_API wae_status wae_batch_bind_sources(wae_batch* batch, const wae_source_binding* items, uint32_t n, void* stream);
@@ -823,7 +838,8 @@ WAE_API wae_status wae_batch_bind_loops(wae_batch* batch, const wae_loop_binding
  * wae_batch_output_device_ptr reports `out` and wae_batch_fetch / wae_batch_fetch_graph read it.  WAE_INVALID_ARGUMENT, with nothing
  * changed: `out` is not 256-byte aligned (as cudaMalloc aligns the batch's own buffer; a torch allocation is, and so is a slice of it at
  * a multiple of 64 floats), not device (or managed) memory of the engine's GPU or [out, out + floats) does not lie in one allocation,
- * `floats` is not the batch's out_floats, or a null `out` comes with floats != 0.  WAE_INVALID_STATE: a graph of the batch connects its
+ * `floats` is not the batch's out_floats, a null `out` comes with floats != 0, or [out, out + floats) overlaps the memory a device input
+ * declared by reference is bound to.  WAE_INVALID_STATE: a graph of the batch connects its
  * destination to another node (that node reads the batch's own buffer).  wae_batch_run_pipelined, which streams the batch's own buffer
  * to host memory, answers WAE_INVALID_STATE while an output is bound.  wae_render_batch and wae_render_many are not affected. */
 WAE_API wae_status wae_batch_bind_output(wae_batch* batch, float* out, uint64_t floats, void* stream);

@@ -204,7 +204,7 @@ WAE_SYMBOLS = [
     "wae_node_set_channel_count", "wae_node_set_channel_count_mode", "wae_node_set_channel_interpretation", "wae_graph_render_order", "wae_hrir_resample", "wae_batch_plan", "wae_buffer_source_set_buffer", "wae_convolver_set_buffer", "wae_wave_shaper_set_curve",
     "wae_oscillator_set_periodic_wave", "wae_node_set_attribute", "wae_disconnect_from", "wae_disconnect_param", "wae_periodic_wave_table", "wae_param_sim_set_walker", "wae_sched_first_frame_at_or_after", "wae_spatial_params", "wae_hrtf_locate",
     "wae_render_many", "wae_batch_prepare_many", "wae_batch_graph_output", "wae_batch_fetch_graph", "wae_batch_plan_many", "wae_batch_plan_quanta",
-    "wae_buffer_source_set_device_input", "wae_batch_bind_sources",
+    "wae_buffer_source_set_device_input", "wae_buffer_source_set_device_input_by_reference", "wae_batch_bind_sources",
     "wae_param_set_device_value", "wae_batch_bind_params",
     "wae_convolver_set_device_response", "wae_batch_bind_responses",
     "wae_wave_shaper_set_device_curve", "wae_batch_bind_curves",
@@ -316,6 +316,7 @@ class Api:
             f("batch_plan_quanta", C.c_int32, [C.POINTER(C.c_void_p), C.c_uint32, C.POINTER(C.c_uint32), C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)])
             # source audio bound from device memory
             f("buffer_source_set_device_input", C.c_int32, [gp, C.c_uint32, C.c_uint32, C.c_uint64, C.c_float])
+            f("buffer_source_set_device_input_by_reference", C.c_int32, [gp, C.c_uint32, C.c_uint32, C.c_uint64, C.c_float])
             f("batch_bind_sources", C.c_int32, [C.c_void_p, C.POINTER(SourceBinding), C.c_uint32, C.c_void_p])
             # param values bound from device memory
             f("param_set_device_value", C.c_int32, [gp, C.c_uint32, C.c_uint32, C.c_float, C.c_float])

@@ -309,14 +309,20 @@ class AudioBufferSourceNode(AudioScheduledSourceNode):
     def set_buffer(self, buffer):
         self._set_buffer("buffer_source_set_buffer", buffer)
 
-    def set_device_input(self, number_of_channels, length, sample_rate):
+    def set_device_input(self, number_of_channels, length, sample_rate, by_reference=False):
         """wae_buffer_source_set_device_input (product only): the node plays audio of this shape that Batch.bind_sources supplies from
-        device memory before each run, instead of an AudioBuffer.  Counts as the node's buffer."""
+        device memory before each run, instead of an AudioBuffer.  Counts as the node's buffer.
+        by_reference (wae_buffer_source_set_device_input_by_reference): the runs read the bound tensor where it lies, and the batch keeps
+        no copy of it.  The tensor must then stay unchanged while runs that read it are queued: write it in place only after
+        Batch.output_tensor() or Batch.sync() has ordered torch after those runs (a ring of input tensors follows that rule)."""
         api = self._ctx._api
         if not api.is_product:
             raise B.WaeError(3, "device inputs are a feature of the GPU engine")
-        api.check(api.buffer_source_set_device_input(self._ctx._g, self.id, int(number_of_channels), int(length), float(sample_rate)))
+        declare = api.buffer_source_set_device_input_by_reference if by_reference else api.buffer_source_set_device_input
+        api.check(declare(self._ctx._g, self.id, int(number_of_channels), int(length), float(sample_rate)))
         self._ctx._device_inputs[self.id] = (int(number_of_channels), int(length))
+        if by_reference:
+            self._ctx._source_refs.add(self.id)
 
     def set_loop(self, value):
         self._set_attribute(B.ATTR_LOOP, 1.0 if value else 0.0)
@@ -556,6 +562,7 @@ class OfflineAudioContext:
         self._suspends = []
         self._current_time = 0.0
         self._device_inputs = {}  # node id -> (channels, length) declared with set_device_input
+        self._source_refs = set()  # ids of the device inputs declared by_reference
         self._device_responses = {}  # node id -> (channels, length) declared with set_device_response
         self._device_curves = {}  # node id -> length declared with set_device_curve
         self._device_waves = {}  # node id -> coefficient count declared with set_device_periodic_wave
@@ -783,6 +790,9 @@ class Batch:
         self._views_out = False  # output_tensor was called: runs into the batch's own buffer are ordered after torch's current stream
         self._out = None  # bind_output: the tensor runs write
         self._out_viewed = False  # output_tensor handed out views of the bound tensor since it was bound: runs into it wait for torch
+        self._src_refs = {}  # bind_sources: (graph, node id) -> the tensor a device input declared by_reference reads
+        self._ref_tensors = []  # the distinct tensors of _src_refs
+        self._has_refs = any(c._source_refs for c in contexts)
         self._backend = ctx0._backend
         self._backend.batches.add(self)
         for i, c in enumerate(contexts):
@@ -790,8 +800,10 @@ class Batch:
 
     def run(self):
         self._after_torch_readers()
+        self._after_torch_writers()
         self.api.check(self.api.batch_run(self.handle))
         self._out_written()
+        self._refs_read()
 
     def upload(self):
         self.api.check(self.api.batch_upload(self.handle))
@@ -816,13 +828,17 @@ class Batch:
     def run_group(self, k):
         """render of ONE graph group, asynchronous on the engine stream (call the groups in order)"""
         self._after_torch_readers()
+        self._after_torch_writers()
         self.api.check(self.api.batch_run_group(self.handle, k))
         self._out_written()
+        self._refs_read()
 
     def run_pipelined(self, host_out_ptr):
         """H2D + render + D2H, overlapped per graph group; `host_out_ptr` = address of [n][ch][length] f32 (pinned)."""
         self._after_torch_readers()
+        self._after_torch_writers()
         self.api.check(self.api.batch_run_pipelined(self.handle, host_out_ptr))
+        self._refs_read()
 
     def fetch(self, out=None):
         if out is None:
@@ -879,9 +895,30 @@ class Batch:
         """wae_batch_bind_sources: pcm[k] ([channels][length] of a float32 CUDA tensor [n][channels][length], unit stride on the last
         dimension) becomes the audio of device input nodes[k] of context graphs[k] (default: 0..n-1).  `nodes`: one node (or id) for all
         graphs (graphs built the same way share ids) or one per graph.  One call, ordered after torch's current stream (its default
-        stream included); the copy runs on the engine stream, and the tensor's memory is kept from reuse until it has (record_stream)."""
+        stream included); the copy runs on the engine stream, and the tensor's memory is kept from reuse until it has (record_stream).
+        Inputs declared by_reference are not copied: the batch keeps `pcm` until they are bound again or the batch is destroyed, and each
+        run reads it (see AudioBufferSourceNode.set_device_input).  A tensor of one shape [1][channels][length] expanded to n rows
+        (stride 0 on the first dimension) names the same memory for every graph."""
         items, n = self._pcm_items("bind_sources", "pcm", nodes, pcm, graphs, "_device_inputs", B.SourceBinding)
         self._bind(self.api.batch_bind_sources, items, n, pcm)
+        if self._has_refs:
+            gs, ids = self._graphs_and_nodes("bind_sources", nodes, graphs, n)
+            keys = [(g, int(nid)) for g, nid in zip(gs, ids) if int(nid) in self.contexts[g]._source_refs]
+            if keys:
+                self._src_refs.update(dict.fromkeys(keys, pcm))
+                self._ref_tensors = list({id(t): t for t in self._src_refs.values()}.values())
+
+    def _after_torch_writers(self):
+        """While a device input declared by_reference is bound, a run reads caller memory: order it after the work torch has queued so
+        far on its current stream (in-place writes to the bound tensors made after the bind included)."""
+        if self._src_refs:
+            import torch
+            self._engine_stream().wait_stream(torch.cuda.current_stream(self._device()))
+
+    def _refs_read(self):
+        """Keeps the tensors read by reference from reuse until the runs queued so far have read them (as bind_output's tensor)."""
+        for t in self._ref_tensors:
+            self._keep_until_read(t)
 
     def bind_responses(self, nodes, ir, graphs=None):
         """wae_batch_bind_responses: ir[k] ([channels][length] of a float32 CUDA tensor [n][channels][length], unit stride on the last
@@ -1239,6 +1276,7 @@ class Batch:
         return out
 
     def destroy(self):
+        self._src_refs, self._ref_tensors = {}, []
         if self.handle:
             if not self._backend.closed:  # a batch must not outlive its engine
                 self.api.batch_destroy(self.handle)

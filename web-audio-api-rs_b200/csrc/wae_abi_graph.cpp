@@ -1212,9 +1212,10 @@ WAE_API wae_status wae_buffer_source_set_buffer(wae_graph* g, wae_node_id node, 
 }
 
 // A device input counts as the node's buffer: the placeholder has the declared shape and rate and no host block.  It is not entered in
-// g->assets, so content sharing never merges two device inputs; each gets its own slot in the group's source slab.
-WAE_API wae_status wae_buffer_source_set_device_input(wae_graph* g, wae_node_id node, uint32_t number_of_channels, uint64_t length,
-                                                      float sample_rate) {
+// g->assets, so content sharing never merges two device inputs; each gets its own slot in the group's source slab, or none when it is
+// read by reference.
+static wae_status declare_device_input(wae_graph* g, wae_node_id node, uint32_t number_of_channels, uint64_t length, float sample_rate,
+                                       bool by_reference) {
     Node* n = node_of_kind(g, node, K_ABSN);
     if (!n) return fail(WAE_INVALID_ARGUMENT, "not an AudioBufferSourceNode");
     // AudioBuffer::new (src/buffer.rs:96-115), as copy_buffer checks it
@@ -1225,6 +1226,7 @@ WAE_API wae_status wae_buffer_source_set_device_input(wae_graph* g, wae_node_id 
     auto p = std::make_shared<PcmBuffer>();
     p->sample_rate = sample_rate;
     p->device_input = true;
+    p->by_reference = by_reference;
     p->stride = (size_t)(length + 3) / 4 * 4;
     p->channels.resize(number_of_channels);
     for (auto& c : p->channels) c.n = (size_t)length;
@@ -1232,6 +1234,16 @@ WAE_API wae_status wae_buffer_source_set_device_input(wae_graph* g, wae_node_id 
     g->device_inputs++;
     end_if_started_without_buffer(g, node, n);
     return WAE_OK;
+}
+
+WAE_API wae_status wae_buffer_source_set_device_input(wae_graph* g, wae_node_id node, uint32_t number_of_channels, uint64_t length,
+                                                      float sample_rate) {
+    return declare_device_input(g, node, number_of_channels, length, sample_rate, false);
+}
+
+WAE_API wae_status wae_buffer_source_set_device_input_by_reference(wae_graph* g, wae_node_id node, uint32_t number_of_channels,
+                                                                   uint64_t length, float sample_rate) {
+    return declare_device_input(g, node, number_of_channels, length, sample_rate, true);
 }
 
 // ConvolverNode::set_buffer (src/node/convolver.rs:259-317): may replace the response; the normalisation is decided now

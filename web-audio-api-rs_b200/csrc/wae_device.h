@@ -736,4 +736,19 @@ struct OutPatch {
     uint64_t off;  // floats from the start of the packed output
 };
 
+// A source-reference entry: the PCM pointer and channel stride of one planned record that plays an AudioBufferSourceNode declared with
+// wae_buffer_source_set_device_input_by_reference (AbsnInst on k_buffer_source or inside a ChainInst, AbsnSlowInst, AbsnBoundInst::s,
+// AbsnSerialInst).  wae_batch_bind_sources writes the caller's pointer and stride into them (k_bind_source_refs).
+struct SrcRefPatch {
+    const float** buf;
+    int64_t* stride;
+};
+// one row of k_bind_source_refs: entry `entry` of the batch now reads `pcm`, channel c at pcm + c * stride
+struct SrcRefBindItem {
+    const float* pcm;
+    int64_t stride;  // floats, >= the declared length, any value
+    int32_t entry;
+    int32_t pad;
+};
+
 }  // namespace wae

@@ -380,6 +380,16 @@ struct StageBuild {
         uint32_t pad;
     };
     std::vector<OutPatchRec> out_patches;
+    // Source-reference entries (wae_buffer_source_set_device_input_by_reference): the PCM pointer `buf` bytes and the channel stride
+    // `stride` bytes into record `rec` of this stage's table (AbsnInst, AbsnSlowInst, AbsnBoundInst, AbsnSerialInst, or the AbsnInst of a
+    // ChainInst)
+    struct SrcRefRec {
+        uint32_t graph;  // batch position
+        wae_node_id node;
+        int32_t rec;
+        uint32_t buf, stride;
+    };
+    std::vector<SrcRefRec> src_refs;
     size_t out_records() const {
         switch (kind) {
             case S_MIX: return mix.size();
@@ -415,6 +425,8 @@ struct StageBuild {
             case S_SPAN: return span.size();
             case S_COMP: return comp.size();
             case S_META: return meta.size();
+            case S_ABSN: return absn.size();
+            case S_ABSN_SLOW: return absn_slow.size();
             case S_ABSN_SERIAL: return absn_serial.size();
             case S_ABSN_BOUND: return absn_bound.size();
             case S_PAN_DYN: return pan_dyn.size();
@@ -436,6 +448,8 @@ struct StageBuild {
             case S_SPAN: return sizeof(SPanInst);
             case S_COMP: return sizeof(CompInst);
             case S_META: return sizeof(MetaInst);
+            case S_ABSN: return sizeof(AbsnInst);
+            case S_ABSN_SLOW: return sizeof(AbsnSlowInst);
             case S_ABSN_SERIAL: return sizeof(AbsnSerialInst);
             case S_ABSN_BOUND: return sizeof(AbsnBoundInst);
             case S_PAN_DYN: return sizeof(PanDynInst);
@@ -584,6 +598,13 @@ struct DevInput {  // wae_buffer_source_set_device_input: the slot in its group'
     float* slot;   // [channels][stride]
     uint32_t channels;
     uint64_t length, stride;
+    // wae_buffer_source_set_device_input_by_reference (no slot): the entries of every record that plays it, in d_src_refs, and the
+    // caller's memory its last bind named (the extent bind_output must not overlap)
+    bool by_reference = false;
+    int32_t p0 = 0, p1 = 0;
+    const float* pcm = nullptr;
+    uint64_t pcm_stride = 0;
+    uint64_t extent_bytes() const { return ((uint64_t)(channels - 1) * pcm_stride + length) * sizeof(float); }
 };
 struct DevResponse {  // wae_convolver_set_device_response: the spectra the planner made
     float2* h;        // [channels][S + WAE_CONV_H_PAD][WAE_CONV_SPEC]
@@ -718,6 +739,7 @@ struct wae_batch {
     IirPatch* d_iir_patches = nullptr;
     SchedPatch* d_sched_patches = nullptr;
     LoopPatch* d_loop_patches = nullptr;
+    SrcRefPatch* d_src_refs = nullptr;  // and of the device inputs declared by reference
     // the looping bound slow-track records whose playhead tables k_absn_loop_schedule derives after every bind of loop points, params or
     // schedules (their inputs); d_loop_overflow: set by a walk that outgrew its table (reported by wae_batch_sync)
     LoopWalk* d_loop_walks = nullptr;
@@ -1122,6 +1144,8 @@ struct Planner {
         std::vector<StageBuild::IirPatchRec> iir_patches;
         // a source whose schedule is bound from device memory: the entry of ChainInst::osc / ::cst (rec set when the chain is emitted)
         std::vector<StageBuild::SchedPatchRec> sched_patches;
+        // a source declared by reference: the entry of ChainInst::absn (rec set when the chain is emitted)
+        std::vector<StageBuild::SrcRefRec> src_refs;
     };
 
     // Node state is allocated through a key (graph, node, n-th allocation of that node, salt): the plans of consecutive
@@ -1406,6 +1430,10 @@ struct Planner {
             r.rec = rec;
             s.sched_patches.push_back(r);
         }
+        for (StageBuild::SrcRefRec r : pc.src_refs) {
+            r.rec = rec;
+            s.src_refs.push_back(r);
+        }
     }
     static bool chain_has_patches(const PendingChain& pc) {
         bool any = !pc.patches.empty();
@@ -1569,11 +1597,17 @@ struct Planner {
     bool lower_const(NodeCtx& nc);
     struct AbsnPlay {  // what every playback path of an AudioBufferSourceNode reads
         const PcmBuffer* pb;
-        float* buf;  // its PCM in the group's slab
+        float* buf;  // its PCM in the group's slab (a device input declared by reference: a placeholder its bind replaces)
         size_t len, stride;
         int ch;
         double duration, ls, le, computed_rate;  // ls / le: the clamped loop boundaries
+        bool by_ref;
     };
+    // the source-reference entry of the last record of `s` that plays declared source `n`, its PCM pointer and channel stride `buf` and
+    // `stride` bytes into the record
+    void add_src_ref(StageBuild& s, const Node& n, size_t buf, size_t stride) {
+        s.src_refs.push_back(StageBuild::SrcRefRec{gi, n.id, (int32_t)s.records() - 1, (uint32_t)buf, (uint32_t)stride});
+    }
     // a patch entry of the schedule of declared source `n` (wae_source_set_device_schedule) for the last record of stage `s`, its fields
     // `off` bytes into it
     SchedPatch sched_entry(const Node& n, int32_t kind) const {
@@ -1681,10 +1715,15 @@ static uint64_t digest_vec_skipping(const std::vector<T>& v, std::initializer_li
 template <typename T>
 static uint64_t digest_vec_without_end(const std::vector<T>& v, uint64_t h) { return digest_vec_skipping(v, {offsetof(T, end)}, h); }
 
-// (the output entries are not part of any record: the split sizing's self-check compares them on their own)
+// (the output and source-reference entries are not part of any record: the split sizing's self-check compares them on their own)
 static uint64_t digest_out_patches(const std::map<std::pair<int, int>, StageBuild>& builds) {
     uint64_t h = 1469598103934665603ull;
     for (auto& kv : builds) h = digest_vec(kv.second.out_patches, h);
+    return h;
+}
+static uint64_t digest_src_refs(const std::map<std::pair<int, int>, StageBuild>& builds) {
+    uint64_t h = 1469598103934665603ull;
+    for (auto& kv : builds) h = digest_vec(kv.second.src_refs, h);
     return h;
 }
 static uint64_t digest_builds(const std::map<std::pair<int, int>, StageBuild>& builds, uint64_t h) {
@@ -1742,6 +1781,7 @@ static void merge_builds(Builds& dst, Builds& src) {
         for (auto& sp : s.spatial)
             if (sp.rec >= 0) sp.rec += (int32_t)bs.spatial;
         for (auto& op : s.out_patches) op.rec += (int32_t)bs.out;
+        for (auto& sr : s.src_refs) sr.rec += (int32_t)bs.records;
         for (auto& ip : s.iir_patches) {
             ip.rec += (int32_t)bs.records;
             if (ip.scan >= 0) ip.scan += (int32_t)bs.scan;
@@ -1782,6 +1822,7 @@ static void merge_builds(Builds& dst, Builds& src) {
         append_vec(d.loop_walks, s.loop_walks);
         append_vec(d.spatial, s.spatial);
         append_vec(d.out_patches, s.out_patches);
+        append_vec(d.src_refs, s.src_refs);
         d.n_scan_coef += s.n_scan_coef;
         d.max_ch = std::max(d.max_ch, s.max_ch);
     }
@@ -2182,7 +2223,8 @@ StageBuild& Planner::emit_chain(PendingChain& pc, int L) {
 
 // may_alias: the consumer reads its input through chan() with any alignment (the convolver's forward transform): a pending chain that
 // is nothing but an AudioBufferSourceNode playing its buffer 1:1 from frame 0, the buffer covering the whole (quantum-padded) render,
-// IS that buffer — no copy into the arena
+// IS that buffer — no copy into the arena.  Not a device input read by reference: the consumer's BufRef would bake the placeholder, and
+// its readers (chain_load_source<CHAIN_SRC_BUFFER>) load 16 B aligned, zero-padded channels, which caller memory need not be.
 bool Planner::materialize(uint32_t nid, bool may_alias) {
     auto it = pending.find(nid);
     if (it == pending.end()) return true;
@@ -2192,7 +2234,8 @@ bool Planner::materialize(uint32_t nid, bool may_alias) {
         const AbsnInst& a = ci.absn;
         bool unit = true;
         for (int i = 0; i < 4; i++) unit = unit && ci.g[i] == 1.f;
-        if (may_alias && ci.src_kind == CHAIN_SRC_ABSN && ci.n_biquad == 0 && !ci.has_shaper && unit && !chain_has_patches(it->second) && it->second.phase == 0 &&
+        if (may_alias && ci.src_kind == CHAIN_SRC_ABSN && ci.n_biquad == 0 && !ci.has_shaper && unit && !chain_has_patches(it->second) &&
+            it->second.src_refs.empty() && it->second.phase == 0 &&
             !it->second.lay.dyn() && a.n_start == 0 && !a.loop && a.buf_offset == 0 && a.buf_len >= lq && a.buf_stride <= 0xffffffffll &&
             seg_start == 0 && seg_end >= lq) {
             sp.out_buf = {BufRef{const_cast<float*>(a.buf), (uint32_t)a.buf_stride, 1}};
@@ -2734,24 +2777,29 @@ bool Planner::lower_absn(NodeCtx& nc) {
     if (!fused && !need_out(nc, ch)) return false;
     size_t len = pb.length();
     size_t stride = (len + 3) / 4 * 4;  // every channel starts 16 B aligned (LDG.128)
-    // one copy of the PCM per AudioBuffer in the group's slab (the grains of a granular patch all play the same one: the graph
-    // holds it once, wae_abi_graph.cpp copy_buffer), shared by the plans of all render segments
-    auto so = src_offsets.find({gi, nc.id});
-    bool first_use = so == src_offsets.end();
-    if (first_use) {
-        auto bo = buf_offsets.find(n.buffer.get());
-        if (bo != buf_offsets.end()) first_use = false;  // (already in the slab for another node)
-        else bo = buf_offsets.emplace(n.buffer.get(), src_cursor).first;
-        so = src_offsets.emplace(std::make_pair(gi, nc.id), bo->second).first;
+    // a device input read by reference has no slab memory: its records get a placeholder pointer and the slab's stride (the plan sizes as
+    // its copy-declared twin's does), and an entry each that its bind rewrites with the caller's pointer and stride
+    float* d_buf = reinterpret_cast<float*>(uintptr_t(256));
+    if (!pb.by_reference) {
+        // one copy of the PCM per AudioBuffer in the group's slab (the grains of a granular patch all play the same one: the graph
+        // holds it once, wae_abi_graph.cpp copy_buffer), shared by the plans of all render segments
+        auto so = src_offsets.find({gi, nc.id});
+        bool first_use = so == src_offsets.end();
+        if (first_use) {
+            auto bo = buf_offsets.find(n.buffer.get());
+            if (bo != buf_offsets.end()) first_use = false;  // (already in the slab for another node)
+            else bo = buf_offsets.emplace(n.buffer.get(), src_cursor).first;
+            so = src_offsets.emplace(std::make_pair(gi, nc.id), bo->second).first;
+        }
+        d_buf = d_src + so->second;
+        if (first_use) {
+            if (src_copies)  // recorded by the sizing pass: uploaded straight from the graph's buffer, planar [ch][stride] like the slab
+                src_copies->push_back(wae_batch::Group::SrcCopy{n.buffer, src_cursor, (size_t)ch * stride, gi, nc.id});
+            src_cursor += (size_t)ch * stride;
+            b->asset_bytes += (size_t)ch * len * 4;
+        }
     }
-    float* d_buf = d_src + so->second;
-    if (first_use) {
-        if (src_copies)  // recorded by the sizing pass: uploaded straight from the graph's buffer, planar [ch][stride] like the slab
-            src_copies->push_back(wae_batch::Group::SrcCopy{n.buffer, src_cursor, (size_t)ch * stride, gi, nc.id});
-        src_cursor += (size_t)ch * stride;
-        b->asset_bytes += (size_t)ch * len * 4;
-    }
-    const AbsnPlay s{&pb, d_buf, len, stride, ch, duration, ls, le, computed_rate};
+    const AbsnPlay s{&pb, d_buf, len, stride, ch, duration, ls, le, computed_rate, pb.by_reference};
     if (serial) return absn_serial(nc, s, pdet, prate);
     if (rate_bound || n.device_schedule || n.device_loop) return absn_bound(nc, s, pdet, prate, q, aligned, rate_hi, loop_cap);
     if (!fast) return absn_slow(nc, s);
@@ -2796,6 +2844,7 @@ bool Planner::absn_serial(NodeCtx& nc, const AbsnPlay& s, const PRef& pdet, cons
     a.out = nc.p.out_buf[0];
     StageBuild& sb = stage(nc.L, S_ABSN_SERIAL);
     sb.absn_serial.push_back(a);
+    if (s.by_ref) add_src_ref(sb, n, offsetof(AbsnSerialInst, buf), offsetof(AbsnSerialInst, buf_stride));
     const PRef* refs[2] = {&pdet, &prate};
     const size_t offs[2] = {offsetof(AbsnSerialInst, detune), offsetof(AbsnSerialInst, rate)};
     for (int i = 0; i < 2; i++)
@@ -2863,7 +2912,9 @@ bool Planner::absn_slow(NodeCtx& nc, const AbsnPlay& s) {
     // layout: silent before the quantum of the first playing frame and after the quantum in which the source ends
     // (stop time, explicit duration, or — not looping — the end of the buffer; audio_buffer_source.rs:826-838)
     a.out = source_out(nc, n_first, d.n_end, s.ch);
-    stage(nc.L, S_ABSN_SLOW).absn_slow.push_back(a);
+    StageBuild& sb = stage(nc.L, S_ABSN_SLOW);
+    sb.absn_slow.push_back(a);
+    if (s.by_ref) add_src_ref(sb, n, offsetof(AbsnSlowInst, buf), offsetof(AbsnSlowInst, buf_stride));
     algorithmic_bytes += (uint64_t)s.ch * 4ull * (uint64_t)std::min<int64_t>(lq, (int64_t)s.len);
     return true;
 }
@@ -2926,6 +2977,8 @@ bool Planner::absn_bound(NodeCtx& nc, const AbsnPlay& s, const PRef& pdet, const
     a.out = nc.p.out_buf[0];
     StageBuild& sb = stage(nc.L, S_ABSN_BOUND);
     sb.absn_bound.push_back(r);
+    if (s.by_ref)
+        add_src_ref(sb, n, offsetof(AbsnBoundInst, s) + offsetof(AbsnSlowInst, buf), offsetof(AbsnBoundInst, s) + offsetof(AbsnSlowInst, buf_stride));
     if (n.device_schedule) {  // the start-dependent fields, re-derived by the bind; the kernel derives the rest per run as before
         SchedPatch sp = sched_entry(n, SCHED_ABSN_BOUND);
         sp.flag = fast_shape;
@@ -2968,10 +3021,15 @@ bool Planner::absn_fast(NodeCtx& nc, const AbsnPlay& s, int64_t q, bool fused) {
         PendingChain pc = source_chain(CHAIN_SRC_ABSN, s.ch);
         pc.inst.absn = a;
         pc.lay = source_lay(a.n_start, a.n_stop, s.ch);
+        if (s.by_ref)
+            pc.src_refs.push_back(StageBuild::SrcRefRec{gi, n.id, -1, (uint32_t)(offsetof(ChainInst, absn) + offsetof(AbsnInst, buf)),
+                                                        (uint32_t)(offsetof(ChainInst, absn) + offsetof(AbsnInst, buf_stride))});
         if (!finish_chain(nc, std::move(pc))) return false;
     } else {
         a.out = source_out(nc, a.n_start, a.n_stop, s.ch);
-        stage(nc.L, S_ABSN).absn.push_back(a);
+        StageBuild& sb = stage(nc.L, S_ABSN);
+        sb.absn.push_back(a);
+        if (s.by_ref) add_src_ref(sb, n, offsetof(AbsnInst, buf), offsetof(AbsnInst, buf_stride));
     }
     // compulsory read of the source PCM that is actually played
     algorithmic_bytes += (uint64_t)s.ch * 4ull * (uint64_t)std::max<int64_t>(0, std::min<int64_t>(lq - a.n_start, n.loop ? lq : (int64_t)s.len));
@@ -4102,6 +4160,7 @@ struct GroupPlan {  // result of phase B for one group
     std::vector<LoopWalk> loop_walks;
     std::vector<StageBuild::SpatialPatchRec> spatial;  // device addresses set, operands still param ids
     std::vector<OutPatch> out_patches;                 // device addresses set
+    std::vector<PatchEntry<SrcRefPatch>> src_refs;     // device addresses set
     std::vector<std::pair<size_t, size_t>> out_zero;   // (offset, floats) of the output no stage writes
     int64_t dest_reader = -1;                          // see Planner::dest_reader
 };
@@ -4365,7 +4424,7 @@ static wae_status prep_begin(wae_engine* eng, wae_graph* const* graphs, uint32_t
             b->groups[k].graph_src_base.clear();
             Planner sizing(b, b->groups[k], ps, &b->groups[k].src_copies);
             const std::vector<int64_t>& bounds = b->groups[k].seg_bounds;
-            uint64_t serial_digest = 0, serial_out_digest = 0;
+            uint64_t serial_digest = 0, serial_out_digest = 0, serial_ref_digest = 0;
             for (size_t sg = 0; sg + 1 < bounds.size(); sg++) {
                 sizing.begin_segment(bounds[sg], bounds[sg + 1]);
                 for (uint32_t i = b->groups[k].g0; i < b->groups[k].g1; i++) {
@@ -4386,6 +4445,7 @@ static wae_status prep_begin(wae_engine* eng, wae_graph* const* graphs, uint32_t
                     if (check_split && one_segment) {
                         serial_digest = digest_builds(sizing.builds, 1469598103934665603ull);
                         serial_out_digest = digest_out_patches(sizing.builds);
+                        serial_ref_digest = digest_src_refs(sizing.builds);
                     }
                 }
             }
@@ -4405,7 +4465,7 @@ static wae_status prep_begin(wae_engine* eng, wae_graph* const* graphs, uint32_t
                     RangeOut abs_out;
                     same = size_group_split(k, nullptr, (int)std::min<uint32_t>(n_in_group, 3u), abs_out, &b->groups[k].graph_src_base) &&
                            abs_out.graph_base == b->groups[k].graph_src_base && digest_builds(abs_out.builds, 1469598103934665603ull) == serial_digest &&
-                           digest_out_patches(abs_out.builds) == serial_out_digest;
+                           digest_out_patches(abs_out.builds) == serial_out_digest && digest_src_refs(abs_out.builds) == serial_ref_digest;
                 }
                 for (size_t c = 0; same && c < out.copies.size(); c++) {
                     const auto& x = out.copies[c];
@@ -4738,6 +4798,9 @@ static void prep_plan_group(wae_batch* b, wae_graph* const* graphs, int k, PrepS
                     p.dst = rec(lp.rec);
                     gp.loop_patches.push_back({lp.graph, lp.node, p});
                 }
+                for (const auto& sr : s.src_refs)  // sources declared by reference: the record's PCM pointer and channel stride
+                    gp.src_refs.push_back({sr.graph, sr.node, SrcRefPatch{reinterpret_cast<const float**>(rec(sr.rec) + sr.buf),
+                                                                         reinterpret_cast<int64_t*>(rec(sr.rec) + sr.stride)}});
                 for (const auto& lw : s.loop_walks)
                     gp.loop_walks.push_back(LoopWalk{reinterpret_cast<AbsnBoundInst*>(rec(lw.rec)), lw.lq, lw.cap, 0});
                 for (StageBuild::SpatialPatchRec sp : s.spatial) {  // static panners: the PanInst or HrtfInst::static_sel they re-derive
@@ -4789,8 +4852,9 @@ static wae_status enqueue_source_copies(wae_batch* b, wae_batch::Group& grp, cud
 }
 
 // The device inputs of the batch (`graphs` in batch order): the slots of the planned groups, then the declared ones the planner gave no
-// slot (a source that is never started renders silence without reading its buffer), which behave like a node given an AudioBuffer of
-// that shape.
+// slot (a source that is never started renders silence without reading its buffer, and an input read by reference has none), which
+// behave like a node given an AudioBuffer of that shape.  Runs wait for an input read by reference once record_declarations has found
+// entries for it.
 static void record_device_inputs(wae_batch* b, wae_graph* const* graphs, uint32_t n_graphs) {
     for (auto& grp : b->groups)
         for (auto& sc : grp.src_copies)
@@ -4801,8 +4865,8 @@ static void record_device_inputs(wae_batch* b, wae_graph* const* graphs, uint32_
             }
     b->sources.seal(graphs, n_graphs, [](uint32_t j, const NodeMap&, const Node& nd, auto& declare) {
         if (nd.kind == K_ABSN && nd.buffer && nd.buffer->device_input)
-            declare({j, nd.id, kNodeLevel},
-                    DevInput{nullptr, (uint32_t)nd.buffer->channels.size(), (uint64_t)nd.buffer->length(), (uint64_t)nd.buffer->stride});
+            declare({j, nd.id, kNodeLevel}, DevInput{nullptr, (uint32_t)nd.buffer->channels.size(), (uint64_t)nd.buffer->length(),
+                                                     (uint64_t)nd.buffer->stride, nd.buffer->by_reference});
     });
 }
 
@@ -4829,12 +4893,12 @@ static wae_status gather_patches(wae_batch* b, Bindings<D>& t, const std::vector
 }  // extern "C++"
 
 // The declared responses, curves, periodic waves, IIR filters, schedules and value curves of the batch (`graphs` in batch order), after
-// planning.  Runs wait for the ones the planner gave memory or patch entries; the patch entries are uploaded from the vectors passed,
-// which the caller keeps alive until the stream has been synchronised.
+// planning, and the entries of the device inputs read by reference.  Runs wait for the ones the planner gave memory or patch entries;
+// the patch entries are uploaded from the vectors passed, which the caller keeps alive until the stream has been synchronised.
 static wae_status record_declarations(wae_batch* b, wae_graph* const* graphs, uint32_t n_graphs, const std::vector<GroupPlan>& gps,
                                       std::vector<CurvePatch>& curve_patches, std::vector<IirPatch>& iir_patches,
                                       std::vector<SchedPatch>& sched_patches, std::vector<LoopPatch>& loop_patches,
-                                      std::vector<LoopWalk>& loop_walks) {
+                                      std::vector<LoopWalk>& loop_walks, std::vector<SrcRefPatch>& src_refs) {
     b->responses.seal(graphs, n_graphs, [](uint32_t j, const NodeMap&, const Node& nd, auto& declare) {
         if (nd.kind == K_CONV && nd.buffer && nd.buffer->device_input)
             declare({j, nd.id, kNodeLevel}, DevResponse{nullptr, (uint32_t)nd.buffer->channels.size(), (uint64_t)nd.buffer->length(), 0,
@@ -4873,6 +4937,7 @@ static wae_status record_declarations(wae_batch* b, wae_graph* const* graphs, ui
     if (st == WAE_OK) st = gather_patches(b, b->iirs, gps, &GroupPlan::iir_patches, iir_patches, &b->d_iir_patches);
     if (st == WAE_OK) st = gather_patches(b, b->schedules, gps, &GroupPlan::sched_patches, sched_patches, &b->d_sched_patches);
     if (st == WAE_OK) st = gather_patches(b, b->loops, gps, &GroupPlan::loop_patches, loop_patches, &b->d_loop_patches);
+    if (st == WAE_OK) st = gather_patches(b, b->sources, gps, &GroupPlan::src_refs, src_refs, &b->d_src_refs);
     for (const auto& gp : gps) loop_walks.insert(loop_walks.end(), gp.loop_walks.begin(), gp.loop_walks.end());
     if (st == WAE_OK && !loop_walks.empty()) {
         b->n_loop_walks = (int)loop_walks.size();
@@ -5031,6 +5096,7 @@ static wae_status prepare_impl(wae_engine* eng, wae_graph* const* graphs, uint32
     std::vector<SchedPatch> sched_patches;
     std::vector<LoopPatch> loop_patches;
     std::vector<LoopWalk> loop_walks;
+    std::vector<SrcRefPatch> src_refs;
     std::vector<ParamSlotInfo> slot_info;
     std::vector<ParamPatch> patches;
     std::vector<SpatialPatch> spatial;
@@ -5039,7 +5105,7 @@ static wae_status prepare_impl(wae_engine* eng, wae_graph* const* graphs, uint32
     for (const auto& gp : gps) out_patches.insert(out_patches.end(), gp.out_patches.begin(), gp.out_patches.end());
     b->n_out_patches = (int)out_patches.size();
     if (!out_patches.empty() && !(b->d_out_patches = b->dupload_now(out_patches))) st = fail(WAE_OUT_OF_MEMORY, "out of device memory (output entries)");
-    if (st == WAE_OK) st = record_declarations(b, graphs, n_graphs, gps, curve_patches, iir_patches, sched_patches, loop_patches, loop_walks);
+    if (st == WAE_OK) st = record_declarations(b, graphs, n_graphs, gps, curve_patches, iir_patches, sched_patches, loop_patches, loop_walks, src_refs);
     if (st == WAE_OK) st = record_params(b, graphs, n_graphs, gps, slot_info, patches, spatial, spatial_resp);
     if (st != WAE_OK) {
         wae_batch_destroy(b);
@@ -5514,6 +5580,26 @@ static void derive_loop_tables(wae_batch* b) {
 }
 
 extern "C++" {
+// The rows of one bind call, staged as one table (Row: the kind's device item)
+template <typename Row>
+struct BindRows : std::vector<Row> {
+    wae_status stage(wae_batch* b) const { return stage_bind_table(b, this->data(), this->size() * sizeof(Row)); }
+};
+// wae_batch_bind_sources: the copied items (k_bind_sources), then one row per entry of the items read by reference (k_bind_source_refs)
+template <>
+struct BindRows<BindItem> {
+    std::vector<BindItem> copies;
+    std::vector<SrcRefBindItem> refs;
+    bool empty() const { return copies.empty() && refs.empty(); }
+    wae_status stage(wae_batch* b) const {
+        const size_t nc = copies.size() * sizeof(BindItem), nr = refs.size() * sizeof(SrcRefBindItem);
+        std::vector<char> t(nc + nr);
+        if (nc) std::memcpy(t.data(), copies.data(), nc);
+        if (nr) std::memcpy(t.data() + nc, refs.data(), nr);
+        return stage_bind_table(b, t.data(), t.size());
+    }
+};
+
 template <typename Item>
 static uint32_t param_of(const Item&) { return kNodeLevel; }
 static uint32_t param_of(const wae_param_binding& it) { return it.param_index; }
@@ -5529,7 +5615,7 @@ static wae_status bind_items(wae_batch* b, Bindings<D> wae_batch::*table, const 
     if (n == 0) return WAE_OK;
     CUDA_TRY(cudaSetDevice(b->engine->device));
     Bindings<D>& t = b->*table;
-    std::vector<Row> rows;
+    BindRows<Row> rows;
     std::vector<char> named(t.keys.size(), 0);
     BindExtents extents{b->engine->device, {}};
     for (uint32_t i = 0; i < n; i++) {
@@ -5550,7 +5636,7 @@ static wae_status bind_items(wae_batch* b, Bindings<D> wae_batch::*table, const 
     }
     if (!rows.empty()) {
         wae_status st = bind_after(b, stream);
-        if (st == WAE_OK) st = stage_bind_table(b, rows.data(), rows.size() * sizeof(Row));
+        if (st == WAE_OK) st = rows.stage(b);
         if (st != WAE_OK) return st;
         launch(static_cast<Row*>(b->d_bind), rows);
         cudaError_t le = cudaGetLastError();
@@ -5562,30 +5648,57 @@ static wae_status bind_items(wae_batch* b, Bindings<D> wae_batch::*table, const 
 }
 }  // extern "C++"
 
+static bool overlaps(const void* p, uint64_t p_bytes, const void* q, uint64_t q_bytes) {
+    return (uintptr_t)p < (uintptr_t)q + q_bytes && (uintptr_t)q < (uintptr_t)p + p_bytes;
+}
+
+// Copied items are copied into their slots (k_bind_sources); items read by reference have their pointer and stride written into the
+// records that play them (k_bind_source_refs), after the copies, from the same staged table
 WAE_API wae_status wae_batch_bind_sources(wae_batch* b, const wae_source_binding* items, uint32_t n, void* stream) {
-    return bind_items<BindItem>(
+    wae_status bs = bind_items<BindItem>(
         b, &wae_batch::sources, items, n, stream,
-        [](const wae_source_binding& it, const DevInput& d, size_t, BindExtents& extents, auto& rows) -> wae_status {
+        [b](const wae_source_binding& it, const DevInput& d, size_t, BindExtents& extents, auto& rows) -> wae_status {
             if (it.channel_stride < d.length)
                 return fail(WAE_INVALID_ARGUMENT, "bind: channel_stride " + std::to_string(it.channel_stride) + " is below the declared length " +
                                                       std::to_string(d.length));
             if (it.channel_stride > (UINT64_MAX / 4 - d.length) / WAE_MAX_CHANNELS)
                 return fail(WAE_INVALID_ARGUMENT, "bind: channel_stride runs past the end of its allocation");
-            wae_status st = extents.check(it.pcm, alignof(float), ((uint64_t)(d.channels - 1) * it.channel_stride + d.length) * sizeof(float), "pcm",
+            const uint64_t bytes = ((uint64_t)(d.channels - 1) * it.channel_stride + d.length) * sizeof(float);
+            wae_status st = extents.check(it.pcm, alignof(float), bytes, "pcm",
                                           "[pcm, pcm + (channels - 1) * channel_stride + length) runs past the end of its allocation");
-            if (st == WAE_OK && d.slot)
-                rows.push_back(BindItem{d.slot, it.pcm, (int64_t)d.stride, (int64_t)it.channel_stride, (int64_t)d.length, (int32_t)d.channels, 0});
-            return st;
+            if (st != WAE_OK) return st;
+            if (d.by_reference) {  // (the runs would read what they write)
+                const uint64_t out_bytes = (uint64_t)b->out_off[b->n_graphs] * sizeof(float);
+                if (overlaps(it.pcm, bytes, b->d_out, out_bytes) || (b->bound_out && overlaps(it.pcm, bytes, b->bound_out, out_bytes)))
+                    return fail(WAE_INVALID_ARGUMENT, "bind: the pcm of node " + std::to_string(it.node) + " of graph " +
+                                                          std::to_string(it.graph_index) + ", read by reference, overlaps the batch's output");
+                for (int32_t e = d.p0; e < d.p1; e++) rows.refs.push_back(SrcRefBindItem{it.pcm, (int64_t)it.channel_stride, e, 0});
+            } else if (d.slot) {
+                rows.copies.push_back(BindItem{d.slot, it.pcm, (int64_t)d.stride, (int64_t)it.channel_stride, (int64_t)d.length, (int32_t)d.channels, 0});
+            }
+            return WAE_OK;
         },
-        [b](const BindItem* dev, const std::vector<BindItem>& rows) {
+        [b](const BindItem* dev, const BindRows<BindItem>& rows) {
             int64_t max_vec = 0;
             int max_ch = 0;
-            for (const BindItem& r : rows) {
+            for (const BindItem& r : rows.copies) {
                 max_vec = std::max<int64_t>(max_vec, r.stride / 4);
                 max_ch = std::max<int>(max_ch, r.channels);
             }
-            launch_bind_sources(dev, (int)rows.size(), max_vec, max_ch, b->engine->stream);
+            if (!rows.copies.empty()) launch_bind_sources(dev, (int)rows.copies.size(), max_vec, max_ch, b->engine->stream);
+            if (!rows.refs.empty())
+                launch_bind_source_refs(reinterpret_cast<const SrcRefBindItem*>(dev + rows.copies.size()), (int)rows.refs.size(), b->d_src_refs,
+                                        b->engine->stream);
         });
+    if (bs != WAE_OK) return bs;
+    for (uint32_t i = 0; i < n; i++) {  // the memory each input read by reference now reads (bind_output must not overlap it)
+        DevInput& d = b->sources.data[b->sources.find({b->batch_pos(items[i].graph_index), items[i].node, kNodeLevel})];
+        if (d.by_reference) {
+            d.pcm = items[i].pcm;
+            d.pcm_stride = items[i].channel_stride;
+        }
+    }
+    return WAE_OK;
 }
 
 WAE_API wae_status wae_batch_bind_params(wae_batch* b, const wae_param_binding* items, uint32_t n, void* stream) {
@@ -5849,6 +5962,13 @@ WAE_API wae_status wae_batch_bind_output(wae_batch* b, float* out, uint64_t floa
         BindExtents extents{b->engine->device, {}};
         wae_status st = extents.check(out, 256, n * sizeof(float), "output", "the output runs past the end of its allocation");
         if (st != WAE_OK) return st;
+        for (size_t k = 0; k < b->sources.keys.size(); k++) {  // (the runs would write what they read)
+            const DevInput& d = b->sources.data[k];
+            if (d.by_reference && d.pcm && overlaps(out, n * sizeof(float), d.pcm, d.extent_bytes()))
+                return fail(WAE_INVALID_ARGUMENT, "bind_output: the output overlaps the memory node " + std::to_string(b->sources.keys[k].node) +
+                                                      " of graph " + std::to_string(b->order.empty() ? b->sources.keys[k].graph : b->order[b->sources.keys[k].graph]) +
+                                                      " reads by reference");
+        }
     }
     wae_status st = bind_after(b, stream);
     if (st != WAE_OK) return st;

@@ -61,6 +61,8 @@ struct PcmBuffer {  // an AudioBuffer asset (src/buffer.rs:69-72), host copy: ON
     // written into the device slab by wae_batch_bind_sources, and nothing copies host memory over it.  The response of a ConvolverNode
     // declared with wae_convolver_set_device_response is such a placeholder too: its spectra are written by wae_batch_bind_responses
     bool device_input = false;
+    // wae_buffer_source_set_device_input_by_reference: a device input read where the caller keeps it (no slab memory, nothing copied)
+    bool by_reference = false;
     PcmBuffer() = default;
     PcmBuffer(const PcmBuffer&) = delete;
     PcmBuffer& operator=(const PcmBuffer&) = delete;

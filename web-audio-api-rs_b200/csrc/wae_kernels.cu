@@ -4736,6 +4736,17 @@ __global__ void __launch_bounds__(128) k_bind_output(const OutPatch* __restrict_
     *e.dst = base + e.off;
 }
 
+// wae_batch_bind_sources, inputs declared by reference: every record that plays one now reads the caller's memory (pointer and channel
+// stride); no audio moves
+__global__ void __launch_bounds__(128) k_bind_source_refs(const SrcRefBindItem* __restrict__ items, int n, const SrcRefPatch* __restrict__ entries) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const SrcRefBindItem it = items[i];
+    const SrcRefPatch e = entries[it.entry];
+    *e.buf = it.pcm;
+    *e.stride = it.stride;
+}
+
 // Host emulation of the transforms above with the SAME butterfly, index and twiddle code (tests/test_conv_fft_host.py pins them against
 // numpy on a machine without a GPU).  mode 0: complex forward, natural -> position order; 1: complex inverse, position -> natural order
 // (unnormalised); 2: 2B reals -> B packed bins in position order; 3: B packed bins -> 2B reals (scaled by 1 / 2B).  data: 2B floats in place.
@@ -5358,6 +5369,9 @@ void launch_absn_loop_schedule(const LoopWalk* d, int n, int* overflow, cudaStre
 }
 void launch_bind_output(const OutPatch* d, int n, float* base, cudaStream_t s) {
     k_bind_output<<<(unsigned)((n + 127) / 128), 128, 0, s>>>(d, n, base);
+}
+void launch_bind_source_refs(const SrcRefBindItem* d, int n, const SrcRefPatch* entries, cudaStream_t s) {
+    k_bind_source_refs<<<(unsigned)((n + 127) / 128), 128, 0, s>>>(d, n, entries);
 }
 void launch_conv_ir_fft(const float* ir, int64_t ir_len, int64_t ir_stride, float2* h, int S, int channels, cudaStream_t s) {
     conv_configure();

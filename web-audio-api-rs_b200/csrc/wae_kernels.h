@@ -375,6 +375,9 @@ void launch_bind_loops(const LoopBindItem* d, int n, cudaStream_t s);
 void launch_absn_loop_schedule(const LoopWalk* d, int n, int* overflow, cudaStream_t s);
 // a bind of the output (k_bind_output, one thread per entry): base + off into each of the n output entries of a batch
 void launch_bind_output(const OutPatch* d, int n, float* base, cudaStream_t s);
+// the reference half of a bind of sources (k_bind_source_refs, one thread per row): each of the n rows writes its pointer and stride into
+// its entry of `entries`
+void launch_bind_source_refs(const SrcRefBindItem* d, int n, const SrcRefPatch* entries, cudaStream_t s);
 void launch_conv_ir_fft(const float* ir, int64_t ir_len, int64_t ir_stride, float2* h, int S, int channels, cudaStream_t s);
 
 }  // namespace wae
