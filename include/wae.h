@@ -436,6 +436,28 @@ WAE_API wae_status wae_batch_stage_time(wae_batch* batch, uint32_t index, char* 
 WAE_API wae_status wae_analyser_get_float_time_domain_data(wae_batch*, uint32_t graph_index, wae_node_id node, float* out, uint32_t len);
 WAE_API wae_status wae_analyser_get_float_frequency_data(wae_batch*, uint32_t graph_index, wae_node_id node, float* out, uint32_t len);
 
+/* AnalyserNode read-outs at declared render times, taken on the GPU during a run of a prepared batch.
+ *
+ * wae_analyser_set_readouts declares read-outs at `times` (seconds, n >= 1, non-decreasing).  Each time is quantised as
+ * suspend_sync quantises it (q = ceil(t * sampleRate / 128), offline.rs:248-251, 0 <= q <= the graph's whole quanta): read-out k
+ * is what Analyser::get_float_frequency_data / get_float_time_domain_data return in a suspend callback at quantum q, i.e. at
+ * current_time = q * 128 / sampleRate over the fftSize frames before frame q * 128 (frames before the render are zeros).
+ * Frequency read-outs smooth in time order from a zero state each run; two read-outs on one quantum give the same row.  The
+ * post-render wae_analyser_get_float_frequency_data continues that smoothing.  `kinds`: WAE_READOUT_* bits.
+ * Refused: a node that is not an analyser, n == 0, a negative / non-finite / decreasing time, a quantum past the render, kinds
+ * 0 or unknown bits (WAE_INVALID_ARGUMENT); a second declaration on the node or a graph with a suspend point
+ * (WAE_INVALID_STATE; wae_graph_suspend refuses a graph with a declaration).  One-shot renders refuse declared graphs.
+ *
+ * After a run: wae_batch_analyser_readouts_device_ptr gives the device memory of one (node, kind) over the whole batch, graphs
+ * in the order they were passed to prepare, each [k][row] (row = fftSize / 2 dB values or fftSize samples; a graph without the
+ * declaration takes no space), `floats` in all; wae_batch_fetch_analyser_readouts copies one graph's [k][row] to the host
+ * (`floats` must be K * row).  Each run overwrites the rows. */
+enum { WAE_READOUT_FREQUENCY = 1, WAE_READOUT_TIME_DOMAIN = 2 };
+WAE_API wae_status wae_analyser_set_readouts(wae_graph* graph, wae_node_id node, const double* times, uint32_t n, uint32_t kinds);
+WAE_API wae_status wae_batch_analyser_readouts_device_ptr(wae_batch* batch, wae_node_id node, uint32_t kind, float** ptr, uint64_t* floats);
+WAE_API wae_status wae_batch_fetch_analyser_readouts(wae_batch* batch, uint32_t graph_index, wae_node_id node, uint32_t kind, float* host_out,
+                                                     uint64_t floats);
+
 /* load_hrtf_processor (src/node/panner.rs:39-68): the HRIR sphere the reference embeds with include_bytes!
  * ("resources/IRC_1003_C.bin": "HRIR" | u32 rate | u32 taps | u32 #vertices | u32 #indices | indices | per vertex xyz,
  * left[taps], right[taps]).  Must be set before a batch with PanningModelType::HRTF panners is prepared; contexts whose

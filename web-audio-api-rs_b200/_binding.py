@@ -190,6 +190,8 @@ CREATE_FUNCS = {
     "create_channel_splitter": ChannelSplitterOptions,
 }
 
+READOUT_FREQUENCY, READOUT_TIME_DOMAIN = 1, 2  # WAE_READOUT_*
+
 # every symbol include/wae.h declares (tests check the product exports all of them)
 WAE_SYMBOLS = [
     "wae_engine_create", "wae_engine_destroy", "wae_last_error", "wae_version", "wae_engine_set_option", "wae_engine_stream",
@@ -214,6 +216,7 @@ WAE_SYMBOLS = [
     "wae_source_set_device_schedule", "wae_batch_bind_schedules", "wae_buffer_source_set_device_offset",
     "wae_buffer_source_set_device_loop", "wae_batch_bind_loops",
     "wae_batch_bind_output",
+    "wae_analyser_set_readouts", "wae_batch_analyser_readouts_device_ptr", "wae_batch_fetch_analyser_readouts",
 ]
 
 
@@ -345,6 +348,10 @@ class Api:
             f("batch_bind_loops", C.c_int32, [C.c_void_p, C.POINTER(LoopBinding), C.c_uint32, C.c_void_p])
             # rendered PCM written to caller device memory
             f("batch_bind_output", C.c_int32, [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p])
+            # analyser read-outs at declared render times
+            f("analyser_set_readouts", C.c_int32, [gp, C.c_uint32, c_double_p, C.c_uint32, C.c_uint32])
+            f("batch_analyser_readouts_device_ptr", C.c_int32, [C.c_void_p, C.c_uint32, C.c_uint32, C.POINTER(c_float_p), C.POINTER(C.c_uint64)])
+            f("batch_fetch_analyser_readouts", C.c_int32, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, c_float_p, C.c_uint64])
         else:
             f("graph_create", C.c_int32, [C.c_uint32, C.c_uint64, C.c_float, C.POINTER(C.c_void_p)])
             f("render", C.c_int32, [gp, c_float_p])

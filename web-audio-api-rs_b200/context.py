@@ -531,6 +531,26 @@ class AnalyserNode(AudioNode):
     def get_byte_frequency_data(self, n=None, out=None):
         return self._ctx._analyser_read(self, "freq", n or self.fft_size // 2, byte=True, out=out)
 
+    # wae_analyser_set_readouts: read-outs taken on the GPU during the render, at `times` (seconds, non-decreasing), each quantised
+    # like a suspend_sync callback's (ceil(t * sampleRate / 128) quanta); fftSize and the smoothing are the node's at render time
+    def set_readouts(self, times, frequency=True, time_domain=False):
+        times = np.ascontiguousarray(times, np.float64).reshape(-1)
+        kinds = (B.READOUT_FREQUENCY if frequency else 0) | (B.READOUT_TIME_DOMAIN if time_domain else 0)
+        api = self._ctx._api
+        if not api.is_product:
+            raise B.WaeError(4, "analyser read-outs are taken by the GPU engine")
+        api.check(api.analyser_set_readouts(self._ctx._g, self.id, times.ctypes.data_as(B.c_double_p), len(times), kinds))
+        self._readouts = len(times)
+        self._ctx._readout_nodes[self.id] = self
+
+    def get_float_frequency_readouts(self):
+        """[K][fftSize / 2] dB of the declared read-outs of the last render"""
+        return self._ctx._readouts(self, B.READOUT_FREQUENCY, self.fft_size // 2)
+
+    def get_float_time_domain_readouts(self):
+        """[K][fftSize] samples of the declared read-outs of the last render"""
+        return self._ctx._readouts(self, B.READOUT_TIME_DOMAIN, self.fft_size)
+
 
 class AudioListener:
     def __init__(self, ctx):
@@ -560,6 +580,7 @@ class OfflineAudioContext:
         self._batch_index = 0
         self._listener = None
         self._suspends = []
+        self._readout_nodes = {}  # node id -> AnalyserNode with declared read-outs (set_readouts)
         self._current_time = 0.0
         self._device_inputs = {}  # node id -> (channels, length) declared with set_device_input
         self._source_refs = set()  # ids of the device inputs declared by_reference
@@ -750,6 +771,14 @@ class OfflineAudioContext:
         """OfflineAudioContext::start_rendering_sync (src/context/offline.rs:157-185): a batch of one."""
         return render_batch([self])[0]
 
+    def _readouts(self, node, kind, row):
+        if self._batch is None:
+            raise B.WaeError(2, "analyser read-outs are available after rendering")
+        k = getattr(node, "_readouts", 0)
+        out = np.empty((k, row), np.float32)
+        self._api.check(self._api.batch_fetch_analyser_readouts(self._batch.handle, self._batch_index, node.id, kind, B.fptr(out), out.size))
+        return out
+
     def _analyser_read(self, node, kind, n, byte=False, out=None):
         if out is None:
             out = np.zeros(n, np.uint8 if byte else np.float32)
@@ -767,6 +796,13 @@ class OfflineAudioContext:
         else:
             api.check(fn(self._g, node.id, ptr, n))
         return out
+
+
+def _readout_kind(kind):
+    kinds = {"frequency": B.READOUT_FREQUENCY, "time_domain": B.READOUT_TIME_DOMAIN}
+    if kind not in kinds:
+        raise B.WaeError(1, f"kind must be one of {sorted(kinds)}")
+    return kinds[kind]
 
 
 class Batch:
@@ -790,6 +826,7 @@ class Batch:
         self._views_out = False  # output_tensor was called: runs into the batch's own buffer are ordered after torch's current stream
         self._out = None  # bind_output: the tensor runs write
         self._out_viewed = False  # output_tensor handed out views of the bound tensor since it was bound: runs into it wait for torch
+        self._readouts_viewed = False  # analyser_readouts handed out views of the read-out rows: every run (bound output or not) waits for torch
         self._src_refs = {}  # bind_sources: (graph, node id) -> the tensor a device input declared by_reference reads
         self._ref_tensors = []  # the distinct tensors of _src_refs
         self._has_refs = any(c._source_refs for c in contexts)
@@ -886,8 +923,9 @@ class Batch:
         """A run overwrites the device output: once output_tensor views of the buffer it writes were handed out, order it after the work
         torch has queued so far on its current stream (the readers of the last output).  Views of another buffer do not hold a run into a
         bound output up: bind_output ordered it after the work queued before the bind, and the readers of the other buffer may run while it
-        renders."""
-        if (self._views_out and self._out is None) or (self._out_viewed and self._out is not None):
+        renders.  Views of the analyser read-out rows hold every run up: the rows are the batch's own memory whether or not an output is
+        bound, and every run rewrites them."""
+        if (self._views_out and self._out is None) or (self._out_viewed and self._out is not None) or self._readouts_viewed:
             import torch
             self._engine_stream().wait_stream(torch.cuda.current_stream(self._device()))
 
@@ -1255,6 +1293,35 @@ class Batch:
             shape = (ch, length)
         view = torch.as_tensor(_DeviceView(self, base + 4 * off, shape), device=self._device())
         self._views_out = True
+        torch.cuda.current_stream(self._device()).wait_stream(self._engine_stream())
+        return view
+
+    def analyser_readouts(self, node, kind="frequency"):
+        """Zero-copy torch view [n][K][row] of the declared read-outs (AnalyserNode.set_readouts) of `node` (an AnalyserNode of context 0,
+        or its id) over the batch, when every context declares them alike on the same node id; otherwise fetch them per context
+        (AnalyserNode.get_float_frequency_readouts / get_float_time_domain_readouts).  Ordered like output_tensor: torch's current
+        stream waits for the engine stream, and later runs, which overwrite the rows, wait for the work then queued on torch's stream."""
+        import torch
+        kind_id = _readout_kind(kind)
+        node_id = int(getattr(node, "id", node))
+        p, floats = B.c_float_p(), C.c_uint64()
+        self.api.check(self.api.batch_analyser_readouts_device_ptr(self.handle, node_id, kind_id, C.byref(p), C.byref(floats)))
+        if floats.value % self.n:
+            raise B.WaeError(2, "analyser_readouts: the contexts declare different read-outs on this node; fetch them per context")
+        per = floats.value // self.n
+        shapes = set()
+        for c in self.contexts:
+            a = c._readout_nodes.get(node_id)
+            shapes.add(None if a is None else (a._readouts, a.fft_size))
+        k = shapes.pop() if len(shapes) == 1 else None
+        if k is None:
+            raise B.WaeError(2, "analyser_readouts: the contexts declare different read-outs on this node; fetch them per context")
+        row = k[1] // 2 if kind_id == B.READOUT_FREQUENCY else k[1]
+        if k[0] * row != per:
+            raise B.WaeError(2, "analyser_readouts: the contexts declare different read-outs on this node; fetch them per context")
+        addr = C.cast(p, C.c_void_p).value
+        view = torch.as_tensor(_DeviceView(self, addr, (self.n, k[0], row)), device=self._device())
+        self._readouts_viewed = True
         torch.cuda.current_stream(self._device()).wait_stream(self._engine_stream())
         return view
 

@@ -701,6 +701,8 @@ WAE_API wae_status wae_graph_suspend(wae_graph* g, double suspend_time) {
         return fail(WAE_INVALID_STATE, "InvalidStateError - the graph has schedules bound from device memory (wae_source_set_device_schedule)");
     if (g->device_loops)  // (the reference allows loop changes after start, which suspend points do not lower)
         return fail(WAE_INVALID_STATE, "InvalidStateError - the graph has loop points bound from device memory (wae_buffer_source_set_device_loop)");
+    if (g->analyser_readouts)  // (read-outs are taken on the GPU; suspend callbacks run on the host before the render)
+        return fail(WAE_INVALID_STATE, "InvalidStateError - the graph has analyser read-outs declared (wae_analyser_set_readouts)");
     g->epochs.push_back(wae_graph::Epoch{quantum * 128, g->nodes});
     return WAE_OK;
 }
@@ -1045,6 +1047,35 @@ WAE_API wae_status wae_source_set_device_schedule(wae_graph* g, wae_node_id node
         n->sched_hi[1] = stop_hi;
     }
     g->device_schedules++;
+    return WAE_OK;
+}
+
+// AnalyserNode read-outs taken during the render at declared times, each quantised like suspend_sync (offline.rs:248-251).  The
+// suspend points a graph with read-outs would need are exactly what it does without: a graph has one or the other.
+WAE_API wae_status wae_analyser_set_readouts(wae_graph* g, wae_node_id node, const double* times, uint32_t n, uint32_t kinds) {
+    if (!g) return fail(WAE_INVALID_ARGUMENT, "null graph");
+    Node* a = g->nodes.get(node);
+    if (!a || a->kind != K_ANALYSER) return fail(WAE_INVALID_ARGUMENT, "not an AnalyserNode");
+    if (n == 0 || !times) return fail(WAE_INVALID_ARGUMENT, "no read-out times");
+    if (kinds == 0 || (kinds & ~(uint32_t)(WAE_READOUT_FREQUENCY | WAE_READOUT_TIME_DOMAIN)))
+        return fail(WAE_INVALID_ARGUMENT, "kinds must be a non-empty set of WAE_READOUT_FREQUENCY | WAE_READOUT_TIME_DOMAIN");
+    const uint64_t total = (g->length + 127) / 128;
+    std::vector<uint64_t> q(n);
+    for (uint32_t k = 0; k < n; k++) {
+        if (!std::isfinite(times[k]) || times[k] < 0.)
+            return fail(WAE_INVALID_ARGUMENT, "RangeError - read-out time " + std::to_string(k) + " is negative or not finite");
+        if (k > 0 && times[k] < times[k - 1])
+            return fail(WAE_INVALID_ARGUMENT, "RangeError - read-out times must not decrease (time " + std::to_string(k) + ")");
+        const double qd = std::ceil(times[k] * (double)g->sample_rate / 128.);
+        if (qd > (double)total)
+            return fail(WAE_INVALID_ARGUMENT, "RangeError - read-out time " + std::to_string(k) + " is after the end of the rendering");
+        q[k] = (uint64_t)qd;
+    }
+    if (a->readout_kinds) return fail(WAE_INVALID_STATE, "InvalidStateError - the analyser already has read-outs declared");
+    if (!g->epochs.empty()) return fail(WAE_INVALID_STATE, "InvalidStateError - analyser read-outs are declared in a graph with a suspend point");
+    a->readout_q = std::move(q);
+    a->readout_kinds = kinds;
+    g->analyser_readouts++;
     return WAE_OK;
 }
 

@@ -312,6 +312,30 @@ struct AnalyserInst {
     int64_t end;  // the graph's last rendered frame + 1: the ring is not written from there on (a shorter graph of a longer group)
 };
 
+// One declared analyser read-out (wae_analyser_set_readouts) at frame F = q * 128: its window is the fftSize mono frames before F,
+// taken from the ring for frames < f0 and from the input buffer for [f0, F) by the read-out kernels of the chunk (f0, f0 + nf] holding F
+// (F = 0: the first chunk), which run before k_analyser writes that chunk into the ring.  A stage's records are sorted by F.
+struct ReadoutInst {
+    BufRef in;            // the analyser's input (AnalyserInst::in)
+    const float* ring;    // the analyser's ring (AnalyserInst::ring)
+    float* row;           // frequency: fftSize / 2 linear magnitudes (dB after k_readout_smooth); time domain: fftSize samples
+    int64_t frame;        // F
+    int32_t ch;
+    int32_t fft_size;
+};
+
+// The frequency read-outs of one analyser, for k_readout_smooth: one thread per bin walks those of a chunk in time order
+struct ReadoutSmoothInst {
+    const int64_t* frames;  // [K] F of each read-out, non-decreasing
+    float* rows;            // [K][bins]
+    float* last_fft;        // the analyser's smoothing state (AnalyserRec::d_last_fft), zeroed per run
+    float* db;              // the analyser's post-render read-out (AnalyserRec::d_db): the last row's dB
+    int32_t n;              // K
+    int32_t bins;
+    float smoothing;
+    int32_t pad;
+};
+
 
 struct RouteInst {  // channel merger / splitter: copy one channel
     BufRef in, out;

@@ -248,12 +248,13 @@ namespace {
 // (the order of the kinds is the launch order inside one level: mixes first; k_delay_mono before the delay reader that needs it)
 enum StageKind : int {
     S_MIX = 0, S_MIX_DYN, S_OSC, S_CONST, S_ABSN, S_BIQUAD, S_IIR, S_GAIN, S_SHAPER, S_SPAN, S_PAN, S_ROUTE, S_DELAY_MONO, S_DELAY, S_DELAY_WRITE, S_COMP, S_ANALYSER,
-    S_CONV_FFT, S_CONV_MAC, S_CONV_MAC_ACC, S_CHAIN, S_PARAM, S_OSC_AR, S_BIQUAD_AR, S_ABSN_SLOW, S_HRTF, S_PAN_DYN, S_ABSN_SERIAL, S_SHAPER_OS, S_META, S_VSUM, S_CONV_CMP, S_ABSN_BOUND, S_KINDS
+    S_CONV_FFT, S_CONV_MAC, S_CONV_MAC_ACC, S_CHAIN, S_PARAM, S_OSC_AR, S_BIQUAD_AR, S_ABSN_SLOW, S_HRTF, S_PAN_DYN, S_ABSN_SERIAL, S_SHAPER_OS, S_META, S_VSUM, S_CONV_CMP, S_ABSN_BOUND,
+    S_READOUT_FFT, S_READOUT_TIME, S_READOUT_SMOOTH, S_KINDS  // (launched before S_ANALYSER of their level: Planner::stage)
 };
 const char* kStageNames[S_KINDS] = {"k_mix", "k_mix_dyn", "k_oscillator", "k_constant", "k_buffer_source", "k_biquad_serial", "k_iir_serial", "k_gain",
                                     "k_shaper", "k_stereo_panner", "k_panner_eq", "k_route", "k_delay_mono", "k_delay_read", "k_ring_write", "k_compressor",
                                     "k_analyser", "k_conv_fft_in", "k_conv_mac_ifft", "k_conv_mac_ifft(acc)", "k_chain", "k_param", "k_osc_arate", "k_biquad_arate", "k_buffer_source_slow", "k_hrtf_fir", "k_panner_dyn", "k_buffer_source_serial", "k_shaper_os", "k_meta", "k_voice_sum", "k_conv_compact",
-                                    "k_buffer_source_slow(bound)"};
+                                    "k_buffer_source_slow(bound)", "k_readout_fft", "k_readout_time", "k_readout_smooth"};
 
 // host-side accumulation of instances for one (level, kind) stage
 struct StageBuild {
@@ -294,6 +295,8 @@ struct StageBuild {
     std::vector<DelayInst> delay;
     std::vector<CompInst> comp;
     std::vector<AnalyserInst> analyser;
+    std::vector<ReadoutInst> readout;                // S_READOUT_FFT / S_READOUT_TIME
+    std::vector<ReadoutSmoothInst> readout_smooth;  // S_READOUT_SMOOTH
     std::vector<MixInst> mix;
     std::vector<MixEdge> mix_edges;
     std::vector<MixDynInst> mix_dyn;
@@ -472,6 +475,7 @@ struct Stage {
     void* d_a = nullptr;  // instances
     void* d_b = nullptr;  // auxiliary table (mix edges, scan coefficients, conv inputs, panner gains)
     void* d_c = nullptr;  // S_VSUM: voice groups
+    std::vector<int64_t> frames;  // S_READOUT_FFT / S_READOUT_TIME: the records' frames (sorted); a chunk launches those it holds
     float ms = 0.f;       // accumulated device time of the last run (when timing is enabled)
     ChainAux chain;       // S_CHAIN with biquads: ticket counter + slab hand-off slots (k_chain)
 };
@@ -487,6 +491,16 @@ struct AnalyserRec {
     bool computed;      // frequency data already computed for the end-of-render time (analysis.rs:353-361)
     double min_db, max_db;
     int64_t lq;         // frames the graph renders (its own length padded to whole quanta): the ring's write index after the render
+    bool end_readout = false;  // its last declared frequency read-out is at lq: each run leaves that row in d_db, computed
+};
+
+// The rows of the declared read-outs (wae_analyser_set_readouts) of one (node id, kind) over the batch: one allocation, graphs in the
+// caller's order, each [k][row]
+struct ReadoutOut {
+    float* d = nullptr;
+    uint64_t floats = 0;
+    std::vector<uint64_t> off;  // [batch position] first float of the graph's rows, or UINT64_MAX: not declared there
+    std::vector<uint64_t> len;  // [batch position] floats of the graph's rows
 };
 
 // One kind of input a prepared batch takes from device memory, as messages name it
@@ -669,6 +683,7 @@ struct wae_batch {
     // state that must be reset before every run
     std::vector<std::pair<void*, size_t>> zero_on_run;
     std::vector<AnalyserRec> analysers;
+    std::map<std::pair<wae_node_id, uint32_t>, ReadoutOut> readout_outs;  // (node, WAE_READOUT_*) -> rows
     struct CompRec { uint32_t graph; wae_node_id node; const float* d_state; };
     std::vector<CompRec> compressors;
     // source PCM assets: device destination <- host source (re-uploadable: wae_batch_upload)
@@ -1265,7 +1280,9 @@ struct Planner {
     int cur_cls = 0;  // class of the node being planned
     StageBuild& stage(int level, int kind, int variant = 0) {
         const int cls = cur_cls;
-        StageBuild& s = builds[{cls * 1000000 + level, kind * 64 + variant}];
+        // the read-out stages run right before k_analyser of their level, which then writes the chunk into the ring
+        const int order = kind >= S_READOUT_FFT ? S_ANALYSER * 64 - 3 + (kind - S_READOUT_FFT) : kind * 64 + variant;
+        StageBuild& s = builds[{cls * 1000000 + level, order}];
         s.cls = cls;
         s.level = level;
         s.kind = kind;
@@ -1648,6 +1665,7 @@ struct Planner {
     bool lower_delay_reader(NodeCtx& nc);
     bool lower_compressor(NodeCtx& nc);
     bool lower_analyser(NodeCtx& nc);
+    bool lower_readouts(NodeCtx& nc, const AnalyserInst& a, float* last, float* db);
     bool lower_merger(NodeCtx& nc);
     bool lower_splitter(NodeCtx& nc);
     bool lower_convolver(NodeCtx& nc);
@@ -1741,6 +1759,8 @@ static uint64_t digest_builds(const std::map<std::pair<int, int>, StageBuild>& b
         if (!s.conv_cmp.empty())
             h = digest_vec_skipping(s.conv_cmp, {offsetof(ConvCmpInst, x) + offsetof(ConvInput, end), offsetof(ConvCmpInst, path) + offsetof(ConvPath, end)}, h);  // (only where it exists: the digests of plans without it stay comparable)
         if (!s.absn_bound.empty()) h = digest_vec(s.absn_bound, h);  // (the same)
+        if (!s.readout.empty()) h = digest_vec(s.readout, h);
+        if (!s.readout_smooth.empty()) h = digest_vec(s.readout_smooth, h);
     }
     return h;
 }
@@ -1814,6 +1834,7 @@ static void merge_builds(Builds& dst, Builds& src) {
         append_vec(d.mix_edges, s.mix_edges); append_vec(d.mix_dyn, s.mix_dyn); append_vec(d.meta, s.meta); append_vec(d.conv_in, s.conv_in);
         append_vec(d.conv_path, s.conv_path); append_vec(d.vgroups, s.vgroups); append_vec(d.conv_cmp, s.conv_cmp);
         append_vec(d.absn_bound, s.absn_bound);
+        append_vec(d.readout, s.readout); append_vec(d.readout_smooth, s.readout_smooth);
         append_vec(d.patches, s.patches);
         append_vec(d.curve_patches, s.curve_patches);
         append_vec(d.iir_patches, s.iir_patches);
@@ -3716,18 +3737,55 @@ bool Planner::lower_analyser(NodeCtx& nc) {
     a.ring = alloc<float>(32768 + 128, true, true);
     if (!a.ring) return bail(WAE_OUT_OF_MEMORY, "out of device memory (analyser ring)");
     stage(nc.L, S_ANALYSER).analyser.push_back(a);
-    {
-        float* last = alloc<float>(16384, true, true);
-        float* db = alloc<float>(16384);
-        if (!last || !db) return bail(WAE_OUT_OF_MEMORY, "out of device memory (analyser)");
-        if (!dry) {
-            std::lock_guard<std::recursive_mutex> lk(b->mu);
-            bool known = false;
-            for (auto& r : b->analysers) known = known || (r.graph_index == gi && r.node == nc.id);
-            if (!known) b->analysers.push_back(AnalyserRec{gi, nc.id, a.ring, n.fft_size, n.smoothing, last, db, false, n.min_db, n.max_db, glq});
+    float* last = alloc<float>(16384, true, true);
+    float* db = alloc<float>(16384);
+    if (!last || !db) return bail(WAE_OUT_OF_MEMORY, "out of device memory (analyser)");
+    const bool freq = (n.readout_kinds & WAE_READOUT_FREQUENCY) != 0;
+    if (!dry) {
+        std::lock_guard<std::recursive_mutex> lk(b->mu);
+        bool known = false;
+        for (auto& r : b->analysers) known = known || (r.graph_index == gi && r.node == nc.id);
+        if (!known) {
+            b->analysers.push_back(AnalyserRec{gi, nc.id, a.ring, n.fft_size, n.smoothing, last, db, false, n.min_db, n.max_db, glq});
+            b->analysers.back().end_readout = freq && (int64_t)n.readout_q.back() * 128 == glq;
         }
     }
     algorithmic_bytes += (uint64_t)lq * 4;  // ring write, SURVEY §8(d)
+    if (n.readout_kinds) return lower_readouts(nc, a, last, db);
+    return true;
+}
+
+// The declared read-outs of an analyser (wae_analyser_set_readouts): one record per distinct frequency read-out frame (a read-out on
+// the quantum of the one before repeats its row: k_readout_smooth copies it), one per time-domain read-out, and the analyser's
+// smoothing walk.  Their rows are the batch's ReadoutOut of (node, kind).
+bool Planner::lower_readouts(NodeCtx& nc, const AnalyserInst& a, float* last, float* db) {
+    const Node& n = nc.n;
+    const std::vector<uint64_t>& q = n.readout_q;
+    const int K = (int)q.size();
+    std::vector<int64_t> frames(K);
+    for (int k = 0; k < K; k++) frames[k] = (int64_t)q[k] * 128;
+    auto rows = [&](uint32_t kind) -> float* {
+        if (dry) return reinterpret_cast<float*>(dry_addr());
+        auto it = b->readout_outs.find({nc.id, kind});
+        return it == b->readout_outs.end() || !it->second.d ? nullptr : it->second.d + it->second.off[gi];
+    };
+    for (uint32_t kind : {(uint32_t)WAE_READOUT_FREQUENCY, (uint32_t)WAE_READOUT_TIME_DOMAIN}) {
+        if (!(n.readout_kinds & kind)) continue;
+        float* base = rows(kind);
+        if (!base) return bail(WAE_INVALID_STATE, "analyser read-out rows missing");
+        const bool f = kind == WAE_READOUT_FREQUENCY;
+        const uint32_t row = f ? n.fft_size / 2 : n.fft_size;
+        StageBuild& sb = stage(nc.L, f ? S_READOUT_FFT : S_READOUT_TIME);
+        for (int k = 0; k < K; k++) {
+            if (f && k > 0 && frames[k] == frames[k - 1]) continue;
+            sb.readout.push_back(ReadoutInst{a.in, a.ring, base + (size_t)k * row, frames[k], a.ch, (int32_t)n.fft_size});
+        }
+        if (f) {
+            const int64_t* d_frames = upload(frames);
+            if (!d_frames) return bail(WAE_OUT_OF_MEMORY, "out of device memory (read-out frames)");
+            stage(nc.L, S_READOUT_SMOOTH).readout_smooth.push_back(ReadoutSmoothInst{d_frames, base, last, db, K, (int32_t)row, (float)n.smoothing, 0});
+        }
+    }
     return true;
 }
 
@@ -4747,6 +4805,23 @@ static void prep_plan_group(wae_batch* b, wae_graph* const* graphs, int k, PrepS
                 case S_DELAY_WRITE: st.n = (int)s.delay.size(); st.d_a = up(b, s.delay); break;
                 case S_COMP: st.n = (int)s.comp.size(); st.d_a = up(b, s.comp); break;
                 case S_ANALYSER: st.n = (int)s.analyser.size(); st.d_a = up(b, s.analyser); break;
+                case S_READOUT_FFT:
+                case S_READOUT_TIME: {
+                    std::vector<ReadoutInst> r = s.readout;
+                    std::stable_sort(r.begin(), r.end(), [](const ReadoutInst& x, const ReadoutInst& y) { return x.frame < y.frame; });
+                    st.n = (int)r.size();
+                    st.d_a = up(b, r);
+                    for (const ReadoutInst& x : r) {
+                        st.frames.push_back(x.frame);
+                        st.n_b = std::max(st.n_b, (int)x.fft_size);
+                    }
+                    break;
+                }
+                case S_READOUT_SMOOTH:
+                    st.n = (int)s.readout_smooth.size();
+                    st.d_a = up(b, s.readout_smooth);
+                    for (const ReadoutSmoothInst& x : s.readout_smooth) st.n_b = std::max(st.n_b, (int)x.bins);
+                    break;
                 case S_CONV_FFT: st.n = (int)s.conv_in.size(); st.d_a = up(b, s.conv_in); last_conv_inputs = st.d_a; break;
                 case S_CONV_CMP: st.n = (int)s.conv_cmp.size(); st.d_a = up(b, s.conv_cmp); break;
                 case S_CONV_MAC:
@@ -5060,6 +5135,33 @@ static wae_status prep_finish(wae_batch* b, PrepState& ps) {
     return WAE_OK;
 }
 
+// The rows of every declared analyser read-out (wae_analyser_set_readouts), before planning: the planner points the records at them.
+// `graphs` in batch order; the rows of one (node, kind) are laid out in the caller's order.
+static wae_status alloc_readout_rows(wae_batch* b, wae_graph* const* graphs, uint32_t n_graphs) {
+    for (uint32_t c = 0; c < n_graphs; c++) {
+        const uint32_t j = b->batch_pos(c);
+        if (!graphs[j]->analyser_readouts) continue;
+        for (const auto& kv : graphs[j]->nodes) {
+            const Node& n = kv.second;
+            if (n.kind != K_ANALYSER || !n.readout_kinds) continue;
+            for (uint32_t kind : {(uint32_t)WAE_READOUT_FREQUENCY, (uint32_t)WAE_READOUT_TIME_DOMAIN}) {
+                if (!(n.readout_kinds & kind)) continue;
+                ReadoutOut& r = b->readout_outs[{kv.first, kind}];
+                if (r.off.empty()) {
+                    r.off.assign(n_graphs, UINT64_MAX);
+                    r.len.assign(n_graphs, 0);
+                }
+                r.off[j] = r.floats;
+                r.len[j] = (uint64_t)n.readout_q.size() * (kind == WAE_READOUT_FREQUENCY ? n.fft_size / 2 : n.fft_size);
+                r.floats += r.len[j];
+            }
+        }
+    }
+    for (auto& kv : b->readout_outs)
+        if (!(kv.second.d = b->dalloc<float>(kv.second.floats))) return fail(WAE_OUT_OF_MEMORY, "out of device memory (analyser read-outs)");
+    return WAE_OK;
+}
+
 // `plan` != nullptr: planning only — grouping, the sizing pass of the planner (which touches no device memory) and the chunk choice,
 // reported through *plan; nothing is allocated and no CUDA call is made (wae_batch_plan: runs without a GPU).
 static wae_status prepare_impl(wae_engine* eng, wae_graph* const* graphs, uint32_t n_graphs, wae_batch** out, wae_plan_info* plan,
@@ -5070,6 +5172,11 @@ static wae_status prepare_impl(wae_engine* eng, wae_graph* const* graphs, uint32
     wae_status st = prep_begin(eng, graphs, n_graphs, plan, &b, ps, true, order);
     if (st != WAE_OK || plan) return st;
     record_device_inputs(b, graphs, n_graphs);
+    st = alloc_readout_rows(b, graphs, n_graphs);
+    if (st != WAE_OK) {
+        wae_batch_destroy(b);
+        return st;
+    }
     const int n_groups = (int)b->groups.size();
     std::vector<GroupPlan> gps(n_groups);
     WorkerPool* pool = (n_groups > 1 && n_graphs >= 64) ? eng->workers() : nullptr;
@@ -5239,6 +5346,18 @@ static void launch_stage(wae_batch* b, Stage& st, ChunkInfo ci) {
         case S_DELAY_WRITE: launch_ring_write((DelayInst*)st.d_a, st.n, ci, s); break;
         case S_COMP: launch_compressor((CompInst*)st.d_a, st.n, ci, s); break;
         case S_ANALYSER: launch_analyser((AnalyserInst*)st.d_a, st.n, ci, s); break;
+        case S_READOUT_FFT:
+        case S_READOUT_TIME: {  // the records with f0 < frame <= f0 + nf (frame 0: the first chunk)
+            const int64_t lo = ci.f0 == 0 ? -1 : ci.f0;
+            const size_t r0 = std::upper_bound(st.frames.begin(), st.frames.end(), lo) - st.frames.begin();
+            const size_t r1 = std::upper_bound(st.frames.begin(), st.frames.end(), ci.f0 + ci.nf) - st.frames.begin();
+            if (r1 <= r0) break;
+            const ReadoutInst* d = (const ReadoutInst*)st.d_a + r0;
+            if (st.kind == S_READOUT_FFT) launch_readout_fft(d, (int)(r1 - r0), st.n_b, ci, s);
+            else launch_readout_time(d, (int)(r1 - r0), st.n_b, ci, s);
+            break;
+        }
+        case S_READOUT_SMOOTH: launch_readout_smooth((ReadoutSmoothInst*)st.d_a, st.n, st.n_b, ci, s); break;
         case S_CONV_FFT: launch_conv_fft_in((ConvInput*)st.d_a, st.n, ci, s); break;
         case S_CONV_MAC:
         case S_CONV_MAC_ACC: launch_conv_mac_ifft((ConvPath*)st.d_a, (ConvInput*)st.d_b, st.n, ci, s); break;
@@ -5374,7 +5493,7 @@ static wae_status begin_run(wae_batch* b) {
     for (auto& z : b->zero_on_run) CUDA_TRY(cudaMemsetAsync(z.first, 0, z.second, s));
     b->timed.clear();
     b->timed_events_used = 0;
-    for (auto& a : b->analysers) a.computed = false;
+    for (auto& a : b->analysers) a.computed = a.end_readout;
     CUDA_TRY(cudaEventRecord(b->ev0, s));
     return WAE_OK;
 }
@@ -6368,11 +6487,15 @@ WAE_API wae_status wae_selftest_conv_fft(float* data, uint32_t mode) {
 
 // a one-shot call renders the graphs before a caller could bind anything to their declarations
 static wae_status refuse_device_inputs(wae_graph* const* graphs, uint32_t n_graphs) {
-    for (uint32_t i = 0; graphs && i < n_graphs; i++)
+    for (uint32_t i = 0; graphs && i < n_graphs; i++) {
         for (const BindKind& kind : kBindKinds)
             if (graphs[i] && graphs[i]->*kind.count)
                 return fail(WAE_INVALID_STATE, "graph " + std::to_string(i) + " has " + kind.plural + ": render it with wae_batch_prepare " +
                                                    "(or _prepare_many), " + kind.bind + " and wae_batch_run");
+        if (graphs[i] && graphs[i]->analyser_readouts)  // (a one-shot render returns no read-outs)
+            return fail(WAE_INVALID_STATE, "graph " + std::to_string(i) + " has analyser read-outs declared: render it with wae_batch_prepare " +
+                                               "(or _prepare_many) and wae_batch_run, and read them with wae_batch_fetch_analyser_readouts");
+    }
     return WAE_OK;
 }
 
@@ -6440,6 +6563,34 @@ WAE_API wae_status wae_analyser_get_float_frequency_data(wae_batch* b, uint32_t 
     }
     uint32_t n = std::min(len, bins);
     CUDA_TRY(cudaMemcpyAsync(out, a->d_db, n * sizeof(float), cudaMemcpyDeviceToHost, b->engine->stream));
+    CUDA_TRY(cudaStreamSynchronize(b->engine->stream));
+    return WAE_OK;
+}
+
+// The rows of the declared read-outs of one (node, kind) over the batch (wae_analyser_set_readouts)
+static const ReadoutOut* find_readouts(wae_batch* b, wae_node_id node, uint32_t kind) {
+    if (!b || (kind != WAE_READOUT_FREQUENCY && kind != WAE_READOUT_TIME_DOMAIN)) return nullptr;
+    auto it = b->readout_outs.find({node, kind});
+    return it == b->readout_outs.end() ? nullptr : &it->second;
+}
+WAE_API wae_status wae_batch_analyser_readouts_device_ptr(wae_batch* b, wae_node_id node, uint32_t kind, float** ptr, uint64_t* floats) {
+    if (!ptr || !floats) return fail(WAE_INVALID_ARGUMENT, "null argument");
+    const ReadoutOut* r = find_readouts(b, node, kind);
+    if (!r) return fail(WAE_INVALID_ARGUMENT, "no graph of this batch declares read-outs of that kind on that node");
+    *ptr = r->d;
+    *floats = r->floats;
+    return WAE_OK;
+}
+WAE_API wae_status wae_batch_fetch_analyser_readouts(wae_batch* b, uint32_t graph_index, wae_node_id node, uint32_t kind, float* host_out,
+                                                     uint64_t floats) {
+    if (!host_out) return fail(WAE_INVALID_ARGUMENT, "null output");
+    const ReadoutOut* r = find_readouts(b, node, kind);
+    if (!r || graph_index >= b->n_graphs || r->off[b->batch_pos(graph_index)] == UINT64_MAX)
+        return fail(WAE_INVALID_ARGUMENT, "graph " + std::to_string(graph_index) + " declares no read-outs of that kind on that node");
+    const uint32_t j = b->batch_pos(graph_index);
+    if (floats != r->len[j]) return fail(WAE_INVALID_ARGUMENT, "the graph's read-outs are " + std::to_string(r->len[j]) + " floats");
+    CUDA_TRY(cudaSetDevice(b->engine->device));
+    CUDA_TRY(cudaMemcpyAsync(host_out, r->d + r->off[j], floats * sizeof(float), cudaMemcpyDeviceToHost, b->engine->stream));
     CUDA_TRY(cudaStreamSynchronize(b->engine->stream));
     return WAE_OK;
 }

@@ -3375,6 +3375,19 @@ __global__ void __launch_bounds__(32) k_compressor(const CompInst* __restrict__ 
     q.state[1] = reduction_gain;
 }
 
+// The analyser's mono down-mix of input frame n of the chunk: mono.mix(1, Speakers) (analyser.rs:267-294)
+__device__ __forceinline__ float analyser_mono(const BufRef& in, int ch, int n, const ChunkInfo& ci) {
+    MixEdge e;
+    e.src = in;
+    e.src_ch = ch;
+    if (in.meta) {  // dynamic input layout: the down-mix sees the channels this quantum has
+        const int qi = meta_qi(ci, n);
+        e.src_ch = buf_count(in, ch, qi);
+        return buf_silent(in, ch, qi) ? 0.f : mixed_sample(e, 1, 0, 0, n, ci);
+    }
+    return mixed_sample(e, 1, 0, 0, n, ci);
+}
+
 // AnalyserRenderer (src/node/analyser.rs:267-294) + AnalyserRingBuffer::write (src/analysis.rs:96-112)
 __global__ void __launch_bounds__(256) k_analyser(const AnalyserInst* __restrict__ insts, int n_inst, ChunkInfo ci) {
     const int RING = 32768 + 128;
@@ -3386,17 +3399,7 @@ __global__ void __launch_bounds__(256) k_analyser(const AnalyserInst* __restrict
         if (n >= ci.nf) continue;
         const bool record = n < nf_end && nf_end - n <= RING;  // (older than the ring: overwritten by this very chunk)
         if (!a.out.p && !record) continue;
-        MixEdge e;
-        e.src = a.in;
-        e.src_ch = a.ch;
-        float mono;
-        if (a.in.meta) {  // dynamic input layout: the down-mix sees the channels this quantum has
-            const int qi = meta_qi(ci, n);
-            e.src_ch = buf_count(a.in, a.ch, qi);
-            mono = buf_silent(a.in, a.ch, qi) ? 0.f : mixed_sample(e, 1, 0, 0, n, ci);
-        } else {
-            mono = mixed_sample(e, 1, 0, 0, n, ci);  // mono.mix(1, Speakers)
-        }
+        const float mono = analyser_mono(a.in, a.ch, n, ci);
         if (a.out.p)
             for (int c = 0; c < a.ch; c++) chan(a.out, c, ci)[n] = chan(a.in, c, ci)[n];
         if (record) a.ring[(ci.f0 + n) % RING] = mono;
@@ -4823,27 +4826,19 @@ void upload_twiddles() {
 // smoothing with the previous read-out -> 20 log10.  One CTA per analyser, radix-2 complex FFT of fftSize/2 points in
 // shared memory (fftSize up to 32768 -> 128 KB), the real-FFT split done on the fly.
 // ---------------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256) k_analyser_fft(const float* __restrict__ ring, uint32_t write_index, int fft_size, float smoothing,
-                                                      float* __restrict__ last_fft, float* __restrict__ out_db) {
-    extern __shared__ float2 zf[];
-    const int RING = 32768 + 128;
-    const int n = fft_size / 2;
-    const int t = threadIdx.x;
+// Blackman window value of sample idx (analysis.rs:13-24)
+__device__ __forceinline__ float analyser_blackman(int idx, int fft_size) {
     const float PI32 = 3.14159265358979323846f;
-    int bits = 0;
-    while ((1 << bits) < n) bits++;
-    for (int i = t; i < n; i += blockDim.x) {
-        float v[2];
-        for (int h = 0; h < 2; h++) {
-            int idx = 2 * i + h;
-            float x = ring[(RING + write_index - fft_size + idx) % RING];
-            float w = 0.42f - 0.5f * cosf(2.f * PI32 * (float)idx / (float)fft_size) + 0.08f * cosf(4.f * PI32 * (float)idx / (float)fft_size);
-            v[h] = x * w;
-        }
-        int r = (int)(__brev((unsigned)i) >> (32 - bits));
-        zf[bits == 0 ? 0 : r] = make_float2(v[0], v[1]);
-    }
-    __syncthreads();
+    return 0.42f - 0.5f * cosf(2.f * PI32 * (float)idx / (float)fft_size) + 0.08f * cosf(4.f * PI32 * (float)idx / (float)fft_size);
+}
+// Windowed samples 2i, 2i+1 -> bit-reversed slot of the complex FFT of fftSize / 2 points (`bits` = log2 of that)
+__device__ __forceinline__ void analyser_store_pair(float2* zf, int i, int bits, float v0, float v1) {
+    const int r = (int)(__brev((unsigned)i) >> (32 - bits));
+    zf[bits == 0 ? 0 : r] = make_float2(v0, v1);
+}
+// In-place radix-2 transform of the n = fftSize / 2 points in zf (all threads of the CTA; the caller synchronises before)
+__device__ __forceinline__ void analyser_fft_passes(float2* zf, int n) {
+    const int t = threadIdx.x;
     for (int len = 2; len <= n; len <<= 1) {
         const int half = len >> 1;
         for (int b = t; b < n / 2; b += blockDim.x) {
@@ -4858,26 +4853,118 @@ __global__ void __launch_bounds__(256) k_analyser_fft(const float* __restrict__ 
         }
         __syncthreads();
     }
-    const float norm = 1.f / (float)fft_size;
-    for (int k = t; k < n; k += blockDim.x) {  // bins 0 .. N/2-1 (the Nyquist bin is ignored, analysis.rs:303-333)
-        float2 X;
-        if (k == 0) {
-            X = make_float2(zf[0].x + zf[0].y, 0.f);
-        } else {
-            float2 zk = zf[k], zc = make_float2(zf[n - k].x, -zf[n - k].y);
-            float2 e = make_float2(0.5f * (zk.x + zc.x), 0.5f * (zk.y + zc.y));
-            float2 d = make_float2(zk.x - zc.x, zk.y - zc.y);
-            float2 o = make_float2(0.5f * d.y, -0.5f * d.x);
-            float sn, cs;
-            sincospif(-2.f * (float)k / (float)fft_size, &sn, &cs);
-            X = make_float2(e.x + (o.x * cs - o.y * sn), e.y + (o.x * sn + o.y * cs));
+}
+// |X[k]| / N of the real input from the transformed points (bins 0 .. N/2-1: the Nyquist bin is ignored, analysis.rs:303-333)
+__device__ __forceinline__ float analyser_bin_magnitude(const float2* zf, int k, int n, int fft_size) {
+    float2 X;
+    if (k == 0) {
+        X = make_float2(zf[0].x + zf[0].y, 0.f);
+    } else {
+        float2 zk = zf[k], zc = make_float2(zf[n - k].x, -zf[n - k].y);
+        float2 e = make_float2(0.5f * (zk.x + zc.x), 0.5f * (zk.y + zc.y));
+        float2 d = make_float2(zk.x - zc.x, zk.y - zc.y);
+        float2 o = make_float2(0.5f * d.y, -0.5f * d.x);
+        float sn, cs;
+        sincospif(-2.f * (float)k / (float)fft_size, &sn, &cs);
+        X = make_float2(e.x + (o.x * cs - o.y * sn), e.y + (o.x * sn + o.y * cs));
+    }
+    return hypotf(X.x, X.y) * (1.f / (float)fft_size);
+}
+// get_float_frequency_data's smoothing with the previous read-out (analysis.rs:335-345): the new state (its dB: 20 log10)
+__device__ __forceinline__ float analyser_smooth(float smoothing, float last, float mag) {
+    float value = smoothing * last + (1.f - smoothing) * mag;
+    if (!isfinite(value)) value = 0.f;
+    return value;
+}
+
+__global__ void __launch_bounds__(256) k_analyser_fft(const float* __restrict__ ring, uint32_t write_index, int fft_size, float smoothing,
+                                                      float* __restrict__ last_fft, float* __restrict__ out_db) {
+    extern __shared__ float2 zf[];
+    const int RING = 32768 + 128;
+    const int n = fft_size / 2;
+    const int t = threadIdx.x;
+    int bits = 0;
+    while ((1 << bits) < n) bits++;
+    for (int i = t; i < n; i += blockDim.x) {
+        float v[2];
+        for (int h = 0; h < 2; h++) {
+            int idx = 2 * i + h;
+            float x = ring[(RING + write_index - fft_size + idx) % RING];
+            v[h] = x * analyser_blackman(idx, fft_size);
         }
-        float mag = hypotf(X.x, X.y) * norm;
-        float value = smoothing * last_fft[k] + (1.f - smoothing) * mag;
-        if (!isfinite(value)) value = 0.f;
+        analyser_store_pair(zf, i, bits, v[0], v[1]);
+    }
+    __syncthreads();
+    analyser_fft_passes(zf, n);
+    for (int k = t; k < n; k += blockDim.x) {
+        float mag = analyser_bin_magnitude(zf, k, n, fft_size);
+        float value = analyser_smooth(smoothing, last_fft[k], mag);
         last_fft[k] = value;
         out_db[k] = 20.f * log10f(value);
     }
+}
+
+// ---------------------------------------------------------------------------------------------------------
+// Declared analyser read-outs (wae_analyser_set_readouts), taken in the analyser's stage of the chunk (f0, f0 + nf] that holds their
+// frame F, before k_analyser writes the chunk into the ring: a chunk longer than the ring overwrites slots an earlier read-out of the
+// same chunk still needs.  Sample idx of the window is frame F - fftSize + idx: zero before the render, the ring before f0, the
+// analyser's own down-mix of the input from f0 on.
+// ---------------------------------------------------------------------------------------------------------
+__device__ __forceinline__ float readout_sample(const ReadoutInst& r, int idx, const ChunkInfo& ci) {
+    const int RING = 32768 + 128;
+    const int64_t m = r.frame - r.fft_size + idx;
+    if (m < 0) return 0.f;
+    if (m < ci.f0) return r.ring[m % RING];
+    return analyser_mono(r.in, r.ch, (int)(m - ci.f0), ci);
+}
+
+// One CTA per read-out of the chunk: the window, Blackman, the transform of k_analyser_fft, linear magnitudes into the row
+// (k_readout_smooth turns them into dB)
+__global__ void __launch_bounds__(256) k_readout_fft(const ReadoutInst* __restrict__ insts, ChunkInfo ci) {
+    extern __shared__ float2 zf[];
+    const ReadoutInst r = insts[blockIdx.x];
+    const int n = r.fft_size / 2;
+    int bits = 0;
+    while ((1 << bits) < n) bits++;
+    for (int i = threadIdx.x; i < n; i += blockDim.x)
+        analyser_store_pair(zf, i, bits, readout_sample(r, 2 * i, ci) * analyser_blackman(2 * i, r.fft_size),
+                            readout_sample(r, 2 * i + 1, ci) * analyser_blackman(2 * i + 1, r.fft_size));
+    __syncthreads();
+    analyser_fft_passes(zf, n);
+    for (int k = threadIdx.x; k < n; k += blockDim.x) r.row[k] = analyser_bin_magnitude(zf, k, n, r.fft_size);
+}
+
+// Time-domain read-outs: the window itself (get_float_time_domain_data, analysis.rs:261-264)
+__global__ void __launch_bounds__(256) k_readout_time(const ReadoutInst* __restrict__ insts, ChunkInfo ci) {
+    const ReadoutInst r = insts[blockIdx.x];
+    for (int i = blockIdx.y * blockDim.x + threadIdx.x; i < r.fft_size; i += gridDim.y * blockDim.x) r.row[i] = readout_sample(r, i, ci);
+}
+
+// One thread per (analyser, bin): the analyser's frequency read-outs of the chunk in time order, smoothed with the state the previous
+// one left (analysis.rs:335-345); a read-out on the quantum of the one before repeats its row without smoothing again (last_fft_time,
+// :347-361).  The state crosses chunks in last_fft; the last read-out's dB row is the analyser's post-render read-out.
+__global__ void __launch_bounds__(256) k_readout_smooth(const ReadoutSmoothInst* __restrict__ insts, ChunkInfo ci) {
+    const ReadoutSmoothInst s = insts[blockIdx.x];
+    const int bin = blockIdx.y * blockDim.x + threadIdx.x;
+    if (bin >= s.bins) return;
+    // first read-out of the chunk: F > f0, or F >= 0 in the first chunk
+    const int64_t lo = ci.f0 == 0 ? -1 : ci.f0, hi = ci.f0 + ci.nf;
+    int a = 0, b = s.n;
+    while (a < b) {
+        const int m = (a + b) >> 1;
+        if (s.frames[m] > lo) b = m;
+        else a = m + 1;
+    }
+    if (a >= s.n || s.frames[a] > hi) return;
+    float last = s.last_fft[bin], db = 0.f;
+    for (int k = a; k < s.n && s.frames[k] <= hi; k++) {
+        float* row = s.rows + (size_t)k * s.bins;
+        if (k > 0 && s.frames[k] == s.frames[k - 1]) db = row[(int64_t)-s.bins + bin];
+        else db = 20.f * log10f(last = analyser_smooth(s.smoothing, last, row[bin]));
+        row[bin] = db;
+        if (k == s.n - 1) s.db[bin] = db;
+    }
+    s.last_fft[bin] = last;
 }
 
 // AudioBuffer::resample (src/buffer.rs:311-363): linear interpolation that keeps the first and the last frame
@@ -5277,6 +5364,20 @@ void launch_analyser_fft(const float* ring, uint32_t write_index, int fft_size, 
         configured = true;
     }
     k_analyser_fft<<<1, 256, (size_t)(fft_size / 2) * sizeof(float2), s>>>(ring, write_index, fft_size, smoothing, last_fft, out_db);
+}
+void launch_readout_fft(const ReadoutInst* d, int n, int max_fft, ChunkInfo ci, cudaStream_t s) {
+    static bool configured = false;
+    if (!configured) {
+        cudaFuncSetAttribute(k_readout_fft, cudaFuncAttributeMaxDynamicSharedMemorySize, 16384 * (int)sizeof(float2));
+        configured = true;
+    }
+    k_readout_fft<<<n, 256, (size_t)(max_fft / 2) * sizeof(float2), s>>>(d, ci);
+}
+void launch_readout_time(const ReadoutInst* d, int n, int max_fft, ChunkInfo ci, cudaStream_t s) {
+    k_readout_time<<<dim3(n, (max_fft + 255) / 256), 256, 0, s>>>(d, ci);
+}
+void launch_readout_smooth(const ReadoutSmoothInst* d, int n, int max_bins, ChunkInfo ci, cudaStream_t s) {
+    k_readout_smooth<<<dim3(n, (max_bins + 255) / 256), 256, 0, s>>>(d, ci);
 }
 void launch_resample_linear(const float* in, int64_t len, float* out, int64_t target_len, cudaStream_t s) {
     k_resample_linear<<<(unsigned)((target_len + 255) / 256), 256, 0, s>>>(in, len, out, target_len);

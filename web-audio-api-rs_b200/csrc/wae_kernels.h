@@ -341,6 +341,10 @@ void launch_resample_linear(const float* in, int64_t len, float* out, int64_t ta
 void launch_param(const ParamInst* d, int n, ChunkInfo ci, cudaStream_t s, int mode);  // 0: k_param, 1: k_param_parallel, 2: k_param_spec
 void launch_compressor(const CompInst* d, int n, ChunkInfo ci, cudaStream_t s);
 void launch_analyser(const AnalyserInst* d, int n, ChunkInfo ci, cudaStream_t s);
+// declared analyser read-outs (wae_analyser_set_readouts): `d` = the chunk's n records, max_fft / max_bins = the largest of the stage
+void launch_readout_fft(const ReadoutInst* d, int n, int max_fft, ChunkInfo ci, cudaStream_t s);
+void launch_readout_time(const ReadoutInst* d, int n, int max_fft, ChunkInfo ci, cudaStream_t s);
+void launch_readout_smooth(const ReadoutSmoothInst* d, int n, int max_bins, ChunkInfo ci, cudaStream_t s);
 void launch_conv_fft_in(const ConvInput* d, int n, ChunkInfo ci, cudaStream_t s);
 void launch_conv_mac_ifft(const ConvPath* p, const ConvInput* in, int n, ChunkInfo ci, cudaStream_t s);
 void launch_conv_compact(const ConvCmpInst* d, int n, ChunkInfo ci, cudaStream_t s);
