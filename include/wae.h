@@ -458,6 +458,39 @@ WAE_API wae_status wae_batch_analyser_readouts_device_ptr(wae_batch* batch, wae_
 WAE_API wae_status wae_batch_fetch_analyser_readouts(wae_batch* batch, uint32_t graph_index, wae_node_id node, uint32_t kind, float* host_out,
                                                      uint64_t floats);
 
+/* Byte read-outs: wae_analyser_set_byte_readouts delivers the declared read-outs of `kinds` (a non-empty subset of the kinds given to
+ * wae_analyser_set_readouts) as bytes too, at the same times: row k is what Analyser::get_byte_frequency_data /
+ * get_byte_time_domain_data return in a suspend callback at quantum q_k (src/analysis.rs:266-276, 371-401).  A byte frequency row is
+ * (u8) clamp(255 / (maxDecibels - minDecibels) * (dB - minDecibels), 0, 255) in f32 of the float row's dB (one smoothing step serves
+ * both, as last_fft_time makes it in the reference; minDecibels / maxDecibels are the node's at render time); a byte time-domain row
+ * is (u8) clamp(128 * (1 + x), 0, 255), NaN -> 0.  The float rows are unchanged by the declaration.  Refused: a node that is not an
+ * analyser, kinds 0, unknown bits (WAE_INVALID_ARGUMENT) or not declared by wae_analyser_set_readouts (WAE_INVALID_ARGUMENT); no
+ * read-outs declared yet, a second declaration or a graph with a suspend point (WAE_INVALID_STATE).
+ * wae_batch_analyser_byte_readouts_device_ptr / wae_batch_fetch_analyser_byte_readouts: as the float pair, laid out alike (one
+ * allocation per (node, kind), graphs in prepare order, each [k][row]; a graph without the byte declaration takes no space). */
+WAE_API wae_status wae_analyser_set_byte_readouts(wae_graph* graph, wae_node_id node, uint32_t kinds);
+WAE_API wae_status wae_batch_analyser_byte_readouts_device_ptr(wae_batch* batch, wae_node_id node, uint32_t kind, uint8_t** ptr,
+                                                               uint64_t* bytes);
+WAE_API wae_status wae_batch_fetch_analyser_byte_readouts(wae_batch* batch, uint32_t graph_index, wae_node_id node, uint32_t kind,
+                                                          uint8_t* host_out, uint64_t bytes);
+
+/* DynamicsCompressorNode::reduction at declared render times, taken on the GPU during a run of a prepared batch.
+ *
+ * wae_compressor_set_readouts declares read-outs at `times` (seconds), validated and quantised as wae_analyser_set_readouts does:
+ * read-out k is what DynamicsCompressorNode::reduction returns in a suspend callback at quantum q_k, i.e. the reduction (dB) of the
+ * last frame of quantum q_k - 1 (dynamics_compressor.rs:440, 450), 0 for q_k = 0; at the end quantum it equals what
+ * wae_compressor_reduction answers after the render.  Refused: a node that is not a DynamicsCompressorNode, n == 0, a negative /
+ * non-finite / decreasing time, a quantum past the render (WAE_INVALID_ARGUMENT); a second declaration on the node or a graph with a
+ * suspend point (WAE_INVALID_STATE; wae_graph_suspend refuses a graph with a declaration).  One-shot renders refuse declared graphs.
+ *
+ * After a run: wae_batch_compressor_readouts_device_ptr gives the device memory of one node's rows over the whole batch, graphs in the
+ * order they were passed to prepare, each [k] (a graph without the declaration takes no space), `floats` in all;
+ * wae_batch_fetch_compressor_readouts copies one graph's [k] to the host (`floats` must be K).  Each run overwrites the rows. */
+WAE_API wae_status wae_compressor_set_readouts(wae_graph* graph, wae_node_id node, const double* times, uint32_t n);
+WAE_API wae_status wae_batch_compressor_readouts_device_ptr(wae_batch* batch, wae_node_id node, float** ptr, uint64_t* floats);
+WAE_API wae_status wae_batch_fetch_compressor_readouts(wae_batch* batch, uint32_t graph_index, wae_node_id node, float* host_out,
+                                                       uint64_t floats);
+
 /* load_hrtf_processor (src/node/panner.rs:39-68): the HRIR sphere the reference embeds with include_bytes!
  * ("resources/IRC_1003_C.bin": "HRIR" | u32 rate | u32 taps | u32 #vertices | u32 #indices | indices | per vertex xyz,
  * left[taps], right[taps]).  Must be set before a batch with PanningModelType::HRTF panners is prepared; contexts whose
@@ -470,6 +503,7 @@ WAE_API wae_status wae_analyser_get_byte_frequency_data(wae_batch* batch, uint32
 
 /* DynamicsCompressorNode::reduction (src/node/dynamics_compressor.rs:204-206): gain reduction (dB) at the end of the render */
 WAE_API wae_status wae_compressor_reduction(wae_batch* batch, uint32_t graph_index, wae_node_id node, float* out);
+/* (the reduction over the render: wae_compressor_set_readouts above) */
 
 /* AudioBuffer::resample (src/buffer.rs:311-363) on the GPU: linear interpolation keeping the first and last frame; the
  * input side of the path (decode_audio_data resamples buffers to the context rate).  Host pointers. */

@@ -217,6 +217,8 @@ WAE_SYMBOLS = [
     "wae_buffer_source_set_device_loop", "wae_batch_bind_loops",
     "wae_batch_bind_output",
     "wae_analyser_set_readouts", "wae_batch_analyser_readouts_device_ptr", "wae_batch_fetch_analyser_readouts",
+    "wae_analyser_set_byte_readouts", "wae_batch_analyser_byte_readouts_device_ptr", "wae_batch_fetch_analyser_byte_readouts",
+    "wae_compressor_set_readouts", "wae_batch_compressor_readouts_device_ptr", "wae_batch_fetch_compressor_readouts",
 ]
 
 
@@ -352,6 +354,13 @@ class Api:
             f("analyser_set_readouts", C.c_int32, [gp, C.c_uint32, c_double_p, C.c_uint32, C.c_uint32])
             f("batch_analyser_readouts_device_ptr", C.c_int32, [C.c_void_p, C.c_uint32, C.c_uint32, C.POINTER(c_float_p), C.POINTER(C.c_uint64)])
             f("batch_fetch_analyser_readouts", C.c_int32, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, c_float_p, C.c_uint64])
+            f("analyser_set_byte_readouts", C.c_int32, [gp, C.c_uint32, C.c_uint32])
+            f("batch_analyser_byte_readouts_device_ptr", C.c_int32, [C.c_void_p, C.c_uint32, C.c_uint32, C.POINTER(C.c_void_p), C.POINTER(C.c_uint64)])
+            f("batch_fetch_analyser_byte_readouts", C.c_int32, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p, C.c_uint64])
+            # compressor reduction read-outs at declared render times
+            f("compressor_set_readouts", C.c_int32, [gp, C.c_uint32, c_double_p, C.c_uint32])
+            f("batch_compressor_readouts_device_ptr", C.c_int32, [C.c_void_p, C.c_uint32, C.POINTER(c_float_p), C.POINTER(C.c_uint64)])
+            f("batch_fetch_compressor_readouts", C.c_int32, [C.c_void_p, C.c_uint32, C.c_uint32, c_float_p, C.c_uint64])
         else:
             f("graph_create", C.c_int32, [C.c_uint32, C.c_uint64, C.c_float, C.POINTER(C.c_void_p)])
             f("render", C.c_int32, [gp, c_float_p])

@@ -494,6 +494,24 @@ class DynamicsCompressorNode(AudioNode):
             api.check(api.compressor_reduction(ctx._g, self.id, C.byref(out)))
         return out.value
 
+    # wae_compressor_set_readouts: reduction() taken on the GPU during the render, at `times` (seconds, non-decreasing), each quantised
+    # like a suspend_sync callback's (ceil(t * sampleRate / 128) quanta)
+    def set_readouts(self, times):
+        times = np.ascontiguousarray(times, np.float64).reshape(-1)
+        api = self._ctx._api
+        if not api.is_product:
+            raise B.WaeError(4, "compressor read-outs are taken by the GPU engine")
+        api.check(api.compressor_set_readouts(self._ctx._g, self.id, times.ctypes.data_as(B.c_double_p), len(times)))
+        self._readouts = len(times)
+        self._ctx._comp_readout_nodes[self.id] = self
+
+    def get_reduction_readouts(self):
+        """[K] reduction (dB) of the declared read-outs of the last render"""
+        ctx = self._ctx
+        out = ctx._readout_array("compressor", (getattr(self, "_readouts", 0),), np.float32)
+        ctx._api.check(ctx._api.batch_fetch_compressor_readouts(ctx._batch.handle, ctx._batch_index, self.id, B.fptr(out), out.size))
+        return out
+
 
 class AnalyserNode(AudioNode):
     def __init__(self, ctx, node_id, fft_size):
@@ -551,6 +569,24 @@ class AnalyserNode(AudioNode):
         """[K][fftSize] samples of the declared read-outs of the last render"""
         return self._ctx._readouts(self, B.READOUT_TIME_DOMAIN, self.fft_size)
 
+    # wae_analyser_set_byte_readouts: the declared read-outs of these kinds (declared by set_readouts) delivered as bytes too, as
+    # get_byte_frequency_data / get_byte_time_domain_data return them; minDecibels / maxDecibels are the node's at render time
+    def set_byte_readouts(self, frequency=False, time_domain=False):
+        kinds = (B.READOUT_FREQUENCY if frequency else 0) | (B.READOUT_TIME_DOMAIN if time_domain else 0)
+        api = self._ctx._api
+        if not api.is_product:
+            raise B.WaeError(4, "analyser read-outs are taken by the GPU engine")
+        api.check(api.analyser_set_byte_readouts(self._ctx._g, self.id, kinds))
+        self._byte_readouts = kinds
+
+    def get_byte_frequency_readouts(self):
+        """[K][fftSize / 2] uint8 of the declared byte read-outs of the last render"""
+        return self._ctx._readouts(self, B.READOUT_FREQUENCY, self.fft_size // 2, byte=True)
+
+    def get_byte_time_domain_readouts(self):
+        """[K][fftSize] uint8 of the declared byte read-outs of the last render"""
+        return self._ctx._readouts(self, B.READOUT_TIME_DOMAIN, self.fft_size, byte=True)
+
 
 class AudioListener:
     def __init__(self, ctx):
@@ -581,6 +617,7 @@ class OfflineAudioContext:
         self._listener = None
         self._suspends = []
         self._readout_nodes = {}  # node id -> AnalyserNode with declared read-outs (set_readouts)
+        self._comp_readout_nodes = {}  # node id -> DynamicsCompressorNode with declared read-outs (set_readouts)
         self._current_time = 0.0
         self._device_inputs = {}  # node id -> (channels, length) declared with set_device_input
         self._source_refs = set()  # ids of the device inputs declared by_reference
@@ -771,12 +808,18 @@ class OfflineAudioContext:
         """OfflineAudioContext::start_rendering_sync (src/context/offline.rs:157-185): a batch of one."""
         return render_batch([self])[0]
 
-    def _readouts(self, node, kind, row):
+    def _readout_array(self, what, shape, dtype):
         if self._batch is None:
-            raise B.WaeError(2, "analyser read-outs are available after rendering")
-        k = getattr(node, "_readouts", 0)
-        out = np.empty((k, row), np.float32)
-        self._api.check(self._api.batch_fetch_analyser_readouts(self._batch.handle, self._batch_index, node.id, kind, B.fptr(out), out.size))
+            raise B.WaeError(2, f"{what} read-outs are available after rendering")
+        return np.empty(shape, dtype)
+
+    def _readouts(self, node, kind, row, byte=False):
+        out = self._readout_array("analyser", (getattr(node, "_readouts", 0), row), np.uint8 if byte else np.float32)
+        api, h = self._api, self._batch.handle
+        if byte:
+            api.check(api.batch_fetch_analyser_byte_readouts(h, self._batch_index, node.id, kind, out.ctypes.data_as(C.c_void_p), out.size))
+        else:
+            api.check(api.batch_fetch_analyser_readouts(h, self._batch_index, node.id, kind, B.fptr(out), out.size))
         return out
 
     def _analyser_read(self, node, kind, n, byte=False, out=None):
@@ -826,7 +869,7 @@ class Batch:
         self._views_out = False  # output_tensor was called: runs into the batch's own buffer are ordered after torch's current stream
         self._out = None  # bind_output: the tensor runs write
         self._out_viewed = False  # output_tensor handed out views of the bound tensor since it was bound: runs into it wait for torch
-        self._readouts_viewed = False  # analyser_readouts handed out views of the read-out rows: every run (bound output or not) waits for torch
+        self._readouts_viewed = False  # analyser_readouts / compressor_readouts handed out views of read-out rows: every run (bound output or not) waits for torch
         self._src_refs = {}  # bind_sources: (graph, node id) -> the tensor a device input declared by_reference reads
         self._ref_tensors = []  # the distinct tensors of _src_refs
         self._has_refs = any(c._source_refs for c in contexts)
@@ -1296,31 +1339,48 @@ class Batch:
         torch.cuda.current_stream(self._device()).wait_stream(self._engine_stream())
         return view
 
-    def analyser_readouts(self, node, kind="frequency"):
+    def analyser_readouts(self, node, kind="frequency", byte=False):
         """Zero-copy torch view [n][K][row] of the declared read-outs (AnalyserNode.set_readouts) of `node` (an AnalyserNode of context 0,
         or its id) over the batch, when every context declares them alike on the same node id; otherwise fetch them per context
-        (AnalyserNode.get_float_frequency_readouts / get_float_time_domain_readouts).  Ordered like output_tensor: torch's current
-        stream waits for the engine stream, and later runs, which overwrite the rows, wait for the work then queued on torch's stream."""
-        import torch
+        (AnalyserNode.get_float_frequency_readouts / get_float_time_domain_readouts).  byte=True: the uint8 rows of
+        AnalyserNode.set_byte_readouts.  Ordered like output_tensor: torch's current stream waits for the engine stream, and later runs,
+        which overwrite the rows, wait for the work then queued on torch's stream."""
         kind_id = _readout_kind(kind)
         node_id = int(getattr(node, "id", node))
-        p, floats = B.c_float_p(), C.c_uint64()
-        self.api.check(self.api.batch_analyser_readouts_device_ptr(self.handle, node_id, kind_id, C.byref(p), C.byref(floats)))
-        if floats.value % self.n:
-            raise B.WaeError(2, "analyser_readouts: the contexts declare different read-outs on this node; fetch them per context")
-        per = floats.value // self.n
+        count = C.c_uint64()
+        if byte:
+            p = C.c_void_p()
+            self.api.check(self.api.batch_analyser_byte_readouts_device_ptr(self.handle, node_id, kind_id, C.byref(p), C.byref(count)))
+        else:
+            p = B.c_float_p()
+            self.api.check(self.api.batch_analyser_readouts_device_ptr(self.handle, node_id, kind_id, C.byref(p), C.byref(count)))
         shapes = set()
         for c in self.contexts:
             a = c._readout_nodes.get(node_id)
-            shapes.add(None if a is None else (a._readouts, a.fft_size))
-        k = shapes.pop() if len(shapes) == 1 else None
-        if k is None:
-            raise B.WaeError(2, "analyser_readouts: the contexts declare different read-outs on this node; fetch them per context")
-        row = k[1] // 2 if kind_id == B.READOUT_FREQUENCY else k[1]
-        if k[0] * row != per:
-            raise B.WaeError(2, "analyser_readouts: the contexts declare different read-outs on this node; fetch them per context")
+            shapes.add(None if a is None else (a._readouts, a.fft_size // 2 if kind_id == B.READOUT_FREQUENCY else a.fft_size))
+        return self._readout_view("analyser_readouts", p, count.value, shapes, "|u1" if byte else "<f4")
+
+    def compressor_readouts(self, node):
+        """Zero-copy torch view [n][K] of the declared reduction read-outs (DynamicsCompressorNode.set_readouts) of `node` (a
+        DynamicsCompressorNode of context 0, or its id) over the batch, when every context declares them alike on the same node id;
+        otherwise fetch them per context (DynamicsCompressorNode.get_reduction_readouts).  Ordered like analyser_readouts."""
+        node_id = int(getattr(node, "id", node))
+        p, count = B.c_float_p(), C.c_uint64()
+        self.api.check(self.api.batch_compressor_readouts_device_ptr(self.handle, node_id, C.byref(p), C.byref(count)))
+        shapes = set()
+        for c in self.contexts:
+            r = c._comp_readout_nodes.get(node_id)
+            shapes.add(None if r is None else (r._readouts,))
+        return self._readout_view("compressor_readouts", p, count.value, shapes, "<f4")
+
+    def _readout_view(self, what, p, count, shapes, typestr):
+        """[n][*shape] view of read-out rows at `p` (`count` elements over the batch) when every context has the one shape in `shapes`"""
+        import torch
+        shape = shapes.pop() if len(shapes) == 1 else None
+        if shape is None or self.n * int(np.prod(shape)) != count:
+            raise B.WaeError(2, f"{what}: the contexts declare different read-outs on this node; fetch them per context")
         addr = C.cast(p, C.c_void_p).value
-        view = torch.as_tensor(_DeviceView(self, addr, (self.n, k[0], row)), device=self._device())
+        view = torch.as_tensor(_DeviceView(self, addr, (self.n,) + shape, typestr), device=self._device())
         self._readouts_viewed = True
         torch.cuda.current_stream(self._device()).wait_stream(self._engine_stream())
         return view
@@ -1357,12 +1417,12 @@ class Batch:
 
 
 class _DeviceView:
-    """__cuda_array_interface__ of a float32 range of a batch's device output; torch.as_tensor keeps this object, and so the batch,
-    alive as long as the tensor."""
+    """__cuda_array_interface__ of a float32 (or, typestr "|u1", uint8) range of a batch's device memory; torch.as_tensor keeps this
+    object, and so the batch, alive as long as the tensor."""
 
-    def __init__(self, batch, ptr, shape):
+    def __init__(self, batch, ptr, shape, typestr="<f4"):
         self.batch = batch
-        self.__cuda_array_interface__ = {"shape": tuple(int(s) for s in shape), "typestr": "<f4", "data": (int(ptr), False),
+        self.__cuda_array_interface__ = {"shape": tuple(int(s) for s in shape), "typestr": typestr, "data": (int(ptr), False),
                                          "version": 2}
 
 

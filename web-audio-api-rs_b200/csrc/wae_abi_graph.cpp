@@ -703,6 +703,8 @@ WAE_API wae_status wae_graph_suspend(wae_graph* g, double suspend_time) {
         return fail(WAE_INVALID_STATE, "InvalidStateError - the graph has loop points bound from device memory (wae_buffer_source_set_device_loop)");
     if (g->analyser_readouts)  // (read-outs are taken on the GPU; suspend callbacks run on the host before the render)
         return fail(WAE_INVALID_STATE, "InvalidStateError - the graph has analyser read-outs declared (wae_analyser_set_readouts)");
+    if (g->compressor_readouts)
+        return fail(WAE_INVALID_STATE, "InvalidStateError - the graph has compressor read-outs declared (wae_compressor_set_readouts)");
     g->epochs.push_back(wae_graph::Epoch{quantum * 128, g->nodes});
     return WAE_OK;
 }
@@ -1052,15 +1054,10 @@ WAE_API wae_status wae_source_set_device_schedule(wae_graph* g, wae_node_id node
 
 // AnalyserNode read-outs taken during the render at declared times, each quantised like suspend_sync (offline.rs:248-251).  The
 // suspend points a graph with read-outs would need are exactly what it does without: a graph has one or the other.
-WAE_API wae_status wae_analyser_set_readouts(wae_graph* g, wae_node_id node, const double* times, uint32_t n, uint32_t kinds) {
-    if (!g) return fail(WAE_INVALID_ARGUMENT, "null graph");
-    Node* a = g->nodes.get(node);
-    if (!a || a->kind != K_ANALYSER) return fail(WAE_INVALID_ARGUMENT, "not an AnalyserNode");
+static wae_status readout_quanta(const wae_graph* g, const double* times, uint32_t n, std::vector<uint64_t>& q) {
     if (n == 0 || !times) return fail(WAE_INVALID_ARGUMENT, "no read-out times");
-    if (kinds == 0 || (kinds & ~(uint32_t)(WAE_READOUT_FREQUENCY | WAE_READOUT_TIME_DOMAIN)))
-        return fail(WAE_INVALID_ARGUMENT, "kinds must be a non-empty set of WAE_READOUT_FREQUENCY | WAE_READOUT_TIME_DOMAIN");
     const uint64_t total = (g->length + 127) / 128;
-    std::vector<uint64_t> q(n);
+    q.assign(n, 0);
     for (uint32_t k = 0; k < n; k++) {
         if (!std::isfinite(times[k]) || times[k] < 0.)
             return fail(WAE_INVALID_ARGUMENT, "RangeError - read-out time " + std::to_string(k) + " is negative or not finite");
@@ -1071,11 +1068,55 @@ WAE_API wae_status wae_analyser_set_readouts(wae_graph* g, wae_node_id node, con
             return fail(WAE_INVALID_ARGUMENT, "RangeError - read-out time " + std::to_string(k) + " is after the end of the rendering");
         q[k] = (uint64_t)qd;
     }
+    return WAE_OK;
+}
+
+WAE_API wae_status wae_analyser_set_readouts(wae_graph* g, wae_node_id node, const double* times, uint32_t n, uint32_t kinds) {
+    if (!g) return fail(WAE_INVALID_ARGUMENT, "null graph");
+    Node* a = g->nodes.get(node);
+    if (!a || a->kind != K_ANALYSER) return fail(WAE_INVALID_ARGUMENT, "not an AnalyserNode");
+    if (n == 0 || !times) return fail(WAE_INVALID_ARGUMENT, "no read-out times");
+    if (kinds == 0 || (kinds & ~(uint32_t)(WAE_READOUT_FREQUENCY | WAE_READOUT_TIME_DOMAIN)))
+        return fail(WAE_INVALID_ARGUMENT, "kinds must be a non-empty set of WAE_READOUT_FREQUENCY | WAE_READOUT_TIME_DOMAIN");
+    std::vector<uint64_t> q;
+    const wae_status st = readout_quanta(g, times, n, q);
+    if (st != WAE_OK) return st;
     if (a->readout_kinds) return fail(WAE_INVALID_STATE, "InvalidStateError - the analyser already has read-outs declared");
     if (!g->epochs.empty()) return fail(WAE_INVALID_STATE, "InvalidStateError - analyser read-outs are declared in a graph with a suspend point");
     a->readout_q = std::move(q);
     a->readout_kinds = kinds;
     g->analyser_readouts++;
+    return WAE_OK;
+}
+
+// The declared read-outs of `kinds` are also delivered as bytes (get_byte_frequency_data / get_byte_time_domain_data), at the same times
+WAE_API wae_status wae_analyser_set_byte_readouts(wae_graph* g, wae_node_id node, uint32_t kinds) {
+    if (!g) return fail(WAE_INVALID_ARGUMENT, "null graph");
+    Node* a = g->nodes.get(node);
+    if (!a || a->kind != K_ANALYSER) return fail(WAE_INVALID_ARGUMENT, "not an AnalyserNode");
+    if (kinds == 0 || (kinds & ~(uint32_t)(WAE_READOUT_FREQUENCY | WAE_READOUT_TIME_DOMAIN)))
+        return fail(WAE_INVALID_ARGUMENT, "kinds must be a non-empty set of WAE_READOUT_FREQUENCY | WAE_READOUT_TIME_DOMAIN");
+    if (!g->epochs.empty()) return fail(WAE_INVALID_STATE, "InvalidStateError - analyser read-outs are declared in a graph with a suspend point");
+    if (!a->readout_kinds)
+        return fail(WAE_INVALID_STATE, "InvalidStateError - the analyser has no read-outs declared (wae_analyser_set_readouts)");
+    if (a->byte_readout_kinds) return fail(WAE_INVALID_STATE, "InvalidStateError - the analyser already has byte read-outs declared");
+    if (kinds & ~a->readout_kinds) return fail(WAE_INVALID_ARGUMENT, "byte read-outs of a kind the analyser's read-outs do not declare");
+    a->byte_readout_kinds = kinds;
+    return WAE_OK;
+}
+
+// DynamicsCompressorNode::reduction read at declared times, each quantised like suspend_sync (offline.rs:248-251)
+WAE_API wae_status wae_compressor_set_readouts(wae_graph* g, wae_node_id node, const double* times, uint32_t n) {
+    if (!g) return fail(WAE_INVALID_ARGUMENT, "null graph");
+    Node* c = g->nodes.get(node);
+    if (!c || c->kind != K_COMP) return fail(WAE_INVALID_ARGUMENT, "not a DynamicsCompressorNode");
+    std::vector<uint64_t> q;
+    const wae_status st = readout_quanta(g, times, n, q);
+    if (st != WAE_OK) return st;
+    if (!c->readout_q.empty()) return fail(WAE_INVALID_STATE, "InvalidStateError - the compressor already has read-outs declared");
+    if (!g->epochs.empty()) return fail(WAE_INVALID_STATE, "InvalidStateError - compressor read-outs are declared in a graph with a suspend point");
+    c->readout_q = std::move(q);
+    g->compressor_readouts++;
     return WAE_OK;
 }
 

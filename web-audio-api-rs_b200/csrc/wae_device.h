@@ -322,6 +322,7 @@ struct ReadoutInst {
     int64_t frame;        // F
     int32_t ch;
     int32_t fft_size;
+    uint8_t* bytes;       // time domain with wae_analyser_set_byte_readouts: fftSize bytes of the same window; nullptr: none
 };
 
 // The frequency read-outs of one analyser, for k_readout_smooth: one thread per bin walks those of a chunk in time order
@@ -333,6 +334,17 @@ struct ReadoutSmoothInst {
     int32_t n;              // K
     int32_t bins;
     float smoothing;
+    int32_t pad;
+    uint8_t* bytes;         // [K][bins] byte rows (wae_analyser_set_byte_readouts) of the same dB; nullptr: none
+    float min_db, max_db;   // the node's at render time (the byte rows' range)
+};
+
+// The declared reduction read-outs of one compressor (wae_compressor_set_readouts), parallel to its CompInst in a stage that runs
+// k_compressor<true>: read-out k is the reduction at frame frames[k] = 128 q_k, written when the quantum that ends there ends
+struct CompReadoutInst {
+    const int64_t* frames;  // [K] non-decreasing
+    float* rows;            // [K]
+    int32_t n;              // K
     int32_t pad;
 };
 

@@ -294,6 +294,7 @@ struct StageBuild {
     std::vector<RouteInst> route;
     std::vector<DelayInst> delay;
     std::vector<CompInst> comp;
+    std::vector<CompReadoutInst> comp_ro;           // S_COMP variant 1 (declared reduction read-outs): parallel to comp
     std::vector<AnalyserInst> analyser;
     std::vector<ReadoutInst> readout;                // S_READOUT_FFT / S_READOUT_TIME
     std::vector<ReadoutSmoothInst> readout_smooth;  // S_READOUT_SMOOTH
@@ -494,14 +495,25 @@ struct AnalyserRec {
     bool end_readout = false;  // its last declared frequency read-out is at lq: each run leaves that row in d_db, computed
 };
 
-// The rows of the declared read-outs (wae_analyser_set_readouts) of one (node id, kind) over the batch: one allocation, graphs in the
-// caller's order, each [k][row]
-struct ReadoutOut {
-    float* d = nullptr;
-    uint64_t floats = 0;
-    std::vector<uint64_t> off;  // [batch position] first float of the graph's rows, or UINT64_MAX: not declared there
-    std::vector<uint64_t> len;  // [batch position] floats of the graph's rows
+// The rows of the declared read-outs of one node (and kind) over the batch: one allocation, graphs in the caller's order, each [k][row]
+// (wae_analyser_set_readouts: float rows, wae_analyser_set_byte_readouts: byte rows; wae_compressor_set_readouts: row = 1 float)
+template <typename T>
+struct ReadoutRows {
+    T* d = nullptr;
+    uint64_t count = 0;         // elements in all
+    std::vector<uint64_t> off;  // [batch position] first element of the graph's rows, or UINT64_MAX: not declared there
+    std::vector<uint64_t> len;  // [batch position] elements of the graph's rows
+    void add(uint32_t n_graphs, uint32_t j, uint64_t elems) {
+        if (off.empty()) {
+            off.assign(n_graphs, UINT64_MAX);
+            len.assign(n_graphs, 0);
+        }
+        off[j] = count;
+        len[j] = elems;
+        count += elems;
+    }
 };
+using ReadoutOut = ReadoutRows<float>;
 
 // One kind of input a prepared batch takes from device memory, as messages name it
 struct BindKind {
@@ -684,6 +696,8 @@ struct wae_batch {
     std::vector<std::pair<void*, size_t>> zero_on_run;
     std::vector<AnalyserRec> analysers;
     std::map<std::pair<wae_node_id, uint32_t>, ReadoutOut> readout_outs;  // (node, WAE_READOUT_*) -> rows
+    std::map<std::pair<wae_node_id, uint32_t>, ReadoutRows<uint8_t>> byte_readout_outs;  // (node, WAE_READOUT_*) -> byte rows
+    std::map<wae_node_id, ReadoutOut> comp_readout_outs;  // compressor node -> reduction rows
     struct CompRec { uint32_t graph; wae_node_id node; const float* d_state; };
     std::vector<CompRec> compressors;
     // source PCM assets: device destination <- host source (re-uploadable: wae_batch_upload)
@@ -1761,6 +1775,7 @@ static uint64_t digest_builds(const std::map<std::pair<int, int>, StageBuild>& b
         if (!s.absn_bound.empty()) h = digest_vec(s.absn_bound, h);  // (the same)
         if (!s.readout.empty()) h = digest_vec(s.readout, h);
         if (!s.readout_smooth.empty()) h = digest_vec(s.readout_smooth, h);
+        if (!s.comp_ro.empty()) h = digest_vec(s.comp_ro, h);
     }
     return h;
 }
@@ -1834,7 +1849,7 @@ static void merge_builds(Builds& dst, Builds& src) {
         append_vec(d.mix_edges, s.mix_edges); append_vec(d.mix_dyn, s.mix_dyn); append_vec(d.meta, s.meta); append_vec(d.conv_in, s.conv_in);
         append_vec(d.conv_path, s.conv_path); append_vec(d.vgroups, s.vgroups); append_vec(d.conv_cmp, s.conv_cmp);
         append_vec(d.absn_bound, s.absn_bound);
-        append_vec(d.readout, s.readout); append_vec(d.readout_smooth, s.readout_smooth);
+        append_vec(d.readout, s.readout); append_vec(d.readout_smooth, s.readout_smooth); append_vec(d.comp_ro, s.comp_ro);
         append_vec(d.patches, s.patches);
         append_vec(d.curve_patches, s.curve_patches);
         append_vec(d.iir_patches, s.iir_patches);
@@ -3702,8 +3717,24 @@ bool Planner::lower_compressor(NodeCtx& nc) {
     for (int i = 0; i < 5; i++) c.track[i] = cp[i].dyn ? cp[i].track : BufRef{nullptr, 0, 0};
     c.sample_rate = g->sample_rate;
     c.end = glq;
-    StageBuild& s = stage(nc.L, S_COMP);
+    // declared reduction read-outs (wae_compressor_set_readouts): a stage of its own, whose records carry them in a parallel table
+    const bool readouts = !nc.n.readout_q.empty();
+    StageBuild& s = stage(nc.L, S_COMP, readouts ? 1 : 0);
     s.comp.push_back(c);
+    if (readouts) {
+        float* rows = nullptr;
+        if (dry) rows = reinterpret_cast<float*>(dry_addr());
+        else {
+            auto it = b->comp_readout_outs.find(nc.id);
+            if (it != b->comp_readout_outs.end() && it->second.d) rows = it->second.d + it->second.off[gi];
+        }
+        if (!rows) return bail(WAE_INVALID_STATE, "compressor read-out rows missing");
+        std::vector<int64_t> frames(nc.n.readout_q.size());
+        for (size_t k = 0; k < frames.size(); k++) frames[k] = (int64_t)nc.n.readout_q[k] * 128;
+        const int64_t* d_frames = upload(frames);
+        if (!d_frames) return bail(WAE_OUT_OF_MEMORY, "out of device memory (read-out frames)");
+        s.comp_ro.push_back(CompReadoutInst{d_frames, rows, (int32_t)frames.size(), 0});
+    }
     const size_t offs[5] = {offsetof(CompInst, attack), offsetof(CompInst, knee), offsetof(CompInst, ratio), offsetof(CompInst, release),
                             offsetof(CompInst, threshold)};
     for (int i = 0; i < 5; i++)
@@ -3769,21 +3800,30 @@ bool Planner::lower_readouts(NodeCtx& nc, const AnalyserInst& a, float* last, fl
         auto it = b->readout_outs.find({nc.id, kind});
         return it == b->readout_outs.end() || !it->second.d ? nullptr : it->second.d + it->second.off[gi];
     };
+    auto byte_rows = [&](uint32_t kind) -> uint8_t* {
+        if (!(n.byte_readout_kinds & kind)) return nullptr;
+        if (dry) return reinterpret_cast<uint8_t*>(dry_addr());
+        auto it = b->byte_readout_outs.find({nc.id, kind});
+        return it == b->byte_readout_outs.end() || !it->second.d ? nullptr : it->second.d + it->second.off[gi];
+    };
     for (uint32_t kind : {(uint32_t)WAE_READOUT_FREQUENCY, (uint32_t)WAE_READOUT_TIME_DOMAIN}) {
         if (!(n.readout_kinds & kind)) continue;
         float* base = rows(kind);
-        if (!base) return bail(WAE_INVALID_STATE, "analyser read-out rows missing");
+        uint8_t* bytes = byte_rows(kind);
+        if (!base || (!bytes && (n.byte_readout_kinds & kind))) return bail(WAE_INVALID_STATE, "analyser read-out rows missing");
         const bool f = kind == WAE_READOUT_FREQUENCY;
         const uint32_t row = f ? n.fft_size / 2 : n.fft_size;
         StageBuild& sb = stage(nc.L, f ? S_READOUT_FFT : S_READOUT_TIME);
         for (int k = 0; k < K; k++) {
             if (f && k > 0 && frames[k] == frames[k - 1]) continue;
-            sb.readout.push_back(ReadoutInst{a.in, a.ring, base + (size_t)k * row, frames[k], a.ch, (int32_t)n.fft_size});
+            sb.readout.push_back(ReadoutInst{a.in, a.ring, base + (size_t)k * row, frames[k], a.ch, (int32_t)n.fft_size,
+                                             f || !bytes ? nullptr : bytes + (size_t)k * row});
         }
         if (f) {
             const int64_t* d_frames = upload(frames);
             if (!d_frames) return bail(WAE_OUT_OF_MEMORY, "out of device memory (read-out frames)");
-            stage(nc.L, S_READOUT_SMOOTH).readout_smooth.push_back(ReadoutSmoothInst{d_frames, base, last, db, K, (int32_t)row, (float)n.smoothing, 0});
+            stage(nc.L, S_READOUT_SMOOTH).readout_smooth.push_back(ReadoutSmoothInst{d_frames, base, last, db, K, (int32_t)row, (float)n.smoothing, 0,
+                                                                                      bytes, (float)n.min_db, (float)n.max_db});
         }
     }
     return true;
@@ -4803,7 +4843,10 @@ static void prep_plan_group(wae_batch* b, wae_graph* const* graphs, int k, PrepS
                 case S_DELAY_MONO:
                 case S_DELAY:
                 case S_DELAY_WRITE: st.n = (int)s.delay.size(); st.d_a = up(b, s.delay); break;
-                case S_COMP: st.n = (int)s.comp.size(); st.d_a = up(b, s.comp); break;
+                case S_COMP:  // (d_b stays null without read-outs: undeclared compressors run k_compressor<false>)
+                    st.n = (int)s.comp.size(); st.d_a = up(b, s.comp);
+                    if (!s.comp_ro.empty() && !(st.d_b = up(b, s.comp_ro))) return oom("compressor read-outs");
+                    break;
                 case S_ANALYSER: st.n = (int)s.analyser.size(); st.d_a = up(b, s.analyser); break;
                 case S_READOUT_FFT:
                 case S_READOUT_TIME: {
@@ -5135,30 +5178,31 @@ static wae_status prep_finish(wae_batch* b, PrepState& ps) {
     return WAE_OK;
 }
 
-// The rows of every declared analyser read-out (wae_analyser_set_readouts), before planning: the planner points the records at them.
+// The rows of every declared analyser and compressor read-out (wae_analyser_set_readouts, wae_analyser_set_byte_readouts,
+// wae_compressor_set_readouts), before planning: the planner points the records at them.
 // `graphs` in batch order; the rows of one (node, kind) are laid out in the caller's order.
 static wae_status alloc_readout_rows(wae_batch* b, wae_graph* const* graphs, uint32_t n_graphs) {
     for (uint32_t c = 0; c < n_graphs; c++) {
         const uint32_t j = b->batch_pos(c);
-        if (!graphs[j]->analyser_readouts) continue;
+        if (!graphs[j]->analyser_readouts && !graphs[j]->compressor_readouts) continue;
         for (const auto& kv : graphs[j]->nodes) {
             const Node& n = kv.second;
+            if (n.kind == K_COMP && !n.readout_q.empty()) b->comp_readout_outs[kv.first].add(n_graphs, j, n.readout_q.size());
             if (n.kind != K_ANALYSER || !n.readout_kinds) continue;
             for (uint32_t kind : {(uint32_t)WAE_READOUT_FREQUENCY, (uint32_t)WAE_READOUT_TIME_DOMAIN}) {
                 if (!(n.readout_kinds & kind)) continue;
-                ReadoutOut& r = b->readout_outs[{kv.first, kind}];
-                if (r.off.empty()) {
-                    r.off.assign(n_graphs, UINT64_MAX);
-                    r.len.assign(n_graphs, 0);
-                }
-                r.off[j] = r.floats;
-                r.len[j] = (uint64_t)n.readout_q.size() * (kind == WAE_READOUT_FREQUENCY ? n.fft_size / 2 : n.fft_size);
-                r.floats += r.len[j];
+                const uint64_t elems = (uint64_t)n.readout_q.size() * (kind == WAE_READOUT_FREQUENCY ? n.fft_size / 2 : n.fft_size);
+                b->readout_outs[{kv.first, kind}].add(n_graphs, j, elems);
+                if (n.byte_readout_kinds & kind) b->byte_readout_outs[{kv.first, kind}].add(n_graphs, j, elems);
             }
         }
     }
     for (auto& kv : b->readout_outs)
-        if (!(kv.second.d = b->dalloc<float>(kv.second.floats))) return fail(WAE_OUT_OF_MEMORY, "out of device memory (analyser read-outs)");
+        if (!(kv.second.d = b->dalloc<float>(kv.second.count))) return fail(WAE_OUT_OF_MEMORY, "out of device memory (analyser read-outs)");
+    for (auto& kv : b->byte_readout_outs)
+        if (!(kv.second.d = b->dalloc<uint8_t>(kv.second.count))) return fail(WAE_OUT_OF_MEMORY, "out of device memory (analyser read-outs)");
+    for (auto& kv : b->comp_readout_outs)
+        if (!(kv.second.d = b->dalloc<float>(kv.second.count, true))) return fail(WAE_OUT_OF_MEMORY, "out of device memory (compressor read-outs)");
     return WAE_OK;
 }
 
@@ -5344,7 +5388,7 @@ static void launch_stage(wae_batch* b, Stage& st, ChunkInfo ci) {
         case S_ROUTE: launch_route((RouteInst*)st.d_a, st.n, ci, s); break;
         case S_DELAY: launch_delay_read((DelayInst*)st.d_a, st.n, ci, s); break;
         case S_DELAY_WRITE: launch_ring_write((DelayInst*)st.d_a, st.n, ci, s); break;
-        case S_COMP: launch_compressor((CompInst*)st.d_a, st.n, ci, s); break;
+        case S_COMP: launch_compressor((CompInst*)st.d_a, (const CompReadoutInst*)st.d_b, st.n, ci, s); break;
         case S_ANALYSER: launch_analyser((AnalyserInst*)st.d_a, st.n, ci, s); break;
         case S_READOUT_FFT:
         case S_READOUT_TIME: {  // the records with f0 < frame <= f0 + nf (frame 0: the first chunk)
@@ -6495,6 +6539,9 @@ static wae_status refuse_device_inputs(wae_graph* const* graphs, uint32_t n_grap
         if (graphs[i] && graphs[i]->analyser_readouts)  // (a one-shot render returns no read-outs)
             return fail(WAE_INVALID_STATE, "graph " + std::to_string(i) + " has analyser read-outs declared: render it with wae_batch_prepare " +
                                                "(or _prepare_many) and wae_batch_run, and read them with wae_batch_fetch_analyser_readouts");
+        if (graphs[i] && graphs[i]->compressor_readouts)
+            return fail(WAE_INVALID_STATE, "graph " + std::to_string(i) + " has compressor read-outs declared: render it with wae_batch_prepare " +
+                                               "(or _prepare_many) and wae_batch_run, and read them with wae_batch_fetch_compressor_readouts");
     }
     return WAE_OK;
 }
@@ -6567,32 +6614,71 @@ WAE_API wae_status wae_analyser_get_float_frequency_data(wae_batch* b, uint32_t 
     return WAE_OK;
 }
 
-// The rows of the declared read-outs of one (node, kind) over the batch (wae_analyser_set_readouts)
-static const ReadoutOut* find_readouts(wae_batch* b, wae_node_id node, uint32_t kind) {
-    if (!b || (kind != WAE_READOUT_FREQUENCY && kind != WAE_READOUT_TIME_DOMAIN)) return nullptr;
-    auto it = b->readout_outs.find({node, kind});
-    return it == b->readout_outs.end() ? nullptr : &it->second;
+// The rows of the declared read-outs over the batch (wae_analyser_set_readouts, wae_analyser_set_byte_readouts, wae_compressor_set_readouts)
+extern "C++" {  // (templates inside the C ABI's extern "C" block)
+template <typename K, typename T>
+static const ReadoutRows<T>* find_rows(wae_batch* b, std::map<K, ReadoutRows<T>> wae_batch::*m, const K& key) {
+    if (!b) return nullptr;
+    auto it = (b->*m).find(key);
+    return it == (b->*m).end() ? nullptr : &it->second;
 }
+static bool readout_kind_ok(uint32_t kind) { return kind == WAE_READOUT_FREQUENCY || kind == WAE_READOUT_TIME_DOMAIN; }
+// one graph's rows to the host; `what`: the declaration, as the refusal names it
+template <typename T>
+static wae_status fetch_rows(wae_batch* b, const ReadoutRows<T>* r, uint32_t graph_index, T* host_out, uint64_t count, const char* what,
+                             const char* unit) {
+    if (!host_out) return fail(WAE_INVALID_ARGUMENT, "null output");
+    if (!r || graph_index >= b->n_graphs || r->off[b->batch_pos(graph_index)] == UINT64_MAX)
+        return fail(WAE_INVALID_ARGUMENT, "graph " + std::to_string(graph_index) + " declares no " + what);
+    const uint32_t j = b->batch_pos(graph_index);
+    if (count != r->len[j]) return fail(WAE_INVALID_ARGUMENT, "the graph's read-outs are " + std::to_string(r->len[j]) + " " + unit);
+    CUDA_TRY(cudaSetDevice(b->engine->device));
+    CUDA_TRY(cudaMemcpyAsync(host_out, r->d + r->off[j], count * sizeof(T), cudaMemcpyDeviceToHost, b->engine->stream));
+    CUDA_TRY(cudaStreamSynchronize(b->engine->stream));
+    return WAE_OK;
+}
+}  // extern "C++"
 WAE_API wae_status wae_batch_analyser_readouts_device_ptr(wae_batch* b, wae_node_id node, uint32_t kind, float** ptr, uint64_t* floats) {
     if (!ptr || !floats) return fail(WAE_INVALID_ARGUMENT, "null argument");
-    const ReadoutOut* r = find_readouts(b, node, kind);
+    const ReadoutOut* r = readout_kind_ok(kind) ? find_rows(b, &wae_batch::readout_outs, {node, kind}) : nullptr;
     if (!r) return fail(WAE_INVALID_ARGUMENT, "no graph of this batch declares read-outs of that kind on that node");
     *ptr = r->d;
-    *floats = r->floats;
+    *floats = r->count;
     return WAE_OK;
 }
 WAE_API wae_status wae_batch_fetch_analyser_readouts(wae_batch* b, uint32_t graph_index, wae_node_id node, uint32_t kind, float* host_out,
                                                      uint64_t floats) {
     if (!host_out) return fail(WAE_INVALID_ARGUMENT, "null output");
-    const ReadoutOut* r = find_readouts(b, node, kind);
-    if (!r || graph_index >= b->n_graphs || r->off[b->batch_pos(graph_index)] == UINT64_MAX)
-        return fail(WAE_INVALID_ARGUMENT, "graph " + std::to_string(graph_index) + " declares no read-outs of that kind on that node");
-    const uint32_t j = b->batch_pos(graph_index);
-    if (floats != r->len[j]) return fail(WAE_INVALID_ARGUMENT, "the graph's read-outs are " + std::to_string(r->len[j]) + " floats");
-    CUDA_TRY(cudaSetDevice(b->engine->device));
-    CUDA_TRY(cudaMemcpyAsync(host_out, r->d + r->off[j], floats * sizeof(float), cudaMemcpyDeviceToHost, b->engine->stream));
-    CUDA_TRY(cudaStreamSynchronize(b->engine->stream));
+    const ReadoutOut* r = readout_kind_ok(kind) ? find_rows(b, &wae_batch::readout_outs, {node, kind}) : nullptr;
+    return fetch_rows(b, r, graph_index, host_out, floats, "read-outs of that kind on that node", "floats");
+}
+WAE_API wae_status wae_batch_analyser_byte_readouts_device_ptr(wae_batch* b, wae_node_id node, uint32_t kind, uint8_t** ptr,
+                                                               uint64_t* bytes) {
+    if (!ptr || !bytes) return fail(WAE_INVALID_ARGUMENT, "null argument");
+    const ReadoutRows<uint8_t>* r = readout_kind_ok(kind) ? find_rows(b, &wae_batch::byte_readout_outs, {node, kind}) : nullptr;
+    if (!r) return fail(WAE_INVALID_ARGUMENT, "no graph of this batch declares byte read-outs of that kind on that node");
+    *ptr = r->d;
+    *bytes = r->count;
     return WAE_OK;
+}
+WAE_API wae_status wae_batch_fetch_analyser_byte_readouts(wae_batch* b, uint32_t graph_index, wae_node_id node, uint32_t kind,
+                                                          uint8_t* host_out, uint64_t bytes) {
+    if (!host_out) return fail(WAE_INVALID_ARGUMENT, "null output");
+    const ReadoutRows<uint8_t>* r = readout_kind_ok(kind) ? find_rows(b, &wae_batch::byte_readout_outs, {node, kind}) : nullptr;
+    return fetch_rows(b, r, graph_index, host_out, bytes, "byte read-outs of that kind on that node", "bytes");
+}
+WAE_API wae_status wae_batch_compressor_readouts_device_ptr(wae_batch* b, wae_node_id node, float** ptr, uint64_t* floats) {
+    if (!ptr || !floats) return fail(WAE_INVALID_ARGUMENT, "null argument");
+    const ReadoutOut* r = find_rows(b, &wae_batch::comp_readout_outs, node);
+    if (!r) return fail(WAE_INVALID_ARGUMENT, "no graph of this batch declares compressor read-outs on that node");
+    *ptr = r->d;
+    *floats = r->count;
+    return WAE_OK;
+}
+WAE_API wae_status wae_batch_fetch_compressor_readouts(wae_batch* b, uint32_t graph_index, wae_node_id node, float* host_out,
+                                                       uint64_t floats) {
+    if (!host_out) return fail(WAE_INVALID_ARGUMENT, "null output");
+    return fetch_rows(b, find_rows(b, &wae_batch::comp_readout_outs, node), graph_index, host_out, floats, "compressor read-outs on that node", "floats");
 }
 
 // Analyser::get_byte_time_domain_data (src/analysis.rs:266-276): 128 (1 + x) clamped to a byte

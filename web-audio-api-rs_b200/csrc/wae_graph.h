@@ -174,9 +174,10 @@ struct Node {
     // analyser
     uint32_t fft_size = 2048;
     double smoothing = 0.8, min_db = -100., max_db = -30.;
-    // wae_analyser_set_readouts: the read-out quanta (non-decreasing) and WAE_READOUT_* kinds.  Empty: not declared
+    // wae_analyser_set_readouts / wae_compressor_set_readouts: the read-out quanta (non-decreasing).  Empty: not declared
     std::vector<uint64_t> readout_q;
-    uint32_t readout_kinds = 0;
+    uint32_t readout_kinds = 0;       // analyser: WAE_READOUT_* kinds
+    uint32_t byte_readout_kinds = 0;  // analyser: the kinds also delivered as bytes (wae_analyser_set_byte_readouts)
     Param param;  // K_PARAM only
 };
 
@@ -295,6 +296,7 @@ struct wae_graph {
     uint32_t device_schedules = 0;     // scheduled sources declared with wae_source_set_device_schedule
     uint32_t device_loops = 0;         // AudioBufferSourceNodes declared with wae_buffer_source_set_device_loop
     uint32_t analyser_readouts = 0;    // AnalyserNodes declared with wae_analyser_set_readouts
+    uint32_t compressor_readouts = 0;  // DynamicsCompressorNodes declared with wae_compressor_set_readouts
 
     uint32_t create_param(uint32_t owner, float def, float mn, float mx, bool a_rate, float initial, bool send_set_value = true,
                           bool fixed_id = false, uint32_t id = 0, bool constrained = false);

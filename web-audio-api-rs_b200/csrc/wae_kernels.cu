@@ -3284,10 +3284,27 @@ __global__ void __launch_bounds__(256) k_ring_write(const DelayInst* __restrict_
 // ---------------------------------------------------------------------------------------------------------
 DEVI float db_to_lin(float v) { return powf(10.0f, v / 20.f); }
 DEVI float lin_to_db(float v) { return v == 0.f ? -1000.f : 20.f * log10f(v); }
-__global__ void __launch_bounds__(32) k_compressor(const CompInst* __restrict__ insts, int n_inst, ChunkInfo ci) {
+// READOUTS: the instances declare reduction read-outs (wae_compressor_set_readouts), `ro` parallel to `insts`: at the end of each
+// quantum the reduction is written to the rows of the read-outs at that frame (those at frame 0: at the start of the first chunk)
+template <bool READOUTS>
+__global__ void __launch_bounds__(32) k_compressor(const CompInst* __restrict__ insts, const CompReadoutInst* __restrict__ ro, int n_inst,
+                                                   ChunkInfo ci) {
     int ii = blockIdx.x * blockDim.x + threadIdx.x;
     if (ii >= n_inst) return;
     const CompInst q = insts[ii];
+    CompReadoutInst r{};
+    int rk = 0;  // the next read-out: the first with frame > f0 (>= 0 in the first chunk)
+    if (READOUTS) {
+        r = ro[ii];
+        const int64_t lo = ci.f0 == 0 ? -1 : ci.f0;
+        int b = r.n;
+        while (rk < b) {
+            const int m = (rk + b) >> 1;
+            if (r.frames[m] > lo) b = m;
+            else rk = m + 1;
+        }
+        for (; rk < r.n && r.frames[rk] == 0; rk++) r.rows[rk] = 0.f;  // before the first quantum (the reference's initial value)
+    }
     float thr = 0.f, half_knee = 0.f, knee_partial = 0.f, attack_tau = 0.f, release_tau = 0.f, makeup_gain = 0.f, ratio = 1.f;
     const bool automated = q.track[0].p || q.track[1].p || q.track[2].p || q.track[3].p || q.track[4].p;
     float prev = q.state[0];
@@ -3356,6 +3373,8 @@ __global__ void __launch_bounds__(32) k_compressor(const CompInst* __restrict__ 
             reduction_gain = red;
             prev = det;
         }
+        if (READOUTS && (n & 127) == 127)
+            for (; rk < r.n && r.frames[rk] == ci.f0 + n + 1; rk++) r.rows[rk] = reduction_gain;
         int64_t m = ci.f0 + n - q.delay_frames;
         for (int c = 0; c < q.ch; c++) {
             float x = 0.f;
@@ -4934,10 +4953,19 @@ __global__ void __launch_bounds__(256) k_readout_fft(const ReadoutInst* __restri
     for (int k = threadIdx.x; k < n; k += blockDim.x) r.row[k] = analyser_bin_magnitude(zf, k, n, r.fft_size);
 }
 
-// Time-domain read-outs: the window itself (get_float_time_domain_data, analysis.rs:261-264)
+// Analyser::get_byte_* (analysis.rs:266-276, 371-401): clamp(v, 0, 255) as u8 in f32 arithmetic; Rust's `as u8` maps NaN to 0
+__device__ __forceinline__ uint8_t readout_byte(float v) {
+    return (uint8_t)__float2uint_rz(!(v > 0.f) ? 0.f : fminf(v, 255.f));
+}
+
+// Time-domain read-outs: the window itself (get_float_time_domain_data, analysis.rs:261-264); its bytes 128 (1 + x) (:266-276)
 __global__ void __launch_bounds__(256) k_readout_time(const ReadoutInst* __restrict__ insts, ChunkInfo ci) {
     const ReadoutInst r = insts[blockIdx.x];
-    for (int i = blockIdx.y * blockDim.x + threadIdx.x; i < r.fft_size; i += gridDim.y * blockDim.x) r.row[i] = readout_sample(r, i, ci);
+    for (int i = blockIdx.y * blockDim.x + threadIdx.x; i < r.fft_size; i += gridDim.y * blockDim.x) {
+        const float x = readout_sample(r, i, ci);
+        r.row[i] = x;
+        if (r.bytes) r.bytes[i] = readout_byte(__fmul_rn(128.f, __fadd_rn(1.f, x)));
+    }
 }
 
 // One thread per (analyser, bin): the analyser's frequency read-outs of the chunk in time order, smoothed with the state the previous
@@ -4957,11 +4985,14 @@ __global__ void __launch_bounds__(256) k_readout_smooth(const ReadoutSmoothInst*
     }
     if (a >= s.n || s.frames[a] > hi) return;
     float last = s.last_fft[bin], db = 0.f;
+    // byte rows: 255 / (max - min) * (dB - min) (analysis.rs:390-398), rounded as numpy's f32 statement of it
+    const float scale = s.bytes ? __fdiv_rn(255.f, __fsub_rn(s.max_db, s.min_db)) : 0.f;
     for (int k = a; k < s.n && s.frames[k] <= hi; k++) {
         float* row = s.rows + (size_t)k * s.bins;
         if (k > 0 && s.frames[k] == s.frames[k - 1]) db = row[(int64_t)-s.bins + bin];
         else db = 20.f * log10f(last = analyser_smooth(s.smoothing, last, row[bin]));
         row[bin] = db;
+        if (s.bytes) s.bytes[(size_t)k * s.bins + bin] = readout_byte(__fmul_rn(scale, __fsub_rn(db, s.min_db)));
         if (k == s.n - 1) s.db[bin] = db;
     }
     s.last_fft[bin] = last;
@@ -5387,7 +5418,10 @@ void launch_param(const ParamInst* d, int n, ChunkInfo ci, cudaStream_t s, int m
     else if (mode == 1) k_param_parallel<<<(n + PARAM_WARPS - 1) / PARAM_WARPS, 32 * PARAM_WARPS, 0, s>>>(d, n, ci);
     else k_param<<<(n + PARAM_WARPS - 1) / PARAM_WARPS, 32 * PARAM_WARPS, 0, s>>>(d, n, ci);
 }
-void launch_compressor(const CompInst* d, int n, ChunkInfo ci, cudaStream_t s) { k_compressor<<<(n + 31) / 32, 32, 0, s>>>(d, n, ci); }
+void launch_compressor(const CompInst* d, const CompReadoutInst* ro, int n, ChunkInfo ci, cudaStream_t s) {
+    if (ro) k_compressor<true><<<(n + 31) / 32, 32, 0, s>>>(d, ro, n, ci);
+    else k_compressor<false><<<(n + 31) / 32, 32, 0, s>>>(d, nullptr, n, ci);
+}
 void launch_analyser(const AnalyserInst* d, int n, ChunkInfo ci, cudaStream_t s) { k_analyser<<<grid_tiles(ci.nf, 256, n), 256, 0, s>>>(d, n, ci); }
 static void conv_configure() {
     static bool configured = false;

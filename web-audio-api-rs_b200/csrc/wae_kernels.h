@@ -339,7 +339,8 @@ void launch_biquad_arate(const BiquadArInst* d, int n, int max_ch, ChunkInfo ci,
 void launch_analyser_fft(const float* ring, uint32_t write_index, int fft_size, float smoothing, float* last_fft, float* out_db, cudaStream_t s);
 void launch_resample_linear(const float* in, int64_t len, float* out, int64_t target_len, cudaStream_t s);
 void launch_param(const ParamInst* d, int n, ChunkInfo ci, cudaStream_t s, int mode);  // 0: k_param, 1: k_param_parallel, 2: k_param_spec
-void launch_compressor(const CompInst* d, int n, ChunkInfo ci, cudaStream_t s);
+// ro != nullptr: the instances' reduction read-outs (wae_compressor_set_readouts), parallel to d
+void launch_compressor(const CompInst* d, const CompReadoutInst* ro, int n, ChunkInfo ci, cudaStream_t s);
 void launch_analyser(const AnalyserInst* d, int n, ChunkInfo ci, cudaStream_t s);
 // declared analyser read-outs (wae_analyser_set_readouts): `d` = the chunk's n records, max_fft / max_bins = the largest of the stage
 void launch_readout_fft(const ReadoutInst* d, int n, int max_fft, ChunkInfo ci, cudaStream_t s);
