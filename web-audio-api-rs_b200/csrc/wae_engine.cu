@@ -18,6 +18,7 @@
 #include <emmintrin.h>
 
 #include <algorithm>
+#include <array>
 #include <atomic>
 #include <chrono>
 #include <condition_variable>
@@ -256,6 +257,54 @@ const char* kStageNames[S_KINDS] = {"k_mix", "k_mix_dyn", "k_oscillator", "k_con
                                     "k_analyser", "k_conv_fft_in", "k_conv_mac_ifft", "k_conv_mac_ifft(acc)", "k_chain", "k_param", "k_osc_arate", "k_biquad_arate", "k_buffer_source_slow", "k_hrtf_fir", "k_panner_dyn", "k_buffer_source_serial", "k_shaper_os", "k_meta", "k_voice_sum", "k_conv_compact",
                                     "k_buffer_source_slow(bound)", "k_readout_fft", "k_readout_time", "k_readout_smooth"};
 
+// Bind entries: what prepare uploads for the binds from device memory to rewrite planned records.  The planner records one Entry per
+// device entry in the stage whose records it reaches.  Its payload is the device entry; the payload's pointers into the stage's records
+// are named by references (table, record, offset into the record) until the tables are uploaded: merge_builds rebases the records,
+// prep_plan_group writes each address into the payload field `field` bytes from its start.  Prepare uploads the entries of each kind
+// in group, stage and planning order.
+enum EntryKind : int32_t {
+    E_PARAM,      // ParamPatch (d_patches): a param bound from device memory (wae_param_set_device_value); operands name their param by
+                  // node id (slot) until prepare numbers the value slots
+    E_SPATIAL,    // SpatialPatch (d_spatial): a static panner whose source or listener is bound from device memory, operands as E_PARAM
+    E_CURVE,      // CurvePatch (d_curve_patches): the int32 field that takes `keeps` or `other` as a bound curve maps 0 to 0 or not
+    E_IIR,        // IirPatch (d_iir_patches): the coefficients of an IirInst or a ChainBiquad, and that biquad's scan constants
+    E_SCHED,      // SchedPatch (d_sched_patches): the fields of a source whose start and stop times are bound from device memory
+    E_LOOP,       // LoopPatch (d_loop_patches): a record whose loop points are bound from device memory
+    E_LOOP_WALK,  // LoopWalk (d_loop_walks): a looping S_ABSN_BOUND record whose playhead table is derived on the device
+    E_OUT,        // OutPatch (d_out_patches): the BufRef::p of a destination writer (wae_batch_bind_output)
+    E_SRC_REF,    // SrcRefPatch (d_src_refs): the PCM pointer and channel stride of a source declared by reference
+    E_KINDS
+};
+constexpr size_t kEntryPayloadBytes[E_KINDS] = {sizeof(ParamPatch), sizeof(SpatialPatch), sizeof(CurvePatch), sizeof(IirPatch),
+                                                sizeof(SchedPatch), sizeof(LoopPatch), sizeof(LoopWalk), sizeof(OutPatch), sizeof(SrcRefPatch)};
+enum StageTable : int32_t { T_NONE = 0, T_A, T_B, T_C };  // Stage::d_a, d_b, d_c (see StageBuild::table)
+struct FieldRef {
+    int32_t table;   // StageTable
+    int32_t rec;     // record of that table
+    uint32_t off;    // bytes into the record
+    uint32_t field;  // bytes into the payload of the pointer that takes the address
+};
+struct Entry {  // (trivially copyable, made zeroed by Planner::entry: its bytes are digested)
+    int32_t kind;      // EntryKind
+    uint32_t graph;    // batch position
+    wae_node_id node;  // the declaration a node-level kind belongs to (E_CURVE, E_IIR, E_SCHED, E_LOOP, E_SRC_REF), else 0
+    FieldRef ref[3];   // T_NONE: unused (addresses the planner sets itself are in the payload already)
+    union Payload {
+        ParamPatch param;
+        SpatialPatch spatial;
+        CurvePatch curve;
+        IirPatch iir;
+        SchedPatch sched;
+        LoopPatch loop;
+        LoopWalk walk;
+        OutPatch out;
+        SrcRefPatch src_ref;
+    } p;
+    float2* spec;  // SPATIAL_RESP: the spectra of `S` partitions its bind transforms the blended pair into
+    int32_t S;
+    void refer(int i, int t, int32_t rec, size_t off, size_t field) { ref[i] = FieldRef{t, rec, (uint32_t)off, (uint32_t)field}; }
+};
+
 // host-side accumulation of instances for one (level, kind) stage
 struct StageBuild {
     int cls = 0;
@@ -307,162 +356,66 @@ struct StageBuild {
     std::vector<ConvCmpInst> conv_cmp;  // S_CONV_CMP: compacted second path of a mono-response convolver
     std::vector<VoiceGroup> vgroups;  // S_VSUM: groups of consecutive `chain` records
     int max_ch = 1;
-    // Patch entries of params bound from device memory (wae_param_set_device_value) into this stage's records: record `rec` of the
-    // stage's own table, `off` bytes into it; `rec2`: the scan constants (S_CHAIN / S_VSUM) or the stereo gains (S_SPAN) it also
-    // re-derives, -1: none.  Operands name their param by node id (patch.slot) until the batch numbers its value slots.
-    struct PatchRec {
-        ParamPatch p;
-        uint32_t graph;  // batch position
-        int32_t rec, rec2;
-        uint32_t off;
+    std::vector<Entry> entries;  // the bind entries of this stage's records, every kind in one list
+    // The stage's tables as prep_plan_group uploads them: T_A (Stage::d_a) holds the instances; T_B (d_b) the mix edges (S_MIX,
+    // S_MIX_DYN), scan constants (S_CHAIN, S_VSUM; the sizing pass counts them without building them), stereo gains (S_SPAN), selection
+    // records of moving panners (S_HRTF) or read-outs (S_COMP); T_C (d_c) the voice groups (S_VSUM).  Rows and bytes of one row.
+    struct Shape {
+        size_t n = 0, bytes = 0;
     };
-    std::vector<PatchRec> patches;
-    // Patch entries of WaveShaper curves bound from device memory (wae_wave_shaper_set_device_curve): the int32 field `off` bytes into
-    // record `rec` of this stage's table takes `keeps` or `other` as the bound curve maps 0 to 0 or not
-    struct CurvePatchRec {
-        uint32_t graph;  // batch position
-        wae_node_id node;
-        int32_t rec;
-        uint32_t off;
-        int32_t keeps, other;
-    };
-    std::vector<CurvePatchRec> curve_patches;
-    // Patch entries of IIR coefficients bound from device memory (wae_iir_filter_set_device_coefficients): record `rec` of this stage's
-    // table, an IirInst (S_IIR, bq = -1) or biquad `bq` of a ChainInst (S_CHAIN / S_VSUM) with its scan constants `scan`
-    struct IirPatchRec {
-        uint32_t graph;  // batch position
-        wae_node_id node;
-        int32_t rec, bq, scan;
-    };
-    std::vector<IirPatchRec> iir_patches;
-    // Patch entries of schedules bound from device memory (wae_source_set_device_schedule): the source's fields `off` bytes into record
-    // `rec` of this stage's table (an OscInst / ConstInst inside a ChainInst, or the record itself)
-    struct SchedPatchRec {
-        uint32_t graph;  // batch position
-        wae_node_id node;
-        int32_t rec;
-        uint32_t off;
-        SchedPatch p;    // dst set when the tables are uploaded
-    };
-    std::vector<SchedPatchRec> sched_patches;
-    // Patch entries of loop points bound from device memory (wae_buffer_source_set_device_loop): record `rec` of this stage's table
-    // (S_ABSN_BOUND / S_ABSN_SERIAL); and the looping S_ABSN_BOUND records whose playhead tables are derived on the device
-    struct LoopPatchRec {
-        uint32_t graph;  // batch position
-        wae_node_id node;
-        int32_t rec;
-        LoopPatch p;     // dst set when the tables are uploaded
-    };
-    std::vector<LoopPatchRec> loop_patches;
-    struct LoopWalkRec {
-        int32_t rec;
-        int32_t cap;
-        int64_t lq;
-    };
-    std::vector<LoopWalkRec> loop_walks;
-    // Spatial entries of static panners whose source or listener is bound from device memory (wae_param_set_device_value): record `rec`
-    // of this stage's table (S_PAN: PanInst, S_HRTF: HrtfInst), `off` bytes into it, or -1 for an HRTF panner lowered to a convolver,
-    // whose entry's dst / resp the planner sets and whose bind also rewrites the spectra `spec` of `S` partitions.  Operands name their
-    // param by node id (p.slot) until the batch numbers its value slots.
-    struct SpatialPatchRec {
-        SpatialPatch p;
-        uint32_t graph;  // batch position
-        int32_t rec;
-        uint32_t off;
-        float2* spec;
-        int32_t S;
-    };
-    std::vector<SpatialPatchRec> spatial;
-    size_t spatial_records() const { return kind == S_PAN ? pan.size() : kind == S_HRTF ? hrtf.size() : 0; }
-    // Output entries (wae_batch_bind_output): the BufRef `off` bytes into record `rec` of this stage's destination-writer table (see
-    // out_records) is the rendered PCM of graph `graph`, `dest` floats into the packed output
-    struct OutPatchRec {
-        uint64_t dest;
-        int32_t rec;
-        uint32_t off;
-        uint32_t graph;  // batch position
-        uint32_t pad;
-    };
-    std::vector<OutPatchRec> out_patches;
-    // Source-reference entries (wae_buffer_source_set_device_input_by_reference): the PCM pointer `buf` bytes and the channel stride
-    // `stride` bytes into record `rec` of this stage's table (AbsnInst, AbsnSlowInst, AbsnBoundInst, AbsnSerialInst, or the AbsnInst of a
-    // ChainInst)
-    struct SrcRefRec {
-        uint32_t graph;  // batch position
-        wae_node_id node;
-        int32_t rec;
-        uint32_t buf, stride;
-    };
-    std::vector<SrcRefRec> src_refs;
-    size_t out_records() const {
+    template <typename T>
+    static Shape shape(const std::vector<T>& v) { return {v.size(), sizeof(T)}; }
+    Shape table(int t) const {
+        if (t == T_B) switch (kind) {
+            case S_MIX: case S_MIX_DYN: return shape(mix_edges);
+            case S_CHAIN: case S_VSUM: return {n_scan_coef, sizeof(ScanCoef)};
+            case S_SPAN: return shape(span_gains);
+            case S_HRTF: return shape(hrtf_sel);
+            case S_COMP: return shape(comp_ro);
+            default: return {};  // (S_CONV_MAC, S_CONV_MAC_ACC: the conv inputs of their level's S_CONV_FFT stage)
+        }
+        if (t == T_C) return kind == S_VSUM ? shape(vgroups) : Shape{};
         switch (kind) {
-            case S_MIX: return mix.size();
-            case S_MIX_DYN: return mix_dyn.size();
-            case S_CHAIN: return chain.size();
-            case S_VSUM: return vgroups.size();
-            case S_CONV_MAC: case S_CONV_MAC_ACC: return conv_path.size();
-            default: return 0;
+            case S_MIX: return shape(mix);
+            case S_MIX_DYN: return shape(mix_dyn);
+            case S_META: return shape(meta);
+            case S_OSC: return shape(osc);
+            case S_CONST: return shape(cst);
+            case S_ABSN: return shape(absn);
+            case S_BIQUAD: return shape(biquad);
+            case S_CHAIN: case S_VSUM: return shape(chain);
+            case S_PARAM: return shape(param);
+            case S_OSC_AR: return shape(osc_ar);
+            case S_BIQUAD_AR: return shape(biquad_ar);
+            case S_ABSN_SLOW: return shape(absn_slow);
+            case S_IIR: return shape(iir);
+            case S_GAIN: return shape(gain);
+            case S_SHAPER: return shape(shaper);
+            case S_SPAN: return shape(span);
+            case S_PAN: return shape(pan);
+            case S_HRTF: return shape(hrtf);
+            case S_PAN_DYN: return shape(pan_dyn);
+            case S_ABSN_SERIAL: return shape(absn_serial);
+            case S_ABSN_BOUND: return shape(absn_bound);
+            case S_SHAPER_OS: return shape(shaper_os);
+            case S_ROUTE: return shape(route);
+            case S_DELAY_MONO: case S_DELAY: case S_DELAY_WRITE: return shape(delay);
+            case S_COMP: return shape(comp);
+            case S_ANALYSER: return shape(analyser);
+            case S_CONV_FFT: return shape(conv_in);
+            case S_CONV_CMP: return shape(conv_cmp);
+            case S_CONV_MAC: case S_CONV_MAC_ACC: return shape(conv_path);
+            default: return {};  // (S_READOUT_*: uploaded sorted by frame, no entry points into them)
         }
     }
-    size_t out_record_bytes() const {
-        switch (kind) {
-            case S_MIX: return sizeof(MixInst);
-            case S_MIX_DYN: return sizeof(MixDynInst);
-            case S_CHAIN: return sizeof(ChainInst);
-            case S_VSUM: return sizeof(VoiceGroup);
-            case S_CONV_MAC: case S_CONV_MAC_ACC: return sizeof(ConvPath);
-            default: return 0;
-        }
-    }
-    // size of the table patch entries point into (S_HRTF: the selection records of its moving panners, the stage's second table)
-    size_t records() const {
-        switch (kind) {
-            case S_OSC: return osc.size();
-            case S_OSC_AR: return osc_ar.size();
-            case S_CONST: return cst.size();
-            case S_IIR: return iir.size();
-            case S_SHAPER_OS: return shaper_os.size();
-            case S_CHAIN: case S_VSUM: return chain.size();
-            case S_BIQUAD: return biquad.size();
-            case S_BIQUAD_AR: return biquad_ar.size();
-            case S_GAIN: return gain.size();
-            case S_SPAN: return span.size();
-            case S_COMP: return comp.size();
-            case S_META: return meta.size();
-            case S_ABSN: return absn.size();
-            case S_ABSN_SLOW: return absn_slow.size();
-            case S_ABSN_SERIAL: return absn_serial.size();
-            case S_ABSN_BOUND: return absn_bound.size();
-            case S_PAN_DYN: return pan_dyn.size();
-            case S_HRTF: return hrtf_sel.size();
-            default: return 0;
-        }
-    }
-    size_t record_bytes() const {  // size of one record of that table
-        switch (kind) {
-            case S_OSC: return sizeof(OscInst);
-            case S_OSC_AR: return sizeof(OscArInst);
-            case S_CONST: return sizeof(ConstInst);
-            case S_IIR: return sizeof(IirInst);
-            case S_SHAPER_OS: return sizeof(ShaperOsInst);
-            case S_CHAIN: case S_VSUM: return sizeof(ChainInst);
-            case S_BIQUAD: return sizeof(BiquadInst);
-            case S_BIQUAD_AR: return sizeof(BiquadArInst);
-            case S_GAIN: return sizeof(GainInst);
-            case S_SPAN: return sizeof(SPanInst);
-            case S_COMP: return sizeof(CompInst);
-            case S_META: return sizeof(MetaInst);
-            case S_ABSN: return sizeof(AbsnInst);
-            case S_ABSN_SLOW: return sizeof(AbsnSlowInst);
-            case S_ABSN_SERIAL: return sizeof(AbsnSerialInst);
-            case S_ABSN_BOUND: return sizeof(AbsnBoundInst);
-            case S_PAN_DYN: return sizeof(PanDynInst);
-            case S_HRTF: return sizeof(HrtfSelInst);
-            default: return 0;
-        }
+    size_t records(int t = T_A) const { return table(t).n; }
+    size_t record_bytes(int t) const { return table(t).bytes; }
+    // records entry `e` for the last record of table `t`, its reference 0 `off` bytes into it (filling the payload field `field`)
+    void add_entry(Entry e, size_t off, size_t field, int t = T_A) {
+        e.refer(0, t, (int32_t)records(t) - 1, off, field);
+        entries.push_back(e);
     }
 };
-using PatchRec = StageBuild::PatchRec;
 
 struct Stage {
     int cls = 0;  // see Planner::stage()
@@ -609,14 +562,6 @@ struct Bindings : BindTable {
                 for (const auto& kv : ep.nodes) visit(j, ep.nodes, kv.second, declare);
         }
     }
-};
-
-// a patch entry of the declaration (graph, node) of a kind declared on a node, its device addresses set
-template <typename P>
-struct PatchEntry {
-    uint32_t graph;  // batch position
-    wae_node_id node;
-    P p;
 };
 
 // What the binds write, per kind
@@ -1161,20 +1106,16 @@ struct Planner {
         int phase = 0;  // 0: before biquad A, 1: after A, 3: after B, 5: after the shaper (canonical chain order)
         int cls = 0;    // scheduling class of the node that opened the chain (see stage())
         Lay lay;        // layout of the chain's output over time (the kernel writes the track when it is not constant)
-        // params bound from device memory: the source oscillator's PATCH_OSC entry and biquad k's patch entries (rec2 = k until the
-        // chain is emitted), and per gain slot the factors folded into it since the first bound one (gain_fold[s].p.n == 0: the slot
-        // has none)
-        std::vector<PatchRec> patches;
-        PatchRec gain_fold[4] = {};
-        // a shaper whose curve is bound from device memory: the entry of shaper_keeps_silence (rec / off set when the chain is emitted)
-        std::vector<StageBuild::CurvePatchRec> curve_patches;
-        // IIR filters whose coefficients are bound from device memory: the entry of their biquad (bq; rec / scan set when the chain is
-        // emitted)
-        std::vector<StageBuild::IirPatchRec> iir_patches;
-        // a source whose schedule is bound from device memory: the entry of ChainInst::osc / ::cst (rec set when the chain is emitted)
-        std::vector<StageBuild::SchedPatchRec> sched_patches;
-        // a source declared by reference: the entry of ChainInst::absn (rec set when the chain is emitted)
-        std::vector<StageBuild::SrcRefRec> src_refs;
+        // the bind entries of the chain's record: their T_A references take the record's index when the chain is emitted, their T_B
+        // references name biquad k until then and its scan constants after; and per gain slot the param entry of the factors folded into
+        // it since the first bound one (gain_fold[s].p.param.n == 0: the slot has none)
+        std::vector<Entry> entries;
+        Entry gain_fold[4] = {};
+        // entry `e` with reference 0 `off` bytes into the chain's record (filling the payload field `field`)
+        void add_entry(Entry e, size_t off, size_t field) {
+            e.refer(0, T_A, -1, off, field);
+            entries.push_back(e);
+        }
     };
 
     // Node state is allocated through a key (graph, node, n-th allocation of that node, salt): the plans of consecutive
@@ -1257,9 +1198,11 @@ struct Planner {
     int64_t lq = 0, glq = 0;
     // the graph's rendered PCM in the packed output: [channels][length], frames from `length` on are not written (limit)
     BufRef dest_ref() const { return BufRef{b->d_out + b->out_off[gi], (uint32_t)g->length, 1}; }
-    // the output entry of the last record of `s`'s destination-writer table, whose BufRef `off` bytes into it is dest_ref()
-    void add_out(StageBuild& s, size_t off) const {
-        s.out_patches.push_back(StageBuild::OutPatchRec{(uint64_t)b->out_off[gi], (int32_t)s.out_records() - 1, (uint32_t)off, gi, 0});
+    // the output entry of the last record of table `t` of `s` (a destination writer), whose BufRef `off` bytes into it is dest_ref()
+    void add_out(StageBuild& s, size_t off, int t = T_A) const {
+        Entry e = entry(E_OUT);
+        e.p.out.off = (uint64_t)b->out_off[gi];
+        s.add_entry(e, off + offsetof(BufRef, p), offsetof(OutPatch, dst), t);
     }
     // a graph planned so far feeds its destination's output to another node, which reads the rendered PCM through a record the output
     // entries do not cover: batch position, -1: none
@@ -1376,99 +1319,65 @@ struct Planner {
         float lo = 0.f, hi = 0.f;  // bound: the range its values are clamped to
     };
     PRef param_ref(uint32_t pid);
-    // a patch entry of this graph; operand i of `r` is `pr` (its id when bound, else its planned value)
-    PatchRec patch(int kind, int n) const {
-        PatchRec r{};
-        r.p.kind = kind;
-        r.p.n = n;
-        for (int i = 0; i < PATCH_OPS; i++) r.p.slot[i] = -1;
-        r.graph = gi;
-        r.rec = r.rec2 = -1;
+    // a bind entry of this graph, of declaration `node` (see Entry::node)
+    Entry entry(int kind, wae_node_id node = 0) const {
+        Entry e;
+        std::memset(&e, 0, sizeof e);
+        e.kind = kind;
+        e.graph = gi;
+        e.node = node;
+        return e;
+    }
+    // a param entry of this graph; operand i of `r` is `pr` (its id when bound, else its planned value)
+    Entry patch(int kind, int n) const {
+        Entry r = entry(E_PARAM);
+        r.p.param.kind = kind;
+        r.p.param.n = n;
+        for (int i = 0; i < PATCH_OPS; i++) r.p.param.slot[i] = -1;
         return r;
     }
-    static void operand(PatchRec& r, int i, const PRef& pr, float planned) {
-        r.p.slot[i] = pr.bound;
-        r.p.val[i] = planned;
+    static void operand(Entry& r, int i, const PRef& pr, float planned) {
+        r.p.param.slot[i] = pr.bound;
+        r.p.param.val[i] = planned;
     }
-    // records patch entry `r` for the last record of stage `s`
-    static void add_patch(StageBuild& s, PatchRec r, uint32_t off, bool with_rec2 = false) {
-        r.rec = (int32_t)s.records() - 1;
-        r.rec2 = with_rec2 ? r.rec : -1;
-        r.off = off;
-        s.patches.push_back(r);
-    }
+    // records param entry `r` for the last record of table `t` of stage `s`, its field `off` bytes into it
+    static void add_patch(StageBuild& s, const Entry& r, size_t off, int t = T_A) { s.add_entry(r, off, offsetof(ParamPatch, dst), t); }
     // the spatial entry of a static panner of this graph; operand i is pr[i] (its id when bound, else its planned value)
-    using SpatialPatchRec = StageBuild::SpatialPatchRec;
-    SpatialPatchRec spatial_entry(int kind, const PRef* pr, const spatial::PanModel& model) const {
-        SpatialPatchRec r{};
-        r.p.kind = kind;
-        r.p.model = model;
+    Entry spatial_entry(int kind, const PRef* pr, const spatial::PanModel& model) const {
+        Entry r = entry(E_SPATIAL);
+        r.p.spatial.kind = kind;
+        r.p.spatial.model = model;
         for (int i = 0; i < 15; i++) {
-            r.p.slot[i] = pr[i].bound;
-            r.p.val[i] = pr[i].v;
+            r.p.spatial.slot[i] = pr[i].bound;
+            r.p.spatial.val[i] = pr[i].v;
         }
-        r.graph = gi;
-        r.rec = -1;
         return r;
     }
-    // records spatial entry `r` for the last record of stage `s` (S_PAN / S_HRTF), `off` bytes into it
-    static void add_spatial(StageBuild& s, SpatialPatchRec r, uint32_t off) {
-        r.rec = (int32_t)s.spatial_records() - 1;
-        r.off = off;
-        s.spatial.push_back(r);
-    }
-    // a moving panner: its bound params are taken raw, PATCH_RAW into SpatialTracks::value of the last record of `s`, `off` bytes into it
-    void raw_spatial_patches(StageBuild& s, const PRef* pr, size_t off) const {
+    // a moving panner: its bound params are taken raw, PATCH_RAW into SpatialTracks::value of the last record of table `t` of `s`, `off`
+    // bytes into it
+    void raw_spatial_patches(StageBuild& s, const PRef* pr, size_t off, int t = T_A) const {
         for (int i = 0; i < 15; i++)
             if (pr[i].bound >= 0) {
-                PatchRec r = patch(PATCH_RAW, 1);
+                Entry r = patch(PATCH_RAW, 1);
                 operand(r, 0, pr[i], pr[i].v);
-                add_patch(s, r, (uint32_t)(off + offsetof(SpatialTracks, value) + (size_t)i * sizeof(float)));
+                add_patch(s, r, off + offsetof(SpatialTracks, value) + (size_t)i * sizeof(float), t);
             }
     }
-    // a chain's patch entries for its record at index `rec` of stage `s` (emit_chain, sum_voices)
-    static void chain_patches(StageBuild& s, const PendingChain& pc, int32_t rec) {
-        for (PatchRec r : pc.patches) {
-            r.rec = rec;
-            if (r.p.kind == PATCH_OSC) {  // the source oscillator's pitch
-                r.off = (uint32_t)offsetof(ChainInst, osc);
-                s.patches.push_back(r);
-                continue;
-            }
-            const int k = r.rec2;
-            r.rec2 = pc.inst.bq[k].coef;
-            r.off = (uint32_t)(offsetof(ChainInst, bq) + (size_t)k * sizeof(ChainBiquad) + offsetof(ChainBiquad, b0));
-            s.patches.push_back(r);
-        }
-        for (int slot = 0; slot < 4; slot++) {
-            if (pc.gain_fold[slot].p.n == 0) continue;
-            PatchRec r = pc.gain_fold[slot];
-            r.rec = rec;
-            r.off = (uint32_t)(offsetof(ChainInst, g) + (size_t)slot * sizeof(float));
-            s.patches.push_back(r);
-        }
-        for (StageBuild::CurvePatchRec r : pc.curve_patches) {
-            r.rec = rec;
-            r.off = (uint32_t)offsetof(ChainInst, shaper_keeps_silence);
-            s.curve_patches.push_back(r);
-        }
-        for (StageBuild::IirPatchRec r : pc.iir_patches) {
-            r.rec = rec;
-            r.scan = pc.inst.bq[r.bq].coef;
-            s.iir_patches.push_back(r);
-        }
-        for (StageBuild::SchedPatchRec r : pc.sched_patches) {
-            r.rec = rec;
-            s.sched_patches.push_back(r);
-        }
-        for (StageBuild::SrcRefRec r : pc.src_refs) {
-            r.rec = rec;
-            s.src_refs.push_back(r);
-        }
+    // a chain's bind entries for its record at index `rec` of stage `s` (emit_chain, sum_voices)
+    static void chain_entries(StageBuild& s, const PendingChain& pc, int32_t rec) {
+        auto emit = [&](Entry e) {
+            for (FieldRef& r : e.ref)
+                if (r.table == T_A) r.rec = rec;
+                else if (r.table == T_B) r.rec = pc.inst.bq[r.rec].coef;
+            s.entries.push_back(e);
+        };
+        for (const Entry& e : pc.entries) emit(e);
+        for (const Entry& f : pc.gain_fold)  // (the gain slots' entries after the others)
+            if (f.p.param.n > 0) emit(f);
     }
-    static bool chain_has_patches(const PendingChain& pc) {
-        bool any = !pc.patches.empty();
-        for (const auto& f : pc.gain_fold) any = any || f.p.n > 0;
+    static bool chain_has_entries(const PendingChain& pc) {
+        bool any = !pc.entries.empty();
+        for (const auto& f : pc.gain_fold) any = any || f.p.param.n > 0;
         return any;
     }
     bool plan_graph(wae_graph* graph, uint32_t graph_index);
@@ -1482,9 +1391,12 @@ struct Planner {
     const float* device_curve(const Node& n);
     float* device_wave(const Node& n);
     float* device_value_curve(const Param& prm, const ParamTimeline& tl);
-    // a patch entry of the declared curve of node `n` for the int32 field `off` bytes into the last record of stage `s`
-    void add_curve_patch(StageBuild& s, const Node& n, uint32_t off, int32_t keeps, int32_t other) {
-        s.curve_patches.push_back(StageBuild::CurvePatchRec{gi, n.id, (int32_t)s.records() - 1, off, keeps, other});
+    // an entry of the declared curve of node `n`, for the int32 field a reference names
+    Entry curve_patch(const Node& n, int32_t keeps, int32_t other) const {
+        Entry e = entry(E_CURVE, n.id);
+        e.p.curve.keeps = keeps;
+        e.p.curve.other = other;
+        return e;
     }
     bool conv_compact_path(PNode& pn, int level, int in_ch, const IrSpectra& spec, int Smax, int blocks_per_chunk);
     // chain fusion
@@ -1540,17 +1452,24 @@ struct Planner {
     // a biquad (or an IIR filter of order <= 2, which opens a chain of its own with a constant layout) appended to the chain it joins
     // `bound`: the patch entry of a biquad with params bound from device memory; `iir_bound`: an IIR filter whose coefficients are bound
     // from device memory
-    bool append_biquad(NodeCtx& nc, double* state, const hm::BiquadCoefs& c, const PatchRec* bound = nullptr, bool iir_bound = false) {
+    bool append_biquad(NodeCtx& nc, double* state, const hm::BiquadCoefs& c, const Entry* bound = nullptr, bool iir_bound = false) {
         PendingChain pc = open_chain(nc);
-        ChainBiquad& st = pc.inst.bq[pc.inst.n_biquad++];
+        const int k = pc.inst.n_biquad++;
+        ChainBiquad& st = pc.inst.bq[k];
         st.state = state;
         st.b0 = c.b0; st.b1 = c.b1; st.b2 = c.b2; st.a1 = c.a1; st.a2 = c.a2;
-        pc.coefs[pc.inst.n_biquad - 1] = c;
-        if (bound) {
-            pc.patches.push_back(*bound);
-            pc.patches.back().rec2 = pc.inst.n_biquad - 1;
+        pc.coefs[k] = c;
+        const size_t coefs = offsetof(ChainInst, bq) + (size_t)k * sizeof(ChainBiquad) + offsetof(ChainBiquad, b0);
+        if (bound) {  // (and the biquad's scan constants)
+            Entry e = *bound;
+            e.refer(1, T_B, k, 0, offsetof(ParamPatch, dst2));
+            pc.add_entry(e, coefs, offsetof(ParamPatch, dst));
         }
-        if (iir_bound) pc.iir_patches.push_back(StageBuild::IirPatchRec{gi, nc.n.id, -1, pc.inst.n_biquad - 1, -1});
+        if (iir_bound) {
+            Entry e = entry(E_IIR, nc.n.id);
+            e.refer(1, T_B, k, 0, offsetof(IirPatch, scan));
+            pc.add_entry(e, coefs, offsetof(IirPatch, b));
+        }
         pc.phase = pc.phase == 0 ? 1 : 3;
         pc.lay = filter_lay(pc.lay);
         return finish_chain(nc, std::move(pc));
@@ -1634,13 +1553,25 @@ struct Planner {
         double duration, ls, le, computed_rate;  // ls / le: the clamped loop boundaries
         bool by_ref;
     };
-    // the source-reference entry of the last record of `s` that plays declared source `n`, its PCM pointer and channel stride `buf` and
-    // `stride` bytes into the record
-    void add_src_ref(StageBuild& s, const Node& n, size_t buf, size_t stride) {
-        s.src_refs.push_back(StageBuild::SrcRefRec{gi, n.id, (int32_t)s.records() - 1, (uint32_t)buf, (uint32_t)stride});
+    // the source-reference entry of a record that plays declared source `n`, its PCM pointer and channel stride `buf` and `stride` bytes
+    // into record `rec` (-1 in a pending chain)
+    Entry src_ref(const Node& n, int32_t rec, size_t buf, size_t stride) const {
+        Entry e = entry(E_SRC_REF, n.id);
+        e.refer(0, T_A, rec, buf, offsetof(SrcRefPatch, buf));
+        e.refer(1, T_A, rec, stride, offsetof(SrcRefPatch, stride));
+        return e;
     }
-    // a patch entry of the schedule of declared source `n` (wae_source_set_device_schedule) for the last record of stage `s`, its fields
-    // `off` bytes into it
+    void add_src_ref(StageBuild& s, const Node& n, size_t buf, size_t stride) { s.entries.push_back(src_ref(n, (int32_t)s.records() - 1, buf, stride)); }
+    // an entry of the schedule of declared source `n` (wae_source_set_device_schedule); add_sched_patch: for the last record of stage
+    // `s`, its fields `off` bytes into it
+    Entry sched_patch(const Node& n, const SchedPatch& p) const {
+        Entry e = entry(E_SCHED, n.id);
+        e.p.sched = p;
+        return e;
+    }
+    void add_sched_patch(StageBuild& s, const Node& n, const SchedPatch& p, size_t off = 0) {
+        s.add_entry(sched_patch(n, p), off, offsetof(SchedPatch, dst));
+    }
     SchedPatch sched_entry(const Node& n, int32_t kind) const {
         SchedPatch p{};
         p.kind = kind;
@@ -1648,9 +1579,6 @@ struct Planner {
         p.stop_time = n.stop_time;
         p.lq = lq;
         return p;
-    }
-    void add_sched_patch(StageBuild& s, const Node& n, const SchedPatch& p, uint32_t off = 0) {
-        s.sched_patches.push_back(StageBuild::SchedPatchRec{gi, n.id, (int32_t)s.records() - 1, off, p});
     }
     bool lower_absn(NodeCtx& nc);
     bool absn_silent(NodeCtx& nc);
@@ -1747,18 +1675,34 @@ static uint64_t digest_vec_skipping(const std::vector<T>& v, std::initializer_li
 template <typename T>
 static uint64_t digest_vec_without_end(const std::vector<T>& v, uint64_t h) { return digest_vec_skipping(v, {offsetof(T, end)}, h); }
 
-// (the output and source-reference entries are not part of any record: the split sizing's self-check compares them on their own)
-static uint64_t digest_out_patches(const std::map<std::pair<int, int>, StageBuild>& builds) {
-    uint64_t h = 1469598103934665603ull;
-    for (auto& kv : builds) h = digest_vec(kv.second.out_patches, h);
-    return h;
+using Builds = std::map<std::pair<int, int>, StageBuild>;
+// The bind entries are not part of any record: the split sizing's self-check compares them on their own, and WAE_PLAN_DIGEST prints them
+// on a line of their own (a graph with declarations and its twin with host values plan the same records, but only the first has
+// entries).  Canonical form, in the order prepare uploads them (kind, stage, planning order): kind, graph, node, each reference's table,
+// record and offset, and the payload with the addresses the references fill zeroed.  `count`: the entries digested.
+static uint64_t digest_entries(const Builds& builds, uint64_t h, size_t& count) {
+    std::vector<uint8_t> bytes;  // (hashed from the heap: fnv1a reads 8-byte words)
+    for (int kind = 0; kind < E_KINDS; kind++)
+        for (auto& kv : builds)
+            for (Entry e : kv.second.entries) {
+                if (e.kind != kind) continue;
+                int32_t head[12] = {e.kind, (int32_t)e.graph, (int32_t)e.node};
+                for (int i = 0; i < 3; i++) {
+                    const FieldRef& r = e.ref[i];
+                    head[3 + 3 * i] = r.table;
+                    head[4 + 3 * i] = r.rec;
+                    head[5 + 3 * i] = (int32_t)r.off;
+                    if (r.table != T_NONE) std::memset(reinterpret_cast<char*>(&e.p) + r.field, 0, sizeof(void*));
+                }
+                const uint8_t* p = reinterpret_cast<const uint8_t*>(head);
+                bytes.insert(bytes.end(), p, p + sizeof head);
+                p = reinterpret_cast<const uint8_t*>(&e.p);
+                bytes.insert(bytes.end(), p, p + kEntryPayloadBytes[kind]);
+                count++;
+            }
+    return fnv1a(bytes.data(), bytes.size(), h);
 }
-static uint64_t digest_src_refs(const std::map<std::pair<int, int>, StageBuild>& builds) {
-    uint64_t h = 1469598103934665603ull;
-    for (auto& kv : builds) h = digest_vec(kv.second.src_refs, h);
-    return h;
-}
-static uint64_t digest_builds(const std::map<std::pair<int, int>, StageBuild>& builds, uint64_t h) {
+static uint64_t digest_builds(const Builds& builds, uint64_t h) {
     for (auto& kv : builds) {
         const StageBuild& s = kv.second;
         const int key[6] = {kv.first.first, kv.first.second, s.cls, s.level, s.kind * 64 + s.variant, s.max_ch};
@@ -1783,54 +1727,36 @@ static uint64_t digest_builds(const std::map<std::pair<int, int>, StageBuild>& b
 // Split planning (a group of few, large graphs planned by several workers, each with its own Planner over a contiguous run of the
 // group's graphs): the runs' stage builds are appended to one another in graph order, which is the order a single planner would have
 // produced.  Records that index a sibling table of their stage are rebased: mix instances -> mix edges, chain biquads -> scan constants,
-// voice groups -> chain records, convolver paths -> the conv-input table of the forward-transform stage of their level.
-using Builds = std::map<std::pair<int, int>, StageBuild>;
+// voice groups -> chain records, convolver paths -> the conv-input table of the forward-transform stage of their level; and so are the
+// references of the bind entries.
 template <typename T>
 static void append_vec(std::vector<T>& d, std::vector<T>& s) {
     if (d.empty()) d = std::move(s);
     else d.insert(d.end(), s.begin(), s.end());
 }
 static void merge_builds(Builds& dst, Builds& src) {
-    struct Base {
-        size_t mix_edges = 0, scan = 0, chain = 0, conv_in = 0, records = 0, spatial = 0, out = 0;
-    };
+    using Base = std::array<size_t, 4>;  // per StageTable
     std::map<std::pair<int, int>, Base> base;  // table sizes of `dst` before anything of `src` is appended
     for (auto& kv : src) {
         auto it = dst.find(kv.first);
-        if (it != dst.end())
-            base[kv.first] = Base{it->second.mix_edges.size(), it->second.n_scan_coef, it->second.chain.size(), it->second.conv_in.size(),
-                                  it->second.records(), it->second.spatial_records(), it->second.out_records()};
-        else base[kv.first] = Base{};
+        Base& bs = base[kv.first];
+        for (int t = T_NONE; t <= T_C; t++) bs[t] = it != dst.end() && t != T_NONE ? it->second.records(t) : 0;
     }
     for (auto& kv : src) {
         StageBuild& s = kv.second;
         const Base bs = base[kv.first];
-        for (auto& pr : s.patches) {
-            pr.rec += (int32_t)bs.records;
-            if (pr.rec2 >= 0) pr.rec2 += (int32_t)(s.kind == S_SPAN ? bs.records : bs.scan);
-        }
-        for (auto& cp : s.curve_patches) cp.rec += (int32_t)bs.records;
-        for (auto& sp : s.sched_patches) sp.rec += (int32_t)bs.records;
-        for (auto& lp : s.loop_patches) lp.rec += (int32_t)bs.records;
-        for (auto& lw : s.loop_walks) lw.rec += (int32_t)bs.records;
-        for (auto& sp : s.spatial)
-            if (sp.rec >= 0) sp.rec += (int32_t)bs.spatial;
-        for (auto& op : s.out_patches) op.rec += (int32_t)bs.out;
-        for (auto& sr : s.src_refs) sr.rec += (int32_t)bs.records;
-        for (auto& ip : s.iir_patches) {
-            ip.rec += (int32_t)bs.records;
-            if (ip.scan >= 0) ip.scan += (int32_t)bs.scan;
-        }
-        for (auto& m : s.mix) m.edge_offset += (uint32_t)bs.mix_edges;
-        for (auto& m : s.mix_dyn) m.edge_offset += (uint32_t)bs.mix_edges;
+        for (Entry& e : s.entries)
+            for (FieldRef& r : e.ref) r.rec += (int32_t)bs[r.table];
+        for (auto& m : s.mix) m.edge_offset += (uint32_t)bs[T_B];
+        for (auto& m : s.mix_dyn) m.edge_offset += (uint32_t)bs[T_B];
         for (auto& c : s.chain)
-            for (int k = 0; k < c.n_biquad; k++) c.bq[k].coef += (int32_t)bs.scan;
-        for (auto& v : s.vgroups) v.first += (int32_t)bs.chain;
+            for (int k = 0; k < c.n_biquad; k++) c.bq[k].coef += (int32_t)bs[T_B];
+        for (auto& v : s.vgroups) v.first += (int32_t)bs[T_A];
         if (s.kind == S_CONV_MAC || s.kind == S_CONV_MAC_ACC) {
             const std::pair<int, int> fft_key{kv.first.first, S_CONV_FFT * 64};
             size_t off = 0;
             auto bi = base.find(fft_key);
-            if (bi != base.end()) off = bi->second.conv_in;
+            if (bi != base.end()) off = bi->second[T_A];
             else if (dst.count(fft_key)) off = dst[fft_key].conv_in.size();
             for (auto& cp : s.conv_path) cp.input += (int32_t)off;
         }
@@ -1850,15 +1776,7 @@ static void merge_builds(Builds& dst, Builds& src) {
         append_vec(d.conv_path, s.conv_path); append_vec(d.vgroups, s.vgroups); append_vec(d.conv_cmp, s.conv_cmp);
         append_vec(d.absn_bound, s.absn_bound);
         append_vec(d.readout, s.readout); append_vec(d.readout_smooth, s.readout_smooth); append_vec(d.comp_ro, s.comp_ro);
-        append_vec(d.patches, s.patches);
-        append_vec(d.curve_patches, s.curve_patches);
-        append_vec(d.iir_patches, s.iir_patches);
-        append_vec(d.sched_patches, s.sched_patches);
-        append_vec(d.loop_patches, s.loop_patches);
-        append_vec(d.loop_walks, s.loop_walks);
-        append_vec(d.spatial, s.spatial);
-        append_vec(d.out_patches, s.out_patches);
-        append_vec(d.src_refs, s.src_refs);
+        append_vec(d.entries, s.entries);
         d.n_scan_coef += s.n_scan_coef;
         d.max_ch = std::max(d.max_ch, s.max_ch);
     }
@@ -2252,7 +2170,7 @@ StageBuild& Planner::emit_chain(PendingChain& pc, int L) {
         pc.inst.bq[k].coef = cs.add_scan_coef(want_scan_coefs, [&] { return make_scan_coef(pc.coefs[k]); });
     }
     cs.max_ch = std::max(cs.max_ch, pc.ch);
-    chain_patches(cs, pc, (int32_t)cs.chain.size());
+    chain_entries(cs, pc, (int32_t)cs.chain.size());
     cs.chain.push_back(pc.inst);
     return cs;
 }
@@ -2270,8 +2188,7 @@ bool Planner::materialize(uint32_t nid, bool may_alias) {
         const AbsnInst& a = ci.absn;
         bool unit = true;
         for (int i = 0; i < 4; i++) unit = unit && ci.g[i] == 1.f;
-        if (may_alias && ci.src_kind == CHAIN_SRC_ABSN && ci.n_biquad == 0 && !ci.has_shaper && unit && !chain_has_patches(it->second) &&
-            it->second.src_refs.empty() && it->second.phase == 0 &&
+        if (may_alias && ci.src_kind == CHAIN_SRC_ABSN && ci.n_biquad == 0 && !ci.has_shaper && unit && !chain_has_entries(it->second) && it->second.phase == 0 &&
             !it->second.lay.dyn() && a.n_start == 0 && !a.loop && a.buf_offset == 0 && a.buf_len >= lq && a.buf_stride <= 0xffffffffll &&
             seg_start == 0 && seg_end >= lq) {
             sp.out_buf = {BufRef{const_cast<float*>(a.buf), (uint32_t)a.buf_stride, 1}};
@@ -2569,11 +2486,11 @@ bool Planner::sum_voices(NodeCtx& nc, int port, int ch, int nb) {
             pc.inst.bq[k].coef = vs.add_scan_coef(want_scan_coefs, [&] { return make_scan_coef(pc.coefs[k]); });
         pc.inst.limit = -1;
         pc.inst.out_dup = 0;
-        chain_patches(vs, pc, (int32_t)vs.chain.size());
+        chain_entries(vs, pc, (int32_t)vs.chain.size());
         vs.chain.push_back(pc.inst);
     }
     vs.vgroups.push_back(vg);
-    if (nc.n.kind == K_DEST) add_out(vs, offsetof(VoiceGroup, out));
+    if (nc.n.kind == K_DEST) add_out(vs, offsetof(VoiceGroup, out), T_C);
     nc.p.in_buf[port] = vg.out;
     return true;
 }
@@ -2636,7 +2553,7 @@ bool Planner::lower_osc(NodeCtx& nc) {
     // (0, Nyquist), so the path and OscInst::fast hold for every value, and a PATCH_OSC entry re-derives the phase fields per bind: from
     // the planned start time, or from the slot a bound schedule writes its start into.
     const bool pitch_bound = pf.bound >= 0 || pd.bound >= 0;
-    PatchRec pitch = patch(PATCH_OSC, 2);
+    Entry pitch = patch(PATCH_OSC, 2);
     if (pitch_bound && !nc.dyn_params) {
         const double f_lo = pf.bound >= 0 ? pf.lo : freq, f_hi = pf.bound >= 0 ? pf.hi : freq;
         const double d_lo = pd.bound >= 0 ? pd.lo : detune, d_hi = pd.bound >= 0 ? pd.hi : detune;
@@ -2650,10 +2567,10 @@ bool Planner::lower_osc(NodeCtx& nc) {
         }
         operand(pitch, 0, pf, freq);
         operand(pitch, 1, pd, detune);
-        pitch.p.sample_rate = g->sample_rate;
+        pitch.p.param.sample_rate = g->sample_rate;
         double* start = upload(std::vector<double>{n.start_time});
         if (!start) return bail(WAE_OUT_OF_MEMORY, "out of device memory (oscillator start time)");
-        pitch.p.dst2 = start;
+        pitch.p.param.dst2 = start;
         if (n.device_schedule) sched.start_out = start;
     }
     if (n.type == WAE_OSC_CUSTOM && n.device_wave) {  // a wave bound from device memory: planned as a host wave of its length
@@ -2688,16 +2605,16 @@ bool Planner::lower_osc(NodeCtx& nc) {
         const size_t offs[2] = {offsetof(OscArInst, f_val), offsetof(OscArInst, d_val)};
         for (int i = 0; i < 2; i++)
             if (refs[i]->bound >= 0) {
-                PatchRec r = patch(PATCH_RAW, 1);
+                Entry r = patch(PATCH_RAW, 1);
                 operand(r, 0, *refs[i], refs[i]->v);
-                add_patch(sb, r, (uint32_t)offs[i]);
+                add_patch(sb, r, offs[i]);
             }
     } else if (nc.fuse_n) {
         PendingChain pc = source_chain(CHAIN_SRC_OSC, 1);
         pc.inst.osc = o;
         pc.lay = source_lay(o.n_first, o.n_stop, 1, n.device_schedule);
-        if (n.device_schedule) pc.sched_patches.push_back(StageBuild::SchedPatchRec{gi, n.id, -1, (uint32_t)offsetof(ChainInst, osc), sched});
-        if (pitch_bound) pc.patches.push_back(pitch);  // (rec / off set when the chain is emitted)
+        if (n.device_schedule) pc.add_entry(sched_patch(n, sched), offsetof(ChainInst, osc), offsetof(SchedPatch, dst));
+        if (pitch_bound) pc.add_entry(pitch, offsetof(ChainInst, osc), offsetof(ParamPatch, dst));
         return finish_chain(nc, std::move(pc));
     } else {
         o.out = source_out(nc, o.n_first, o.n_stop, 1, track_sched);
@@ -2733,7 +2650,7 @@ bool Planner::lower_const(NodeCtx& nc) {
         PendingChain pc = source_chain(CHAIN_SRC_CONST, 1);
         pc.inst.cst = c;
         pc.lay = source_lay(c.n_first, c.n_stop, 1, n.device_schedule);
-        if (n.device_schedule) pc.sched_patches.push_back(StageBuild::SchedPatchRec{gi, n.id, -1, (uint32_t)offsetof(ChainInst, cst), sched});
+        if (n.device_schedule) pc.add_entry(sched_patch(n, sched), offsetof(ChainInst, cst), offsetof(SchedPatch, dst));
         return finish_chain(nc, std::move(pc));
     }
     c.out = source_out(nc, c.n_first, c.n_stop, 1, n.device_schedule ? &meta_sched : nullptr);
@@ -2885,13 +2802,16 @@ bool Planner::absn_serial(NodeCtx& nc, const AbsnPlay& s, const PRef& pdet, cons
     const size_t offs[2] = {offsetof(AbsnSerialInst, detune), offsetof(AbsnSerialInst, rate)};
     for (int i = 0; i < 2; i++)
         if (refs[i]->bound >= 0) {  // bound from device memory (the kernel takes the raw values)
-            PatchRec r = patch(PATCH_RAW, 1);
+            Entry r = patch(PATCH_RAW, 1);
             operand(r, 0, *refs[i], refs[i]->v);
-            add_patch(sb, r, (uint32_t)offs[i]);
+            add_patch(sb, r, offs[i]);
         }
     if (n.device_schedule) add_sched_patch(sb, n, sched_entry(n, SCHED_ABSN_SERIAL));  // (the raw start / stop times)
-    if (n.device_loop)  // (the loop points after clamp_loop_boundaries)
-        sb.loop_patches.push_back(StageBuild::LoopPatchRec{gi, n.id, (int32_t)sb.records() - 1, LoopPatch{nullptr, LOOP_SERIAL, 0, s.duration}});
+    if (n.device_loop) {  // (the loop points after clamp_loop_boundaries)
+        Entry e = entry(E_LOOP, n.id);
+        e.p.loop = LoopPatch{nullptr, LOOP_SERIAL, 0, s.duration};
+        sb.add_entry(e, 0, offsetof(LoopPatch, dst));
+    }
     algorithmic_bytes += (uint64_t)s.ch * 4ull * (uint64_t)std::min<int64_t>(lq, (int64_t)s.len);
     return true;
 }
@@ -3023,17 +2943,19 @@ bool Planner::absn_bound(NodeCtx& nc, const AbsnPlay& s, const PRef& pdet, const
         add_sched_patch(sb, n, sp);
     }
     if (n.device_loop) {
-        const int32_t rec = (int32_t)sb.records() - 1;
-        sb.loop_patches.push_back(StageBuild::LoopPatchRec{gi, n.id, rec, LoopPatch{nullptr, LOOP_BOUND, 0, s.duration}});
-        sb.loop_walks.push_back(StageBuild::LoopWalkRec{rec, loop_cap, lq});
+        Entry e = entry(E_LOOP, n.id), w = entry(E_LOOP_WALK);
+        e.p.loop = LoopPatch{nullptr, LOOP_BOUND, 0, s.duration};
+        w.p.walk = LoopWalk{nullptr, lq, loop_cap, 0};
+        sb.add_entry(e, 0, offsetof(LoopPatch, dst));
+        sb.add_entry(w, 0, offsetof(LoopWalk, rec));
     }
     const PRef* refs[2] = {&pdet, &prate};
     const size_t offs[2] = {offsetof(AbsnBoundInst, detune), offsetof(AbsnBoundInst, rate)};
     for (int i = 0; i < 2; i++)
         if (refs[i]->bound >= 0) {
-            PatchRec pr = patch(PATCH_RAW, 1);
+            Entry pr = patch(PATCH_RAW, 1);
             operand(pr, 0, *refs[i], refs[i]->v);
-            add_patch(sb, pr, (uint32_t)offs[i]);
+            add_patch(sb, pr, offs[i]);
         }
     algorithmic_bytes += (uint64_t)s.ch * 4ull * (uint64_t)std::min<int64_t>(lq, (int64_t)s.len);
     return true;
@@ -3058,8 +2980,7 @@ bool Planner::absn_fast(NodeCtx& nc, const AbsnPlay& s, int64_t q, bool fused) {
         pc.inst.absn = a;
         pc.lay = source_lay(a.n_start, a.n_stop, s.ch);
         if (s.by_ref)
-            pc.src_refs.push_back(StageBuild::SrcRefRec{gi, n.id, -1, (uint32_t)(offsetof(ChainInst, absn) + offsetof(AbsnInst, buf)),
-                                                        (uint32_t)(offsetof(ChainInst, absn) + offsetof(AbsnInst, buf_stride))});
+            pc.entries.push_back(src_ref(n, -1, offsetof(ChainInst, absn) + offsetof(AbsnInst, buf), offsetof(ChainInst, absn) + offsetof(AbsnInst, buf_stride)));
         if (!finish_chain(nc, std::move(pc))) return false;
     } else {
         a.out = source_out(nc, a.n_start, a.n_stop, s.ch);
@@ -3111,9 +3032,9 @@ bool Planner::lower_biquad(NodeCtx& nc) {
                                 offsetof(BiquadArInst, gain_val)};
         for (int i = 0; i < 4; i++)
             if (refs[i]->bound >= 0) {
-                PatchRec r = patch(PATCH_RAW, 1);
+                Entry r = patch(PATCH_RAW, 1);
                 operand(r, 0, *refs[i], refs[i]->v);
-                add_patch(sb, r, (uint32_t)offs[i]);
+                add_patch(sb, r, offs[i]);
             }
         return true;
     }
@@ -3121,8 +3042,8 @@ bool Planner::lower_biquad(NodeCtx& nc) {
     hm::BiquadCoefs c = hm::biquad_coefs(n.type, (double)g->sample_rate, (double)cf, (double)gain, (double)q);
     // coefficients that depend on params bound from device memory: re-derived per bind
     const bool bound = pq.bound >= 0 || pdt.bound >= 0 || pfr.bound >= 0 || pg.bound >= 0;
-    PatchRec bp = patch(PATCH_BIQUAD, n.type);
-    bp.p.sample_rate = g->sample_rate;
+    Entry bp = patch(PATCH_BIQUAD, n.type);
+    bp.p.param.sample_rate = g->sample_rate;
     operand(bp, 0, pq, q);
     operand(bp, 1, pdt, detune);
     operand(bp, 2, pfr, freq);
@@ -3145,7 +3066,7 @@ bool Planner::lower_biquad(NodeCtx& nc) {
     StageBuild& s = stage(nc.L, S_BIQUAD);
     s.max_ch = std::max(s.max_ch, ch);
     s.biquad.push_back(bi);
-    if (bound) add_patch(s, bp, (uint32_t)offsetof(BiquadInst, b0));
+    if (bound) add_patch(s, bp, offsetof(BiquadInst, b0));
     return true;
 }
 
@@ -3190,7 +3111,11 @@ bool Planner::lower_iir(NodeCtx& nc) {
     s.iir.push_back(ii);
     // coefficients bound from device memory (wae_iir_filter_set_device_coefficients): the bind rewrites b[0..n) and a[0..n) of this
     // segment's record
-    if (n.device_iir) s.iir_patches.push_back(StageBuild::IirPatchRec{gi, n.id, (int32_t)s.iir.size() - 1, -1, -1});
+    if (n.device_iir) {
+        Entry e = entry(E_IIR, n.id);
+        e.refer(1, T_A, (int32_t)s.records() - 1, offsetof(IirInst, a), offsetof(IirPatch, a));
+        s.add_entry(e, offsetof(IirInst, b), offsetof(IirPatch, b));
+    }
     return true;
 }
 
@@ -3218,14 +3143,15 @@ bool Planner::lower_gain(NodeCtx& nc) {
         PendingChain pc = open_chain(nc);
         // consecutive gains of one slot are folded (differs from two f32 multiplies by <= 1 ulp)
         const int slot = pc.phase == 0 ? 0 : (pc.phase == 1 ? 1 : (pc.phase == 3 ? 2 : 3));
-        PatchRec& fold = pc.gain_fold[slot];
-        if (bound || fold.p.n > 0) {  // the slot's factors in node order, from the first bound one on (the constant product before it first)
-            if (fold.p.n == 0) {
+        Entry& fold = pc.gain_fold[slot];
+        if (bound || fold.p.param.n > 0) {  // the slot's factors in node order, from the first bound one on (the constant product before it first)
+            if (fold.p.param.n == 0) {
                 fold = patch(PATCH_GAIN, 1);
-                fold.p.val[0] = pc.inst.g[slot];
+                fold.p.param.val[0] = pc.inst.g[slot];
+                fold.refer(0, T_A, -1, offsetof(ChainInst, g) + (size_t)slot * sizeof(float), offsetof(ParamPatch, dst));
             }
-            if (fold.p.n >= PATCH_OPS) return bail(WAE_UNSUPPORTED, "too many gains folded into one chain slot behind a gain bound from device memory");
-            operand(fold, fold.p.n++, pgn, gv);
+            if (fold.p.param.n >= PATCH_OPS) return bail(WAE_UNSUPPORTED, "too many gains folded into one chain slot behind a gain bound from device memory");
+            operand(fold, fold.p.param.n++, pgn, gv);
         }
         pc.inst.g[slot] *= gv;
         if (may_zero) pc.lay = Lay{1, pc.lay.hi, pc.lay.nlo, pc.lay.nhi, true};  // (k_chain reports a zero slot on its track rows)
@@ -3233,15 +3159,15 @@ bool Planner::lower_gain(NodeCtx& nc) {
         return finish_chain(nc, std::move(pc));
     }
     if (!need_out(nc, ch)) return false;
-    PatchRec gp = patch(PATCH_GAIN, 1);
+    Entry gp = patch(PATCH_GAIN, 1);
     operand(gp, 0, pgn, gv);
     if (may_zero) {
         out_dynamic(nc, or_silent);
         if (p.out_buf[0].meta) {  // META_COPY, or silent (META_CONST with count 1 and the silent flag) while the bound gain is about zero
             meta_stage(nc.L, META_COPY, p.in_buf[0], ch, p.out_buf[0], ch, 1, 1);
-            PatchRec mp = gp;
-            mp.p.kind = PATCH_META;
-            add_patch(stage(nc.L, S_META), mp, (uint32_t)offsetof(MetaInst, mode));
+            Entry mp = gp;
+            mp.p.param.kind = PATCH_META;
+            add_patch(stage(nc.L, S_META), mp, offsetof(MetaInst, mode));
         }
     } else if (gv == 0.f && !bound) {
         out_dynamic(nc, Lay{1, 1, 1, 1, true});
@@ -3251,7 +3177,7 @@ bool Planner::lower_gain(NodeCtx& nc) {
     }
     StageBuild& s = stage(nc.L, S_GAIN);
     s.gain.push_back(GainInst{p.in_buf[0], p.out_buf[0], gv, ch, BufRef{nullptr, 0, 0}});
-    if (bound) add_patch(s, gp, (uint32_t)offsetof(GainInst, gain));
+    if (bound) add_patch(s, gp, offsetof(GainInst, gain));
     return true;
 }
 
@@ -3283,7 +3209,7 @@ bool Planner::lower_shaper(NodeCtx& nc) {
         out_dynamic(nc, shaper_lay(in0));
         if (!p.out_buf[0].meta) return;
         meta_stage(nc.L, META_COPY, p.in_buf[0], ch, p.out_buf[0], ch);
-        add_curve_patch(stage(nc.L, S_META), n, (uint32_t)offsetof(MetaInst, mode), META_COPY, META_SHAPER);
+        stage(nc.L, S_META).add_entry(curve_patch(n, META_COPY, META_SHAPER), offsetof(MetaInst, mode), offsetof(CurvePatch, dst));
     };
     if (n.oversample && n.has_curve) {  // waveshaper.rs:409-480: up-sample, shape, down-sample
         // input that can fall silent: a curve that maps 0 to 0 makes the node return early WITHOUT feeding its resamplers
@@ -3342,7 +3268,7 @@ bool Planner::lower_shaper(NodeCtx& nc) {
         StageBuild& os = stage(nc.L, S_SHAPER_OS);
         os.max_ch = std::max(os.max_ch, ch);
         os.shaper_os.push_back(so);
-        if (declared && rebuild) add_curve_patch(os, n, (uint32_t)offsetof(ShaperOsInst, rebuild), 2, 1);
+        if (declared && rebuild) os.add_entry(curve_patch(n, 2, 1), offsetof(ShaperOsInst, rebuild), offsetof(CurvePatch, dst));
         return true;
     }
     if (nc.fuse_n) {
@@ -3351,7 +3277,7 @@ bool Planner::lower_shaper(NodeCtx& nc) {
         pc.inst.curve = curve;
         pc.inst.shaper_n = curve_n;
         pc.inst.shaper_keeps_silence = keeps_silence ? 1 : 0;
-        if (declared) pc.curve_patches.push_back(StageBuild::CurvePatchRec{gi, n.id, -1, 0, 1, 0});
+        if (declared) pc.add_entry(curve_patch(n, 1, 0), offsetof(ChainInst, shaper_keeps_silence), offsetof(CurvePatch, dst));
         pc.lay = shaper_lay(pc.lay);
         pc.phase = 5;
         return finish_chain(nc, std::move(pc));
@@ -3391,9 +3317,10 @@ bool Planner::lower_stereo_panner(NodeCtx& nc) {
     s.span.push_back(SPanInst{p.in_buf[0], p.out_buf[0], pan, ch, ppan.dyn ? ppan.track : BufRef{nullptr, 0, 0}});
     s.span_gains.push_back(make_float2(gl, gr));
     if (ppan.bound >= 0) {
-        PatchRec r = patch(PATCH_SPAN, ch);
+        Entry r = patch(PATCH_SPAN, ch);
         operand(r, 0, ppan, pan);
-        add_patch(s, r, (uint32_t)offsetof(SPanInst, pan), true);
+        r.refer(1, T_B, (int32_t)s.records(T_B) - 1, 0, offsetof(ParamPatch, dst2));  // (and its stereo gains)
+        add_patch(s, r, offsetof(SPanInst, pan));
     }
     return true;
 }
@@ -3463,7 +3390,7 @@ bool Planner::lower_panner(NodeCtx& nc) {
     pi.cone_gain = sp0.cone_gain;
     StageBuild& ps = stage(nc.L, S_PAN);
     ps.pan.push_back(pi);
-    if (bound) add_spatial(ps, spatial_entry(SPATIAL_PAN, pr, model), 0);
+    if (bound) ps.add_entry(spatial_entry(SPATIAL_PAN, pr, model), 0, offsetof(SpatialPatch, dst));
     return true;
 }
 
@@ -3530,23 +3457,23 @@ bool Planner::panner_hrtf_conv(NodeCtx& nc, const spatial::SpatialParams& sp0, c
         const int S = (int)((taps + WAE_CONV_BLOCK - 1) / WAE_CONV_BLOCK);
         if (!bound_panner_spectra(nc.n, S, spec) || !plan_convolver(nc.p, nc.L, nullptr, -1, &resp, &spec)) return false;
         if (dry) return true;
-        SpatialPatchRec r = spatial_entry(SPATIAL_RESP, pr, model);
-        r.p.pos = eng->d_sphere_pos;
-        r.p.tri = eng->d_sphere_tri;
-        r.p.n_faces = (int32_t)(eng->sphere->tri.size() / 3);
-        r.p.ir = hr.d_ir;
-        r.p.taps = (int32_t)taps;
-        r.p.correction = corr;
+        Entry r = spatial_entry(SPATIAL_RESP, pr, model);
+        r.p.spatial.pos = eng->d_sphere_pos;
+        r.p.spatial.tri = eng->d_sphere_tri;
+        r.p.spatial.n_faces = (int32_t)(eng->sphere->tri.size() / 3);
+        r.p.spatial.ir = hr.d_ir;
+        r.p.spatial.taps = (int32_t)taps;
+        r.p.spatial.correction = corr;
         const size_t sel_floats = sizeof(HrtfSel) / sizeof(float);
         std::lock_guard<std::recursive_mutex> lk(b->mu);  // (groups are planned on worker threads)
         float* scratch = b->dalloc<float>((size_t)2 * taps + sel_floats, true);  // the pair, then the selection
         if (!scratch) return bail(WAE_OUT_OF_MEMORY, "out of device memory (hrtf response)");
         b->asset_bytes += ((size_t)2 * taps + sel_floats) * sizeof(float);
-        r.p.resp = scratch;
-        r.p.dst = scratch + (size_t)2 * taps;
+        r.p.spatial.resp = scratch;
+        r.p.spatial.dst = scratch + (size_t)2 * taps;
         r.spec = spec.h;
         r.S = S;
-        stage(nc.L, S_CONV_FFT).spatial.push_back(r);
+        stage(nc.L, S_CONV_FFT).entries.push_back(r);
         return true;
     }
     const HrtfSel sel = static_hrtf_sel(sp0);
@@ -3595,17 +3522,17 @@ bool Planner::panner_hrtf_fir(NodeCtx& nc, const spatial::SpatialParams& sp0, co
         if (!si.sel) return bail(WAE_OUT_OF_MEMORY, "out of device memory (hrtf selection)");
         h.sel = si.sel;
         hs.hrtf_sel.push_back(si);
-        if (pr) raw_spatial_patches(hs, pr, offsetof(HrtfSelInst, sp));
+        if (pr) raw_spatial_patches(hs, pr, offsetof(HrtfSelInst, sp), T_B);
     } else {
         h.static_sel = static_hrtf_sel(sp0);
     }
     hs.hrtf.push_back(h);
     if (pr && !moving) {  // (the sphere operands: the ones a moving panner's HrtfSelInst holds)
-        SpatialPatchRec r = spatial_entry(SPATIAL_SEL, pr, model);
-        r.p.pos = eng->d_sphere_pos;
-        r.p.tri = eng->d_sphere_tri;
-        r.p.n_faces = (int32_t)(sph->tri.size() / 3);
-        add_spatial(hs, r, (uint32_t)offsetof(HrtfInst, static_sel));
+        Entry r = spatial_entry(SPATIAL_SEL, pr, model);
+        r.p.spatial.pos = eng->d_sphere_pos;
+        r.p.spatial.tri = eng->d_sphere_tri;
+        r.p.spatial.n_faces = (int32_t)(sph->tri.size() / 3);
+        hs.add_entry(r, offsetof(HrtfInst, static_sel), offsetof(SpatialPatch, dst));
     }
     return true;
 }
@@ -3739,9 +3666,9 @@ bool Planner::lower_compressor(NodeCtx& nc) {
                             offsetof(CompInst, threshold)};
     for (int i = 0; i < 5; i++)
         if (cp[i].bound >= 0) {  // (the kernel takes the raw values)
-            PatchRec r = patch(PATCH_RAW, 1);
+            Entry r = patch(PATCH_RAW, 1);
             operand(r, 0, cp[i], cp[i].v);
-            add_patch(s, r, (uint32_t)offs[i]);
+            add_patch(s, r, offs[i]);
         }
     if (!dry) {
         std::lock_guard<std::recursive_mutex> lk(b->mu);  // (groups are planned on worker threads)
@@ -4250,15 +4177,7 @@ struct GroupPlan {  // result of phase B for one group
     uint64_t algorithmic_bytes = 0;
     int code = WAE_OK;
     std::string error;
-    std::vector<std::pair<uint32_t, ParamPatch>> patches;  // (batch position, entry): device addresses set, operands still param ids
-    std::vector<PatchEntry<CurvePatch>> curve_patches;
-    std::vector<PatchEntry<IirPatch>> iir_patches;
-    std::vector<PatchEntry<SchedPatch>> sched_patches;
-    std::vector<PatchEntry<LoopPatch>> loop_patches;
-    std::vector<LoopWalk> loop_walks;
-    std::vector<StageBuild::SpatialPatchRec> spatial;  // device addresses set, operands still param ids
-    std::vector<OutPatch> out_patches;                 // device addresses set
-    std::vector<PatchEntry<SrcRefPatch>> src_refs;     // device addresses set
+    std::vector<Entry> entries;                        // device addresses set (operands of E_PARAM / E_SPATIAL still param ids)
     std::vector<std::pair<size_t, size_t>> out_zero;   // (offset, floats) of the output no stage writes
     int64_t dest_reader = -1;                          // see Planner::dest_reader
 };
@@ -4416,7 +4335,8 @@ static wae_status prep_begin(wae_engine* eng, wae_graph* const* graphs, uint32_t
         bool has_feedback = false;
         std::map<std::pair<uint32_t, uint32_t>, int> delay_ch_seen;
         std::vector<std::vector<int>> stage_lists;
-        uint64_t digest = 1469598103934665603ull;
+        uint64_t digest = 1469598103934665603ull, entries_digest = 1469598103934665603ull;
+        size_t n_entries = 0;
         int code = WAE_OK;
         std::string error;
     };
@@ -4522,7 +4442,8 @@ static wae_status prep_begin(wae_engine* eng, wae_graph* const* graphs, uint32_t
             b->groups[k].graph_src_base.clear();
             Planner sizing(b, b->groups[k], ps, &b->groups[k].src_copies);
             const std::vector<int64_t>& bounds = b->groups[k].seg_bounds;
-            uint64_t serial_digest = 0, serial_out_digest = 0, serial_ref_digest = 0;
+            uint64_t serial_digest = 0, serial_entries = 0;
+            size_t unused = 0;
             for (size_t sg = 0; sg + 1 < bounds.size(); sg++) {
                 sizing.begin_segment(bounds[sg], bounds[sg + 1]);
                 for (uint32_t i = b->groups[k].g0; i < b->groups[k].g1; i++) {
@@ -4539,11 +4460,13 @@ static wae_status prep_begin(wae_engine* eng, wae_graph* const* graphs, uint32_t
                     std::vector<int> kinds;
                     for (auto& kv : sizing.builds) kinds.push_back(kv.second.kind);
                     so[k].stage_lists.push_back(std::move(kinds));
-                    if (plan_digest_wanted()) so[k].digest = digest_builds(sizing.builds, so[k].digest);
+                    if (plan_digest_wanted()) {
+                        so[k].digest = digest_builds(sizing.builds, so[k].digest);
+                        so[k].entries_digest = digest_entries(sizing.builds, so[k].entries_digest, so[k].n_entries);
+                    }
                     if (check_split && one_segment) {
                         serial_digest = digest_builds(sizing.builds, 1469598103934665603ull);
-                        serial_out_digest = digest_out_patches(sizing.builds);
-                        serial_ref_digest = digest_src_refs(sizing.builds);
+                        serial_entries = digest_entries(sizing.builds, 1469598103934665603ull, unused);
                     }
                 }
             }
@@ -4563,7 +4486,7 @@ static wae_status prep_begin(wae_engine* eng, wae_graph* const* graphs, uint32_t
                     RangeOut abs_out;
                     same = size_group_split(k, nullptr, (int)std::min<uint32_t>(n_in_group, 3u), abs_out, &b->groups[k].graph_src_base) &&
                            abs_out.graph_base == b->groups[k].graph_src_base && digest_builds(abs_out.builds, 1469598103934665603ull) == serial_digest &&
-                           digest_out_patches(abs_out.builds) == serial_out_digest && digest_src_refs(abs_out.builds) == serial_ref_digest;
+                           digest_entries(abs_out.builds, 1469598103934665603ull, unused) == serial_entries;
                 }
                 for (size_t c = 0; same && c < out.copies.size(); c++) {
                     const auto& x = out.copies[c];
@@ -4589,7 +4512,10 @@ static wae_status prep_begin(wae_engine* eng, wae_graph* const* graphs, uint32_t
             fpf = std::max(fpf, so[k].fpf);
             has_feedback = has_feedback || so[k].has_feedback;
             for (auto& l : so[k].stage_lists) plan_stage_lists.push_back(std::move(l));
-            if (plan && plan_digest_wanted()) std::fprintf(stderr, "[wae plan digest] group %d fpf %llu src %zu: %016llx\n", k, (unsigned long long)so[k].fpf, b->groups[k].src_floats, (unsigned long long)so[k].digest);
+            if (plan && plan_digest_wanted()) {
+                std::fprintf(stderr, "[wae plan digest] group %d fpf %llu src %zu: %016llx\n", k, (unsigned long long)so[k].fpf, b->groups[k].src_floats, (unsigned long long)so[k].digest);
+                std::fprintf(stderr, "[wae plan entries] group %d entries %zu: %016llx\n", k, so[k].n_entries, (unsigned long long)so[k].entries_digest);
+            }
             for (auto& kv : so[k].delay_ch_seen) {
                 auto it = ps.delay_ch_hint.find(kv.first);
                 int cur = it == ps.delay_ch_hint.end() ? 1 : it->second;
@@ -4878,65 +4804,25 @@ static void prep_plan_group(wae_batch* b, wae_graph* const* graphs, int k, PrepS
                 if (!st.d_a) return oom("stage tables");
                 gp.stages.push_back(st);
             }
-            if (st.n > 0) {  // patch entries: the device addresses of the fields they set
-                const size_t rec_size = s.record_bytes();
-                auto rec = [&](int32_t k) { return static_cast<char*>(st.d_a) + (size_t)k * rec_size; };
-                // params: the field and the scan constants (S_CHAIN / S_VSUM) or stereo gains (S_SPAN) it re-derives (PATCH_OSC: dst2 is
-                // the start time's address, set by the planner)
-                const size_t rec2_size = s.kind == S_SPAN ? sizeof(float2) : sizeof(ScanCoef);
-                char* const param_table = static_cast<char*>(s.kind == S_HRTF ? st.d_b : st.d_a);  // (see StageBuild::records)
-                for (const PatchRec& pr : s.patches) {
-                    ParamPatch p = pr.p;
-                    p.dst = param_table + (size_t)pr.rec * rec_size + pr.off;
-                    if (pr.rec2 >= 0) p.dst2 = static_cast<char*>(st.d_b) + (size_t)pr.rec2 * rec2_size;
-                    gp.patches.push_back({pr.graph, p});
+            if (st.n > 0) {  // bind entries: the device addresses of the record fields their references name (this pass builds the
+                             // scan constants of every chain biquad, which the T_B references of its entries name)
+                char* const tables[4] = {nullptr, static_cast<char*>(st.d_a), static_cast<char*>(st.d_b), static_cast<char*>(st.d_c)};
+                for (Entry e : s.entries) {
+                    for (const FieldRef& r : e.ref)
+                        if (r.table != T_NONE) {
+                            char* const at = tables[r.table] + (size_t)r.rec * s.record_bytes(r.table) + r.off;
+                            std::memcpy(reinterpret_cast<char*>(&e.p) + r.field, &at, sizeof at);
+                        }
+                    gp.entries.push_back(e);
                 }
-                for (const auto& cp : s.curve_patches)  // curves: the int32 field
-                    gp.curve_patches.push_back({cp.graph, cp.node, CurvePatch{reinterpret_cast<int32_t*>(rec(cp.rec) + cp.off), cp.keeps, cp.other}});
-                // IIR coefficients: the coefficient fields of the IirInst or ChainBiquad, and the biquad's scan constants where they were built
-                for (const auto& ip : s.iir_patches) {
-                    IirPatch p{};
-                    if (ip.bq < 0) {
-                        p.b = reinterpret_cast<double*>(rec(ip.rec) + offsetof(IirInst, b));
-                        p.a = reinterpret_cast<double*>(rec(ip.rec) + offsetof(IirInst, a));
-                    } else {
-                        p.b = reinterpret_cast<double*>(rec(ip.rec) + offsetof(ChainInst, bq) + (size_t)ip.bq * sizeof(ChainBiquad) +
-                                                        offsetof(ChainBiquad, b0));
-                        if (ip.scan >= 0 && (size_t)ip.scan < s.scan_coef.size()) p.scan = static_cast<ScanCoef*>(st.d_b) + ip.scan;
-                    }
-                    gp.iir_patches.push_back({ip.graph, ip.node, p});
-                }
-                for (const auto& sp : s.sched_patches) {  // schedules: the record whose fields the times reach
-                    SchedPatch p = sp.p;
-                    p.dst = rec(sp.rec) + sp.off;
-                    gp.sched_patches.push_back({sp.graph, sp.node, p});
-                }
-                for (const auto& lp : s.loop_patches) {  // loop points: the record
-                    LoopPatch p = lp.p;
-                    p.dst = rec(lp.rec);
-                    gp.loop_patches.push_back({lp.graph, lp.node, p});
-                }
-                for (const auto& sr : s.src_refs)  // sources declared by reference: the record's PCM pointer and channel stride
-                    gp.src_refs.push_back({sr.graph, sr.node, SrcRefPatch{reinterpret_cast<const float**>(rec(sr.rec) + sr.buf),
-                                                                         reinterpret_cast<int64_t*>(rec(sr.rec) + sr.stride)}});
-                for (const auto& lw : s.loop_walks)
-                    gp.loop_walks.push_back(LoopWalk{reinterpret_cast<AbsnBoundInst*>(rec(lw.rec)), lw.lq, lw.cap, 0});
-                for (StageBuild::SpatialPatchRec sp : s.spatial) {  // static panners: the PanInst or HrtfInst::static_sel they re-derive
-                    if (sp.rec >= 0)
-                        sp.p.dst = static_cast<char*>(st.d_a) + (size_t)sp.rec * (s.kind == S_PAN ? sizeof(PanInst) : sizeof(HrtfInst)) + sp.off;
-                    gp.spatial.push_back(sp);
-                }
-                char* const out_table = static_cast<char*>(s.kind == S_VSUM ? st.d_c : st.d_a);  // (see StageBuild::out_records)
-                for (const auto& op : s.out_patches)  // destination writers: the BufRef::p of the rendered PCM
-                    gp.out_patches.push_back(
-                        OutPatch{reinterpret_cast<float**>(out_table + (size_t)op.rec * s.out_record_bytes() + op.off + offsetof(BufRef, p)), op.dest});
             }
         }
         // the frames of this segment of the graphs no stage writes: zeroed by every run into a bound output (the batch's own buffer
         // keeps the zeros it was allocated with)
         std::vector<char> written(grp.g1 - grp.g0, 0);
         for (auto& kv : pl.builds)
-            for (const auto& op : kv.second.out_patches) written[op.graph - grp.g0] = 1;
+            for (const Entry& e : kv.second.entries)
+                if (e.kind == E_OUT) written[e.graph - grp.g0] = 1;
         for (uint32_t j = grp.g0; j < grp.g1; j++) {
             const int64_t len = (int64_t)b->shape[j].second, f1 = std::min<int64_t>(pl.seg_end, len);
             if (written[j - grp.g0] || f1 <= pl.seg_start) continue;
@@ -4988,16 +4874,17 @@ static void record_device_inputs(wae_batch* b, wae_graph* const* graphs, uint32_
     });
 }
 
-// The patch entries of the planned groups (`entries` of each GroupPlan) gathered per declaration of `t`, each declaration's range [p0, p1)
+// The entries of kind `kind` of the planned groups (their `payload`) gathered per declaration of `t`, each declaration's range [p0, p1)
 // set, and uploaded to *d (from `patches`, which the caller keeps alive until the stream has been synchronised).  Runs wait for a
 // declaration with entries.
 extern "C++" {
 template <typename D, typename P>
-static wae_status gather_patches(wae_batch* b, Bindings<D>& t, const std::vector<GroupPlan>& gps,
-                                 std::vector<PatchEntry<P>> GroupPlan::*entries, std::vector<P>& patches, P** d) {
+static wae_status gather_patches(wae_batch* b, Bindings<D>& t, const std::vector<GroupPlan>& gps, int kind, P Entry::Payload::*payload,
+                                 std::vector<P>& patches, P** d) {
     std::vector<std::vector<P>> per(t.keys.size());
     for (const auto& gp : gps)
-        for (const auto& e : gp.*entries) per[t.index.at({e.graph, e.node, kNodeLevel})].push_back(e.p);
+        for (const Entry& e : gp.entries)
+            if (e.kind == kind) per[t.index.at({e.graph, e.node, kNodeLevel})].push_back(e.p.*payload);
     for (size_t k = 0; k < per.size(); k++) {
         t.data[k].p0 = (int32_t)patches.size();
         patches.insert(patches.end(), per[k].begin(), per[k].end());
@@ -5051,12 +4938,14 @@ static wae_status record_declarations(wae_batch* b, wae_graph* const* graphs, ui
         if (nd.kind == K_ABSN && nd.device_loop)
             declare({j, nd.id, kNodeLevel}, DevLoop{{nd.loop_lo[0], nd.loop_lo[1]}, {nd.loop_hi[0], nd.loop_hi[1]}, 0, 0});
     });
-    wae_status st = gather_patches(b, b->curves, gps, &GroupPlan::curve_patches, curve_patches, &b->d_curve_patches);
-    if (st == WAE_OK) st = gather_patches(b, b->iirs, gps, &GroupPlan::iir_patches, iir_patches, &b->d_iir_patches);
-    if (st == WAE_OK) st = gather_patches(b, b->schedules, gps, &GroupPlan::sched_patches, sched_patches, &b->d_sched_patches);
-    if (st == WAE_OK) st = gather_patches(b, b->loops, gps, &GroupPlan::loop_patches, loop_patches, &b->d_loop_patches);
-    if (st == WAE_OK) st = gather_patches(b, b->sources, gps, &GroupPlan::src_refs, src_refs, &b->d_src_refs);
-    for (const auto& gp : gps) loop_walks.insert(loop_walks.end(), gp.loop_walks.begin(), gp.loop_walks.end());
+    wae_status st = gather_patches(b, b->curves, gps, E_CURVE, &Entry::Payload::curve, curve_patches, &b->d_curve_patches);
+    if (st == WAE_OK) st = gather_patches(b, b->iirs, gps, E_IIR, &Entry::Payload::iir, iir_patches, &b->d_iir_patches);
+    if (st == WAE_OK) st = gather_patches(b, b->schedules, gps, E_SCHED, &Entry::Payload::sched, sched_patches, &b->d_sched_patches);
+    if (st == WAE_OK) st = gather_patches(b, b->loops, gps, E_LOOP, &Entry::Payload::loop, loop_patches, &b->d_loop_patches);
+    if (st == WAE_OK) st = gather_patches(b, b->sources, gps, E_SRC_REF, &Entry::Payload::src_ref, src_refs, &b->d_src_refs);
+    for (const auto& gp : gps)
+        for (const Entry& e : gp.entries)
+            if (e.kind == E_LOOP_WALK) loop_walks.push_back(e.p.walk);
     if (st == WAE_OK && !loop_walks.empty()) {
         b->n_loop_walks = (int)loop_walks.size();
         b->d_loop_walks = b->dupload_now(loop_walks);
@@ -5107,15 +4996,17 @@ static wae_status record_params(wae_batch* b, wae_graph* const* graphs, uint32_t
         info.push_back(b->params.data[k].info);
     }
     for (auto& gp : gps)
-        for (auto& gpp : gp.patches) {
-            ParamPatch p = gpp.second;
+        for (const Entry& e : gp.entries) {
+            if (e.kind != E_PARAM) continue;
+            ParamPatch p = e.p.param;
             for (int i = 0; i < PATCH_OPS; i++)
-                if (p.slot[i] >= 0) p.slot[i] = slot_of.at((uint64_t)gpp.first << 32 | (uint32_t)p.slot[i]);
+                if (p.slot[i] >= 0) p.slot[i] = slot_of.at((uint64_t)e.graph << 32 | (uint32_t)p.slot[i]);
             patches.push_back(p);
         }
     for (auto& gp : gps)
-        for (const auto& sr : gp.spatial) {
-            SpatialPatch p = sr.p;
+        for (const Entry& sr : gp.entries) {
+            if (sr.kind != E_SPATIAL) continue;
+            SpatialPatch p = sr.p.spatial;
             for (int i = 0; i < 15; i++)
                 if (p.slot[i] >= 0) p.slot[i] = slot_of.at((uint64_t)sr.graph << 32 | (uint32_t)p.slot[i]);
             spatial.push_back(p);
@@ -5253,7 +5144,9 @@ static wae_status prepare_impl(wae_engine* eng, wae_graph* const* graphs, uint32
     std::vector<SpatialPatch> spatial;
     std::vector<RespBindItem> spatial_resp;
     std::vector<OutPatch> out_patches;
-    for (const auto& gp : gps) out_patches.insert(out_patches.end(), gp.out_patches.begin(), gp.out_patches.end());
+    for (const auto& gp : gps)
+        for (const Entry& e : gp.entries)
+            if (e.kind == E_OUT) out_patches.push_back(e.p.out);
     b->n_out_patches = (int)out_patches.size();
     if (!out_patches.empty() && !(b->d_out_patches = b->dupload_now(out_patches))) st = fail(WAE_OUT_OF_MEMORY, "out of device memory (output entries)");
     if (st == WAE_OK) st = record_declarations(b, graphs, n_graphs, gps, curve_patches, iir_patches, sched_patches, loop_patches, loop_walks, src_refs);
